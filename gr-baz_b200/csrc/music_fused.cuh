@@ -27,7 +27,7 @@
 //                window tickets have run out and `mma_fin_max` covariance warps are done, no new pass is started:
 //                every warp that has nothing left to do - covariance warps as they finish, the scan warps after
 //                their last pass, the eigenvector warp at the end - becomes a drain worker and takes (group of 4
-//                windows - fewer only for the CTA's very last ones -, 1/nch of the bins, interleaved in steps of 32)
+//                windows - fewer only for the CTA's very last ones -, 1/FZ_NCH of the bins, interleaved in steps of 32)
 //                units of an all-fp64 scan (drain_bin = scan_bin's arithmetic from the unfused scan_peak1_kernel; the
 //                FP64 pipe is free by then), merged per group by the warp that finishes the group's last unit.  Same
 //                formula, same tie rule: bit-identical to the tensor-core path, at ~4 k cycles of the whole SM per
@@ -63,13 +63,7 @@
 
 namespace music {
 
-#ifndef FZ_COV_WARPS_BUILD
-#define FZ_COV_WARPS_BUILD 8
-#endif
-#ifndef FZ_STAGES_BUILD
-#define FZ_STAGES_BUILD 4
-#endif
-constexpr int FZ_COV_WARPS = FZ_COV_WARPS_BUILD;
+constexpr int FZ_COV_WARPS = 8;
 constexpr int FZ_SCAN_WARPS = 7;
 constexpr int FZ_THREADS = 32 * (FZ_COV_WARPS + 1 + FZ_SCAN_WARPS);  // 512
 constexpr int FZ_SCAN_THREADS = 32 * FZ_SCAN_WARPS;                  // 224
@@ -78,7 +72,7 @@ constexpr int FZ_MPW = 4;        // MMA tiles (16 rows) per scan warp and table 
 constexpr int FZ_BINS = 16 * FZ_SCAN_WARPS * FZ_MPW;  // table rows per ring tile
 constexpr int FZ_Q = 64;        // window queue slots per CTA
 constexpr int FZ_WPT = 8;       // windows per scan pass = 2 column groups of 4 windows x {re, im} (8 MMA columns each)
-constexpr int FZ_STAGES = FZ_STAGES_BUILD;    // 4 KiB TMA stages per covariance warp
+constexpr int FZ_STAGES = 4;    // 4 KiB TMA stages per covariance warp
 constexpr int FZ_TS = 3;        // steering-table tile stages (cp.async ring shared by the scan warps)
 constexpr int FZ_FRAG_BYTES = 512;  // one 16 x 8 fp32 A tile in fragment order (16 B per lane)
 constexpr int FZ_TILE_BYTES = (FZ_BINS / 16) * FZ_FRAG_BYTES + FZ_BINS * 4;  // fragment tiles + fp32 ||a||^2
@@ -87,8 +81,9 @@ constexpr float FZ_B = 3.0517578125e-05f;  // 2^-15, see "Screen error bound"
 
 constexpr int FZ_TRACE = 32;    // int64 trace words per CTA (MUSIC_B200_TRACE=1)
 constexpr int FZ_DG = 4;         // windows per drain group (= scan_bin's windows per thread)
-constexpr int FZ_NCH = 32;       // most interleaved bin chunks per drain group (the launch parameter `nch` picks 1..FZ_NCH): (group, chunk) is the unit a drain worker (one warp) takes
+constexpr int FZ_NCH = 16;       // interleaved bin chunks per drain group: (group, chunk) is the unit a drain worker (one warp) takes
 constexpr int FZ_NGS = 4;        // drain groups in flight
+constexpr unsigned FZ_IDLE_NS = 100;  // sleep of a drain worker that found no unit
 
 struct FusedCtl {               // shared-memory control block
     unsigned cov_seq;           // queue sequence numbers handed to finished covariances (atomic)
@@ -358,7 +353,7 @@ __device__ __forceinline__ void fused_retire(unsigned char *smem, const unsigned
 // + lane, i = 0, 1, ..), the next row is requested before the current one is evaluated.  Returns the number of units
 // this warp processed.
 template <bool TRACE, bool SPEC>
-__device__ __noinline__ int fused_drain_worker(unsigned char *smem, const float *__restrict__ tab_c64, const unsigned idle_ns, const int nch, const int early_drain, const int K,
+__device__ __noinline__ int fused_drain_worker(unsigned char *smem, const float *__restrict__ tab_c64, const int K,
                                                float *__restrict__ spec /* [W][K] or null */, const PeakOut out, long long *__restrict__ dbg_in, const long long t_start)
 {
     long long *const dbg_cta = TRACE ? dbg_in : nullptr;
@@ -383,9 +378,9 @@ __device__ __noinline__ int fused_drain_worker(unsigned char *smem, const float 
             fz_lock(ctl, lane);
             if (lane == 0) {
                 const int cur = ctl->dg_open;
-                if (cur >= 0 && grp[cur].next_chunk < (unsigned)nch) {
+                if (cur >= 0 && grp[cur].next_chunk < (unsigned)FZ_NCH) {
                     slot = cur; chunk = (int)grp[cur].next_chunk++; gs = grp[cur].gs; gc = grp[cur].gc;
-                } else if (ctl->mma_off || (early_drain && ctl->tout)) {
+                } else if (ctl->mma_off) {
                     const unsigned start = ctl->claim, avail = ctl->eig_done - start;
                     // every window of this CTA has its eigenvectors: what is left may go out as a partial group
                     const bool last = ctl->cov_finished == (unsigned)FZ_COV_WARPS &&
@@ -413,7 +408,7 @@ __device__ __noinline__ int fused_drain_worker(unsigned char *smem, const float 
             all_done = __shfl_sync(0xffffffffu, all_done, 0);
             if (slot >= 0) break;
             if (all_done) { slot = -2; break; }
-            __nanosleep(idle_ns);
+            __nanosleep(FZ_IDLE_NS);
         }
         if (dbg_cta && lane == 0) ph[3] += clock64() - tw0;
         if (slot < 0) {
@@ -459,7 +454,7 @@ __device__ __noinline__ int fused_drain_worker(unsigned char *smem, const float 
         if (SPEC) {  // (compile time: the default instantiation carries neither the strengths nor the row pointers)
 #pragma unroll 1
             while (k < K) {
-                const int kn = k + nch * 32;
+                const int kn = k + FZ_NCH * 32;
                 if (kn < K) load_row(kn, nr, ni, nna);
                 drain_bin<true>(ar, ai, na, k, ev, ps, tab_c64, pol_keep, bestP, spec_row, gc);
 #pragma unroll
@@ -470,7 +465,7 @@ __device__ __noinline__ int fused_drain_worker(unsigned char *smem, const float 
         } else {
 #pragma unroll 1
             while (k < K) {
-                const int kn = k + nch * 32;
+                const int kn = k + FZ_NCH * 32;
                 if (kn < K) load_row(kn, nr, ni, nna);
                 drain_bin<false>(ar, ai, na, k, ev, ps, tab_c64, pol_keep, bestP, spec_row, gc);
 #pragma unroll
@@ -507,7 +502,7 @@ __device__ __noinline__ int fused_drain_worker(unsigned char *smem, const float 
                 resk[(slot * FZ_NCH + chunk) * FZ_DG + b] = kk[b];
             }
             __threadfence_block();
-            last = atomicAdd(&grp[slot].done, 1u) == (unsigned)nch - 1 ? 1 : 0;
+            last = atomicAdd(&grp[slot].done, 1u) == (unsigned)FZ_NCH - 1 ? 1 : 0;
             __threadfence_block();
             if (dbg_cta) {  // phases of this unit, accumulated in registers and written once when the worker returns
                 const long long tp4 = clock64();
@@ -523,7 +518,7 @@ __device__ __noinline__ int fused_drain_worker(unsigned char *smem, const float 
                 double Pm = resP[(slot * FZ_NCH) * FZ_DG + lane];
                 int km = resk[(slot * FZ_NCH) * FZ_DG + lane];
 #pragma unroll 1
-                for (int c = 1; c < nch; ++c) {
+                for (int c = 1; c < FZ_NCH; ++c) {
                     const double Pc = resP[(slot * FZ_NCH + c) * FZ_DG + lane];
                     const int kc = resk[(slot * FZ_NCH + c) * FZ_DG + lane];
                     if (peak_better(Pc, kc, Pm, km)) { Pm = Pc; km = kc; }
@@ -556,9 +551,6 @@ music4_fused_kernel(const float *__restrict__ in, const PlanarStreams S, unsigne
                     const int eig_mode /* 0: principal eigenvector by squaring (Jacobi fallback), otherwise: Jacobi, four lanes per window */,
                     const GatherFlags gather_flags /* epoch flags of the fused bins all-gather (out.npeer > 0) */,
                     const int mma_fin_max /* no tensor-core pass starts once the window tickets have run out and this many covariance warps are done (0: once the tickets have run out); < 0: never any */,
-                    const unsigned idle_ns /* sleep of a drain worker that found no unit */,
-                    const int nch /* drain units per group, 1..FZ_NCH */,
-                    const int early_drain /* finished covariance warps start draining as soon as the tickets have run out, beside the tensor-core passes */,
                     float *__restrict__ spec /* optional spectrum port [W][K] (float): every window then goes through the fp64 drain workers, which write it */)
 {
     long long *const dbg = TRACE ? dbg_in : nullptr;
@@ -736,8 +728,8 @@ music4_fused_kernel(const float *__restrict__ in, const PlanarStreams S, unsigne
             if (dbg && fin == 0) dbg[blockIdx.x * FZ_TRACE + 1] = clock64() - t_start;                           // first one
         }
         __syncwarp();
-        if (spec) fused_drain_worker<TRACE, true>(fz_smem, tab_c64, idle_ns, nch, early_drain, K, spec, out, dbg ? dbg + blockIdx.x * FZ_TRACE : nullptr, t_start);
-        else fused_drain_worker<TRACE, false>(fz_smem, tab_c64, idle_ns, nch, early_drain, K, nullptr, out, dbg ? dbg + blockIdx.x * FZ_TRACE : nullptr, t_start);
+        if (spec) fused_drain_worker<TRACE, true>(fz_smem, tab_c64, K, spec, out, dbg ? dbg + blockIdx.x * FZ_TRACE : nullptr, t_start);
+        else fused_drain_worker<TRACE, false>(fz_smem, tab_c64, K, nullptr, out, dbg ? dbg + blockIdx.x * FZ_TRACE : nullptr, t_start);
     } else if (warp == FZ_COV_WARPS) {
         // ================= eigensolver warp =================
         long long eig_busy = 0, eig_rounds = 0, eig_jacobi = 0;
@@ -781,8 +773,8 @@ music4_fused_kernel(const float *__restrict__ in, const PlanarStreams S, unsigne
             dbg[blockIdx.x * FZ_TRACE + 10] = eig_rounds;
             dbg[blockIdx.x * FZ_TRACE + 19] = eig_jacobi;
         }
-        if (spec) fused_drain_worker<TRACE, true>(fz_smem, tab_c64, idle_ns, nch, early_drain, K, spec, out, dbg ? dbg + blockIdx.x * FZ_TRACE : nullptr, t_start);
-        else fused_drain_worker<TRACE, false>(fz_smem, tab_c64, idle_ns, nch, early_drain, K, nullptr, out, dbg ? dbg + blockIdx.x * FZ_TRACE : nullptr, t_start);
+        if (spec) fused_drain_worker<TRACE, true>(fz_smem, tab_c64, K, spec, out, dbg ? dbg + blockIdx.x * FZ_TRACE : nullptr, t_start);
+        else fused_drain_worker<TRACE, false>(fz_smem, tab_c64, K, nullptr, out, dbg ? dbg + blockIdx.x * FZ_TRACE : nullptr, t_start);
     } else {
         // ================= scan warps =================
         const int st = threadIdx.x - 32 * (FZ_COV_WARPS + 1);  // 0..223
@@ -1118,8 +1110,8 @@ music4_fused_kernel(const float *__restrict__ in, const PlanarStreams S, unsigne
             dbg[blockIdx.x * FZ_TRACE + 3] = (long long)(g_end - g_start);   // ns, this CTA's lifetime (overwrites covariance warp 3's slot)
             dbg[blockIdx.x * FZ_TRACE + 2] = (long long)g_start;             // ns, absolute start (overwrites covariance warp 2's slot)
         }
-        if (spec) fused_drain_worker<TRACE, true>(fz_smem, tab_c64, idle_ns, nch, early_drain, K, spec, out, dbg ? dbg + blockIdx.x * FZ_TRACE : nullptr, t_start);
-        else fused_drain_worker<TRACE, false>(fz_smem, tab_c64, idle_ns, nch, early_drain, K, nullptr, out, dbg ? dbg + blockIdx.x * FZ_TRACE : nullptr, t_start);
+        if (spec) fused_drain_worker<TRACE, true>(fz_smem, tab_c64, K, spec, out, dbg ? dbg + blockIdx.x * FZ_TRACE : nullptr, t_start);
+        else fused_drain_worker<TRACE, false>(fz_smem, tab_c64, K, nullptr, out, dbg ? dbg + blockIdx.x * FZ_TRACE : nullptr, t_start);
     }
     // The last CTA to finish re-arms the ticket counter for the next launch (launches of one handle are
     // serialised by the host, and by now every covariance warp has drawn a ticket >= W).

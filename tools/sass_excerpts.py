@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """cuobjdump -sass of the built library, condensed: per kernel the code size, the count of the mnemonics that show what the
 kernel is made of (bulk / tensor-map copies, tensor-core MMAs, FP64, cache-hinted accesses, warp reductions, PDL) and the
-first occurrence of each.  Usage: python tools/sass_excerpts.py > profiles/<round>_sass_excerpts.txt"""
+first occurrence of each.  Usage: python tools/sass_excerpts.py > sass_excerpts.txt"""
 import collections
 import os
 import re
