@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """Generates tests/golden/reference/work.npz: what the reference's own work() returns on the inputs of
-tests/test_ref_shim.py and tests/test_gpu_zz_reference_source.py (case lists in tests/helpers.py); and
+tests/test_ref_shim.py and tests/test_gpu_zz_reference_source.py (case lists and random sweeps in tests/helpers.py;
+the wide-array sweep's keys come last, after every earlier key); and
 tests/golden/reference/interface.json: the signature of the reference's GRC descriptor and the C++ declarations of its
 block header that tests/test_boundary_files.py holds ours to.
 
@@ -89,12 +90,12 @@ def main():
     x = synth.gen_windows_numpy(cfg, s, 0, W)
     store(out, "mirror", x, ref_build.work_batch(x, cfg["m"], cfg["n"], helpers.table_for(cfg)), cfg["resolution"], seed)
     seed += 1
-    for trial, m, n, snaps, K, table, x in helpers.random_small_shapes():
-        ref = ref_build.work_batch(x, m, n, table)
-        key = helpers.case_key("random", trial)
-        finite = bool(np.all(np.isfinite(ref["levels"])) and np.all(np.isfinite(ref["spectrum"])))
-        store(out, key, x, ref, K, seed, finite)
-        seed += 1
+    for kind, shapes in (("random", helpers.random_small_shapes), ("wide", helpers.random_wide_shapes)):
+        for trial, m, n, snaps, K, table, x in shapes():
+            ref = ref_build.work_batch(x, m, n, table)
+            finite = bool(np.all(np.isfinite(ref["levels"])) and np.all(np.isfinite(ref["spectrum"])))
+            store(out, helpers.case_key(kind, trial), x, ref, K, seed, finite)
+            seed += 1
     path = helpers.REFERENCE_GOLDEN
     np.savez_compressed(path, **pack(out))
     print("%s: %d cases, %d bytes" % (path, len(out), os.path.getsize(path)))
