@@ -27,6 +27,7 @@
 #include "music_steer.cuh"
 #include "music_planar.cuh"
 #include "music_reduce.cuh"
+#include "music_sources.cuh"
 
 using namespace music;
 
@@ -44,7 +45,8 @@ struct DeviceTable {
 
 struct Workspace {
     double *R = nullptr, *ev = nullptr, *Vt = nullptr, *P64 = nullptr;
-    uint32_t cap = 0, p64_cap = 0;
+    int32_t *cnt = nullptr;  // per-window source counts (source rule other than FIXED)
+    uint32_t cap = 0, p64_cap = 0, cnt_cap = 0;
     cudaEvent_t scan_done = nullptr;
     bool used = false;
 };
@@ -68,6 +70,7 @@ struct music_b200 {
     float *steer_vals = nullptr;
     int peak_mode = MUSIC_B200_PEAKS_TOP_BINS;  // set_peak_mode()
     uint32_t peak_excl = 0;
+    int source_rule = MUSIC_B200_SOURCES_FIXED;  // set_source_rule()
     unsigned steer_guarded = 0;    // entries of the last built table re-evaluated with the host libm
 
     // fp64 workspace slots (R, eigenvalues, sorted eigenvectors, optional strengths) of the unfused path: one per
@@ -93,11 +96,11 @@ struct music_b200 {
     cudaStream_t streams[2] = {nullptr, nullptr};
     float *d_in[2] = {nullptr, nullptr};
     float *d_ang[2] = {nullptr, nullptr}, *d_lvl[2] = {nullptr, nullptr}, *d_spec[2] = {nullptr, nullptr};
-    int32_t *d_bins[2] = {nullptr, nullptr};
+    int32_t *d_bins[2] = {nullptr, nullptr}, *d_cnt[2] = {nullptr, nullptr};
     // pinned host mirrors of d_ang/d_lvl/d_bins: device->host copies into caller memory would be synchronous when that
     // memory is pageable (numpy arrays, GNU Radio buffers) and stall the enqueue of the next chunk's upload
     float *p_ang[2] = {nullptr, nullptr}, *p_lvl[2] = {nullptr, nullptr};
-    int32_t *p_bins[2] = {nullptr, nullptr};
+    int32_t *p_bins[2] = {nullptr, nullptr}, *p_cnt[2] = {nullptr, nullptr};
     uint32_t slot_w0[2] = {0, 0}, slot_W[2] = {0, 0};
     uint32_t host_chunk = 0;
     bool host_spec_alloc = false;
@@ -258,7 +261,8 @@ constexpr unsigned CTR_RING = 256;  // ticket-counter pairs per slot (see ticket
 // Windows per sub-batch bounding one workspace slot to ~384 MiB.
 uint32_t max_sub_windows(const music_b200 *h, bool need_p64)
 {
-    const size_t per_win = (size_t)h->m * h->m * 2 * 8 * 2 + h->m * 8 + (need_p64 ? (size_t)h->K * 8 : 0);
+    const size_t per_win = (size_t)h->m * h->m * 2 * 8 * 2 + h->m * 8 + (need_p64 ? (size_t)h->K * 8 : 0) +
+                           (h->source_rule != MUSIC_B200_SOURCES_FIXED ? sizeof(int32_t) : 0);
     size_t c = ((size_t)384 << 20) / per_win;
     c = std::max<size_t>(SCAN_B, std::min<size_t>(c, 1u << 20));
     return (uint32_t)(c / SCAN_B * SCAN_B);
@@ -283,19 +287,30 @@ int ensure_slot(music_b200 *h, Workspace &ws, uint32_t windows, bool need_p64)
         CU(h, cudaMalloc(&ws.P64, (size_t)windows * h->K * sizeof(double)));
         ws.p64_cap = windows;
     }
+    if (h->source_rule != MUSIC_B200_SOURCES_FIXED && windows > ws.cnt_cap) {
+        if (ws.used) CU(h, cudaEventSynchronize(ws.scan_done));
+        cudaFree(ws.cnt); ws.cnt = nullptr; ws.cnt_cap = 0;
+        CU(h, cudaMalloc(&ws.cnt, (size_t)windows * sizeof(int32_t)));
+        ws.cnt_cap = windows;
+    }
     return MUSIC_B200_OK;
 }
 
 template <int MT>
 void launch_scan(music_b200 *h, const Workspace &ws, const double *soa, uint32_t W, bool argmax, bool p64, bool spec,
-                 PeakOut po, float *d_spec, double *d_p64, cudaStream_t st)
+                 PeakOut po, float *d_spec, double *d_p64, const int32_t *counts, cudaStream_t st)
 {
     const int grid = (W + SCAN_B - 1) / SCAN_B;
     const size_t smem = (size_t)SCAN_B * h->m * h->m * 2 * sizeof(double);
-#define SCAN_CASE(A, P, S)                                                                              \
-    if (argmax == A && p64 == P && spec == S)                                                           \
-        scan_kernel<MT, A, P, S><<<grid, TILE, smem, st>>>(soa, ws.Vt, (int)h->m, (int)h->n, (int)h->K,  \
-                                                           (int)W, po, d_spec, d_p64);
+#define SCAN_CASE(A, P, S)                                                                                        \
+    if (argmax == A && p64 == P && spec == S) {                                                                   \
+        if (counts)                                                                                               \
+            scan_kernel<MT, A, P, S, true><<<grid, TILE, smem, st>>>(soa, ws.Vt, (int)h->m, (int)h->n, (int)h->K, \
+                                                                     (int)W, po, d_spec, d_p64, counts);          \
+        else                                                                                                      \
+            scan_kernel<MT, A, P, S><<<grid, TILE, smem, st>>>(soa, ws.Vt, (int)h->m, (int)h->n, (int)h->K,       \
+                                                               (int)W, po, d_spec, d_p64, nullptr);               \
+    }
     SCAN_CASE(true, false, false)
     SCAN_CASE(true, false, true)
     SCAN_CASE(true, true, false)
@@ -443,9 +458,10 @@ __global__ void gather_wait_kernel(const unsigned *flags, int npeer, unsigned ep
     }
 }
 
-// K2 + K3 (+ top-n) of W windows from ws.R, on `st`.  tev (optional) = timing events [1..4].
+// K2 (+ source count) + K3 (+ top-n) of W windows from ws.R, on `st`.  tev (optional) = timing events [1..4].
+// d_counts_out (may be NULL): the caller's copy of the per-window source counts (source rule other than FIXED).
 int launch_eig_scan(music_b200 *h, const Workspace &ws, uint32_t W, const PeakOut &po, float *d_spec,
-                    double *d_P64_out, double *d_R_out, double *d_ev_out, cudaStream_t st, cudaEvent_t *tev)
+                    double *d_P64_out, double *d_R_out, double *d_ev_out, int32_t *d_counts_out, cudaStream_t st, cudaEvent_t *tev)
 {
     const int M = (int)h->m;
     const double *soa = h->table[h->cur_table].soa;
@@ -463,6 +479,13 @@ int launch_eig_scan(music_b200 *h, const Workspace &ws, uint32_t W, const PeakOu
         }
         h->launches++;
     }
+    // per-window model order from the eigenvalues just written (timed with the eigensolver)
+    const int32_t *cnt = nullptr;
+    if (h->source_rule != MUSIC_B200_SOURCES_FIXED) {
+        source_count_kernel<<<(W + 127) / 128, 128, 0, st>>>(ws.ev, M, (int)h->n, (int)h->N, h->source_rule, (int)W, ws.cnt, d_counts_out);
+        h->launches++;
+        cnt = ws.cnt;
+    }
     if (tev) cudaEventRecord(tev[2], st);
     const bool local = h->peak_mode == MUSIC_B200_PEAKS_LOCAL_MAXIMA;
     const bool argmax = (h->n == 1) && !local;
@@ -471,22 +494,22 @@ int launch_eig_scan(music_b200 *h, const Workspace &ws, uint32_t W, const PeakOu
     const bool fast = argmax && !need_p64 && !d_spec && (M == 4 || M == 8 || M == 16);
     if (fast) {
         const int grid = (W + SCAN_B - 1) / SCAN_B;
-        if (M == 4) scan_peak1_kernel<4><<<grid, TILE, 0, st>>>(soa, ws.Vt, (int)h->K, (int)W, po);
-        else if (M == 8) scan_peak1_kernel<8><<<grid, TILE, 0, st>>>(soa, ws.Vt, (int)h->K, (int)W, po);
-        else scan_peak1_kernel<16><<<grid, TILE, 0, st>>>(soa, ws.Vt, (int)h->K, (int)W, po);
+        if (M == 4) scan_peak1_kernel<4><<<grid, TILE, 0, st>>>(soa, ws.Vt, (int)h->K, (int)W, po, cnt);
+        else if (M == 8) scan_peak1_kernel<8><<<grid, TILE, 0, st>>>(soa, ws.Vt, (int)h->K, (int)W, po, cnt);
+        else scan_peak1_kernel<16><<<grid, TILE, 0, st>>>(soa, ws.Vt, (int)h->K, (int)W, po, cnt);
         h->launches++;
     } else {
         switch (M) {
-        case 4: launch_scan<4>(h, ws, soa, W, argmax, need_p64, d_spec != nullptr, po, d_spec, p64, st); break;
-        case 8: launch_scan<8>(h, ws, soa, W, argmax, need_p64, d_spec != nullptr, po, d_spec, p64, st); break;
-        case 16: launch_scan<16>(h, ws, soa, W, argmax, need_p64, d_spec != nullptr, po, d_spec, p64, st); break;
-        default: launch_scan<0>(h, ws, soa, W, argmax, need_p64, d_spec != nullptr, po, d_spec, p64, st); break;
+        case 4: launch_scan<4>(h, ws, soa, W, argmax, need_p64, d_spec != nullptr, po, d_spec, p64, cnt, st); break;
+        case 8: launch_scan<8>(h, ws, soa, W, argmax, need_p64, d_spec != nullptr, po, d_spec, p64, cnt, st); break;
+        case 16: launch_scan<16>(h, ws, soa, W, argmax, need_p64, d_spec != nullptr, po, d_spec, p64, cnt, st); break;
+        default: launch_scan<0>(h, ws, soa, W, argmax, need_p64, d_spec != nullptr, po, d_spec, p64, cnt, st); break;
         }
     }
     if (tev) cudaEventRecord(tev[3], st);
     if (!argmax) {
-        if (local) topn_local_kernel<<<(W + 7) / 8, 256, 0, st>>>(p64, (int)h->n, (int)h->K, (int)W, (int)h->peak_excl, po);
-        else topn_kernel<<<(W + 7) / 8, 256, 0, st>>>(p64, (int)h->n, (int)h->K, (int)W, po);
+        if (local) topn_local_kernel<<<(W + 7) / 8, 256, 0, st>>>(p64, (int)h->n, (int)h->K, (int)W, (int)h->peak_excl, po, cnt);
+        else topn_kernel<<<(W + 7) / 8, 256, 0, st>>>(p64, (int)h->n, (int)h->K, (int)W, po, cnt);
         h->launches++;
     }
     if (tev) cudaEventRecord(tev[4], st);
@@ -514,13 +537,20 @@ void launch_cov_planar(music_b200 *h, const Workspace &ws, const PlanarStreams &
 
 // Enqueue `nwindows` windows on `st`: one persistent fused launch where the shape allows it, otherwise the unfused
 // kernels in sub-batches of at most max_sub_windows(), which bounds the workspace slot `slot` (0 / 1) they run in.
+// d_counts (may be NULL): receives the per-window source counts; under the FIXED rule every count is n.
 int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, float *d_ang, float *d_lvl, float *d_spec,
-                   int32_t *d_bins, double *d_P64, double *d_R, double *d_ev, cudaStream_t st, int slot,
+                   int32_t *d_bins, double *d_P64, double *d_R, double *d_ev, int32_t *d_counts, cudaStream_t st, int slot,
                    const PlanarStreams *planar = nullptr, unsigned hop = 0)
 {
     if (nwindows == 0) return MUSIC_B200_OK;
     if ((!planar && !d_in) || !d_ang) return fail(h, MUSIC_B200_EINVAL, "d_in_c64 and d_angles must not be NULL");
     if (!planar && (reinterpret_cast<uintptr_t>(d_in) & 15u) != 0) return fail(h, MUSIC_B200_EINVAL, "d_in_c64 must be 16-byte aligned");
+    const bool fixed_n = h->source_rule == MUSIC_B200_SOURCES_FIXED;
+    if (fixed_n && d_counts) {
+        fill_counts_kernel<<<(nwindows + 255) / 256, 256, 0, st>>>(d_counts, (int)h->n, (int)nwindows);
+        h->launches++;
+        CU(h, cudaGetLastError());
+    }
     // planar streams can take the fused path when the 16-byte granularity of bulk copies allows it
     bool planar_fusable = false;
     if (planar) {
@@ -528,7 +558,8 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, float *d
         for (uint32_t r = 0; r < h->m; ++r) planar_fusable = planar_fusable && (reinterpret_cast<uintptr_t>(planar->p[r]) & 15u) == 0;
     }
     const bool local_peaks = h->peak_mode == MUSIC_B200_PEAKS_LOCAL_MAXIMA;
-    if ((!planar || planar_fusable) && h->fused && !local_peaks && h->m == 4 && h->n == 1 && (!d_spec || h->fused_spec) && !d_P64 && !d_R && !d_ev) {
+    // the fused kernels find the principal eigenvector only, not every eigenvalue a source count needs
+    if ((!planar || planar_fusable) && h->fused && fixed_n && !local_peaks && h->m == 4 && h->n == 1 && (!d_spec || h->fused_spec) && !d_P64 && !d_R && !d_ev) {
         // whole call in one persistent launch (music_fused.cuh); no workspace involved
         cudaEvent_t *tev = timing_events(h);
         if (tev) cudaEventRecord(tev[0], st);
@@ -567,7 +598,7 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, float *d
         CU(h, cudaGetLastError());
         return MUSIC_B200_OK;
     }
-    if (!planar && h->fused && !local_peaks && h->m == 8 && h->n == 1 && !d_spec && !d_P64 && !d_R && !d_ev && h->N >= 128 &&
+    if (!planar && h->fused && fixed_n && !local_peaks && h->m == 8 && h->n == 1 && !d_spec && !d_P64 && !d_R && !d_ev && h->N >= 128 &&
         h->N % 2 == 0 && encode_tiled_fn()) {
         // M = 8: whole call in one persistent launch (music_fused8.cuh); R and the eigenvectors stay in shared memory
         CUtensorMap tm;
@@ -608,7 +639,8 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, float *d
                                            d_bins ? d_bins + (size_t)w0 * h->n : nullptr, w0),
                              d_spec ? d_spec + (size_t)w0 * h->K : nullptr,
                              d_P64 ? d_P64 + (size_t)w0 * h->K : nullptr, d_R ? d_R + (size_t)w0 * h->m * h->m * 2 : nullptr,
-                             d_ev ? d_ev + (size_t)w0 * h->m : nullptr, st, tev);
+                             d_ev ? d_ev + (size_t)w0 * h->m : nullptr,
+                             !fixed_n && d_counts ? d_counts + w0 : nullptr, st, tev);
         if (rc) return rc;
         CU(h, cudaEventRecord(ws.scan_done, st));
         ws.used = true;
@@ -675,11 +707,12 @@ void free_host_staging(music_b200 *h)
 {
     for (int i = 0; i < 2; ++i) {
         cudaFree(h->d_in[i]); cudaFree(h->d_ang[i]); cudaFree(h->d_lvl[i]); cudaFree(h->d_spec[i]); cudaFree(h->d_bins[i]);
-        cudaFreeHost(h->p_ang[i]); cudaFreeHost(h->p_lvl[i]); cudaFreeHost(h->p_bins[i]);
+        cudaFree(h->d_cnt[i]);
+        cudaFreeHost(h->p_ang[i]); cudaFreeHost(h->p_lvl[i]); cudaFreeHost(h->p_bins[i]); cudaFreeHost(h->p_cnt[i]);
         h->d_in[i] = h->d_ang[i] = h->d_lvl[i] = h->d_spec[i] = nullptr;
-        h->d_bins[i] = nullptr;
+        h->d_bins[i] = h->d_cnt[i] = nullptr;
         h->p_ang[i] = h->p_lvl[i] = nullptr;
-        h->p_bins[i] = nullptr;
+        h->p_bins[i] = h->p_cnt[i] = nullptr;
         h->slot_W[i] = 0;
     }
     h->host_chunk = 0;
@@ -699,6 +732,8 @@ int ensure_host_staging(music_b200 *h, uint32_t chunk, bool spec)
         CU(h, cudaHostAlloc(&h->p_ang[i], (size_t)cap * h->n * sizeof(float), cudaHostAllocDefault));
         CU(h, cudaHostAlloc(&h->p_lvl[i], (size_t)cap * h->n * sizeof(float), cudaHostAllocDefault));
         CU(h, cudaHostAlloc(&h->p_bins[i], (size_t)cap * h->n * sizeof(int32_t), cudaHostAllocDefault));
+        CU(h, cudaMalloc(&h->d_cnt[i], (size_t)cap * sizeof(int32_t)));
+        CU(h, cudaHostAlloc(&h->p_cnt[i], (size_t)cap * sizeof(int32_t), cudaHostAllocDefault));
         if (spec) CU(h, cudaMalloc(&h->d_spec[i], (size_t)cap * h->K * sizeof(float)));
     }
     h->host_chunk = cap;
@@ -708,7 +743,8 @@ int ensure_host_staging(music_b200 *h, uint32_t chunk, bool spec)
 
 // results of the chunk last computed in staging slot s: pinned mirror -> caller memory (the slot's stream is idle).
 // The chunk holds the windows w = (slot_w0 + i) * G + g of the call (G = 1, g = 0 on a single-device handle).
-void flush_host_slot(music_b200 *h, int s, float *angles, float *levels, int32_t *bins, uint32_t G = 1, uint32_t g = 0)
+// counts (may be NULL): one source count per window, dealt like the bins.
+void flush_host_slot(music_b200 *h, int s, float *angles, float *levels, int32_t *bins, int32_t *counts, uint32_t G = 1, uint32_t g = 0)
 {
     const uint32_t W = h->slot_W[s];
     if (!W) return;
@@ -718,8 +754,10 @@ void flush_host_slot(music_b200 *h, int s, float *angles, float *levels, int32_t
         memcpy(angles + off, h->p_ang[s], cnt * sizeof(float));
         if (levels) memcpy(levels + off, h->p_lvl[s], cnt * sizeof(float));
         if (bins) memcpy(bins + off, h->p_bins[s], cnt * sizeof(int32_t));
+        if (counts) memcpy(counts + h->slot_w0[s], h->p_cnt[s], (size_t)W * sizeof(int32_t));
     } else {
         for (uint32_t i = 0; i < W; ++i) {
+            if (counts) counts[(size_t)(h->slot_w0[s] + i) * G + g] = h->p_cnt[s][i];
             const size_t off = ((size_t)(h->slot_w0[s] + i) * G + g) * n;
             for (size_t r = 0; r < n; ++r) {
                 angles[off + r] = h->p_ang[s][i * n + r];
@@ -732,8 +770,9 @@ void flush_host_slot(music_b200 *h, int s, float *angles, float *levels, int32_t
 }
 
 // device -> pinned mirrors of slot s (asynchronous on st whatever memory the caller's outputs live in)
-int download_host_slot(music_b200 *h, int s, uint32_t w0, uint32_t W, bool levels, bool bins, cudaStream_t st)
+int download_host_slot(music_b200 *h, int s, uint32_t w0, uint32_t W, bool levels, bool bins, bool counts, cudaStream_t st)
 {
+    if (counts) CU(h, cudaMemcpyAsync(h->p_cnt[s], h->d_cnt[s], (size_t)W * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     CU(h, cudaMemcpyAsync(h->p_ang[s], h->d_ang[s], (size_t)W * h->n * sizeof(float), cudaMemcpyDeviceToHost, st));
     if (levels) CU(h, cudaMemcpyAsync(h->p_lvl[s], h->d_lvl[s], (size_t)W * h->n * sizeof(float), cudaMemcpyDeviceToHost, st));
     if (bins) CU(h, cudaMemcpyAsync(h->p_bins[s], h->d_bins[s], (size_t)W * h->n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
@@ -946,7 +985,7 @@ int music_b200_process_planar_device(music_b200 *h, const float *const *d_stream
     }
     std::lock_guard<std::mutex> g(h->mutex);
     CU(h, cudaSetDevice(h->device));
-    return enqueue_device(h, nullptr, nwindows, d_angles, d_levels, d_spectrum, d_bins, nullptr, nullptr, nullptr,
+    return enqueue_device(h, nullptr, nwindows, d_angles, d_levels, d_spectrum, d_bins, nullptr, nullptr, nullptr, nullptr,
                           static_cast<cudaStream_t>(stream), 0, &S, hop);
 }
 
@@ -981,7 +1020,7 @@ int music_b200_process_planar_host(music_b200 *h, const float *const *streams, u
         cudaStream_t st = h->streams[s];
         if (it >= 2) {
             CU_BREAK(h, rc, cudaStreamSynchronize(st));
-            flush_host_slot(h, s, angles, levels, bins);
+            flush_host_slot(h, s, angles, levels, bins, nullptr);
         }
         const size_t seg = (size_t)(W - 1) * hop + N;  // snapshots of each stream this chunk touches
         PlanarStreams S;
@@ -993,9 +1032,9 @@ int music_b200_process_planar_host(music_b200 *h, const float *const *streams, u
         }
         if (rc) break;
         rc = enqueue_device(h, nullptr, W, h->d_ang[s], h->d_lvl[s], spectrum ? h->d_spec[s] : nullptr, h->d_bins[s],
-                            nullptr, nullptr, nullptr, st, s, &S, hop);
+                            nullptr, nullptr, nullptr, nullptr, st, s, &S, hop);
         if (rc) break;
-        rc = download_host_slot(h, s, w0, W, levels != nullptr, bins != nullptr, st);
+        rc = download_host_slot(h, s, w0, W, levels != nullptr, bins != nullptr, false, st);
         if (rc) break;
         if (spectrum) CU_BREAK(h, rc, cudaMemcpyAsync(spectrum + (size_t)w0 * h->K, h->d_spec[s], (size_t)W * h->K * sizeof(float), cudaMemcpyDeviceToHost, st));
     }
@@ -1005,8 +1044,8 @@ int music_b200_process_planar_host(music_b200 *h, const float *const *streams, u
     if (rc) return rc;
     if (e0 != cudaSuccess || e1 != cudaSuccess)
         return fail(h, MUSIC_B200_ECUDA, "stream sync failed: %s", cudaGetErrorString(e0 != cudaSuccess ? e0 : e1));
-    flush_host_slot(h, 0, angles, levels, bins);
-    flush_host_slot(h, 1, angles, levels, bins);
+    flush_host_slot(h, 0, angles, levels, bins, nullptr);
+    flush_host_slot(h, 1, angles, levels, bins, nullptr);
     return MUSIC_B200_OK;
 }
 
@@ -1162,9 +1201,14 @@ int music_b200_get_table(music_b200 *h, float *table_c64)
     return MUSIC_B200_OK;
 }
 
-int music_b200_process_device_ex(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_angles,
-                                 float *d_levels, float *d_spectrum, int32_t *d_bins, double *d_P64, double *d_R,
-                                 double *d_eigvals, void *stream)
+}  // extern "C"
+
+namespace {
+
+// process_device_ex plus the per-window source counts (music_b200_process_device_counts)
+int process_device_impl(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_angles, float *d_levels,
+                        float *d_spectrum, int32_t *d_bins, double *d_P64, double *d_R, double *d_eigvals, int32_t *d_counts,
+                        void *stream)
 {
     if (!h) return MUSIC_B200_EINVAL;
     if (!h->kids.empty()) {
@@ -1176,7 +1220,7 @@ int music_b200_process_device_ex(music_b200 *h, const float *d_in_c64, uint32_t 
         }
         for (music_b200 *c : h->kids)
             if (c->device == at.device) {
-                const int rc = music_b200_process_device_ex(c, d_in_c64, nwindows, d_angles, d_levels, d_spectrum, d_bins, d_P64, d_R, d_eigvals, stream);
+                const int rc = process_device_impl(c, d_in_c64, nwindows, d_angles, d_levels, d_spectrum, d_bins, d_P64, d_R, d_eigvals, d_counts, stream);
                 if (rc) fail(h, rc, "%s", music_b200_last_error(c));
                 return rc;
             }
@@ -1189,8 +1233,29 @@ int music_b200_process_device_ex(music_b200 *h, const float *d_in_c64, uint32_t 
         if ((size_t)nwindows * h->gather_G * h->n > h->gather_cap) return fail(h, MUSIC_B200_EINVAL, "gather buffer holds %zu entries, the call needs %zu", h->gather_cap, (size_t)nwindows * h->gather_G * h->n);
         ++h->gather_epoch;
     }
-    return enqueue_device(h, d_in_c64, nwindows, d_angles, d_levels, d_spectrum, d_bins, d_P64, d_R, d_eigvals,
+    return enqueue_device(h, d_in_c64, nwindows, d_angles, d_levels, d_spectrum, d_bins, d_P64, d_R, d_eigvals, d_counts,
                           static_cast<cudaStream_t>(stream), 0);
+}
+
+// process_host plus the per-window source counts (music_b200_process_host_counts)
+int process_host_impl(music_b200 *h, const float *in_c64, uint32_t nwindows, float *angles, float *levels,
+                      float *spectrum, int32_t *bins, int32_t *counts);
+
+}  // namespace
+
+extern "C" {
+
+int music_b200_process_device_ex(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_angles,
+                                 float *d_levels, float *d_spectrum, int32_t *d_bins, double *d_P64, double *d_R,
+                                 double *d_eigvals, void *stream)
+{
+    return process_device_impl(h, d_in_c64, nwindows, d_angles, d_levels, d_spectrum, d_bins, d_P64, d_R, d_eigvals, nullptr, stream);
+}
+
+int music_b200_process_device_counts(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_angles,
+                                     float *d_levels, float *d_spectrum, int32_t *d_bins, int32_t *d_counts, void *stream)
+{
+    return process_device_impl(h, d_in_c64, nwindows, d_angles, d_levels, d_spectrum, d_bins, nullptr, nullptr, nullptr, d_counts, stream);
 }
 
 int music_b200_process_device(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_angles,
@@ -1203,10 +1268,47 @@ int music_b200_process_device(music_b200 *h, const float *d_in_c64, uint32_t nwi
 int music_b200_process_host(music_b200 *h, const float *in_c64, uint32_t nwindows, float *angles, float *levels,
                             float *spectrum, int32_t *bins)
 {
+    return process_host_impl(h, in_c64, nwindows, angles, levels, spectrum, bins, nullptr);
+}
+
+int music_b200_process_host_counts(music_b200 *h, const float *in_c64, uint32_t nwindows, float *angles, float *levels,
+                                   float *spectrum, int32_t *bins, int32_t *counts)
+{
+    return process_host_impl(h, in_c64, nwindows, angles, levels, spectrum, bins, counts);
+}
+
+int music_b200_set_source_rule(music_b200 *h, int rule)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (rule != MUSIC_B200_SOURCES_FIXED && rule != MUSIC_B200_SOURCES_MDL && rule != MUSIC_B200_SOURCES_AIC)
+        return fail(h, MUSIC_B200_EINVAL, "unknown source rule %d", rule);
+    if (rule != MUSIC_B200_SOURCES_FIXED && h->N <= h->m)
+        return fail(h, MUSIC_B200_EINVAL, "MDL / AIC need more snapshots than antennas (N = %u, m = %u)", h->N, h->m);
+    std::lock_guard<std::mutex> g(h->mutex);
+    for (music_b200 *c : h->kids) {
+        const int rc = music_b200_set_source_rule(c, rule);
+        if (rc) return fail(h, rc, "%s", music_b200_last_error(c));
+    }
+    h->source_rule = rule;
+    return MUSIC_B200_OK;
+}
+
+}  // extern "C"
+
+namespace {
+
+int process_host_impl(music_b200 *h, const float *in_c64, uint32_t nwindows, float *angles, float *levels,
+                      float *spectrum, int32_t *bins, int32_t *counts)
+{
     if (!h) return MUSIC_B200_EINVAL;
     if (nwindows == 0) return MUSIC_B200_OK;
     if (!in_c64 || !angles) return fail(h, MUSIC_B200_EINVAL, "in_c64 and angles must not be NULL");
     std::lock_guard<std::mutex> g(h->mutex);
+    // under the FIXED rule every count is n: nothing to compute or copy
+    if (counts && h->source_rule == MUSIC_B200_SOURCES_FIXED) {
+        for (uint32_t w = 0; w < nwindows; ++w) counts[w] = (int32_t)h->n;
+        counts = nullptr;
+    }
     NvtxRange range("music_b200_process_host");
     // lanes: the handle itself, or the per-device children of a multi-device handle; lane g takes the windows
     // w = i * G + g (round-robin at window granularity, SURVEY.md section 8e) - every lane feeds its own PCIe link
@@ -1247,7 +1349,7 @@ int music_b200_process_host(music_b200 *h, const float *in_c64, uint32_t nwindow
             CU_BREAK(h, rc, cudaSetDevice(c->device));
             if (it >= 2) {
                 CU_BREAK(h, rc, cudaStreamSynchronize(st));  // slot buffers free again (its D2H finished)
-                flush_host_slot(c, s, angles, levels, bins, G, l);
+                flush_host_slot(c, s, angles, levels, bins, counts, G, l);
             }
             const float *src = in_c64 + ((size_t)i0 * G + l) * h->nsamples * 2;
             {
@@ -1258,12 +1360,12 @@ int music_b200_process_host(music_b200 *h, const float *in_c64, uint32_t nwindow
             {
                 NvtxRange r("music_b200: kernels");
                 rc = enqueue_device(c, c->d_in[s], W, c->d_ang[s], c->d_lvl[s], spectrum ? c->d_spec[s] : nullptr, c->d_bins[s],
-                                    nullptr, nullptr, nullptr, st, s);
+                                    nullptr, nullptr, nullptr, counts ? c->d_cnt[s] : nullptr, st, s);
                 if (rc && c != h) fail(h, rc, "%s", std::string(c->error).c_str());
                 if (rc) break;
             }
             NvtxRange r("music_b200: D2H");
-            rc = download_host_slot(c, s, i0, W, levels != nullptr, bins != nullptr, st);
+            rc = download_host_slot(c, s, i0, W, levels != nullptr, bins != nullptr, counts != nullptr, st);
             if (rc && c != h) fail(h, rc, "%s", std::string(c->error).c_str());
             if (rc) break;
             if (spectrum) {
@@ -1288,14 +1390,18 @@ int music_b200_process_host(music_b200 *h, const float *in_c64, uint32_t nwindow
     for (uint32_t l = 0; l < G; ++l) {
         music_b200 *c = lanes[l];
         if (rc == MUSIC_B200_OK) {
-            flush_host_slot(c, 0, angles, levels, bins, G, l);
-            flush_host_slot(c, 1, angles, levels, bins, G, l);
+            flush_host_slot(c, 0, angles, levels, bins, counts, G, l);
+            flush_host_slot(c, 1, angles, levels, bins, counts, G, l);
         } else {
             c->slot_W[0] = c->slot_W[1] = 0;  // nothing valid to hand out
         }
     }
     return rc;
 }
+
+}  // namespace
+
+extern "C" {
 
 int music_b200_create_multi(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples, uint32_t resolution,
                             const float *table_c64, const int *devices, int ndev)
@@ -1435,7 +1541,7 @@ int music_b200_process_device_sharded(music_b200 *h, const float *const *d_in_c6
         c->gather_rank = l;
         for (int p = 0; p < G; ++p) { c->peer_bins[p] = d_bins_all ? d_bins_all[p] : nullptr; c->peer_flags[p] = nullptr; }
         rc = enqueue_device(c, d_in_c64[l], Wl, d_angles[l], d_levels ? d_levels[l] : nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
-                            streams ? static_cast<cudaStream_t>(streams[l]) : nullptr, 0);
+                            nullptr, streams ? static_cast<cudaStream_t>(streams[l]) : nullptr, 0);
         c->gather_G = 0;
         if (rc) fail(h, rc, "%s", std::string(c->error).c_str());
     }
@@ -1465,7 +1571,7 @@ void music_b200_destroy(music_b200 *h)
     for (int i = 0; i < 2; ++i) {
         cudaFree(h->table[i].c64); cudaFree(h->table[i].soa); cudaFree(h->table[i].fz); cudaFree(h->table[i].na_max);
         if (h->streams[i]) cudaStreamDestroy(h->streams[i]);
-        cudaFree(h->ws[i].R); cudaFree(h->ws[i].ev); cudaFree(h->ws[i].Vt); cudaFree(h->ws[i].P64);
+        cudaFree(h->ws[i].R); cudaFree(h->ws[i].ev); cudaFree(h->ws[i].Vt); cudaFree(h->ws[i].P64); cudaFree(h->ws[i].cnt);
         if (h->ws[i].scan_done) cudaEventDestroy(h->ws[i].scan_done);
     }
     for (cudaEvent_t e : h->tev) cudaEventDestroy(e);

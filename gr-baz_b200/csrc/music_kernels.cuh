@@ -1004,19 +1004,29 @@ __device__ __forceinline__ double strength_denominator(const double *ar, const d
     return d;
 }
 
-template <int MT, bool ARGMAX, bool WRITE_P64, bool WRITE_SPEC>
+// COUNTS (counts != nullptr, music_sources.cuh): window w has counts[w] <= n sources, so its noise subspace is the
+// M - counts[w] smallest-eigenvalue vectors; with ARGMAX (n == 1) a window with count 0 reports no peak.
+template <int MT, bool ARGMAX, bool WRITE_P64, bool WRITE_SPEC, bool COUNTS = false>
 __global__ void __launch_bounds__(TILE) scan_kernel(const double *__restrict__ soa, const double *__restrict__ Vt,
                                                     int Mrt, int n, int K, int W, PeakOut out,
-                                                    float *__restrict__ spectrum, double *__restrict__ P64)
+                                                    float *__restrict__ spectrum, double *__restrict__ P64,
+                                                    const int32_t *__restrict__ counts)
 {
     constexpr int MA = MT ? MT : MAXM;
     const int M = MT ? MT : Mrt;
     extern __shared__ __align__(16) double smem[];
     double *sV = smem;  // [SCAN_B][M*M*2]
+    __shared__ int sn[SCAN_B];  // COUNTS: per-window source count, and whether the signal (complement) form is shorter
+    __shared__ bool ssig[SCAN_B];
     const int w0 = blockIdx.x * SCAN_B;
     const int nb = min(SCAN_B, W - w0);
     const int vsz = M * M * 2;
     for (int i = threadIdx.x; i < nb * vsz; i += blockDim.x) sV[i] = Vt[(size_t)w0 * vsz + i];
+    if (COUNTS && threadIdx.x < nb) {
+        const int c = counts[w0 + threadIdx.x];
+        sn[threadIdx.x] = c;
+        ssig[threadIdx.x] = c < M - c;
+    }
     __syncthreads();
 
     const bool use_sig = (n < M - n);
@@ -1048,7 +1058,7 @@ __global__ void __launch_bounds__(TILE) scan_kernel(const double *__restrict__ s
 #pragma unroll
             for (int b = 0; b < SCAN_B; ++b) {
                 if (b < nb) {
-                    const double d = strength_denominator<MT>(ar, ai, na, sV + b * vsz, M, n, use_sig);
+                    const double d = strength_denominator<MT>(ar, ai, na, sV + b * vsz, M, COUNTS ? sn[b] : n, COUNTS ? ssig[b] : use_sig);
                     if (FAST) {
                         if (d < best[b]) {
                             if (d < best[b] * 0.99999999999999911182 /* 1 - 2^-50 */ || 1.0 / d > 1.0 / best[b]) {
@@ -1092,6 +1102,7 @@ __global__ void __launch_bounds__(TILE) scan_kernel(const double *__restrict__ s
             for (int q = 1; q < TILE / 32; ++q)
                 if (peak_better(rP[b][q], rk[b][q], P, kk)) { P = rP[b][q]; kk = rk[b][q]; }
             const size_t o = (size_t)(w0 + b);  // n == 1
+            if (COUNTS && sn[b] == 0) kk = -1;
             if (kk >= 0) {
                 out.angles[o] = (float)((double)kk * 360.0 / (double)K);  // :134, :153
                 if (out.levels) out.levels[o] = (float)P;                 // :154
@@ -1246,9 +1257,10 @@ __device__ __forceinline__ void scan_bin(const double (&ar)[M], const double (&a
     }
 }
 
+// counts (may be null, music_sources.cuh): per-window source count in {0, 1}; a window with count 0 reports no peak
 template <int M>
 __global__ void __launch_bounds__(TILE, 3) scan_peak1_kernel(const double *__restrict__ soa, const double *__restrict__ Vt,
-                                                             int K, int W, PeakOut out)
+                                                             int K, int W, PeakOut out, const int32_t *__restrict__ counts)
 {
     constexpr int vsz = M * M * 2;
     __shared__ __align__(16) double sV[SCAN_B * vsz];
@@ -1305,6 +1317,7 @@ __global__ void __launch_bounds__(TILE, 3) scan_peak1_kernel(const double *__res
         for (int q = 1; q < WPG; ++q)
             if (peak_better(rP[b][q], rk[b][q], P, kk)) { P = rP[b][q]; kk = rk[b][q]; }
         const size_t o = (size_t)(w0 + b);
+        if (counts && counts[o] == 0) kk = -1;
         if (kk >= 0) {
             out.angles[o] = (float)((double)kk * 360.0 / (double)K);  // :134, :153
             if (out.levels) out.levels[o] = (float)P;                 // :154
@@ -1318,20 +1331,22 @@ __global__ void __launch_bounds__(TILE, 3) scan_peak1_kernel(const double *__res
 
 // Top-n for n >= 2 from the fp64 strengths: one warp per window, n rounds of a warp arg-max in
 // the reference's total order (P desc, bin asc; P > 0 strictly; NaN never) - equivalent to the
-// insertion loop at :129-141.
-__global__ void __launch_bounds__(256) topn_kernel(const double *__restrict__ P64, int n, int K, int W, PeakOut out)
+// insertion loop at :129-141.  counts (may be null, music_sources.cuh): window w fills only its first counts[w] slots.
+__global__ void __launch_bounds__(256) topn_kernel(const double *__restrict__ P64, int n, int K, int W, PeakOut out,
+                                                   const int32_t *__restrict__ counts)
 {
     const int w = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (w >= W) return;
     const double *P = P64 + (size_t)w * K;
+    const int nr = counts ? counts[w] : n;
     double prevP = 0.0;
     int prevk = -1;
     bool first = true;
     for (int r = 0; r < n; ++r) {
         double bP = 0.0;
         int bk = -1;
-        if (first || prevk >= 0) {
+        if (r < nr && (first || prevk >= 0)) {
             for (int k = lane; k < K; k += 32) {
                 const double p = P[k];
                 const bool after = first || (p < prevP) || (p == prevP && k > prevk);
@@ -1364,8 +1379,9 @@ __global__ void __launch_bounds__(256) topn_kernel(const double *__restrict__ P6
 // Opt-in peak rule (not in the reference; SURVEY.md section 8(f) rank 3, oracle/music_oracle.py::pick_local_maxima):
 // the n largest circular local maxima of P, at least `excl` + 1 bins apart.  One warp per window; pass r finds the
 // best remaining candidate (P[k] > 0, P[k] > P[k-1], P[k] >= P[k+1], farther than excl bins from every peak taken
-// so far; ties -> lowest k).
-__global__ void __launch_bounds__(256) topn_local_kernel(const double *__restrict__ P64, int n, int K, int W, int excl, PeakOut out)
+// so far; ties -> lowest k).  counts (may be null, music_sources.cuh): window w fills only its first counts[w] slots.
+__global__ void __launch_bounds__(256) topn_local_kernel(const double *__restrict__ P64, int n, int K, int W, int excl, PeakOut out,
+                                                         const int32_t *__restrict__ counts)
 {
     __shared__ int taken_all[8][MAXM];  // per warp: bins of the picks made so far
     const int w = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -1373,11 +1389,12 @@ __global__ void __launch_bounds__(256) topn_local_kernel(const double *__restric
     if (w >= W) return;
     volatile int *taken = taken_all[threadIdx.x >> 5];
     const double *P = P64 + (size_t)w * K;
+    const int nr = counts ? counts[w] : n;
     bool dry = false;
     for (int r = 0; r < n; ++r) {
         double bP = 0.0;
         int bk = -1;
-        if (!dry) {
+        if (!dry && r < nr) {
             for (int k = lane; k < K; k += 32) {
                 const double p = P[k];
                 if (!(p > 0.0) || !(p > bP)) continue;  // also skips NaN; an equal p at a higher k never wins

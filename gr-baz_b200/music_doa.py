@@ -108,6 +108,26 @@ class music_doa(object):
             raise ValueError("mode must be one of %s" % sorted(modes))
         _capi.check(self._lib.music_b200_set_peak_mode(self._h, modes[mode], int(exclusion_bins)), self._h)
 
+    # -- extension: per-window estimate of the number of sources ---------------------------------
+    SOURCE_RULES = {"fixed": 0, "mdl": 1, "aic": 2}
+
+    def set_source_rule(self, rule="fixed"):
+        """``"fixed"`` (default): every window has the n sources given at construction.  ``"mdl"`` / ``"aic"``: n is
+        the maximum, and each window's count d in [0, n] is estimated from its covariance eigenvalues (Wax-Kailath
+        MDL / AIC, include/music_b200.h); the peak rule fills the first d slots, the rest stay (0, 0, bin -1).
+        Needs more snapshots than antennas (nsamples / m > m)."""
+        if rule not in self.SOURCE_RULES:
+            raise ValueError("rule must be one of %s" % sorted(self.SOURCE_RULES))
+        _capi.check(self._lib.music_b200_set_source_rule(self._h, self.SOURCE_RULES[rule]), self._h)
+        self._source_rule = rule
+
+    def source_rule(self):
+        return getattr(self, "_source_rule", "fixed")
+
+    def last_counts(self):
+        """int32 (W,) number of sources of each window of the last work() call (all n under the "fixed" rule)."""
+        return self._last_counts
+
     # -- extension (SURVEY.md section 8(f) rank 4): GUI-rate reducers -----------------------------
     def reduce_angles(self, angles, levels=None, weighted=False):
         """Circular mean (degrees), mean resultant length and total weight per angle slot over the
@@ -160,9 +180,14 @@ class music_doa(object):
         lvl = outs[1] if len(outs) > 1 else None
         spec = outs[2] if len(outs) > 2 else None
         self._last_bins = np.empty((W, self.n), np.int32)
-        rc = self._lib.music_b200_process_host(
-            self._h, x.ctypes.data, W, ang.ctypes.data, lvl.ctypes.data if lvl is not None else None,
-            spec.ctypes.data if spec is not None else None, self._last_bins.ctypes.data)
+        lvl_p, spec_p = lvl.ctypes.data if lvl is not None else None, spec.ctypes.data if spec is not None else None
+        if self.source_rule() == "fixed":
+            rc = self._lib.music_b200_process_host(self._h, x.ctypes.data, W, ang.ctypes.data, lvl_p, spec_p, self._last_bins.ctypes.data)
+            self._last_counts = np.full(W, self.n, np.int32)
+        else:
+            self._last_counts = np.empty(W, np.int32)
+            rc = self._lib.music_b200_process_host_counts(self._h, x.ctypes.data, W, ang.ctypes.data, lvl_p, spec_p,
+                                                          self._last_bins.ctypes.data, self._last_counts.ctypes.data)
         _capi.check(rc, self._h)
         return W
 
@@ -172,8 +197,16 @@ class music_doa(object):
         return self._last_bins
 
     def process_device(self, d_in, nwindows, d_angles, d_levels=None, d_spectrum=None, d_bins=None,
-                       stream=None, d_P64=None, d_R=None, d_eigvals=None):
-        """Raw device-pointer entry (ints); buffers stay resident in HBM."""
+                       stream=None, d_P64=None, d_R=None, d_eigvals=None, d_counts=None):
+        """Raw device-pointer entry (ints); buffers stay resident in HBM.  ``d_counts``: int32 [nwindows] device
+        array that receives the per-window source counts (music_b200_process_device_counts; no fp64 internals)."""
+        if d_counts is not None:
+            if d_P64 is not None or d_R is not None or d_eigvals is not None:
+                raise ValueError("d_counts cannot be combined with d_P64 / d_R / d_eigvals")
+            rc = self._lib.music_b200_process_device_counts(
+                self._h, d_in, int(nwindows), d_angles, d_levels, d_spectrum, d_bins, d_counts, stream)
+            _capi.check(rc, self._h)
+            return
         rc = self._lib.music_b200_process_device_ex(
             self._h, d_in, int(nwindows), d_angles, d_levels, d_spectrum, d_bins, d_P64, d_R, d_eigvals, stream)
         _capi.check(rc, self._h)

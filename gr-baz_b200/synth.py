@@ -123,7 +123,7 @@ def window_params(cfg, seed: int, w0: int = 0, W: int = 0, indices=None):
         for s in range(S):
             hb = _h32(h1 ^ (0x9E3779B1 * (s + 1) & M32))
             cols.append(((hb % K) + frac) * 360.0 / K)
-        ang = np.stack(cols, axis=1)
+        ang = np.stack(cols, axis=1) if S else np.zeros((len(w), 0))  # n = 0: noise-only windows
     a = steering(cfg["antenna_array"], ang)  # (W, S, M) c128, unit power per source
     jpow = np.array([1, 1j, -1, -1j], dtype=np.complex128)
     rot = a[..., None] * jpow  # (W, S, M, 4)
@@ -158,7 +158,8 @@ def gen_windows_numpy(cfg, seed: int, w0: int = 0, W: int = 0, indices=None):
         rs = np.ascontiguousarray(rot32[:, s].transpose(0, 2, 1, 3))  # (W, 4, M, 2)
         term = rs[np.arange(W)[:, None], sym]  # (W, N, M, 2)
         sig = term if sig is None else sig + term
-    x = sig + x
+    if sig is not None:
+        x = sig + x
     return np.ascontiguousarray(x.reshape(W, N * M * 2)).view(np.complex64)
 
 
@@ -196,7 +197,8 @@ def gen_windows_torch(cfg, seed: int, w0: int, W: int, device, out=None, chunk: 
             rs = rot[:, s].permute(0, 2, 1, 3).contiguous()  # (cw, 4, M, 2)
             term = rs[ar, sym]  # (cw, N, M, 2)
             sig = term if sig is None else sig + term
-        x = sig + x
+        if sig is not None:
+            x = sig + x
         out[c0 : c0 + cw] = x.reshape(cw, N * M * 2)
     return out
 

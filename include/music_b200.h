@@ -121,6 +121,25 @@ int music_b200_set_table(music_b200 *h, const float *table_c64);
 int music_b200_set_peak_mode(music_b200 *h, int mode, uint32_t exclusion_bins);
 
 /*
+ * Source-count rule (extension, no reference counterpart).  MUSIC_B200_SOURCES_FIXED (default) uses the n of
+ * create() for every window.  With MUSIC_B200_SOURCES_MDL or _AIC, n becomes the MAXIMUM number of sources: for each
+ * window the engine estimates d in [0, n] from the window's ascending eigenvalues l_0 <= ... <= l_{m-1} and the
+ * N = nsamples / m snapshots (Wax & Kailath, 1985).  For d = 0 .. n, p = m - d, sums over i = 0 .. p-1:
+ *     L(d) = N (p log(sum l_i / p) - sum log l_i)
+ *     MDL(d) = L(d) + d (2m - d) log(N) / 2          AIC(d) = 2 L(d) + 2 d (2m - d)
+ * d is the smallest minimiser (NaN never wins), and 0 when l_0 <= 0 or any eigenvalue is not finite.  The noise
+ * subspace is then the m - d smallest-eigenvalue eigenvectors, the peak rule fills the first d slots and slots
+ * d .. n-1 stay unfilled (angle 0, level 0, bin -1).  With d = 0 the spectrum is 1 / ||a||^2 and no peak is reported.
+ * MDL and AIC run the unfused kernels (the fused m = 4 / m = 8 kernels do not compute every eigenvalue).
+ * Returns EINVAL for an unknown rule, or for MDL / AIC when N <= m (R is rank-deficient, the criteria meaningless).
+ * Applies to later process_*() calls and to every device of a multi-device handle.
+ */
+#define MUSIC_B200_SOURCES_FIXED 0
+#define MUSIC_B200_SOURCES_MDL 1
+#define MUSIC_B200_SOURCES_AIC 2
+int music_b200_set_source_rule(music_b200 *h, int rule);
+
+/*
  * Downstream reducers (extension, no reference counterpart): what a GUI-rate consumer such as the DOA
  * compass (/root/reference/python/doa_compass_control.py:102-108) or a plot sink
  * (/root/reference/python/plot_sink.py:38) needs from millions of windows per second.
@@ -220,6 +239,16 @@ int music_b200_process_device_ex(music_b200 *h, const float *d_in_c64, uint32_t 
                                  float *d_angles, float *d_levels, float *d_spectrum,
                                  int32_t *d_bins, double *d_P64, double *d_R,
                                  double *d_eigvals, void *stream);
+
+/*
+ * process_host / process_device plus the per-window source counts (music_b200_set_source_rule):
+ * counts / d_counts: int32 [nwindows] in host / device memory (may be NULL), in stream order on a multi-device handle.
+ * Under the FIXED rule every count is n.  The planar and sharded entries honour the rule too, but return no counts.
+ */
+int music_b200_process_host_counts(music_b200 *h, const float *in_c64, uint32_t nwindows, float *angles, float *levels,
+                                   float *spectrum, int32_t *bins, int32_t *counts);
+int music_b200_process_device_counts(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_angles,
+                                     float *d_levels, float *d_spectrum, int32_t *d_bins, int32_t *d_counts, void *stream);
 
 /* Number of CUDA kernels this handle has launched so far (bench.py's gpu_launches). */
 uint64_t music_b200_launch_count(const music_b200 *h);

@@ -69,7 +69,7 @@ baz_music_doa::baz_music_doa(unsigned int m, unsigned int n, unsigned int nsampl
                              const array_response_t &array_response, unsigned int resolution)
     : gr::sync_block("music_doa", gr::io_signature::make(1, 1, nsamples * sizeof(gr_complex)),
                      gr::io_signature::make3(1, 3, n * sizeof(float), n * sizeof(float), resolution * sizeof(float))),
-      d_m(m), d_n(n), d_nsamples(nsamples), d_resolution(resolution), d_handle(NULL)
+      d_m(m), d_n(n), d_nsamples(nsamples), d_resolution(resolution), d_handle(NULL), d_source_rule(MUSIC_B200_SOURCES_FIXED)
 {
     if (array_response.size() != resolution) throw std::invalid_argument("music_doa: array_response.size() != resolution");
     const std::vector<float> table = flatten(array_response);
@@ -141,6 +141,15 @@ void baz_music_doa::set_peak_mode(int mode, unsigned int exclusion_bins)
     if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa: ") + music_b200_last_error(d_handle));
 }
 
+/* Extension (not in the reference): per-window estimate of the number of sources, see include/music_b200.h. */
+void baz_music_doa::set_source_rule(int rule)
+{
+    gr::thread::scoped_lock guard(d_mutex);
+    const int rc = music_b200_set_source_rule(d_handle, rule);
+    if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa: ") + music_b200_last_error(d_handle));
+    d_source_rule = rule;
+}
+
 int baz_music_doa::work(int noutput_items, gr_vector_const_void_star &input_items, gr_vector_void_star &output_items)
 {
     if (noutput_items <= 0) return 0;
@@ -151,7 +160,14 @@ int baz_music_doa::work(int noutput_items, gr_vector_const_void_star &input_item
 
     gr::thread::scoped_lock guard(d_mutex);
     d_bins.resize((size_t)noutput_items * d_n);
-    const int rc = music_b200_process_host(d_handle, in, (uint32_t)noutput_items, out, lvl, out_spectrum, d_bins.data());
+    int rc;
+    if (d_source_rule == MUSIC_B200_SOURCES_FIXED) {
+        rc = music_b200_process_host(d_handle, in, (uint32_t)noutput_items, out, lvl, out_spectrum, d_bins.data());
+        d_counts.assign((size_t)noutput_items, (int)d_n);
+    } else {
+        d_counts.resize((size_t)noutput_items);
+        rc = music_b200_process_host_counts(d_handle, in, (uint32_t)noutput_items, out, lvl, out_spectrum, d_bins.data(), d_counts.data());
+    }
     if (rc != MUSIC_B200_OK) throw std::runtime_error(std::string("music_doa: ") + music_b200_last_error(d_handle));
     return noutput_items;
 }

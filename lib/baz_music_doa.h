@@ -53,10 +53,15 @@ public:
     void set_array_geometry(const std::vector<std::vector<double> > &positions_xy, double wavelength);
     /* extension: 0 = the reference's n largest bins (default), 1 = n largest local maxima > exclusion_bins apart */
     void set_peak_mode(int mode, unsigned int exclusion_bins);
+    /* extension: 0 = n sources in every window (default), 1 = MDL, 2 = AIC estimate of 0..n sources per window */
+    void set_source_rule(int rule);
 
     /* Integer peak-bin indices of the items produced by the last work() call, [items][n]
      * (not in the reference; -1 marks a slot the reference would leave at (0, 0)). */
     const std::vector<int> &last_bins() const { return d_bins; }
+    /* Number of sources of each item produced by the last work() call, [items] (n unless set_source_rule() chose
+     * MDL or AIC; slots at and beyond the count are left at (0, 0) with bin -1). */
+    const std::vector<int> &last_counts() const { return d_counts; }
 
 private:
     std::vector<float> flatten(const array_response_t &array_response) const;
@@ -67,6 +72,8 @@ private:
     unsigned int d_resolution;
     music_b200 *d_handle;
     std::vector<int> d_bins;
+    std::vector<int> d_counts;
+    int d_source_rule;
     gr::thread::mutex d_mutex;
 };
 

@@ -4,6 +4,8 @@
 // outputs next to it; the Python test compares them with the oracle.
 //   file layout (little endian): u32 m, n, nsamples, resolution, nwindows;
 //                                table[resolution*m*2] f32; table2[resolution*m*2] f32; in[nwindows*nsamples*2] f32
+// With a third argument RULE (1 = MDL, 2 = AIC) it instead runs one work() call with 3 outputs under that source rule
+// and writes angles, levels, spectrum, bins and the per-window counts (table2 is not used).
 #include <baz_music_doa.h>
 
 #include <cstdio>
@@ -17,6 +19,31 @@ static array_response_t to_response(const float *t, unsigned K, unsigned m)
     for (unsigned k = 0; k < K; ++k)
         for (unsigned i = 0; i < m; ++i) r[k][i] = gr_complex(t[2 * (k * m + i)], t[2 * (k * m + i) + 1]);
     return r;
+}
+
+static int run_source_rule(baz_music_doa_sptr blk, int rule, unsigned n, unsigned K, unsigned W, const std::vector<float> &in,
+                           const char *out_path)
+{
+    bool threw = false;
+    try { blk->set_source_rule(7); } catch (const std::invalid_argument &) { threw = true; }
+    if (!threw) { fprintf(stderr, "expected invalid_argument for source rule 7\n"); return 3; }
+    blk->set_source_rule(rule);
+    std::vector<float> ang((size_t)W * n), lvl((size_t)W * n), spec((size_t)W * K);
+    gr_vector_const_void_star ins(1, in.data());
+    gr_vector_void_star outs;
+    outs.push_back(ang.data()); outs.push_back(lvl.data()); outs.push_back(spec.data());
+    if (blk->work((int)W, ins, outs) != (int)W) return 5;
+    const std::vector<int> bins = blk->last_bins(), counts = blk->last_counts();
+    if (counts.size() != W) return 5;
+    FILE *o = fopen(out_path, "wb");
+    if (!o) return 2;
+    fwrite(ang.data(), 4, ang.size(), o);
+    fwrite(lvl.data(), 4, lvl.size(), o);
+    fwrite(spec.data(), 4, spec.size(), o);
+    fwrite(bins.data(), 4, bins.size(), o);
+    fwrite(counts.data(), 4, counts.size(), o);
+    fclose(o);
+    return 0;
 }
 
 int main(int argc, char **argv)
@@ -39,6 +66,7 @@ int main(int argc, char **argv)
     if (!threw) { fprintf(stderr, "expected invalid_argument for n == m\n"); return 3; }
 
     baz_music_doa_sptr blk = baz_make_music_doa(m, n, ns, to_response(t1.data(), K, m), K);
+    if (argc > 3) return run_source_rule(blk, atoi(argv[3]), n, K, W, in, argv[2]);
     if (blk->input_signature()->sizeof_stream_item(0) != (int)(ns * sizeof(gr_complex))) return 4;
     if (blk->output_signature()->max_streams() != 3 || blk->output_signature()->sizeof_stream_item(2) != (int)(K * 4)) return 4;
 
