@@ -28,6 +28,7 @@
 #include "music_planar.cuh"
 #include "music_reduce.cuh"
 #include "music_sources.cuh"
+#include "music_refine.cuh"
 
 using namespace music;
 
@@ -41,12 +42,15 @@ struct DeviceTable {
     double *soa = nullptr;  // [ntiles][2M+1][TILE]
     unsigned char *fz = nullptr;  // fused kernel's tensor-core screen layout (music_fused.cuh, M = 4 only)
     float *na_max = nullptr;      // max ||a||^2 over the table rows (screen threshold)
+    bool geometric = false;       // built by set_geometry() from `geo` (set_table() tables are not)
+    RefineGeom geo = {};          // element positions and wavelength of a geometric table (peak refinement)
 };
 
 struct Workspace {
     double *R = nullptr, *ev = nullptr, *Vt = nullptr, *P64 = nullptr;
     int32_t *cnt = nullptr;  // per-window source counts (source rule other than FIXED)
-    uint32_t cap = 0, p64_cap = 0, cnt_cap = 0;
+    int32_t *bins = nullptr; // [cap][n] peak bins for the refinement when the caller asked for none
+    uint32_t cap = 0, p64_cap = 0, cnt_cap = 0, bins_cap = 0;
     cudaEvent_t scan_done = nullptr;
     bool used = false;
 };
@@ -71,6 +75,7 @@ struct music_b200 {
     int peak_mode = MUSIC_B200_PEAKS_TOP_BINS;  // set_peak_mode()
     uint32_t peak_excl = 0;
     int source_rule = MUSIC_B200_SOURCES_FIXED;  // set_source_rule()
+    int refine = MUSIC_B200_REFINE_OFF;          // set_refine()
     unsigned steer_guarded = 0;    // entries of the last built table re-evaluated with the host libm
 
     // fp64 workspace slots (R, eigenvalues, sorted eigenvectors, optional strengths) of the unfused path: one per
@@ -177,6 +182,7 @@ int finish_table(music_b200 *h, int slot, cudaStream_t st)
 
 int upload_table(music_b200 *h, int slot, const float *table_c64, cudaStream_t st)
 {
+    h->table[slot].geometric = false;
     CU(h, cudaMemcpyAsync(h->table[slot].c64, table_c64, (size_t)h->K * h->m * 2 * sizeof(float), cudaMemcpyHostToDevice, st));
     return finish_table(h, slot, st);
 }
@@ -187,6 +193,7 @@ int build_table(music_b200 *h, int slot, const double *pos_xy, double lambda, cu
 {
     DeviceTable &t = h->table[slot];
     const int K = (int)h->K, M = (int)h->m;
+    t.geometric = false;
     if (!h->steer_pos) {
         CU(h, cudaMalloc(&h->steer_pos, sizeof(double) * 2 * MUSIC_B200_MAX_M));
         CU(h, cudaMalloc(&h->steer_count, sizeof(unsigned)));
@@ -224,7 +231,12 @@ int build_table(music_b200 *h, int slot, const double *pos_xy, double lambda, cu
         CU(h, cudaGetLastError());
         CU(h, cudaStreamSynchronize(st));  // vals is a local
     }
-    return finish_table(h, slot, st);
+    const int rc = finish_table(h, slot, st);
+    if (rc) return rc;
+    t.geometric = true;
+    for (int i = 0; i < 2 * M; ++i) t.geo.pos[i] = pos_xy[i];
+    t.geo.lambda = lambda;
+    return MUSIC_B200_OK;
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
@@ -262,7 +274,8 @@ constexpr unsigned CTR_RING = 256;  // ticket-counter pairs per slot (see ticket
 uint32_t max_sub_windows(const music_b200 *h, bool need_p64)
 {
     const size_t per_win = (size_t)h->m * h->m * 2 * 8 * 2 + h->m * 8 + (need_p64 ? (size_t)h->K * 8 : 0) +
-                           (h->source_rule != MUSIC_B200_SOURCES_FIXED ? sizeof(int32_t) : 0);
+                           (h->source_rule != MUSIC_B200_SOURCES_FIXED ? sizeof(int32_t) : 0) +
+                           (h->refine != MUSIC_B200_REFINE_OFF ? h->n * sizeof(int32_t) : 0);
     size_t c = ((size_t)384 << 20) / per_win;
     c = std::max<size_t>(SCAN_B, std::min<size_t>(c, 1u << 20));
     return (uint32_t)(c / SCAN_B * SCAN_B);
@@ -292,6 +305,12 @@ int ensure_slot(music_b200 *h, Workspace &ws, uint32_t windows, bool need_p64)
         cudaFree(ws.cnt); ws.cnt = nullptr; ws.cnt_cap = 0;
         CU(h, cudaMalloc(&ws.cnt, (size_t)windows * sizeof(int32_t)));
         ws.cnt_cap = windows;
+    }
+    if (h->refine != MUSIC_B200_REFINE_OFF && windows > ws.bins_cap) {
+        if (ws.used) CU(h, cudaEventSynchronize(ws.scan_done));
+        cudaFree(ws.bins); ws.bins = nullptr; ws.bins_cap = 0;
+        CU(h, cudaMalloc(&ws.bins, (size_t)windows * h->n * sizeof(int32_t)));
+        ws.bins_cap = windows;
     }
     return MUSIC_B200_OK;
 }
@@ -460,11 +479,17 @@ __global__ void gather_wait_kernel(const unsigned *flags, int npeer, unsigned ep
 
 // K2 (+ source count) + K3 (+ top-n) of W windows from ws.R, on `st`.  tev (optional) = timing events [1..4].
 // d_counts_out (may be NULL): the caller's copy of the per-window source counts (source rule other than FIXED).
-int launch_eig_scan(music_b200 *h, const Workspace &ws, uint32_t W, const PeakOut &po, float *d_spec,
+// With refinement on, the refine kernel follows the peak rule (timed with top-n) and reads the bins it wrote: from the
+// caller's array, or from the workspace when the caller asked for none.
+int launch_eig_scan(music_b200 *h, const Workspace &ws, uint32_t W, const PeakOut &po_in, float *d_spec,
                     double *d_P64_out, double *d_R_out, double *d_ev_out, int32_t *d_counts_out, cudaStream_t st, cudaEvent_t *tev)
 {
     const int M = (int)h->m;
-    const double *soa = h->table[h->cur_table].soa;
+    const DeviceTable &tb = h->table[h->cur_table];
+    const double *soa = tb.soa;
+    const bool refine = h->refine != MUSIC_B200_REFINE_OFF;
+    PeakOut po = po_in;
+    if (refine && !po.bins) po.bins = ws.bins;
     {
         const int grid = (W + 127) / 128;
         switch (M) {
@@ -512,6 +537,12 @@ int launch_eig_scan(music_b200 *h, const Workspace &ws, uint32_t W, const PeakOu
         else topn_kernel<<<(W + 7) / 8, 256, 0, st>>>(p64, (int)h->n, (int)h->K, (int)W, po, cnt);
         h->launches++;
     }
+    if (refine) {
+        const int slots = (int)(W * h->n);
+        refine_peaks_kernel<<<(slots + REFINE_THREADS - 1) / REFINE_THREADS, REFINE_THREADS, 0, st>>>(ws.Vt, cnt, po.bins, M, (int)h->n, (int)h->K, (int)W, tb.geo,
+                                                                po.angles, po.levels);
+        h->launches++;
+    }
     if (tev) cudaEventRecord(tev[4], st);
     if (d_R_out)
         CU(h, cudaMemcpyAsync(d_R_out, ws.R, (size_t)W * M * M * 2 * sizeof(double), cudaMemcpyDeviceToDevice, st));
@@ -546,6 +577,10 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, float *d
     if ((!planar && !d_in) || !d_ang) return fail(h, MUSIC_B200_EINVAL, "d_in_c64 and d_angles must not be NULL");
     if (!planar && (reinterpret_cast<uintptr_t>(d_in) & 15u) != 0) return fail(h, MUSIC_B200_EINVAL, "d_in_c64 must be 16-byte aligned");
     const bool fixed_n = h->source_rule == MUSIC_B200_SOURCES_FIXED;
+    const bool refine = h->refine != MUSIC_B200_REFINE_OFF;
+    if (refine && !h->table[h->cur_table].geometric)
+        return fail(h, MUSIC_B200_EINVAL, "peak refinement needs a table built by music_b200_set_geometry(); the current one came from "
+                                          "set_table() (call set_geometry(), or set_refine(OFF))");
     if (fixed_n && d_counts) {
         fill_counts_kernel<<<(nwindows + 255) / 256, 256, 0, st>>>(d_counts, (int)h->n, (int)nwindows);
         h->launches++;
@@ -558,8 +593,9 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, float *d
         for (uint32_t r = 0; r < h->m; ++r) planar_fusable = planar_fusable && (reinterpret_cast<uintptr_t>(planar->p[r]) & 15u) == 0;
     }
     const bool local_peaks = h->peak_mode == MUSIC_B200_PEAKS_LOCAL_MAXIMA;
-    // the fused kernels find the principal eigenvector only, not every eigenvalue a source count needs
-    if ((!planar || planar_fusable) && h->fused && fixed_n && !local_peaks && h->m == 4 && h->n == 1 && (!d_spec || h->fused_spec) && !d_P64 && !d_R && !d_ev) {
+    // the fused kernels find the principal eigenvector only, not every eigenvalue a source count needs nor the noise
+    // eigenvectors the peak refinement needs
+    if ((!planar || planar_fusable) && h->fused && fixed_n && !refine && !local_peaks && h->m == 4 && h->n == 1 && (!d_spec || h->fused_spec) && !d_P64 && !d_R && !d_ev) {
         // whole call in one persistent launch (music_fused.cuh); no workspace involved
         cudaEvent_t *tev = timing_events(h);
         if (tev) cudaEventRecord(tev[0], st);
@@ -598,7 +634,7 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, float *d
         CU(h, cudaGetLastError());
         return MUSIC_B200_OK;
     }
-    if (!planar && h->fused && fixed_n && !local_peaks && h->m == 8 && h->n == 1 && !d_spec && !d_P64 && !d_R && !d_ev && h->N >= 128 &&
+    if (!planar && h->fused && fixed_n && !refine && !local_peaks && h->m == 8 && h->n == 1 && !d_spec && !d_P64 && !d_R && !d_ev && h->N >= 128 &&
         h->N % 2 == 0 && encode_tiled_fn()) {
         // M = 8: whole call in one persistent launch (music_fused8.cuh); R and the eigenvectors stay in shared memory
         CUtensorMap tm;
@@ -1293,6 +1329,21 @@ int music_b200_set_source_rule(music_b200 *h, int rule)
     return MUSIC_B200_OK;
 }
 
+int music_b200_set_refine(music_b200 *h, int mode)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (mode != MUSIC_B200_REFINE_OFF && mode != MUSIC_B200_REFINE_NEWTON) return fail(h, MUSIC_B200_EINVAL, "unknown refine mode %d", mode);
+    std::lock_guard<std::mutex> g(h->mutex);
+    for (music_b200 *c : h->kids) {
+        const int rc = music_b200_set_refine(c, mode);
+        if (rc) return fail(h, rc, "%s", music_b200_last_error(c));
+    }
+    if (h->kids.empty() && mode != MUSIC_B200_REFINE_OFF && !h->table[h->cur_table].geometric)
+        return fail(h, MUSIC_B200_EINVAL, "peak refinement needs a table built by music_b200_set_geometry(); the current one came from set_table()");
+    h->refine = mode;
+    return MUSIC_B200_OK;
+}
+
 }  // extern "C"
 
 namespace {
@@ -1571,7 +1622,7 @@ void music_b200_destroy(music_b200 *h)
     for (int i = 0; i < 2; ++i) {
         cudaFree(h->table[i].c64); cudaFree(h->table[i].soa); cudaFree(h->table[i].fz); cudaFree(h->table[i].na_max);
         if (h->streams[i]) cudaStreamDestroy(h->streams[i]);
-        cudaFree(h->ws[i].R); cudaFree(h->ws[i].ev); cudaFree(h->ws[i].Vt); cudaFree(h->ws[i].P64); cudaFree(h->ws[i].cnt);
+        cudaFree(h->ws[i].R); cudaFree(h->ws[i].ev); cudaFree(h->ws[i].Vt); cudaFree(h->ws[i].P64); cudaFree(h->ws[i].cnt); cudaFree(h->ws[i].bins);
         if (h->ws[i].scan_done) cudaEventDestroy(h->ws[i].scan_done);
     }
     for (cudaEvent_t e : h->tev) cudaEventDestroy(e);

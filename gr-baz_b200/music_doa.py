@@ -128,6 +128,18 @@ class music_doa(object):
         """int32 (W,) number of sources of each window of the last work() call (all n under the "fixed" rule)."""
         return self._last_counts
 
+    # -- extension: off-grid peak refinement -------------------------------------------------------
+    def set_refine(self, enable):
+        """True: every reported peak is refined off the grid by safeguarded Newton steps on the exact fp64 MUSIC
+        spectrum of the array geometry (include/music_b200.h); angles and levels change, bins and the spectrum stay the
+        grid results.  Needs a table installed with ``set_array_geometry``; False (default) reports grid angles."""
+        _capi.check(self._lib.music_b200_set_refine(self._h, 1 if enable else 0), self._h)
+        self._refine = bool(enable)
+
+    @property
+    def refine(self):
+        return getattr(self, "_refine", False)
+
     # -- extension (SURVEY.md section 8(f) rank 4): GUI-rate reducers -----------------------------
     def reduce_angles(self, angles, levels=None, weighted=False):
         """Circular mean (degrees), mean resultant length and total weight per angle slot over the

@@ -36,7 +36,7 @@ def calculate_antenna_array_response(antenna_array, angular_resolution, l):
 
 class music_doa_helper(object):
     def __init__(self, m, n, nsamples, angular_resolution, frequency, array_spacing, antenna_array,
-                 output_spectrum=False, device=0, device_table=False):
+                 output_spectrum=False, device=0, device_table=False, refine=False):
         self.m = m
         self.n = n
         self.nsamples = nsamples
@@ -47,6 +47,9 @@ class music_doa_helper(object):
         # extension: device_table=True makes set_frequency() rebuild the table on the GPU
         # (music_b200_set_geometry) instead of the K x M Python loop + re-marshalling; same table, bit for bit
         self.device_table = bool(device_table)
+        # extension: refine=True reports off-grid angles (music_b200_set_refine); the block then needs the geometry, so
+        # the table is installed with set_array_geometry (bit-identical to the one computed below) here and on retunes
+        self.refine = bool(refine)
 
         if (nsamples % m) != 0:
             raise Exception("nsamples must be multiple of m")  # :58-59
@@ -61,11 +64,14 @@ class music_doa_helper(object):
         self.array_response = calculate_antenna_array_response(self.antenna_array, self.angular_resolution, self.l)
         self.impl = music_doa(self.m, self.n, self.nsamples, self.array_response, self.angular_resolution,
                               device=device)  # :89
+        if self.refine:
+            self.impl.set_array_geometry(self.antenna_array, self.l)
+            self.impl.set_refine(True)
 
     def set_frequency(self, frequency):
         """:100-103"""
         self.l = 299792458.0 / frequency
-        if self.device_table:
+        if self.device_table or self.refine:
             self.impl.set_array_geometry(self.antenna_array, self.l)
             self.array_response = None  # lives on the device; impl.array_response_c64() reads it back
             return

@@ -140,6 +140,40 @@ int music_b200_set_peak_mode(music_b200 *h, int mode, uint32_t exclusion_bins);
 int music_b200_set_source_rule(music_b200 *h, int rule);
 
 /*
+ * Off-grid peak refinement (extension, no reference counterpart).  MUSIC_B200_REFINE_OFF (default) reports grid
+ * angles k * 360 / K.  With MUSIC_B200_REFINE_NEWTON every filled slot (w, i) with grid bin b >= 0 is moved to the
+ * minimum of the exact MUSIC denominator of the array geometry near b:
+ *   G      the noise eigenvectors the scan used (the m - n smallest, or m - d under MDL / AIC);
+ *   a(t)   the unrounded fp64 steering vector of the current geometry (music_b200_set_geometry), t in radians:
+ *          a_m(t) = exp(-j phi_m),  phi_m = 2 pi (p_x,m cos t + p_y,m sin t) / lambda;
+ *   D(t)   = sum_j |g_j^H a(t)|^2 (always the direct noise-subspace form), with the analytic derivatives
+ *          psi_m = dphi_m/dt = 2 pi (-p_x,m sin t + p_y,m cos t) / lambda,  phi_m'' = -phi_m,
+ *          a' = -j psi a,  a'' = (j phi - psi^2) a,  s = G^H a, s' = G^H a', s'' = G^H a'':
+ *          D' = 2 sum Re(conj(s) s'),  D'' = 2 sum (|s'|^2 + Re(conj(s) s''));
+ *   bracket [lo, hi] = [t_b - delta, t_b + delta], t_b = b * 360 / K degrees, delta = 360 / K degrees.
+ *          If D'(lo) < 0 < D'(hi), safeguarded
+ *          Newton on D' = 0 starts at t_b: a step that would leave the bracket or not halve it is a bisection step
+ *          (rtsafe); it stops at D' = 0 exactly, when a step is at most 1e-12 rad, or after 50 iterations.  The result
+ *          t* is accepted iff t* != t_b and D(t*) <= D(t_b) (same fp64 formula); otherwise the slot keeps t_b.
+ * Outputs: angles[w][i] = (float) of t* in degrees wrapped into [0, 360) (a value that rounds to 360.0f becomes 0.0f;
+ * a kept slot keeps its grid angle); levels[w][i] = (float)(1 / D(t*)).  bins, spectrum, P64, R, eigenvalues and
+ * counts are the grid results, unchanged; unfilled slots stay (0, 0, bin -1).
+ * Caveats: with refinement on a level is the analytic fp64 spectrum, not the value from the float32-rounded table.  P
+ * is conditioned about 4000x (DESIGN.md section 3), so even where t* = t_b the level can differ from the unrefined
+ * level by about 1e-4 relative.  With TOP_BINS and n >= 2, neighbouring bins of one peak can refine to the same angle:
+ * use MUSIC_B200_PEAKS_LOCAL_MAXIMA for n >= 2.
+ * Refinement runs the unfused kernels (the fused m = 4 / m = 8 kernels keep only the principal eigenvector) plus one
+ * fp64 kernel per sub-batch, timed in the top-n slot of the stage timing.
+ * Returns EINVAL for an unknown mode, and for NEWTON when the current table came from music_b200_set_table() (it has
+ * no geometry).  A process_*() call with refinement on whose current table came from set_table() (set_table() after
+ * set_refine()) fails with EINVAL; there is no silent fall-back to grid angles.
+ * Applies to later process_*() calls and to every device of a multi-device handle.
+ */
+#define MUSIC_B200_REFINE_OFF 0
+#define MUSIC_B200_REFINE_NEWTON 1
+int music_b200_set_refine(music_b200 *h, int mode);
+
+/*
  * Downstream reducers (extension, no reference counterpart): what a GUI-rate consumer such as the DOA
  * compass (/root/reference/python/doa_compass_control.py:102-108) or a plot sink
  * (/root/reference/python/plot_sink.py:38) needs from millions of windows per second.

@@ -150,6 +150,15 @@ void baz_music_doa::set_source_rule(int rule)
     d_source_rule = rule;
 }
 
+/* Extension (not in the reference): off-grid peak refinement on the exact spectrum of the array geometry, see
+   include/music_b200.h.  Needs a table installed with set_array_geometry(). */
+void baz_music_doa::set_refine(bool enable)
+{
+    gr::thread::scoped_lock guard(d_mutex);
+    const int rc = music_b200_set_refine(d_handle, enable ? MUSIC_B200_REFINE_NEWTON : MUSIC_B200_REFINE_OFF);
+    if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa: ") + music_b200_last_error(d_handle));
+}
+
 int baz_music_doa::work(int noutput_items, gr_vector_const_void_star &input_items, gr_vector_void_star &output_items)
 {
     if (noutput_items <= 0) return 0;

@@ -55,6 +55,9 @@ public:
     void set_peak_mode(int mode, unsigned int exclusion_bins);
     /* extension: 0 = n sources in every window (default), 1 = MDL, 2 = AIC estimate of 0..n sources per window */
     void set_source_rule(int rule);
+    /* extension: true = refine every peak off the grid on the exact spectrum of the geometry set by
+     * set_array_geometry() (bins stay the grid bins); false = grid angles (default) */
+    void set_refine(bool enable);
 
     /* Integer peak-bin indices of the items produced by the last work() call, [items][n]
      * (not in the reference; -1 marks a slot the reference would leave at (0, 0)). */

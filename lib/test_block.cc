@@ -5,7 +5,9 @@
 //   file layout (little endian): u32 m, n, nsamples, resolution, nwindows;
 //                                table[resolution*m*2] f32; table2[resolution*m*2] f32; in[nwindows*nsamples*2] f32
 // With a third argument RULE (1 = MDL, 2 = AIC) it instead runs one work() call with 3 outputs under that source rule
-// and writes angles, levels, spectrum, bins and the per-window counts (table2 is not used).
+// and writes angles, levels, spectrum, bins and the per-window counts (table2 is not used).  With a fourth argument
+// GEOM (a file of m (x, y) f64 positions in metres followed by the f64 wavelength) it also installs that geometry with
+// set_array_geometry() and turns the peak refinement on before the work() call (RULE 0 keeps the fixed source count).
 #include <baz_music_doa.h>
 
 #include <cstdio>
@@ -19,6 +21,25 @@ static array_response_t to_response(const float *t, unsigned K, unsigned m)
     for (unsigned k = 0; k < K; ++k)
         for (unsigned i = 0; i < m; ++i) r[k][i] = gr_complex(t[2 * (k * m + i)], t[2 * (k * m + i) + 1]);
     return r;
+}
+
+// geometry file -> set_array_geometry(), then set_refine(true); the table-only block must refuse the refinement first
+static int install_geometry_and_refine(baz_music_doa_sptr blk, unsigned m, const char *geom_path)
+{
+    FILE *g = fopen(geom_path, "rb");
+    if (!g) return 2;
+    std::vector<double> v(2 * (size_t)m + 1);
+    const size_t got = fread(v.data(), 8, v.size(), g);
+    fclose(g);
+    if (got != v.size()) return 2;
+    bool threw = false;
+    try { blk->set_refine(true); } catch (const std::invalid_argument &) { threw = true; }
+    if (!threw) { fprintf(stderr, "expected invalid_argument for set_refine on a table without geometry\n"); return 3; }
+    std::vector<std::vector<double> > pos(m, std::vector<double>(2));
+    for (unsigned i = 0; i < m; ++i) { pos[i][0] = v[2 * i]; pos[i][1] = v[2 * i + 1]; }
+    blk->set_array_geometry(pos, v[2 * (size_t)m]);
+    blk->set_refine(true);
+    return 0;
 }
 
 static int run_source_rule(baz_music_doa_sptr blk, int rule, unsigned n, unsigned K, unsigned W, const std::vector<float> &in,
@@ -66,6 +87,10 @@ int main(int argc, char **argv)
     if (!threw) { fprintf(stderr, "expected invalid_argument for n == m\n"); return 3; }
 
     baz_music_doa_sptr blk = baz_make_music_doa(m, n, ns, to_response(t1.data(), K, m), K);
+    if (argc > 4) {
+        const int rc = install_geometry_and_refine(blk, m, argv[4]);
+        if (rc) return rc;
+    }
     if (argc > 3) return run_source_rule(blk, atoi(argv[3]), n, K, W, in, argv[2]);
     if (blk->input_signature()->sizeof_stream_item(0) != (int)(ns * sizeof(gr_complex))) return 4;
     if (blk->output_signature()->max_streams() != 3 || blk->output_signature()->sizeof_stream_item(2) != (int)(K * 4)) return 4;
