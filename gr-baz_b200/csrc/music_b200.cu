@@ -89,8 +89,9 @@ struct music_b200 {
     bool fused_used[2] = {false, false};
     int eig_mode = 0;                 // fused kernel: 0 principal eigenvector by squaring (default), 1 / 2 Jacobi with four lanes / one lane per window (MUSIC_B200_EIG=jacobi|jacobi1)
     unsigned *f8_stats = nullptr;     // fused M = 8 kernel: windows solved by squaring / by the Jacobi fallback
-    int mma_fin_max = 3;              // fused kernel: no tensor-core pass starts once the tickets have run out and this many covariance warps are done (MUSIC_B200_MMA_FIN; 0: at ticket exhaustion, -1: fp64 drain only)
+    int mma_fin_max = 2;              // fused kernel: no tensor-core pass starts once the tickets have run out and this many covariance warps are done (MUSIC_B200_MMA_FIN; 0: at ticket exhaustion, -1: fp64 drain only)
     long long *fused_trace = nullptr;  // MUSIC_B200_TRACE=1: per-CTA clock64 trace of the fused kernel (tools/fused_trace.py)
+    unsigned trace_seq = 0;            // next launch's slot in the trace ring (FZ_TRACE_LAUNCHES launches of FZ_TRACE_CTAS rows)
     bool fused = true;       // MUSIC_B200_FUSED=0 forces the three-kernel path
     // optional per-stage timing (bench.py's roofline leg): events around K1/K2/K3/top-n per chunk
     bool timing = false;
@@ -371,9 +372,9 @@ unsigned *ticket_counter(music_b200 *h, int slot, cudaStream_t st)
     h->fused_used[slot] = true;
     h->last_fused_stream[slot] = st;
     // Every launch draws its own pair from the slot's ring: with programmatic dependent launch the CTAs of launch k + 1
-    // start on the SMs launch k has left while k's last CTAs are still running, so the two must not share tickets.  A
-    // pair is reused CTR_RING launches later; launches on one stream overlap only with their neighbours, and each
-    // persistent CTA owns a whole SM, so fewer than CTR_RING launches are ever resident together.
+    // run next to those of launch k (the fused M = 4 kernel: in the other half of each SM), so the two must not share
+    // tickets.  A pair is reused CTR_RING launches later; launches on one stream overlap only with their neighbours (a
+    // launch's CTAs leave only after the previous launch has finished), so fewer than CTR_RING launches are ever resident together.
     const unsigned e = h->ctr_seq[slot]++ % CTR_RING;
     return h->work_ctr + 2 * ((size_t)slot * CTR_RING + e);
 }
@@ -605,9 +606,10 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, float *d
         const PeakOut po = make_peak_out(h, d_ang, d_lvl, d_bins, 0);
         const GatherFlags gf = make_gather_flags(h, true);
         // Programmatic dependent launch: when the previous operation on `st` is another launch of this kernel, the new
-        // CTAs are placed as soon as the old ones leave their SMs (every CTA signals launch_dependents at its start) instead
-        // of after the whole grid has drained; the kernel orders its own output writes behind the previous grid with
-        // griddepcontrol.wait.  After any other kind of operation the launch is an ordinary stream-ordered one.
+        // CTAs are placed at once in the free half of every SM (every CTA signals launch_dependents at its start; the grid,
+        // at most one CTA per SM, leaves the other half free) instead of after the whole grid has drained; the kernel
+        // orders its own output writes behind the previous grid (fused_emit).  After any other kind of operation the launch
+        // is an ordinary stream-ordered one.
         cudaLaunchConfig_t lc = {};
         lc.gridDim = dim3((unsigned)grid); lc.blockDim = dim3(FZ_THREADS); lc.dynamicSmemBytes = FZ_SMEM; lc.stream = st;
         cudaLaunchAttribute la[1];
@@ -616,16 +618,18 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, float *d
         lc.attrs = la; lc.numAttrs = h->pdl ? 1 : 0;
         const int W_i = (int)nwindows, N_i = (int)h->N, K_i = (int)h->K;
         const bool tr = h->fused_trace != nullptr;  // MUSIC_B200_TRACE=1: the instantiation with the clock64 trace
+        // each launch writes its own slot of the trace ring, so launches that are resident together do not mix their rows
+        long long *trace = tr ? h->fused_trace + (size_t)(h->trace_seq++ % FZ_TRACE_LAUNCHES) * FZ_TRACE_CTAS * FZ_TRACE : nullptr;
         const unsigned char *fz = tb.fz;
         const float *c64 = tb.c64, *na_max = tb.na_max;
         cudaError_t le;
         if (planar) {
             auto kern = tr ? music4_fused_kernel<true, true> : music4_fused_kernel<true, false>;
             le = cudaLaunchKernelEx(&lc, kern, (const float *)nullptr, *planar, 0ull, (unsigned)hop, fz, c64, na_max, W_i, N_i, K_i, po, ctr,
-                                    h->fused_trace, h->eig_mode, gf, h->mma_fin_max, d_spec);
+                                    trace, h->eig_mode, gf, h->mma_fin_max, d_spec);
         } else {
             auto kern = tr ? music4_fused_kernel<false, true> : music4_fused_kernel<false, false>;
-            le = cudaLaunchKernelEx(&lc, kern, d_in, PlanarStreams{}, 0ull, 0u, fz, c64, na_max, W_i, N_i, K_i, po, ctr, h->fused_trace,
+            le = cudaLaunchKernelEx(&lc, kern, d_in, PlanarStreams{}, 0ull, 0u, fz, c64, na_max, W_i, N_i, K_i, po, ctr, trace,
                                     h->eig_mode, gf, h->mma_fin_max, d_spec);
         }
         CU(h, le);
@@ -853,7 +857,8 @@ int music_b200_debug_fused_trace(music_b200 *h, long long *host_out, int max_cta
     std::lock_guard<std::mutex> g(h->mutex);
     CU(h, cudaSetDevice(h->device));
     CU(h, cudaDeviceSynchronize());
-    CU(h, cudaMemcpy(host_out, h->fused_trace, (size_t)std::min(max_ctas, 1024) * FZ_TRACE * sizeof(long long), cudaMemcpyDeviceToHost));
+    CU(h, cudaMemcpy(host_out, h->fused_trace, (size_t)std::min(max_ctas, FZ_TRACE_LAUNCHES * FZ_TRACE_CTAS) * FZ_TRACE * sizeof(long long),
+                     cudaMemcpyDeviceToHost));
     return MUSIC_B200_OK;
 }
 
@@ -948,7 +953,7 @@ int music_b200_create(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsample
         if (const char *e = getenv("MUSIC_B200_EIG")) h->eig_mode = !strcmp(e, "jacobi") ? 1 : !strcmp(e, "jacobi1") ? 2 : 0;
         if (const char *e = getenv("MUSIC_B200_PDL")) h->pdl = atoi(e) != 0;
         if (const char *e = getenv("MUSIC_B200_FUSED_SPEC")) h->fused_spec = atoi(e) != 0;
-        if (const char *e = getenv("MUSIC_B200_MMA_FIN")) h->mma_fin_max = std::max(-1, std::min(8, atoi(e)));
+        if (const char *e = getenv("MUSIC_B200_MMA_FIN")) h->mma_fin_max = std::max(-1, std::min(FZ_COV_WARPS, atoi(e)));
         CU(h, cudaFuncSetAttribute(covN_tma_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CN_SMEM));
         CU(h, cudaFuncSetAttribute(covN_tma_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CN_SMEM));
         CU(h, cudaFuncSetAttribute(music8_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)F8_SMEM));
@@ -959,13 +964,16 @@ int music_b200_create(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsample
         CU(h, cudaMemset(h->work_ctr, 0, 2 * CTR_RING * 2 * sizeof(unsigned)));
         if (const char *e = getenv("MUSIC_B200_HOSTREG")) h->hostreg = atoi(e) != 0;
         if (getenv("MUSIC_B200_TRACE")) {
-            CU(h, cudaMalloc(&h->fused_trace, FZ_TRACE * sizeof(long long) * 1024));
-            CU(h, cudaMemset(h->fused_trace, 0, FZ_TRACE * sizeof(long long) * 1024));
+            const size_t tb = (size_t)FZ_TRACE_LAUNCHES * FZ_TRACE_CTAS * FZ_TRACE * sizeof(long long);
+            CU(h, cudaMalloc(&h->fused_trace, tb));
+            CU(h, cudaMemset(h->fused_trace, 0, tb));
         }
-        CU(h, cudaFuncSetAttribute(music4_fused_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FZ_SMEM));
-        CU(h, cudaFuncSetAttribute(music4_fused_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FZ_SMEM));
-        CU(h, cudaFuncSetAttribute(music4_fused_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FZ_SMEM));
-        CU(h, cudaFuncSetAttribute(music4_fused_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FZ_SMEM));
+        // the fused M = 4 kernel runs two CTAs per SM: all of the SM's unified L1 / shared memory goes to shared memory
+        for (const void *k : {(const void *)music4_fused_kernel<false, false>, (const void *)music4_fused_kernel<true, false>,
+                              (const void *)music4_fused_kernel<false, true>, (const void *)music4_fused_kernel<true, true>}) {
+            CU(h, cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FZ_SMEM));
+            CU(h, cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+        }
         CU(h, cudaFuncSetAttribute(cov4_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)COV_SMEM));
         return upload_table(h, 0, table_c64, h->streams[0]);
     };

@@ -1,14 +1,15 @@
 // music_fused.cuh - FUSED persistent kernel for the headline shape class (M = 4 antennas, n = 1
 // source, peak outputs only): covariance + eigenvectors + pseudospectrum scan + peak pick in
-// ONE launch, one CTA per SM, warp-specialised.  R and the eigenvectors never leave shared memory.
+// ONE launch, persistent CTAs of 8 warps, two per SM (one of this launch, one of the next), warp-specialised.  R and the
+// eigenvectors never leave shared memory.
 //
-//   warps 0..7   covariance (FP64 pipe): per-warp TMA ring exactly as cov4_tma_kernel; a finished
-//                window's R is written to a 64-slot shared-memory queue and marked ready (per-slot flag).
-//   warp  8      eigenvectors, four lanes per queued window (8 windows per round): principal eigenvector by
+//   warps 0..3   covariance (FP64 pipe): per-warp TMA ring exactly as cov4_tma_kernel; a finished
+//                window's R is written to a 32-slot shared-memory queue and marked ready (per-slot flag).
+//   warp  4      eigenvectors, four lanes per queued window (8 windows per round): principal eigenvector by
 //                repeated squaring + Householder basis of its complement (music_eig4p.cuh; 7.5 k cycles per
 //                round under the covariance warps' FP64 load); windows that do not converge (noise only, NaN) go through the full Jacobi solver
 //                (herm_eig4_coop in music_kernels.cuh, ~26 k cycles), which MUSIC_B200_EIG=jacobi selects for all.
-//   warps 9..15  pseudospectrum scan + peak pick, 8 windows per pass (two sweeps of the table):
+//   warps 5..7   pseudospectrum scan + peak pick, 8 windows per pass (two sweeps of the table):
 //                  1. SCREEN on the tensor cores: c_k = e_s^H a_k for all bins k and the 4 windows as a
 //                     [bins x 8] x [8 x 8] product in 3xTF32 (mma.sync m16n8k8, hi/lo split of both
 //                     operands, fp32 accumulate), d~_k = ||a_k||^2 - |c_k|^2 in fp32.  The FP64 pipe -
@@ -32,9 +33,10 @@
 //                FP64 pipe is free by then), merged per group by the warp that finishes the group's last unit.  Same
 //                formula, same tie rule: bit-identical to the tensor-core path, at ~4 k cycles of the whole SM per
 //                window instead of a 35 k-cycle pass.  With the spectrum port connected every window goes this way.
-//   LAUNCH       programmatic dependent launch: the next launch's CTAs take over each SM as this one leaves it
-//                (griddepcontrol.launch_dependents at the start; every writer waits with griddepcontrol.wait before
-//                its first output so that results land in stream order); per-launch ticket counters.
+//   LAUNCH       programmatic dependent launch: the grid takes one half of every SM (grid <= SM count) and signals
+//                griddepcontrol.launch_dependents at its start, so the next launch's CTAs move into the other halves at once
+//                and stream their input while this launch finishes its last windows - no SM's input stream stands still
+//                between calls.  Results still land in stream order (OUTPUT ORDER at fused_emit); per-launch ticket counters.
 //
 // Screen error bound.  a is stored in fp32 exactly (the block's table IS complex64) and split at run
 // time by truncation: a_hi = a & ~0x1fff (|a - a_hi| < 2^-10|a|), a_lo = (a - a_hi) & ~0x1fff (the
@@ -46,7 +48,7 @@
 // fl32(||a||^2).  FZ_B = 2^-15 leaves > 3x margin over this (already pessimistic) bound; a CPU emulation of the
 // screen with truncating fp32 accumulation measures <= 5e-7 ||a||^2, 60x below FZ_B (tests/test_screen_bound.py).
 //
-// INSTRUCTION FOOTPRINT.  Sixteen warps in four roles share one SM's instruction caches (L0 ~6 KB per sub-partition,
+// INSTRUCTION FOOTPRINT.  Sixteen warps in four roles (two CTAs) share one SM's instruction caches (L0 ~6 KB per sub-partition,
 // L1.5 32 KB per SM; beyond that instructions come from the L2, which this kernel keeps saturated with the input stream).
 // The first version of this file inlined everything (211 KB of SASS): code that runs once per pass / per drain unit then
 // cost ~50 cycles per INSTRUCTION (a 500-instruction lane merge: 26 k cycles) while loop bodies ran at ~6.  Hence:
@@ -63,27 +65,33 @@
 
 namespace music {
 
-constexpr int FZ_COV_WARPS = 8;
-constexpr int FZ_SCAN_WARPS = 7;
-constexpr int FZ_THREADS = 32 * (FZ_COV_WARPS + 1 + FZ_SCAN_WARPS);  // 512
-constexpr int FZ_SCAN_THREADS = 32 * FZ_SCAN_WARPS;                  // 224
+// Half an SM per CTA (two CTAs per SM): a launch's grid takes one of the two slots of every SM, so the next launch on the
+// stream is placed in the other slot at once and streams its input while this one finishes its last windows.
+constexpr int FZ_COV_WARPS = 4;
+constexpr int FZ_SCAN_WARPS = 3;
+constexpr int FZ_THREADS = 32 * (FZ_COV_WARPS + 1 + FZ_SCAN_WARPS);  // 256
+constexpr int FZ_SCAN_THREADS = 32 * FZ_SCAN_WARPS;                  // 96
 constexpr int FZ_MPW = 4;        // MMA tiles (16 rows) per scan warp and table tile: more work per ring iteration
                                  // amortises the fixed load -> split -> MMA -> reduce latency chain of a warp
 constexpr int FZ_BINS = 16 * FZ_SCAN_WARPS * FZ_MPW;  // table rows per ring tile
-constexpr int FZ_Q = 64;        // window queue slots per CTA
+constexpr int FZ_Q = 32;        // window queue slots per CTA
 constexpr int FZ_WPT = 8;       // windows per scan pass = 2 column groups of 4 windows x {re, im} (8 MMA columns each)
 constexpr int FZ_STAGES = 4;    // 4 KiB TMA stages per covariance warp
 constexpr int FZ_TS = 3;        // steering-table tile stages (cp.async ring shared by the scan warps)
 constexpr int FZ_FRAG_BYTES = 512;  // one 16 x 8 fp32 A tile in fragment order (16 B per lane)
 constexpr int FZ_TILE_BYTES = (FZ_BINS / 16) * FZ_FRAG_BYTES + FZ_BINS * 4;  // fragment tiles + fp32 ||a||^2
-constexpr int FZ_CMAX = 256;    // exact candidates kept per window before falling back to a full fp64 scan
+constexpr int FZ_CMAX = 192;    // exact candidates kept per window before falling back to a full fp64 scan
 constexpr float FZ_B = 3.0517578125e-05f;  // 2^-15, see "Screen error bound"
 
-constexpr int FZ_TRACE = 32;    // int64 trace words per CTA (MUSIC_B200_TRACE=1)
+constexpr int FZ_TRACE = 40;    // int64 trace words per CTA (MUSIC_B200_TRACE=1)
+constexpr int FZ_TRACE_CTAS = 1024;    // trace rows per launch
+constexpr int FZ_TRACE_LAUNCHES = 32;  // launches kept in the trace ring: launch l writes rows [(l % 32) * 1024, ..)
 constexpr int FZ_DG = 4;         // windows per drain group (= scan_bin's windows per thread)
 constexpr int FZ_NCH = 16;       // interleaved bin chunks per drain group: (group, chunk) is the unit a drain worker (one warp) takes
 constexpr int FZ_NGS = 4;        // drain groups in flight
 constexpr unsigned FZ_IDLE_NS = 100;  // sleep of a drain worker that found no unit
+constexpr int FZ_STG = 64;       // finished windows staged per CTA until the previous launch's outputs are written (fused_emit)
+constexpr int FZ_IPT = 4;        // exact candidates per scan thread and pass (kept in registers)
 
 struct FusedCtl {               // shared-memory control block
     unsigned cov_seq;           // queue sequence numbers handed to finished covariances (atomic)
@@ -98,6 +106,14 @@ struct FusedCtl {               // shared-memory control block
     volatile int dg_open;       // drain group currently handing out chunks (-1: none)
     unsigned drained_windows;   // statistics (trace)
     unsigned drain_groups;
+    unsigned stg_lock;          // spin lock of the output stage
+    volatile unsigned stg_n;    // windows in the output stage
+    volatile unsigned ordered;  // the previous launch's outputs are written: results go straight to global memory
+};
+struct StagedPeak {             // a finished window waiting in the output stage
+    unsigned o;
+    int kk;
+    double P;
 };
 struct DrainGroup {
     volatile unsigned gs;       // first queue sequence number of the group
@@ -107,31 +123,30 @@ struct DrainGroup {
     int pad[3];
 };
 
-constexpr size_t FZ_OFF_TBAR = 512;     // uint64 tfull[FZ_TS], tempty[FZ_TS]
-constexpr size_t FZ_OFF_WRING = 768;    // int wring[FZ_COV_WARPS][8]: window ids claimed by each covariance warp
-constexpr size_t FZ_OFF_CTL = 1024;     // FusedCtl (64 B)
-constexpr size_t FZ_OFF_WIN = 1088;     // int qwin[FZ_Q]
-constexpr size_t FZ_OFF_RMIN = 1344;    // float redmin[FZ_SCAN_WARPS][FZ_WPT]
-constexpr size_t FZ_OFF_CCNT = 1568;    // int cand_cnt[FZ_WPT]
-constexpr size_t FZ_OFF_CBIN = 1664;    // int cand_bin[FZ_WPT][FZ_CMAX]
-constexpr size_t FZ_OFF_RED = 9856;     // double redP[FZ_SCAN_WARPS]; int redk[FZ_SCAN_WARPS]  (fallback scan)
-constexpr size_t FZ_OFF_BEST = 9984;    // u64 bestP[FZ_WPT]; int bestk[FZ_WPT]; int admitted[FZ_WPT]
-constexpr size_t FZ_OFF_QRDY = 10112;   // unsigned qready[FZ_Q]: sequence number + 1 of the R held by the slot
+constexpr size_t fz_align(size_t x, size_t a) { return (x + a - 1) / a * a; }
+// uint64 cov barriers [FZ_COV_WARPS][FZ_STAGES] at offset 0
+constexpr size_t FZ_OFF_TBAR = fz_align(8 * FZ_COV_WARPS * FZ_STAGES, 64);  // uint64 tfull[FZ_TS], tempty[FZ_TS]
+constexpr size_t FZ_OFF_WRING = fz_align(FZ_OFF_TBAR + 16 * FZ_TS, 64);     // int wring[FZ_COV_WARPS][8]: window ids claimed by each covariance warp
+constexpr size_t FZ_OFF_CTL = FZ_OFF_WRING + 32 * FZ_COV_WARPS;             // FusedCtl (64 B)
+constexpr size_t FZ_OFF_WIN = FZ_OFF_CTL + 64;                              // int qwin[FZ_Q]
+constexpr size_t FZ_OFF_RMIN = FZ_OFF_WIN + 4 * FZ_Q;                       // float redmin[FZ_SCAN_WARPS][FZ_WPT]
+constexpr size_t FZ_OFF_CCNT = FZ_OFF_RMIN + 4 * FZ_SCAN_WARPS * FZ_WPT;    // int cand_cnt[FZ_WPT]
+constexpr size_t FZ_OFF_CBIN = FZ_OFF_CCNT + 4 * FZ_WPT;                    // int cand_bin[FZ_WPT][FZ_CMAX]
+constexpr size_t FZ_OFF_RED = fz_align(FZ_OFF_CBIN + 4 * FZ_WPT * FZ_CMAX, 16);  // double redP[FZ_SCAN_WARPS]; int redk[FZ_SCAN_WARPS]  (fallback scan)
+constexpr size_t FZ_OFF_BEST = fz_align(FZ_OFF_RED + 12 * FZ_SCAN_WARPS, 16);    // u64 bestP[FZ_WPT]; int bestk[FZ_WPT]; int admitted[FZ_WPT]
+constexpr size_t FZ_OFF_QRDY = FZ_OFF_BEST + 16 * FZ_WPT;   // unsigned qready[FZ_Q]: sequence number + 1 of the R held by the slot
 constexpr size_t FZ_OFF_QDONE = FZ_OFF_QRDY + 4 * FZ_Q;    // unsigned qdone[FZ_Q]: the slot's window is finished
 constexpr size_t FZ_OFF_DGRP = FZ_OFF_QDONE + 4 * FZ_Q;    // DrainGroup grp[FZ_NGS]
 constexpr size_t FZ_OFF_DRES = FZ_OFF_DGRP + 32 * FZ_NGS;  // double resP[FZ_NGS][FZ_NCH][FZ_DG]; int resk[...]
-constexpr size_t FZ_OFF_RQ = (FZ_OFF_DRES + 12 * FZ_NGS * FZ_NCH * FZ_DG + 255) / 256 * 256;  // double Rq[FZ_Q][32]
+constexpr size_t FZ_OFF_STG = fz_align(FZ_OFF_DRES + 12 * FZ_NGS * FZ_NCH * FZ_DG, 16);  // StagedPeak stg[FZ_STG]
+constexpr size_t FZ_OFF_RQ = fz_align(FZ_OFF_STG + sizeof(StagedPeak) * FZ_STG, 256);   // double Rq[FZ_Q][32]
 constexpr size_t FZ_OFF_VQ = FZ_OFF_RQ + (size_t)FZ_Q * 256;  // double Vq[FZ_Q][32]
 constexpr size_t FZ_OFF_TBL = FZ_OFF_VQ + (size_t)FZ_Q * 256; // FZ_TS table tiles
-constexpr size_t FZ_OFF_RING = (FZ_OFF_TBL + (size_t)FZ_TS * FZ_TILE_BYTES + 127) / 128 * 128;
+constexpr size_t FZ_OFF_RING = fz_align(FZ_OFF_TBL + (size_t)FZ_TS * FZ_TILE_BYTES, 128);
 constexpr size_t FZ_SMEM = FZ_OFF_RING + (size_t)FZ_COV_WARPS * FZ_STAGES * COV_CHUNK;
-static_assert(sizeof(FusedCtl) <= 64 && sizeof(DrainGroup) == 32, "control block layout");
-static_assert(FZ_COV_WARPS * FZ_STAGES * 8 <= FZ_OFF_TBAR, "covariance barriers overlap the table barriers");
-static_assert(FZ_OFF_RMIN + 4 * FZ_SCAN_WARPS * FZ_WPT <= FZ_OFF_CCNT && FZ_OFF_CCNT + 4 * FZ_WPT <= FZ_OFF_CBIN &&
-                  FZ_OFF_CBIN + 4 * FZ_WPT * FZ_CMAX <= FZ_OFF_RED && FZ_OFF_RED + 12 * FZ_SCAN_WARPS <= FZ_OFF_BEST &&
-                  FZ_OFF_BEST + 16 * FZ_WPT <= FZ_OFF_QRDY,
-              "scan scratch layout");
-static_assert(FZ_SMEM <= 227 * 1024, "fused kernel shared memory");
+static_assert(sizeof(FusedCtl) <= 64 && sizeof(DrainGroup) == 32 && sizeof(StagedPeak) == 16, "control block layout");
+// two CTAs per SM: 228 KiB of shared memory per SM, 1 KiB of it reserved per CTA
+static_assert(FZ_SMEM <= (228 - 2 * 1) * 1024 / 2, "fused kernel shared memory: two CTAs must fit on one SM");
 constexpr int FZ_CPT = (FZ_TILE_BYTES / 16 + FZ_SCAN_THREADS - 1) / FZ_SCAN_THREADS;  // 16-byte copies per thread and tile
 static_assert(FZ_TILE_BYTES % 16 == 0, "table tile copy plan");
 
@@ -152,7 +167,7 @@ __device__ __forceinline__ uint32_t to_tf32(float x)
     return r;
 }
 
-// Steering table in the tensor-core screen's layout.  Per 224-row tile: 14 MMA A-fragment tiles
+// Steering table in the tensor-core screen's layout.  Per FZ_BINS-row tile: FZ_BINS / 16 MMA A-fragment tiles
 // (16 rows x 8 columns; the complex64 row [Re a0, Im a0, .., Re a3, Im a3] IS the A row), stored in
 // fragment order - lane l holds {a0..a3} (fp32, split into tf32 hi/lo at run time) with a0 = A[g][t], a1 = A[g+8][t],
 // a2 = A[g][t+4], a3 = A[g+8][t+4], g = l/4, t = l%4 - followed by fl32(||a||^2) per row
@@ -299,21 +314,23 @@ __device__ __forceinline__ void drain_bin(const double (&ar)[4], const double (&
 // `if (lane == 0) { for (;;) { lock ... __nanosleep } }`: after such a block the warp stayed split (lane 0 | lanes 1-31,
 // measured with __activemask() in the TRACE build: every drain unit ran twice, every warp collective took its
 // divergent slow path - 26 k cycles for a 60-shuffle merge).
-__device__ __forceinline__ void fz_lock(FusedCtl *ctl, const int lane)  // all lanes call; lane 0 holds the lock afterwards
+__device__ __forceinline__ void fz_lock(unsigned *lock, const int lane)  // all lanes call; lane 0 holds the lock afterwards
 {
     for (;;) {
         unsigned got = 0u;
-        if (lane == 0) got = atomicCAS(&ctl->lock, 0u, 1u) == 0u ? 1u : 0u;
+        if (lane == 0) got = atomicCAS(lock, 0u, 1u) == 0u ? 1u : 0u;
         if (__shfl_sync(0xffffffffu, got, 0)) break;
     }
     __threadfence_block();
 }
-__device__ __forceinline__ void fz_unlock(FusedCtl *ctl, const int lane)  // all lanes call
+__device__ __forceinline__ void fz_unlock(unsigned *lock, const int lane)  // all lanes call
 {
     __threadfence_block();
-    if (lane == 0) atomicExch(&ctl->lock, 0u);
+    if (lane == 0) atomicExch(lock, 0u);
     __syncwarp();
 }
+__device__ __forceinline__ void fz_lock(FusedCtl *ctl, const int lane) { fz_lock(&ctl->lock, lane); }
+__device__ __forceinline__ void fz_unlock(FusedCtl *ctl, const int lane) { fz_unlock(&ctl->lock, lane); }
 
 // peak of one window -> the block's outputs (reference :134, :153-154; (0, 0) initial pair :95)
 __device__ __forceinline__ void fused_write_peak(const PeakOut &out, const size_t o, const int kk, const double P, const int K)
@@ -326,6 +343,54 @@ __device__ __forceinline__ void fused_write_peak(const PeakOut &out, const size_
         if (out.levels) out.levels[o] = 0.f;
     }
     peak_store_bin(out, o, kk);
+}
+
+// OUTPUT ORDER.  Results must land after those of the previous launch on the stream, which under programmatic dependent
+// launch runs alongside this one (often in the other half of the same SM) for most of this launch.  Waiting for it
+// (griddepcontrol.wait) before the first store would stall the scan, fill the queue and stop the covariance warps, so
+// finished windows are staged in shared memory instead.  The first writer that finds the stage full - or warp 0 at CTA exit -
+// waits for the previous launch once, flushes the stage and marks the CTA `ordered`; from then on results are stored directly.
+// fused_stage_flush: the whole calling warp, holding stg_lock (or alone in the CTA).
+__device__ __noinline__ void fused_stage_flush(unsigned char *smem, const PeakOut out, const int K)
+{
+    FusedCtl *ctl = reinterpret_cast<FusedCtl *>(smem + FZ_OFF_CTL);
+    const StagedPeak *stg = reinterpret_cast<const StagedPeak *>(smem + FZ_OFF_STG);
+    asm volatile("griddepcontrol.wait;" ::: "memory");  // the previous launch has finished and its writes are visible
+    const unsigned n = ctl->stg_n;
+    for (unsigned i = threadIdx.x & 31; i < n; i += 32) fused_write_peak(out, stg[i].o, stg[i].kk, stg[i].P, K);
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) { ctl->stg_n = 0u; ctl->ordered = 1u; }
+    __syncwarp();
+}
+// The peak (kk, P) of window o, for every lane with `valid`; all lanes of one warp call.
+__device__ __forceinline__ void fused_emit(unsigned char *smem, const PeakOut out, const bool valid, const unsigned o, const int kk,
+                                        const double P, const int K)
+{
+    FusedCtl *ctl = reinterpret_cast<FusedCtl *>(smem + FZ_OFF_CTL);
+    StagedPeak *stg = reinterpret_cast<StagedPeak *>(smem + FZ_OFF_STG);
+    const int lane = threadIdx.x & 31;
+    unsigned ord = 0u;
+    if (lane == 0) ord = ctl->ordered;
+    if (!__shfl_sync(0xffffffffu, ord, 0)) {
+        fz_lock(&ctl->stg_lock, lane);
+        const unsigned mask = __ballot_sync(0xffffffffu, valid);
+        unsigned n = 0u;
+        if (lane == 0) { n = ctl->stg_n; ord = ctl->ordered; }
+        n = __shfl_sync(0xffffffffu, n, 0);
+        ord = __shfl_sync(0xffffffffu, ord, 0);
+        if (!ord) {
+            if (n + __popc(mask) > (unsigned)FZ_STG) {
+                fused_stage_flush(smem, out, K);
+                ord = 1u;
+            } else {
+                if (valid) stg[n + __popc(mask & ((1u << lane) - 1u))] = StagedPeak{o, kk, P};
+                if (lane == 0) ctl->stg_n = n + __popc(mask);
+            }
+        }
+        fz_unlock(&ctl->stg_lock, lane);
+        if (!ord) return;
+    }
+    if (valid) fused_write_peak(out, o, kk, P, K);
 }
 
 // windows [start, start + cnt) are finished: mark their queue slots and advance scan_done over every finished slot
@@ -368,7 +433,8 @@ __device__ __noinline__ int fused_drain_worker(unsigned char *smem, const float 
     long long ph[4] = {0, 0, 0, 0};  // trace: table sweep | merge + publish | whole unit | waiting for a unit
     int ndiv0 = 0, ndiv1 = 0;
     const uint64_t pol_keep = l2_policy_evict_last();
-    asm volatile("griddepcontrol.wait;" ::: "memory");  // outputs are written in stream order (no-op once the previous grid is done)
+    // the spectrum rows are stored as they are computed, not staged: they wait for the previous launch here (peaks: fused_emit)
+    if (SPEC) asm volatile("griddepcontrol.wait;" ::: "memory");
     for (;;) {
         int slot = -1, chunk = 0, gc = 0;
         unsigned gs = 0;
@@ -514,17 +580,21 @@ __device__ __noinline__ int fused_drain_worker(unsigned char *smem, const float 
         if (last) {
             // this warp finished the group's last unit: merge the chunks (lane b <-> window b; any order gives the same
             // result, (P desc, bin asc) is a total order)
+            double Pm = 0.0;
+            int km = -1;
+            unsigned o = 0u;
             if (lane < gc) {
-                double Pm = resP[(slot * FZ_NCH) * FZ_DG + lane];
-                int km = resk[(slot * FZ_NCH) * FZ_DG + lane];
+                Pm = resP[(slot * FZ_NCH) * FZ_DG + lane];
+                km = resk[(slot * FZ_NCH) * FZ_DG + lane];
 #pragma unroll 1
                 for (int c = 1; c < FZ_NCH; ++c) {
                     const double Pc = resP[(slot * FZ_NCH + c) * FZ_DG + lane];
                     const int kc = resk[(slot * FZ_NCH + c) * FZ_DG + lane];
                     if (peak_better(Pc, kc, Pm, km)) { Pm = Pc; km = kc; }
                 }
-                fused_write_peak(out, (size_t)qwin[(gs + lane) % FZ_Q], km, Pm, K);
+                o = (unsigned)qwin[(gs + lane) % FZ_Q];
             }
+            fused_emit(smem, out, lane < gc, o, km, Pm, K);
             __syncwarp();
             fused_retire(smem, gs, (unsigned)gc, lane);
             if (lane == 0) {
@@ -542,7 +612,7 @@ __device__ __noinline__ int fused_drain_worker(unsigned char *smem, const float 
 // aligned streams and even first_snapshot, hop and N (bulk copies move multiples of 16 bytes).
 // TRACE = true: the instantiation tools/fused_trace.py runs (MUSIC_B200_TRACE=1): per-CTA clock64 trace in dbg_in.
 template <bool PLANAR, bool TRACE>
-__global__ void __launch_bounds__(FZ_THREADS, 1)
+__global__ void __launch_bounds__(FZ_THREADS, 2)
 music4_fused_kernel(const float *__restrict__ in, const PlanarStreams S, unsigned long long first_snapshot, unsigned hop,
                     const unsigned char *__restrict__ tbl /* fused_table_bytes(K) */,
                     const float *__restrict__ tab_c64 /* [K][4] complex64 */, const float *__restrict__ na_max_p, int W, int N,
@@ -554,8 +624,8 @@ music4_fused_kernel(const float *__restrict__ in, const PlanarStreams S, unsigne
                     float *__restrict__ spec /* optional spectrum port [W][K] (float): every window then goes through the fp64 drain workers, which write it */)
 {
     long long *const dbg = TRACE ? dbg_in : nullptr;
-    // programmatic dependent launch: the next launch on this stream may take the SMs this grid leaves (it needs a whole
-    // SM per CTA, so it cannot disturb a running one); see griddepcontrol.wait below for the other half
+    // programmatic dependent launch: the next launch on this stream may be placed at once, in the other half of each SM;
+    // see OUTPUT ORDER (fused_emit) for the other half
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     const long long t_start = clock64();
     unsigned long long g_start = 0;
@@ -578,6 +648,7 @@ music4_fused_kernel(const float *__restrict__ in, const PlanarStreams S, unsigne
         ctl->cov_seq = 0; ctl->lock = 0; ctl->eig_done = 0; ctl->scan_done = 0; ctl->cov_finished = 0;
         ctl->batch_start = 0; ctl->batch_cnt = 0; ctl->claim = 0; ctl->tout = 0; ctl->mma_off = (mma_fin_max < 0 || spec != nullptr) ? 1u : 0u;
         ctl->dg_open = -1; ctl->drained_windows = 0; ctl->drain_groups = 0;
+        ctl->stg_lock = 0; ctl->stg_n = 0; ctl->ordered = 0;
         const uint32_t tb0 = smem_u32(fz_smem + FZ_OFF_TBAR);
         for (int s = 0; s < FZ_TS; ++s) {
             mbar_init(tb0 + 8 * s, FZ_SCAN_THREADS);            // tfull: one cp.async-completion arrival per scan thread
@@ -594,7 +665,7 @@ music4_fused_kernel(const float *__restrict__ in, const PlanarStreams S, unsigne
         unsigned char *ring = fz_smem + FZ_OFF_RING + (size_t)warp * FZ_STAGES * COV_CHUNK;
         const uint32_t bar0 = smem_u32(bars), ring0 = smem_u32(ring);
         // Windows are claimed one at a time from a global ticket counter (dynamic balance: 10 000 windows over
-        // 1184 warps would otherwise leave 8 or 9 per warp, i.e. a 12 % longer critical path).  The producer
+        // 528 warps would otherwise leave 18 or 19 per warp, i.e. a 5 % longer critical path).  The producer
         // (lane 0) claims the next window when it requests the last chunk of the current one and hands the id
         // to the consumer side through a small per-warp ring; -1 ends the stream.
         volatile int *wring = reinterpret_cast<volatile int *>(fz_smem + FZ_OFF_WRING) + warp * 8;
@@ -654,6 +725,11 @@ music4_fused_kernel(const float *__restrict__ in, const PlanarStreams S, unsigne
             if (wcur < 0) break;
             for (int q = 0; q < cpw; ++q) {
                 while (!mbar_try_wait(bar0 + 8 * slot, parity)) {}
+                if (dbg && warp == 0 && lane == 0 && rd == 0 && q == 0) {  // first input bytes of this CTA have arrived
+                    unsigned long long g;
+                    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g));
+                    dbg[blockIdx.x * FZ_TRACE + 32] = (long long)g;
+                }
                 const size_t off = (size_t)q * COV_CHUNK;
                 const int nsnap = (int)(min((size_t)COV_CHUNK, win_bytes - off) >> 5);
                 const float4 *buf = reinterpret_cast<const float4 *>(ring + (size_t)slot * COV_CHUNK);
@@ -724,7 +800,12 @@ music4_fused_kernel(const float *__restrict__ in, const PlanarStreams S, unsigne
         if (lane == 0) {
             __threadfence_block();
             const unsigned fin = atomicAdd((unsigned *)&ctl->cov_finished, 1u);
-            if (dbg && fin == (unsigned)FZ_COV_WARPS - 1) dbg[blockIdx.x * FZ_TRACE + 0] = clock64() - t_start;  // last covariance warp
+            if (dbg && fin == (unsigned)FZ_COV_WARPS - 1) {  // last covariance warp: this SM's input stream ends here
+                dbg[blockIdx.x * FZ_TRACE + 0] = clock64() - t_start;
+                unsigned long long g;
+                asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g));
+                dbg[blockIdx.x * FZ_TRACE + 33] = (long long)g;
+            }
             if (dbg && fin == 0) dbg[blockIdx.x * FZ_TRACE + 1] = clock64() - t_start;                           // first one
         }
         __syncwarp();
@@ -777,7 +858,7 @@ music4_fused_kernel(const float *__restrict__ in, const PlanarStreams S, unsigne
         else fused_drain_worker<TRACE, false>(fz_smem, tab_c64, K, nullptr, out, dbg ? dbg + blockIdx.x * FZ_TRACE : nullptr, t_start);
     } else {
         // ================= scan warps =================
-        const int st = threadIdx.x - 32 * (FZ_COV_WARPS + 1);  // 0..223
+        const int st = threadIdx.x - 32 * (FZ_COV_WARPS + 1);  // 0 .. FZ_SCAN_THREADS - 1
         const int swarp = st >> 5;
         const int g = lane >> 2, t = lane & 3;                 // MMA fragment coordinates; t = this thread's window
         float *redmin = reinterpret_cast<float *>(fz_smem + FZ_OFF_RMIN);
@@ -793,10 +874,6 @@ music4_fused_kernel(const float *__restrict__ in, const PlanarStreams S, unsigne
         unsigned T = 0;  // table tiles consumed so far (identical in every scan thread)
         long long scan_busy = 0, scan_passes = 0, scan_exact = 0, scan_fallbacks = 0, scan_ncand = 0;
         long long tr_issue = 0, tr_full = 0, tr_comp = 0;
-        // Output writes must land after those of the previous launch on the stream (which may still be draining on other
-        // SMs under programmatic dependent launch): the writers wait for it here - the covariance warps do not, the
-        // 64-slot queue absorbs the few microseconds this can take.
-        asm volatile("griddepcontrol.wait;" ::: "memory");
 
         for (;;) {
             if (swarp == 0) {  // (the whole first scan warp, in uniform control flow; lane 0 decides)
@@ -908,7 +985,7 @@ music4_fused_kernel(const float *__restrict__ in, const PlanarStreams S, unsigne
                     float na0[FZ_MPW], na1[FZ_MPW];
 #pragma unroll
                     for (int m = 0; m < FZ_MPW; ++m) {
-                        const int mt = m * FZ_SCAN_WARPS + swarp;  // MMA tile within the 224-row tile (round-robin over warps)
+                        const int mt = m * FZ_SCAN_WARPS + swarp;  // MMA tile within the FZ_BINS-row tile (round-robin over warps)
                         uint32_t av[4];
                         asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(av[0]), "=r"(av[1]), "=r"(av[2]), "=r"(av[3]) : "r"(tile + mt * FZ_FRAG_BYTES + lane * 16));
                         asm volatile("ld.shared.f32 %0, [%1];" : "=f"(na0[m]) : "r"(tile + (FZ_BINS / 16) * FZ_FRAG_BYTES + 4 * (mt * 16 + g)));
@@ -1006,7 +1083,7 @@ music4_fused_kernel(const float *__restrict__ in, const PlanarStreams S, unsigne
             unsigned long long *bestP = reinterpret_cast<unsigned long long *>(fz_smem + FZ_OFF_BEST);
             int *bestk = reinterpret_cast<int *>(fz_smem + FZ_OFF_BEST + 8 * FZ_WPT);
             int *admitted = reinterpret_cast<int *>(fz_smem + FZ_OFF_BEST + 12 * FZ_WPT);
-            constexpr int IPT = 4;  // candidates per thread kept in registers
+            constexpr int IPT = FZ_IPT;
             int pre[FZ_WPT + 1];
             pre[0] = 0;
 #pragma unroll
@@ -1040,19 +1117,11 @@ music4_fused_kernel(const float *__restrict__ in, const PlanarStreams S, unsigne
             for (int r = 0; r < IPT; ++r)
                 if (myk[r] >= 0 && (unsigned long long)__double_as_longlong(myP[r]) == bestP[myw[r]]) atomicMin(&bestk[myw[r]], myk[r]);
             bar_sync_scan();
-            if ((unsigned)st < cnt && admitted[st]) {
-                const int w = st;
-                const int kk = bestk[w] == 0x7fffffff ? -1 : bestk[w];
-                const double P = __longlong_as_double((long long)bestP[w]);
-                const size_t o = (size_t)qwin[(start + w) % FZ_Q];
-                if (kk >= 0) {
-                    out.angles[o] = (float)((double)kk * 360.0 / (double)K);  // reference :134, :153
-                    if (out.levels) out.levels[o] = (float)P;                 // reference :154
-                } else {
-                    out.angles[o] = 0.f;                                      // (0,0) initial pair, reference :95
-                    if (out.levels) out.levels[o] = 0.f;
-                }
-                peak_store_bin(out, o, kk);
+            if (swarp == 0) {  // (cnt <= FZ_WPT: every window of the pass belongs to a lane of the first scan warp)
+                const bool v = (unsigned)st < cnt && admitted[st];
+                const int kk = v ? (bestk[st] == 0x7fffffff ? -1 : bestk[st]) : -1;
+                const double P = v ? __longlong_as_double((long long)bestP[st]) : 0.0;
+                fused_emit(fz_smem, out, v, v ? (unsigned)qwin[(start + st) % FZ_Q] : 0u, kk, P, K);
             }
             if (dbg && st == 0) scan_ncand += pre[FZ_WPT];
             // ---- fallback: too many candidates (flat spectrum) -> every bin in fp64 ----
@@ -1076,17 +1145,9 @@ music4_fused_kernel(const float *__restrict__ in, const PlanarStreams S, unsigne
                 if (st == 0) {
                     for (int q = 1; q < FZ_SCAN_WARPS; ++q)
                         if (peak_better(redP[q], redk[q], P, kk)) { P = redP[q]; kk = redk[q]; }
-                    const size_t o = (size_t)qwin[(start + w) % FZ_Q];
-                    if (kk >= 0) {
-                        out.angles[o] = (float)((double)kk * 360.0 / (double)K);
-                        if (out.levels) out.levels[o] = (float)P;
-                    } else {
-                        out.angles[o] = 0.f;
-                        if (out.levels) out.levels[o] = 0.f;
-                    }
-                    peak_store_bin(out, o, kk);
                     ++scan_fallbacks;
                 }
+                if (swarp == 0) fused_emit(fz_smem, out, st == 0, (unsigned)qwin[(start + w) % FZ_Q], kk, P, K);
                 bar_sync_scan();
             }
             if (dbg) scan_exact += clock64() - te0;
@@ -1116,11 +1177,18 @@ music4_fused_kernel(const float *__restrict__ in, const PlanarStreams S, unsigne
     // The last CTA to finish re-arms the ticket counter for the next launch (launches of one handle are
     // serialised by the host, and by now every covariance warp has drawn a ticket >= W).
     __syncthreads();
+    if (warp == 0 && !ctl->ordered) fused_stage_flush(fz_smem, out, K);  // (uniform: no warp is left to change `ordered`)
     if (threadIdx.x == 0) {
         if (dbg) {
             dbg[blockIdx.x * FZ_TRACE + 17] = ctl->drained_windows;
             dbg[blockIdx.x * FZ_TRACE + 20] = ctl->drain_groups;
             dbg[blockIdx.x * FZ_TRACE + 18] = clock64() - t_start;  // every window of this CTA is finished
+            unsigned long long g;
+            unsigned smid;
+            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g));
+            asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+            dbg[blockIdx.x * FZ_TRACE + 31] = (long long)g;  // ns, absolute: CTA exit
+            dbg[blockIdx.x * FZ_TRACE + 30] = (long long)smid;
         }
         if (out.npeer > 0) __threadfence_system(); else __threadfence();
         if (atomicAdd(&work_ctr[1], 1u) == gridDim.x - 1) {

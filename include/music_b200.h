@@ -297,8 +297,9 @@ uint64_t music_b200_launch_count(const music_b200 *h);
 int music_b200_set_stage_timing(music_b200 *h, int enable);
 int music_b200_get_stage_times(music_b200 *h, double *ms4, uint64_t *chunks);
 
-/* Debug: copy the fused kernel's per-CTA clock64 trace (16 int64 per CTA; only when the handle
- * was created with MUSIC_B200_TRACE=1 in the environment). */
+/* Debug: copy the first max_ctas rows of the fused kernel's per-CTA trace (40 int64 per row; only when
+ * the handle was created with MUSIC_B200_TRACE=1 in the environment).  The trace is a ring of 32
+ * launches of 1024 rows: the l-th fused launch of the handle writes rows [(l % 32) * 1024, .. + grid). */
 int music_b200_debug_fused_trace(music_b200 *h, long long *host_out, int max_ctas);
 
 /* Debug: cumulative window counts of the fused M = 8 kernel - out2[0] solved by the principal-eigenvector (squaring) solver,
