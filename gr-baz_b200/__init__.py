@@ -5,3 +5,5 @@ Only the hot path of /root/reference/lib/baz_music_doa.cc (work()) and its Pytho
 The directory name carries a hyphen, so it is imported through the ``gr_baz_b200`` alias
 package at the repo root.
 """
+
+from .music_doa_azel import music_doa_azel  # noqa: E402,F401  (azimuth + elevation, include/music_b200.h)

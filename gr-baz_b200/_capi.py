@@ -93,6 +93,15 @@ def load():
         L.music_b200_process_host_counts.restype = ctypes.c_int
         L.music_b200_process_device_counts.argtypes = [vp, fp, u32, fp, fp, fp, fp, fp, vp]
         L.music_b200_process_device_counts.restype = ctypes.c_int
+        dbl = ctypes.c_double
+        L.music_b200_create_azel.argtypes = [ctypes.POINTER(vp), u32, u32, u32, u32, u32, dbl, dbl, fp, dbl, ctypes.c_int]
+        L.music_b200_create_azel.restype = ctypes.c_int
+        L.music_b200_set_geometry_azel.argtypes = [vp, fp, dbl]
+        L.music_b200_set_geometry_azel.restype = ctypes.c_int
+        L.music_b200_process_azel_host.argtypes = [vp, fp, u32, fp, fp, fp, fp, fp, fp]
+        L.music_b200_process_azel_host.restype = ctypes.c_int
+        L.music_b200_process_azel_device.argtypes = [vp, fp, u32, fp, fp, fp, fp, fp, fp, vp]
+        L.music_b200_process_azel_device.restype = ctypes.c_int
         L.music_b200_launch_count.argtypes = [vp]
         L.music_b200_launch_count.restype = ctypes.c_uint64
         L.music_b200_set_stage_timing.argtypes = [vp, ctypes.c_int]
@@ -122,6 +131,7 @@ EXPORTS = [
     "music_b200_process_planar_device", "music_b200_launch_count",
     "music_b200_set_stage_timing", "music_b200_get_stage_times", "music_b200_debug_fused_trace", "music_b200_debug_fused8_stats",
     "music_b200_last_error", "music_b200_destroy",
+    "music_b200_create_azel", "music_b200_set_geometry_azel", "music_b200_process_azel_host", "music_b200_process_azel_device",
 ]
 
 

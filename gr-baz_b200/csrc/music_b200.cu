@@ -29,6 +29,7 @@
 #include "music_reduce.cuh"
 #include "music_sources.cuh"
 #include "music_refine.cuh"
+#include "music_azel.cuh"
 
 using namespace music;
 
@@ -44,6 +45,7 @@ struct DeviceTable {
     float *na_max = nullptr;      // max ||a||^2 over the table rows (screen threshold)
     bool geometric = false;       // built by set_geometry() from `geo` (set_table() tables are not)
     RefineGeom geo = {};          // element positions and wavelength of a geometric table (peak refinement)
+    AzelGeom ageo = {};           // the same for an az-el handle (music_b200_create_azel): [M][x, y, z] and the grid
 };
 
 struct Workspace {
@@ -77,6 +79,8 @@ struct music_b200 {
     int source_rule = MUSIC_B200_SOURCES_FIXED;  // set_source_rule()
     int refine = MUSIC_B200_REFINE_OFF;          // set_refine()
     unsigned steer_guarded = 0;    // entries of the last built table re-evaluated with the host libm
+    bool azel = false;             // music_b200_create_azel(): K = n_az * n_el rows, elevation-major (music_azel.cuh)
+    AzelGrid grid = {};
 
     // fp64 workspace slots (R, eigenvalues, sorted eigenvectors, optional strengths) of the unfused path: one per
     // staging stream of the host entry points (slot 0 also serves the device entry points)
@@ -107,6 +111,7 @@ struct music_b200 {
     // memory is pageable (numpy arrays, GNU Radio buffers) and stall the enqueue of the next chunk's upload
     float *p_ang[2] = {nullptr, nullptr}, *p_lvl[2] = {nullptr, nullptr};
     int32_t *p_bins[2] = {nullptr, nullptr}, *p_cnt[2] = {nullptr, nullptr};
+    float *d_el[2] = {nullptr, nullptr}, *p_el[2] = {nullptr, nullptr};  // az-el handles: elevations and their pinned mirror
     uint32_t slot_w0[2] = {0, 0}, slot_W[2] = {0, 0};
     uint32_t host_chunk = 0;
     bool host_spec_alloc = false;
@@ -240,6 +245,27 @@ int build_table(music_b200 *h, int slot, const double *pos_xy, double lambda, cu
     return MUSIC_B200_OK;
 }
 
+// Steering table of an az-el handle, built on the device from the element positions [M][x, y, z] (music_azel.cuh).
+// No host patching: the table is defined to within one float32 ulp, not bit for bit.
+int build_table_azel(music_b200 *h, int slot, const double *pos_xyz, double lambda, cudaStream_t st)
+{
+    DeviceTable &t = h->table[slot];
+    const int K = (int)h->K, M = (int)h->m;
+    t.geometric = false;
+    AzelGeom g = {};
+    for (int i = 0; i < 3 * M; ++i) g.pos[i] = pos_xyz[i];
+    g.lambda = lambda;
+    g.grid = h->grid;
+    azel_table_kernel<<<(K * M + 255) / 256, 256, 0, st>>>(g, M, reinterpret_cast<float2 *>(t.c64));
+    h->launches++;
+    CU(h, cudaGetLastError());
+    const int rc = finish_table(h, slot, st);
+    if (rc) return rc;
+    t.geometric = true;
+    t.ageo = g;
+    return MUSIC_B200_OK;
+}
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
                                   const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -276,7 +302,7 @@ uint32_t max_sub_windows(const music_b200 *h, bool need_p64)
 {
     const size_t per_win = (size_t)h->m * h->m * 2 * 8 * 2 + h->m * 8 + (need_p64 ? (size_t)h->K * 8 : 0) +
                            (h->source_rule != MUSIC_B200_SOURCES_FIXED ? sizeof(int32_t) : 0) +
-                           (h->refine != MUSIC_B200_REFINE_OFF ? h->n * sizeof(int32_t) : 0);
+                           (h->refine != MUSIC_B200_REFINE_OFF || h->azel ? h->n * sizeof(int32_t) : 0);
     size_t c = ((size_t)384 << 20) / per_win;
     c = std::max<size_t>(SCAN_B, std::min<size_t>(c, 1u << 20));
     return (uint32_t)(c / SCAN_B * SCAN_B);
@@ -307,7 +333,7 @@ int ensure_slot(music_b200 *h, Workspace &ws, uint32_t windows, bool need_p64)
         CU(h, cudaMalloc(&ws.cnt, (size_t)windows * sizeof(int32_t)));
         ws.cnt_cap = windows;
     }
-    if (h->refine != MUSIC_B200_REFINE_OFF && windows > ws.bins_cap) {
+    if ((h->refine != MUSIC_B200_REFINE_OFF || h->azel) && windows > ws.bins_cap) {
         if (ws.used) CU(h, cudaEventSynchronize(ws.scan_done));
         cudaFree(ws.bins); ws.bins = nullptr; ws.bins_cap = 0;
         CU(h, cudaMalloc(&ws.bins, (size_t)windows * h->n * sizeof(int32_t)));
@@ -482,15 +508,17 @@ __global__ void gather_wait_kernel(const unsigned *flags, int npeer, unsigned ep
 // d_counts_out (may be NULL): the caller's copy of the per-window source counts (source rule other than FIXED).
 // With refinement on, the refine kernel follows the peak rule (timed with top-n) and reads the bins it wrote: from the
 // caller's array, or from the workspace when the caller asked for none.
+// d_el: an az-el handle's elevation outputs; its peak bins are then decoded into (azimuth, elevation) after the peak rule.
 int launch_eig_scan(music_b200 *h, const Workspace &ws, uint32_t W, const PeakOut &po_in, float *d_spec,
-                    double *d_P64_out, double *d_R_out, double *d_ev_out, int32_t *d_counts_out, cudaStream_t st, cudaEvent_t *tev)
+                    double *d_P64_out, double *d_R_out, double *d_ev_out, int32_t *d_counts_out, cudaStream_t st, cudaEvent_t *tev,
+                    float *d_el = nullptr)
 {
     const int M = (int)h->m;
     const DeviceTable &tb = h->table[h->cur_table];
     const double *soa = tb.soa;
     const bool refine = h->refine != MUSIC_B200_REFINE_OFF;
     PeakOut po = po_in;
-    if (refine && !po.bins) po.bins = ws.bins;
+    if ((refine || h->azel) && !po.bins) po.bins = ws.bins;
     {
         const int grid = (W + 127) / 128;
         switch (M) {
@@ -534,11 +562,23 @@ int launch_eig_scan(music_b200 *h, const Workspace &ws, uint32_t W, const PeakOu
     }
     if (tev) cudaEventRecord(tev[3], st);
     if (!argmax) {
-        if (local) topn_local_kernel<<<(W + 7) / 8, 256, 0, st>>>(p64, (int)h->n, (int)h->K, (int)W, (int)h->peak_excl, po, cnt);
+        if (local && h->azel)
+            topn_local2d_kernel<<<W, AZEL_LM_THREADS, 0, st>>>(p64, (int)h->n, h->grid.n_az, h->grid.n_el, (int)h->peak_excl, po, cnt);
+        else if (local) topn_local_kernel<<<(W + 7) / 8, 256, 0, st>>>(p64, (int)h->n, (int)h->K, (int)W, (int)h->peak_excl, po, cnt);
         else topn_kernel<<<(W + 7) / 8, 256, 0, st>>>(p64, (int)h->n, (int)h->K, (int)W, po, cnt);
         h->launches++;
     }
-    if (refine) {
+    if (h->azel) {
+        const int slots = (int)(W * h->n);
+        azel_decode_kernel<<<(slots + 255) / 256, 256, 0, st>>>(po.bins, slots, h->grid, po.angles, d_el);
+        h->launches++;
+    }
+    if (refine && h->azel) {
+        const int slots = (int)(W * h->n);
+        refine_azel_kernel<<<(slots + REFINE_THREADS - 1) / REFINE_THREADS, REFINE_THREADS, 0, st>>>(ws.Vt, cnt, po.bins, M, (int)h->n, (int)W,
+                                                                                                   tb.ageo, po.angles, d_el, po.levels);
+        h->launches++;
+    } else if (refine) {
         const int slots = (int)(W * h->n);
         refine_peaks_kernel<<<(slots + REFINE_THREADS - 1) / REFINE_THREADS, REFINE_THREADS, 0, st>>>(ws.Vt, cnt, po.bins, M, (int)h->n, (int)h->K, (int)W, tb.geo,
                                                                 po.angles, po.levels);
@@ -572,10 +612,11 @@ void launch_cov_planar(music_b200 *h, const Workspace &ws, const PlanarStreams &
 // d_counts (may be NULL): receives the per-window source counts; under the FIXED rule every count is n.
 int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, float *d_ang, float *d_lvl, float *d_spec,
                    int32_t *d_bins, double *d_P64, double *d_R, double *d_ev, int32_t *d_counts, cudaStream_t st, int slot,
-                   const PlanarStreams *planar = nullptr, unsigned hop = 0)
+                   const PlanarStreams *planar = nullptr, unsigned hop = 0, float *d_el = nullptr)
 {
     if (nwindows == 0) return MUSIC_B200_OK;
     if ((!planar && !d_in) || !d_ang) return fail(h, MUSIC_B200_EINVAL, "d_in_c64 and d_angles must not be NULL");
+    if (h->azel && !d_el) return fail(h, MUSIC_B200_EINVAL, "an az-el handle needs the elevation output");
     if (!planar && (reinterpret_cast<uintptr_t>(d_in) & 15u) != 0) return fail(h, MUSIC_B200_EINVAL, "d_in_c64 must be 16-byte aligned");
     const bool fixed_n = h->source_rule == MUSIC_B200_SOURCES_FIXED;
     const bool refine = h->refine != MUSIC_B200_REFINE_OFF;
@@ -596,7 +637,7 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, float *d
     const bool local_peaks = h->peak_mode == MUSIC_B200_PEAKS_LOCAL_MAXIMA;
     // the fused kernels find the principal eigenvector only, not every eigenvalue a source count needs nor the noise
     // eigenvectors the peak refinement needs
-    if ((!planar || planar_fusable) && h->fused && fixed_n && !refine && !local_peaks && h->m == 4 && h->n == 1 && (!d_spec || h->fused_spec) && !d_P64 && !d_R && !d_ev) {
+    if ((!planar || planar_fusable) && h->fused && !h->azel && fixed_n && !refine && !local_peaks && h->m == 4 && h->n == 1 && (!d_spec || h->fused_spec) && !d_P64 && !d_R && !d_ev) {
         // whole call in one persistent launch (music_fused.cuh); no workspace involved
         cudaEvent_t *tev = timing_events(h);
         if (tev) cudaEventRecord(tev[0], st);
@@ -638,7 +679,7 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, float *d
         CU(h, cudaGetLastError());
         return MUSIC_B200_OK;
     }
-    if (!planar && h->fused && fixed_n && !refine && !local_peaks && h->m == 8 && h->n == 1 && !d_spec && !d_P64 && !d_R && !d_ev && h->N >= 128 &&
+    if (!planar && h->fused && !h->azel && fixed_n && !refine && !local_peaks && h->m == 8 && h->n == 1 && !d_spec && !d_P64 && !d_R && !d_ev && h->N >= 128 &&
         h->N % 2 == 0 && encode_tiled_fn()) {
         // M = 8: whole call in one persistent launch (music_fused8.cuh); R and the eigenvectors stay in shared memory
         CUtensorMap tm;
@@ -680,7 +721,7 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, float *d
                              d_spec ? d_spec + (size_t)w0 * h->K : nullptr,
                              d_P64 ? d_P64 + (size_t)w0 * h->K : nullptr, d_R ? d_R + (size_t)w0 * h->m * h->m * 2 : nullptr,
                              d_ev ? d_ev + (size_t)w0 * h->m : nullptr,
-                             !fixed_n && d_counts ? d_counts + w0 : nullptr, st, tev);
+                             !fixed_n && d_counts ? d_counts + w0 : nullptr, st, tev, d_el ? d_el + (size_t)w0 * h->n : nullptr);
         if (rc) return rc;
         CU(h, cudaEventRecord(ws.scan_done, st));
         ws.used = true;
@@ -749,6 +790,8 @@ void free_host_staging(music_b200 *h)
         cudaFree(h->d_in[i]); cudaFree(h->d_ang[i]); cudaFree(h->d_lvl[i]); cudaFree(h->d_spec[i]); cudaFree(h->d_bins[i]);
         cudaFree(h->d_cnt[i]);
         cudaFreeHost(h->p_ang[i]); cudaFreeHost(h->p_lvl[i]); cudaFreeHost(h->p_bins[i]); cudaFreeHost(h->p_cnt[i]);
+        cudaFree(h->d_el[i]); cudaFreeHost(h->p_el[i]);
+        h->d_el[i] = h->p_el[i] = nullptr;
         h->d_in[i] = h->d_ang[i] = h->d_lvl[i] = h->d_spec[i] = nullptr;
         h->d_bins[i] = h->d_cnt[i] = nullptr;
         h->p_ang[i] = h->p_lvl[i] = nullptr;
@@ -775,6 +818,10 @@ int ensure_host_staging(music_b200 *h, uint32_t chunk, bool spec)
         CU(h, cudaMalloc(&h->d_cnt[i], (size_t)cap * sizeof(int32_t)));
         CU(h, cudaHostAlloc(&h->p_cnt[i], (size_t)cap * sizeof(int32_t), cudaHostAllocDefault));
         if (spec) CU(h, cudaMalloc(&h->d_spec[i], (size_t)cap * h->K * sizeof(float)));
+        if (h->azel) {
+            CU(h, cudaMalloc(&h->d_el[i], (size_t)cap * h->n * sizeof(float)));
+            CU(h, cudaHostAlloc(&h->p_el[i], (size_t)cap * h->n * sizeof(float), cudaHostAllocDefault));
+        }
     }
     h->host_chunk = cap;
     h->host_spec_alloc = spec;
@@ -784,7 +831,9 @@ int ensure_host_staging(music_b200 *h, uint32_t chunk, bool spec)
 // results of the chunk last computed in staging slot s: pinned mirror -> caller memory (the slot's stream is idle).
 // The chunk holds the windows w = (slot_w0 + i) * G + g of the call (G = 1, g = 0 on a single-device handle).
 // counts (may be NULL): one source count per window, dealt like the bins.
-void flush_host_slot(music_b200 *h, int s, float *angles, float *levels, int32_t *bins, int32_t *counts, uint32_t G = 1, uint32_t g = 0)
+// elev (az-el handles only, single device): the elevations.
+void flush_host_slot(music_b200 *h, int s, float *angles, float *levels, int32_t *bins, int32_t *counts, uint32_t G = 1, uint32_t g = 0,
+                     float *elev = nullptr)
 {
     const uint32_t W = h->slot_W[s];
     if (!W) return;
@@ -795,6 +844,7 @@ void flush_host_slot(music_b200 *h, int s, float *angles, float *levels, int32_t
         if (levels) memcpy(levels + off, h->p_lvl[s], cnt * sizeof(float));
         if (bins) memcpy(bins + off, h->p_bins[s], cnt * sizeof(int32_t));
         if (counts) memcpy(counts + h->slot_w0[s], h->p_cnt[s], (size_t)W * sizeof(int32_t));
+        if (elev) memcpy(elev + off, h->p_el[s], cnt * sizeof(float));
     } else {
         for (uint32_t i = 0; i < W; ++i) {
             if (counts) counts[(size_t)(h->slot_w0[s] + i) * G + g] = h->p_cnt[s][i];
@@ -810,8 +860,9 @@ void flush_host_slot(music_b200 *h, int s, float *angles, float *levels, int32_t
 }
 
 // device -> pinned mirrors of slot s (asynchronous on st whatever memory the caller's outputs live in)
-int download_host_slot(music_b200 *h, int s, uint32_t w0, uint32_t W, bool levels, bool bins, bool counts, cudaStream_t st)
+int download_host_slot(music_b200 *h, int s, uint32_t w0, uint32_t W, bool levels, bool bins, bool counts, cudaStream_t st, bool elev = false)
 {
+    if (elev) CU(h, cudaMemcpyAsync(h->p_el[s], h->d_el[s], (size_t)W * h->n * sizeof(float), cudaMemcpyDeviceToHost, st));
     if (counts) CU(h, cudaMemcpyAsync(h->p_cnt[s], h->d_cnt[s], (size_t)W * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
     CU(h, cudaMemcpyAsync(h->p_ang[s], h->d_ang[s], (size_t)W * h->n * sizeof(float), cudaMemcpyDeviceToHost, st));
     if (levels) CU(h, cudaMemcpyAsync(h->p_lvl[s], h->d_lvl[s], (size_t)W * h->n * sizeof(float), cudaMemcpyDeviceToHost, st));
@@ -821,6 +872,84 @@ int download_host_slot(music_b200 *h, int s, uint32_t w0, uint32_t W, bool level
     return MUSIC_B200_OK;
 }
 
+
+// The device part of create() / create_azel(), after their argument checks: device checks, buffers, the first table
+// (uploaded, or for an az-el handle (grid != NULL) built from pos_xyz / wavelength).
+int create_on_device(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples, uint32_t resolution, const float *table_c64,
+                     int device, const AzelGrid *grid, const double *pos_xyz, double wavelength)
+{
+    int ndev = 0;
+    cudaError_t e = cudaGetDeviceCount(&ndev);
+    if (e != cudaSuccess || ndev == 0)
+        return fail(nullptr, MUSIC_B200_ENODEVICE, "no CUDA device (%s); this library has no CPU path", e == cudaSuccess ? "count 0" : cudaGetErrorString(e));
+    if (device < 0 || device >= ndev) return fail(nullptr, MUSIC_B200_ENODEVICE, "device %d out of range (0..%d)", device, ndev - 1);
+    cudaDeviceProp prop;
+    if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess)
+        return fail(nullptr, MUSIC_B200_ECUDA, "cudaGetDeviceProperties: %s", cudaGetErrorString(e));
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(nullptr, MUSIC_B200_ENODEVICE, "device %d is sm_%d%d; this build targets sm_90a only", device, prop.major, prop.minor);
+
+    music_b200 *h = new (std::nothrow) music_b200();
+    if (!h) return fail(nullptr, MUSIC_B200_ENOMEM, "out of host memory");
+    h->m = m; h->n = n; h->nsamples = nsamples; h->K = resolution; h->N = nsamples / m;
+    h->device = device; h->sm_count = prop.multiProcessorCount;
+    if (grid) {
+        h->azel = true;
+        h->grid = *grid;
+    }
+
+    int rc = MUSIC_B200_OK;
+    auto init = [&]() -> int {
+        CU(h, cudaSetDevice(device));
+        for (int i = 0; i < 2; ++i) {
+            CU(h, cudaStreamCreateWithFlags(&h->streams[i], cudaStreamNonBlocking));
+            CU(h, cudaEventCreateWithFlags(&h->ws[i].scan_done, cudaEventDisableTiming));
+            CU(h, cudaMalloc(&h->table[i].c64, (size_t)resolution * m * 2 * sizeof(float)));
+            CU(h, cudaMalloc(&h->table[i].soa, soa_doubles(resolution, m) * sizeof(double)));
+            if (m == 4 && !grid) {  // the fused M = 4 kernel's screen layout; an az-el handle never runs that kernel
+                CU(h, cudaMalloc(&h->table[i].fz, fused_table_bytes((int)resolution)));
+                CU(h, cudaMalloc(&h->table[i].na_max, sizeof(float)));
+            }
+        }
+        // scan kernels with M = 16 need 32 KiB dynamic smem (< 48 KiB default), nothing to opt in.
+        if (const char *e = getenv("MUSIC_B200_FUSED")) h->fused = atoi(e) != 0;
+        if (const char *e = getenv("MUSIC_B200_EIG")) h->eig_mode = !strcmp(e, "jacobi") ? 1 : !strcmp(e, "jacobi1") ? 2 : 0;
+        if (const char *e = getenv("MUSIC_B200_PDL")) h->pdl = atoi(e) != 0;
+        if (const char *e = getenv("MUSIC_B200_FUSED_SPEC")) h->fused_spec = atoi(e) != 0;
+        if (const char *e = getenv("MUSIC_B200_MMA_FIN")) h->mma_fin_max = std::max(-1, std::min(FZ_COV_WARPS, atoi(e)));
+        CU(h, cudaFuncSetAttribute(covN_tma_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CN_SMEM));
+        CU(h, cudaFuncSetAttribute(covN_tma_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CN_SMEM));
+        CU(h, cudaFuncSetAttribute(music8_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)F8_SMEM));
+        CU(h, cudaMalloc(&h->f8_stats, 2 * sizeof(unsigned)));
+        CU(h, cudaMemset(h->f8_stats, 0, 2 * sizeof(unsigned)));
+        CU(h, cudaEventCreateWithFlags(&h->fused_done, cudaEventDisableTiming));
+        CU(h, cudaMalloc(&h->work_ctr, 2 * CTR_RING * 2 * sizeof(unsigned)));  // self-resetting (tickets, finished CTAs) pairs
+        CU(h, cudaMemset(h->work_ctr, 0, 2 * CTR_RING * 2 * sizeof(unsigned)));
+        if (const char *e = getenv("MUSIC_B200_HOSTREG")) h->hostreg = atoi(e) != 0;
+        if (getenv("MUSIC_B200_TRACE")) {
+            const size_t tb = (size_t)FZ_TRACE_LAUNCHES * FZ_TRACE_CTAS * FZ_TRACE * sizeof(long long);
+            CU(h, cudaMalloc(&h->fused_trace, tb));
+            CU(h, cudaMemset(h->fused_trace, 0, tb));
+        }
+        // the fused M = 4 kernel runs two CTAs per SM: all of the SM's unified L1 / shared memory goes to shared memory
+        for (const void *k : {(const void *)music4_fused_kernel<false, false>, (const void *)music4_fused_kernel<true, false>,
+                              (const void *)music4_fused_kernel<false, true>, (const void *)music4_fused_kernel<true, true>}) {
+            CU(h, cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FZ_SMEM));
+            CU(h, cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
+        }
+        CU(h, cudaFuncSetAttribute(cov4_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)COV_SMEM));
+        return grid ? build_table_azel(h, 0, pos_xyz, wavelength, h->streams[0]) : upload_table(h, 0, table_c64, h->streams[0]);
+    };
+    rc = init();
+    if (rc != MUSIC_B200_OK) {
+        fail(nullptr, rc, "%s", std::string(h->error).c_str());
+        music_b200_destroy(h);
+        return rc;
+    }
+    h->cur_table = 0;
+    *out = h;
+    return MUSIC_B200_OK;
+}
 
 }  // namespace
 
@@ -919,73 +1048,7 @@ int music_b200_create(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsample
     if (resolution == 0) return fail(nullptr, MUSIC_B200_EINVAL, "resolution must be > 0");
     if (!table_c64) return fail(nullptr, MUSIC_B200_EINVAL, "array response table must not be NULL");
 
-    int ndev = 0;
-    cudaError_t e = cudaGetDeviceCount(&ndev);
-    if (e != cudaSuccess || ndev == 0)
-        return fail(nullptr, MUSIC_B200_ENODEVICE, "no CUDA device (%s); this library has no CPU path", e == cudaSuccess ? "count 0" : cudaGetErrorString(e));
-    if (device < 0 || device >= ndev) return fail(nullptr, MUSIC_B200_ENODEVICE, "device %d out of range (0..%d)", device, ndev - 1);
-    cudaDeviceProp prop;
-    if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess)
-        return fail(nullptr, MUSIC_B200_ECUDA, "cudaGetDeviceProperties: %s", cudaGetErrorString(e));
-    if (prop.major != 9 || prop.minor != 0)
-        return fail(nullptr, MUSIC_B200_ENODEVICE, "device %d is sm_%d%d; this build targets sm_90a only", device, prop.major, prop.minor);
-
-    music_b200 *h = new (std::nothrow) music_b200();
-    if (!h) return fail(nullptr, MUSIC_B200_ENOMEM, "out of host memory");
-    h->m = m; h->n = n; h->nsamples = nsamples; h->K = resolution; h->N = nsamples / m;
-    h->device = device; h->sm_count = prop.multiProcessorCount;
-
-    int rc = MUSIC_B200_OK;
-    auto init = [&]() -> int {
-        CU(h, cudaSetDevice(device));
-        for (int i = 0; i < 2; ++i) {
-            CU(h, cudaStreamCreateWithFlags(&h->streams[i], cudaStreamNonBlocking));
-            CU(h, cudaEventCreateWithFlags(&h->ws[i].scan_done, cudaEventDisableTiming));
-            CU(h, cudaMalloc(&h->table[i].c64, (size_t)resolution * m * 2 * sizeof(float)));
-            CU(h, cudaMalloc(&h->table[i].soa, soa_doubles(resolution, m) * sizeof(double)));
-            if (m == 4) {
-                CU(h, cudaMalloc(&h->table[i].fz, fused_table_bytes((int)resolution)));
-                CU(h, cudaMalloc(&h->table[i].na_max, sizeof(float)));
-            }
-        }
-        // scan kernels with M = 16 need 32 KiB dynamic smem (< 48 KiB default), nothing to opt in.
-        if (const char *e = getenv("MUSIC_B200_FUSED")) h->fused = atoi(e) != 0;
-        if (const char *e = getenv("MUSIC_B200_EIG")) h->eig_mode = !strcmp(e, "jacobi") ? 1 : !strcmp(e, "jacobi1") ? 2 : 0;
-        if (const char *e = getenv("MUSIC_B200_PDL")) h->pdl = atoi(e) != 0;
-        if (const char *e = getenv("MUSIC_B200_FUSED_SPEC")) h->fused_spec = atoi(e) != 0;
-        if (const char *e = getenv("MUSIC_B200_MMA_FIN")) h->mma_fin_max = std::max(-1, std::min(FZ_COV_WARPS, atoi(e)));
-        CU(h, cudaFuncSetAttribute(covN_tma_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CN_SMEM));
-        CU(h, cudaFuncSetAttribute(covN_tma_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CN_SMEM));
-        CU(h, cudaFuncSetAttribute(music8_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)F8_SMEM));
-        CU(h, cudaMalloc(&h->f8_stats, 2 * sizeof(unsigned)));
-        CU(h, cudaMemset(h->f8_stats, 0, 2 * sizeof(unsigned)));
-        CU(h, cudaEventCreateWithFlags(&h->fused_done, cudaEventDisableTiming));
-        CU(h, cudaMalloc(&h->work_ctr, 2 * CTR_RING * 2 * sizeof(unsigned)));  // self-resetting (tickets, finished CTAs) pairs
-        CU(h, cudaMemset(h->work_ctr, 0, 2 * CTR_RING * 2 * sizeof(unsigned)));
-        if (const char *e = getenv("MUSIC_B200_HOSTREG")) h->hostreg = atoi(e) != 0;
-        if (getenv("MUSIC_B200_TRACE")) {
-            const size_t tb = (size_t)FZ_TRACE_LAUNCHES * FZ_TRACE_CTAS * FZ_TRACE * sizeof(long long);
-            CU(h, cudaMalloc(&h->fused_trace, tb));
-            CU(h, cudaMemset(h->fused_trace, 0, tb));
-        }
-        // the fused M = 4 kernel runs two CTAs per SM: all of the SM's unified L1 / shared memory goes to shared memory
-        for (const void *k : {(const void *)music4_fused_kernel<false, false>, (const void *)music4_fused_kernel<true, false>,
-                              (const void *)music4_fused_kernel<false, true>, (const void *)music4_fused_kernel<true, true>}) {
-            CU(h, cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FZ_SMEM));
-            CU(h, cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
-        }
-        CU(h, cudaFuncSetAttribute(cov4_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)COV_SMEM));
-        return upload_table(h, 0, table_c64, h->streams[0]);
-    };
-    rc = init();
-    if (rc != MUSIC_B200_OK) {
-        fail(nullptr, rc, "%s", std::string(h->error).c_str());
-        music_b200_destroy(h);
-        return rc;
-    }
-    h->cur_table = 0;
-    *out = h;
-    return MUSIC_B200_OK;
+    return create_on_device(out, m, n, nsamples, resolution, table_c64, device, nullptr, nullptr, 0.0);
 }
 
 int music_b200_set_table(music_b200 *h, const float *table_c64)
@@ -1017,6 +1080,7 @@ int music_b200_process_planar_device(music_b200 *h, const float *const *d_stream
 {
     if (h && !h->kids.empty()) return music_b200_process_planar_device(h->kids[0], d_streams, hop, nwindows, d_angles, d_levels, d_spectrum, d_bins, stream);  // multi-device handle: device 0 serves this entry
     if (!h) return MUSIC_B200_EINVAL;
+    if (h->azel) return fail(h, MUSIC_B200_EINVAL, "planar input is not supported on an az-el handle");
     if (nwindows == 0) return MUSIC_B200_OK;
     if (!d_streams) return fail(h, MUSIC_B200_EINVAL, "d_streams must not be NULL");
     if (hop == 0) return fail(h, MUSIC_B200_EINVAL, "hop must be >= 1 snapshot");
@@ -1038,6 +1102,7 @@ int music_b200_process_planar_host(music_b200 *h, const float *const *streams, u
 {
     if (h && !h->kids.empty()) return music_b200_process_planar_host(h->kids[0], streams, hop, nwindows, angles, levels, spectrum, bins);  // multi-device handle: device 0 serves this entry
     if (!h) return MUSIC_B200_EINVAL;
+    if (h->azel) return fail(h, MUSIC_B200_EINVAL, "planar input is not supported on an az-el handle");
     if (nwindows == 0) return MUSIC_B200_OK;
     if (!streams || !angles) return fail(h, MUSIC_B200_EINVAL, "streams and angles must not be NULL");
     if (hop == 0) return fail(h, MUSIC_B200_EINVAL, "hop must be >= 1 snapshot");
@@ -1206,6 +1271,7 @@ int music_b200_set_peak_mode(music_b200 *h, int mode, uint32_t exclusion_bins)
 int music_b200_set_geometry(music_b200 *h, const double *positions_xy, double wavelength, uint32_t *guarded)
 {
     if (!h) return MUSIC_B200_EINVAL;
+    if (h->azel) return fail(h, MUSIC_B200_EINVAL, "an az-el handle takes music_b200_set_geometry_azel()");
     if (!positions_xy) return fail(h, MUSIC_B200_EINVAL, "element positions must not be NULL");
     if (!(wavelength > 0.0) || !std::isfinite(wavelength)) return fail(h, MUSIC_B200_EINVAL, "wavelength must be positive and finite");
     for (uint32_t i = 0; i < 2 * h->m; ++i)
@@ -1270,6 +1336,7 @@ int process_device_impl(music_b200 *h, const float *d_in_c64, uint32_t nwindows,
             }
         return fail(h, MUSIC_B200_EINVAL, "d_in_c64 lives on device %d, which this handle does not own", at.device);
     }
+    if (h->azel) return fail(h, MUSIC_B200_EINVAL, "an az-el handle takes music_b200_process_azel_device()");
     std::lock_guard<std::mutex> g(h->mutex);
     NvtxRange range("music_b200_process_device");
     CU(h, cudaSetDevice(h->device));
@@ -1282,8 +1349,9 @@ int process_device_impl(music_b200 *h, const float *d_in_c64, uint32_t nwindows,
 }
 
 // process_host plus the per-window source counts (music_b200_process_host_counts)
+// elevation: the az-el entry's elevation output (NULL for the 1-D entries)
 int process_host_impl(music_b200 *h, const float *in_c64, uint32_t nwindows, float *angles, float *levels,
-                      float *spectrum, int32_t *bins, int32_t *counts);
+                      float *spectrum, int32_t *bins, int32_t *counts, float *elevation = nullptr);
 
 }  // namespace
 
@@ -1357,9 +1425,10 @@ int music_b200_set_refine(music_b200 *h, int mode)
 namespace {
 
 int process_host_impl(music_b200 *h, const float *in_c64, uint32_t nwindows, float *angles, float *levels,
-                      float *spectrum, int32_t *bins, int32_t *counts)
+                      float *spectrum, int32_t *bins, int32_t *counts, float *elevation)
 {
     if (!h) return MUSIC_B200_EINVAL;
+    if (h->azel && !elevation) return fail(h, MUSIC_B200_EINVAL, "an az-el handle takes music_b200_process_azel_host()");
     if (nwindows == 0) return MUSIC_B200_OK;
     if (!in_c64 || !angles) return fail(h, MUSIC_B200_EINVAL, "in_c64 and angles must not be NULL");
     std::lock_guard<std::mutex> g(h->mutex);
@@ -1408,7 +1477,7 @@ int process_host_impl(music_b200 *h, const float *in_c64, uint32_t nwindows, flo
             CU_BREAK(h, rc, cudaSetDevice(c->device));
             if (it >= 2) {
                 CU_BREAK(h, rc, cudaStreamSynchronize(st));  // slot buffers free again (its D2H finished)
-                flush_host_slot(c, s, angles, levels, bins, counts, G, l);
+                flush_host_slot(c, s, angles, levels, bins, counts, G, l, elevation);
             }
             const float *src = in_c64 + ((size_t)i0 * G + l) * h->nsamples * 2;
             {
@@ -1419,12 +1488,13 @@ int process_host_impl(music_b200 *h, const float *in_c64, uint32_t nwindows, flo
             {
                 NvtxRange r("music_b200: kernels");
                 rc = enqueue_device(c, c->d_in[s], W, c->d_ang[s], c->d_lvl[s], spectrum ? c->d_spec[s] : nullptr, c->d_bins[s],
-                                    nullptr, nullptr, nullptr, counts ? c->d_cnt[s] : nullptr, st, s);
+                                    nullptr, nullptr, nullptr, counts ? c->d_cnt[s] : nullptr, st, s, nullptr, 0,
+                                    elevation ? c->d_el[s] : nullptr);
                 if (rc && c != h) fail(h, rc, "%s", std::string(c->error).c_str());
                 if (rc) break;
             }
             NvtxRange r("music_b200: D2H");
-            rc = download_host_slot(c, s, i0, W, levels != nullptr, bins != nullptr, counts != nullptr, st);
+            rc = download_host_slot(c, s, i0, W, levels != nullptr, bins != nullptr, counts != nullptr, st, elevation != nullptr);
             if (rc && c != h) fail(h, rc, "%s", std::string(c->error).c_str());
             if (rc) break;
             if (spectrum) {
@@ -1449,8 +1519,8 @@ int process_host_impl(music_b200 *h, const float *in_c64, uint32_t nwindows, flo
     for (uint32_t l = 0; l < G; ++l) {
         music_b200 *c = lanes[l];
         if (rc == MUSIC_B200_OK) {
-            flush_host_slot(c, 0, angles, levels, bins, counts, G, l);
-            flush_host_slot(c, 1, angles, levels, bins, counts, G, l);
+            flush_host_slot(c, 0, angles, levels, bins, counts, G, l, elevation);
+            flush_host_slot(c, 1, angles, levels, bins, counts, G, l, elevation);
         } else {
             c->slot_W[0] = c->slot_W[1] = 0;  // nothing valid to hand out
         }
@@ -1508,6 +1578,7 @@ int music_b200_gather_create(music_b200 *h, uint32_t total_windows, unsigned cha
 {
     if (!h || !ipc_handles) return MUSIC_B200_EINVAL;
     if (!h->kids.empty()) return fail(h, MUSIC_B200_EINVAL, "gather_create applies to single-device handles (a multi-device handle gathers in process_device_sharded)");
+    if (h->azel) return fail(h, MUSIC_B200_EINVAL, "the bins all-gather is not supported on an az-el handle");
     std::lock_guard<std::mutex> g(h->mutex);
     CU(h, cudaSetDevice(h->device));
     if (h->gather_buf) return fail(h, MUSIC_B200_EINVAL, "gather buffer already created");
@@ -1530,6 +1601,7 @@ int music_b200_gather_attach(music_b200 *h, int nranks, int rank, const unsigned
 {
     if (!h || !all_handles) return MUSIC_B200_EINVAL;
     if (nranks < 1 || nranks > MAX_PEERS || rank < 0 || rank >= nranks) return fail(h, MUSIC_B200_EINVAL, "need 1 <= nranks <= %d and 0 <= rank < nranks", MAX_PEERS);
+    if (h->azel) return fail(h, MUSIC_B200_EINVAL, "the bins all-gather is not supported on an az-el handle");
     std::lock_guard<std::mutex> g(h->mutex);
     if (!h->gather_buf) return fail(h, MUSIC_B200_EINVAL, "call gather_create first");
     CU(h, cudaSetDevice(h->device));
@@ -1605,6 +1677,79 @@ int music_b200_process_device_sharded(music_b200 *h, const float *const *d_in_c6
         if (rc) fail(h, rc, "%s", std::string(c->error).c_str());
     }
     return rc;
+}
+
+/* ---- (azimuth, elevation) MUSIC (music_azel.cuh) ---- */
+namespace {
+
+// positions_xyz [m][3] and the wavelength: finite, wavelength > 0
+int check_azel_geometry(music_b200 *h, uint32_t m, const double *positions_xyz, double wavelength)
+{
+    if (!positions_xyz) return fail(h, MUSIC_B200_EINVAL, "element positions must not be NULL");
+    if (!(wavelength > 0.0) || !std::isfinite(wavelength)) return fail(h, MUSIC_B200_EINVAL, "wavelength must be positive and finite");
+    for (uint32_t i = 0; i < 3 * m; ++i)
+        if (!std::isfinite(positions_xyz[i])) return fail(h, MUSIC_B200_EINVAL, "element positions must be finite");
+    return MUSIC_B200_OK;
+}
+
+}  // namespace
+
+int music_b200_create_azel(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples, uint32_t n_az, uint32_t n_el,
+                           double el_lo_deg, double el_hi_deg, const double *positions_xyz, double wavelength, int device)
+{
+    if (!out) return fail(nullptr, MUSIC_B200_EINVAL, "out must not be NULL");
+    *out = nullptr;
+    if (m == 0 || m > MUSIC_B200_MAX_M) return fail(nullptr, MUSIC_B200_EINVAL, "m must be in 1..%d (got %u)", MUSIC_B200_MAX_M, m);
+    if (n == 0 || n >= m) return fail(nullptr, MUSIC_B200_EINVAL, "need 1 <= n < m (got n=%u, m=%u)", n, m);
+    if (nsamples == 0 || nsamples % m != 0) return fail(nullptr, MUSIC_B200_EINVAL, "nsamples must be a positive multiple of m (got %u)", nsamples);
+    if (n_az == 0 || n_el == 0) return fail(nullptr, MUSIC_B200_EINVAL, "n_az and n_el must be > 0");
+    if ((uint64_t)n_az * n_el > MUSIC_B200_AZEL_MAX_BINS)
+        return fail(nullptr, MUSIC_B200_EINVAL, "n_az * n_el must be at most %u (got %llu)", (unsigned)MUSIC_B200_AZEL_MAX_BINS, (unsigned long long)n_az * n_el);
+    if (!(el_lo_deg >= -90.0 && el_lo_deg <= el_hi_deg && el_hi_deg <= 90.0))
+        return fail(nullptr, MUSIC_B200_EINVAL, "need -90 <= el_lo <= el_hi <= 90 degrees (got %g, %g)", el_lo_deg, el_hi_deg);
+    if (n_el >= 2 && !(el_lo_deg < el_hi_deg)) return fail(nullptr, MUSIC_B200_EINVAL, "n_el >= 2 needs el_lo < el_hi");
+    const int rc = check_azel_geometry(nullptr, m, positions_xyz, wavelength);
+    if (rc) return rc;
+    const AzelGrid grid = {(int)n_az, (int)n_el, el_lo_deg, el_hi_deg};
+    return create_on_device(out, m, n, nsamples, n_az * n_el, nullptr, device, &grid, positions_xyz, wavelength);
+}
+
+int music_b200_set_geometry_azel(music_b200 *h, const double *positions_xyz, double wavelength)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (!h->azel) return fail(h, MUSIC_B200_EINVAL, "set_geometry_azel needs a handle from music_b200_create_azel");
+    const int rc = check_azel_geometry(h, h->m, positions_xyz, wavelength);
+    if (rc) return rc;
+    std::lock_guard<std::mutex> g(h->mutex);
+    CU(h, cudaSetDevice(h->device));
+    CU(h, cudaDeviceSynchronize());  // as in set_table(): the slot being rebuilt must be idle
+    const int slot = h->cur_table ^ 1;
+    const int rb = build_table_azel(h, slot, positions_xyz, wavelength, h->streams[0]);
+    if (rb) return rb;
+    h->cur_table = slot;
+    return MUSIC_B200_OK;
+}
+
+int music_b200_process_azel_device(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_azimuth, float *d_elevation,
+                                   float *d_levels, float *d_spectrum, int32_t *d_bins, int32_t *d_counts, void *stream)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (!h->azel) return fail(h, MUSIC_B200_EINVAL, "process_azel_device needs a handle from music_b200_create_azel");
+    if (nwindows && (!d_azimuth || !d_elevation)) return fail(h, MUSIC_B200_EINVAL, "d_azimuth and d_elevation must not be NULL");
+    std::lock_guard<std::mutex> g(h->mutex);
+    NvtxRange range("music_b200_process_azel_device");
+    CU(h, cudaSetDevice(h->device));
+    return enqueue_device(h, d_in_c64, nwindows, d_azimuth, d_levels, d_spectrum, d_bins, nullptr, nullptr, nullptr, d_counts,
+                          static_cast<cudaStream_t>(stream), 0, nullptr, 0, d_elevation);
+}
+
+int music_b200_process_azel_host(music_b200 *h, const float *in_c64, uint32_t nwindows, float *azimuth, float *elevation,
+                                 float *levels, float *spectrum, int32_t *bins, int32_t *counts)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (!h->azel) return fail(h, MUSIC_B200_EINVAL, "process_azel_host needs a handle from music_b200_create_azel");
+    if (nwindows && !elevation) return fail(h, MUSIC_B200_EINVAL, "elevation must not be NULL");
+    return process_host_impl(h, in_c64, nwindows, azimuth, levels, spectrum, bins, counts, elevation);
 }
 
 void music_b200_destroy(music_b200 *h)

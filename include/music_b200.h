@@ -232,6 +232,67 @@ int music_b200_set_geometry(music_b200 *h, const double *positions_xy, double wa
 void music_b200_steer_entry_host(const double *positions_xy, double wavelength, uint32_t resolution, uint32_t step,
                                  uint32_t antenna, float *re_im);
 
+/*
+ * (azimuth, elevation) MUSIC over a 3-D array geometry (extension, no reference counterpart).
+ * An az-el handle has n_az azimuth steps, n_el elevation steps, an elevation range [el_lo, el_hi] in degrees
+ * (-90 <= el_lo <= el_hi <= 90), element positions p_m = (x, y, z) in metres and a wavelength lambda.
+ *   grid       az_k = k * 360 / n_az degrees (k < n_az);  el_i = el_lo + (i * (el_hi - el_lo)) / (n_el - 1), el_0 = el_lo
+ *              for n_el = 1; both evaluated in fp64 in exactly this order.
+ *   direction  u(az, el) = (cos el cos az, cos el sin az, sin el), el measured from the xy-plane (at el = 0 this is the
+ *              reference helper's unit_vect).
+ *   steering   a_m(az, el) = exp(-j 2 pi <p_m, u> / lambda) (the helper's sign convention).
+ *   table      table[i][k][m] = a_m(az_k, el_i) in fp64 rounded to complex64, flat bin b = i * n_az + k, so the handle
+ *              scans K = n_az * n_el rows, elevation-major.  Each component is within one float32 ulp of the fp64 value
+ *              (there is no host helper to be bit-identical to); music_b200_get_table() returns the table in use.
+ *   per window R, eigenvectors, noise subspace and P[b] = 1 / ||G^H a_b||^2 exactly as for a 1-D handle with K = n_az * n_el;
+ *              the source rules (FIXED / MDL / AIC) apply unchanged.
+ *   outputs    bins = b;  azimuth = (float)(k * 360.0 / n_az) (the 1-D angle expression);  elevation = (float)el_i;
+ *              level = (float)P[b];  unfilled slots (0, 0, 0, bin -1);  spectrum [W][n_el][n_az] float32.
+ *   peak rules MUSIC_B200_PEAKS_TOP_BINS (default): the reference's rule on the flat index (the n largest bins, strict
+ *              '>', lowest b on ties).  MUSIC_B200_PEAKS_LOCAL_MAXIMA: b is a candidate iff P[b] > 0 and, for each of its
+ *              up to 8 grid neighbours j (azimuth circular, elevation rows do not wrap), P[b] > P[j] or (P[b] == P[j] and
+ *              b < j); peaks are taken in descending strength, ties to the lowest b, skipping a candidate whose Chebyshev
+ *              grid distance max(min(|dk|, n_az - |dk|), |di|) to a peak already taken is <= exclusion_bins.  The tie
+ *              clause gives a constant row (the zenith row of a planar array) exactly one maximum.
+ *   refinement MUSIC_B200_REFINE_NEWTON (geometric tables only, as in 1-D) minimises the exact fp64
+ *              D(az, el) = sum_j |g_j^H a(az, el)|^2 (G the noise eigenvectors the scan used) inside the box
+ *              [az_b -+ d_az] x [max(el_b - d_el, el_lo), min(el_b + d_el, el_hi)], d_az = 360 / n_az, d_el = one
+ *              elevation step (0 for n_el = 1), angles in radians, gradient g and Hessian H analytic
+ *              (theta_m = 2 pi <p_m, u> / lambda; d2 theta_m / d el2 = -theta_m).  At most 50 iterations of:
+ *                1. s = -H^-1 g if H11 > 0 and det H > 0, else s = -g d_az / ||g||; stop if g = 0;
+ *                2. s = clamp(x + s) - x, the clamp componentwise into the box;
+ *                3. halve t from 1 while t > 2^-30 until D(x + t s) <= D(x); stop if there is no such t;
+ *                4. x = x + t s; stop once max |t s| <= 1e-12 rad.
+ *              x* is kept iff x* != x_b and D(x*) <= D(x_b): azimuth = (float) of x*_az in degrees wrapped into
+ *              [0, 360) as in 1-D, elevation = (float) of x*_el in degrees; otherwise the slot keeps its grid angles.
+ *              level = (float)(1 / D) at the point kept (as in 1-D, the analytic level even where the grid point is
+ *              kept).  Bins, spectrum and counts stay the grid results.
+ * Caveat: for a planar array (all z equal) +el and -el have bit-identical table rows, so on a grid with el_lo < 0 the
+ * tie rules resolve every such pair to the negative elevation (the lower b).  Use el_lo >= 0 for planar arrays.
+ * An az-el handle is single-device and always runs the unfused kernels (plus the decode and, with refinement, the 2-D
+ * refinement kernel, both timed in the top-n slot of the stage timing).  set_table() accepts a [n_el][n_az][m] table (a
+ * measured or calibrated manifold; refinement then returns EINVAL, as in 1-D); set_peak_mode(), set_source_rule(),
+ * set_refine(), the stage timing, get_table(), the reducers and launch_count() work as on a 1-D handle.  The 1-D
+ * process_* entries, set_geometry(), the planar entries and the gather / sharded entries return EINVAL on an az-el
+ * handle; set_geometry_azel() and the _azel entries return EINVAL on a 1-D handle.
+ *
+ * create_azel: positions_xyz [m][3] doubles (finite), wavelength finite and > 0, 1 <= n < m <= MUSIC_B200_MAX_M,
+ * nsamples a positive multiple of m, n_az, n_el >= 1 with n_az * n_el <= MUSIC_B200_AZEL_MAX_BINS, el_lo < el_hi when
+ * n_el >= 2.  The argument checks come first (EINVAL); ENODEVICE without an sm_90 device.
+ * set_geometry_azel: retune, with the locking and double buffering of music_b200_set_table().
+ * process_azel_host / _device: as process_host_counts / process_device_counts, plus the elevations (n floats per
+ * window, required like the azimuths); levels, spectrum, bins and counts may be NULL.
+ */
+#define MUSIC_B200_AZEL_MAX_BINS (1u << 20)
+int music_b200_create_azel(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples, uint32_t n_az, uint32_t n_el,
+                           double el_lo_deg, double el_hi_deg, const double *positions_xyz /* [m][3] */, double wavelength,
+                           int device);
+int music_b200_set_geometry_azel(music_b200 *h, const double *positions_xyz /* [m][3] */, double wavelength);
+int music_b200_process_azel_host(music_b200 *h, const float *in_c64, uint32_t nwindows, float *azimuth, float *elevation,
+                                 float *levels, float *spectrum, int32_t *bins, int32_t *counts);
+int music_b200_process_azel_device(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_azimuth, float *d_elevation,
+                                   float *d_levels, float *d_spectrum, int32_t *d_bins, int32_t *d_counts, void *stream);
+
 /* Copies the table currently in use (float[resolution][m][2]) back to host memory. */
 int music_b200_get_table(music_b200 *h, float *table_c64);
 

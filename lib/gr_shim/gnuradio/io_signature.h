@@ -24,6 +24,10 @@ public:
         v.push_back(s1); v.push_back(s2); v.push_back(s3);
         return sptr(new io_signature(min_streams, max_streams, v));
     }
+    static sptr makev(int min_streams, int max_streams, const std::vector<int> &sizeof_stream_items)
+    {
+        return sptr(new io_signature(min_streams, max_streams, sizeof_stream_items));
+    }
     int min_streams() const { return d_min; }
     int max_streams() const { return d_max; }
     int sizeof_stream_item(int index) const
