@@ -77,6 +77,8 @@ def load():
         L.music_b200_set_source_rule.restype = ctypes.c_int
         L.music_b200_set_refine.argtypes = [vp, ctypes.c_int]
         L.music_b200_set_refine.restype = ctypes.c_int
+        L.music_b200_set_estimator.argtypes = [vp, ctypes.c_int, ctypes.c_double]
+        L.music_b200_set_estimator.restype = ctypes.c_int
         L.music_b200_set_geometry.argtypes = [vp, fp, ctypes.c_double, ctypes.POINTER(u32)]
         L.music_b200_set_geometry.restype = ctypes.c_int
         L.music_b200_steer_entry_host.argtypes = [fp, ctypes.c_double, u32, u32, u32, fp]
@@ -123,7 +125,7 @@ def load():
 EXPORTS = [
     "music_b200_version", "music_b200_create", "music_b200_create_multi", "music_b200_device_count",
     "music_b200_process_device_sharded", "music_b200_gather_create", "music_b200_gather_attach", "music_b200_gather_wait",
-    "music_b200_gather_buffer", "music_b200_gather_read", "music_b200_set_table", "music_b200_set_geometry", "music_b200_set_peak_mode", "music_b200_set_source_rule", "music_b200_set_refine", "music_b200_reduce_angles_device",
+    "music_b200_gather_buffer", "music_b200_gather_read", "music_b200_set_table", "music_b200_set_geometry", "music_b200_set_peak_mode", "music_b200_set_source_rule", "music_b200_set_refine", "music_b200_set_estimator", "music_b200_reduce_angles_device",
     "music_b200_reduce_spectrum_device", "music_b200_reduce_angles_host", "music_b200_reduce_spectrum_host",
     "music_b200_get_table", "music_b200_steer_entry_host", "music_b200_process_host",
     "music_b200_process_device", "music_b200_process_device_ex", "music_b200_process_host_counts",

@@ -245,6 +245,66 @@ __device__ __noinline__ void azel_eval(const AzelGeom &geo, const double2 *__res
     }
 }
 
+// F = -B, B(ph, ep) = a^H R a, with its gradient and Hessian in e (EST_BARTLETT, music_refine.cuh).  With y = R a,
+// y_u = R a_u:  B_u = 2 Re(a_u^H y),  B_uv = 2 (Re(a_u^H y_v) + Re(a_uv^H y)),  a_u = -j theta_u a,
+// a_uv = (-theta_u theta_v - j theta_uv) a; theta and its derivatives as in azel_eval.
+__device__ __noinline__ void bartlett_azel_eval(const AzelGeom &geo, const double2 *__restrict__ Rw, int M, double ph, double ep,
+                                                double *e)
+{
+    double sp, cp, se, ce;
+    sincos(ph, &sp, &cp);
+    sincos(ep, &se, &ce);
+    double ar[MAXM], ai[MAXM], th[MAXM], tp[MAXM], te[MAXM], tpp[MAXM], tpe[MAXM];
+    for (int m = 0; m < M; ++m) {
+        const double x = geo.pos[3 * m], y = geo.pos[3 * m + 1], z = geo.pos[3 * m + 2];
+        const double h = x * cp + y * sp, v = y * cp - x * sp;
+        th[m] = STEER_TWO_PI * ((ce * h + z * se) / geo.lambda);
+        tp[m] = STEER_TWO_PI * ((ce * v) / geo.lambda);
+        te[m] = STEER_TWO_PI * ((z * ce - se * h) / geo.lambda);
+        tpp[m] = -STEER_TWO_PI * ((ce * h) / geo.lambda);
+        tpe[m] = -STEER_TWO_PI * ((se * v) / geo.lambda);
+        double s, c;
+        sincos(th[m], &s, &c);
+        ar[m] = c;
+        ai[m] = -s;
+    }
+    double b[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    for (int i = 0; i < M; ++i) {
+        double yr = 0.0, yi = 0.0, ypr = 0.0, ypi = 0.0, yer = 0.0, yei = 0.0;  // (R a)_i, (R a_ph)_i, (R a_ep)_i
+        for (int j = 0; j < M; ++j) {
+            const double2 r = Rw[i * M + j];
+            const double cr = r.x * ar[j] - r.y * ai[j], ci = r.x * ai[j] + r.y * ar[j];  // R_ij a_j
+            yr += cr;
+            yi += ci;
+            ypr += tp[j] * ci;  // R_ij a_u,j = theta_u (ci - j cr)
+            ypi -= tp[j] * cr;
+            yer += te[j] * ci;
+            yei -= te[j] * cr;
+        }
+        const double pr = tp[i] * ai[i], pi = -tp[i] * ar[i];  // a_ph,i
+        const double er = te[i] * ai[i], ei = -te[i] * ar[i];  // a_ep,i
+        const double qpp = tp[i] * tp[i], qpe = tp[i] * te[i], qee = te[i] * te[i];
+        const double ppr = -qpp * ar[i] + tpp[i] * ai[i], ppi = -qpp * ai[i] - tpp[i] * ar[i];  // a_phph,i
+        const double per = -qpe * ar[i] + tpe[i] * ai[i], pei = -qpe * ai[i] - tpe[i] * ar[i];  // a_phep,i
+        const double eer = -qee * ar[i] - th[i] * ai[i], eei = -qee * ai[i] + th[i] * ar[i];   // a_epep,i (theta_epep = -theta)
+        b[0] += ar[i] * yr + ai[i] * yi;
+        b[1] += 2.0 * (pr * yr + pi * yi);
+        b[2] += 2.0 * (er * yr + ei * yi);
+        b[3] += 2.0 * (pr * ypr + pi * ypi + ppr * yr + ppi * yi);
+        b[4] += 2.0 * (pr * yer + pi * yei + per * yr + pei * yi);
+        b[5] += 2.0 * (er * yer + ei * yei + eer * yr + eei * yi);
+    }
+    for (int q = 0; q < 6; ++q) e[q] = -b[q];
+}
+
+template <int EST>
+__device__ __forceinline__ void azel_est_eval(const AzelGeom &geo, const double2 *__restrict__ G, int M, int p, double ph, double ep,
+                                              double *e)
+{
+    if constexpr (EST == EST_BARTLETT) bartlett_azel_eval(geo, G, M, ph, ep, e);
+    else azel_eval(geo, G, M, p, ph, ep, e);
+}
+
 __device__ __forceinline__ double azel_clamp(double v, double lo, double hi) { return v < lo ? lo : (v > hi ? hi : v); }
 
 constexpr double AZEL_T_MIN = 9.313225746154785e-10;  // 2^-30: smallest step fraction of the line search (exclusive)
@@ -252,6 +312,8 @@ constexpr double AZEL_T_MIN = 9.313225746154785e-10;  // 2^-30: smallest step fr
 // Slot o = w * n + i with bins[o] >= 0: projected Newton on D inside the box of one grid step either side of the grid
 // point (the elevation range clipped to [el_lo, el_hi]); a result that moved and does not raise D replaces the decoded
 // grid angles.  levels[o] (may be null) = 1 / D at the point kept.  counts (may be null): per-window source count.
+// EST and Vt as for refine_peaks_kernel (music_refine.cuh); under EST_BARTLETT the level is -F / M^2 = B / M^2.
+template <int EST = EST_MUSIC>
 __global__ void __launch_bounds__(REFINE_THREADS) refine_azel_kernel(const double *__restrict__ Vt, const int32_t *__restrict__ counts,
                                                                      const int32_t *__restrict__ bins, int M, int n, int W,
                                                                      const AzelGeom geo, float *__restrict__ angles,
@@ -262,7 +324,8 @@ __global__ void __launch_bounds__(REFINE_THREADS) refine_azel_kernel(const doubl
     const int b = bins[o];
     if (b < 0) return;
     const int w = o / n;
-    const int p = M - (counts ? counts[w] : n);
+    int p = M;
+    if constexpr (EST == EST_MUSIC) p = M - (counts ? counts[w] : n);
     const double2 *G = reinterpret_cast<const double2 *>(Vt) + (size_t)w * M * M;
     const AzelGrid &g = geo.grid;
     const int i = b / g.n_az, k = b - i * g.n_az;
@@ -273,7 +336,7 @@ __global__ void __launch_bounds__(REFINE_THREADS) refine_azel_kernel(const doubl
     const double plo = ph_b - dph, phi = ph_b + dph;
     const double elo = fmax(ep_b - dep, g.el_lo * STEER_DEG2RAD), ehi = fmin(ep_b + dep, g.el_hi * STEER_DEG2RAD);
     double e[6], f[6];
-    azel_eval(geo, G, M, p, ph_b, ep_b, e);
+    azel_est_eval<EST>(geo, G, M, p, ph_b, ep_b, e);
     const double Db = e[0];
     double x0 = ph_b, x1 = ep_b;
     for (int it = 0; it < REFINE_MAX_IT; ++it) {
@@ -296,7 +359,7 @@ __global__ void __launch_bounds__(REFINE_THREADS) refine_azel_kernel(const doubl
         while (t > AZEL_T_MIN) {
             y0 = __dadd_rn(x0, __dmul_rn(t, s0));
             y1 = __dadd_rn(x1, __dmul_rn(t, s1));
-            azel_eval(geo, G, M, p, y0, y1, f);
+            azel_est_eval<EST>(geo, G, M, p, y0, y1, f);
             if (f[0] <= e[0]) { ok = true; break; }
             t *= 0.5;
         }
@@ -317,7 +380,11 @@ __global__ void __launch_bounds__(REFINE_THREADS) refine_azel_kernel(const doubl
         angles[o] = az;
         elev[o] = (float)(x1 * REFINE_RAD2DEG);
     }
-    if (levels) levels[o] = (float)(1.0 / D);
+    if constexpr (EST == EST_BARTLETT) {
+        if (levels) levels[o] = (float)(-D / ((double)M * (double)M));
+    } else {
+        if (levels) levels[o] = (float)(1.0 / D);
+    }
 }
 
 }  // namespace music

@@ -30,6 +30,7 @@
 #include "music_sources.cuh"
 #include "music_refine.cuh"
 #include "music_azel.cuh"
+#include "music_estimators.cuh"
 
 using namespace music;
 
@@ -78,6 +79,8 @@ struct music_b200 {
     uint32_t peak_excl = 0;
     int source_rule = MUSIC_B200_SOURCES_FIXED;  // set_source_rule()
     int refine = MUSIC_B200_REFINE_OFF;          // set_refine()
+    int estimator = MUSIC_B200_ESTIMATOR_MUSIC;  // set_estimator()
+    double loading = 0.0;                        // MVDR diagonal loading (set_estimator())
     unsigned steer_guarded = 0;    // entries of the last built table re-evaluated with the host libm
     bool azel = false;             // music_b200_create_azel(): K = n_az * n_el rows, elevation-major (music_azel.cuh)
     AzelGrid grid = {};
@@ -367,6 +370,32 @@ void launch_scan(music_b200 *h, const Workspace &ws, const double *soa, uint32_t
     h->launches++;
 }
 
+// K3 of the MVDR / Bartlett spectra (music_estimators.cuh): q = the g_j of mvdr_prep_kernel (MVDR) or R (Bartlett)
+template <int MT>
+void launch_scan_quad(music_b200 *h, int est, const double *q, const double *soa, uint32_t W, bool argmax, bool p64, bool spec,
+                      PeakOut po, float *d_spec, double *d_p64, const int32_t *counts, cudaStream_t st)
+{
+    const int grid = (W + SCAN_B - 1) / SCAN_B;
+    const size_t smem = (size_t)SCAN_B * h->m * h->m * 2 * sizeof(double);
+#define QUAD_CASE(A, P, S)                                                                                                    \
+    if (argmax == A && p64 == P && spec == S) {                                                                               \
+        if (est == MUSIC_B200_ESTIMATOR_MVDR)                                                                                 \
+            scan_quad_kernel<MT, QUAD_MVDR, A, P, S><<<grid, TILE, smem, st>>>(soa, q, (int)h->m, (int)h->K, (int)W, po, d_spec, \
+                                                                               d_p64, counts);                               \
+        else                                                                                                                  \
+            scan_quad_kernel<MT, QUAD_BARTLETT, A, P, S><<<grid, TILE, smem, st>>>(soa, q, (int)h->m, (int)h->K, (int)W, po,    \
+                                                                                   d_spec, d_p64, counts);                   \
+    }
+    QUAD_CASE(true, false, false)
+    QUAD_CASE(true, false, true)
+    QUAD_CASE(true, true, false)
+    QUAD_CASE(true, true, true)
+    QUAD_CASE(false, true, false)
+    QUAD_CASE(false, true, true)
+#undef QUAD_CASE
+    h->launches++;
+}
+
 cudaEvent_t *timing_events(music_b200 *h)
 {
     if (!h->timing) return nullptr;
@@ -519,7 +548,10 @@ int launch_eig_scan(music_b200 *h, const Workspace &ws, uint32_t W, const PeakOu
     const bool refine = h->refine != MUSIC_B200_REFINE_OFF;
     PeakOut po = po_in;
     if ((refine || h->azel) && !po.bins) po.bins = ws.bins;
-    {
+    const int est = h->estimator;
+    const bool music_est = est == MUSIC_B200_ESTIMATOR_MUSIC;
+    // MVDR and Bartlett need the eigensolver only to count sources or when the caller asked for the eigenvalues
+    if (music_est || h->source_rule != MUSIC_B200_SOURCES_FIXED || d_ev_out) {
         const int grid = (W + 127) / 128;
         switch (M) {
         case 4: eig_kernel<4, true><<<grid, 128, 0, st>>>(ws.R, ws.ev, ws.Vt, M, (int)W); break;
@@ -540,13 +572,27 @@ int launch_eig_scan(music_b200 *h, const Workspace &ws, uint32_t W, const PeakOu
         h->launches++;
         cnt = ws.cnt;
     }
+    // MVDR: the rows of L^-1 of R + delta I into ws.Vt (timed with the eigensolver)
+    if (est == MUSIC_B200_ESTIMATOR_MVDR) {
+        mvdr_prep_kernel<<<(W + PREP_WARPS - 1) / PREP_WARPS, PREP_WARPS * 32, 0, st>>>(ws.R, ws.Vt, M, (int)W, h->loading);
+        h->launches++;
+    }
     if (tev) cudaEventRecord(tev[2], st);
     const bool local = h->peak_mode == MUSIC_B200_PEAKS_LOCAL_MAXIMA;
     const bool argmax = (h->n == 1) && !local;
     const bool need_p64 = !argmax || d_P64_out != nullptr;
     double *p64 = d_P64_out ? d_P64_out : ws.P64;
     const bool fast = argmax && !need_p64 && !d_spec && (M == 4 || M == 8 || M == 16);
-    if (fast) {
+    if (!music_est) {
+        const double *q = est == MUSIC_B200_ESTIMATOR_MVDR ? ws.Vt : ws.R;
+        const bool spec = d_spec != nullptr;
+        switch (M) {
+        case 4: launch_scan_quad<4>(h, est, q, soa, W, argmax, need_p64, spec, po, d_spec, p64, cnt, st); break;
+        case 8: launch_scan_quad<8>(h, est, q, soa, W, argmax, need_p64, spec, po, d_spec, p64, cnt, st); break;
+        case 16: launch_scan_quad<16>(h, est, q, soa, W, argmax, need_p64, spec, po, d_spec, p64, cnt, st); break;
+        default: launch_scan_quad<0>(h, est, q, soa, W, argmax, need_p64, spec, po, d_spec, p64, cnt, st); break;
+        }
+    } else if (fast) {
         const int grid = (W + SCAN_B - 1) / SCAN_B;
         if (M == 4) scan_peak1_kernel<4><<<grid, TILE, 0, st>>>(soa, ws.Vt, (int)h->K, (int)W, po, cnt);
         else if (M == 8) scan_peak1_kernel<8><<<grid, TILE, 0, st>>>(soa, ws.Vt, (int)h->K, (int)W, po, cnt);
@@ -573,15 +619,21 @@ int launch_eig_scan(music_b200 *h, const Workspace &ws, uint32_t W, const PeakOu
         azel_decode_kernel<<<(slots + 255) / 256, 256, 0, st>>>(po.bins, slots, h->grid, po.angles, d_el);
         h->launches++;
     }
-    if (refine && h->azel) {
-        const int slots = (int)(W * h->n);
-        refine_azel_kernel<<<(slots + REFINE_THREADS - 1) / REFINE_THREADS, REFINE_THREADS, 0, st>>>(ws.Vt, cnt, po.bins, M, (int)h->n, (int)W,
-                                                                                                   tb.ageo, po.angles, d_el, po.levels);
-        h->launches++;
-    } else if (refine) {
-        const int slots = (int)(W * h->n);
-        refine_peaks_kernel<<<(slots + REFINE_THREADS - 1) / REFINE_THREADS, REFINE_THREADS, 0, st>>>(ws.Vt, cnt, po.bins, M, (int)h->n, (int)h->K, (int)W, tb.geo,
-                                                                po.angles, po.levels);
+    if (refine) {
+        const int slots = (int)(W * h->n), rgrid = (slots + REFINE_THREADS - 1) / REFINE_THREADS;
+        // the vectors the refined objective is built from: noise eigenvectors (MUSIC), rows of L^-1 (MVDR), R (Bartlett)
+        const double *rv = est == MUSIC_B200_ESTIMATOR_BARTLETT ? ws.R : ws.Vt;
+#define REFINE_CASE(E)                                                                                                         \
+        if (h->azel)                                                                                                           \
+            refine_azel_kernel<E><<<rgrid, REFINE_THREADS, 0, st>>>(rv, cnt, po.bins, M, (int)h->n, (int)W, tb.ageo, po.angles, d_el, \
+                                                                    po.levels);                                                \
+        else                                                                                                                   \
+            refine_peaks_kernel<E><<<rgrid, REFINE_THREADS, 0, st>>>(rv, cnt, po.bins, M, (int)h->n, (int)h->K, (int)W, tb.geo,   \
+                                                                     po.angles, po.levels);
+        if (est == MUSIC_B200_ESTIMATOR_MVDR) { REFINE_CASE(EST_MVDR) }
+        else if (est == MUSIC_B200_ESTIMATOR_BARTLETT) { REFINE_CASE(EST_BARTLETT) }
+        else { REFINE_CASE(EST_MUSIC) }
+#undef REFINE_CASE
         h->launches++;
     }
     if (tev) cudaEventRecord(tev[4], st);
@@ -635,9 +687,10 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, float *d
         for (uint32_t r = 0; r < h->m; ++r) planar_fusable = planar_fusable && (reinterpret_cast<uintptr_t>(planar->p[r]) & 15u) == 0;
     }
     const bool local_peaks = h->peak_mode == MUSIC_B200_PEAKS_LOCAL_MAXIMA;
+    const bool music_est = h->estimator == MUSIC_B200_ESTIMATOR_MUSIC;
     // the fused kernels find the principal eigenvector only, not every eigenvalue a source count needs nor the noise
-    // eigenvectors the peak refinement needs
-    if ((!planar || planar_fusable) && h->fused && !h->azel && fixed_n && !refine && !local_peaks && h->m == 4 && h->n == 1 && (!d_spec || h->fused_spec) && !d_P64 && !d_R && !d_ev) {
+    // eigenvectors the peak refinement needs; they compute the MUSIC spectrum only
+    if ((!planar || planar_fusable) && h->fused && !h->azel && music_est && fixed_n && !refine && !local_peaks && h->m == 4 && h->n == 1 && (!d_spec || h->fused_spec) && !d_P64 && !d_R && !d_ev) {
         // whole call in one persistent launch (music_fused.cuh); no workspace involved
         cudaEvent_t *tev = timing_events(h);
         if (tev) cudaEventRecord(tev[0], st);
@@ -679,7 +732,7 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, float *d
         CU(h, cudaGetLastError());
         return MUSIC_B200_OK;
     }
-    if (!planar && h->fused && !h->azel && fixed_n && !refine && !local_peaks && h->m == 8 && h->n == 1 && !d_spec && !d_P64 && !d_R && !d_ev && h->N >= 128 &&
+    if (!planar && h->fused && !h->azel && music_est && fixed_n && !refine && !local_peaks && h->m == 8 && h->n == 1 && !d_spec && !d_P64 && !d_R && !d_ev && h->N >= 128 &&
         h->N % 2 == 0 && encode_tiled_fn()) {
         // M = 8: whole call in one persistent launch (music_fused8.cuh); R and the eigenvectors stay in shared memory
         CUtensorMap tm;
@@ -1417,6 +1470,27 @@ int music_b200_set_refine(music_b200 *h, int mode)
     if (h->kids.empty() && mode != MUSIC_B200_REFINE_OFF && !h->table[h->cur_table].geometric)
         return fail(h, MUSIC_B200_EINVAL, "peak refinement needs a table built by music_b200_set_geometry(); the current one came from set_table()");
     h->refine = mode;
+    return MUSIC_B200_OK;
+}
+
+int music_b200_set_estimator(music_b200 *h, int estimator, double loading)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (estimator != MUSIC_B200_ESTIMATOR_MUSIC && estimator != MUSIC_B200_ESTIMATOR_MVDR && estimator != MUSIC_B200_ESTIMATOR_BARTLETT)
+        return fail(h, MUSIC_B200_EINVAL, "unknown estimator %d", estimator);
+    if (!std::isfinite(loading) || loading < 0.0) return fail(h, MUSIC_B200_EINVAL, "loading must be finite and >= 0 (got %g)", loading);
+    if (estimator != MUSIC_B200_ESTIMATOR_MVDR && loading != 0.0)
+        return fail(h, MUSIC_B200_EINVAL, "diagonal loading applies to MVDR only (got %g)", loading);
+    if (estimator == MUSIC_B200_ESTIMATOR_MVDR && loading == 0.0 && h->N <= h->m)
+        return fail(h, MUSIC_B200_EINVAL, "MVDR without diagonal loading needs more snapshots than antennas (N = %u, m = %u): R is singular",
+                    h->N, h->m);
+    std::lock_guard<std::mutex> g(h->mutex);
+    for (music_b200 *c : h->kids) {
+        const int rc = music_b200_set_estimator(c, estimator, loading);
+        if (rc) return fail(h, rc, "%s", music_b200_last_error(c));
+    }
+    h->estimator = estimator;
+    h->loading = loading;
     return MUSIC_B200_OK;
 }
 

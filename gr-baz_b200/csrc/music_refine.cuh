@@ -75,10 +75,71 @@ __device__ __noinline__ void refine_eval(const RefineGeom &geo, const double2 *_
     *D2 = d2;
 }
 
+// The estimator whose spectrum the refinement follows (music_b200_set_estimator, music_estimators.cuh):
+//   EST_MUSIC     D = sum_j |g_j^H a|^2 over the p noise eigenvectors, level 1 / D;
+//   EST_MVDR      the same D over p = M vectors g_j = conj(row j of L^-1), i.e. a^H R_L^-1 a, level 1 / D;
+//   EST_BARTLETT  D = F = -a^H R a (maximising B = a^H R a is minimising F), level -F / M^2 (||a||^2 = M).
+constexpr int EST_MUSIC = 0, EST_MVDR = 1, EST_BARTLETT = 2;
+
+// F = -B, F', F'' with B(theta) = a^H R a for the window's covariance R[i][j] (row i contiguous):
+//   B' = 2 Re(a'^H R a),  B'' = 2 (a'^H R a' + Re(a''^H R a)),  a' = -j psi a,  a'' = (j phi - psi^2) a.
+__device__ __noinline__ void bartlett_eval(const RefineGeom &geo, const double2 *__restrict__ Rw, int M, double th, double *F,
+                                           double *F1, double *F2)
+{
+    double st, ct;
+    sincos(th, &st, &ct);
+    double ar[MAXM], ai[MAXM], ps[MAXM], ph[MAXM];
+    for (int m = 0; m < M; ++m) {
+        const double px = geo.pos[2 * m], py = geo.pos[2 * m + 1];
+        const double phi = STEER_TWO_PI * (fma(py, st, px * ct) / geo.lambda);
+        const double psi = STEER_TWO_PI * (fma(py, ct, -(px * st)) / geo.lambda);
+        double sp, cp;
+        sincos(phi, &sp, &cp);
+        ar[m] = cp;
+        ai[m] = -sp;
+        ps[m] = psi;
+        ph[m] = phi;
+    }
+    double b0 = 0.0, b1 = 0.0, b2 = 0.0;
+    for (int i = 0; i < M; ++i) {
+        double yr = 0.0, yi = 0.0, y1r = 0.0, y1i = 0.0;  // (R a)_i, (R a')_i
+        for (int j = 0; j < M; ++j) {
+            const double2 r = Rw[i * M + j];
+            const double cr = r.x * ar[j] - r.y * ai[j], ci = r.x * ai[j] + r.y * ar[j];  // R_ij a_j
+            yr += cr;
+            yi += ci;
+            y1r += ps[j] * ci;  // R_ij a'_j = psi_j (ci - j cr)
+            y1i -= ps[j] * cr;
+        }
+        const double q = ps[i] * ps[i];
+        const double d1r = ps[i] * ai[i], d1i = -ps[i] * ar[i];                         // a'_i
+        const double d2r = -q * ar[i] - ph[i] * ai[i], d2i = ph[i] * ar[i] - q * ai[i];  // a''_i
+        b0 += ar[i] * yr + ai[i] * yi;
+        b1 += 2.0 * (d1r * yr + d1i * yi);
+        b2 += 2.0 * (d1r * y1r + d1i * y1i + d2r * yr + d2i * yi);
+    }
+    *F = -b0;
+    *F1 = -b1;
+    *F2 = -b2;
+}
+
+template <int EST>
+__device__ __forceinline__ void est_eval(const RefineGeom &geo, const double2 *__restrict__ G, int M, int p, double th, double *D,
+                                         double *D1, double *D2)
+{
+    if constexpr (EST == EST_BARTLETT) bartlett_eval(geo, G, M, th, D, D1, D2);
+    else refine_eval(geo, G, M, p, th, D, D1, D2);
+}
+
 // Slot o = w * n + i with bins[o] >= 0: angles[o] / levels[o] (levels may be null) become the refined angle and
 // 1 / D there; slots with bin -1 are left as the peak rule wrote them.  counts (may be null): per-window source
 // count, so that the noise subspace is the M - counts[w] smallest-eigenvalue vectors, as in the scan.
-__global__ void __launch_bounds__(REFINE_THREADS) refine_peaks_kernel(const double *__restrict__ Vt, const int32_t *__restrict__ counts,
+// Vt: per window M * M complex doubles - the sorted eigenvectors (MUSIC), the g_j of mvdr_prep_kernel (MVDR) or R
+// (BARTLETT); the non-MUSIC estimators ignore n and counts beyond the bins.  The minimum-blocks hint of the non-MUSIC
+// instantiations lets ptxas keep the values live across the evaluation calls in registers (without it the MVDR
+// instantiation spills); the MUSIC instantiation keeps its original bounds.
+template <int EST = EST_MUSIC>
+__global__ void __launch_bounds__(REFINE_THREADS, EST == EST_MUSIC ? 0 : 1) refine_peaks_kernel(const double *__restrict__ Vt, const int32_t *__restrict__ counts,
                                                            const int32_t *__restrict__ bins, int M, int n, int K, int W,
                                                            const RefineGeom geo, float *__restrict__ angles, float *__restrict__ levels)
 {
@@ -87,16 +148,17 @@ __global__ void __launch_bounds__(REFINE_THREADS) refine_peaks_kernel(const doub
     const int b = bins[o];
     if (b < 0) return;
     const int w = o / n;
-    const int p = M - (counts ? counts[w] : n);
+    int p = M;
+    if constexpr (EST == EST_MUSIC) p = M - (counts ? counts[w] : n);
     const double2 *G = reinterpret_cast<const double2 *>(Vt) + (size_t)w * M * M;
     const double deg_b = (double)b * 360.0 / (double)K;  // the grid angle the peak rule reported
     const double tb = deg_b * STEER_DEG2RAD, delta = (360.0 / (double)K) * STEER_DEG2RAD;
     double Db, f, df, Dx, fx, dfx;
-    refine_eval(geo, G, M, p, tb, &Db, &f, &df);
+    est_eval<EST>(geo, G, M, p, tb, &Db, &f, &df);
     double lo = tb - delta, hi = tb + delta;
     double fl, fh;
-    refine_eval(geo, G, M, p, lo, &Dx, &fl, &dfx);
-    refine_eval(geo, G, M, p, hi, &Dx, &fh, &dfx);
+    est_eval<EST>(geo, G, M, p, lo, &Dx, &fl, &dfx);
+    est_eval<EST>(geo, G, M, p, hi, &Dx, &fh, &dfx);
     double x = tb;
     if (fl < 0.0 && fh > 0.0) {
         double dxold = hi - lo, dx = dxold;
@@ -112,7 +174,7 @@ __global__ void __launch_bounds__(REFINE_THREADS) refine_peaks_kernel(const doub
                 x -= dx;
             }
             if (fabs(dx) <= REFINE_TOL) break;
-            refine_eval(geo, G, M, p, x, &Dx, &f, &df);
+            est_eval<EST>(geo, G, M, p, x, &Dx, &f, &df);
             if (f < 0.0) lo = x;
             else hi = x;
         }
@@ -120,7 +182,7 @@ __global__ void __launch_bounds__(REFINE_THREADS) refine_peaks_kernel(const doub
     double D = Db;
     float ang = (float)deg_b;
     if (x != tb) {
-        refine_eval(geo, G, M, p, x, &Dx, &fx, &dfx);
+        est_eval<EST>(geo, G, M, p, x, &Dx, &fx, &dfx);
         if (Dx <= Db) {  // NaN keeps the grid angle
             D = Dx;
             double a = fmod(x * REFINE_RAD2DEG, 360.0);
@@ -130,7 +192,11 @@ __global__ void __launch_bounds__(REFINE_THREADS) refine_peaks_kernel(const doub
         }
     }
     angles[o] = ang;
-    if (levels) levels[o] = (float)(1.0 / D);
+    if constexpr (EST == EST_BARTLETT) {
+        if (levels) levels[o] = (float)(-D / ((double)M * (double)M));
+    } else {
+        if (levels) levels[o] = (float)(1.0 / D);
+    }
 }
 
 }  // namespace music

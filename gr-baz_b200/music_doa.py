@@ -140,6 +140,25 @@ class music_doa(object):
     def refine(self):
         return getattr(self, "_refine", False)
 
+    # -- extension: the spectrum estimator -----------------------------------------------------------
+    ESTIMATORS = {"music": 0, "mvdr": 1, "bartlett": 2}
+
+    def set_estimator(self, kind="music", loading=0.0):
+        """``"music"`` (default): P = 1 / ||G^H a||^2.  ``"bartlett"``: the delay-and-sum beamscan,
+        P = a^H R a / (a^H a)^2.  ``"mvdr"``: the Capon spectrum P = 1 / (a^H (R + delta I)^-1 a) with the diagonal
+        loading delta = loading * tr(R) / m; loading 0 needs more snapshots than antennas.  Both new spectra are power
+        estimates (include/music_b200.h); the peak rule, ``n`` slots, the source rule and the refinement apply to them
+        unchanged.  ``loading`` must be 0 for "music" and "bartlett"."""
+        if kind not in self.ESTIMATORS:
+            raise ValueError("kind must be one of %s" % sorted(self.ESTIMATORS))
+        _capi.check(self._lib.music_b200_set_estimator(self._h, self.ESTIMATORS[kind], float(loading)), self._h)
+        self._estimator = (kind, float(loading))
+
+    @property
+    def estimator(self):
+        """(kind, loading) in use"""
+        return getattr(self, "_estimator", ("music", 0.0))
+
     # -- extension (SURVEY.md section 8(f) rank 4): GUI-rate reducers -----------------------------
     def reduce_angles(self, angles, levels=None, weighted=False):
         """Circular mean (degrees), mean resultant length and total weight per angle slot over the

@@ -36,7 +36,8 @@ def calculate_antenna_array_response(antenna_array, angular_resolution, l):
 
 class music_doa_helper(object):
     def __init__(self, m, n, nsamples, angular_resolution, frequency, array_spacing, antenna_array,
-                 output_spectrum=False, device=0, device_table=False, refine=False):
+                 output_spectrum=False, device=0, device_table=False, refine=False,
+                 estimator="music", loading=0.0):
         self.m = m
         self.n = n
         self.nsamples = nsamples
@@ -64,6 +65,9 @@ class music_doa_helper(object):
         self.array_response = calculate_antenna_array_response(self.antenna_array, self.angular_resolution, self.l)
         self.impl = music_doa(self.m, self.n, self.nsamples, self.array_response, self.angular_resolution,
                               device=device)  # :89
+        # extension: estimator="mvdr" / "bartlett" (music_doa.set_estimator); the default keeps the MUSIC spectrum
+        if estimator != "music" or loading != 0.0:
+            self.impl.set_estimator(estimator, loading)
         if self.refine:
             self.impl.set_array_geometry(self.antenna_array, self.l)
             self.impl.set_refine(True)

@@ -174,6 +174,41 @@ int music_b200_set_source_rule(music_b200 *h, int rule);
 int music_b200_set_refine(music_b200 *h, int mode);
 
 /*
+ * Spectrum estimator (extension, no reference counterpart).  R is the window's covariance, a = a_k table row k widened
+ * to fp64, M = m.
+ *   MUSIC_B200_ESTIMATOR_MUSIC (default)  P[k] = 1 / ||G^H a||^2, unchanged.
+ *   MUSIC_B200_ESTIMATOR_BARTLETT         P[k] = (a^H R a) / (a^H a)^2: the output power of the unit-gain beam
+ *                                         w = a / ||a||^2 (delay-and-sum beamscan).  No eigendecomposition, no n.
+ *   MUSIC_B200_ESTIMATOR_MVDR             delta = loading * tr(R) / M,  R_L = R + delta I,  P[k] = 1 / (a^H R_L^-1 a):
+ *                                         the output power of the distortionless (Capon) beam.  Evaluated as
+ *                                         ||L^-1 a||^2 with the Cholesky factor R_L = L L^H.  If the factorisation meets
+ *                                         a pivot that is not > 0 (NaN included), every P[k] of that window is NaN: the
+ *                                         window reports no peak, (0, 0, bin -1), and its spectrum row is NaN (as a NaN
+ *                                         window under MUSIC).
+ * For one source, R = p a0 a0^H + s2 I with ||a0||^2 = M, both give P(theta0) = p + (s2 + delta) / M (delta = 0 for
+ * Bartlett): their levels are power estimates.
+ * Unchanged: the peak rules, the float casts, levels = (float)P at the peak, the spectrum / P64 outputs and the bins,
+ * now of the chosen estimator's P; n (1 <= n < m) is the number of peak slots.  Under MDL / AIC the eigensolver runs
+ * only to count: the peak rule fills d slots of the estimator's spectrum, which does not depend on d.
+ * Refinement (MUSIC_B200_REFINE_NEWTON, geometric tables only) works for all three, with the 1-D bracket and accept
+ * rule and the az-el projected Newton steps of music_b200_set_refine, on:
+ *   MVDR      D(t) = a(t)^H R_L^-1 a(t) (minimised), level = (float)(1 / D(t*));
+ *   BARTLETT  F(t) = -B(t), B(t) = a(t)^H R a(t) (B maximised): the 1-D bracket condition is B'(lo) > 0 > B'(hi), a step
+ *             is accepted iff B(t*) >= B(t_b), level = (float)(B(t*) / M^2) (||a(t)||^2 = M for the analytic a).
+ * BARTLETT and MVDR run the unfused kernels: covariance, [eigensolver + source count only under MDL / AIC or when
+ * process_device_ex asks for the eigenvalues], [MVDR: Cholesky preparation, timed in the eigensolver slot], the
+ * quadratic-form scan, then the peak rule / decode / refinement as for MUSIC.
+ * Returns EINVAL for an unknown estimator, loading not finite or < 0, loading != 0 for MUSIC or BARTLETT, and MVDR with
+ * loading == 0 when N <= m (R is singular).  Setting MUSIC (loading 0) again restores the default behaviour exactly.
+ * Applies to later process_*() calls (host, device, _ex, _counts, planar, sharded, az-el) and to every device of a
+ * multi-device handle.
+ */
+#define MUSIC_B200_ESTIMATOR_MUSIC 0
+#define MUSIC_B200_ESTIMATOR_MVDR 1
+#define MUSIC_B200_ESTIMATOR_BARTLETT 2
+int music_b200_set_estimator(music_b200 *h, int estimator, double loading);
+
+/*
  * Downstream reducers (extension, no reference counterpart): what a GUI-rate consumer such as the DOA
  * compass (/root/reference/python/doa_compass_control.py:102-108) or a plot sink
  * (/root/reference/python/plot_sink.py:38) needs from millions of windows per second.

@@ -58,6 +58,9 @@ public:
     /* extension: true = refine every peak off the grid on the exact spectrum of the geometry set by
      * set_array_geometry() (bins stay the grid bins); false = grid angles (default) */
     void set_refine(bool enable);
+    /* extension: 0 = MUSIC (default), 1 = MVDR / Capon with diagonal loading loading * tr(R) / m, 2 = Bartlett
+     * beamscan (loading must be 0 for 0 and 2) */
+    void set_estimator(int estimator, double loading);
 
     /* Integer peak-bin indices of the items produced by the last work() call, [items][n]
      * (not in the reference; -1 marks a slot the reference would leave at (0, 0)). */

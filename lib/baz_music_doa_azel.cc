@@ -101,6 +101,13 @@ void baz_music_doa_azel::set_refine(bool enable)
     if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa_azel: ") + music_b200_last_error(d_handle));
 }
 
+void baz_music_doa_azel::set_estimator(int estimator, double loading)
+{
+    gr::thread::scoped_lock guard(d_mutex);
+    const int rc = music_b200_set_estimator(d_handle, estimator, loading);
+    if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa_azel: ") + music_b200_last_error(d_handle));
+}
+
 int baz_music_doa_azel::work(int noutput_items, gr_vector_const_void_star &input_items, gr_vector_void_star &output_items)
 {
     if (noutput_items <= 0) return 0;

@@ -51,6 +51,8 @@ public:
     void set_source_rule(int rule);
     /* true = refine every peak off the grid on the exact spectrum of the geometry (bins stay the grid bins) */
     void set_refine(bool enable);
+    /* 0 = MUSIC (default), 1 = MVDR with diagonal loading loading * tr(R) / m, 2 = Bartlett (loading 0 for 0 and 2) */
+    void set_estimator(int estimator, double loading);
 
     /* flat peak bins b = i * n_az + k of the items produced by the last work() call, [items][n] (-1: unfilled slot) */
     const std::vector<int> &last_bins() const { return d_bins; }
