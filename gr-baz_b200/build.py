@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(CSRC, "libmusic_b200.so")
 SOURCES = ["music_b200.cu"]
-DEPS = ["music_b200.cu", "music_kernels.cuh", "music_fused.cuh", "music_eig4p.cuh", "music_covn.cuh", "music_fused8.cuh", "music_steer.cuh", "music_planar.cuh", "music_reduce.cuh", "music_sources.cuh", "music_refine.cuh", "music_azel.cuh", "music_estimators.cuh", os.path.join("..", "..", "include", "music_b200.h")]
+DEPS = ["music_b200.cu", "music_kernels.cuh", "music_fused.cuh", "music_eig4p.cuh", "music_covn.cuh", "music_fused8.cuh", "music_steer.cuh", "music_planar.cuh", "music_reduce.cuh", "music_sources.cuh", "music_refine.cuh", "music_azel.cuh", "music_estimators.cuh", "music_roots.cuh", os.path.join("..", "..", "include", "music_b200.h")]
 
 NVCC_FLAGS = [
     "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",

@@ -31,6 +31,7 @@
 #include "music_refine.cuh"
 #include "music_azel.cuh"
 #include "music_estimators.cuh"
+#include "music_roots.cuh"
 
 using namespace music;
 
@@ -47,6 +48,7 @@ struct DeviceTable {
     bool geometric = false;       // built by set_geometry() from `geo` (set_table() tables are not)
     RefineGeom geo = {};          // element positions and wavelength of a geometric table (peak refinement)
     AzelGeom ageo = {};           // the same for an az-el handle (music_b200_create_azel): [M][x, y, z] and the grid
+    UlaGeom ula = {};             // whether `geo` is a uniform linear array the root mode accepts, and its p_0 and step
 };
 
 struct Workspace {
@@ -196,6 +198,29 @@ int upload_table(music_b200 *h, int slot, const float *table_c64, cudaStream_t s
     return finish_table(h, slot, st);
 }
 
+// The root mode's ULA condition (include/music_b200.h) on positions [M][x, y]: s = (p_{M-1} - p_0) / (M - 1), |s| > 0,
+// every element within 1e-6 |s| of p_0 + m s, |s| <= (lambda / 2)(1 + 1e-12).
+UlaGeom ula_geometry(const double *pos, int M, double lambda)
+{
+    UlaGeom u = {};
+    u.p0[0] = pos[0];
+    u.p0[1] = pos[1];
+    u.s[0] = (pos[2 * (M - 1)] - pos[0]) / (M - 1);
+    u.s[1] = (pos[2 * (M - 1) + 1] - pos[1]) / (M - 1);
+    const double sa = std::hypot(u.s[0], u.s[1]);
+    double dev = 0.0;
+    for (int m = 0; m < M; ++m)
+        dev = std::max(dev, std::hypot(pos[2 * m] - (u.p0[0] + m * u.s[0]), pos[2 * m + 1] - (u.p0[1] + m * u.s[1])));
+    u.ula = sa > 0.0 && dev <= 1e-6 * sa && sa <= 0.5 * lambda * (1.0 + 1e-12);
+    return u;
+}
+
+bool roots_table(const music_b200 *h)
+{
+    const DeviceTable &t = h->table[h->cur_table];
+    return t.geometric && t.ula.ula;
+}
+
 // Steering table built on the device from the element positions (music_steer.cuh), then patched at the
 // few entries whose float32 rounding could depend on the libm in use.
 int build_table(music_b200 *h, int slot, const double *pos_xy, double lambda, cudaStream_t st)
@@ -245,6 +270,7 @@ int build_table(music_b200 *h, int slot, const double *pos_xy, double lambda, cu
     t.geometric = true;
     for (int i = 0; i < 2 * M; ++i) t.geo.pos[i] = pos_xy[i];
     t.geo.lambda = lambda;
+    t.ula = ula_geometry(pos_xy, M, lambda);
     return MUSIC_B200_OK;
 }
 
@@ -579,7 +605,8 @@ int launch_eig_scan(music_b200 *h, const Workspace &ws, uint32_t W, const PeakOu
     }
     if (tev) cudaEventRecord(tev[2], st);
     const bool local = h->peak_mode == MUSIC_B200_PEAKS_LOCAL_MAXIMA;
-    const bool argmax = (h->n == 1) && !local;
+    const bool roots = h->peak_mode == MUSIC_B200_PEAKS_ROOTS;
+    const bool argmax = (h->n == 1) && !local && !roots;
     const bool need_p64 = !argmax || d_P64_out != nullptr;
     double *p64 = d_P64_out ? d_P64_out : ws.P64;
     const bool fast = argmax && !need_p64 && !d_spec && (M == 4 || M == 8 || M == 16);
@@ -591,6 +618,16 @@ int launch_eig_scan(music_b200 *h, const Workspace &ws, uint32_t W, const PeakOu
         case 8: launch_scan_quad<8>(h, est, q, soa, W, argmax, need_p64, spec, po, d_spec, p64, cnt, st); break;
         case 16: launch_scan_quad<16>(h, est, q, soa, W, argmax, need_p64, spec, po, d_spec, p64, cnt, st); break;
         default: launch_scan_quad<0>(h, est, q, soa, W, argmax, need_p64, spec, po, d_spec, p64, cnt, st); break;
+        }
+    } else if (roots) {
+        // the grid spectrum only when the caller asked for it; the angles come from the root kernel below
+        if (d_spec || d_P64_out) {
+            switch (M) {
+            case 4: launch_scan<4>(h, ws, soa, W, false, true, d_spec != nullptr, po, d_spec, p64, cnt, st); break;
+            case 8: launch_scan<8>(h, ws, soa, W, false, true, d_spec != nullptr, po, d_spec, p64, cnt, st); break;
+            case 16: launch_scan<16>(h, ws, soa, W, false, true, d_spec != nullptr, po, d_spec, p64, cnt, st); break;
+            default: launch_scan<0>(h, ws, soa, W, false, true, d_spec != nullptr, po, d_spec, p64, cnt, st); break;
+            }
         }
     } else if (fast) {
         const int grid = (W + SCAN_B - 1) / SCAN_B;
@@ -607,7 +644,11 @@ int launch_eig_scan(music_b200 *h, const Workspace &ws, uint32_t W, const PeakOu
         }
     }
     if (tev) cudaEventRecord(tev[3], st);
-    if (!argmax) {
+    if (roots) {
+        roots_kernel<<<(W + ROOTS_WARPS - 1) / ROOTS_WARPS, ROOTS_WARPS * 32, 0, st>>>(ws.Vt, cnt, M, (int)h->n, (int)h->K, (int)W, tb.geo,
+                                                                                  tb.ula, po);
+        h->launches++;
+    } else if (!argmax) {
         if (local && h->azel)
             topn_local2d_kernel<<<W, AZEL_LM_THREADS, 0, st>>>(p64, (int)h->n, h->grid.n_az, h->grid.n_el, (int)h->peak_excl, po, cnt);
         else if (local) topn_local_kernel<<<(W + 7) / 8, 256, 0, st>>>(p64, (int)h->n, (int)h->K, (int)W, (int)h->peak_excl, po, cnt);
@@ -675,6 +716,10 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, float *d
     if (refine && !h->table[h->cur_table].geometric)
         return fail(h, MUSIC_B200_EINVAL, "peak refinement needs a table built by music_b200_set_geometry(); the current one came from "
                                           "set_table() (call set_geometry(), or set_refine(OFF))");
+    const bool roots = h->peak_mode == MUSIC_B200_PEAKS_ROOTS;
+    if (roots && !roots_table(h))
+        return fail(h, MUSIC_B200_EINVAL, "the root peak mode needs a table built by music_b200_set_geometry() from a uniform linear "
+                                          "array with spacing <= lambda / 2 (call set_geometry(), or another peak mode)");
     if (fixed_n && d_counts) {
         fill_counts_kernel<<<(nwindows + 255) / 256, 256, 0, st>>>(d_counts, (int)h->n, (int)nwindows);
         h->launches++;
@@ -687,10 +732,11 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, float *d
         for (uint32_t r = 0; r < h->m; ++r) planar_fusable = planar_fusable && (reinterpret_cast<uintptr_t>(planar->p[r]) & 15u) == 0;
     }
     const bool local_peaks = h->peak_mode == MUSIC_B200_PEAKS_LOCAL_MAXIMA;
+    const bool top_bins = h->peak_mode == MUSIC_B200_PEAKS_TOP_BINS;
     const bool music_est = h->estimator == MUSIC_B200_ESTIMATOR_MUSIC;
     // the fused kernels find the principal eigenvector only, not every eigenvalue a source count needs nor the noise
     // eigenvectors the peak refinement needs; they compute the MUSIC spectrum only
-    if ((!planar || planar_fusable) && h->fused && !h->azel && music_est && fixed_n && !refine && !local_peaks && h->m == 4 && h->n == 1 && (!d_spec || h->fused_spec) && !d_P64 && !d_R && !d_ev) {
+    if ((!planar || planar_fusable) && h->fused && !h->azel && music_est && fixed_n && !refine && top_bins && h->m == 4 && h->n == 1 && (!d_spec || h->fused_spec) && !d_P64 && !d_R && !d_ev) {
         // whole call in one persistent launch (music_fused.cuh); no workspace involved
         cudaEvent_t *tev = timing_events(h);
         if (tev) cudaEventRecord(tev[0], st);
@@ -732,7 +778,7 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, float *d
         CU(h, cudaGetLastError());
         return MUSIC_B200_OK;
     }
-    if (!planar && h->fused && !h->azel && music_est && fixed_n && !refine && !local_peaks && h->m == 8 && h->n == 1 && !d_spec && !d_P64 && !d_R && !d_ev && h->N >= 128 &&
+    if (!planar && h->fused && !h->azel && music_est && fixed_n && !refine && top_bins && h->m == 8 && h->n == 1 && !d_spec && !d_P64 && !d_R && !d_ev && h->N >= 128 &&
         h->N % 2 == 0 && encode_tiled_fn()) {
         // M = 8: whole call in one persistent launch (music_fused8.cuh); R and the eigenvectors stay in shared memory
         CUtensorMap tm;
@@ -755,7 +801,8 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, float *d
             return MUSIC_B200_OK;
         }
     }
-    const bool internal_p64 = (h->n != 1 || local_peaks) && !d_P64;
+    // the root mode writes P64 only for the spectrum; the peak rules read it whenever they are not the n = 1 arg-max
+    const bool internal_p64 = (roots ? d_spec != nullptr : (h->n != 1 || local_peaks)) && !d_P64;
     const uint32_t sub = std::min((nwindows + SCAN_B - 1) / SCAN_B * SCAN_B, max_sub_windows(h, internal_p64));
     Workspace &ws = h->ws[slot];
     int rc = ensure_slot(h, ws, sub, internal_p64);
@@ -1309,13 +1356,23 @@ int music_b200_reduce_spectrum_host(music_b200 *h, const float *spectrum, uint32
 int music_b200_set_peak_mode(music_b200 *h, int mode, uint32_t exclusion_bins)
 {
     if (!h) return MUSIC_B200_EINVAL;
-    if (mode != MUSIC_B200_PEAKS_TOP_BINS && mode != MUSIC_B200_PEAKS_LOCAL_MAXIMA) return fail(h, MUSIC_B200_EINVAL, "unknown peak mode %d", mode);
+    if (mode != MUSIC_B200_PEAKS_TOP_BINS && mode != MUSIC_B200_PEAKS_LOCAL_MAXIMA && mode != MUSIC_B200_PEAKS_ROOTS)
+        return fail(h, MUSIC_B200_EINVAL, "unknown peak mode %d", mode);
     if (exclusion_bins >= h->K) return fail(h, MUSIC_B200_EINVAL, "exclusion_bins must be < resolution");
+    if (mode == MUSIC_B200_PEAKS_ROOTS) {
+        if (exclusion_bins != 0) return fail(h, MUSIC_B200_EINVAL, "the root peak mode takes exclusion_bins = 0");
+        if (h->azel) return fail(h, MUSIC_B200_EINVAL, "the root peak mode is not supported on an az-el handle");
+        if (h->estimator != MUSIC_B200_ESTIMATOR_MUSIC) return fail(h, MUSIC_B200_EINVAL, "the root peak mode needs the MUSIC estimator");
+        if (h->refine != MUSIC_B200_REFINE_OFF) return fail(h, MUSIC_B200_EINVAL, "the root peak mode needs refinement off");
+    }
     std::lock_guard<std::mutex> g(h->mutex);
     for (music_b200 *c : h->kids) {
         const int rc = music_b200_set_peak_mode(c, mode, exclusion_bins);
         if (rc) return fail(h, rc, "%s", music_b200_last_error(c));
     }
+    if (h->kids.empty() && mode == MUSIC_B200_PEAKS_ROOTS && !roots_table(h))
+        return fail(h, MUSIC_B200_EINVAL, "the root peak mode needs a table built by music_b200_set_geometry() from a uniform linear "
+                                          "array with spacing <= lambda / 2");
     h->peak_mode = mode;
     h->peak_excl = exclusion_bins;
     return MUSIC_B200_OK;
@@ -1467,6 +1524,8 @@ int music_b200_set_refine(music_b200 *h, int mode)
         const int rc = music_b200_set_refine(c, mode);
         if (rc) return fail(h, rc, "%s", music_b200_last_error(c));
     }
+    if (mode != MUSIC_B200_REFINE_OFF && h->peak_mode == MUSIC_B200_PEAKS_ROOTS)
+        return fail(h, MUSIC_B200_EINVAL, "peak refinement does not apply to the root peak mode");
     if (h->kids.empty() && mode != MUSIC_B200_REFINE_OFF && !h->table[h->cur_table].geometric)
         return fail(h, MUSIC_B200_EINVAL, "peak refinement needs a table built by music_b200_set_geometry(); the current one came from set_table()");
     h->refine = mode;
@@ -1481,6 +1540,8 @@ int music_b200_set_estimator(music_b200 *h, int estimator, double loading)
     if (!std::isfinite(loading) || loading < 0.0) return fail(h, MUSIC_B200_EINVAL, "loading must be finite and >= 0 (got %g)", loading);
     if (estimator != MUSIC_B200_ESTIMATOR_MVDR && loading != 0.0)
         return fail(h, MUSIC_B200_EINVAL, "diagonal loading applies to MVDR only (got %g)", loading);
+    if (estimator != MUSIC_B200_ESTIMATOR_MUSIC && h->peak_mode == MUSIC_B200_PEAKS_ROOTS)
+        return fail(h, MUSIC_B200_EINVAL, "the root peak mode needs the MUSIC estimator");
     if (estimator == MUSIC_B200_ESTIMATOR_MVDR && loading == 0.0 && h->N <= h->m)
         return fail(h, MUSIC_B200_EINVAL, "MVDR without diagonal loading needs more snapshots than antennas (N = %u, m = %u): R is singular",
                     h->N, h->m);

@@ -102,8 +102,11 @@ class music_doa(object):
     # -- extension (SURVEY.md section 8(f) rank 3): opt-in local-maximum peak rule --------------
     def set_peak_mode(self, mode="top_bins", exclusion_bins=0):
         """``"top_bins"`` (default) = the reference's rule (/root/reference/lib/baz_music_doa.cc:129-141);
-        ``"local_maxima"`` = the n largest circular local maxima more than ``exclusion_bins`` apart."""
-        modes = {"top_bins": 0, "local_maxima": 1}
+        ``"local_maxima"`` = the n largest circular local maxima more than ``exclusion_bins`` apart;
+        ``"roots"`` = root-MUSIC: gridless angles from the roots of the noise-subspace polynomial, for a uniform linear
+        array with spacing <= lambda / 2 installed with ``set_array_geometry`` (include/music_b200.h).  It needs
+        ``exclusion_bins`` = 0, the "music" estimator and refinement off."""
+        modes = {"top_bins": 0, "local_maxima": 1, "roots": 2}
         if mode not in modes:
             raise ValueError("mode must be one of %s" % sorted(modes))
         _capi.check(self._lib.music_b200_set_peak_mode(self._h, modes[mode], int(exclusion_bins)), self._h)

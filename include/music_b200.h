@@ -115,9 +115,42 @@ int music_b200_set_table(music_b200 *h, const float *table_c64);
  * largest circular local maxima (P[k] > P[k-1] and P[k] >= P[k+1], P[k] > 0), each more than
  * exclusion_bins away from every stronger peak taken; outputs in descending strength, unfilled slots
  * (0, 0, bin -1).  Applies to later process_*() calls.
+ *
+ * MUSIC_B200_PEAKS_ROOTS (extension, root-MUSIC): angles from the roots of the noise-subspace polynomial instead of a
+ * search over the table, for a uniform linear array.  Covariance, eigensolver, source rules and spectrum are unchanged.
+ *   ULA        the geometry set_geometry() recorded with the current table, p_0 .. p_{M-1}, s = (p_{M-1} - p_0) / (M - 1):
+ *              |s| > 0, max_m ||p_m - (p_0 + m s)|| <= 1e-6 |s| and |s| <= (lambda / 2)(1 + 1e-12) (either element order,
+ *              any origin and axis direction; a wider spacing maps a root to several directions).
+ *   polynomial G = the M - d noise eigenvectors the scan would use (d = n, or the MDL / AIC count), C = G G^H,
+ *              c_l = sum_{j - i = l} C_ij (l = -(M-1) .. M-1, c_{-l} = conj(c_l)), Q(z) = sum_l c_l z^(l + M - 1), so that
+ *              D(t) = sum_l c_l z0^l with z0 = exp(-j 2 pi (s . u(t)) / lambda), all fp64.  Each outermost pair
+ *              c_{+-l} that is exactly zero contributes a root at 0 and one at infinity.
+ *   roots      Aberth-Ehrlich iteration in fp64 (starting points on the unit circle, at most 100 steps).  Two roots that
+ *              are each other's nearest and closer than 1e-6 max(|z_a|, |z_b|) are one double root on the unit circle
+ *              (D >= 0 there, so a root on the circle has even multiplicity): both become their midpoint, with modulus
+ *              taken as 1, and the copy of the higher index sorts after every other root of modulus 1.
+ *   selection  sort the 2M - 2 roots by ascending modulus and keep the first M - 1 (one of each pair z, 1 / conj(z));
+ *              slots 0 .. d-1 take the d kept roots of largest modulus, in descending modulus, exact ties to the lower
+ *              angle.  A kept root at 0 has no direction: its slot stays unfilled.
+ *   angle      cpsi = clamp(-arg(z) lambda / (2 pi |s|), -1, 1), psi = acos(cpsi), alpha = atan2(s_y, s_x); the slot
+ *              reports t* = the smaller of alpha + psi and alpha - psi wrapped into [0, 360) degrees (the mirror the grid's
+ *              lower-bin tie rule picks: on an x-axis ULA [0, 180]); float cast and 360 -> 0 as in refinement.
+ *   outputs    level = (float)(1 / D(t*)), D the direct fp64 form of the refinement; bin = floor(t* K / 360 + 0.5) mod K.
+ *              Slots d .. n-1, windows with d = 0 and windows whose C or roots are not finite report (0, 0, bin -1).
+ *              Spectrum, P64, R, eigenvalues and counts are unchanged; the MUSIC grid spectrum is computed only when the
+ *              spectrum or P64 is requested (then by the unfused scan), otherwise no table scan runs at all.
+ * Caveats: near end-fire (psi -> 0 or 180 degrees) acos amplifies the root error; as |s| / lambda shrinks every root
+ * crowds towards z = 1 (a placeholder geometry such as 1 m elements at 1 Hz is meaningless here).
+ * ROOTS needs exclusion_bins = 0, estimator MUSIC and refinement OFF (set_peak_mode(ROOTS) under MVDR / Bartlett or
+ * NEWTON, and set_estimator(MVDR / BARTLETT) or set_refine(NEWTON) under ROOTS, return EINVAL), and a current table from
+ * set_geometry() of a ULA: set_peak_mode(ROOTS) returns EINVAL otherwise, and so does a process_*() call whose current
+ * table came from set_table() or from set_geometry() of another geometry (no fall-back to grid peaks).  Az-el handles
+ * return EINVAL.  It runs the unfused kernels: covariance, eigensolver (+ source count), [scan], then one root kernel
+ * per sub-batch, timed in the top-n slot of the stage timing.
  */
 #define MUSIC_B200_PEAKS_TOP_BINS 0
 #define MUSIC_B200_PEAKS_LOCAL_MAXIMA 1
+#define MUSIC_B200_PEAKS_ROOTS 2
 int music_b200_set_peak_mode(music_b200 *h, int mode, uint32_t exclusion_bins);
 
 /*

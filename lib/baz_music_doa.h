@@ -51,7 +51,8 @@ public:
     void set_array_response(const array_response_t &array_response);
     /* extension: device-side table build from element positions [m][x, y] (metres) and the wavelength */
     void set_array_geometry(const std::vector<std::vector<double> > &positions_xy, double wavelength);
-    /* extension: 0 = the reference's n largest bins (default), 1 = n largest local maxima > exclusion_bins apart */
+    /* extension: 0 = the reference's n largest bins (default), 1 = n largest local maxima > exclusion_bins apart,
+     * 2 = root-MUSIC on a uniform linear array set by set_array_geometry() (exclusion_bins must be 0) */
     void set_peak_mode(int mode, unsigned int exclusion_bins);
     /* extension: 0 = n sources in every window (default), 1 = MDL, 2 = AIC estimate of 0..n sources per window */
     void set_source_rule(int rule);
