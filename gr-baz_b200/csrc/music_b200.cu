@@ -45,6 +45,7 @@ struct DeviceTable {
     double *soa = nullptr;  // [ntiles][2M+1][TILE]
     unsigned char *fz = nullptr;  // fused kernel's tensor-core screen layout (music_fused.cuh, M = 4 only)
     float *na_max = nullptr;      // max ||a||^2 over the table rows (screen threshold)
+    bool screen_ok = true;        // the fused M = 4 kernel's fp32 screen bound holds for every row (screen_bounds_table)
     bool geometric = false;       // built by set_geometry() from `geo` (set_table() tables are not)
     RefineGeom geo = {};          // element positions and wavelength of a geometric table (peak refinement)
     AzelGeom ageo = {};           // the same for an az-el handle (music_b200_create_azel): [M][x, y, z] and the grid
@@ -191,9 +192,32 @@ int finish_table(music_b200 *h, int slot, cudaStream_t st)
     return MUSIC_B200_OK;
 }
 
+// Whether the fused M = 4 kernel's tensor-core screen can bound a [K][4] complex64 table (music_fused.cuh, "Screen
+// error bound"): the bound is relative to each row's fl32(||a||^2), so that value and every fp32 quantity of the screen
+// must be finite and far from the subnormal range.  Rows of zeros are exact in the screen (d~ = 0) and pass.  A table
+// that fails (a calibrated table scaled near the float32 limits) runs on the kernel's all-fp64 drain instead: same
+// results, without the tensor-core passes.
+bool screen_bounds_table(const float *tab, uint32_t K)
+{
+    const double lo = 0x1p-100, hi = 0x1p100;
+    for (uint32_t k = 0; k < K; ++k) {
+        const float *row = tab + (size_t)k * 8;
+        double na = 0.0;
+        bool zero = true;
+        for (int i = 0; i < 4; ++i) {
+            na = std::fma((double)row[2 * i], (double)row[2 * i], std::fma((double)row[2 * i + 1], (double)row[2 * i + 1], na));
+            zero = zero && row[2 * i] == 0.f && row[2 * i + 1] == 0.f;
+        }
+        const double f = (double)(float)na;
+        if (!zero && !(f >= lo && f <= hi)) return false;  // NaN fails too
+    }
+    return true;
+}
+
 int upload_table(music_b200 *h, int slot, const float *table_c64, cudaStream_t st)
 {
     h->table[slot].geometric = false;
+    h->table[slot].screen_ok = h->m != 4 || screen_bounds_table(table_c64, h->K);
     CU(h, cudaMemcpyAsync(h->table[slot].c64, table_c64, (size_t)h->K * h->m * 2 * sizeof(float), cudaMemcpyHostToDevice, st));
     return finish_table(h, slot, st);
 }
@@ -228,6 +252,7 @@ int build_table(music_b200 *h, int slot, const double *pos_xy, double lambda, cu
     DeviceTable &t = h->table[slot];
     const int K = (int)h->K, M = (int)h->m;
     t.geometric = false;
+    t.screen_ok = true;  // unit-modulus rows: ||a||^2 = M
     if (!h->steer_pos) {
         CU(h, cudaMalloc(&h->steer_pos, sizeof(double) * 2 * MUSIC_B200_MAX_M));
         CU(h, cudaMalloc(&h->steer_count, sizeof(unsigned)));
@@ -762,15 +787,16 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, float *d
         long long *trace = tr ? h->fused_trace + (size_t)(h->trace_seq++ % FZ_TRACE_LAUNCHES) * FZ_TRACE_CTAS * FZ_TRACE : nullptr;
         const unsigned char *fz = tb.fz;
         const float *c64 = tb.c64, *na_max = tb.na_max;
+        const int mma_fin = tb.screen_ok ? h->mma_fin_max : -1;  // a table the screen cannot bound: fp64 drain only
         cudaError_t le;
         if (planar) {
             auto kern = tr ? music4_fused_kernel<true, true> : music4_fused_kernel<true, false>;
             le = cudaLaunchKernelEx(&lc, kern, (const float *)nullptr, *planar, 0ull, (unsigned)hop, fz, c64, na_max, W_i, N_i, K_i, po, ctr,
-                                    trace, h->eig_mode, gf, h->mma_fin_max, d_spec);
+                                    trace, h->eig_mode, gf, mma_fin, d_spec);
         } else {
             auto kern = tr ? music4_fused_kernel<false, true> : music4_fused_kernel<false, false>;
             le = cudaLaunchKernelEx(&lc, kern, d_in, PlanarStreams{}, 0ull, 0u, fz, c64, na_max, W_i, N_i, K_i, po, ctr, trace,
-                                    h->eig_mode, gf, h->mma_fin_max, d_spec);
+                                    h->eig_mode, gf, mma_fin, d_spec);
         }
         CU(h, le);
         h->launches++;

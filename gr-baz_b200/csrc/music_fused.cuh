@@ -47,6 +47,8 @@
 // hence ||c~|^2 - |c|^2| <= 2^-16.8||a||^2, plus 2^-22 for the fp32 squares and the subtraction from
 // fl32(||a||^2).  FZ_B = 2^-15 leaves > 3x margin over this (already pessimistic) bound; a CPU emulation of the
 // screen with truncating fp32 accumulation measures <= 5e-7 ||a||^2, 60x below FZ_B (tests/test_screen_bound.py).
+// The bound assumes fp32 never overflows or goes subnormal: a table with a non-zero row whose fl32(||a||^2) lies outside
+// [2^-100, 2^100] (screen_bounds_table in music_b200.cu) runs every window on the fp64 drain instead (tests/test_gpu_tables.py).
 //
 // INSTRUCTION FOOTPRINT.  Sixteen warps in four roles (two CTAs) share one SM's instruction caches (L0 ~6 KB per sub-partition,
 // L1.5 32 KB per SM; beyond that instructions come from the L2, which this kernel keeps saturated with the input stream).

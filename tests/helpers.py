@@ -180,6 +180,90 @@ def assert_bins_equal_up_to_exact_ties(got, ref):
     return len(bad)
 
 
+# ---- arbitrary array-response tables (set_array_response): tests/test_gpu_tables.py, tests/test_ref_tables.py --------
+def planar_table(m, K, seed):
+    """[K][m] complex64 steering table of a random planar array (positions in wavelengths), theta_k = k * 360 / K"""
+    pos = np.random.default_rng(seed).uniform(-1.5, 1.5, (m, 2))
+    th = np.arange(K) * (2.0 * np.pi / K)
+    return np.exp(-2j * np.pi * (np.outer(np.cos(th), pos[:, 0]) + np.outer(np.sin(th), pos[:, 1]))).astype(np.complex64)
+
+
+def calibrated_table(table, seed):
+    """a geometric table as a calibration would leave it: a fixed gain (0.5 .. 2) and phase error per element, a
+    power-of-two factor 2^j per row (j in [-20, 20]) and a small complex perturbation of every entry"""
+    rng = np.random.default_rng(seed)
+    K, m = table.shape
+    gain = rng.uniform(0.5, 2.0, m) * np.exp(1j * rng.uniform(-0.3, 0.3, m))
+    row = 2.0 ** rng.integers(-20, 21, K)
+    eps = 1e-3 * (rng.standard_normal((K, m)) + 1j * rng.standard_normal((K, m)))
+    return ((table.astype(np.complex128) * gain[None, :] + eps) * row[:, None]).astype(np.complex64)
+
+
+def random_table(m, K, seed):
+    """i.i.d. complex Gaussian rows: a spectrum with a local maximum at about every third bin"""
+    rng = np.random.default_rng(seed)
+    return ((rng.standard_normal((K, m)) + 1j * rng.standard_normal((K, m))) / np.sqrt(2.0)).astype(np.complex64)
+
+
+def source_windows(rng, vectors, m, N, amp=5.0):
+    """one window per entry of `vectors` (each None or a list of complex (m,) source directions): unit complex noise
+    plus sources of amplitude `amp` along the directions, each normalised to ||a||^2 = m; (W, N * m) complex64"""
+    W = len(vectors)
+    x = (rng.standard_normal((W, N, m)) + 1j * rng.standard_normal((W, N, m))) / np.sqrt(2.0)
+    for w, vs in enumerate(vectors):
+        for a in vs or []:
+            a = np.asarray(a, np.complex128)
+            a = a * np.sqrt(m) / np.linalg.norm(a)
+            x[w] += amp * a[None, :] * (rng.standard_normal((N, 1)) + 1j * rng.standard_normal((N, 1)))
+    return x.reshape(W, N * m).astype(np.complex64)
+
+
+# reference outputs on these tables: tests/golden/reference/tables.npz (make_reference_tables_golden.py)
+REFERENCE_TABLES = os.path.join(GOLDEN, "reference", "tables.npz")
+TABLE_ZERO_ROWS = (5, 200, 201)
+TABLE_DUPLICATES = ((37, 100), (0, 399))  # (row copied, row overwritten)
+
+
+def table_golden_cases():
+    """(key, m, n, table, x) of the small batches stored with the reference's outputs: M = 4, K = 400, tables scaled by
+    2^63 and 2^-70, calibrated, with duplicated rows (a strong source along the duplicated row) and with zero rows"""
+    m, K, N, W = 4, 400, 64, 4
+    base = planar_table(m, K, 4040)
+    rng = np.random.default_rng(4041)
+    dup = base.copy()
+    for src, dst in TABLE_DUPLICATES:
+        dup[dst] = dup[src]
+    zero = base.copy()
+    zero[list(TABLE_ZERO_ROWS)] = 0
+    tables = {"scaled63": (base.astype(np.complex128) * 2.0 ** 63).astype(np.complex64),
+              "scaled-70": (base.astype(np.complex128) * 2.0 ** -70).astype(np.complex64),
+              "calibrated": calibrated_table(base, 4042), "duplicate": dup, "zero": zero}
+    for name, t in tables.items():
+        srcs = [[t[37]], [t[37], t[250]], [t[0]], None] if name == "duplicate" else \
+               [[base[int(k)]] for k in rng.integers(0, K, W - 1)] + [None]
+        x = source_windows(rng, srcs, m, N, amp=20.0 if name == "duplicate" else 5.0)
+        for n in (1, 2):
+            yield "%s_n%d" % (name, n), m, n, t, x
+
+
+def table_reference_outputs(key, x, table):
+    """the reference's angles, levels and full spectrum of table_golden_cases() entry `key`, after checking that x and
+    the table are the ones it was computed from"""
+    g = np.load(REFERENCE_TABLES)
+    assert str(g[key + "/in_sha256"]) == sha256(x), key
+    assert str(g[key + "/table_sha256"]) == sha256(table), key
+    return {f: g[key + "/" + f] for f in ("angles", "levels", "spectrum")}
+
+
+def assert_float32_close(got, ref, rtol, ctx):
+    """non-finite values (NaN included) and zeros bit-equal, the rest within rtol"""
+    got, ref = np.asarray(got, np.float64), np.asarray(ref, np.float64)
+    exact = ~np.isfinite(ref) | (ref == 0)
+    assert np.array_equal(got[exact], ref[exact], equal_nan=True), ctx
+    if np.any(~exact):
+        assert rel_err(got[~exact], ref[~exact]) <= rtol, ctx
+
+
 _reference_golden = None
 
 
