@@ -33,6 +33,7 @@
 #include "music_azel.cuh"
 #include "music_estimators.cuh"
 #include "music_roots.cuh"
+#include "music_esprit.cuh"
 
 using namespace music;
 
@@ -303,12 +304,15 @@ UlaGeom ula_geometry(const double *pos, int M, double lambda)
     return u;
 }
 
+// The peak modes that take their angles from the ULA geometry instead of the table: ROOTS and ESPRIT
+bool gridless_ula(int peak) { return peak == MUSIC_B200_PEAKS_ROOTS || peak == MUSIC_B200_PEAKS_ESPRIT; }
+
 // Whether handle h can run with modes p; if not, records why and returns EINVAL.  With a table t, also whether p can run
-// on it: the root peak mode needs a ULA geometry, the refinement a geometric table.  Tables are checked on handles that
+// on it: the gridless ULA peak modes need a ULA geometry, the refinement a geometric table.  Tables are checked on handles that
 // hold one (single-device handles, and the children of a multi-device handle).
 int check_modes(music_b200 *h, const Modes &p, const DeviceTable *t)
 {
-    if (p.peak != MUSIC_B200_PEAKS_TOP_BINS && p.peak != MUSIC_B200_PEAKS_LOCAL_MAXIMA && p.peak != MUSIC_B200_PEAKS_ROOTS)
+    if (p.peak != MUSIC_B200_PEAKS_TOP_BINS && p.peak != MUSIC_B200_PEAKS_LOCAL_MAXIMA && !gridless_ula(p.peak))
         return fail(h, MUSIC_B200_EINVAL, "unknown peak mode %d", p.peak);
     if (p.excl >= h->K) return fail(h, MUSIC_B200_EINVAL, "exclusion_bins must be < resolution");
     if (p.refine != MUSIC_B200_REFINE_OFF && p.refine != MUSIC_B200_REFINE_NEWTON) return fail(h, MUSIC_B200_EINVAL, "unknown refine mode %d", p.refine);
@@ -320,14 +324,15 @@ int check_modes(music_b200 *h, const Modes &p, const DeviceTable *t)
     if (p.est == MUSIC_B200_ESTIMATOR_MVDR && p.loading == 0.0 && h->N <= h->m)
         return fail(h, MUSIC_B200_EINVAL, "MVDR without diagonal loading needs more snapshots than antennas (N = %u, m = %u): R is singular",
                     h->N, h->m);
-    if (p.peak == MUSIC_B200_PEAKS_ROOTS) {
-        if (p.excl != 0) return fail(h, MUSIC_B200_EINVAL, "the root peak mode takes exclusion_bins = 0");
-        if (h->azel) return fail(h, MUSIC_B200_EINVAL, "the root peak mode is not supported on an az-el handle");
-        if (p.est != MUSIC_B200_ESTIMATOR_MUSIC) return fail(h, MUSIC_B200_EINVAL, "the root peak mode needs the MUSIC estimator");
-        if (p.refine != MUSIC_B200_REFINE_OFF) return fail(h, MUSIC_B200_EINVAL, "the root peak mode needs refinement off");
+    if (gridless_ula(p.peak)) {
+        const char *name = p.peak == MUSIC_B200_PEAKS_ROOTS ? "root" : "ESPRIT";
+        if (p.excl != 0) return fail(h, MUSIC_B200_EINVAL, "the %s peak mode takes exclusion_bins = 0", name);
+        if (h->azel) return fail(h, MUSIC_B200_EINVAL, "the %s peak mode is not supported on an az-el handle", name);
+        if (p.est != MUSIC_B200_ESTIMATOR_MUSIC) return fail(h, MUSIC_B200_EINVAL, "the %s peak mode needs the MUSIC estimator", name);
+        if (p.refine != MUSIC_B200_REFINE_OFF) return fail(h, MUSIC_B200_EINVAL, "the %s peak mode needs refinement off", name);
         if (t && !(t->geometric && t->ula.ula))
-            return fail(h, MUSIC_B200_EINVAL, "the root peak mode needs a table built by music_b200_set_geometry() from a uniform linear "
-                                              "array with spacing <= lambda / 2 (call set_geometry(), or another peak mode)");
+            return fail(h, MUSIC_B200_EINVAL, "the %s peak mode needs a table built by music_b200_set_geometry() from a uniform linear "
+                                              "array with spacing <= lambda / 2 (call set_geometry(), or another peak mode)", name);
     }
     if (t && p.refine != MUSIC_B200_REFINE_OFF && !t->geometric)
         return fail(h, MUSIC_B200_EINVAL, "peak refinement needs a table built by music_b200_set_geometry(); the current one came from "
@@ -459,7 +464,7 @@ constexpr unsigned CTR_RING = 256;  // ticket-counter pairs per slot (see ticket
 
 enum class Path { Unfused, Fused4, Fused8 };
 enum class Scan { None, Peak1, Music, Quad };              // scan_peak1_kernel, scan_kernel, scan_quad_kernel
-enum class Peaks { None, TopN, Local, Local2D, Roots };     // topn, topn_local, topn_local2d, roots kernels
+enum class Peaks { None, TopN, Local, Local2D, Roots, Esprit };  // topn, topn_local, topn_local2d, roots, esprit kernels
 
 // What one call runs, from the handle's modes, the requested outputs and the input form (plan_call).
 struct Plan {
@@ -480,7 +485,7 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
     const bool fixed_n = h->source_rule == MUSIC_B200_SOURCES_FIXED;
     const bool music_est = md.est == MUSIC_B200_ESTIMATOR_MUSIC;
     const bool local = md.peak == MUSIC_B200_PEAKS_LOCAL_MAXIMA;
-    const bool roots = md.peak == MUSIC_B200_PEAKS_ROOTS;
+    const bool gridless = gridless_ula(md.peak);
     Plan p;
     // The fused kernels find the principal eigenvector only, not every eigenvalue a source count needs nor the noise
     // eigenvectors the peak refinement needs; they compute the MUSIC spectrum only.  Planar streams can take the M = 4
@@ -497,13 +502,13 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
     p.count = !fixed_n;
     p.mvdr = md.est == MUSIC_B200_ESTIMATOR_MVDR;
     p.est = md.est;
-    p.argmax = h->n == 1 && !local && !roots;
+    p.argmax = h->n == 1 && !local && !gridless;
     p.spec = o.spec != nullptr;
     if (!music_est) {
         p.scan = Scan::Quad;
         p.p64 = !p.argmax || o.P64;
-    } else if (roots) {
-        // the grid spectrum only when the caller asked for it; the angles come from the root kernel
+    } else if (gridless) {
+        // the grid spectrum only when the caller asked for it; the angles come from the root or ESPRIT kernel
         p.scan = o.spec || o.P64 ? Scan::Music : Scan::None;
         p.p64 = p.scan == Scan::Music;
     } else if (p.argmax && !o.P64 && !o.spec && (h->m == 4 || h->m == 8 || h->m == 16)) {
@@ -512,7 +517,7 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
         p.scan = Scan::Music;
         p.p64 = !p.argmax || o.P64;
     }
-    if (roots) p.peaks = Peaks::Roots;
+    if (gridless) p.peaks = md.peak == MUSIC_B200_PEAKS_ROOTS ? Peaks::Roots : Peaks::Esprit;
     else if (!p.argmax) p.peaks = local && h->azel ? Peaks::Local2D : local ? Peaks::Local : Peaks::TopN;
     p.decode = h->azel;
     p.refine = md.refine != MUSIC_B200_REFINE_OFF;
@@ -811,6 +816,10 @@ int launch_eig_scan(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t 
     case Peaks::Roots:
         roots_kernel<<<(W + ROOTS_WARPS - 1) / ROOTS_WARPS, ROOTS_WARPS * 32, 0, st>>>(ws.Vt, cnt, M, (int)h->n, (int)h->K, (int)W, tb.geo,
                                                                                   tb.ula, po);
+        break;
+    case Peaks::Esprit:
+        esprit_kernel<<<(W + ESPRIT_WARPS - 1) / ESPRIT_WARPS, ESPRIT_WARPS * 32, 0, st>>>(ws.Vt, cnt, M, (int)h->n, (int)h->K, (int)W,
+                                                                                        tb.geo, tb.ula, po);
         break;
     case Peaks::Local2D: topn_local2d_kernel<<<W, AZEL_LM_THREADS, 0, st>>>(p64, (int)h->n, h->grid.n_az, h->grid.n_el, excl, po, cnt); break;
     case Peaks::Local: topn_local_kernel<<<(W + 7) / 8, 256, 0, st>>>(p64, (int)h->n, (int)h->K, (int)W, excl, po, cnt); break;
@@ -1564,7 +1573,7 @@ int music_b200_set_peak_mode(music_b200 *h, int mode, uint32_t exclusion_bins)
     Modes p = h->modes;
     p.peak = mode;
     p.excl = exclusion_bins;
-    if (const int rc = check_modes(h, p, mode == MUSIC_B200_PEAKS_ROOTS ? own_table(h) : nullptr)) return rc;
+    if (const int rc = check_modes(h, p, gridless_ula(mode) ? own_table(h) : nullptr)) return rc;
     if (const int rc = for_each_child(h, [&](music_b200 *c) { return music_b200_set_peak_mode(c, mode, exclusion_bins); })) return rc;
     h->modes = p;
     return MUSIC_B200_OK;

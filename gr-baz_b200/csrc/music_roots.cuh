@@ -39,6 +39,32 @@ __device__ __forceinline__ double2 shfl2(double2 v, int src)
     return make_double2(__shfl_sync(0xffffffffu, v.x, src), __shfl_sync(0xffffffffu, v.y, src));
 }
 
+// The direction of z0 = z on the ULA (shared by the gridless ULA modes, ROOTS and ESPRIT): cos(t - alpha) =
+// -arg(z) lambda / (2 pi |s|); the lower of alpha +- psi in [0, 360) degrees
+__device__ __forceinline__ double ula_direction(double2 z, const RefineGeom &geo, const UlaGeom &ula)
+{
+    const double sabs = hypot(ula.s[0], ula.s[1]);
+    double cpsi = -atan2(z.y, z.x) * geo.lambda / (STEER_TWO_PI * sabs);
+    cpsi = fmin(1.0, fmax(-1.0, cpsi));
+    const double psi = acos(cpsi), alpha = atan2(ula.s[1], ula.s[0]);
+    double a1 = fmod((alpha + psi) * REFINE_RAD2DEG, 360.0), a2 = fmod((alpha - psi) * REFINE_RAD2DEG, 360.0);
+    if (a1 < 0.0) a1 += 360.0;
+    if (a2 < 0.0) a2 += 360.0;
+    return fmin(a1, a2);
+}
+
+// A filled slot of a gridless ULA mode: the angle t* (float cast, 360 -> 0), level 1 / D(t*) and the nearest grid bin
+__device__ __forceinline__ void ula_store_slot(const PeakOut &out, size_t o, double tdeg, double D, int K)
+{
+    float ang = (float)tdeg;
+    if (ang >= 360.0f || ang == 0.0f) ang = 0.0f;
+    out.angles[o] = ang;
+    if (out.levels) out.levels[o] = (float)(1.0 / D);
+    int b = (int)floor(tdeg * (double)K / 360.0 + 0.5);
+    if (b >= K) b -= K;
+    peak_store_bin(out, o, b);
+}
+
 // Vt: per window M * M complex doubles, eigenvector j contiguous, ascending eigenvalues; counts (may be null): the
 // per-window source count d (else d = n); the noise subspace is eigenvectors 0 .. M - d - 1, as in the scan.
 __global__ void __launch_bounds__(ROOTS_WARPS * 32) roots_kernel(const double *__restrict__ Vt, const int32_t *__restrict__ counts,
@@ -131,15 +157,7 @@ __global__ void __launch_bounds__(ROOTS_WARPS * 32) roots_kernel(const double *_
         }
     }
 
-    // direction of the root: cos(t - alpha) = -arg(z) lambda / (2 pi |s|); report the lower of alpha +- psi in [0, 360)
-    const double sabs = hypot(ula.s[0], ula.s[1]);
-    double cpsi = -atan2(z.y, z.x) * geo.lambda / (STEER_TWO_PI * sabs);
-    cpsi = fmin(1.0, fmax(-1.0, cpsi));
-    const double psi = acos(cpsi), alpha = atan2(ula.s[1], ula.s[0]);
-    double a1 = fmod((alpha + psi) * REFINE_RAD2DEG, 360.0), a2 = fmod((alpha - psi) * REFINE_RAD2DEG, 360.0);
-    if (a1 < 0.0) a1 += 360.0;
-    if (a2 < 0.0) a2 += 360.0;
-    const double tdeg = fmin(a1, a2);
+    const double tdeg = ula_direction(z, geo, ula);
 
     // keep the M - 1 - t inside roots (ascending modulus, a double root's second copy after every other root of equal
     // modulus, then lane); fill slots in descending modulus, ties to the lower angle
@@ -161,13 +179,7 @@ __global__ void __launch_bounds__(ROOTS_WARPS * 32) roots_kernel(const double *_
         const size_t o = (size_t)w * n + r2;
         double D, D1, D2;
         refine_eval(geo, G, M, p, tdeg * STEER_DEG2RAD, &D, &D1, &D2);
-        float ang = (float)tdeg;
-        if (ang >= 360.0f || ang == 0.0f) ang = 0.0f;
-        out.angles[o] = ang;
-        if (out.levels) out.levels[o] = (float)(1.0 / D);
-        int b = (int)floor(tdeg * (double)K / 360.0 + 0.5);
-        if (b >= K) b -= K;
-        peak_store_bin(out, o, b);
+        ula_store_slot(out, o, tdeg, D, K);
     }
     if (lane >= f && lane < n) {
         const size_t o = (size_t)w * n + lane;

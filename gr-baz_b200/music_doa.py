@@ -105,8 +105,10 @@ class music_doa(object):
         ``"local_maxima"`` = the n largest circular local maxima more than ``exclusion_bins`` apart;
         ``"roots"`` = root-MUSIC: gridless angles from the roots of the noise-subspace polynomial, for a uniform linear
         array with spacing <= lambda / 2 installed with ``set_array_geometry`` (include/music_b200.h).  It needs
-        ``exclusion_bins`` = 0, the "music" estimator and refinement off."""
-        modes = {"top_bins": 0, "local_maxima": 1, "roots": 2}
+        ``exclusion_bins`` = 0, the "music" estimator and refinement off;
+        ``"esprit"`` = LS-ESPRIT: gridless angles from the eigenvalues of the signal subspace's shift-invariance matrix,
+        for the same arrays and with the same restrictions as ``"roots"``."""
+        modes = {"top_bins": 0, "local_maxima": 1, "roots": 2, "esprit": 3}
         if mode not in modes:
             raise ValueError("mode must be one of %s" % sorted(modes))
         _capi.check(self._lib.music_b200_set_peak_mode(self._h, modes[mode], int(exclusion_bins)), self._h)

@@ -147,10 +147,34 @@ int music_b200_set_table(music_b200 *h, const float *table_c64);
  * table came from set_table() or from set_geometry() of another geometry (no fall-back to grid peaks).  Az-el handles
  * return EINVAL.  It runs the unfused kernels: covariance, eigensolver (+ source count), [scan], then one root kernel
  * per sub-batch, timed in the top-n slot of the stage timing.
+ *
+ * MUSIC_B200_PEAKS_ESPRIT (extension, LS-ESPRIT): angles from the shift invariance of the signal subspace, for the same
+ * uniform linear arrays as ROOTS (the ULA condition, p_0, s and the angle rule above).
+ *   subspace   E_s = the d eigenvectors of largest eigenvalue (M x d, orthonormal; d = n, or the MDL / AIC count),
+ *              E1 = rows 0 .. M-2 of E_s, E2 = rows 1 .. M-1.
+ *   matrix     Psi = (E1^H E1)^-1 E1^H E2 (d x d, fp64).  Windows where E1^H E1 is not positive definite or Psi is not
+ *              finite report no peaks.  (E1^H E1 = I - r^H r with r = the last row of E_s, so the condition is
+ *              |r|^2 < 1, and the inverse is I + r^H r / (1 - |r|^2).)
+ *   eigenvalues  phi_1 .. phi_d of Psi in fp64: Householder reduction to Hessenberg form, then single-shift complex QR
+ *              with Wilkinson shifts, deflating a subdiagonal h_{l,l-1} once |h_{l,l-1}| <= 2^-52 (|h_{l-1,l-1}| +
+ *              |h_{l,l}|); a window that needs more than 30 QR steps between two deflations reports no peaks.  On a ULA
+ *              each phi is z0 = exp(-j 2 pi (s . u) / lambda) of one source, the z of ROOTS.
+ *   outputs    each eigenvalue phi gives t* by ROOTS's angle rule (z = phi), level = (float)(1 / D(t*)) with D the direct
+ *              fp64 form over the M - d noise eigenvectors, bin = floor(t* K / 360 + 0.5) mod K.  An eigenvalue exactly
+ *              0 has no direction: its slot stays unfilled.  All d directions fill slots 0 .. d-1 in descending fp64
+ *              level 1 / D, exact ties to the lower t*, then to the lower eigenvalue index (the diagonal position at
+ *              which the QR deflated it).  Slots d .. n-1, windows with d = 0 and windows with a NaN level report (0, 0, bin -1).
+ *              Spectrum, P64, R, eigenvalues and counts are unchanged, and the grid scan runs only for the spectrum
+ *              or P64, as under ROOTS.
+ * ESPRIT has ROOTS's restrictions, checked the same way in either order: exclusion_bins = 0, estimator MUSIC,
+ * refinement OFF, a current table from set_geometry() of a ULA (a process_*() call on any other table returns EINVAL,
+ * with no fall-back to grid peaks), and no az-el handle.  It runs the unfused kernels: covariance, eigensolver (+ source
+ * count), [scan], then one ESPRIT kernel per sub-batch, timed in the top-n slot of the stage timing.
  */
 #define MUSIC_B200_PEAKS_TOP_BINS 0
 #define MUSIC_B200_PEAKS_LOCAL_MAXIMA 1
 #define MUSIC_B200_PEAKS_ROOTS 2
+#define MUSIC_B200_PEAKS_ESPRIT 3
 int music_b200_set_peak_mode(music_b200 *h, int mode, uint32_t exclusion_bins);
 
 /*
