@@ -34,6 +34,7 @@
 #include "music_estimators.cuh"
 #include "music_roots.cuh"
 #include "music_esprit.cuh"
+#include "music_dml.cuh"
 
 using namespace music;
 
@@ -312,7 +313,8 @@ bool gridless_ula(int peak) { return peak == MUSIC_B200_PEAKS_ROOTS || peak == M
 // hold one (single-device handles, and the children of a multi-device handle).
 int check_modes(music_b200 *h, const Modes &p, const DeviceTable *t)
 {
-    if (p.peak != MUSIC_B200_PEAKS_TOP_BINS && p.peak != MUSIC_B200_PEAKS_LOCAL_MAXIMA && !gridless_ula(p.peak))
+    if (p.peak != MUSIC_B200_PEAKS_TOP_BINS && p.peak != MUSIC_B200_PEAKS_LOCAL_MAXIMA && !gridless_ula(p.peak) &&
+        p.peak != MUSIC_B200_PEAKS_DML)
         return fail(h, MUSIC_B200_EINVAL, "unknown peak mode %d", p.peak);
     if (p.excl >= h->K) return fail(h, MUSIC_B200_EINVAL, "exclusion_bins must be < resolution");
     if (p.refine != MUSIC_B200_REFINE_OFF && p.refine != MUSIC_B200_REFINE_NEWTON) return fail(h, MUSIC_B200_EINVAL, "unknown refine mode %d", p.refine);
@@ -333,6 +335,14 @@ int check_modes(music_b200 *h, const Modes &p, const DeviceTable *t)
         if (t && !(t->geometric && t->ula.ula))
             return fail(h, MUSIC_B200_EINVAL, "the %s peak mode needs a table built by music_b200_set_geometry() from a uniform linear "
                                               "array with spacing <= lambda / 2 (call set_geometry(), or another peak mode)", name);
+    }
+    if (p.peak == MUSIC_B200_PEAKS_DML) {
+        // any 1-D table: DML reads table rows only
+        if (p.excl != 0) return fail(h, MUSIC_B200_EINVAL, "the DML peak mode takes exclusion_bins = 0");
+        if (h->azel) return fail(h, MUSIC_B200_EINVAL, "the DML peak mode is not supported on an az-el handle");
+        if (p.est != MUSIC_B200_ESTIMATOR_MUSIC) return fail(h, MUSIC_B200_EINVAL, "the DML peak mode needs the MUSIC estimator");
+        if (p.refine != MUSIC_B200_REFINE_OFF)
+            return fail(h, MUSIC_B200_EINVAL, "the DML peak mode needs refinement off (NEWTON refines the MUSIC objective)");
     }
     if (t && p.refine != MUSIC_B200_REFINE_OFF && !t->geometric)
         return fail(h, MUSIC_B200_EINVAL, "peak refinement needs a table built by music_b200_set_geometry(); the current one came from "
@@ -464,7 +474,7 @@ constexpr unsigned CTR_RING = 256;  // ticket-counter pairs per slot (see ticket
 
 enum class Path { Unfused, Fused4, Fused8 };
 enum class Scan { None, Peak1, Music, Quad };              // scan_peak1_kernel, scan_kernel, scan_quad_kernel
-enum class Peaks { None, TopN, Local, Local2D, Roots, Esprit };  // topn, topn_local, topn_local2d, roots, esprit kernels
+enum class Peaks { None, TopN, Local, Local2D, Roots, Esprit, Dml };  // topn, topn_local, topn_local2d, roots, esprit, dml kernels
 
 // What one call runs, from the handle's modes, the requested outputs and the input form (plan_call).
 struct Plan {
@@ -486,6 +496,7 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
     const bool music_est = md.est == MUSIC_B200_ESTIMATOR_MUSIC;
     const bool local = md.peak == MUSIC_B200_PEAKS_LOCAL_MAXIMA;
     const bool gridless = gridless_ula(md.peak);
+    const bool dml = md.peak == MUSIC_B200_PEAKS_DML;
     Plan p;
     // The fused kernels find the principal eigenvector only, not every eigenvalue a source count needs nor the noise
     // eigenvectors the peak refinement needs; they compute the MUSIC spectrum only.  Planar streams can take the M = 4
@@ -497,18 +508,19 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
     if (fusable && h->m == 4 && planar_fusable && (!o.spec || h->fused_spec)) p.path = Path::Fused4;
     else if (fusable && h->m == 8 && !planar && !o.spec && h->N >= 128 && h->N % 2 == 0) p.path = Path::Fused8;
 
-    // MVDR and Bartlett need the eigensolver only to count sources or when the caller asked for the eigenvalues
-    p.eig = music_est || !fixed_n || o.ev;
+    // MVDR and Bartlett need the eigensolver only to count sources or when the caller asked for the eigenvalues; DML
+    // (which reads R only) also for the MUSIC spectrum or P64
+    p.eig = (music_est && (!dml || o.spec || o.P64)) || !fixed_n || o.ev;
     p.count = !fixed_n;
     p.mvdr = md.est == MUSIC_B200_ESTIMATOR_MVDR;
     p.est = md.est;
-    p.argmax = h->n == 1 && !local && !gridless;
+    p.argmax = h->n == 1 && !local && !gridless && !dml;
     p.spec = o.spec != nullptr;
     if (!music_est) {
         p.scan = Scan::Quad;
         p.p64 = !p.argmax || o.P64;
-    } else if (gridless) {
-        // the grid spectrum only when the caller asked for it; the angles come from the root or ESPRIT kernel
+    } else if (gridless || dml) {
+        // the grid spectrum only when the caller asked for it; the angles come from the root, ESPRIT or DML kernel
         p.scan = o.spec || o.P64 ? Scan::Music : Scan::None;
         p.p64 = p.scan == Scan::Music;
     } else if (p.argmax && !o.P64 && !o.spec && (h->m == 4 || h->m == 8 || h->m == 16)) {
@@ -518,6 +530,7 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
         p.p64 = !p.argmax || o.P64;
     }
     if (gridless) p.peaks = md.peak == MUSIC_B200_PEAKS_ROOTS ? Peaks::Roots : Peaks::Esprit;
+    else if (dml) p.peaks = Peaks::Dml;
     else if (!p.argmax) p.peaks = local && h->azel ? Peaks::Local2D : local ? Peaks::Local : Peaks::TopN;
     p.decode = h->azel;
     p.refine = md.refine != MUSIC_B200_REFINE_OFF;
@@ -820,6 +833,13 @@ int launch_eig_scan(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t 
     case Peaks::Esprit:
         esprit_kernel<<<(W + ESPRIT_WARPS - 1) / ESPRIT_WARPS, ESPRIT_WARPS * 32, 0, st>>>(ws.Vt, cnt, M, (int)h->n, (int)h->K, (int)W,
                                                                                         tb.geo, tb.ula, po);
+        break;
+    case Peaks::Dml:
+        // M = 16 runs the runtime-M instantiation (its loops have the same 16-entry bound): the fixed-M one spills
+        with_scan_m(h->m, [&](auto mt) {
+            constexpr int MT = decltype(mt)::value == 16 ? 0 : decltype(mt)::value;
+            dml_kernel<MT><<<W, DML_THREADS, 0, st>>>(ws.R, tb.soa, cnt, M, (int)h->n, (int)h->K, po);
+        });
         break;
     case Peaks::Local2D: topn_local2d_kernel<<<W, AZEL_LM_THREADS, 0, st>>>(p64, (int)h->n, h->grid.n_az, h->grid.n_el, excl, po, cnt); break;
     case Peaks::Local: topn_local_kernel<<<(W + 7) / 8, 256, 0, st>>>(p64, (int)h->n, (int)h->K, (int)W, excl, po, cnt); break;

@@ -107,8 +107,12 @@ class music_doa(object):
         array with spacing <= lambda / 2 installed with ``set_array_geometry`` (include/music_b200.h).  It needs
         ``exclusion_bins`` = 0, the "music" estimator and refinement off;
         ``"esprit"`` = LS-ESPRIT: gridless angles from the eigenvalues of the signal subspace's shift-invariance matrix,
-        for the same arrays and with the same restrictions as ``"roots"``."""
-        modes = {"top_bins": 0, "local_maxima": 1, "roots": 2, "esprit": 3}
+        for the same arrays and with the same restrictions as ``"roots"``;
+        ``"dml"`` = deterministic maximum likelihood by alternating projection: the n table rows whose span captures the
+        most power of the covariance, so coherent sources (multipath) are resolved, on any table; levels are
+        least-squares source powers.  It needs ``exclusion_bins`` = 0, the "music" estimator and refinement off; use the
+        "fixed" source rule for coherent sources."""
+        modes = {"top_bins": 0, "local_maxima": 1, "roots": 2, "esprit": 3, "dml": 4}
         if mode not in modes:
             raise ValueError("mode must be one of %s" % sorted(modes))
         _capi.check(self._lib.music_b200_set_peak_mode(self._h, modes[mode], int(exclusion_bins)), self._h)

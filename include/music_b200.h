@@ -170,11 +170,40 @@ int music_b200_set_table(music_b200 *h, const float *table_c64);
  * refinement OFF, a current table from set_geometry() of a ULA (a process_*() call on any other table returns EINVAL,
  * with no fall-back to grid peaks), and no az-el handle.  It runs the unfused kernels: covariance, eigensolver (+ source
  * count), [scan], then one ESPRIT kernel per sub-batch, timed in the top-n slot of the stage timing.
+ *
+ * MUSIC_B200_PEAKS_DML (extension, deterministic maximum likelihood by alternating projection): the d table rows whose
+ * span captures the most power of R, tr(P_A R).  It needs no signal-subspace rank, so it resolves coherent sources (a
+ * path and its reflection, one emitter seen twice) that every subspace method merges, on any 1-D table.
+ *   inputs     R = the window's fp64 covariance (the R output); a_k = table row k widened to fp64, ||a_k||^2 in fp64;
+ *              d = n, or the MDL / AIC count.  d = 0, any non-finite entry of R, or tr R <= 0 (no power to place)
+ *              gives a window with no peaks.
+ *   search     S(B), B a set of slot bins: Q_B = modified Gram-Schmidt, applied twice, of the rows a_b (b in B) in slot
+ *              order; P = I - Q_B Q_B^H; num(k) = a_k^H P R P a_k (a_k^H R a_k for B empty); den(k) = ||a_k||^2 -
+ *              ||Q_B^H a_k||^2.  Bin k is a candidate iff den(k) > 2^-30 ||a_k||^2 and f(k) = num(k) / den(k) is
+ *              finite (so a row in span(B), such as a line array's mirror row or a row already in B, and a zero row are
+ *              never candidates).  S(B) = the candidate of largest f, exact ties to the lower bin; no candidate: the
+ *              window reports no peaks.
+ *   init       slot i = S({slots 0 .. i-1}), i = 0 .. d-1.
+ *   sweeps     s = 1 .. 20: for i = 0 .. d-1, slot i = S({every other slot}) with the updated slots (Gauss-Seidel);
+ *              stop after the first sweep that changed no slot, else keep the bins of sweep 20.  tr(P_A R) never
+ *              decreases; with d = 1 a sweep repeats the first search and is skipped.
+ *   levels     A = [a_slot0 .. a_slot(d-1)] = Q_A T (MGS twice as above), s2 = (tr R - tr(Q_A^H R Q_A)) / (M - d),
+ *              p = diag(T^-1 (Q_A^H R Q_A - s2 I) T^-H): least-squares source powers in R's units (as MVDR's and
+ *              Bartlett's levels; unlike MUSIC's 1 / D).  A level can be <= 0 at low SNR; its slot is still filled.
+ *   outputs    slots 0 .. d-1 in descending fp64 p, exact ties to the lower bin; angle = (float)(bin * 360 / K) as
+ *              under TOP_BINS, level = (float)p, bin through the peak-bin all-gather of sharded calls.  Slots d .. n-1
+ *              report (0, 0, bin -1).  Spectrum, P64, R, eigenvalues and counts are unchanged.
+ * Coherent sources lower the rank MDL / AIC count: use FIXED for them.  DML needs exclusion_bins = 0, estimator MUSIC
+ * and refinement OFF (NEWTON refines the MUSIC objective), checked in either order, and no az-el handle; any table from
+ * set_table() or set_geometry() is accepted.  It runs the unfused kernels: covariance, the eigensolver only for MDL /
+ * AIC, the eigenvalues, the spectrum or P64, the MUSIC scan only for the spectrum or P64, then one DML kernel per
+ * sub-batch (one CTA per window for all its searches), timed in the top-n slot of the stage timing.
  */
 #define MUSIC_B200_PEAKS_TOP_BINS 0
 #define MUSIC_B200_PEAKS_LOCAL_MAXIMA 1
 #define MUSIC_B200_PEAKS_ROOTS 2
 #define MUSIC_B200_PEAKS_ESPRIT 3
+#define MUSIC_B200_PEAKS_DML 4
 int music_b200_set_peak_mode(music_b200 *h, int mode, uint32_t exclusion_bins);
 
 /*
