@@ -147,12 +147,7 @@ __global__ void __launch_bounds__(AZEL_LM_THREADS) topn_local2d_kernel(const dou
                 if (ok) { bP = p; bk = b; }
             }
         }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const double Po = __shfl_xor_sync(0xffffffffu, bP, o);
-            const int ko = __shfl_xor_sync(0xffffffffu, bk, o);
-            if (peak_better(Po, ko, bP, bk)) { bP = Po; bk = ko; }
-        }
+        warp_argmax(bP, bk);
         if (lane == 0) { rP[wid] = bP; rk[wid] = bk; }
         __syncthreads();
         if (threadIdx.x == 0) {

@@ -473,7 +473,7 @@ EncodeTiledFn encode_tiled_fn()
 constexpr unsigned CTR_RING = 256;  // ticket-counter pairs per slot (see ticket_counter)
 
 enum class Path { Unfused, Fused4, Fused8 };
-enum class Scan { None, Peak1, Music, Quad };              // scan_peak1_kernel, scan_kernel, scan_quad_kernel
+enum class Scan { None, Peak1, Grid };                     // scan_peak1_kernel, scan_kernel
 enum class Peaks { None, TopN, Local, Local2D, Roots, Esprit, Dml };  // topn, topn_local, topn_local2d, roots, esprit, dml kernels
 
 // What one call runs, from the handle's modes, the requested outputs and the input form (plan_call).
@@ -482,8 +482,8 @@ struct Plan {
     // the unfused path, per sub-batch:
     bool eig = false, count = false, mvdr = false;  // eigensolver, source count, MVDR preparation
     Scan scan = Scan::None;
-    bool argmax = false, p64 = false, spec = false;  // template flags of scan_kernel / scan_quad_kernel
-    int est = MUSIC_B200_ESTIMATOR_MUSIC;            // the form of scan_quad_kernel and the refined objective
+    bool argmax = false, p64 = false, spec = false;  // template flags of scan_kernel
+    int est = MUSIC_B200_ESTIMATOR_MUSIC;            // the form of scan_kernel and the refined objective
     Peaks peaks = Peaks::None;
     bool decode = false, refine = false;             // az-el bin decode; peak refinement (the az-el kind after a decode)
     bool ws_p64 = false, ws_counts = false, ws_bins = false;  // workspace buffers the kernels write
@@ -516,17 +516,14 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
     p.est = md.est;
     p.argmax = h->n == 1 && !local && !gridless && !dml;
     p.spec = o.spec != nullptr;
-    if (!music_est) {
-        p.scan = Scan::Quad;
-        p.p64 = !p.argmax || o.P64;
-    } else if (gridless || dml) {
+    if (music_est && (gridless || dml)) {
         // the grid spectrum only when the caller asked for it; the angles come from the root, ESPRIT or DML kernel
-        p.scan = o.spec || o.P64 ? Scan::Music : Scan::None;
-        p.p64 = p.scan == Scan::Music;
-    } else if (p.argmax && !o.P64 && !o.spec && (h->m == 4 || h->m == 8 || h->m == 16)) {
+        p.scan = o.spec || o.P64 ? Scan::Grid : Scan::None;
+        p.p64 = p.scan == Scan::Grid;
+    } else if (music_est && p.argmax && !o.P64 && !o.spec && (h->m == 4 || h->m == 8 || h->m == 16)) {
         p.scan = Scan::Peak1;
     } else {
-        p.scan = Scan::Music;
+        p.scan = Scan::Grid;
         p.p64 = !p.argmax || o.P64;
     }
     if (gridless) p.peaks = md.peak == MUSIC_B200_PEAKS_ROOTS ? Peaks::Roots : Peaks::Esprit;
@@ -602,7 +599,7 @@ struct ScanFlags {
     static constexpr bool argmax = A, p64 = P, spec = S;
 };
 
-// The six (argmax, p64, spec) instantiations of scan_kernel and scan_quad_kernel: without the arg-max the peak rule
+// The six (argmax, p64, spec) instantiations of scan_kernel per form: without the arg-max the peak rule
 // reads P64, so P64 is written.  f receives the matching ScanFlags.
 template <class F>
 void with_scan_flags(const Plan &p, F f)
@@ -615,14 +612,32 @@ void with_scan_flags(const Plan &p, F f)
     else if (!p.argmax && p.p64 && p.spec) f(ScanFlags<false, true, true>());
 }
 
+template <int F, bool C>
+struct ScanForm {
+    static constexpr int form = F;
+    static constexpr bool counts = C;
+};
+
+// The (FORM, COUNTS) instantiations of scan_kernel: the estimator's strength, and for MUSIC whether the scan reads the
+// per-window source counts (cnt).  f receives the matching ScanForm.
+template <class F>
+void with_scan_form(const Plan &p, const int32_t *cnt, F f)
+{
+    if (p.est == MUSIC_B200_ESTIMATOR_MVDR) f(ScanForm<EST_MVDR, false>());
+    else if (p.est == MUSIC_B200_ESTIMATOR_BARTLETT) f(ScanForm<EST_BARTLETT, false>());
+    else if (cnt) f(ScanForm<EST_MUSIC, true>());
+    else f(ScanForm<EST_MUSIC, false>());
+}
+
 // K3, the grid scan of W windows the plan chose, into the outputs o of these windows.  cnt: the per-window source counts
-// (NULL under the FIXED rule).  scan_quad_kernel (music_estimators.cuh) reads the g_j of mvdr_prep_kernel (MVDR) or R
-// (Bartlett).
+// (NULL under the FIXED rule).  scan_kernel stages per window the eigenvectors (MUSIC), the g_j of mvdr_prep_kernel
+// (MVDR) or R (Bartlett).
 void launch_scan(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t W, const Outputs &o, const PeakOut &po,
                  const int32_t *cnt, cudaStream_t st)
 {
     if (p.scan == Scan::None) return;
     const double *soa = h->table[h->cur_table].soa;
+    const double *V = p.est == MUSIC_B200_ESTIMATOR_BARTLETT ? ws.R : ws.Vt;
     float *d_spec = o.spec;
     double *d_p64 = o.P64 ? o.P64 : ws.P64;
     const int M = (int)h->m, n = (int)h->n, K = (int)h->K, grid = (W + SCAN_B - 1) / SCAN_B;
@@ -633,16 +648,13 @@ void launch_scan(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t W, 
             if constexpr (MT != 0) scan_peak1_kernel<MT><<<grid, TILE, 0, st>>>(soa, ws.Vt, K, (int)W, po, cnt);  // (planned for M = 4, 8, 16 only)
             return;
         }
-        with_scan_flags(p, [&](auto f) {
-            using Fl = decltype(f);
-            if (p.scan == Scan::Quad && p.mvdr)
-                scan_quad_kernel<MT, QUAD_MVDR, Fl::argmax, Fl::p64, Fl::spec><<<grid, TILE, smem, st>>>(soa, ws.Vt, M, K, (int)W, po, d_spec, d_p64, cnt);
-            else if (p.scan == Scan::Quad)
-                scan_quad_kernel<MT, QUAD_BARTLETT, Fl::argmax, Fl::p64, Fl::spec><<<grid, TILE, smem, st>>>(soa, ws.R, M, K, (int)W, po, d_spec, d_p64, cnt);
-            else if (cnt)
-                scan_kernel<MT, Fl::argmax, Fl::p64, Fl::spec, true><<<grid, TILE, smem, st>>>(soa, ws.Vt, M, n, K, (int)W, po, d_spec, d_p64, cnt);
-            else
-                scan_kernel<MT, Fl::argmax, Fl::p64, Fl::spec><<<grid, TILE, smem, st>>>(soa, ws.Vt, M, n, K, (int)W, po, d_spec, d_p64, nullptr);
+        with_scan_form(p, cnt, [&](auto fm) {
+            with_scan_flags(p, [&](auto f) {
+                using Fm = decltype(fm);
+                using Fl = decltype(f);
+                scan_kernel<MT, Fm::form, Fl::argmax, Fl::p64, Fl::spec, Fm::counts>
+                    <<<grid, TILE, smem, st>>>(soa, V, M, n, K, (int)W, po, d_spec, d_p64, cnt);
+            });
         });
     });
     h->launches++;

@@ -6,7 +6,7 @@
 // every subspace method sees one source.  Alternating projection (Ziskind & Wax, 1988) turns the d-dimensional search
 // into 1-D table searches S(B): with Q_B an orthonormal basis of the rows already held (B) and P = I - Q_B Q_B^H,
 //     f(k) = a_k^H P R P a_k / (||a_k||^2 - ||Q_B^H a_k||^2),
-// the power gained by adding row k.  Each search is the Bartlett scan of scan_quad_kernel (bartlett_form) on R' = P R P,
+// the power gained by adding row k.  Each search is the Bartlett grid scan (bartlett_form) on R' = P R P,
 // plus the denominator.  The full definition (candidate rule, sweeps, least-squares levels, slot order) is in
 // include/music_b200.h and is restated by tests/dml_oracle.py.
 //
@@ -22,17 +22,6 @@ constexpr int DML_THREADS = 128;
 constexpr int DML_WARPS = DML_THREADS / 32;
 constexpr int DML_MAX_SWEEPS = 20;
 constexpr double DML_DEN_MIN = 9.313225746154785e-10;  // 2^-30: den(k) must exceed this fraction of ||a_k||^2
-
-__device__ __forceinline__ double2 dml_cmul(double2 a, double2 b) { return make_double2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
-// conj(a) b
-__device__ __forceinline__ double2 dml_cjmul(double2 a, double2 b) { return make_double2(a.x * b.x + a.y * b.y, a.x * b.y - a.y * b.x); }
-
-__device__ __forceinline__ double dml_warp_sum(double v)
-{
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
 
 // Row k of the SoA table, entry i (re, im), and ||a_k||^2
 __device__ __forceinline__ const double *dml_row(const double *soa, int k, int M)
@@ -56,14 +45,14 @@ __device__ __forceinline__ void dml_mgs2(const double *soa, const int *bins, int
         for (int pass = 0; pass < 2; ++pass) {
             for (int j = 0; j < l; ++j) {
                 const double2 q = lane < M ? Q[j * MAXM + lane] : make_double2(0.0, 0.0);
-                const double2 p = dml_cjmul(q, v);
-                const double2 c = make_double2(dml_warp_sum(p.x), dml_warp_sum(p.y));
+                const double2 p = cjmul(q, v);
+                const double2 c = make_double2(warp_sum(p.x), warp_sum(p.y));
                 v.x -= c.x * q.x - c.y * q.y;
                 v.y -= c.x * q.y + c.y * q.x;
                 if (T && lane == 0) { T[j * MAXM + l].x += c.x; T[j * MAXM + l].y += c.y; }
             }
         }
-        const double nrm = sqrt(dml_warp_sum(v.x * v.x + v.y * v.y));
+        const double nrm = sqrt(warp_sum(v.x * v.x + v.y * v.y));
         if (lane < M) Q[l * MAXM + lane] = make_double2(v.x / nrm, v.y / nrm);
         if (T && lane == 0) T[l * MAXM + l] = make_double2(nrm, 0.0);
         __syncwarp();
@@ -114,7 +103,7 @@ __global__ void __launch_bounds__(DML_THREADS) dml_kernel(const double *__restri
             const int i = e / M, j = e - i * M;
             double2 s = make_double2(i == j ? 1.0 : 0.0, 0.0);
             for (int l = 0; l < r; ++l) {
-                const double2 t = dml_cmul(sQ[l * MAXM + i], make_double2(sQ[l * MAXM + j].x, -sQ[l * MAXM + j].y));
+                const double2 t = cmul(sQ[l * MAXM + i], make_double2(sQ[l * MAXM + j].x, -sQ[l * MAXM + j].y));
                 s.x -= t.x;
                 s.y -= t.y;
             }
@@ -125,7 +114,7 @@ __global__ void __launch_bounds__(DML_THREADS) dml_kernel(const double *__restri
             const int i = e / M, j = e - i * M;
             double2 s = make_double2(0.0, 0.0);
             for (int q = 0; q < M; ++q) {
-                const double2 t = dml_cmul(sP[i * M + q], sR[q * M + j]);
+                const double2 t = cmul(sP[i * M + q], sR[q * M + j]);
                 s.x += t.x;
                 s.y += t.y;
             }
@@ -136,7 +125,7 @@ __global__ void __launch_bounds__(DML_THREADS) dml_kernel(const double *__restri
             const int i = e / M, j = e - i * M;
             double2 s = make_double2(0.0, 0.0);
             for (int q = 0; q < M; ++q) {
-                const double2 t = dml_cmul(sX[i * M + q], sP[q * M + j]);
+                const double2 t = cmul(sX[i * M + q], sP[q * M + j]);
                 s.x += t.x;
                 s.y += t.y;
             }
@@ -175,12 +164,7 @@ __global__ void __launch_bounds__(DML_THREADS) dml_kernel(const double *__restri
             const double f = bartlett_form<MT>(ar, ai, Rp, M) / den;
             if (den > DML_DEN_MIN * na && isfinite(f) && f > best) { best = f; bk = k; }
         }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const double fo = __shfl_xor_sync(0xffffffffu, best, o);
-            const int ko = __shfl_xor_sync(0xffffffffu, bk, o);
-            if (peak_better(fo, ko, best, bk)) { best = fo; bk = ko; }
-        }
+        warp_argmax(best, bk);
         if (lane == 0) { rf[wid] = best; rk[wid] = bk; }
         __syncthreads();
         if (tid == 0) {
@@ -227,11 +211,11 @@ __global__ void __launch_bounds__(DML_THREADS) dml_kernel(const double *__restri
             for (int i = 0; i < M; ++i) {
                 double2 y = make_double2(0.0, 0.0);  // (R q_b)_i
                 for (int j = 0; j < M; ++j) {
-                    const double2 t = dml_cmul(sR[i * M + j], sQ[b * MAXM + j]);
+                    const double2 t = cmul(sR[i * M + j], sQ[b * MAXM + j]);
                     y.x += t.x;
                     y.y += t.y;
                 }
-                const double2 t = dml_cjmul(sQ[a * MAXM + i], y);
+                const double2 t = cjmul(sQ[a * MAXM + i], y);
                 s.x += t.x;
                 s.y += t.y;
             }
@@ -251,7 +235,7 @@ __global__ void __launch_bounds__(DML_THREADS) dml_kernel(const double *__restri
                 double2 s = make_double2(i == c ? 1.0 : 0.0, 0.0);
                 if (i <= c) {
                     for (int q = i + 1; q <= c; ++q) {
-                        const double2 t = dml_cmul(sT[i * MAXM + q], U[q * MAXM + c]);
+                        const double2 t = cmul(sT[i * MAXM + q], U[q * MAXM + c]);
                         s.x -= t.x;
                         s.y -= t.y;
                     }
@@ -270,11 +254,11 @@ __global__ void __launch_bounds__(DML_THREADS) dml_kernel(const double *__restri
             for (int a = lane; a < d; ++a) {
                 double2 y = make_double2(0.0, 0.0);
                 for (int b = lane; b < d; ++b) {
-                    const double2 t = dml_cmul(sX[a * MAXM + b], make_double2(U[lane * MAXM + b].x, -U[lane * MAXM + b].y));
+                    const double2 t = cmul(sX[a * MAXM + b], make_double2(U[lane * MAXM + b].x, -U[lane * MAXM + b].y));
                     y.x += t.x;
                     y.y += t.y;
                 }
-                p += dml_cmul(U[lane * MAXM + a], y).x;
+                p += cmul(U[lane * MAXM + a], y).x;
             }
             s_p[lane] = p;
         }
@@ -285,22 +269,16 @@ __global__ void __launch_bounds__(DML_THREADS) dml_kernel(const double *__restri
 
     // outputs: slots in descending p, exact ties to the lower bin; slots d .. n-1 (every slot without peaks) (0, 0, -1)
     if (tid < n) {
-        const size_t o = w * n + tid;
+        int rnk = tid, k = -1;
+        double p = 0.0;
         if (!s_none && tid < d) {
-            const double p = s_p[tid];
-            const int k = slot[tid];
-            int rnk = 0;
+            p = s_p[tid];
+            k = slot[tid];
+            rnk = 0;
             for (int j = 0; j < d; ++j)
                 if (s_p[j] > p || (s_p[j] == p && slot[j] < k)) ++rnk;
-            const size_t od = w * n + rnk;
-            out.angles[od] = (float)((double)k * 360.0 / (double)K);
-            if (out.levels) out.levels[od] = (float)p;
-            peak_store_bin(out, od, k);
-        } else {
-            out.angles[o] = 0.f;
-            if (out.levels) out.levels[o] = 0.f;
-            peak_store_bin(out, o, -1);
         }
+        peak_write(out, w * n + rnk, k, p, K);
     }
 }
 

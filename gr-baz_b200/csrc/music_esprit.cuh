@@ -194,12 +194,7 @@ __global__ void __launch_bounds__(ESPRIT_WARPS * 32) esprit_kernel(const double 
     }
     const int f = __popc(__ballot_sync(0xffffffffu, filled));
     if (filled) ula_store_slot(out, (size_t)w * n + r, tdeg, D, K);
-    if (lane >= f && lane < n) {
-        const size_t o = (size_t)w * n + lane;
-        out.angles[o] = 0.f;
-        if (out.levels) out.levels[o] = 0.f;
-        peak_store_bin(out, o, -1);
-    }
+    if (lane >= f && lane < n) peak_write(out, (size_t)w * n + lane, -1, 0.0, K);
 }
 
 }  // namespace music

@@ -8,15 +8,12 @@
 // conjugated, into the window's ws.Vt slot as g_j = conj(row j of L^-1), so that
 //     a^H R_L^-1 a = ||L^-1 a||^2 = sum_j |g_j^H a|^2,
 // which cannot cancel and is the form the refinement kernels already evaluate (music_refine.cuh, with p = M vectors).
-// scan_quad_kernel is scan_kernel (music_kernels.cuh) with the strength replaced by one of the two forms.  The full
-// definition is in include/music_b200.h and is restated literally by tests/estimator_oracle.py.
+// The grid scan is scan_kernel (music_kernels.cuh) with FORM = EST_MVDR or EST_BARTLETT.  The full definition is in
+// include/music_b200.h and is restated literally by tests/estimator_oracle.py.
 #pragma once
 #include "music_kernels.cuh"
 
 namespace music {
-
-constexpr int QUAD_MVDR = 1;      // MUSIC_B200_ESTIMATOR_MVDR
-constexpr int QUAD_BARTLETT = 2;  // MUSIC_B200_ESTIMATOR_BARTLETT
 
 // ---- MVDR preparation: one warp per window, the matrix in shared memory --------------------------------------------
 // A 16 x 16 complex fp64 matrix is 4 KiB: too large for one thread's registers, so each window gets a warp and two
@@ -100,7 +97,7 @@ __global__ void __launch_bounds__(PREP_WARPS * 32) mvdr_prep_kernel(const double
     }
 }
 
-// ---- the quadratic-form scan ------------------------------------------------------------------------------------------
+// ---- the strengths of the quadratic-form scan (scan_kernel) --------------------------------------------------------
 // MVDR: a^H R_L^-1 a = sum_j |g_j^H a|^2 over the triangular g (M (M + 1) / 2 complex MACs)
 template <int MT>
 __device__ __forceinline__ double mvdr_form(const double *ar, const double *ai, const double *g, int M)
@@ -144,93 +141,6 @@ __device__ __forceinline__ double bartlett_form(const double *ar, const double *
         acc = fma(2.0, fma(ar[i], ur, ai[i] * ui), acc);
     }
     return acc;
-}
-
-// scan_kernel with P[k] of the chosen form.  Q: per window M*M complex doubles, the g_j of mvdr_prep_kernel (MVDR) or
-// R itself (BARTLETT), staged in shared memory for SCAN_B windows; thread <-> bin.  ARGMAX: n == 1 fused peak pick
-// (P desc, bin asc, P > 0 strictly, NaN never).  counts (may be null, music_sources.cuh): with ARGMAX a window with
-// count 0 reports no peak; the spectrum itself does not depend on the count.
-template <int MT, int FORM, bool ARGMAX, bool WRITE_P64, bool WRITE_SPEC>
-__global__ void __launch_bounds__(TILE) scan_quad_kernel(const double *__restrict__ soa, const double *__restrict__ Q, int Mrt, int K,
-                                                         int W, PeakOut out, float *__restrict__ spectrum, double *__restrict__ P64,
-                                                         const int32_t *__restrict__ counts)
-{
-    constexpr int MA = MT ? MT : MAXM;
-    const int M = MT ? MT : Mrt;
-    extern __shared__ __align__(16) double smem[];
-    const int w0 = blockIdx.x * SCAN_B;
-    const int nb = min(SCAN_B, W - w0);
-    const int vsz = M * M * 2;
-    for (int i = threadIdx.x; i < nb * vsz; i += blockDim.x) smem[i] = Q[(size_t)w0 * vsz + i];
-    __syncthreads();
-
-    double best[SCAN_B];
-    int bestk[SCAN_B];
-#pragma unroll
-    for (int b = 0; b < SCAN_B; ++b) { best[b] = 0.0; bestk[b] = -1; }
-
-    const int ntiles = (K + TILE - 1) / TILE;
-    for (int tile = 0; tile < ntiles; ++tile) {
-        const int k = tile * TILE + threadIdx.x;
-        const double *tb = soa + (size_t)tile * (2 * M + 1) * TILE + threadIdx.x;
-        double ar[MA], ai[MA];
-#pragma unroll
-        for (int i = 0; i < MA; ++i) {
-            if (!MT && i >= M) break;
-            ar[i] = tb[(size_t)(2 * i) * TILE];
-            ai[i] = tb[(size_t)(2 * i + 1) * TILE];
-        }
-        const double na = tb[(size_t)(2 * M) * TILE];
-        if (k < K) {
-#pragma unroll
-            for (int b = 0; b < SCAN_B; ++b) {
-                if (b < nb) {
-                    const double *q = smem + b * vsz;
-                    const double P = FORM == QUAD_MVDR ? 1.0 / mvdr_form<MT>(ar, ai, q, M) : bartlett_form<MT>(ar, ai, q, M) / (na * na);
-                    if (WRITE_SPEC) spectrum[(size_t)(w0 + b) * K + k] = (float)P;
-                    if (WRITE_P64) P64[(size_t)(w0 + b) * K + k] = P;
-                    if (ARGMAX) {
-                        if (P > best[b]) { best[b] = P; bestk[b] = k; }  // k ascending per thread: strict > keeps the lower bin
-                    }
-                }
-            }
-        }
-    }
-    if (ARGMAX) {
-        __shared__ double rP[SCAN_B][TILE / 32];
-        __shared__ int rk[SCAN_B][TILE / 32];
-        const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-#pragma unroll
-        for (int b = 0; b < SCAN_B; ++b) {
-            int kk = bestk[b];
-            double P = best[b];
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const double Po = __shfl_xor_sync(0xffffffffu, P, o);
-                const int ko = __shfl_xor_sync(0xffffffffu, kk, o);
-                if (peak_better(Po, ko, P, kk)) { P = Po; kk = ko; }
-            }
-            if (lane == 0) { rP[b][wid] = P; rk[b][wid] = kk; }
-        }
-        __syncthreads();
-        if (threadIdx.x < nb) {
-            const int b = threadIdx.x;
-            double P = rP[b][0];
-            int kk = rk[b][0];
-            for (int q = 1; q < TILE / 32; ++q)
-                if (peak_better(rP[b][q], rk[b][q], P, kk)) { P = rP[b][q]; kk = rk[b][q]; }
-            const size_t o = (size_t)(w0 + b);  // n == 1
-            if (counts && counts[o] == 0) kk = -1;
-            if (kk >= 0) {
-                out.angles[o] = (float)((double)kk * 360.0 / (double)K);
-                if (out.levels) out.levels[o] = (float)P;
-            } else {
-                out.angles[o] = 0.f;
-                if (out.levels) out.levels[o] = 0.f;
-            }
-            peak_store_bin(out, o, kk);
-        }
-    }
 }
 
 }  // namespace music

@@ -334,19 +334,6 @@ __device__ __forceinline__ void fz_unlock(unsigned *lock, const int lane)  // al
 __device__ __forceinline__ void fz_lock(FusedCtl *ctl, const int lane) { fz_lock(&ctl->lock, lane); }
 __device__ __forceinline__ void fz_unlock(FusedCtl *ctl, const int lane) { fz_unlock(&ctl->lock, lane); }
 
-// peak of one window -> the block's outputs (reference :134, :153-154; (0, 0) initial pair :95)
-__device__ __forceinline__ void fused_write_peak(const PeakOut &out, const size_t o, const int kk, const double P, const int K)
-{
-    if (kk >= 0) {
-        out.angles[o] = (float)((double)kk * 360.0 / (double)K);
-        if (out.levels) out.levels[o] = (float)P;
-    } else {
-        out.angles[o] = 0.f;
-        if (out.levels) out.levels[o] = 0.f;
-    }
-    peak_store_bin(out, o, kk);
-}
-
 // OUTPUT ORDER.  Results must land after those of the previous launch on the stream, which under programmatic dependent
 // launch runs alongside this one (often in the other half of the same SM) for most of this launch.  Waiting for it
 // (griddepcontrol.wait) before the first store would stall the scan, fill the queue and stop the covariance warps, so
@@ -359,7 +346,7 @@ __device__ __noinline__ void fused_stage_flush(unsigned char *smem, const PeakOu
     const StagedPeak *stg = reinterpret_cast<const StagedPeak *>(smem + FZ_OFF_STG);
     asm volatile("griddepcontrol.wait;" ::: "memory");  // the previous launch has finished and its writes are visible
     const unsigned n = ctl->stg_n;
-    for (unsigned i = threadIdx.x & 31; i < n; i += 32) fused_write_peak(out, stg[i].o, stg[i].kk, stg[i].P, K);
+    for (unsigned i = threadIdx.x & 31; i < n; i += 32) peak_write(out, stg[i].o, stg[i].kk, stg[i].P, K);
     __syncwarp();
     if ((threadIdx.x & 31) == 0) { ctl->stg_n = 0u; ctl->ordered = 1u; }
     __syncwarp();
@@ -392,7 +379,7 @@ __device__ __forceinline__ void fused_emit(unsigned char *smem, const PeakOut ou
         fz_unlock(&ctl->stg_lock, lane);
         if (!ord) return;
     }
-    if (valid) fused_write_peak(out, o, kk, P, K);
+    if (valid) peak_write(out, o, kk, P, K);
 }
 
 // windows [start, start + cnt) are finished: mark their queue slots and advance scan_done over every finished slot
@@ -1136,12 +1123,7 @@ music4_fused_kernel(const float *__restrict__ in, const PlanarStreams S, unsigne
                     const double p = fused_exact_P(tab_c64, k, ev, pol_keep);
                     if (p > P) { P = p; kk = k; }  // k ascending per thread: strict '>' keeps the lower bin
                 }
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) {
-                    const double Po = __shfl_xor_sync(0xffffffffu, P, o);
-                    const int ko = __shfl_xor_sync(0xffffffffu, kk, o);
-                    if (peak_better(Po, ko, P, kk)) { P = Po; kk = ko; }
-                }
+                warp_argmax(P, kk);
                 if (lane == 0) { redP[swarp] = P; redk[swarp] = kk; }
                 bar_sync_scan();
                 if (st == 0) {

@@ -262,23 +262,8 @@ music8_fused_kernel(const __grid_constant__ CUtensorMap tm, const double *__rest
         for (int b = 0; b < F8_BATCH; ++b) {
             int kk = ps.bestk[b];
             double P = kk >= 0 ? 1.0 / ps.bestd[b] : 0.0;
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const double Po = __shfl_xor_sync(0xffffffffu, P, o);
-                const int ko = __shfl_xor_sync(0xffffffffu, kk, o);
-                if (peak_better(Po, ko, P, kk)) { P = Po; kk = ko; }
-            }
-            if (lane == b && b < nb) {
-                const size_t o = (size_t)wid[b];
-                if (kk >= 0) {
-                    out.angles[o] = (float)((double)kk * 360.0 / (double)K);  // reference :134, :153
-                    if (out.levels) out.levels[o] = (float)P;                 // reference :154
-                } else {
-                    out.angles[o] = 0.f;                                      // (0,0) initial pair, reference :95
-                    if (out.levels) out.levels[o] = 0.f;
-                }
-                peak_store_bin(out, o, kk);
-            }
+            warp_argmax(P, kk);
+            if (lane == b && b < nb) peak_write(out, (size_t)wid[b], kk, P, K);
         }
         __syncwarp();
         nb = 0;

@@ -26,6 +26,10 @@ __device__ __forceinline__ double warp_sum(double v)
     return v;
 }
 
+__device__ __forceinline__ double2 cmul(double2 a, double2 b) { return make_double2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
+// conj(a) b
+__device__ __forceinline__ double2 cjmul(double2 a, double2 b) { return make_double2(a.x * b.x + a.y * b.y, a.x * b.y - a.y * b.x); }
+
 __device__ __forceinline__ float4 ldg_stream(const float4 *p)
 {
     float4 r;
@@ -923,10 +927,11 @@ __global__ void prep_table_kernel(const float2 *__restrict__ tab, double *__rest
 // ------------------------------------------------------------------------------------------
 // K3: pseudospectrum scan.  One CTA per batch of SCAN_B windows; thread <-> angle bin within a
 // 256-bin table tile (its 2M+1 doubles live in registers), inner loop over the batch's windows
-// with the eigenvectors broadcast from shared memory.  Every bin is computed by the same
-// instruction sequence, so bit-equal table rows give bit-equal strengths (mirror ties).
+// with the eigenvectors (or the MVDR / Bartlett matrices) broadcast from shared memory.  Every
+// bin is computed by the same instruction sequence, so bit-equal table rows give bit-equal
+// strengths (mirror ties).
 //
-//   d_k = ||G^H a_k||^2 is evaluated through the signal-subspace complement
+//   MUSIC: d_k = ||G^H a_k||^2 is evaluated through the signal-subspace complement
 //         d = ||a||^2 - sum_s |e_s^H a|^2         (n < M-n: fewer flops)
 //   and recomputed in the direct noise-subspace form wherever d < 2^-7 ||a||^2 (near the
 //   peaks), so cancellation never costs more than ~2 digits.  P = 1.0 / d.
@@ -967,6 +972,35 @@ __device__ __forceinline__ bool peak_better(double Pa, int ka, double Pb, int kb
     return (Pa > Pb) || (Pa == Pb && ka >= 0 && (kb < 0 || ka < kb));
 }
 
+// (P, k) := the best of the warp's 32 candidates under peak_better, in every lane
+__device__ __forceinline__ void warp_argmax(double &P, int &k)
+{
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const double Po = __shfl_xor_sync(0xffffffffu, P, o);
+        const int ko = __shfl_xor_sync(0xffffffffu, k, o);
+        if (peak_better(Po, ko, P, k)) { P = Po; k = ko; }
+    }
+}
+
+// grid peak (bin k, level P) -> output slot o: angle k * 360 / K and the level (reference :134, :153-154), or the (0, 0)
+// initial pair (:95) with bin -1 when k < 0; the bin also goes to the peers' gather buffers
+__device__ __forceinline__ void peak_write(const PeakOut &out, const size_t o, const int k, const double P, const int K)
+{
+    if (k >= 0) {
+        out.angles[o] = (float)((double)k * 360.0 / (double)K);
+        if (out.levels) out.levels[o] = (float)P;
+    } else {
+        out.angles[o] = 0.f;
+        if (out.levels) out.levels[o] = 0.f;
+    }
+    peak_store_bin(out, o, k);
+}
+
+// The estimators (music_b200_set_estimator): the strength of the grid scan and the objective of the refinement
+// (music_estimators.cuh, music_refine.cuh)
+constexpr int EST_MUSIC = 0, EST_MVDR = 1, EST_BARTLETT = 2;
+
 template <int MT>
 __device__ __forceinline__ double strength_denominator(const double *ar, const double *ai, double na,
                                                        const double *sv, int M, int n, bool use_sig)
@@ -1004,10 +1038,22 @@ __device__ __forceinline__ double strength_denominator(const double *ar, const d
     return d;
 }
 
+// The quadratic forms of the MVDR and Bartlett strengths (music_estimators.cuh)
+template <int MT>
+__device__ __forceinline__ double mvdr_form(const double *ar, const double *ai, const double *g, int M);
+template <int MT>
+__device__ __forceinline__ double bartlett_form(const double *ar, const double *ai, const double *R, int M);
+
+// FORM (EST_*) picks the strength P[k] and what V holds per window (M*M complex doubles):
+//   EST_MUSIC     P = 1 / strength_denominator, V = the sorted eigenvectors (ws.Vt);
+//   EST_MVDR      P = 1 / mvdr_form,            V = the g_j of mvdr_prep_kernel (ws.Vt);
+//   EST_BARTLETT  P = bartlett_form / ||a||^4,  V = R (ws.R).
 // COUNTS (counts != nullptr, music_sources.cuh): window w has counts[w] <= n sources, so its noise subspace is the
-// M - counts[w] smallest-eigenvalue vectors; with ARGMAX (n == 1) a window with count 0 reports no peak.
-template <int MT, bool ARGMAX, bool WRITE_P64, bool WRITE_SPEC, bool COUNTS = false>
-__global__ void __launch_bounds__(TILE) scan_kernel(const double *__restrict__ soa, const double *__restrict__ Vt,
+// M - counts[w] smallest-eigenvalue vectors; with ARGMAX (n == 1) a window with count 0 reports no peak.  The MVDR and
+// Bartlett spectra do not depend on the count: they run with COUNTS = false and read counts (may be null) for the
+// count-0 rule only.
+template <int MT, int FORM, bool ARGMAX, bool WRITE_P64, bool WRITE_SPEC, bool COUNTS = false>
+__global__ void __launch_bounds__(TILE) scan_kernel(const double *__restrict__ soa, const double *__restrict__ V,
                                                     int Mrt, int n, int K, int W, PeakOut out,
                                                     float *__restrict__ spectrum, double *__restrict__ P64,
                                                     const int32_t *__restrict__ counts)
@@ -1021,7 +1067,7 @@ __global__ void __launch_bounds__(TILE) scan_kernel(const double *__restrict__ s
     const int w0 = blockIdx.x * SCAN_B;
     const int nb = min(SCAN_B, W - w0);
     const int vsz = M * M * 2;
-    for (int i = threadIdx.x; i < nb * vsz; i += blockDim.x) sV[i] = Vt[(size_t)w0 * vsz + i];
+    for (int i = threadIdx.x; i < nb * vsz; i += blockDim.x) sV[i] = V[(size_t)w0 * vsz + i];
     if (COUNTS && threadIdx.x < nb) {
         const int c = counts[w0 + threadIdx.x];
         sn[threadIdx.x] = c;
@@ -1035,8 +1081,8 @@ __global__ void __launch_bounds__(TILE) scan_kernel(const double *__restrict__ s
     // exactly "P_new > P_best" (the reference's strict '>' on strengths, :132): a candidate that
     // is smaller by more than 2^-50 relative has a strictly larger reciprocal; inside that sliver
     // the two reciprocals are compared.  d is never negative (direct form is a sum of squares,
-    // complement form is only kept above 2^-7 ||a||^2), NaN fails `d < best`.
-    constexpr bool FAST = ARGMAX && !WRITE_P64 && !WRITE_SPEC;
+    // complement form is only kept above 2^-7 ||a||^2), NaN fails `d < best`.  MUSIC only.
+    constexpr bool FAST = FORM == EST_MUSIC && ARGMAX && !WRITE_P64 && !WRITE_SPEC;
     double best[SCAN_B];  // FAST: min d; otherwise: max P
     int bestk[SCAN_B];
 #pragma unroll
@@ -1058,7 +1104,8 @@ __global__ void __launch_bounds__(TILE) scan_kernel(const double *__restrict__ s
 #pragma unroll
             for (int b = 0; b < SCAN_B; ++b) {
                 if (b < nb) {
-                    const double d = strength_denominator<MT>(ar, ai, na, sV + b * vsz, M, COUNTS ? sn[b] : n, COUNTS ? ssig[b] : use_sig);
+                    const double *v = sV + b * vsz;
+                    const double d = FORM == EST_MUSIC ? strength_denominator<MT>(ar, ai, na, v, M, COUNTS ? sn[b] : n, COUNTS ? ssig[b] : use_sig) : 0.0;
                     if (FAST) {
                         if (d < best[b]) {
                             if (d < best[b] * 0.99999999999999911182 /* 1 - 2^-50 */ || 1.0 / d > 1.0 / best[b]) {
@@ -1067,7 +1114,9 @@ __global__ void __launch_bounds__(TILE) scan_kernel(const double *__restrict__ s
                             }
                         }
                     } else {
-                        const double P = 1.0 / d;
+                        const double P = FORM == EST_MVDR       ? 1.0 / mvdr_form<MT>(ar, ai, v, M)
+                                         : FORM == EST_BARTLETT ? bartlett_form<MT>(ar, ai, v, M) / (na * na)
+                                                                : 1.0 / d;
                         if (WRITE_SPEC) spectrum[(size_t)(w0 + b) * K + k] = (float)P;
                         if (WRITE_P64) P64[(size_t)(w0 + b) * K + k] = P;
                         if (ARGMAX) {
@@ -1086,12 +1135,7 @@ __global__ void __launch_bounds__(TILE) scan_kernel(const double *__restrict__ s
         for (int b = 0; b < SCAN_B; ++b) {
             int kk = bestk[b];
             double P = FAST ? (kk >= 0 ? 1.0 / best[b] : 0.0) : best[b];
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const double Po = __shfl_xor_sync(0xffffffffu, P, o);
-                const int ko = __shfl_xor_sync(0xffffffffu, kk, o);
-                if (peak_better(Po, ko, P, kk)) { P = Po; kk = ko; }
-            }
+            warp_argmax(P, kk);
             if (lane == 0) { rP[b][wid] = P; rk[b][wid] = kk; }
         }
         __syncthreads();
@@ -1102,15 +1146,8 @@ __global__ void __launch_bounds__(TILE) scan_kernel(const double *__restrict__ s
             for (int q = 1; q < TILE / 32; ++q)
                 if (peak_better(rP[b][q], rk[b][q], P, kk)) { P = rP[b][q]; kk = rk[b][q]; }
             const size_t o = (size_t)(w0 + b);  // n == 1
-            if (COUNTS && sn[b] == 0) kk = -1;
-            if (kk >= 0) {
-                out.angles[o] = (float)((double)kk * 360.0 / (double)K);  // :134, :153
-                if (out.levels) out.levels[o] = (float)P;                 // :154
-            } else {
-                out.angles[o] = 0.f;                                      // (0,0) initial pair, :95
-                if (out.levels) out.levels[o] = 0.f;
-            }
-            peak_store_bin(out, o, kk);
+            if (COUNTS ? sn[b] == 0 : FORM != EST_MUSIC && counts && counts[o] == 0) kk = -1;
+            peak_write(out, o, kk, P, K);
         }
     }
 }
@@ -1301,12 +1338,7 @@ __global__ void __launch_bounds__(TILE, 3) scan_peak1_kernel(const double *__res
     for (int b = 0; b < SCAN_WPT; ++b) {
         int kk = ps.bestk[b];
         double P = kk >= 0 ? 1.0 / ps.bestd[b] : 0.0;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const double Po = __shfl_xor_sync(0xffffffffu, P, o);
-            const int ko = __shfl_xor_sync(0xffffffffu, kk, o);
-            if (peak_better(Po, ko, P, kk)) { P = Po; kk = ko; }
-        }
+        warp_argmax(P, kk);
         if (lane == 0) { rP[g * SCAN_WPT + b][wig] = P; rk[g * SCAN_WPT + b][wig] = kk; }
     }
     __syncthreads();
@@ -1318,14 +1350,7 @@ __global__ void __launch_bounds__(TILE, 3) scan_peak1_kernel(const double *__res
             if (peak_better(rP[b][q], rk[b][q], P, kk)) { P = rP[b][q]; kk = rk[b][q]; }
         const size_t o = (size_t)(w0 + b);
         if (counts && counts[o] == 0) kk = -1;
-        if (kk >= 0) {
-            out.angles[o] = (float)((double)kk * 360.0 / (double)K);  // :134, :153
-            if (out.levels) out.levels[o] = (float)P;                 // :154
-        } else {
-            out.angles[o] = 0.f;                                      // (0,0) initial pair, :95
-            if (out.levels) out.levels[o] = 0.f;
-        }
-        peak_store_bin(out, o, kk);
+        peak_write(out, o, kk, P, K);
     }
 }
 
@@ -1352,24 +1377,9 @@ __global__ void __launch_bounds__(256) topn_kernel(const double *__restrict__ P6
                 const bool after = first || (p < prevP) || (p == prevP && k > prevk);
                 if (after && p > 0.0 && p > bP) { bP = p; bk = k; }
             }
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const double Po = __shfl_xor_sync(0xffffffffu, bP, o);
-                const int ko = __shfl_xor_sync(0xffffffffu, bk, o);
-                if (peak_better(Po, ko, bP, bk)) { bP = Po; bk = ko; }
-            }
+            warp_argmax(bP, bk);
         }
-        if (lane == 0) {
-            const size_t o = (size_t)w * n + r;
-            if (bk >= 0) {
-                out.angles[o] = (float)((double)bk * 360.0 / (double)K);
-                if (out.levels) out.levels[o] = (float)bP;
-            } else {
-                out.angles[o] = 0.f;
-                if (out.levels) out.levels[o] = 0.f;
-            }
-            peak_store_bin(out, o, bk);
-        }
+        if (lane == 0) peak_write(out, (size_t)w * n + r, bk, bP, K);
         first = false;
         prevP = bP;
         prevk = bk;
@@ -1411,24 +1421,11 @@ __global__ void __launch_bounds__(256) topn_local_kernel(const double *__restric
             }
         }
         __syncwarp();  // lanes leave the k loop after different trip counts
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const double Po = __shfl_xor_sync(0xffffffffu, bP, o);
-            const int ko = __shfl_xor_sync(0xffffffffu, bk, o);
-            if (peak_better(Po, ko, bP, bk)) { bP = Po; bk = ko; }
-        }
+        warp_argmax(bP, bk);
         if (bk < 0) dry = true;
         if (lane == 0) {
             if (r < MAXM) taken[r] = bk;
-            const size_t o = (size_t)w * n + r;
-            if (bk >= 0) {
-                out.angles[o] = (float)((double)bk * 360.0 / (double)K);
-                if (out.levels) out.levels[o] = (float)bP;
-            } else {
-                out.angles[o] = 0.f;
-                if (out.levels) out.levels[o] = 0.f;
-            }
-            peak_store_bin(out, o, bk);
+            peak_write(out, (size_t)w * n + r, bk, bP, K);
         }
         __syncwarp();
     }

@@ -79,7 +79,6 @@ __device__ __noinline__ void refine_eval(const RefineGeom &geo, const double2 *_
 //   EST_MUSIC     D = sum_j |g_j^H a|^2 over the p noise eigenvectors, level 1 / D;
 //   EST_MVDR      the same D over p = M vectors g_j = conj(row j of L^-1), i.e. a^H R_L^-1 a, level 1 / D;
 //   EST_BARTLETT  D = F = -a^H R a (maximising B = a^H R a is minimising F), level -F / M^2 (||a||^2 = M).
-constexpr int EST_MUSIC = 0, EST_MVDR = 1, EST_BARTLETT = 2;
 
 // F = -B, F', F'' with B(theta) = a^H R a for the window's covariance R[i][j] (row i contiguous):
 //   B' = 2 Re(a'^H R a),  B'' = 2 (a'^H R a' + Re(a''^H R a)),  a' = -j psi a,  a'' = (j phi - psi^2) a.

@@ -28,7 +28,6 @@ constexpr double ROOTS_EPS = 2.220446049250313e-16;  // 2^-52
 constexpr double ROOTS_STOP = 4.0 * ROOTS_EPS;        // stop once every correction is <= 4 ulps of |z|
 constexpr double ROOTS_MERGE = 1e-6;                  // two roots this close (relative) are one double root
 
-__device__ __forceinline__ double2 cmul(double2 a, double2 b) { return make_double2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
 __device__ __forceinline__ double2 cdiv(double2 a, double2 b)
 {
     const double r = 1.0 / (b.x * b.x + b.y * b.y);
@@ -181,12 +180,7 @@ __global__ void __launch_bounds__(ROOTS_WARPS * 32) roots_kernel(const double *_
         refine_eval(geo, G, M, p, tdeg * STEER_DEG2RAD, &D, &D1, &D2);
         ula_store_slot(out, o, tdeg, D, K);
     }
-    if (lane >= f && lane < n) {
-        const size_t o = (size_t)w * n + lane;
-        out.angles[o] = 0.f;
-        if (out.levels) out.levels[o] = 0.f;
-        peak_store_bin(out, o, -1);
-    }
+    if (lane >= f && lane < n) peak_write(out, (size_t)w * n + lane, -1, 0.0, K);
 }
 
 }  // namespace music

@@ -63,9 +63,9 @@ PATHS = {
     "topn16":        (16, 3, 256, 4, {}),
     "local4":        (4, 2, 256, 4, {"peak": "local"}),                    # + topn_local_kernel
     "local8":        (8, 1, 256, 4, {"peak": "local"}),
-    "mvdr":          (4, 1, 256, 3, {"est": ("mvdr", 0.0), "p64": True}),  # cov, mvdr_prep, scan_quad<4>
+    "mvdr":          (4, 1, 256, 3, {"est": ("mvdr", 0.0), "p64": True}),  # cov, mvdr_prep, scan<4, MVDR>
     "mvdr_loaded":   (8, 2, 256, 4, {"est": ("mvdr", 0.01), "p64": True}), # + topn_kernel
-    "bartlett":      (4, 2, 256, 3, {"est": ("bartlett", 0.0), "p64": True}),  # cov, scan_quad<4>, topn_kernel
+    "bartlett":      (4, 2, 256, 3, {"est": ("bartlett", 0.0), "p64": True}),  # cov, scan<4, BARTLETT>, topn_kernel
     "mdl":           (4, 2, 256, 5, {"rule": "mdl", "p64": True}),         # cov, eig, source count, scan, top-n
 }
 
