@@ -96,6 +96,12 @@ def load():
         L.music_b200_process_device_counts.argtypes = [vp, fp, u32, fp, fp, fp, fp, fp, vp]
         L.music_b200_process_device_counts.restype = ctypes.c_int
         dbl = ctypes.c_double
+        L.music_b200_set_beamformer.argtypes = [vp, ctypes.c_int, ctypes.c_double]
+        L.music_b200_set_beamformer.restype = ctypes.c_int
+        L.music_b200_process_device_beams.argtypes = [vp, fp, u32, fp, fp, fp, fp, fp, fp, fp, vp]
+        L.music_b200_process_device_beams.restype = ctypes.c_int
+        L.music_b200_process_host_beams.argtypes = [vp, fp, u32, fp, fp, fp, fp, fp, fp, fp]
+        L.music_b200_process_host_beams.restype = ctypes.c_int
         L.music_b200_create_azel.argtypes = [ctypes.POINTER(vp), u32, u32, u32, u32, u32, dbl, dbl, fp, dbl, ctypes.c_int]
         L.music_b200_create_azel.restype = ctypes.c_int
         L.music_b200_set_geometry_azel.argtypes = [vp, fp, dbl]
@@ -134,6 +140,7 @@ EXPORTS = [
     "music_b200_set_stage_timing", "music_b200_get_stage_times", "music_b200_debug_fused_trace", "music_b200_debug_fused8_stats",
     "music_b200_last_error", "music_b200_destroy",
     "music_b200_create_azel", "music_b200_set_geometry_azel", "music_b200_process_azel_host", "music_b200_process_azel_device",
+    "music_b200_set_beamformer", "music_b200_process_device_beams", "music_b200_process_host_beams",
 ]
 
 

@@ -35,6 +35,7 @@
 #include "music_roots.cuh"
 #include "music_esprit.cuh"
 #include "music_dml.cuh"
+#include "music_beams.cuh"
 
 using namespace music;
 
@@ -58,8 +59,9 @@ struct DeviceTable {
 struct Workspace {
     double *R = nullptr, *ev = nullptr, *Vt = nullptr, *P64 = nullptr;
     int32_t *cnt = nullptr;  // per-window source counts (source rule other than FIXED)
-    int32_t *bins = nullptr; // [cap][n] peak bins for the refinement when the caller asked for none
-    uint32_t cap = 0, p64_cap = 0, cnt_cap = 0, bins_cap = 0;
+    int32_t *bins = nullptr; // [cap][n] peak bins for the refinement and the beams when the caller asked for none
+    double *wts = nullptr;   // [cap][n][m] complex beam weights when a beams call asked for none
+    uint32_t cap = 0, p64_cap = 0, cnt_cap = 0, bins_cap = 0, wts_cap = 0;
     cudaEvent_t scan_done = nullptr;
     bool used = false;
 };
@@ -92,8 +94,10 @@ struct Outputs {
     double *P64 = nullptr;      // [W][K]
     double *R = nullptr;        // [W][m][m] complex
     double *ev = nullptr;       // [W][m]
+    double *wts = nullptr;      // [W][n][m] complex beam weights: beams entry points only
+    float *beams = nullptr;     // [W][n][N] complex64 beams: beams entry points only
     Gather gather;
-    uint32_t n = 0, K = 0, m = 0;
+    uint32_t n = 0, K = 0, m = 0, N = 0;
 
     // the shape of h's calls and the all-gather h was attached to (music_b200_gather_attach)
     Outputs &shaped(const music_b200 *h);
@@ -112,6 +116,8 @@ struct Outputs {
         skip(o.P64, K);
         skip(o.R, (size_t)m * m * 2);
         skip(o.ev, m);
+        skip(o.wts, (size_t)n * m * 2);
+        skip(o.beams, (size_t)n * N * 2);
         for (int p = 0; p < gather.G; ++p) skip(o.gather.peer[p], (size_t)gather.G * n);
         return o;
     }
@@ -119,6 +125,13 @@ struct Outputs {
     // the per-window outputs a host call stages through pinned memory (4-byte elements), with their elements per window
     struct Field { void *p; uint32_t per_win; };
     std::array<Field, 5> window_fields() const { return {{{angles, n}, {elev, n}, {levels, n}, {bins, n}, {counts, 1}}}; }
+
+    // the rows of a beams call a host call stages through pinned memory, with their bytes per window
+    struct Row { void *p; size_t bytes; };
+    std::array<Row, 2> row_fields() const
+    {
+        return {{{wts, (size_t)n * m * 2 * sizeof(double)}, {beams, (size_t)n * N * 2 * sizeof(float)}}};
+    }
 };
 
 // One staging stream of the host entry points: the input and output buffers of a chunk, and which windows of the call
@@ -127,7 +140,7 @@ struct Outputs {
 struct HostSlot {
     float *in = nullptr;
     Outputs dev;   // device outputs (the spectrum only when a call asked for it)
-    Outputs pin;   // pinned host mirrors of dev's per-window outputs
+    Outputs pin;   // pinned host mirrors of dev's per-window outputs and of its beam and weight rows
     uint32_t w0 = 0, W = 0;  // W = 0: nothing pending
 };
 
@@ -150,6 +163,8 @@ struct music_b200 {
     float *steer_vals = nullptr;
     Modes modes;
     int source_rule = MUSIC_B200_SOURCES_FIXED;  // set_source_rule()
+    int beam_rule = MUSIC_B200_BEAMS_OFF;        // set_beamformer(): read by the beams entry points only
+    double beam_loading = 0.0;
     unsigned steer_guarded = 0;    // entries of the last built table re-evaluated with the host libm
     bool azel = false;             // music_b200_create_azel(): K = n_az * n_el rows, elevation-major (music_azel.cuh)
     AzelGrid grid = {};
@@ -179,6 +194,7 @@ struct music_b200 {
     HostSlot stage[2];
     uint32_t host_chunk = 0;
     bool host_spec_alloc = false;
+    bool host_beam_alloc = false;      // the staging slots hold beam and weight rows
     cudaStream_t last_fused_stream[2] = {nullptr, nullptr};  // per ticket counter: launches on one stream need no event
 
     // caller memory registered for DMA (cudaHostRegister), newest last: GNU Radio hands work() the same pageable
@@ -207,6 +223,7 @@ Outputs &Outputs::shaped(const music_b200 *h)
     n = h->n;
     K = h->K;
     m = h->m;
+    N = h->N;
     gather = h->gather;
     return *this;
 }
@@ -486,7 +503,8 @@ struct Plan {
     int est = MUSIC_B200_ESTIMATOR_MUSIC;            // the form of scan_kernel and the refined objective
     Peaks peaks = Peaks::None;
     bool decode = false, refine = false;             // az-el bin decode; peak refinement (the az-el kind after a decode)
-    bool ws_p64 = false, ws_counts = false, ws_bins = false;  // workspace buffers the kernels write
+    bool beams = false;                              // beam weights (+ beams) after the peaks: the beams entry points
+    bool ws_p64 = false, ws_counts = false, ws_bins = false, ws_wts = false;  // workspace buffers the kernels write
 };
 
 Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *planar, unsigned hop)
@@ -503,8 +521,10 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
     // kernel when the 16-byte granularity of its bulk copies allows it.
     bool planar_fusable = !planar || (hop % 2 == 0 && h->N % 2 == 0);
     for (uint32_t r = 0; planar && r < h->m; ++r) planar_fusable = planar_fusable && (reinterpret_cast<uintptr_t>(planar->p[r]) & 15u) == 0;
+    // A beams call needs R, which the fused kernels keep in registers: it runs the unfused plan of a call that asks for R.
+    const bool beams = o.wts || o.beams;
     const bool fusable = h->fused && !h->azel && music_est && fixed_n && md.refine == MUSIC_B200_REFINE_OFF &&
-                         md.peak == MUSIC_B200_PEAKS_TOP_BINS && h->n == 1 && !o.P64 && !o.R && !o.ev;
+                         md.peak == MUSIC_B200_PEAKS_TOP_BINS && h->n == 1 && !o.P64 && !o.R && !o.ev && !beams;
     if (fusable && h->m == 4 && planar_fusable && (!o.spec || h->fused_spec)) p.path = Path::Fused4;
     else if (fusable && h->m == 8 && !planar && !o.spec && h->N >= 128 && h->N % 2 == 0) p.path = Path::Fused8;
 
@@ -533,7 +553,9 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
     p.refine = md.refine != MUSIC_B200_REFINE_OFF;
     p.ws_p64 = p.p64 && !o.P64;
     p.ws_counts = p.count;
-    p.ws_bins = p.decode || p.refine;
+    p.beams = beams;
+    p.ws_bins = p.decode || p.refine || (beams && !o.bins);
+    p.ws_wts = beams && !o.wts;
     return p;
 }
 
@@ -541,7 +563,8 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
 uint32_t max_sub_windows(const music_b200 *h, const Plan &p)
 {
     const size_t per_win = (size_t)h->m * h->m * 2 * 8 * 2 + h->m * 8 + (p.ws_p64 ? (size_t)h->K * 8 : 0) +
-                           (p.ws_counts ? sizeof(int32_t) : 0) + (p.ws_bins ? h->n * sizeof(int32_t) : 0);
+                           (p.ws_counts ? sizeof(int32_t) : 0) + (p.ws_bins ? h->n * sizeof(int32_t) : 0) +
+                           (p.ws_wts ? (size_t)h->n * h->m * 2 * sizeof(double) : 0);
     size_t c = ((size_t)384 << 20) / per_win;
     c = std::max<size_t>(SCAN_B, std::min<size_t>(c, 1u << 20));
     return (uint32_t)(c / SCAN_B * SCAN_B);
@@ -577,6 +600,12 @@ int ensure_slot(music_b200 *h, Workspace &ws, uint32_t windows, const Plan &p)
         cudaFree(ws.bins); ws.bins = nullptr; ws.bins_cap = 0;
         CU(h, cudaMalloc(&ws.bins, (size_t)windows * h->n * sizeof(int32_t)));
         ws.bins_cap = windows;
+    }
+    if (p.ws_wts && windows > ws.wts_cap) {
+        if (ws.used) CU(h, cudaEventSynchronize(ws.scan_done));
+        cudaFree(ws.wts); ws.wts = nullptr; ws.wts_cap = 0;
+        CU(h, cudaMalloc(&ws.wts, (size_t)windows * h->n * h->m * 2 * sizeof(double)));
+        ws.wts_cap = windows;
     }
     return MUSIC_B200_OK;
 }
@@ -796,11 +825,34 @@ __global__ void gather_wait_kernel(const unsigned *flags, int npeer, unsigned ep
     }
 }
 
+// The beam weights of W windows from ws.R, the angles and bins po holds, into o.wts (or the workspace), then the beams
+// of the W windows at d_in into o.beams when the caller asked for them (music_beams.cuh).
+void launch_beams(music_b200 *h, const Workspace &ws, uint32_t W, const Outputs &o, const PeakOut &po, const float *d_in, cudaStream_t st)
+{
+    const DeviceTable &tb = h->table[h->cur_table];
+    const int M = (int)h->m, n = (int)h->n, N = (int)h->N;
+    double *wts = o.wts ? o.wts : ws.wts;
+    beam_weights_kernel<<<(W + BEAM_WARPS - 1) / BEAM_WARPS, BEAM_WARPS * 32, 0, st>>>(
+        ws.R, po.angles, po.bins, reinterpret_cast<const float2 *>(tb.c64), M, n, (int)W, h->beam_rule, h->beam_loading, tb.geometric,
+        tb.geo, wts);
+    h->launches++;
+    if (!o.beams) return;
+    const int spans = (N + BEAM_SPAN - 1) / BEAM_SPAN;
+    const size_t smem = beam_apply_smem(M, n);
+    with_scan_m(h->m, [&](auto mt) {
+        constexpr int MT = decltype(mt)::value;
+        beam_apply_kernel<MT><<<(unsigned)((size_t)W * spans), BEAM_SPAN, smem, st>>>(d_in, wts, M, n, N, spans, o.beams);
+    });
+    h->launches++;
+}
+
 // K2 (+ source count) + K3 (+ peak rule) of W windows from ws.R into the outputs o (of these W windows), on `st`, as
 // planned.  tev (optional) = timing events [1..4].  An az-el handle's peak bins are decoded into (azimuth, elevation)
 // after the peak rule.  With refinement on, the refine kernel follows (timed with the peak rule) and reads the bins
-// written before it: from the caller's array, or from the workspace when the caller asked for none.
-int launch_eig_scan(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t W, const Outputs &o, cudaStream_t st, cudaEvent_t *tev)
+// written before it: from the caller's array, or from the workspace when the caller asked for none.  A beams call
+// then forms the weights and beams of the windows at d_in (timed with the peak rule as well).
+int launch_eig_scan(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t W, const Outputs &o, cudaStream_t st, cudaEvent_t *tev,
+                    const float *d_in = nullptr)
 {
     const int M = (int)h->m;
     const DeviceTable &tb = h->table[h->cur_table];
@@ -881,6 +933,7 @@ int launch_eig_scan(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t 
 #undef REFINE_CASE
         h->launches++;
     }
+    if (p.beams) launch_beams(h, ws, W, o, po, d_in, st);
     if (tev) cudaEventRecord(tev[4], st);
     if (o.R)
         CU(h, cudaMemcpyAsync(o.R, ws.R, (size_t)W * M * M * 2 * sizeof(double), cudaMemcpyDeviceToDevice, st));
@@ -999,7 +1052,7 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, const Ou
         if (planar) launch_cov_planar(h, ws, *planar, (unsigned long long)w0 * hop, hop, W, st);
         else launch_cov(h, ws, d_in + (size_t)w0 * h->nsamples * 2, W, st, slot);
         if (tev) cudaEventRecord(tev[1], st);
-        rc = launch_eig_scan(h, plan, ws, W, out.at(w0), st, tev);
+        rc = launch_eig_scan(h, plan, ws, W, out.at(w0), st, tev, planar ? nullptr : d_in + (size_t)w0 * h->nsamples * 2);
         if (rc) return rc;
         CU(h, cudaEventRecord(ws.scan_done, st));
         ws.used = true;
@@ -1065,6 +1118,10 @@ void free_host_staging(music_b200 *h)
     for (HostSlot &sl : h->stage) {
         cudaFree(sl.in);
         cudaFree(sl.dev.spec);
+        cudaFree(sl.dev.wts);
+        cudaFree(sl.dev.beams);
+        cudaFreeHost(sl.pin.wts);
+        cudaFreeHost(sl.pin.beams);
         const auto dev = sl.dev.window_fields(), pin = sl.pin.window_fields();
         for (size_t f = 0; f < dev.size(); ++f) {
             cudaFree(dev[f].p);
@@ -1074,11 +1131,14 @@ void free_host_staging(music_b200 *h)
     }
     h->host_chunk = 0;
     h->host_spec_alloc = false;
+    h->host_beam_alloc = false;
 }
 
-int ensure_host_staging(music_b200 *h, uint32_t chunk, bool spec)
+int ensure_host_staging(music_b200 *h, uint32_t chunk, bool spec, bool beams)
 {
-    if (chunk <= h->host_chunk && (!spec || h->host_spec_alloc)) return MUSIC_B200_OK;
+    if (chunk <= h->host_chunk && (!spec || h->host_spec_alloc) && (!beams || h->host_beam_alloc)) return MUSIC_B200_OK;
+    spec = spec || h->host_spec_alloc;
+    beams = beams || h->host_beam_alloc;
     const uint32_t cap = std::max(chunk, h->host_chunk);
     free_host_staging(h);
     const size_t wn = (size_t)cap * h->n;
@@ -1095,6 +1155,12 @@ int ensure_host_staging(music_b200 *h, uint32_t chunk, bool spec)
         CU(h, cudaMalloc(&sl.dev.counts, (size_t)cap * sizeof(int32_t)));
         CU(h, cudaHostAlloc(&sl.pin.counts, (size_t)cap * sizeof(int32_t), cudaHostAllocDefault));
         if (spec) CU(h, cudaMalloc(&sl.dev.spec, (size_t)cap * h->K * sizeof(float)));
+        if (beams) {
+            CU(h, cudaMalloc(&sl.dev.wts, wn * h->m * 2 * sizeof(double)));
+            CU(h, cudaMalloc(&sl.dev.beams, wn * h->N * 2 * sizeof(float)));
+            CU(h, cudaHostAlloc(&sl.pin.wts, wn * h->m * 2 * sizeof(double), cudaHostAllocDefault));
+            CU(h, cudaHostAlloc(&sl.pin.beams, wn * h->N * 2 * sizeof(float), cudaHostAllocDefault));
+        }
         if (h->azel) {
             CU(h, cudaMalloc(&sl.dev.elev, wn * sizeof(float)));
             CU(h, cudaHostAlloc(&sl.pin.elev, wn * sizeof(float), cudaHostAllocDefault));
@@ -1102,6 +1168,7 @@ int ensure_host_staging(music_b200 *h, uint32_t chunk, bool spec)
     }
     h->host_chunk = cap;
     h->host_spec_alloc = spec;
+    h->host_beam_alloc = beams;
     return MUSIC_B200_OK;
 }
 
@@ -1123,6 +1190,18 @@ void flush_host_slot(music_b200 *h, int s, const Outputs &dst, uint32_t G, uint3
             for (uint32_t i = 0; i < sl.W; ++i) memcpy(d + ((size_t)(sl.w0 + i) * G + g) * row, src + i * row, row);
         }
     }
+    const auto rfrom = sl.pin.row_fields(), rto = dst.row_fields();
+    for (size_t f = 0; f < rto.size(); ++f) {
+        if (!rto[f].p) continue;
+        const size_t row = rto[f].bytes;
+        char *d = static_cast<char *>(rto[f].p);
+        const char *src = static_cast<const char *>(rfrom[f].p);
+        if (G == 1) {
+            memcpy(d + sl.w0 * row, src, sl.W * row);
+        } else {
+            for (uint32_t i = 0; i < sl.W; ++i) memcpy(d + ((size_t)(sl.w0 + i) * G + g) * row, src + i * row, row);
+        }
+    }
     sl.W = 0;
 }
 
@@ -1133,6 +1212,9 @@ int download_host_slot(music_b200 *h, int s, uint32_t w0, uint32_t W, const Outp
     const auto want = dst.window_fields(), from = sl.dev.window_fields(), to = sl.pin.window_fields();
     for (size_t f = 0; f < want.size(); ++f)
         if (want[f].p) CU(h, cudaMemcpyAsync(to[f].p, from[f].p, (size_t)W * want[f].per_win * sizeof(float), cudaMemcpyDeviceToHost, st));
+    const auto rwant = dst.row_fields(), rfrom = sl.dev.row_fields(), rto = sl.pin.row_fields();
+    for (size_t f = 0; f < rwant.size(); ++f)
+        if (rwant[f].p) CU(h, cudaMemcpyAsync(rto[f].p, rfrom[f].p, (size_t)W * rwant[f].bytes, cudaMemcpyDeviceToHost, st));
     sl.w0 = w0;
     sl.W = W;
     return MUSIC_B200_OK;
@@ -1169,9 +1251,12 @@ int stage_host(music_b200 *h, const HostInput &in, uint32_t nwindows, const Outp
     const size_t N = h->N, win_bytes = (size_t)h->nsamples * 2 * sizeof(float);
     const uint32_t per_lane = (nwindows + G - 1) / G;
     // chunk: ~32 MiB of input per copy, so that H2D of chunk i+1 overlaps compute of chunk i (with the spectrum port
-    // connected a window also returns K floats: bound the chunk by the larger of the two), and at most half the call
-    // while a chunk still fills whole scan CTAs
-    const size_t per_win = std::max(win_bytes, dst.spec ? (size_t)h->K * sizeof(float) : (size_t)0);
+    // connected a window also returns K floats, with beams n * N complex64 and n * m complex fp64: bound the chunk by
+    // the larger of the input and the output), and at most half the call while a chunk still fills whole scan CTAs
+    const size_t out_bytes = (dst.spec ? (size_t)h->K * sizeof(float) : 0) + (dst.beams ? (size_t)h->n * N * 2 * sizeof(float) : 0) +
+                             (dst.wts ? (size_t)h->n * h->m * 2 * sizeof(double) : 0);
+    const size_t per_win = std::max(win_bytes, out_bytes);
+    const bool beams = dst.beams || dst.wts;
     const uint32_t base = (uint32_t)std::max<size_t>(SCAN_B, ((size_t)32 << 20) / per_win);
     const uint32_t half = (per_lane + 1) / 2 > SCAN_B ? (per_lane + 1) / 2 : per_lane;
     // Staging holds `host_chunk` windows of m * N samples per slot.  Planar, a chunk of C windows needs m * ((C - 1) *
@@ -1182,7 +1267,7 @@ int stage_host(music_b200 *h, const HostInput &in, uint32_t nwindows, const Outp
         music_b200 *c = lanes[l];
         if (cudaSetDevice(c->device) != cudaSuccess) { rc = fail(h, MUSIC_B200_ECUDA, "cudaSetDevice(%d) failed", c->device); break; }
         c->stage[0].W = c->stage[1].W = 0;  // nothing pending from an earlier (possibly failed) call
-        rc = ensure_host_staging(c, staged, dst.spec != nullptr);
+        rc = ensure_host_staging(c, staged, dst.spec != nullptr, beams);
         if (rc && c != h) fail(h, rc, "%s", std::string(c->error).c_str());
     }
     const size_t cap = lanes[0]->host_chunk;
@@ -1225,6 +1310,8 @@ int stage_host(music_b200 *h, const HostInput &in, uint32_t nwindows, const Outp
                 o.gather = c->gather;
                 if (!dst.spec) o.spec = nullptr;
                 if (!dst.counts) o.counts = nullptr;
+                if (!dst.wts) o.wts = nullptr;
+                if (!dst.beams) o.beams = nullptr;
                 rc = enqueue_device(c, in.streams ? nullptr : sl.in, W, o, st, s, in.streams ? &S : nullptr, in.hop);
                 if (rc && c != h) fail(h, rc, "%s", std::string(c->error).c_str());
                 if (rc) break;
@@ -1750,6 +1837,64 @@ int music_b200_process_host_counts(music_b200 *h, const float *in_c64, uint32_t 
     return process_host_impl(h, in_c64, nwindows, o);
 }
 
+namespace {
+
+// the checks every beams entry point makes before it runs: a beamformer set, an output asked for, the alignment
+int check_beams_call(music_b200 *h, const void *weights, const void *beams)
+{
+    if (h->beam_rule == MUSIC_B200_BEAMS_OFF)
+        return fail(h, MUSIC_B200_EINVAL, "no beamformer set (call music_b200_set_beamformer() with DAS, MVDR or LCMV)");
+    if (!weights && !beams) return fail(h, MUSIC_B200_EINVAL, "weights and beams must not both be NULL");
+    if ((reinterpret_cast<uintptr_t>(beams) & 7u) != 0) return fail(h, MUSIC_B200_EINVAL, "beams must be 8-byte aligned");
+    if ((reinterpret_cast<uintptr_t>(weights) & 15u) != 0) return fail(h, MUSIC_B200_EINVAL, "weights must be 16-byte aligned");
+    return MUSIC_B200_OK;
+}
+
+}  // namespace
+
+int music_b200_set_beamformer(music_b200 *h, int rule, double loading)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (h->azel) return fail(h, MUSIC_B200_EINVAL, "the beamformer is not supported on an az-el handle");
+    if (rule != MUSIC_B200_BEAMS_OFF && rule != MUSIC_B200_BEAMS_DAS && rule != MUSIC_B200_BEAMS_MVDR && rule != MUSIC_B200_BEAMS_LCMV)
+        return fail(h, MUSIC_B200_EINVAL, "unknown beamformer %d", rule);
+    if (!std::isfinite(loading) || loading < 0.0) return fail(h, MUSIC_B200_EINVAL, "loading must be finite and >= 0 (got %g)", loading);
+    if (loading != 0.0 && (rule == MUSIC_B200_BEAMS_OFF || rule == MUSIC_B200_BEAMS_DAS))
+        return fail(h, MUSIC_B200_EINVAL, "diagonal loading applies to MVDR and LCMV beams only (got %g)", loading);
+    if ((rule == MUSIC_B200_BEAMS_MVDR || rule == MUSIC_B200_BEAMS_LCMV) && loading == 0.0 && h->N <= h->m)
+        return fail(h, MUSIC_B200_EINVAL, "MVDR and LCMV beams without diagonal loading need more snapshots than antennas (N = %u, m = %u): R is singular",
+                    h->N, h->m);
+    std::lock_guard<std::mutex> g(h->mutex);
+    if (const int rc = for_each_child(h, [&](music_b200 *c) { return music_b200_set_beamformer(c, rule, loading); })) return rc;
+    h->beam_rule = rule;
+    h->beam_loading = loading;
+    return MUSIC_B200_OK;
+}
+
+int music_b200_process_device_beams(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_angles, float *d_levels,
+                                    float *d_spectrum, int32_t *d_bins, int32_t *d_counts, double *d_weights, float *d_beams, void *stream)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (const int rc = check_beams_call(h, d_weights, d_beams)) return rc;
+    Outputs o = caller_outputs(d_angles, d_levels, d_spectrum, d_bins);
+    o.counts = d_counts;
+    o.wts = d_weights;
+    o.beams = d_beams;
+    return process_device_impl(h, d_in_c64, nwindows, o, stream);
+}
+
+int music_b200_process_host_beams(music_b200 *h, const float *in_c64, uint32_t nwindows, float *angles, float *levels, float *spectrum,
+                                  int32_t *bins, int32_t *counts, double *weights, float *beams)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (const int rc = check_beams_call(h, weights, beams)) return rc;
+    Outputs o = caller_outputs(angles, levels, spectrum, bins);
+    o.counts = counts;
+    o.wts = weights;
+    o.beams = beams;
+    return process_host_impl(h, in_c64, nwindows, o);
+}
+
 int music_b200_set_source_rule(music_b200 *h, int rule)
 {
     if (!h) return MUSIC_B200_EINVAL;
@@ -2042,6 +2187,7 @@ void music_b200_destroy(music_b200 *h)
         cudaFree(h->table[i].c64); cudaFree(h->table[i].soa); cudaFree(h->table[i].fz); cudaFree(h->table[i].na_max);
         if (h->streams[i]) cudaStreamDestroy(h->streams[i]);
         cudaFree(h->ws[i].R); cudaFree(h->ws[i].ev); cudaFree(h->ws[i].Vt); cudaFree(h->ws[i].P64); cudaFree(h->ws[i].cnt); cudaFree(h->ws[i].bins);
+        cudaFree(h->ws[i].wts);
         if (h->ws[i].scan_done) cudaEventDestroy(h->ws[i].scan_done);
     }
     for (cudaEvent_t e : h->tev) cudaEventDestroy(e);

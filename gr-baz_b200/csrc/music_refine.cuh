@@ -34,6 +34,15 @@ constexpr int REFINE_MAX_IT = 50;
 constexpr double REFINE_TOL = 1e-12;  // radians: stop once a step is this small
 constexpr double REFINE_RAD2DEG = 180.0 / 3.14159265358979323846;
 
+// The phase phi_m and its derivative psi_m of element m at the angle theta with (sin theta, cos theta) = (st, ct); the
+// steering entry is a_m = exp(-j phi_m).  Shared by the refinement and the beam weights (music_beams.cuh).
+__device__ __forceinline__ void steer_phase(const RefineGeom &geo, int m, double st, double ct, double *phi, double *psi)
+{
+    const double px = geo.pos[2 * m], py = geo.pos[2 * m + 1];
+    *phi = STEER_TWO_PI * (fma(py, st, px * ct) / geo.lambda);
+    *psi = STEER_TWO_PI * (fma(py, ct, -(px * st)) / geo.lambda);
+}
+
 // D(theta), D'(theta), D''(theta) for the p noise vectors G[j][m] (eigenvector j contiguous) of one window
 __device__ __noinline__ void refine_eval(const RefineGeom &geo, const double2 *__restrict__ G, int M, int p, double th,
                                          double *D, double *D1, double *D2)
@@ -42,9 +51,8 @@ __device__ __noinline__ void refine_eval(const RefineGeom &geo, const double2 *_
     sincos(th, &st, &ct);
     double ar[MAXM], ai[MAXM], ps[MAXM], ph[MAXM];
     for (int m = 0; m < M; ++m) {
-        const double px = geo.pos[2 * m], py = geo.pos[2 * m + 1];
-        const double phi = STEER_TWO_PI * (fma(py, st, px * ct) / geo.lambda);
-        const double psi = STEER_TWO_PI * (fma(py, ct, -(px * st)) / geo.lambda);
+        double phi, psi;
+        steer_phase(geo, m, st, ct, &phi, &psi);
         double sp, cp;
         sincos(phi, &sp, &cp);
         ar[m] = cp;
@@ -89,9 +97,8 @@ __device__ __noinline__ void bartlett_eval(const RefineGeom &geo, const double2 
     sincos(th, &st, &ct);
     double ar[MAXM], ai[MAXM], ps[MAXM], ph[MAXM];
     for (int m = 0; m < M; ++m) {
-        const double px = geo.pos[2 * m], py = geo.pos[2 * m + 1];
-        const double phi = STEER_TWO_PI * (fma(py, st, px * ct) / geo.lambda);
-        const double psi = STEER_TWO_PI * (fma(py, ct, -(px * st)) / geo.lambda);
+        double phi, psi;
+        steer_phase(geo, m, st, ct, &phi, &psi);
         double sp, cp;
         sincos(phi, &sp, &cp);
         ar[m] = cp;

@@ -168,6 +168,42 @@ class music_doa(object):
         """(kind, loading) in use"""
         return getattr(self, "_estimator", ("music", 0.0))
 
+    # -- extension: beamformed source signals ------------------------------------------------------------
+    BEAMFORMERS = {"off": 0, "das": 1, "mvdr": 2, "lcmv": 3}
+
+    def set_beamformer(self, kind="off", loading=0.0):
+        """Receive every reported source: ``"das"`` (delay-and-sum, w = a / a^H a), ``"mvdr"`` (distortionless,
+        minimum output power on R + delta I, delta = loading * tr(R) / m) or ``"lcmv"`` (unit gain on its own source,
+        a null on every other filled slot of the window).  While it is not ``"off"`` (default), ``work()`` also returns
+        the beams and weights of its windows through ``last_beams()`` / ``last_weights()`` (include/music_b200.h).
+        ``loading`` must be 0 for "off" and "das"; loading 0 under "mvdr" / "lcmv" needs more snapshots than antennas.
+        With coherent sources (the "dml" peak mode) MVDR and LCMV beams cancel the signal: use "das" there."""
+        if kind not in self.BEAMFORMERS:
+            raise ValueError("kind must be one of %s" % sorted(self.BEAMFORMERS))
+        _capi.check(self._lib.music_b200_set_beamformer(self._h, self.BEAMFORMERS[kind], float(loading)), self._h)
+        self._beamformer = (kind, float(loading))
+
+    def beamformer(self):
+        """(kind, loading) in use"""
+        return getattr(self, "_beamformer", ("off", 0.0))
+
+    def last_beams(self):
+        """complex64 (W, n, N) beams of the last work() call (N = nsamples / m), zeros for unfilled slots; None while the
+        beamformer is off."""
+        return getattr(self, "_last_beams", None)
+
+    def last_weights(self):
+        """complex128 (W, n, m) beam weights of the last work() call; None while the beamformer is off."""
+        return getattr(self, "_last_weights", None)
+
+    def process_device_beams(self, d_in, nwindows, d_angles, d_levels=None, d_spectrum=None, d_bins=None, d_counts=None,
+                             d_weights=None, d_beams=None, stream=None):
+        """Raw device-pointer entry (ints): the outputs of ``process_device(..., d_counts=...)`` plus ``d_weights``
+        (complex fp64 [nwindows][n][m]) and ``d_beams`` (complex64 [nwindows][n][N]); one of the two may be None."""
+        rc = self._lib.music_b200_process_device_beams(self._h, d_in, int(nwindows), d_angles, d_levels, d_spectrum, d_bins,
+                                                        d_counts, d_weights, d_beams, stream)
+        _capi.check(rc, self._h)
+
     # -- extension (SURVEY.md section 8(f) rank 4): GUI-rate reducers -----------------------------
     def reduce_angles(self, angles, levels=None, weighted=False):
         """Circular mean (degrees), mean resultant length and total weight per angle slot over the
@@ -221,7 +257,16 @@ class music_doa(object):
         spec = outs[2] if len(outs) > 2 else None
         self._last_bins = np.empty((W, self.n), np.int32)
         lvl_p, spec_p = lvl.ctypes.data if lvl is not None else None, spec.ctypes.data if spec is not None else None
-        if self.source_rule() == "fixed":
+        self._last_beams = self._last_weights = None
+        if self.beamformer()[0] != "off":
+            N = self.nsamples // self.m
+            self._last_counts = np.empty(W, np.int32)
+            self._last_weights = np.empty((W, self.n, self.m), np.complex128)
+            self._last_beams = np.empty((W, self.n, N), np.complex64)
+            rc = self._lib.music_b200_process_host_beams(self._h, x.ctypes.data, W, ang.ctypes.data, lvl_p, spec_p,
+                                                         self._last_bins.ctypes.data, self._last_counts.ctypes.data,
+                                                         self._last_weights.ctypes.data, self._last_beams.ctypes.data)
+        elif self.source_rule() == "fixed":
             rc = self._lib.music_b200_process_host(self._h, x.ctypes.data, W, ang.ctypes.data, lvl_p, spec_p, self._last_bins.ctypes.data)
             self._last_counts = np.full(W, self.n, np.int32)
         else:

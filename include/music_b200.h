@@ -295,6 +295,54 @@ int music_b200_set_refine(music_b200 *h, int mode);
 int music_b200_set_estimator(music_b200 *h, int estimator, double loading);
 
 /*
+ * Beamformed source signals (extension, no reference counterpart): receive each reported source, a beam steered at
+ * every filled peak slot of a window, from the same window's covariance.
+ * music_b200_set_beamformer() takes MUSIC_B200_BEAMS_OFF (default), _DAS, _MVDR or _LCMV and a diagonal loading.  The
+ * setting is read only by music_b200_process_device_beams() and music_b200_process_host_beams(); every other entry point
+ * ignores it.  It applies to every device of a multi-device handle.  EINVAL: an unknown rule; loading not finite or < 0;
+ * loading != 0 with OFF or DAS; MVDR or LCMV with loading == 0 when N <= m (R is singular); an az-el handle.
+ * For window w the filled slots are S = {i : bins[w][i] >= 0} as the call's peak stage reported them, under every peak
+ * mode, source rule, estimator and refinement setting (the slots need not form a prefix).  M = m, x(r, c) = in[c m + r].
+ *   steering   a_i (fp64): if the current table came from set_geometry(), a_m = exp(-j phi_m),
+ *              phi_m = 2 pi (p_x,m cos t + p_y,m sin t) / lambda, t = the reported float angle (double)angles[w][i] in
+ *              radians (the refinement's convention, so refined, ROOTS and ESPRIT angles steer off the grid); if it came
+ *              from set_table(), table row bins[w][i] widened to fp64.
+ *   DAS        w_i = a_i / (a_i^H a_i).  It reads no R.
+ *   MVDR       R_L = R + delta I, delta = loading * tr(R) / M; R_L = L L^H with the MVDR estimator's Cholesky (a pivot
+ *              that is not > 0 fails); y_i = L^-1 a_i, z_i = L^-H y_i, w_i = z_i / ||y_i||^2.
+ *   LCMV       unit gain on its own source, a null on every other filled slot: Y = [y_i], Z = [z_i] over i in S (slot
+ *              order), G = Y^H Y (d x d), G = C C^H where every pivot g_k (before its square root) must satisfy
+ *              g_k > 2^-20 G_kk (G_kk = the diagonal entry before elimination); W = Z G^-1, column i is w_i, and
+ *              w_i^H a_j = delta_ij.  With d = 1, LCMV equals MVDR.
+ *   failure    every weight and beam of the window is 0 when the Cholesky of R_L fails (MVDR, LCMV), when LCMV's pivot
+ *              test fails (e.g. the two mirror slots of an x-axis ULA under LOCAL_MAXIMA: their steering vectors are
+ *              nearly identical), or when any weight is not finite.  Unfilled slots always get zero weights and beams.
+ *   outputs    weights[w][i][m] = w_i as fp64 (re, im) pairs; beams[w][i][t] = (float)(sum_m conj(w_im) x_m(t)) for
+ *              t < N, accumulated in fp64, re and im each rounded once; layout [W][n][N] complex64, one contiguous time
+ *              series per slot.
+ * Caveat: with coherent sources (what the DML peak mode resolves) an MVDR or LCMV beam built from R suffers signal
+ * cancellation; that is physics, not a defect.  Use DAS there.
+ * The beams entry points take the outputs of music_b200_process_device_counts() / _host_counts() plus weights and beams;
+ * either of the two may be NULL, not both (EINVAL).  With the rule OFF they return EINVAL.  beams must be 8-byte
+ * aligned and weights 16-byte aligned.  The host entry deals windows over a multi-device handle as process_host does;
+ * the device entry goes to the device the input lives on.  A beams call always runs the unfused kernels (the fused
+ * kernels keep no R): its angles, levels, spectrum, bins and counts are byte-identical to process_device_ex() with d_R
+ * on the same windows.  Per sub-batch it adds beam_weights_kernel and (with beams) beam_apply_kernel after the peak
+ * stage, timed in the top-n slot of the stage timing.  The apply kernel reads the input a second time: n N complex64
+ * out, m N in per window.
+ */
+#define MUSIC_B200_BEAMS_OFF 0
+#define MUSIC_B200_BEAMS_DAS 1
+#define MUSIC_B200_BEAMS_MVDR 2
+#define MUSIC_B200_BEAMS_LCMV 3
+int music_b200_set_beamformer(music_b200 *h, int rule, double loading);
+int music_b200_process_device_beams(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_angles, float *d_levels,
+                                    float *d_spectrum, int32_t *d_bins, int32_t *d_counts, double *d_weights, float *d_beams,
+                                    void *stream);
+int music_b200_process_host_beams(music_b200 *h, const float *in_c64, uint32_t nwindows, float *angles, float *levels,
+                                  float *spectrum, int32_t *bins, int32_t *counts, double *weights, float *beams);
+
+/*
  * Downstream reducers (extension, no reference counterpart): what a GUI-rate consumer such as the DOA
  * compass (/root/reference/python/doa_compass_control.py:102-108) or a plot sink
  * (/root/reference/python/plot_sink.py:38) needs from millions of windows per second.

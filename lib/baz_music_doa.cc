@@ -69,7 +69,8 @@ baz_music_doa::baz_music_doa(unsigned int m, unsigned int n, unsigned int nsampl
                              const array_response_t &array_response, unsigned int resolution)
     : gr::sync_block("music_doa", gr::io_signature::make(1, 1, nsamples * sizeof(gr_complex)),
                      gr::io_signature::make3(1, 3, n * sizeof(float), n * sizeof(float), resolution * sizeof(float))),
-      d_m(m), d_n(n), d_nsamples(nsamples), d_resolution(resolution), d_handle(NULL), d_source_rule(MUSIC_B200_SOURCES_FIXED)
+      d_m(m), d_n(n), d_nsamples(nsamples), d_resolution(resolution), d_handle(NULL), d_source_rule(MUSIC_B200_SOURCES_FIXED),
+      d_beam_rule(MUSIC_B200_BEAMS_OFF)
 {
     if (array_response.size() != resolution) throw std::invalid_argument("music_doa: array_response.size() != resolution");
     const std::vector<float> table = flatten(array_response);
@@ -168,6 +169,15 @@ void baz_music_doa::set_estimator(int estimator, double loading)
     if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa: ") + music_b200_last_error(d_handle));
 }
 
+/* Extension (not in the reference): beamformed source signals, see include/music_b200.h. */
+void baz_music_doa::set_beamformer(int rule, double loading)
+{
+    gr::thread::scoped_lock guard(d_mutex);
+    const int rc = music_b200_set_beamformer(d_handle, rule, loading);
+    if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa: ") + music_b200_last_error(d_handle));
+    d_beam_rule = rule;
+}
+
 int baz_music_doa::work(int noutput_items, gr_vector_const_void_star &input_items, gr_vector_void_star &output_items)
 {
     if (noutput_items <= 0) return 0;
@@ -178,8 +188,14 @@ int baz_music_doa::work(int noutput_items, gr_vector_const_void_star &input_item
 
     gr::thread::scoped_lock guard(d_mutex);
     d_bins.resize((size_t)noutput_items * d_n);
+    d_beams.clear();
     int rc;
-    if (d_source_rule == MUSIC_B200_SOURCES_FIXED) {
+    if (d_beam_rule != MUSIC_B200_BEAMS_OFF) {
+        d_counts.resize((size_t)noutput_items);
+        d_beams.resize((size_t)noutput_items * d_n * (d_nsamples / d_m));
+        rc = music_b200_process_host_beams(d_handle, in, (uint32_t)noutput_items, out, lvl, out_spectrum, d_bins.data(), d_counts.data(),
+                                           NULL, reinterpret_cast<float *>(d_beams.data()));
+    } else if (d_source_rule == MUSIC_B200_SOURCES_FIXED) {
         rc = music_b200_process_host(d_handle, in, (uint32_t)noutput_items, out, lvl, out_spectrum, d_bins.data());
         d_counts.assign((size_t)noutput_items, (int)d_n);
     } else {

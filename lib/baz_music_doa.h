@@ -63,6 +63,10 @@ public:
     /* extension: 0 = MUSIC (default), 1 = MVDR / Capon with diagonal loading loading * tr(R) / m, 2 = Bartlett
      * beamscan (loading must be 0 for 0 and 2) */
     void set_estimator(int estimator, double loading);
+    /* extension: beamformed source signals - 0 = off (default), 1 = delay-and-sum, 2 = MVDR, 3 = LCMV, with diagonal
+     * loading loading * tr(R) / m for 2 and 3 (must be 0 for 0 and 1).  While it is on, work() also forms one beam per
+     * filled peak slot of every item (include/music_b200.h), read back with last_beams(). */
+    void set_beamformer(int rule, double loading);
 
     /* Integer peak-bin indices of the items produced by the last work() call, [items][n]
      * (not in the reference; -1 marks a slot the reference would leave at (0, 0)). */
@@ -70,6 +74,9 @@ public:
     /* Number of sources of each item produced by the last work() call, [items] (n unless set_source_rule() chose
      * MDL or AIC; slots at and beyond the count are left at (0, 0) with bin -1). */
     const std::vector<int> &last_counts() const { return d_counts; }
+    /* Beams of the items produced by the last work() call while set_beamformer() is on, [items][n][nsamples / m]
+     * (zeros for unfilled slots); empty while it is off. */
+    const std::vector<gr_complex> &last_beams() const { return d_beams; }
 
 private:
     std::vector<float> flatten(const array_response_t &array_response) const;
@@ -81,7 +88,9 @@ private:
     music_b200 *d_handle;
     std::vector<int> d_bins;
     std::vector<int> d_counts;
+    std::vector<gr_complex> d_beams;
     int d_source_rule;
+    int d_beam_rule;
     gr::thread::mutex d_mutex;
 };
 
