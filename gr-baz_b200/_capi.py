@@ -102,6 +102,18 @@ def load():
         L.music_b200_process_device_beams.restype = ctypes.c_int
         L.music_b200_process_host_beams.argtypes = [vp, fp, u32, fp, fp, fp, fp, fp, fp, fp]
         L.music_b200_process_host_beams.restype = ctypes.c_int
+        L.music_b200_set_calibration.argtypes = [vp, fp]
+        L.music_b200_set_calibration.restype = ctypes.c_int
+        L.music_b200_get_calibration.argtypes = [vp, fp]
+        L.music_b200_get_calibration.restype = ctypes.c_int
+        L.music_b200_calib_reset.argtypes = [vp]
+        L.music_b200_calib_reset.restype = ctypes.c_int
+        L.music_b200_calib_accumulate_device.argtypes = [vp, fp, u32, vp]
+        L.music_b200_calib_accumulate_device.restype = ctypes.c_int
+        L.music_b200_calib_accumulate_host.argtypes = [vp, fp, u32]
+        L.music_b200_calib_accumulate_host.restype = ctypes.c_int
+        L.music_b200_calib_solve.argtypes = [vp, dbl, dbl, ctypes.c_int, fp, fp]
+        L.music_b200_calib_solve.restype = ctypes.c_int
         L.music_b200_create_azel.argtypes = [ctypes.POINTER(vp), u32, u32, u32, u32, u32, dbl, dbl, fp, dbl, ctypes.c_int]
         L.music_b200_create_azel.restype = ctypes.c_int
         L.music_b200_set_geometry_azel.argtypes = [vp, fp, dbl]
@@ -141,6 +153,8 @@ EXPORTS = [
     "music_b200_last_error", "music_b200_destroy",
     "music_b200_create_azel", "music_b200_set_geometry_azel", "music_b200_process_azel_host", "music_b200_process_azel_device",
     "music_b200_set_beamformer", "music_b200_process_device_beams", "music_b200_process_host_beams",
+    "music_b200_set_calibration", "music_b200_get_calibration", "music_b200_calib_reset", "music_b200_calib_accumulate_device",
+    "music_b200_calib_accumulate_host", "music_b200_calib_solve",
 ]
 
 

@@ -36,6 +36,7 @@
 #include "music_esprit.cuh"
 #include "music_dml.cuh"
 #include "music_beams.cuh"
+#include "music_calib.cuh"
 
 using namespace music;
 
@@ -165,6 +166,16 @@ struct music_b200 {
     int source_rule = MUSIC_B200_SOURCES_FIXED;  // set_source_rule()
     int beam_rule = MUSIC_B200_BEAMS_OFF;        // set_beamformer(): read by the beams entry points only
     double beam_loading = 0.0;
+    // receiver calibration (music_b200_set_calibration): c_m = 1 / g_m applied to every window's R while `calib` is set
+    bool calib = false;
+    CalibVec cal_c = {};
+    double cal_g[2 * MUSIC_B200_MAX_M] = {};  // the gains as set
+    // the calibration accumulator (music_b200_calib_*; the served device of a multi-device handle): sum of the raw R
+    // over cal_windows windows, the accumulate kernel's per-CTA partial sums and counter, the solve kernel's result
+    double2 *cal_acc = nullptr, *cal_part = nullptr;
+    unsigned *cal_ctr = nullptr;
+    double *cal_out = nullptr;
+    uint64_t cal_windows = 0;
     unsigned steer_guarded = 0;    // entries of the last built table re-evaluated with the host libm
     bool azel = false;             // music_b200_create_azel(): K = n_az * n_el rows, elevation-major (music_azel.cuh)
     AzelGrid grid = {};
@@ -504,6 +515,7 @@ struct Plan {
     Peaks peaks = Peaks::None;
     bool decode = false, refine = false;             // az-el bin decode; peak refinement (the az-el kind after a decode)
     bool beams = false;                              // beam weights (+ beams) after the peaks: the beams entry points
+    bool calib = false;                              // correct R after the covariance (and the beam weights) by the calibration
     bool ws_p64 = false, ws_counts = false, ws_bins = false, ws_wts = false;  // workspace buffers the kernels write
 };
 
@@ -524,7 +536,7 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
     // A beams call needs R, which the fused kernels keep in registers: it runs the unfused plan of a call that asks for R.
     const bool beams = o.wts || o.beams;
     const bool fusable = h->fused && !h->azel && music_est && fixed_n && md.refine == MUSIC_B200_REFINE_OFF &&
-                         md.peak == MUSIC_B200_PEAKS_TOP_BINS && h->n == 1 && !o.P64 && !o.R && !o.ev && !beams;
+                         md.peak == MUSIC_B200_PEAKS_TOP_BINS && h->n == 1 && !o.P64 && !o.R && !o.ev && !beams && !h->calib;
     if (fusable && h->m == 4 && planar_fusable && (!o.spec || h->fused_spec)) p.path = Path::Fused4;
     else if (fusable && h->m == 8 && !planar && !o.spec && h->N >= 128 && h->N % 2 == 0) p.path = Path::Fused8;
 
@@ -554,6 +566,7 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
     p.ws_p64 = p.p64 && !o.P64;
     p.ws_counts = p.count;
     p.beams = beams;
+    p.calib = h->calib;
     p.ws_bins = p.decode || p.refine || (beams && !o.bins);
     p.ws_wts = beams && !o.wts;
     return p;
@@ -826,8 +839,10 @@ __global__ void gather_wait_kernel(const unsigned *flags, int npeer, unsigned ep
 }
 
 // The beam weights of W windows from ws.R, the angles and bins po holds, into o.wts (or the workspace), then the beams
-// of the W windows at d_in into o.beams when the caller asked for them (music_beams.cuh).
-void launch_beams(music_b200 *h, const Workspace &ws, uint32_t W, const Outputs &o, const PeakOut &po, const float *d_in, cudaStream_t st)
+// of the W windows at d_in into o.beams when the caller asked for them (music_beams.cuh).  With a calibration set the
+// weights are taken back to raw-input coordinates before the beams are formed (music_calib.cuh).
+void launch_beams(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t W, const Outputs &o, const PeakOut &po, const float *d_in,
+                  cudaStream_t st)
 {
     const DeviceTable &tb = h->table[h->cur_table];
     const int M = (int)h->m, n = (int)h->n, N = (int)h->N;
@@ -836,6 +851,11 @@ void launch_beams(music_b200 *h, const Workspace &ws, uint32_t W, const Outputs 
         ws.R, po.angles, po.bins, reinterpret_cast<const float2 *>(tb.c64), M, n, (int)W, h->beam_rule, h->beam_loading, tb.geometric,
         tb.geo, wts);
     h->launches++;
+    if (p.calib) {
+        const size_t e = (size_t)W * n * M;
+        calib_weights_kernel<<<(unsigned)((e + CALIB_THREADS - 1) / CALIB_THREADS), CALIB_THREADS, 0, st>>>(wts, M, n, (int)W, h->cal_c);
+        h->launches++;
+    }
     if (!o.beams) return;
     const int spans = (N + BEAM_SPAN - 1) / BEAM_SPAN;
     const size_t smem = beam_apply_smem(M, n);
@@ -933,7 +953,7 @@ int launch_eig_scan(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t 
 #undef REFINE_CASE
         h->launches++;
     }
-    if (p.beams) launch_beams(h, ws, W, o, po, d_in, st);
+    if (p.beams) launch_beams(h, p, ws, W, o, po, d_in, st);
     if (tev) cudaEventRecord(tev[4], st);
     if (o.R)
         CU(h, cudaMemcpyAsync(o.R, ws.R, (size_t)W * M * M * 2 * sizeof(double), cudaMemcpyDeviceToDevice, st));
@@ -1051,6 +1071,12 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, const Ou
         if (tev) cudaEventRecord(tev[0], st);
         if (planar) launch_cov_planar(h, ws, *planar, (unsigned long long)w0 * hop, hop, W, st);
         else launch_cov(h, ws, d_in + (size_t)w0 * h->nsamples * 2, W, st, slot);
+        if (plan.calib) {
+            // the receiver correction of R, inside the covariance slot of the stage timing
+            const size_t e = (size_t)W * h->m * h->m;
+            calib_apply_kernel<<<(unsigned)((e + CALIB_THREADS - 1) / CALIB_THREADS), CALIB_THREADS, 0, st>>>(ws.R, (int)h->m, (int)W, h->cal_c);
+            h->launches++;
+        }
         if (tev) cudaEventRecord(tev[1], st);
         rc = launch_eig_scan(h, plan, ws, W, out.at(w0), st, tev, planar ? nullptr : d_in + (size_t)w0 * h->nsamples * 2);
         if (rc) return rc;
@@ -1895,6 +1921,195 @@ int music_b200_process_host_beams(music_b200 *h, const float *in_c64, uint32_t n
     return process_host_impl(h, in_c64, nwindows, o);
 }
 
+/* ---- receiver calibration (music_calib.cuh) ---- */
+int music_b200_set_calibration(music_b200 *h, const double *gains)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    CalibVec cv = {};
+    if (gains) {
+        for (uint32_t m = 0; m < h->m; ++m) {
+            const double gr = gains[2 * m], gi = gains[2 * m + 1];
+            if (!std::isfinite(gr) || !std::isfinite(gi)) return fail(h, MUSIC_B200_EINVAL, "gain %u is not finite", m);
+            // c = 1 / g = conj(g) / |g|^2 in fp64
+            const double d = gr * gr + gi * gi;
+            cv.c[m] = make_double2(gr / d, -gi / d);
+            if (!(d > 0.0) || !std::isfinite(cv.c[m].x) || !std::isfinite(cv.c[m].y))
+                return fail(h, MUSIC_B200_EINVAL, "gain %u must have a modulus > 0 whose inverse is finite", m);
+        }
+    }
+    std::lock_guard<std::mutex> g(h->mutex);
+    if (const int rc = for_each_child(h, [&](music_b200 *c) { return music_b200_set_calibration(c, gains); })) return rc;
+    h->calib = gains != nullptr;
+    h->cal_c = cv;
+    for (uint32_t i = 0; i < 2 * h->m; ++i) h->cal_g[i] = gains ? gains[i] : (i % 2 == 0 ? 1.0 : 0.0);
+    return MUSIC_B200_OK;
+}
+
+int music_b200_get_calibration(music_b200 *h, double *gains)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (!gains) return fail(h, MUSIC_B200_EINVAL, "gains must not be NULL");
+    std::lock_guard<std::mutex> g(h->mutex);
+    for (uint32_t i = 0; i < 2 * h->m; ++i) gains[i] = h->calib ? h->cal_g[i] : (i % 2 == 0 ? 1.0 : 0.0);
+    return MUSIC_B200_OK;
+}
+
+}  // extern "C"
+
+namespace {
+
+// the accumulator, partial sums, counter and result buffer of a served handle (zeroed on first use)
+int ensure_calib_buffers(music_b200 *h)
+{
+    if (h->cal_acc) return MUSIC_B200_OK;
+    const size_t mm = (size_t)h->m * h->m;
+    CU(h, cudaMalloc(&h->cal_acc, mm * sizeof(double2)));
+    CU(h, cudaMalloc(&h->cal_part, (size_t)CALIB_ACC_MAX_CTAS * mm * sizeof(double2)));
+    CU(h, cudaMalloc(&h->cal_ctr, sizeof(unsigned)));
+    CU(h, cudaMalloc(&h->cal_out, CALIB_OUT * sizeof(double)));
+    CU(h, cudaMemset(h->cal_acc, 0, mm * sizeof(double2)));
+    CU(h, cudaMemset(h->cal_ctr, 0, sizeof(unsigned)));
+    CU(h, cudaDeviceSynchronize());  // the memsets ran on the legacy stream; the kernels run on non-blocking ones
+    h->cal_windows = 0;
+    return MUSIC_B200_OK;
+}
+
+// Adds the raw covariance of nwindows windows at d_in (device memory of h, served and locked) to the accumulator, on
+// st: the covariance kernels in sub-batches through workspace slot 0, each followed by calib_accum_kernel.
+int calib_accumulate(music_b200 *h, const float *d_in, uint32_t nwindows, cudaStream_t st)
+{
+    if (nwindows == 0) return MUSIC_B200_OK;
+    if (const int rc = ensure_calib_buffers(h)) return rc;
+    Plan plan;  // R only
+    const uint32_t sub = std::min((nwindows + SCAN_B - 1) / SCAN_B * SCAN_B, max_sub_windows(h, plan));
+    Workspace &ws = h->ws[0];
+    if (const int rc = ensure_slot(h, ws, sub, plan)) return rc;
+    if (ws.used) CU(h, cudaStreamWaitEvent(st, ws.scan_done, 0));
+    for (uint32_t w0 = 0; w0 < nwindows; w0 += sub) {
+        const uint32_t W = std::min(sub, nwindows - w0);
+        launch_cov(h, ws, d_in + (size_t)w0 * h->nsamples * 2, W, st, 0);
+        const int wpc = calib_acc_wpc((int)W);
+        calib_accum_kernel<<<(W + wpc - 1) / wpc, CALIB_THREADS, 0, st>>>(ws.R, (int)h->m, (int)W, wpc, h->cal_part, h->cal_ctr, h->cal_acc);
+        h->launches++;
+        CU(h, cudaGetLastError());
+        CU(h, cudaEventRecord(ws.scan_done, st));
+        ws.used = true;
+    }
+    h->cal_windows += nwindows;
+    return MUSIC_B200_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int music_b200_calib_reset(music_b200 *h)
+{
+    h = served(h);
+    if (!h) return MUSIC_B200_EINVAL;
+    std::lock_guard<std::mutex> g(h->mutex);
+    CU(h, cudaSetDevice(h->device));
+    if (const int rc = ensure_calib_buffers(h)) return rc;
+    CU(h, cudaDeviceSynchronize());  // accumulate calls still in flight on any stream
+    CU(h, cudaMemset(h->cal_acc, 0, (size_t)h->m * h->m * sizeof(double2)));
+    CU(h, cudaDeviceSynchronize());
+    h->cal_windows = 0;
+    return MUSIC_B200_OK;
+}
+
+int music_b200_calib_accumulate_device(music_b200 *h, const float *d_in_c64, uint32_t nwindows, void *stream)
+{
+    h = served(h);
+    if (!h) return MUSIC_B200_EINVAL;
+    if (nwindows == 0) return MUSIC_B200_OK;
+    if (!d_in_c64) return fail(h, MUSIC_B200_EINVAL, "d_in_c64 must not be NULL");
+    if ((reinterpret_cast<uintptr_t>(d_in_c64) & 15u) != 0) return fail(h, MUSIC_B200_EINVAL, "d_in_c64 must be 16-byte aligned");
+    std::lock_guard<std::mutex> g(h->mutex);
+    CU(h, cudaSetDevice(h->device));
+    return calib_accumulate(h, d_in_c64, nwindows, static_cast<cudaStream_t>(stream));
+}
+
+int music_b200_calib_accumulate_host(music_b200 *h, const float *in_c64, uint32_t nwindows)
+{
+    h = served(h);
+    if (!h) return MUSIC_B200_EINVAL;
+    if (nwindows == 0) return MUSIC_B200_OK;
+    if (!in_c64) return fail(h, MUSIC_B200_EINVAL, "in_c64 must not be NULL");
+    std::lock_guard<std::mutex> g(h->mutex);
+    CU(h, cudaSetDevice(h->device));
+    // chunks of ~32 MiB through one pinned and one device buffer on the handle's first stream (not a throughput path; the
+    // pinned copy makes the transfer independent of how the caller's memory is, or partly is, registered)
+    const size_t win_bytes = (size_t)h->nsamples * 2 * sizeof(float);
+    const uint32_t chunk = (uint32_t)std::max<size_t>(1, std::min<size_t>(nwindows, ((size_t)32 << 20) / win_bytes));
+    float *d = nullptr, *pin = nullptr;
+    cudaStream_t st = h->streams[0];
+    int rc = MUSIC_B200_OK;
+    if (cudaMalloc(&d, chunk * win_bytes) != cudaSuccess || cudaHostAlloc(&pin, chunk * win_bytes, cudaHostAllocDefault) != cudaSuccess)
+        rc = fail(h, MUSIC_B200_ENOMEM, "cannot allocate the calibration staging buffers");
+    for (uint32_t w0 = 0; w0 < nwindows && rc == MUSIC_B200_OK; w0 += chunk) {
+        const uint32_t W = std::min(chunk, nwindows - w0);
+        CU_BREAK(h, rc, cudaStreamSynchronize(st));  // the previous chunk's upload has left the pinned buffer
+        memcpy(pin, in_c64 + (size_t)w0 * h->nsamples * 2, W * win_bytes);
+        CU_BREAK(h, rc, cudaMemcpyAsync(d, pin, W * win_bytes, cudaMemcpyHostToDevice, st));
+        rc = calib_accumulate(h, d, W, st);
+    }
+    const cudaError_t e = cudaStreamSynchronize(st);
+    cudaFree(d);
+    cudaFreeHost(pin);
+    if (rc == MUSIC_B200_OK && e != cudaSuccess) rc = fail(h, MUSIC_B200_ECUDA, "stream sync failed: %s", cudaGetErrorString(e));
+    return rc;
+}
+
+int music_b200_calib_solve(music_b200 *h, double az_deg, double el_deg, int kind, double *gains, double *stats)
+{
+    h = served(h);
+    if (!h) return MUSIC_B200_EINVAL;
+    if (!gains) return fail(h, MUSIC_B200_EINVAL, "gains must not be NULL");
+    if (kind != MUSIC_B200_CALIB_PHASE && kind != MUSIC_B200_CALIB_GAIN_PHASE) return fail(h, MUSIC_B200_EINVAL, "unknown calibration kind %d", kind);
+    if (kind == MUSIC_B200_CALIB_GAIN_PHASE && h->m < 3)
+        return fail(h, MUSIC_B200_EINVAL, "gain and phase calibration needs m >= 3 (with two elements the magnitudes cannot be "
+                                          "identified; use MUSIC_B200_CALIB_PHASE)");
+    if (!std::isfinite(az_deg) || !std::isfinite(el_deg)) return fail(h, MUSIC_B200_EINVAL, "the source direction must be finite");
+    if (!h->azel && el_deg != 0.0) return fail(h, MUSIC_B200_EINVAL, "a 1-D handle takes el_deg = 0 (got %g)", el_deg);
+    std::lock_guard<std::mutex> g(h->mutex);
+    const DeviceTable &tb = h->table[h->cur_table];
+    if (!tb.geometric)
+        return fail(h, MUSIC_B200_EINVAL, "calibration needs a table built from the array geometry (set_geometry / set_geometry_azel); "
+                                          "the current one came from set_table()");
+    if (h->cal_windows == 0) return fail(h, MUSIC_B200_EINVAL, "no calibration windows accumulated");
+    CalibSource src = {};
+    for (uint32_t m = 0; m < h->m; ++m) {
+        src.pos[3 * m] = h->azel ? tb.ageo.pos[3 * m] : tb.geo.pos[2 * m];
+        src.pos[3 * m + 1] = h->azel ? tb.ageo.pos[3 * m + 1] : tb.geo.pos[2 * m + 1];
+        src.pos[3 * m + 2] = h->azel ? tb.ageo.pos[3 * m + 2] : 0.0;
+    }
+    src.lambda = h->azel ? tb.ageo.lambda : tb.geo.lambda;
+    src.az = az_deg * STEER_DEG2RAD;
+    src.el = el_deg * STEER_DEG2RAD;
+    src.azel = h->azel;
+    CU(h, cudaSetDevice(h->device));
+    CU(h, cudaDeviceSynchronize());  // every accumulate call, on whatever stream, has landed
+    cudaStream_t st = h->streams[0];
+    calib_solve_kernel<<<1, 32, 0, st>>>(h->cal_acc, (double)h->cal_windows, (int)h->m, src, kind, h->cal_out);
+    h->launches++;
+    CU(h, cudaGetLastError());
+    double out[CALIB_OUT];
+    CU(h, cudaMemcpyAsync(out, h->cal_out, sizeof out, cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    switch ((int)out[2 * MAXM + 2]) {
+    case CALIB_OK: break;
+    case CALIB_NOPOWER: return fail(h, MUSIC_B200_EINVAL, "calibration failed: the accumulated covariance has no power on its diagonal");
+    case CALIB_DEAD: return fail(h, MUSIC_B200_EINVAL, "calibration failed: an element has zero gain (a dead channel)");
+    default: return fail(h, MUSIC_B200_EINVAL, "calibration failed: a non-finite value in the accumulated covariance or the fit");
+    }
+    for (uint32_t i = 0; i < 2 * h->m; ++i) gains[i] = out[i];
+    if (stats) {
+        stats[0] = out[2 * MAXM];
+        stats[1] = out[2 * MAXM + 1];
+    }
+    return MUSIC_B200_OK;
+}
+
 int music_b200_set_source_rule(music_b200 *h, int rule)
 {
     if (!h) return MUSIC_B200_EINVAL;
@@ -2181,6 +2396,7 @@ void music_b200_destroy(music_b200 *h)
     cudaFree(h->fused_trace);
     cudaFree(h->f8_stats);
     cudaFree(h->work_ctr);
+    cudaFree(h->cal_acc); cudaFree(h->cal_part); cudaFree(h->cal_ctr); cudaFree(h->cal_out);
     cudaFree(h->steer_pos); cudaFree(h->steer_count); cudaFree(h->steer_list); cudaFree(h->steer_vals);
     if (h->fused_done) cudaEventDestroy(h->fused_done);
     for (int i = 0; i < 2; ++i) {

@@ -204,6 +204,61 @@ class music_doa(object):
                                                         d_counts, d_weights, d_beams, stream)
         _capi.check(rc, self._h)
 
+    # -- extension: receiver calibration -----------------------------------------------------------------
+    CALIBRATIONS = {"phase": 1, "gain_phase": 2}
+
+    def set_calibration(self, gains=None):
+        """Correct every element's receiver gain on the device: ``gains`` = complex (m,) g_m, the chain of element m
+        multiplies its signal by g_m; every later call works on the covariance corrected by c_m = 1 / g_m, in every mode
+        (include/music_b200.h).  ``None`` clears it.  The setting survives ``set_array_response`` and
+        ``set_array_geometry``; beam weights are returned for the raw input."""
+        if gains is None:
+            _capi.check(self._lib.music_b200_set_calibration(self._h, None), self._h)
+            return
+        g = np.asarray(gains, dtype=np.complex128).reshape(-1)
+        if g.size != self.m:
+            raise ValueError("gains must hold m = %d complex values" % self.m)
+        g = np.ascontiguousarray(g)
+        _capi.check(self._lib.music_b200_set_calibration(self._h, g.ctypes.data), self._h)
+
+    def calibration(self):
+        """complex128 (m,) gains in use, all 1 when none is set"""
+        g = np.empty(self.m, np.complex128)
+        _capi.check(self._lib.music_b200_get_calibration(self._h, g.ctypes.data), self._h)
+        return g
+
+    def calib_reset(self):
+        _capi.check(self._lib.music_b200_calib_reset(self._h), self._h)
+
+    def calib_accumulate(self, windows):
+        """adds the raw covariance of ``windows`` (complex64 (W, nsamples), host memory) to the calibration accumulator"""
+        x = np.ascontiguousarray(windows, dtype=np.complex64).reshape(-1, self.nsamples)
+        _capi.check(self._lib.music_b200_calib_accumulate_host(self._h, x.ctypes.data, x.shape[0]), self._h)
+
+    def calib_accumulate_device(self, d_in, nwindows, stream=None):
+        """raw device-pointer form of ``calib_accumulate`` (enqueued on ``stream``)"""
+        _capi.check(self._lib.music_b200_calib_accumulate_device(self._h, d_in, int(nwindows), stream), self._h)
+
+    def calib_solve(self, angle_deg, el_deg=0.0, kind="gain_phase"):
+        """the gains fitted to the accumulated windows of one source at (``angle_deg``, ``el_deg``): (complex128 (m,)
+        gains, residual, sweeps).  The accumulator is kept; nothing is applied."""
+        if kind not in self.CALIBRATIONS:
+            raise ValueError("kind must be one of %s" % sorted(self.CALIBRATIONS))
+        g = np.empty(self.m, np.complex128)
+        st = np.empty(2, np.float64)
+        _capi.check(self._lib.music_b200_calib_solve(self._h, float(angle_deg), float(el_deg), self.CALIBRATIONS[kind], g.ctypes.data,
+                                                     st.ctypes.data), self._h)
+        return g, float(st[0]), int(st[1])
+
+    def calibrate(self, windows, angle_deg, el_deg=0.0, kind="gain_phase"):
+        """Estimate the receiver gains from ``windows`` (complex64 (W, nsamples)) of one dominant source at the known
+        direction (``angle_deg``, ``el_deg``; el 0 on a 1-D block): reset, accumulate and solve on the device.  Returns
+        (gains, residual, sweeps); apply the gains with ``set_calibration`` once the residual looks right.  ``kind``:
+        "gain_phase" (m >= 3) or "phase".  Needs a table installed with ``set_array_geometry``."""
+        self.calib_reset()
+        self.calib_accumulate(windows)
+        return self.calib_solve(angle_deg, el_deg, kind)
+
     # -- extension (SURVEY.md section 8(f) rank 4): GUI-rate reducers -----------------------------
     def reduce_angles(self, angles, levels=None, weighted=False):
         """Circular mean (degrees), mean resultant length and total weight per angle slot over the

@@ -343,6 +343,67 @@ int music_b200_process_host_beams(music_b200 *h, const float *in_c64, uint32_t n
                                   float *spectrum, int32_t *bins, int32_t *counts, double *weights, float *beams);
 
 /*
+ * Receiver calibration (extension, no reference counterpart): estimate each element's complex gain from a known source
+ * and correct it on the device in every mode.
+ *   model      each receiver chain multiplies what its element sees by a gain g_m (cable length, filter group delay, the
+ *              LO phase of each channel, which changes at every retune), after the receiver noise:
+ *              x_raw(t) = G (A s(t) + n(t)), G = diag(g).  The correction is x = C x_raw, C = diag(c), c_m = 1 / g_m,
+ *              which makes the noise white again.  (Correcting the table instead, a -> g o a, would leave the noise
+ *              coloured by |g_m|^2: the correction goes on the data side, as a transform of R.)
+ *   apply      music_b200_set_calibration(h, gains) sets gains [m][2] doubles (re, im); NULL clears it.  Every entry must
+ *              be finite, every |g_m| > 0 and 1 / g_m finite, otherwise EINVAL and the old setting stays.  While a
+ *              calibration is set, every process call transforms each window's fp64 covariance right after the covariance
+ *              kernel: R_ij <- (c_i R_ij) conj(c_j), with c_m = 1 / g_m = conj(g_m) / |g_m|^2 computed on the host in fp64.
+ *              Everything downstream sees the corrected R: eigensolver, source count, MVDR preparation, scans, every peak
+ *              mode, refinement, ROOTS, ESPRIT, DML, az-el decode and refinement, and beam weights; process_device_ex's
+ *              d_R returns the corrected R.  Beam weights are returned in raw-input coordinates, w_raw = conj(c) o w, and
+ *              the beams are formed from the raw input: beams = w_raw^H x_raw = w^H x, and LCMV's w_i^H a_j = delta_ij
+ *              still holds in corrected coordinates.  The setting persists across set_table(), set_geometry() and
+ *              set_geometry_azel() (it belongs to the receivers, not to the table), applies to every device of a
+ *              multi-device handle and is read by every process entry (host, device, _ex, _counts, planar, sharded, az-el,
+ *              beams).  A calibrated call runs the unfused kernels (the fused M = 4 / M = 8 kernels keep R in registers),
+ *              plus calib_apply_kernel per sub-batch, timed in the covariance slot of the stage timing, and with beams
+ *              calib_weights_kernel after the weights, timed in the top-n slot.
+ *              music_b200_get_calibration returns the gains in use, all (1, 0) when none is set.
+ *   estimate   from windows of one dominant source at a known direction (az, el) in degrees; el must be 0 on a 1-D handle.
+ *              a0 = the unrounded fp64 steering vector of the current geometry (the refinement's convention on a 1-D
+ *              handle, the 3-D direction u(az, el) on an az-el handle); a table from set_table() gives EINVAL.
+ *              Rbar = (1 / W) sum_w R_w, the fp64 covariance of each raw window (before any calibration that is set),
+ *              accumulated over one or more accumulate calls.  h minimises the off-diagonal misfit
+ *              sum_{i != j} |Rbar_ij - h_i conj(h_j)|^2: noise and its colouring live on the diagonal only, so unlike the
+ *              principal eigenvector of Rbar the minimiser recovers g o a0 exactly on a population covariance at any
+ *              noise level.
+ *                start   r = argmax_i Rbar_ii (lowest index on ties), h_r = sqrt(Rbar_rr), h_i = Rbar_ir / sqrt(Rbar_rr);
+ *                sweeps  Gauss-Seidel: for i = 0 .. M-1 in turn, h_i <- (sum_{j != i} Rbar_ij h_j) / (sum_{j != i} |h_j|^2),
+ *                        with the updated entries; stop after the first sweep whose largest change |h_i,new - h_i,old| is
+ *                        <= 2^-40 max_i |h_i|, or after 200 sweeps.
+ *              g_m = h_m / a0_m, rotated by a common phase so that g_0 is real and positive, then
+ *                MUSIC_B200_CALIB_GAIN_PHASE  scaled to sum |g_m|^2 = M; needs m >= 3 (with two elements the split of the
+ *                                             magnitudes between the chains cannot be identified);
+ *                MUSIC_B200_CALIB_PHASE       g_m <- g_m / |g_m|; any m >= 2, including a two-channel receiver.
+ *              stats: the residual rho = sqrt(sum_{i != j} |Rbar_ij - h_i conj(h_j)|^2 / sum_{i != j} |Rbar_ij|^2) (small
+ *              when one source dominates) and the number of sweeps.
+ *              EINVAL, and nothing written, when no windows were accumulated, Rbar_rr <= 0, anything is not finite, or
+ *              some h_m = 0 (a dead channel).
+ *   calls      accumulation and solving run on the device.  calib_accumulate_device needs d_in 16-byte aligned, is enqueued
+ *              on `stream` and does not synchronise; calib_accumulate_host copies in chunks and returns when done.  solve
+ *              synchronises, leaves the accumulator unchanged (more windows can be added and solved again) and does not
+ *              apply the gains: the caller inspects rho, then calls set_calibration.  reset empties the accumulator.  On
+ *              a multi-device handle the accumulator and solve are served by devices[0], and accumulate_device needs
+ *              its input there.  The accumulated sum is deterministic for a given sequence of calls; its rounding may
+ *              depend on how the windows are split across calls.
+ */
+#define MUSIC_B200_CALIB_PHASE 1
+#define MUSIC_B200_CALIB_GAIN_PHASE 2
+int music_b200_set_calibration(music_b200 *h, const double *gains /* [m][2] or NULL */);
+int music_b200_get_calibration(music_b200 *h, double *gains /* [m][2] */);
+int music_b200_calib_reset(music_b200 *h);
+int music_b200_calib_accumulate_device(music_b200 *h, const float *d_in_c64, uint32_t nwindows, void *stream);
+int music_b200_calib_accumulate_host(music_b200 *h, const float *in_c64, uint32_t nwindows);
+int music_b200_calib_solve(music_b200 *h, double az_deg, double el_deg, int kind, double *gains /* host [m][2] */,
+                           double *stats /* host [2]: residual, sweeps; may be NULL */);
+
+/*
  * Downstream reducers (extension, no reference counterpart): what a GUI-rate consumer such as the DOA
  * compass (/root/reference/python/doa_compass_control.py:102-108) or a plot sink
  * (/root/reference/python/plot_sink.py:38) needs from millions of windows per second.

@@ -28,8 +28,11 @@
 #include <gnuradio/io_signature.h>
 #include <music_b200.h>
 
+#include "calibration_step.h"
+
 #include <cstdio>
 #include <cstdlib>
+#include <limits>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -70,7 +73,8 @@ baz_music_doa::baz_music_doa(unsigned int m, unsigned int n, unsigned int nsampl
     : gr::sync_block("music_doa", gr::io_signature::make(1, 1, nsamples * sizeof(gr_complex)),
                      gr::io_signature::make3(1, 3, n * sizeof(float), n * sizeof(float), resolution * sizeof(float))),
       d_m(m), d_n(n), d_nsamples(nsamples), d_resolution(resolution), d_handle(NULL), d_source_rule(MUSIC_B200_SOURCES_FIXED),
-      d_beam_rule(MUSIC_B200_BEAMS_OFF)
+      d_beam_rule(MUSIC_B200_BEAMS_OFF), d_cal_remaining(0), d_cal_angle(0.0), d_cal_kind(MUSIC_B200_CALIB_GAIN_PHASE),
+      d_cal_residual(std::numeric_limits<double>::quiet_NaN())
 {
     if (array_response.size() != resolution) throw std::invalid_argument("music_doa: array_response.size() != resolution");
     const std::vector<float> table = flatten(array_response);
@@ -178,6 +182,43 @@ void baz_music_doa::set_beamformer(int rule, double loading)
     d_beam_rule = rule;
 }
 
+/* Extension (not in the reference): receiver calibration, see include/music_b200.h. */
+void baz_music_doa::set_calibration(const std::vector<std::complex<double> > &gains)
+{
+    if (!gains.empty() && gains.size() != d_m) throw std::invalid_argument("music_doa: gains.size() != m");
+    std::vector<double> flat;
+    for (size_t i = 0; i < gains.size(); ++i) {
+        flat.push_back(gains[i].real());
+        flat.push_back(gains[i].imag());
+    }
+    gr::thread::scoped_lock guard(d_mutex);
+    const int rc = music_b200_set_calibration(d_handle, gains.empty() ? NULL : flat.data());
+    if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa: ") + music_b200_last_error(d_handle));
+}
+
+std::vector<std::complex<double> > baz_music_doa::calibration()
+{
+    std::vector<double> flat(2 * (size_t)d_m);
+    gr::thread::scoped_lock guard(d_mutex);
+    const int rc = music_b200_get_calibration(d_handle, flat.data());
+    if (rc != MUSIC_B200_OK) throw std::runtime_error(std::string("music_doa: ") + music_b200_last_error(d_handle));
+    std::vector<std::complex<double> > g(d_m);
+    for (unsigned int i = 0; i < d_m; ++i) g[i] = std::complex<double>(flat[2 * i], flat[2 * i + 1]);
+    return g;
+}
+
+void baz_music_doa::calibrate(double angle_deg, int kind, int nitems)
+{
+    if (nitems <= 0) throw std::invalid_argument("music_doa: calibrate() needs nitems > 0");
+    if (kind != MUSIC_B200_CALIB_PHASE && kind != MUSIC_B200_CALIB_GAIN_PHASE) throw std::invalid_argument("music_doa: unknown calibration kind");
+    gr::thread::scoped_lock guard(d_mutex);
+    const int rc = music_b200_calib_reset(d_handle);
+    if (rc != MUSIC_B200_OK) throw std::runtime_error(std::string("music_doa: ") + music_b200_last_error(d_handle));
+    d_cal_remaining = nitems;
+    d_cal_angle = angle_deg;
+    d_cal_kind = kind;
+}
+
 int baz_music_doa::work(int noutput_items, gr_vector_const_void_star &input_items, gr_vector_void_star &output_items)
 {
     if (noutput_items <= 0) return 0;
@@ -203,5 +244,6 @@ int baz_music_doa::work(int noutput_items, gr_vector_const_void_star &input_item
         rc = music_b200_process_host_counts(d_handle, in, (uint32_t)noutput_items, out, lvl, out_spectrum, d_bins.data(), d_counts.data());
     }
     if (rc != MUSIC_B200_OK) throw std::runtime_error(std::string("music_doa: ") + music_b200_last_error(d_handle));
+    calibration_step(d_handle, in, noutput_items, d_cal_remaining, d_cal_angle, 0.0, d_cal_kind, d_cal_residual);
     return noutput_items;
 }

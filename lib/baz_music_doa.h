@@ -67,6 +67,17 @@ public:
      * loading loading * tr(R) / m for 2 and 3 (must be 0 for 0 and 1).  While it is on, work() also forms one beam per
      * filled peak slot of every item (include/music_b200.h), read back with last_beams(). */
     void set_beamformer(int rule, double loading);
+    /* extension: receiver calibration (include/music_b200.h).  set_calibration(): the complex gain g_m of each element's
+     * receiver chain; every later work() call corrects the covariance by 1 / g_m, in every mode (an empty vector clears
+     * it).  calibration(): the gains in use (all 1 when none is set).  calibrate(): arms the block - the next nitems
+     * items work() receives, from one dominant source at the known direction, are also accumulated (their outputs are
+     * produced as usual); then the block solves for the gains (kind 1 = phase only, 2 = gain and phase, m >= 3) and
+     * applies them.  last_calibration_residual(): the fit's relative off-diagonal residual, NaN when the solve failed
+     * (the old gains are kept), or before any calibration finished.  Needs a table from set_array_geometry(). */
+    void set_calibration(const std::vector<std::complex<double> > &gains);
+    std::vector<std::complex<double> > calibration();
+    void calibrate(double angle_deg, int kind, int nitems);
+    double last_calibration_residual() const { return d_cal_residual; }
 
     /* Integer peak-bin indices of the items produced by the last work() call, [items][n]
      * (not in the reference; -1 marks a slot the reference would leave at (0, 0)). */
@@ -91,6 +102,11 @@ private:
     std::vector<gr_complex> d_beams;
     int d_source_rule;
     int d_beam_rule;
+    /* calibrate(): items still to accumulate (0: not armed), the source direction and the kind; the last residual */
+    int d_cal_remaining;
+    double d_cal_angle;
+    int d_cal_kind;
+    double d_cal_residual;
     gr::thread::mutex d_mutex;
 };
 

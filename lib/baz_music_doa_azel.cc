@@ -14,8 +14,11 @@
 #include <gnuradio/io_signature.h>
 #include <music_b200.h>
 
+#include "calibration_step.h"
+
 #include <cstdio>
 #include <cstdlib>
+#include <limits>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -45,7 +48,8 @@ baz_music_doa_azel::baz_music_doa_azel(unsigned int m, unsigned int n, unsigned 
                                        const std::vector<std::vector<double> > &positions_xyz, double wavelength)
     : gr::sync_block("music_doa_azel", gr::io_signature::make(1, 1, nsamples * sizeof(gr_complex)),
                      gr::io_signature::makev(2, 4, output_sizes(n, n_az, n_el))),
-      d_m(m), d_n(n), d_handle(NULL)
+      d_m(m), d_n(n), d_handle(NULL), d_cal_remaining(0), d_cal_az(0.0), d_cal_el(0.0), d_cal_kind(MUSIC_B200_CALIB_GAIN_PHASE),
+      d_cal_residual(std::numeric_limits<double>::quiet_NaN())
 {
     const std::vector<double> pos = flatten(positions_xyz);
     const int rc = music_b200_create_azel(&d_handle, m, n, nsamples, n_az, n_el, el_lo, el_hi, pos.data(), wavelength, device_from_env());
@@ -108,6 +112,43 @@ void baz_music_doa_azel::set_estimator(int estimator, double loading)
     if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa_azel: ") + music_b200_last_error(d_handle));
 }
 
+void baz_music_doa_azel::set_calibration(const std::vector<std::complex<double> > &gains)
+{
+    if (!gains.empty() && gains.size() != d_m) throw std::invalid_argument("music_doa_azel: gains.size() != m");
+    std::vector<double> flat;
+    for (size_t i = 0; i < gains.size(); ++i) {
+        flat.push_back(gains[i].real());
+        flat.push_back(gains[i].imag());
+    }
+    gr::thread::scoped_lock guard(d_mutex);
+    const int rc = music_b200_set_calibration(d_handle, gains.empty() ? NULL : flat.data());
+    if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa_azel: ") + music_b200_last_error(d_handle));
+}
+
+std::vector<std::complex<double> > baz_music_doa_azel::calibration()
+{
+    std::vector<double> flat(2 * (size_t)d_m);
+    gr::thread::scoped_lock guard(d_mutex);
+    const int rc = music_b200_get_calibration(d_handle, flat.data());
+    if (rc != MUSIC_B200_OK) throw std::runtime_error(std::string("music_doa_azel: ") + music_b200_last_error(d_handle));
+    std::vector<std::complex<double> > g(d_m);
+    for (unsigned int i = 0; i < d_m; ++i) g[i] = std::complex<double>(flat[2 * i], flat[2 * i + 1]);
+    return g;
+}
+
+void baz_music_doa_azel::calibrate(double az_deg, double el_deg, int kind, int nitems)
+{
+    if (nitems <= 0) throw std::invalid_argument("music_doa_azel: calibrate() needs nitems > 0");
+    if (kind != MUSIC_B200_CALIB_PHASE && kind != MUSIC_B200_CALIB_GAIN_PHASE) throw std::invalid_argument("music_doa_azel: unknown calibration kind");
+    gr::thread::scoped_lock guard(d_mutex);
+    const int rc = music_b200_calib_reset(d_handle);
+    if (rc != MUSIC_B200_OK) throw std::runtime_error(std::string("music_doa_azel: ") + music_b200_last_error(d_handle));
+    d_cal_remaining = nitems;
+    d_cal_az = az_deg;
+    d_cal_el = el_deg;
+    d_cal_kind = kind;
+}
+
 int baz_music_doa_azel::work(int noutput_items, gr_vector_const_void_star &input_items, gr_vector_void_star &output_items)
 {
     if (noutput_items <= 0) return 0;
@@ -123,5 +164,6 @@ int baz_music_doa_azel::work(int noutput_items, gr_vector_const_void_star &input
     d_counts.resize((size_t)noutput_items);
     const int rc = music_b200_process_azel_host(d_handle, in, (uint32_t)noutput_items, az, el, lvl, spectrum, d_bins.data(), d_counts.data());
     if (rc != MUSIC_B200_OK) throw std::runtime_error(std::string("music_doa_azel: ") + music_b200_last_error(d_handle));
+    calibration_step(d_handle, in, noutput_items, d_cal_remaining, d_cal_az, d_cal_el, d_cal_kind, d_cal_residual);
     return noutput_items;
 }

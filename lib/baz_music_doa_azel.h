@@ -15,6 +15,7 @@
 #include <gnuradio/sync_block.h>
 #include <gnuradio/thread/thread.h>
 #include <boost/shared_ptr.hpp>
+#include <complex>
 #include <vector>
 
 struct music_b200; /* opaque, include/music_b200.h */
@@ -53,6 +54,11 @@ public:
     void set_refine(bool enable);
     /* 0 = MUSIC (default), 1 = MVDR with diagonal loading loading * tr(R) / m, 2 = Bartlett (loading 0 for 0 and 2) */
     void set_estimator(int estimator, double loading);
+    /* receiver calibration, as for baz_music_doa; calibrate() takes the source's azimuth and elevation */
+    void set_calibration(const std::vector<std::complex<double> > &gains);
+    std::vector<std::complex<double> > calibration();
+    void calibrate(double az_deg, double el_deg, int kind, int nitems);
+    double last_calibration_residual() const { return d_cal_residual; }
 
     /* flat peak bins b = i * n_az + k of the items produced by the last work() call, [items][n] (-1: unfilled slot) */
     const std::vector<int> &last_bins() const { return d_bins; }
@@ -67,6 +73,10 @@ private:
     music_b200 *d_handle;
     std::vector<int> d_bins;
     std::vector<int> d_counts;
+    int d_cal_remaining;
+    double d_cal_az, d_cal_el;
+    int d_cal_kind;
+    double d_cal_residual;
     gr::thread::mutex d_mutex;
 };
 
