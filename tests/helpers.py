@@ -1,6 +1,7 @@
 """Shared helpers for the test-suite (oracle-side: allowed to import oracle/)."""
 import glob
 import hashlib
+import math
 import os
 import re
 
@@ -8,6 +9,10 @@ import numpy as np
 
 from gr_baz_b200 import synth
 from oracle import music_oracle as mo
+
+import beams_oracle as bo
+import refine_oracle as ro
+import root_music_oracle as rm
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(ROOT, "tests", "golden")
@@ -289,3 +294,262 @@ def reference_outputs(key, x=None):
     if x is not None:
         assert sha256(x) == ref["in_sha256"], "%s: the inputs differ from those the reference was run on" % key
     return ref
+
+
+# ---- fixtures of the GPU tests (numpy only) --------------------------------------------------------------------------
+LAM = synth.C_LIGHT / synth.FREQUENCY  # wavelength (metres) of the geometric tables the 1-D GPU tests install
+SNAPS = 1024                           # snapshots per window of angle_windows() and the DML resolution rows
+
+
+def ula(m, kind):
+    """x-axis, y-axis, an oblique offset ULA and the x-axis ULA in reversed order, lambda / 2 apart"""
+    axis, p0, rev = {"x": (0.0, (0.0, 0.0), False), "y": (90.0, (0.0, 0.0), False),
+                     "oblique": (30.0, (0.7, -1.3), False), "reversed": (0.0, (0.0, 0.0), True)}[kind]
+    a = math.radians(axis)
+    pos = np.array([[p0[0] + 0.5 * i * math.cos(a), p0[1] + 0.5 * i * math.sin(a)] for i in range(m)])
+    return pos[::-1].copy() if rev else pos
+
+
+def positions(geometry, m):
+    """element positions (metres) of a synth geometry ("ula_x", "ula_y", "uca")"""
+    return np.asarray(mo.scaled_antenna_array(synth.SPACING, synth.antenna_array(geometry, m)), np.float64)
+
+
+def array_wl(kind, m, seed=0):
+    """element positions in wavelengths: UCA (adjacent elements lambda / 2 apart), x- / y-axis ULA, random planar"""
+    if kind == "random":
+        return np.random.default_rng(seed).uniform(-1.5, 1.5, (m, 2))
+    geo = {"uca": "uca", "x": "ula_x", "y": "ula_y"}[kind]
+    return np.asarray(synth.antenna_array(geo, m), np.float64) * synth.SPACING
+
+
+def steering_wl(pos, deg):
+    """a(theta) [.., M] for a geometry in wavelengths, exp(-j 2 pi (x cos + y sin))"""
+    t = np.radians(np.asarray(deg, np.float64))[..., None]
+    return np.exp(-2j * np.pi * (pos[:, 0] * np.cos(t) + pos[:, 1] * np.sin(t)))
+
+
+def table_wl(pos, Kt=360):
+    return steering_wl(pos, np.arange(Kt) * 360.0 / Kt).astype(np.complex64)
+
+
+def angle_windows(pos, th, coherent, W, seed, snr_db=20.0, snaps=SNAPS):
+    """(x [W][snaps * M] complex64): sources at the angles th[w] of a geometry in wavelengths, 20 dB each over unit
+    noise; coherent sources carry one signal with a random unit phase between them (a path and its reflection)"""
+    rng = np.random.default_rng(seed)
+    m = pos.shape[0]
+    amp = 10.0 ** (snr_db / 20.0)
+    xs = []
+    for w in range(W):
+        X = (rng.standard_normal((m, snaps)) + 1j * rng.standard_normal((m, snaps))) / np.sqrt(2.0)
+        s = (rng.standard_normal(snaps) + 1j * rng.standard_normal(snaps)) / np.sqrt(2.0)
+        for j, t in enumerate(th[w]):
+            if not coherent and j:
+                s = (rng.standard_normal(snaps) + 1j * rng.standard_normal(snaps)) / np.sqrt(2.0)
+            g = np.exp(2j * np.pi * rng.uniform()) if coherent and j else 1.0
+            X += amp * g * steering_wl(pos, t)[:, None] * s[None, :]
+        xs.append(X.T.reshape(-1))
+    return np.ascontiguousarray(np.array(xs).astype(np.complex64))
+
+
+def resolution_case(kind, m, coherent, sep, W=40):
+    """the windows of one row of the DML resolution table: seeded first angles (x-ULA: inside (20, 160 - sep) degrees,
+    away from end-fire, so that each source is the lower bin of its mirror pair)"""
+    seed = 1000 * m + 10 * sep + (1 if coherent else 0) + (5 if kind == "x" else 0)
+    rng = np.random.default_rng(seed)
+    t0 = rng.uniform(20.0, 160.0 - sep, W) if kind == "x" else rng.uniform(0.0, 360.0, W)
+    th = np.stack([t0, (t0 + sep) % 360.0], axis=1)
+    pos = array_wl(kind, m)
+    return pos, table_wl(pos), angle_windows(pos, th, coherent, W, seed + 7), th
+
+
+# (kind, M, coherent, separation) -> (MUSIC resolved, DML resolved) of 40 windows: tests/dml_oracle.py's counts, fixed
+RESOLUTION = {
+    ("uca", 8, True, 20): (0, 30),
+    ("uca", 8, True, 40): (3, 27),
+    ("uca", 16, True, 20): (4, 34),
+    ("uca", 16, True, 40): (8, 40),
+    ("x", 8, True, 20): (0, 38),
+    ("x", 8, False, 20): (0, 39),
+    ("uca", 8, False, 20): (40, 40),
+    ("uca", 16, False, 40): (40, 40),
+}
+
+
+def circ(a, b):
+    """circular distance in degrees (element-wise)"""
+    d = np.abs(np.asarray(a, np.float64) - np.asarray(b, np.float64)) % 360.0
+    return np.minimum(d, 360.0 - d)
+
+
+def resolved(angles, truth, tol=2.0):
+    """both sources within tol degrees of a reported slot"""
+    return all(min(circ(a, t) for a in angles) <= tol for t in truth)
+
+
+def near_half(tdeg, K):
+    """an angle within 1e-6 bins of the midpoint between two grid bins"""
+    f = float(tdeg) * K / 360.0
+    return abs(f - math.floor(f) - 0.5) <= 1e-6
+
+
+def random_gains(rng, m):
+    """complex receiver gains: +-3 dB and any phase per element"""
+    return 10.0 ** (rng.uniform(-3.0, 3.0, m) / 20.0) * np.exp(1j * rng.uniform(-math.pi, math.pi, m))
+
+
+def corrupt(x, g):
+    """x_raw = g o x per snapshot, rounded to complex64 (exact for real powers of two)"""
+    m = len(g)
+    X = x.astype(np.complex128).reshape(x.shape[0], -1, m) * np.asarray(g)[None, None, :]
+    return np.ascontiguousarray(X.reshape(x.shape[0], -1).astype(np.complex64))
+
+
+def antenna_streams(x, m):
+    """the windows x [W][N * m] as m back-to-back antenna streams (hop = N)"""
+    W = x.shape[0]
+    return [np.ascontiguousarray(x.reshape(W, -1, m)[:, :, r].reshape(-1)) for r in range(m)]
+
+
+def streams_for(cfg, seed, total_snapshots):
+    """m planar streams cut out of the synthetic generator: consecutive generator windows laid end to end."""
+    N = cfg["snapshots"]
+    nwin = (total_snapshots + N - 1) // N
+    x = synth.gen_windows_numpy(cfg, seed, 0, nwin).reshape(nwin * N, cfg["m"])  # [snapshot][antenna]
+    return [np.ascontiguousarray(x[:total_snapshots, r]) for r in range(cfg["m"])]
+
+
+def form_windows(streams, hop, W, N):
+    """what interleave + stream_to_vector (+ overlap) hand to the reference block"""
+    m = len(streams)
+    out = np.empty((W, N * m), np.complex64)
+    for w in range(W):
+        seg = np.stack([s[w * hop:w * hop + N] for s in streams], axis=1)  # (N, m): sample-interleaved
+        out[w] = seg.reshape(-1)
+    return out
+
+
+# ---- beam weights and beams against tests/beams_oracle.py ------------------------------------------------------------
+W_RTOL = 1e-9
+
+
+def gram_cond(R, ang, bins, loading, table, pos):
+    """condition number of the LCMV Gram of one window (1 when fewer than two slots are filled)"""
+    A = bo.steering_vectors(ang, bins, table, pos, LAM)
+    if len(A) < 2:
+        return 1.0
+    M = R.shape[0]
+    RL = R + loading * np.trace(R).real / M * np.eye(M)
+    Ys = [np.linalg.solve(np.linalg.cholesky(RL), A[i]) for i in sorted(A)]
+    Y = np.array(Ys).T
+    return float(np.linalg.cond(Y.conj().T @ Y))
+
+
+def check_weights(got, ref_R, out, rule, loading, table, pos, ctx):
+    """the GPU's weights against the oracle's on the GPU's R, angles and bins"""
+    for w in range(len(ref_R)):
+        ref = bo.weights(ref_R[w], out["angles"][w], out["bins"][w], rule, loading, table=table, pos=pos, lam=LAM)
+        g = got[w]
+        assert np.array_equal(g == 0, ref == 0), (ctx, w, g, ref)
+        if not np.any(ref):
+            continue
+        tol = W_RTOL
+        if rule == bo.LCMV:
+            tol *= max(1.0, gram_cond(ref_R[w], out["angles"][w], out["bins"][w], loading, table, pos))
+        for i in range(ref.shape[0]):
+            s = np.max(np.abs(ref[i]))
+            if s:
+                assert np.max(np.abs(g[i] - ref[i])) <= tol * s, (ctx, w, i, g[i], ref[i], tol)
+
+
+def check_beams(x, got_w, got_b):
+    """beams within one float32 rounding of numpy applying the GPU's weights (+ fp64 accumulation order)"""
+    Wn, n, M = got_w.shape
+    X = x.astype(np.complex128).reshape(Wn, -1, M)  # [W][N][M]
+    ref = np.einsum("wtm,wim->wit", X, np.conj(got_w))
+    bound = np.einsum("wtm,wim->wit", np.abs(X), np.abs(got_w))
+    dead = ~np.any(got_w != 0, axis=2)
+    ref[dead] = 0
+    bound[dead] = 0
+    err = np.abs(got_b.astype(np.complex128) - ref)
+    assert np.all(err <= 2.0 ** -24 * np.abs(ref) + 1e-12 * bound), np.max(err - 2.0 ** -24 * np.abs(ref))
+
+
+# ---- ULA windows of the gridless peak modes (tests/test_gpu_root_music.py, tests/test_gpu_esprit.py) -------------------
+# (sources, snr_db or None for noiseless) per window
+PLAN = [(0, 0.0), (1, 40.0), (2, 40.0), (1, 20.0), (2, 20.0), (3, 20.0), (1, 0.0), (2, 0.0), (3, 0.0), (1, None),
+        (2, None), (3, 10.0)]
+
+
+def axis_deg(pos):
+    s = rm.ula_geometry(pos, LAM)[2]
+    return math.degrees(math.atan2(s[1], s[0]))
+
+
+def source_angles(rng, S, alpha, min_cos=0.05):
+    """S angles over [0, 360), at least 2 degrees from end-fire, with distinct cos(t - alpha)"""
+    while True:
+        t = rng.uniform(0.0, 360.0, S)
+        off = (t - alpha) % 180.0
+        if np.any(np.minimum(off, 180.0 - off) < 2.0):
+            continue
+        cs = np.cos(np.radians(t - alpha))
+        if S < 2 or np.min(np.abs(np.subtract.outer(cs, cs))[np.triu_indices(S, 1)]) >= min_cos:
+            return t
+
+
+def plan_windows(pos, plan, seed, snaps):
+    """complex64 windows; plan[w] = (sources, snr_db or None for noiseless); returns (x, truth per window)"""
+    rng = np.random.default_rng(seed)
+    m = pos.shape[0]
+    alpha = axis_deg(pos)
+    xs, truth = [], []
+    for S, snr in plan:
+        X = np.zeros((m, snaps), np.complex128)
+        if snr is not None:
+            X += (rng.standard_normal((m, snaps)) + 1j * rng.standard_normal((m, snaps))) / np.sqrt(2.0)
+        angs = source_angles(rng, S, alpha) if S else np.zeros(0)
+        amp = 1.0 if snr is None else 10.0 ** (snr / 20.0)
+        for t in angs:
+            a = ro.steering(pos, LAM, math.radians(t))[0]
+            X += amp * a[:, None] * (rng.standard_normal(snaps) + 1j * rng.standard_normal(snaps))[None, :] / np.sqrt(2.0)
+        xs.append(X.T.reshape(-1))
+        truth.append(angs)
+    return np.ascontiguousarray(np.array(xs).astype(np.complex64)), truth
+
+
+def two_source_windows(pos, th, snr_db, snaps, Wn, seed):
+    """Wn windows of two uncorrelated sources at the angles th, snr_db each over unit noise"""
+    rng = np.random.default_rng(seed)
+    m = pos.shape[0]
+    amp = 10.0 ** (snr_db / 20.0)
+    xs = []
+    for _ in range(Wn):
+        X = (rng.standard_normal((m, snaps)) + 1j * rng.standard_normal((m, snaps))) / np.sqrt(2.0)
+        for t in th:
+            a = ro.steering(pos, LAM, math.radians(t))[0]
+            X += amp * a[:, None] * (rng.standard_normal(snaps) + 1j * rng.standard_normal(snaps))[None, :] / np.sqrt(2.0)
+        xs.append(X.T.reshape(-1))
+    return np.array(xs).astype(np.complex64)
+
+
+# ---- off-grid windows of the refinement and estimator tests -------------------------------------------------------------
+def offgrid_windows(pos, n_of, seed, snaps, noise=0.1, sep=None):
+    """complex64 windows; window w holds n_of[w] unit-power sources (random off-grid angles, or two `sep` degrees apart)
+    plus complex white noise of power noise^2 (20 dB at the default); returns (x, true angles per window)"""
+    rng = np.random.default_rng(seed)
+    m = pos.shape[0]
+    xs, truth = [], []
+    for S in n_of:
+        X = noise * (rng.standard_normal((m, snaps)) + 1j * rng.standard_normal((m, snaps))) / np.sqrt(2.0)
+        if sep is None:
+            angs = rng.uniform(0.0, 360.0, S)
+        else:
+            t0 = rng.uniform(0.0, 360.0)
+            angs = np.array([t0, t0 + sep])
+        for t in angs:
+            a = ro.steering(pos, LAM, np.deg2rad(t))[0]
+            X += a[:, None] * np.exp(2j * np.pi * rng.uniform(0.0, 1.0, snaps))[None, :]
+        xs.append(X.T.reshape(-1))  # x(r, c) = in[c * m + r]
+        truth.append(angs)
+    return np.ascontiguousarray(np.array(xs).astype(np.complex64)), truth

@@ -1,76 +1,18 @@
 """CPU: the DML oracle (tests/dml_oracle.py) against its definition's consequences: the Bartlett bin for one source,
 true bins on noiseless windows of every array kind, coherent-source resolution where MUSIC fails, a non-decreasing
 objective, mirror rows never taken twice, exact least-squares levels, exact power-of-two table scaling and the
-degenerate windows.  The windows of the resolution rows are shared with tests/test_gpu_dml.py."""
+degenerate windows.  The windows of the resolution rows (tests/helpers.py) are shared with tests/test_gpu_dml.py."""
 import numpy as np
 import pytest
 
-from gr_baz_b200 import synth
 from oracle import music_oracle as mo
 
 import dml_oracle as dm
 import estimator_oracle as eo
+from helpers import RESOLUTION, resolution_case, resolved
+from helpers import angle_windows as source_windows, array_wl as array, table_wl as table
 
 K = 360
-SNAPS = 1024
-
-
-def array(kind, m, seed=0):
-    """element positions in wavelengths: UCA (adjacent elements lambda / 2 apart), x- / y-axis ULA, random planar"""
-    if kind == "random":
-        return np.random.default_rng(seed).uniform(-1.5, 1.5, (m, 2))
-    geo = {"uca": "uca", "x": "ula_x", "y": "ula_y"}[kind]
-    return np.asarray(synth.antenna_array(geo, m), np.float64) * synth.SPACING
-
-
-def steering(pos, deg):
-    """a(theta) [.., M] for a geometry in wavelengths, exp(-j 2 pi (x cos + y sin))"""
-    t = np.radians(np.asarray(deg, np.float64))[..., None]
-    return np.exp(-2j * np.pi * (pos[:, 0] * np.cos(t) + pos[:, 1] * np.sin(t)))
-
-
-def table(pos, Kt=K):
-    return steering(pos, np.arange(Kt) * 360.0 / Kt).astype(np.complex64)
-
-
-def source_windows(pos, th, coherent, W, seed, snr_db=20.0, snaps=SNAPS):
-    """(x [W][snaps * M] complex64, truth [W][2]): two sources per window at th[w], 20 dB each over unit noise; coherent
-    sources carry one signal with a random unit phase between them (a path and its reflection)"""
-    rng = np.random.default_rng(seed)
-    m = pos.shape[0]
-    amp = 10.0 ** (snr_db / 20.0)
-    xs = []
-    for w in range(W):
-        X = (rng.standard_normal((m, snaps)) + 1j * rng.standard_normal((m, snaps))) / np.sqrt(2.0)
-        s = (rng.standard_normal(snaps) + 1j * rng.standard_normal(snaps)) / np.sqrt(2.0)
-        for j, t in enumerate(th[w]):
-            if not coherent and j:
-                s = (rng.standard_normal(snaps) + 1j * rng.standard_normal(snaps)) / np.sqrt(2.0)
-            g = np.exp(2j * np.pi * rng.uniform()) if coherent and j else 1.0
-            X += amp * g * steering(pos, t)[:, None] * s[None, :]
-        xs.append(X.T.reshape(-1))
-    return np.ascontiguousarray(np.array(xs).astype(np.complex64))
-
-
-def resolution_case(kind, m, coherent, sep, W=40):
-    """the windows of one row of the resolution table: seeded first angles (x-ULA: inside (20, 160 - sep) degrees, away
-    from end-fire, so that each source is the lower bin of its mirror pair)"""
-    seed = 1000 * m + 10 * sep + (1 if coherent else 0) + (5 if kind == "x" else 0)
-    rng = np.random.default_rng(seed)
-    t0 = rng.uniform(20.0, 160.0 - sep, W) if kind == "x" else rng.uniform(0.0, 360.0, W)
-    th = np.stack([t0, (t0 + sep) % 360.0], axis=1)
-    pos = array(kind, m)
-    return pos, table(pos), source_windows(pos, th, coherent, W, seed + 7), th
-
-
-def circ(a, b):
-    d = np.abs(np.asarray(a, np.float64) - np.asarray(b, np.float64)) % 360.0
-    return np.minimum(d, 360.0 - d)
-
-
-def resolved(angles, truth, tol=2.0):
-    """both sources within tol degrees of a reported slot"""
-    return all(min(circ(a, t) for a in angles) <= tol for t in truth)
 
 
 def music_local(R, tab, n):
@@ -81,19 +23,6 @@ def music_local(R, tab, n):
     a = tab.astype(np.complex128)
     P = 1.0 / np.sum(np.abs(a.conj() @ G) ** 2, axis=1)
     return [q[0] for q in mo.pick_local_maxima(P, n, tab.shape[0]) if q[2] >= 0]
-
-
-# (kind, M, coherent, separation) -> (MUSIC resolved, DML resolved) of 40 windows: this oracle's counts, fixed
-RESOLUTION = {
-    ("uca", 8, True, 20): (0, 30),
-    ("uca", 8, True, 40): (3, 27),
-    ("uca", 16, True, 20): (4, 34),
-    ("uca", 16, True, 40): (8, 40),
-    ("x", 8, True, 20): (0, 38),
-    ("x", 8, False, 20): (0, 39),
-    ("uca", 8, False, 20): (40, 40),
-    ("uca", 16, False, 40): (40, 40),
-}
 
 
 # ---- definition --------------------------------------------------------------------------------------------------------

@@ -3,28 +3,25 @@ every entry point, and its refusals.
 
 The oracle runs on the device table read back with get_table (the table itself is checked to one float32 ulp), so what
 is compared is the pipeline: flat scan, both peak rules, the decode and the 2-D refinement."""
-import os
 import struct
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
-from gr_baz_b200 import _capi, build
+from gr_baz_b200 import _capi
 from gr_baz_b200.music_doa_azel import music_doa_azel
 from oracle import music_oracle as mo
 
 import azel_oracle as ao
+import gpu_harness as gh
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LAM = 1.0
 SNAPS = 256
 W = 4
 EXCL = 2
-SENTINEL = -7
 TIE = 1e-12      # bins may differ where the oracle's strengths at the two bins agree to this
 FLIP = 1e-9      # refinement decisions this close to flipping may go either way
 L_RTOL = 1e-5
@@ -36,32 +33,11 @@ GEOMETRIES = {
     "ura": (lambda m: ao.ura_xyz(4, 4, LAM), (0.0, 90.0)),
 }
 MATRIX = [(m, g) for m in (3, 4, 8, 16) for g in ("uca", "uca_z")] + [(16, "ura")]
+ALL = ("levels", "spectrum", "bins", "counts")
 
 
 def handle(m, n, grid, pos, snaps=SNAPS):
     return music_doa_azel(m, n, m * snaps, grid.n_az, grid.n_el, (grid.el_lo, grid.el_hi), pos, LAM)
-
-
-def dev_call(blk, x, n, K, spectrum=True, bins=True, levels=True, counts=True):
-    dev = torch.device("cuda:0")
-    Wn = x.shape[0]
-    d_in = torch.from_numpy(x.view(np.float32)).to(dev)
-    o = {"azimuth": torch.full((Wn, n), SENTINEL, dtype=torch.float32, device=dev),
-         "elevation": torch.full((Wn, n), SENTINEL, dtype=torch.float32, device=dev)}
-    if levels:
-        o["levels"] = torch.full((Wn, n), SENTINEL, dtype=torch.float32, device=dev)
-    if spectrum:
-        o["spectrum"] = torch.full((Wn, K), SENTINEL, dtype=torch.float32, device=dev)
-    if bins:
-        o["bins"] = torch.full((Wn, n), SENTINEL, dtype=torch.int32, device=dev)
-    if counts:
-        o["counts"] = torch.full((Wn,), SENTINEL, dtype=torch.int32, device=dev)
-    p = lambda k: o[k].data_ptr() if k in o else None
-    l0 = blk.launch_count()
-    blk.process_device(d_in.data_ptr(), Wn, p("azimuth"), p("elevation"), p("levels"), p("spectrum"), p("bins"), p("counts"),
-                       stream=torch.cuda.current_stream().cuda_stream)
-    torch.cuda.synchronize()
-    return {k: v.cpu().numpy() for k, v in o.items()}, blk.launch_count() - l0
 
 
 def ulps_apart(a, b, circular=True):
@@ -101,9 +77,9 @@ def test_parity_with_oracle(m, geometry):
                     ctx = (m, geometry, n_az, n_el, n, rule, peak)
                     blk.set_peak_mode("top_bins" if peak == "top" else "local_maxima", EXCL)
                     blk.set_refine(False)
-                    off, _ = dev_call(blk, x, n, grid.K)
+                    off, _ = gh.device_call(blk, x, ALL)
                     blk.set_refine(True)
-                    on, _ = dev_call(blk, x, n, grid.K)
+                    on, _ = gh.device_call(blk, x, ALL)
                     for k in ("bins", "spectrum", "counts"):
                         assert np.array_equal(on[k].view(np.int32), off[k].view(np.int32)), (ctx, k)
                     for w in range(W):
@@ -153,7 +129,7 @@ def test_refinement_beats_the_half_step_at_20db():
     err = {}
     for refine in (False, True):
         blk.set_refine(refine)
-        o, _ = dev_call(blk, x, n, grid.K, spectrum=False)
+        o, _ = gh.device_call(blk, x, ("levels", "bins", "counts"))
         ea = [abs((float(o["azimuth"][w, 0]) - truth[w][0][0] + 180.0) % 360.0 - 180.0) for w in range(len(x))]
         ee = [abs(float(o["elevation"][w, 0]) - truth[w][0][1]) for w in range(len(x))]
         err[refine] = (float(np.sqrt(np.mean(np.square(ea)))), float(np.sqrt(np.mean(np.square(ee)))))
@@ -174,7 +150,7 @@ def test_host_and_device_entries_agree():
         blk.set_peak_mode("local_maxima", EXCL)
         blk.set_refine(True)
         spec = Wn * grid.K * 4 < (1 << 30)
-        ref, launches = dev_call(blk, x, n, grid.K, spectrum=spec)
+        ref, launches = gh.device_call(blk, x, ("levels", "bins", "counts") + (("spectrum",) if spec else ()))
         if n_el == 181:
             assert launches > 2 * 6, launches  # more than one workspace sub-batch
         outs = [np.zeros((Wn, n), np.float32) for _ in range(3)] + ([np.zeros((Wn, grid.K), np.float32)] if spec else [])
@@ -187,7 +163,7 @@ def test_host_and_device_entries_agree():
         a2, e2 = np.zeros((Wn, n), np.float32), np.zeros((Wn, n), np.float32)
         blk.work(Wn, [x], [a2, e2])
         assert np.array_equal(a2, ref["azimuth"]) and np.array_equal(e2, ref["elevation"])
-        nb, _ = dev_call(blk, x, n, grid.K, spectrum=False, bins=False, levels=False, counts=False)
+        nb, _ = gh.device_call(blk, x)
         assert np.array_equal(nb["azimuth"], ref["azimuth"]) and np.array_equal(nb["elevation"], ref["elevation"])
         blk.close()
 
@@ -198,10 +174,10 @@ def test_fused_kernels_never_run():
         grid = ao.Grid(36, 10, 0.0, 90.0)
         blk = handle(m, 1, grid, pos, snaps=1024)
         x, _ = ao.windows(pos, LAM, [1] * 16, 5, 1024)
-        _, launches = dev_call(blk, x, 1, grid.K, spectrum=False, levels=True, bins=False, counts=False)
+        _, launches = gh.device_call(blk, x, ("levels",))
         assert launches == 4, launches  # covariance + eigenvectors + peak scan + decode
         blk.set_refine(True)
-        _, launches = dev_call(blk, x, 1, grid.K, spectrum=False, levels=True, bins=False, counts=False)
+        _, launches = gh.device_call(blk, x, ("levels",))
         assert launches == 5, launches
         blk.close()
 
@@ -212,11 +188,11 @@ def test_settable_table_stage_timing_and_reducers():
     grid = ao.Grid(36, 10, 0.0, 90.0)
     blk = handle(m, n, grid, pos)
     x, _ = ao.windows(pos, LAM, [1] * 8, 9, SNAPS)
-    geo, _ = dev_call(blk, x, n, grid.K)
+    geo, _ = gh.device_call(blk, x, ALL)
     T = blk.array_response_c64()
     assert T.shape == (grid.n_el, grid.n_az, m)
     blk.set_array_response(T)  # the same manifold as a measured table: same grid results
-    tab, _ = dev_call(blk, x, n, grid.K)
+    tab, _ = gh.device_call(blk, x, ALL)
     for k in geo:
         assert np.array_equal(geo[k].view(np.int32), tab[k].view(np.int32)), k
     with pytest.raises(_capi.MusicB200Error) as e:
@@ -225,7 +201,7 @@ def test_settable_table_stage_timing_and_reducers():
     blk.set_array_geometry(pos, LAM)
     blk.set_refine(True)
     blk.set_stage_timing(True)
-    dev_call(blk, x, n, grid.K)
+    gh.device_call(blk, x, ALL)
     ms, chunks = blk.stage_times_ms()
     assert chunks == 1 and all(v > 0 for v in ms)
     mean, res, wsum = blk.reduce_angles(geo["azimuth"], geo["levels"])
@@ -288,27 +264,16 @@ def music_oracle_handle(m, n):
     return music_doa(m, n, m * SNAPS, mo.steering_table_c64([[0.5 * e, 0.0] for e in range(m)], K, LAM), K)
 
 
-def test_cpp_block_azel(tmp_path):
-    build.build_cuda()
-    subprocess.check_call(["make", "-C", os.path.join(ROOT, "lib"), "-s"])
+def test_cpp_block_azel():
     m, n, Wn = 8, 2, 12
     pos = ao.uca_xyz(m, LAM, alternate_z=True)
     grid = ao.Grid(72, 19, -90.0, 90.0)
     x, _ = ao.windows(pos, LAM, [n] * Wn, 55, SNAPS, (-90.0, 90.0))
-    fin, fout = tmp_path / "in.bin", tmp_path / "out.bin"
-    with open(fin, "wb") as f:
-        f.write(struct.pack("<10I", m, n, m * SNAPS, grid.n_az, grid.n_el, Wn, 1, EXCL, 1, 1))
-        f.write(struct.pack("<3d", grid.el_lo, grid.el_hi, LAM))
-        f.write(np.ascontiguousarray(pos).tobytes())
-        f.write(x.view(np.float32).tobytes())
-    r = subprocess.run([os.path.join(ROOT, "lib", "_build", "test_block_azel"), str(fin), str(fout)], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    raw = np.fromfile(fout, dtype=np.float32)
-    o, got = 0, {}
-    for k, size in (("azimuth", n), ("elevation", n), ("levels", n), ("spectrum", grid.K), ("bins", n), ("counts", 1)):
-        got[k] = raw[o:o + Wn * size].reshape(Wn, size)
-        o += Wn * size
-    assert o == raw.size
+    c = gh.run_cpp_block("test_block_azel", struct.pack("<10I", m, n, m * SNAPS, grid.n_az, grid.n_el, Wn, 1, EXCL, 1, 1) +
+                         struct.pack("<3d", grid.el_lo, grid.el_hi, LAM), [np.ascontiguousarray(pos), x],
+                         [(k, np.float32, Wn * size) for k, size in (("azimuth", n), ("elevation", n), ("levels", n),
+                                                                     ("spectrum", grid.K), ("bins", n), ("counts", 1))])
+    got = {k: v.reshape(Wn, -1) for k, v in c.items()}
     py = handle(m, n, grid, pos)
     py.set_peak_mode("local_maxima", EXCL)
     py.set_source_rule("mdl")

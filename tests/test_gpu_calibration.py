@@ -1,30 +1,25 @@
 """GPU: receiver calibration (music_b200_set_calibration, music_b200_calib_*) - the correction of R in every entry and
 mode, and the gain estimate against its fp64 definition (tests/calibration_oracle.py) and against the truth."""
 import math
-import os
 import struct
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 import torch
 
 from gr_baz_b200 import _capi
-from gr_baz_b200.music_doa import music_doa
 from gr_baz_b200.music_doa_azel import music_doa_azel
 
 import calibration_oracle as co
+import gpu_harness as gh
+import helpers
 import refine_oracle as ro
-import test_dml_oracle as td
-from test_gpu_root_music import LAM, ula
+from helpers import LAM, array_wl, corrupt, random_gains, ula
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SENTINEL = -7
-DEV = torch.device("cuda:0")
-STREAM = lambda: torch.cuda.current_stream().cuda_stream
+ALL = ("levels", "bins", "spectrum", "P64", "R", "eigvals")
+BEAMS = ("levels", "bins", "counts", "weights", "beams")
 
 
 # ---- fixtures --------------------------------------------------------------------------------------------------------
@@ -44,53 +39,12 @@ def windows(pos, degs_per_window, seed, snaps, snr_db=20.0, azel=False):
     return np.ascontiguousarray(np.array(xs).astype(np.complex64))
 
 
-def corrupt(x, g):
-    """x_raw = g o x per snapshot, rounded to complex64 (exact for real powers of two)"""
-    m = len(g)
-    X = x.astype(np.complex128).reshape(x.shape[0], -1, m) * np.asarray(g)[None, None, :]
-    return np.ascontiguousarray(X.reshape(x.shape[0], -1).astype(np.complex64))
-
-
-def random_gains(rng, m):
-    return 10.0 ** (rng.uniform(-3.0, 3.0, m) / 20.0) * np.exp(1j * rng.uniform(-math.pi, math.pi, m))
-
-
 def pow2_gains(rng, m):
     return rng.choice([-1.0, 1.0], m) * 2.0 ** rng.integers(-2, 3, m)
 
 
 def handle(m, n, snaps, K, pos, mode="top_bins", rule="fixed", est=("music", 0.0), refine=False, devices=None):
-    blk = music_doa(m, n, m * snaps, np.ones((K, m), np.complex64), K, devices=devices)
-    blk.set_array_geometry(pos, LAM)
-    blk.set_estimator(*est)
-    blk.set_source_rule(rule)
-    blk.set_peak_mode(mode, 0)
-    if refine:
-        blk.set_refine(True)
-    return blk
-
-
-def ex_call(blk, x, K, spectrum=True, p64=True, R=True, ev=True):
-    """one process_device_ex call with every output; returns (outputs, launches)"""
-    W, m, n = x.shape[0], blk.m, blk.n
-    d_in = torch.from_numpy(x.view(np.float32)).to(DEV)
-    o = {"angles": torch.full((W, n), SENTINEL, dtype=torch.float32, device=DEV),
-         "levels": torch.full((W, n), SENTINEL, dtype=torch.float32, device=DEV),
-         "bins": torch.full((W, n), SENTINEL, dtype=torch.int32, device=DEV)}
-    if spectrum:
-        o["spectrum"] = torch.full((W, K), SENTINEL, dtype=torch.float32, device=DEV)
-    if p64:
-        o["P64"] = torch.full((W, K), SENTINEL, dtype=torch.float64, device=DEV)
-    if R:
-        o["R"] = torch.full((W, m, m, 2), SENTINEL, dtype=torch.float64, device=DEV)
-    if ev:
-        o["ev"] = torch.full((W, m), SENTINEL, dtype=torch.float64, device=DEV)
-    p = lambda k: o[k].data_ptr() if k in o else None
-    l0 = blk.launch_count()
-    blk.process_device(d_in.data_ptr(), W, p("angles"), p("levels"), p("spectrum"), p("bins"), stream=STREAM(), d_P64=p("P64"),
-                       d_R=p("R"), d_eigvals=p("ev"))
-    torch.cuda.synchronize()
-    return {k: v.cpu().numpy() for k, v in o.items()}, blk.launch_count() - l0
+    return gh.make_block(m, n, snaps, K, pos=pos, est=est, rule=rule, mode=mode, refine=refine, devices=devices)
 
 
 def same(a, b, ctx):
@@ -101,17 +55,17 @@ def same(a, b, ctx):
 
 # ---- 1. identity is a no-op --------------------------------------------------------------------------------------------
 MODES = [  # (name, m, n, pos, handle kwargs)
-    ("top_bins", 8, 2, td.array("uca", 8), {}),
-    ("local", 8, 2, td.array("uca", 8), {"mode": "local_maxima"}),
+    ("top_bins", 8, 2, array_wl("uca", 8), {}),
+    ("local", 8, 2, array_wl("uca", 8), {"mode": "local_maxima"}),
     ("roots", 8, 2, ula(8, "x"), {"mode": "roots"}),
     ("esprit", 8, 2, ula(8, "x"), {"mode": "esprit"}),
-    ("dml", 8, 2, td.array("uca", 8), {"mode": "dml"}),
-    ("mvdr", 8, 2, td.array("uca", 8), {"est": ("mvdr", 0.01), "mode": "local_maxima"}),
-    ("bartlett", 8, 2, td.array("uca", 8), {"est": ("bartlett", 0.0), "mode": "local_maxima"}),
-    ("mdl", 8, 3, td.array("uca", 8), {"rule": "mdl", "mode": "local_maxima"}),
-    ("refine", 8, 2, td.array("uca", 8), {"refine": True, "mode": "local_maxima"}),
-    ("m4", 4, 1, td.array("uca", 4), {}),
-    ("m5", 5, 2, td.array("uca", 5), {}),
+    ("dml", 8, 2, array_wl("uca", 8), {"mode": "dml"}),
+    ("mvdr", 8, 2, array_wl("uca", 8), {"est": ("mvdr", 0.01), "mode": "local_maxima"}),
+    ("bartlett", 8, 2, array_wl("uca", 8), {"est": ("bartlett", 0.0), "mode": "local_maxima"}),
+    ("mdl", 8, 3, array_wl("uca", 8), {"rule": "mdl", "mode": "local_maxima"}),
+    ("refine", 8, 2, array_wl("uca", 8), {"refine": True, "mode": "local_maxima"}),
+    ("m4", 4, 1, array_wl("uca", 4), {}),
+    ("m5", 5, 2, array_wl("uca", 5), {}),
 ]
 
 
@@ -124,12 +78,12 @@ def test_identity_is_a_no_op(name, m, n, pos, kw):
     a, b = handle(m, n, snaps, K, pos, **kw), handle(m, n, snaps, K, pos, **kw)
     b.set_calibration(np.ones(m))
     assert np.array_equal(b.calibration(), np.ones(m))
-    ra, _ = ex_call(a, x, K)
-    rb, _ = ex_call(b, x, K)
+    ra, _ = gh.device_call(a, x, ALL)
+    rb, _ = gh.device_call(b, x, ALL)
     same(ra, rb, name)
     if name in ("top_bins", "m4"):
         # bins of the default (fused where the shape allows) call
-        rd, _ = ex_call(a, x, K, spectrum=False, p64=False, R=False, ev=False)
+        rd, _ = gh.device_call(a, x, ("levels", "bins"))
         assert np.array_equal(rd["bins"], rb["bins"])
     a.close()
     b.close()
@@ -142,14 +96,14 @@ def test_exact_correction_device(m, n, mode):
     """x_raw = g o x and R_raw = G R G^H are exact, and so is the correction: a calibrated handle on x_raw is
     byte-identical to an uncalibrated one on x (process_device_ex with d_R: both unfused)"""
     K, snaps = 720, 256
-    pos = td.array("uca", m)
+    pos = array_wl("uca", m)
     rng = np.random.default_rng(20 + m)
     x = windows(pos, [rng.uniform(0, 360, n) for _ in range(10)], 21 + m, snaps)
     g = pow2_gains(rng, m)
     a, b = handle(m, n, snaps, K, pos, mode=mode), handle(m, n, snaps, K, pos, mode=mode)
     b.set_calibration(g)
-    ra, la = ex_call(a, x, K)
-    rb, lb = ex_call(b, corrupt(x, g), K)
+    ra, la = gh.device_call(a, x, ALL)
+    rb, lb = gh.device_call(b, corrupt(x, g), ALL)
     same(ra, rb, (m, n, mode))
     assert lb == la + 1  # plus the apply kernel
     a.close()
@@ -159,7 +113,7 @@ def test_exact_correction_device(m, n, mode):
 def test_exact_correction_every_entry():
     """host, device, _counts, planar host / device and the default peak-only call (n = 2: unfused) agree byte for byte"""
     m, n, K, snaps, W = 8, 2, 720, 256, 24
-    pos = td.array("uca", m)
+    pos = array_wl("uca", m)
     rng = np.random.default_rng(31)
     x = windows(pos, [rng.uniform(0, 360, 2) for _ in range(W)], 32, snaps)
     g = pow2_gains(rng, m)
@@ -173,28 +127,15 @@ def test_exact_correction_every_entry():
         return {"a": ang, "l": lvl, "s": spec, "b": blk.last_bins().copy()}
 
     def counts(blk, xin):
-        d_in = torch.from_numpy(xin.view(np.float32)).to(DEV)
-        o = {k: torch.full((W, n), SENTINEL, dtype=dt, device=DEV) for k, dt in (("a", torch.float32), ("l", torch.float32), ("b", torch.int32))}
-        o["c"] = torch.full((W,), SENTINEL, dtype=torch.int32, device=DEV)
-        blk.process_device(d_in.data_ptr(), W, o["a"].data_ptr(), o["l"].data_ptr(), None, o["b"].data_ptr(), stream=STREAM(),
-                           d_counts=o["c"].data_ptr())
-        torch.cuda.synchronize()
-        return {k: v.cpu().numpy() for k, v in o.items()}
+        return gh.device_call(blk, xin, ("levels", "bins", "counts"))[0]
 
     def planar_host(blk, xin):
-        streams = [np.ascontiguousarray(xin.reshape(W, snaps, m)[:, :, r].reshape(-1)) for r in range(m)]
         ang, lvl = np.zeros((W, n), np.float32), np.zeros((W, n), np.float32)
-        assert blk.work_planar(W, streams, [ang, lvl]) == W
+        assert blk.work_planar(W, helpers.antenna_streams(xin, m), [ang, lvl]) == W
         return {"a": ang, "l": lvl, "b": blk.last_bins().copy()}
 
     def planar_device(blk, xin):
-        streams = [torch.from_numpy(np.ascontiguousarray(xin.reshape(W, snaps, m)[:, :, r].reshape(-1)).view(np.float32)).to(DEV)
-                   for r in range(m)]
-        o = {k: torch.full((W, n), SENTINEL, dtype=dt, device=DEV) for k, dt in (("a", torch.float32), ("l", torch.float32), ("b", torch.int32))}
-        blk.process_planar_device([s.data_ptr() for s in streams], snaps, W, o["a"].data_ptr(), o["l"].data_ptr(), None, o["b"].data_ptr(),
-                                  stream=STREAM())
-        torch.cuda.synchronize()
-        return {k: v.cpu().numpy() for k, v in o.items()}
+        return gh.planar_device_call(blk, helpers.antenna_streams(xin, m), snaps, W, ("levels", "bins"))[0]
 
     for f in (host, counts, planar_host, planar_device):
         same(f(a, x), f(b, xr), f.__name__)
@@ -205,7 +146,7 @@ def test_exact_correction_every_entry():
 def test_exact_correction_azel():
     """an az-el handle: calibrated on x_raw equals uncalibrated on x, host and device"""
     m, n, snaps, W = 8, 2, 256, 12
-    pos = np.c_[td.array("uca", m), np.r_[np.zeros(4), 0.3 * np.ones(4)]]
+    pos = np.c_[array_wl("uca", m), np.r_[np.zeros(4), 0.3 * np.ones(4)]]
     rng = np.random.default_rng(41)
     x = windows(pos, [[(rng.uniform(0, 360), rng.uniform(0, 40)) for _ in range(2)] for _ in range(W)], 42, snaps, azel=True)
     g = pow2_gains(rng, m)
@@ -226,9 +167,8 @@ def test_exact_correction_azel():
 
 def test_exact_correction_beams():
     """beams entries: the weights of the calibrated handle are c o w exactly and the beams are identical"""
-    from test_gpu_beams import beams_call
     m, n, K, snaps, W = 8, 2, 720, 256, 12
-    pos = td.array("uca", m)
+    pos = array_wl("uca", m)
     rng = np.random.default_rng(51)
     x = windows(pos, [rng.uniform(0, 360, 2) for _ in range(W)], 52, snaps)
     g = pow2_gains(rng, m)
@@ -237,8 +177,8 @@ def test_exact_correction_beams():
         for blk in (a, b):
             blk.set_beamformer(rule, loading)
         b.set_calibration(g)
-        ra, la = beams_call(a, x, n, K)
-        rb, lb = beams_call(b, corrupt(x, g), n, K)
+        ra, la = gh.device_call(a, x, BEAMS)
+        rb, lb = gh.device_call(b, corrupt(x, g), BEAMS)
         for k in ("angles", "levels", "bins", "counts", "beams"):
             assert ra[k].tobytes() == rb[k].tobytes(), (rule, k)
         c = co.inverse(g)
@@ -254,7 +194,7 @@ def test_multi_device_entries():
     if G < 2:
         pytest.skip("needs two GPUs")
     m, n, K, snaps, W = 8, 2, 720, 256, 16
-    pos = td.array("uca", m)
+    pos = array_wl("uca", m)
     rng = np.random.default_rng(61)
     x = windows(pos, [rng.uniform(0, 360, 2) for _ in range(W)], 62, snaps)
     g = pow2_gains(rng, m)
@@ -275,16 +215,15 @@ def test_multi_device_entries():
 def test_complex_gains_correct_R(m):
     """d_R of a calibrated handle = C R_raw C^H from an uncalibrated call's d_R, to 1e-15 |R_ij| per entry"""
     K, snaps, W = 360, 128, 8
-    pos = td.array("uca", m) if m > 2 else ula(2, "x")
+    pos = array_wl("uca", m) if m > 2 else ula(2, "x")
     rng = np.random.default_rng(70 + m)
     g = random_gains(rng, m)
     xr = corrupt(windows(pos, [rng.uniform(0, 360, 1) for _ in range(W)], 71, snaps), g)
     a, b = handle(m, 1, snaps, K, pos), handle(m, 1, snaps, K, pos)
     b.set_calibration(g)
     assert np.array_equal(b.calibration(), g)
-    Ra = ex_call(a, xr, K)[0]["R"]
-    Rb = ex_call(b, xr, K)[0]["R"]
-    Ra, Rb = Ra[..., 0] + 1j * Ra[..., 1], Rb[..., 0] + 1j * Rb[..., 1]
+    Ra = gh.device_call(a, xr, ALL)[0]["R"]
+    Rb = gh.device_call(b, xr, ALL)[0]["R"]
     want = np.array([co.correct(R, g) for R in Ra])
     assert np.all(np.abs(Rb - want) <= 1e-15 * np.abs(want))
     a.close()
@@ -293,7 +232,7 @@ def test_complex_gains_correct_R(m):
 
 # ---- 4 / 5. the estimator against the oracle and against the truth -----------------------------------------------------
 EST_CASES = [("ula2", ula(2, "x"), co.PHASE, 25.0), ("ula4", ula(4, "x"), co.GAIN_PHASE, 50.0),
-             ("uca8", td.array("uca", 8), co.GAIN_PHASE, 130.0), ("uca16", td.array("uca", 16), co.GAIN_PHASE, 290.0)]
+             ("uca8", array_wl("uca", 8), co.GAIN_PHASE, 130.0), ("uca16", array_wl("uca", 16), co.GAIN_PHASE, 290.0)]
 KINDS = {co.PHASE: "phase", co.GAIN_PHASE: "gain_phase"}
 
 
@@ -320,10 +259,10 @@ def test_estimator(name, pos, kind, az):
     assert abs(sweeps - sw_ref) <= 1 and abs(rho - rho_ref) <= 1e-9
     # device accumulation, split over three calls
     blk.calib_reset()
-    d_in = torch.from_numpy(xr.view(np.float32).reshape(-1)).to(DEV)
+    d_in = torch.from_numpy(xr.view(np.float32).reshape(-1)).to(gh.DEV)
     step = m * snaps * 2
     for lo, hi in ((0, 5), (5, 6), (6, W)):
-        blk.calib_accumulate_device(d_in[lo * step:].data_ptr(), hi - lo, stream=STREAM())
+        blk.calib_accumulate_device(d_in[lo * step:].data_ptr(), hi - lo, stream=gh.stream())
     gd, rho_d, sw_d = blk.calib_solve(az, 0.0, KINDS[kind])
     assert np.max(np.abs(gd - got)) <= 1e-12 * np.max(np.abs(got)) and abs(sw_d - sweeps) <= 1
     # the accumulator is kept: a second solve gives the same answer
@@ -337,7 +276,7 @@ def test_estimator(name, pos, kind, az):
 
 def test_estimator_azel():
     m, snaps, W = 8, 1024, 16
-    pos = np.c_[td.array("uca", m), np.r_[np.zeros(4), 0.3 * np.ones(4)]]
+    pos = np.c_[array_wl("uca", m), np.r_[np.zeros(4), 0.3 * np.ones(4)]]
     rng = np.random.default_rng(91)
     g = random_gains(rng, m)
     az, el = 200.0, 25.0
@@ -366,7 +305,7 @@ def test_doa_restored(case):
     """uncalibrated errors on corrupted windows are large; with the estimated gains the RMS error is within 1.5x of the
     same handle on clean windows"""
     if case == "uca8_local":
-        m, n, pos, mode, cal_az = 8, 2, td.array("uca", 8), "local_maxima", 130.0
+        m, n, pos, mode, cal_az = 8, 2, array_wl("uca", 8), "local_maxima", 130.0
     else:
         m, n, pos, mode, cal_az = 8, 2, ula(8, "x"), "roots", 50.0
     K, snaps, W = 3600, 512, 40
@@ -404,7 +343,7 @@ def test_doa_restored(case):
 def test_errors_and_persistence():
     L = _capi.load()
     m, snaps, K = 4, 64, 360
-    pos = td.array("uca", m)
+    pos = array_wl("uca", m)
     blk = handle(m, 1, snaps, K, pos)
     EINVAL = _capi.EINVAL
     g = np.ones(2 * m)
@@ -463,29 +402,16 @@ def test_errors_and_persistence():
 def test_cpp_block():
     """calibrate() armed on the C++ block, corrupted items over several work() calls: the gains it applies equal the
     Python block's estimate on the same items, and its later DOA outputs equal the Python block's with those gains"""
-    exe = os.path.join(ROOT, "lib", "_build", "test_block_calibration")
     m, n, K, snaps, C, W, chunk = 8, 2, 720, 256, 12, 10, 5
-    pos = td.array("uca", m)
+    pos = array_wl("uca", m)
     rng = np.random.default_rng(111)
     g = random_gains(rng, m)
     cal = corrupt(windows(pos, [[70.0]] * C, 112, snaps), g)
     x = corrupt(windows(pos, [rng.uniform(0, 360, 2) for _ in range(W)], 113, snaps), g)
-    with tempfile.TemporaryDirectory() as tdir:
-        fin, fout = os.path.join(tdir, "in.bin"), os.path.join(tdir, "out.bin")
-        with open(fin, "wb") as f:
-            f.write(struct.pack("<9I", m, n, m * snaps, K, C, W, 1, 2, chunk))
-            f.write(struct.pack("<2d", 70.0, LAM))
-            f.write(np.ascontiguousarray(pos, np.float64).tobytes())
-            f.write(cal.view(np.float32).tobytes())
-            f.write(x.view(np.float32).tobytes())
-        r = subprocess.run([exe, fin, fout], capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr
-        raw = open(fout, "rb").read()
-    cg = np.frombuffer(raw[:16 * m], np.complex128)
-    crho = np.frombuffer(raw[16 * m:16 * m + 8], np.float64)[0]
-    o = 16 * m + 8
-    ca = np.frombuffer(raw[o:o + 4 * W * n], np.float32)
-    cb = np.frombuffer(raw[o + 4 * W * n:o + 8 * W * n], np.int32)
+    c = gh.run_cpp_block("test_block_calibration", struct.pack("<9I", m, n, m * snaps, K, C, W, 1, 2, chunk) +
+                         struct.pack("<2d", 70.0, LAM), [np.ascontiguousarray(pos, np.float64), cal, x],
+                         [("g", np.complex128, m), ("rho", np.float64, 1), ("a", np.float32, W * n), ("b", np.int32, W * n)])
+    cg, crho, ca, cb = c["g"], c["rho"][0], c["a"], c["b"]
     blk = handle(m, n, snaps, K, pos, mode="local_maxima")
     blk.calib_reset()
     for lo in range(0, C, chunk):  # the same split over accumulate calls as the block's work() calls

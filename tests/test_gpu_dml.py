@@ -3,10 +3,7 @@ point, on geometric, planar, calibrated, scaled and zero-row tables, and the oth
 
 The oracle runs on the GPU's own covariance (d_R), so what is compared is the DML stage itself.  A window whose oracle
 trajectory passed through a search with a relative margin <= 1e-9 (a near-tie) may take the other branch."""
-import os
 import struct
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
@@ -17,29 +14,25 @@ from gr_baz_b200.music_doa import music_doa
 from gr_baz_b200.music_doa_azel import music_doa_azel
 
 import dml_oracle as dm
+import gpu_harness as gh
 import helpers
-import test_dml_oracle as td
-from test_gpu_root_music import LAM, dev_call
+from helpers import LAM, RESOLUTION, SNAPS, angle_windows, array_wl, resolution_case, resolved, table_wl
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 DML = 4
 FLIP = 1e-9
+PEAKS = ("levels", "bins")
 
 
 def handle(tab, n, snaps, rule="fixed", mode="dml", devices=None):
-    K, m = tab.shape
-    blk = music_doa(m, n, m * snaps, tab, K, devices=devices)
-    blk.set_source_rule(rule)
-    blk.set_peak_mode(mode, 0)
-    return blk
+    return gh.make_block(tab.shape[1], n, snaps, table=tab, rule=rule, mode=mode, devices=devices)
 
 
 def tables(m, K):
     """(name, [K][m] complex64): x-axis ULA, UCA, random planar array and a calibrated UCA"""
-    uca = td.table(td.array("uca", m), K)
-    return [("ula_x", td.table(td.array("x", m), K)), ("uca", uca), ("planar", helpers.planar_table(m, K, 50 + m)),
+    uca = table_wl(array_wl("uca", m), K)
+    return [("ula_x", table_wl(array_wl("x", m), K)), ("uca", uca), ("planar", helpers.planar_table(m, K, 50 + m)),
             ("calibrated", helpers.calibrated_table(uca, 60 + m))]
 
 
@@ -50,9 +43,9 @@ def mixed_windows(m, tab_pos, seed, snaps=256):
     for coherent, S in ((True, 2), (True, 2), (False, 2), (False, 3), (False, 1), (False, 0)):
         th = [rng.uniform(0.0, 360.0, S)]
         if S == 0:
-            out.append(td.source_windows(tab_pos, [[]], False, 1, seed + len(out), snaps=snaps))
+            out.append(angle_windows(tab_pos, [[]], False, 1, seed + len(out), snaps=snaps))
         else:
-            out.append(td.source_windows(tab_pos, th, coherent, 1, seed + len(out), snaps=snaps))
+            out.append(angle_windows(tab_pos, th, coherent, 1, seed + len(out), snaps=snaps))
     return np.concatenate(out)
 
 
@@ -85,7 +78,7 @@ def test_parity_with_oracle(m):
     K, snaps = 360, 256
     edge = total = 0
     for ti, (name, tab) in enumerate(tables(m, K)):
-        pos = td.array("uca", m) if name in ("uca", "calibrated") else td.array("x", m) if name == "ula_x" else None
+        pos = array_wl("uca", m) if name in ("uca", "calibrated") else array_wl("x", m) if name == "ula_x" else None
         if pos is None:  # the planar table's own positions are not kept: sources along random table rows
             rng = np.random.default_rng(m + 5)
             vecs = [[tab[k] for k in rng.choice(K, S, replace=False)] for S in (2, 2, 1, 3, 0, 2)]
@@ -97,10 +90,10 @@ def test_parity_with_oracle(m):
                 continue
             for rule in ("fixed", "mdl"):
                 blk = handle(tab, n, snaps, rule)
-                out, _ = dev_call(blk, x, n, K, R=True)
+                out, _ = gh.device_call(blk, x, PEAKS + ("R",))
                 counts = None
                 if rule == "mdl":
-                    cnt, _ = dev_call(blk, x, n, K, counts=True)
+                    cnt, _ = gh.device_call(blk, x, PEAKS + ("counts",))
                     assert np.array_equal(cnt["bins"], out["bins"]) and np.array_equal(cnt["levels"], out["levels"])
                     counts = cnt["counts"]
                 blk.close()
@@ -116,11 +109,11 @@ def test_single_source_is_the_bartlett_bin():
     x = synth.gen_windows_numpy(cfg, synth.BASE_SEED + 2, 0, W)
     tab = helpers.table_for(cfg)
     blk = handle(tab, 1, cfg["snapshots"])
-    out, launches = dev_call(blk, x, 1, K, R=True)
+    out, launches = gh.device_call(blk, x, PEAKS + ("R",))
     blk.close()
     bart = music_doa(4, 1, cfg["nsamples"], tab, K)
     bart.set_estimator("bartlett", 0.0)
-    bo, _ = dev_call(bart, x, 1, K)
+    bo, _ = gh.device_call(bart, x, PEAKS)
     bart.close()
     for w in range(W):
         if out["bins"][w, 0] != bo["bins"][w, 0]:
@@ -134,19 +127,19 @@ def test_coherent_resolution(case):
     """the seeded coherent rows of the oracle's resolution table: the GPU resolves the oracle's count (up to near-ties),
     MUSIC LOCAL_MAXIMA on the same windows far fewer"""
     kind, m, coherent, sep = case
-    pos, tab, x, th = td.resolution_case(kind, m, coherent, sep)
+    pos, tab, x, th = resolution_case(kind, m, coherent, sep)
     K = tab.shape[0]
-    blk = handle(tab, 2, td.SNAPS)
-    out, _ = dev_call(blk, x, 2, K, R=True)
+    blk = handle(tab, 2, SNAPS)
+    out, _ = gh.device_call(blk, x, PEAKS + ("R",))
     blk.close()
     edge = check_parity(out, out["R"], tab, 2, ctx=case)
-    got = sum(td.resolved(out["angles"][w], th[w]) for w in range(len(x)))
-    music_want, dml_want = td.RESOLUTION[case]
+    got = sum(resolved(out["angles"][w], th[w]) for w in range(len(x)))
+    music_want, dml_want = RESOLUTION[case]
     assert abs(got - dml_want) <= edge, (got, dml_want, edge)
-    loc = handle(tab, 2, td.SNAPS, mode="local_maxima")
-    lo, _ = dev_call(loc, x, 2, K)
+    loc = handle(tab, 2, SNAPS, mode="local_maxima")
+    lo, _ = gh.device_call(loc, x, PEAKS)
     loc.close()
-    got_music = sum(td.resolved([a for a, b in zip(lo["angles"][w], lo["bins"][w]) if b >= 0], th[w]) for w in range(len(x)))
+    got_music = sum(resolved([a for a, b in zip(lo["angles"][w], lo["bins"][w]) if b >= 0], th[w]) for w in range(len(x)))
     assert got_music <= music_want + 2 and got_music * 3 < got, (got_music, got)
 
 
@@ -155,94 +148,66 @@ def test_entries_agree():
     """host, device, _ex, _counts, planar host and planar device agree byte for byte, and so do multi-device handles and
     sharded calls; spectrum, P64, R, eigenvalues and counts are a TOP_BINS handle's"""
     m, n, snaps, Wn = 8, 2, 512, 24
-    pos = td.array("uca", m)
-    tab = td.table(pos, 720)
+    pos = array_wl("uca", m)
+    tab = table_wl(pos, 720)
     K = tab.shape[0]
     rng = np.random.default_rng(4)
-    x = td.source_windows(pos, rng.uniform(0, 360, (Wn, 2)), True, Wn, 5, snaps=snaps)
+    x = angle_windows(pos, rng.uniform(0, 360, (Wn, 2)), True, Wn, 5, snaps=snaps)
     blk = handle(tab, n, snaps)
-    ref, _ = dev_call(blk, x, n, K)
+    ref, _ = gh.device_call(blk, x, PEAKS)
     assert np.all(ref["bins"] >= 0)
-    ex, _ = dev_call(blk, x, n, K, spectrum=True, p64=True, R=True)
-    cn, _ = dev_call(blk, x, n, K, counts=True)
+    ex, _ = gh.device_call(blk, x, PEAKS + ("spectrum", "P64", "R"))
+    cn, _ = gh.device_call(blk, x, PEAKS + ("counts",))
     for o in (ex, cn):
         assert all(np.array_equal(o[k], ref[k]) for k in ("angles", "levels", "bins"))
     assert np.all(cn["counts"] == n)
     top = handle(tab, n, snaps, mode="top_bins")
-    to, _ = dev_call(top, x, n, K, spectrum=True, p64=True, R=True)
-    tc, _ = dev_call(top, x, n, K, counts=True)
+    to, _ = gh.device_call(top, x, PEAKS + ("spectrum", "P64", "R"))
+    tc, _ = gh.device_call(top, x, PEAKS + ("counts",))
     assert all(np.array_equal(to[k], ex[k]) for k in ("spectrum", "P64", "R"))
     assert np.array_equal(tc["counts"], cn["counts"])
-    dev = torch.device("cuda:0")
-    d_in = torch.from_numpy(x.view(np.float32)).to(dev)
-    evs = []
-    for b in (blk, top):
-        a = torch.zeros((Wn, n), dtype=torch.float32, device=dev)
-        ev = torch.zeros((Wn, m), dtype=torch.float64, device=dev)
-        b.process_device(d_in.data_ptr(), Wn, a.data_ptr(), stream=torch.cuda.current_stream().cuda_stream, d_eigvals=ev.data_ptr())
-        torch.cuda.synchronize()
-        evs.append(ev.cpu().numpy())
+    evs = [gh.device_call(b, x, ("eigvals",))[0]["eigvals"] for b in (blk, top)]
     assert np.array_equal(evs[0], evs[1])
     top.close()
-    ang, lvl, spec = np.zeros((Wn, n), np.float32), np.zeros((Wn, n), np.float32), np.zeros((Wn, K), np.float32)
-    blk.work(Wn, [x], [ang, lvl, spec])
-    assert np.array_equal(ang, ref["angles"]) and np.array_equal(lvl, ref["levels"]) and np.array_equal(blk.last_bins(), ref["bins"])
-    assert np.array_equal(spec, ex["spectrum"])
-    streams = [np.ascontiguousarray(x.reshape(Wn, snaps, m)[:, :, r].reshape(-1)) for r in range(m)]
-    pa, pl = np.zeros((Wn, n), np.float32), np.zeros((Wn, n), np.float32)
-    blk.work_planar(Wn, streams, [pa, pl])
-    assert np.array_equal(pa, ref["angles"]) and np.array_equal(pl, ref["levels"]) and np.array_equal(blk.last_bins(), ref["bins"])
-    d_streams = [torch.from_numpy(s.view(np.float32)).to(dev) for s in streams]
-    da = torch.zeros((Wn, n), dtype=torch.float32, device=dev)
-    blk.process_planar_device([t.data_ptr() for t in d_streams], snaps, Wn, da.data_ptr(), stream=torch.cuda.current_stream().cuda_stream)
-    torch.cuda.synchronize()
-    assert np.array_equal(da.cpu().numpy(), ref["angles"])
     blk.close()
+    e = gh.entry_outputs(lambda devices=None: handle(tab, n, snaps, devices=devices), x, spectrum=True, multi_device=False)
+    h = e["host"]
+    assert np.array_equal(h["angles"], ref["angles"]) and np.array_equal(h["levels"], ref["levels"]) and np.array_equal(h["bins"], ref["bins"])
+    assert np.array_equal(h["spectrum"], ex["spectrum"])
+    ph = e["planar_host"]
+    assert np.array_equal(ph["angles"], ref["angles"]) and np.array_equal(ph["levels"], ref["levels"]) and np.array_equal(ph["bins"], ref["bins"])
+    assert np.array_equal(e["planar_device"]["angles"], ref["angles"])
     G = torch.cuda.device_count()
     for devices in ([0], list(range(G))):
-        mb = handle(tab, n, snaps, devices=devices)
-        a2, l2 = np.zeros((Wn, n), np.float32), np.zeros((Wn, n), np.float32)
-        mb.work(Wn, [x], [a2, l2])
-        assert np.array_equal(a2, ref["angles"]) and np.array_equal(l2, ref["levels"]), devices
-        mb.close()
+        a2 = e["multi_host%s" % devices]
+        assert np.array_equal(a2["angles"], ref["angles"]) and np.array_equal(a2["levels"], ref["levels"]), devices
     if G < 2:
         return
-    mb = handle(tab, n, snaps, devices=list(range(G)))
-    ins, angs, bins_all = [], [], []
-    for g in range(G):
-        d = torch.device("cuda", g)
-        ins.append(torch.from_numpy(np.ascontiguousarray(x[g::G]).view(np.float32)).to(d))
-        angs.append(torch.zeros((len(x[g::G]), n), dtype=torch.float32, device=d))
-        bins_all.append(torch.full((Wn, n), -7, dtype=torch.int32, device=d))
-    mb.process_device_sharded([t.data_ptr() for t in ins], Wn, [t.data_ptr() for t in angs], None, [t.data_ptr() for t in bins_all])
-    for g in range(G):
-        torch.cuda.synchronize(g)
-    for g in range(G):
-        assert np.array_equal(angs[g].cpu().numpy(), ref["angles"][g::G]), g
-        assert np.array_equal(bins_all[g].cpu().numpy(), ref["bins"]), g
-    mb.close()
+    for g, sh in enumerate(e["sharded"]):
+        assert np.array_equal(sh["angles"], ref["angles"][g::G]), g
+        assert np.array_equal(sh["bins"], ref["bins"]), g
 
 
 def test_launch_counts_and_sub_batches():
     """per sub-batch: covariance + DML; the eigensolver (+ source count) only under MDL or for the spectrum, + the scan
     with the spectrum; a call of several sub-batches equals its halves"""
     m, n, snaps = 4, 1, 256
-    pos = td.array("x", m)
-    tab = td.table(pos, 3600)
-    x = td.source_windows(pos, [(40.0,)] * 3, False, 3, 9, snaps=snaps)
+    pos = array_wl("x", m)
+    tab = table_wl(pos, 3600)
+    x = angle_windows(pos, [(40.0,)] * 3, False, 3, 9, snaps=snaps)
     for rule, spectrum, want in (("fixed", False, 2), ("mdl", False, 4), ("fixed", True, 4), ("mdl", True, 5)):
         blk = handle(tab, n, snaps, rule)
-        _, launches = dev_call(blk, x, n, 3600, spectrum=spectrum)
+        _, launches = gh.device_call(blk, x, PEAKS + (("spectrum",) if spectrum else ()))
         assert launches == want, (rule, spectrum, launches)
         blk.close()
     Kb, Wb, Nb = 36000, 3000, 64
-    tb = td.table(pos, Kb)
-    xb = td.source_windows(pos, [(40.0,)] * Wb, False, Wb, 10, snaps=Nb)
+    tb = table_wl(pos, Kb)
+    xb = angle_windows(pos, [(40.0,)] * Wb, False, Wb, 10, snaps=Nb)
     blk = handle(tb, n, Nb)
-    whole, launches = dev_call(blk, xb, n, Kb, spectrum=True)
+    whole, launches = gh.device_call(blk, xb, PEAKS + ("spectrum",))
     assert launches % 4 == 0 and launches // 4 >= 2, launches
-    first, _ = dev_call(blk, xb[: Wb // 2], n, Kb, spectrum=True)
-    second, _ = dev_call(blk, xb[Wb // 2:], n, Kb, spectrum=True)
+    first, _ = gh.device_call(blk, xb[: Wb // 2], PEAKS + ("spectrum",))
+    second, _ = gh.device_call(blk, xb[Wb // 2:], PEAKS + ("spectrum",))
     for k in ("angles", "levels", "bins", "spectrum"):
         assert np.array_equal(whole[k], np.concatenate([first[k], second[k]])), k
     blk.close()
@@ -255,13 +220,13 @@ def test_switching_back_to_top_bins():
     tab = helpers.table_for(cfg)
     K = cfg["resolution"]
     fresh = handle(tab, 1, cfg["snapshots"], mode="top_bins")
-    ref, l_ref = dev_call(fresh, x, 1, K)
+    ref, l_ref = gh.device_call(fresh, x, PEAKS)
     fresh.close()
     blk = handle(tab, 1, cfg["snapshots"])
-    _, l_dml = dev_call(blk, x, 1, K)
+    _, l_dml = gh.device_call(blk, x, PEAKS)
     assert l_dml == 2
     blk.set_peak_mode("top_bins", 0)
-    got, l_top = dev_call(blk, x, 1, K)
+    got, l_top = gh.device_call(blk, x, PEAKS)
     assert l_ref == l_top == 1
     assert all(np.array_equal(got[k], ref[k]) for k in ("angles", "levels", "bins"))
     blk.close()
@@ -272,16 +237,16 @@ def test_scaled_and_zero_row_tables():
     """a table scaled by 2^s: the same bins, levels times exactly 2^(-2 s) (every s here keeps them normal); zero rows,
     placed at the sources' own bins, are never picked"""
     m, n, snaps = 8, 2, 1024
-    pos, tab, x, th = td.resolution_case("uca", m, True, 40, W=12)
+    pos, tab, x, th = resolution_case("uca", m, True, 40, W=12)
     K = tab.shape[0]
     blk = handle(tab, n, snaps)
-    ref, _ = dev_call(blk, x, n, K)
+    ref, _ = gh.device_call(blk, x, PEAKS)
     blk.close()
     assert np.all(ref["bins"] >= 0) and np.all(np.abs(ref["levels"]) > 1e-3)
     for s in (-40, -20, -3, 4, 20, 40):
         st = (tab.astype(np.complex128) * 2.0 ** s).astype(np.complex64)
         blk = handle(st, n, snaps)
-        got, _ = dev_call(blk, x, n, K)
+        got, _ = gh.device_call(blk, x, PEAKS)
         blk.close()
         assert np.array_equal(got["bins"], ref["bins"]), s
         assert np.array_equal(got["levels"], (ref["levels"].astype(np.float64) * 2.0 ** (-2 * s)).astype(np.float32)), s
@@ -289,7 +254,7 @@ def test_scaled_and_zero_row_tables():
     zt = tab.copy()
     zt[zero] = 0
     blk = handle(zt, n, snaps)
-    got, _ = dev_call(blk, x, n, K, R=True)
+    got, _ = gh.device_call(blk, x, PEAKS + ("R",))
     blk.close()
     assert np.all(got["bins"] >= 0) and not np.isin(got["bins"], zero).any()
     check_parity(got, got["R"], zt, n, ctx="zero rows")
@@ -298,15 +263,15 @@ def test_scaled_and_zero_row_tables():
 def test_degenerate_windows():
     """NaN and all-zero windows report (0, 0, -1); MDL with d = 0 reports no peak"""
     m, n, snaps = 4, 2, 256
-    pos = td.array("x", m)
-    tab = td.table(pos)
-    x = td.source_windows(pos, [(40.0, 100.0)] * 4, False, 4, 3, snaps=snaps)
-    x[2] = td.source_windows(pos, [[]], False, 1, 4, snaps=snaps)[0]
+    pos = array_wl("x", m)
+    tab = table_wl(pos)
+    x = angle_windows(pos, [(40.0, 100.0)] * 4, False, 4, 3, snaps=snaps)
+    x[2] = angle_windows(pos, [[]], False, 1, 4, snaps=snaps)[0]
     x[0] = 0
     x[1, 17] = np.nan
     for rule in ("fixed", "mdl"):
         blk = handle(tab, n, snaps, rule)
-        out, _ = dev_call(blk, x, n, 360)
+        out, _ = gh.device_call(blk, x, PEAKS)
         blk.close()
         for w in ([0, 1] if rule == "fixed" else [0, 1, 2]):
             assert np.all(out["bins"][w] == -1) and np.all(out["angles"][w] == 0.0) and np.all(out["levels"][w] == 0.0), (rule, w, out)
@@ -325,7 +290,7 @@ def test_invalid_combinations():
         blk.set_estimator(kind, loading)
         assert L.music_b200_set_peak_mode(blk._h, DML, 0) == EINVAL
         blk.set_estimator("music", 0.0)
-    blk.set_array_geometry(td.array("uca", m), LAM)
+    blk.set_array_geometry(array_wl("uca", m), LAM)
     blk.set_refine(True)
     assert L.music_b200_set_peak_mode(blk._h, DML, 0) == EINVAL
     blk.set_refine(False)
@@ -335,13 +300,13 @@ def test_invalid_combinations():
     assert L.music_b200_set_refine(blk._h, 1) == EINVAL
     assert L.music_b200_set_peak_mode(blk._h, DML, 2) == EINVAL
     blk.set_array_response(tab)  # a set_table() table is accepted, unlike under ROOTS and ESPRIT
-    x = td.source_windows(td.array("x", m), [(40.0,)], False, 1, 2, snaps=snaps)
-    out, _ = dev_call(blk, x, n, K)
+    x = angle_windows(array_wl("x", m), [(40.0,)], False, 1, 2, snaps=snaps)
+    out, _ = gh.device_call(blk, x, PEAKS)
     assert out["bins"][0, 0] >= 0
     with pytest.raises(ValueError):
         blk.set_peak_mode("DML")
     blk.close()
-    az = music_doa_azel(m, n, m * snaps, 36, 3, (0.0, 30.0), np.c_[td.array("x", m), np.zeros(m)], LAM)
+    az = music_doa_azel(m, n, m * snaps, 36, 3, (0.0, 30.0), np.c_[array_wl("x", m), np.zeros(m)], LAM)
     assert L.music_b200_set_peak_mode(az._h, DML, 0) == EINVAL
     with pytest.raises(_capi.MusicB200Error):
         az.set_peak_mode("dml")
@@ -350,27 +315,14 @@ def test_invalid_combinations():
 
 def test_cpp_block():
     """the C++ block through set_array_response() and set_peak_mode(4, 0) equals the Python block"""
-    exe = os.path.join(ROOT, "lib", "_build", "test_block_dml")
     m, n, K, snaps, Wn = 8, 2, 720, 256, 16
-    pos = td.array("uca", m)
-    tab = helpers.calibrated_table(td.table(pos, K), 8)
-    x = td.source_windows(pos, np.random.default_rng(8).uniform(0, 360, (Wn, 2)), True, Wn, 78, snaps=snaps)
-    with tempfile.TemporaryDirectory() as tdir:
-        fin, fout = os.path.join(tdir, "in.bin"), os.path.join(tdir, "out.bin")
-        with open(fin, "wb") as f:
-            f.write(struct.pack("<6I", m, n, m * snaps, K, Wn, 0))
-            f.write(np.ascontiguousarray(tab).view(np.float32).tobytes())
-            f.write(x.view(np.float32).tobytes())
-        r = subprocess.run([exe, fin, fout], capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr
-        raw = open(fout, "rb").read()
-    o = 0
-    take = lambda cnt, dt: np.frombuffer(raw[o:o + 4 * cnt], dt)
-    ca = take(Wn * n, np.float32); o += 4 * Wn * n
-    cl = take(Wn * n, np.float32); o += 4 * Wn * n
-    cs = take(Wn * K, np.float32); o += 4 * Wn * K
-    cb = take(Wn * n, np.int32); o += 4 * Wn * n
-    cc = take(Wn, np.int32)
+    pos = array_wl("uca", m)
+    tab = helpers.calibrated_table(table_wl(pos, K), 8)
+    x = angle_windows(pos, np.random.default_rng(8).uniform(0, 360, (Wn, 2)), True, Wn, 78, snaps=snaps)
+    c = gh.run_cpp_block("test_block_dml", struct.pack("<6I", m, n, m * snaps, K, Wn, 0), [tab, x],
+                         [("a", np.float32, Wn * n), ("l", np.float32, Wn * n), ("s", np.float32, Wn * K),
+                          ("b", np.int32, Wn * n), ("c", np.int32, Wn)])
+    ca, cl, cs, cb, cc = c["a"], c["l"], c["s"], c["b"], c["c"]
     blk = handle(tab, n, snaps)
     ang, lvl, spec = np.zeros((Wn, n), np.float32), np.zeros((Wn, n), np.float32), np.zeros((Wn, K), np.float32)
     blk.work(Wn, [x], [ang, lvl, spec])

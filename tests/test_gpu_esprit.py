@@ -4,9 +4,7 @@ unchanged.
 
 The oracle runs on the GPU's own covariance (d_R), so what is compared is the ESPRIT stage itself."""
 import math
-import os
 import struct
-import subprocess
 
 import numpy as np
 import pytest
@@ -17,37 +15,19 @@ from gr_baz_b200.music_doa import music_doa
 from gr_baz_b200.music_doa_azel import music_doa_azel
 
 import esprit_oracle as eo
-import refine_oracle as ro
-from test_gpu_root_music import LAM, PLAN, axis_deg, circ, dev_call, near_half, ula, windows
+import gpu_harness as gh
+from helpers import LAM, PLAN, axis_deg, circ, near_half, plan_windows as windows, two_source_windows, ula
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ESPRIT = 3
 FLIP = 1e-9     # orderings or subspaces the oracle sees this close to flipping may go either way
 L_RTOL = 1e-5
+PEAKS = ("levels", "bins")
 
 
 def handle(m, n, K, pos, snaps, mode="esprit", rule="fixed", devices=None):
-    blk = music_doa(m, n, m * snaps, np.ones((K, m), np.complex64), K, devices=devices)
-    blk.set_array_geometry(pos, LAM)
-    blk.set_source_rule(rule)
-    blk.set_peak_mode(mode, 0)
-    return blk
-
-
-def two_source_windows(pos, th, snr_db, snaps, Wn, seed):
-    rng = np.random.default_rng(seed)
-    m = pos.shape[0]
-    amp = 10.0 ** (snr_db / 20.0)
-    xs = []
-    for _ in range(Wn):
-        X = (rng.standard_normal((m, snaps)) + 1j * rng.standard_normal((m, snaps))) / np.sqrt(2.0)
-        for t in th:
-            a = ro.steering(pos, LAM, math.radians(t))[0]
-            X += amp * a[:, None] * (rng.standard_normal(snaps) + 1j * rng.standard_normal(snaps))[None, :] / np.sqrt(2.0)
-        xs.append(X.T.reshape(-1))
-    return np.array(xs).astype(np.complex64)
+    return gh.make_block(m, n, snaps, K, pos=pos, rule=rule, mode=mode, devices=devices)
 
 
 # ---- parity with the oracle ------------------------------------------------------------------------------------------
@@ -67,12 +47,12 @@ def test_parity_with_oracle(m):
             for rule in ("fixed", "mdl"):
                 K = 3600 if (gi + n) % 2 else 360
                 blk = handle(m, n, K, pos, snaps, rule=rule)
-                out, _ = dev_call(blk, x, n, K, R=True)
+                out, _ = gh.device_call(blk, x, PEAKS + ("R",))
                 counts = None
                 if rule == "mdl":
-                    cnt, _ = dev_call(blk, x, n, K, counts=True)
+                    cnt, _ = gh.device_call(blk, x, PEAKS + ("counts",))
                     top = handle(m, n, K, pos, snaps, mode="top_bins", rule=rule)
-                    tc, _ = dev_call(top, x, n, K, counts=True)
+                    tc, _ = gh.device_call(top, x, PEAKS + ("counts",))
                     top.close()
                     assert np.array_equal(cnt["counts"], tc["counts"]), (m, n, kind)
                     assert np.array_equal(cnt["angles"], out["angles"]) and np.array_equal(cnt["bins"], out["bins"])
@@ -117,7 +97,7 @@ def test_degenerate_windows():
     x[1, 17] = np.nan
     for rule in ("fixed", "mdl"):
         blk = handle(m, n, K, pos, snaps, rule=rule)
-        out, _ = dev_call(blk, x, n, K)
+        out, _ = gh.device_call(blk, x, PEAKS)
         empty = [0, 1] if rule == "fixed" else [0, 1, 2]
         for w in empty:
             assert np.all(out["bins"][w] == -1) and np.all(out["angles"][w] == 0.0) and np.all(out["levels"][w] == 0.0), (rule, w, out)
@@ -133,59 +113,37 @@ def test_entries_agree():
     pos = ula(m, "x")
     x, _ = windows(pos, [(1, 20.0)] * Wn, 41, snaps)
     blk = handle(m, n, K, pos, snaps)
-    ref, _ = dev_call(blk, x, n, K)
+    ref, _ = gh.device_call(blk, x, PEAKS)
     assert np.all(ref["bins"] >= 0)
-    ex, _ = dev_call(blk, x, n, K, spectrum=True, p64=True, R=True)
-    cn, _ = dev_call(blk, x, n, K, counts=True)
+    ex, _ = gh.device_call(blk, x, PEAKS + ("spectrum", "P64", "R"))
+    cn, _ = gh.device_call(blk, x, PEAKS + ("counts",))
     for o in (ex, cn):
         assert all(np.array_equal(o[k], ref[k]) for k in ("angles", "levels", "bins"))
     assert np.all(cn["counts"] == n)
     loc = handle(m, n, K, pos, snaps, mode="local_maxima")
-    lo, _ = dev_call(loc, x, n, K, spectrum=True, p64=True)
+    lo, _ = gh.device_call(loc, x, PEAKS + ("spectrum", "P64"))
     loc.close()
     assert np.array_equal(lo["spectrum"], ex["spectrum"]) and np.array_equal(lo["P64"], ex["P64"])
-    ang, lvl, spec = np.zeros((Wn, n), np.float32), np.zeros((Wn, n), np.float32), np.zeros((Wn, K), np.float32)
-    blk.work(Wn, [x], [ang, lvl, spec])
-    assert np.array_equal(ang, ref["angles"]) and np.array_equal(lvl, ref["levels"]) and np.array_equal(blk.last_bins(), ref["bins"])
-    assert np.array_equal(spec, ex["spectrum"])
-    streams = [np.ascontiguousarray(x.reshape(Wn, snaps, m)[:, :, r].reshape(-1)) for r in range(m)]
-    pa, pl = np.zeros((Wn, n), np.float32), np.zeros((Wn, n), np.float32)
-    blk.work_planar(Wn, streams, [pa, pl])
-    assert np.array_equal(pa, ref["angles"]) and np.array_equal(pl, ref["levels"]) and np.array_equal(blk.last_bins(), ref["bins"])
-    dev = torch.device("cuda:0")
-    d_streams = [torch.from_numpy(s.view(np.float32)).to(dev) for s in streams]
-    da = torch.zeros((Wn, n), dtype=torch.float32, device=dev)
-    l0 = blk.launch_count()
-    blk.process_planar_device([t.data_ptr() for t in d_streams], snaps, Wn, da.data_ptr(), stream=torch.cuda.current_stream().cuda_stream)
-    torch.cuda.synchronize()
-    assert blk.launch_count() - l0 == 3  # the planar covariance, eig, ESPRIT: never the fused kernel
-    assert np.array_equal(da.cpu().numpy(), ref["angles"])
     blk.close()
+    e = gh.entry_outputs(lambda devices=None: handle(m, n, K, pos, snaps, devices=devices), x, spectrum=True)
+    h = e["host"]
+    assert np.array_equal(h["angles"], ref["angles"]) and np.array_equal(h["levels"], ref["levels"]) and np.array_equal(h["bins"], ref["bins"])
+    assert np.array_equal(h["spectrum"], ex["spectrum"])
+    ph = e["planar_host"]
+    assert np.array_equal(ph["angles"], ref["angles"]) and np.array_equal(ph["levels"], ref["levels"]) and np.array_equal(ph["bins"], ref["bins"])
+    assert e["planar_launches"] == 3  # the planar covariance, eig, ESPRIT: never the fused kernel
+    assert np.array_equal(e["planar_device"]["angles"], ref["angles"])
     G = torch.cuda.device_count()
     for devices in ([0], list(range(G))):
-        mb = handle(m, n, K, pos, snaps, devices=devices)
-        a2, l2 = np.zeros((Wn, n), np.float32), np.zeros((Wn, n), np.float32)
-        mb.work(Wn, [x], [a2, l2])
-        assert np.array_equal(a2, ref["angles"]) and np.array_equal(l2, ref["levels"]), devices
-        g, _ = dev_call(mb, x, n, K)
+        a2 = e["multi_host%s" % devices]
+        assert np.array_equal(a2["angles"], ref["angles"]) and np.array_equal(a2["levels"], ref["levels"]), devices
+        g = e["multi_device%s" % devices]
         assert np.array_equal(g["angles"], ref["angles"]) and np.array_equal(g["bins"], ref["bins"]), devices
-        mb.close()
     if G < 2:
         return
-    mb = handle(m, n, K, pos, snaps, devices=list(range(G)))
-    ins, angs, bins_all = [], [], []
-    for g in range(G):
-        d = torch.device("cuda", g)
-        ins.append(torch.from_numpy(np.ascontiguousarray(x[g::G]).view(np.float32)).to(d))
-        angs.append(torch.zeros((len(x[g::G]), n), dtype=torch.float32, device=d))
-        bins_all.append(torch.full((Wn, n), -7, dtype=torch.int32, device=d))
-    mb.process_device_sharded([t.data_ptr() for t in ins], Wn, [t.data_ptr() for t in angs], None, [t.data_ptr() for t in bins_all])
-    for g in range(G):
-        torch.cuda.synchronize(g)
-    for g in range(G):
-        assert np.array_equal(angs[g].cpu().numpy(), ref["angles"][g::G]), g
-        assert np.array_equal(bins_all[g].cpu().numpy(), ref["bins"]), g
-    mb.close()
+    for g, sh in enumerate(e["sharded"]):
+        assert np.array_equal(sh["angles"], ref["angles"][g::G]), g
+        assert np.array_equal(sh["bins"], ref["bins"]), g
 
 
 def test_launch_counts_and_sub_batches():
@@ -195,17 +153,17 @@ def test_launch_counts_and_sub_batches():
     x, _ = windows(pos, [(1, 20.0)], 3, snaps)
     for rule, spectrum, want in (("fixed", False, 3), ("mdl", False, 4), ("fixed", True, 4), ("mdl", True, 5)):
         blk = handle(m, n, K, pos, snaps, rule=rule)
-        _, launches = dev_call(blk, x, n, K, spectrum=spectrum)
+        _, launches = gh.device_call(blk, x, PEAKS + (("spectrum",) if spectrum else ()))
         assert launches == want, (rule, spectrum, launches)
         blk.close()
     # several sub-batches (the internal fp64 spectrum of K bins per window bounds one); the whole call equals its halves
     Kb, Wb, Nb = 36000, 3000, 64
     xb, _ = windows(pos, [(1, 20.0)] * Wb, 809, Nb)
     blk = handle(m, n, Kb, pos, Nb)
-    whole, launches = dev_call(blk, xb, n, Kb, spectrum=True)
+    whole, launches = gh.device_call(blk, xb, PEAKS + ("spectrum",))
     assert launches % 4 == 0 and launches // 4 >= 2, launches
-    first, _ = dev_call(blk, xb[: Wb // 2], n, Kb, spectrum=True)
-    second, _ = dev_call(blk, xb[Wb // 2:], n, Kb, spectrum=True)
+    first, _ = gh.device_call(blk, xb[: Wb // 2], PEAKS + ("spectrum",))
+    second, _ = gh.device_call(blk, xb[Wb // 2:], PEAKS + ("spectrum",))
     for k in ("angles", "levels", "bins", "spectrum"):
         assert np.array_equal(whole[k], np.concatenate([first[k], second[k]])), k
     blk.close()
@@ -217,13 +175,13 @@ def test_switching_back_to_top_bins():
     x = synth.gen_windows_numpy(cfg, 12, 0, 64)
     pos = ula(4, "x")
     fresh = handle(4, 1, cfg["resolution"], pos, cfg["snapshots"], mode="top_bins")
-    ref, l_ref = dev_call(fresh, x, 1, cfg["resolution"])
+    ref, l_ref = gh.device_call(fresh, x, PEAKS)
     fresh.close()
     blk = handle(4, 1, cfg["resolution"], pos, cfg["snapshots"])
-    _, l_esprit = dev_call(blk, x, 1, cfg["resolution"])
+    _, l_esprit = gh.device_call(blk, x, PEAKS)
     assert l_esprit == 3
     blk.set_peak_mode("top_bins", 0)
-    got, l_top = dev_call(blk, x, 1, cfg["resolution"])
+    got, l_top = gh.device_call(blk, x, PEAKS)
     assert l_ref == l_top == 1
     assert all(np.array_equal(got[k], ref[k]) for k in ("angles", "levels", "bins"))
     blk.close()
@@ -236,7 +194,7 @@ def test_mirror_case():
     pos = ula(m, "x")
     x = two_source_windows(pos, (40.0, 110.0), 20.0, snaps, Wn, 40)
     blk = handle(m, n, K, pos, snaps)
-    out, _ = dev_call(blk, x, n, K)
+    out, _ = gh.device_call(blk, x, PEAKS)
     blk.close()
     got = np.sort(out["angles"], axis=1)
     assert np.all(np.abs(got[:, 0] - 40.0) < 1.0) and np.all(np.abs(got[:, 1] - 110.0) < 1.0), got
@@ -249,7 +207,7 @@ def test_resolution(m, th):
     pos = ula(m, "x")
     x = two_source_windows(pos, th, 0.0, snaps, Wn, 7 * m)
     blk = handle(m, n, K, pos, snaps)
-    out, _ = dev_call(blk, x, n, K)
+    out, _ = gh.device_call(blk, x, PEAKS)
     blk.close()
     got = np.sort(out["angles"], axis=1)
     ok = np.all(np.abs(got - np.array(th)[None, :]) < (th[1] - th[0]) / 2.0, axis=1)
@@ -288,14 +246,14 @@ def test_invalid_combinations():
     for bad in (uca, bent, ula(m, "x") * 1.2):
         blk.set_array_geometry(bad, LAM)  # set_geometry() itself keeps its behaviour
         with pytest.raises(_capi.MusicB200Error):
-            dev_call(blk, x, n, K)
+            gh.device_call(blk, x, PEAKS)
         assert L.music_b200_set_peak_mode(blk._h, ESPRIT, 0) == EINVAL
         blk.set_array_geometry(pos, LAM)
         assert L.music_b200_set_peak_mode(blk._h, ESPRIT, 0) == _capi.OK
     # set_table() after set_peak_mode(ESPRIT): the call fails, no fall-back to grid peaks
     blk.set_array_response(np.ones((K, m), np.complex64))
     with pytest.raises(_capi.MusicB200Error):
-        dev_call(blk, x, n, K)
+        gh.device_call(blk, x, PEAKS)
     ang = np.zeros((1, n), np.float32)
     with pytest.raises(_capi.MusicB200Error):
         blk.work(1, [x], [ang])
@@ -312,28 +270,14 @@ def test_invalid_combinations():
 
 def test_cpp_block():
     """the C++ block through set_estimator(0) and set_peak_mode(3, 0) equals the Python block"""
-    exe = os.path.join(ROOT, "lib", "_build", "test_block_estimator")
     m, n, K, snaps, Wn = 8, 2, 720, 256, 16
     pos = ula(m, "oblique")
     x, _ = windows(pos, [(2, 20.0)] * Wn, 78, snaps)
-    import tempfile
-    with tempfile.TemporaryDirectory() as td:
-        fin, fout = os.path.join(td, "in.bin"), os.path.join(td, "out.bin")
-        with open(fin, "wb") as f:
-            f.write(struct.pack("<10I", m, n, m * snaps, K, Wn, 0, ESPRIT, 0, 1, 0))
-            f.write(struct.pack("<2d", 0.0, LAM))
-            f.write(np.ascontiguousarray(pos, np.float64).tobytes())
-            f.write(x.view(np.float32).tobytes())
-        r = subprocess.run([exe, fin, fout], capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr
-        raw = open(fout, "rb").read()
-    o = 0
-    take = lambda cnt, dt: np.frombuffer(raw[o:o + 4 * cnt], dt)
-    ca = take(Wn * n, np.float32); o += 4 * Wn * n
-    cl = take(Wn * n, np.float32); o += 4 * Wn * n
-    cs = take(Wn * K, np.float32); o += 4 * Wn * K
-    cb = take(Wn * n, np.int32); o += 4 * Wn * n
-    cc = take(Wn, np.int32)
+    c = gh.run_cpp_block("test_block_estimator", struct.pack("<10I", m, n, m * snaps, K, Wn, 0, ESPRIT, 0, 1, 0) +
+                         struct.pack("<2d", 0.0, LAM), [np.ascontiguousarray(pos, np.float64), x],
+                         [("a", np.float32, Wn * n), ("l", np.float32, Wn * n), ("s", np.float32, Wn * K),
+                          ("b", np.int32, Wn * n), ("c", np.int32, Wn)])
+    ca, cl, cs, cb, cc = c["a"], c["l"], c["s"], c["b"], c["c"]
     blk = handle(m, n, K, pos, snaps, rule="mdl")
     ang, lvl, spec = np.zeros((Wn, n), np.float32), np.zeros((Wn, n), np.float32), np.zeros((Wn, K), np.float32)
     blk.work(Wn, [x], [ang, lvl, spec])

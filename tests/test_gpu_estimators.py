@@ -3,16 +3,13 @@ through every branch of the pipeline, and the default MUSIC path unchanged.
 
 Every GPU result is compared with the oracle evaluated on the GPU's own covariance (d_R) and table (get_table), so what
 is compared is the estimator itself."""
-import math
-import os
 import struct
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
-from gr_baz_b200 import _capi, build, synth
+from gr_baz_b200 import _capi, synth
 from gr_baz_b200.music_doa import music_doa
 from gr_baz_b200.music_doa_azel import music_doa_azel
 from gr_baz_b200.music_doa_helper import music_doa_helper
@@ -20,76 +17,20 @@ from oracle import music_oracle as mo
 
 import azel_oracle as ao
 import estimator_oracle as eo
+import gpu_harness as gh
 import refine_oracle as ro
+from helpers import LAM, offgrid_windows as windows, positions
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-LAM = synth.C_LIGHT / synth.FREQUENCY
-SENTINEL = -7
 P_RTOL = 1e-9
 EXCL = 3
-
-
-def positions(geometry, m):
-    return np.asarray(mo.scaled_antenna_array(synth.SPACING, synth.antenna_array(geometry, m)), np.float64)
-
-
-def windows(pos, n_of, seed, snaps, noise=0.1, sep=None):
-    """complex64 windows; window w holds n_of[w] unit-power sources (random angles, or two `sep` degrees apart) plus
-    complex white noise of power noise^2; returns (x, true angles per window)"""
-    rng = np.random.default_rng(seed)
-    m = pos.shape[0]
-    xs, truth = [], []
-    for S in n_of:
-        X = noise * (rng.standard_normal((m, snaps)) + 1j * rng.standard_normal((m, snaps))) / np.sqrt(2.0)
-        if sep is None:
-            angs = rng.uniform(0.0, 360.0, S)
-        else:
-            t0 = rng.uniform(0.0, 360.0)
-            angs = np.array([t0, t0 + sep])
-        for t in angs:
-            a = ro.steering(pos, LAM, np.deg2rad(t))[0]
-            X += a[:, None] * np.exp(2j * np.pi * rng.uniform(0.0, 1.0, snaps))[None, :]
-        xs.append(X.T.reshape(-1))
-        truth.append(angs)
-    return np.ascontiguousarray(np.array(xs).astype(np.complex64)), truth
+PEAKS = ("levels", "bins")
+ALL = PEAKS + ("spectrum", "P64", "R")
 
 
 def handle(m, n, K, pos, snaps, kind="music", loading=0.0, devices=None):
-    blk = music_doa(m, n, m * snaps, np.ones((K, m), np.complex64), K, devices=devices)
-    blk.set_array_geometry(pos, LAM)
-    blk.set_estimator(kind, loading)
-    return blk
-
-
-def dev_call(blk, x, n, K, spectrum=True, p64=True, R=True, bins=True, levels=True, eig=False):
-    """one process_device_ex call; returns (outputs as numpy, kernel launches)"""
-    dev = torch.device("cuda:0")
-    Wn, m = x.shape[0], blk.m
-    d_in = torch.from_numpy(x.view(np.float32)).to(dev)
-    o = {"angles": torch.full((Wn, n), SENTINEL, dtype=torch.float32, device=dev)}
-    if levels:
-        o["levels"] = torch.full((Wn, n), SENTINEL, dtype=torch.float32, device=dev)
-    if bins:
-        o["bins"] = torch.full((Wn, n), SENTINEL, dtype=torch.int32, device=dev)
-    if spectrum:
-        o["spectrum"] = torch.full((Wn, K), SENTINEL, dtype=torch.float32, device=dev)
-    if p64:
-        o["P64"] = torch.full((Wn, K), SENTINEL, dtype=torch.float64, device=dev)
-    if R:
-        o["R"] = torch.zeros((Wn, m, m, 2), dtype=torch.float64, device=dev)
-    if eig:
-        o["eig"] = torch.zeros((Wn, m), dtype=torch.float64, device=dev)
-    p = lambda k: o[k].data_ptr() if k in o else None
-    l0 = blk.launch_count()
-    blk.process_device(d_in.data_ptr(), Wn, p("angles"), p("levels"), p("spectrum"), p("bins"),
-                       stream=torch.cuda.current_stream().cuda_stream, d_P64=p("P64"), d_R=p("R"), d_eigvals=p("eig"))
-    torch.cuda.synchronize()
-    out = {k: v.cpu().numpy() for k, v in o.items()}
-    if "R" in out:
-        out["R"] = out["R"][..., 0] + 1j * out["R"][..., 1]
-    return out, blk.launch_count() - l0
+    return gh.make_block(m, n, snaps, K, pos=pos, est=(kind, loading), devices=devices)
 
 
 def assert_bins_match(got, P, ref_bins, ctx):
@@ -114,13 +55,13 @@ def test_p64_and_bins_against_oracle(m):
         pos = positions(geometry, m)
         x, _ = windows(pos, [n] * W, 100 * m + gi, snaps)
         music = handle(m, n, K, pos, snaps)
-        _, l_music = dev_call(music, x, n, K)
+        _, l_music = gh.device_call(music, x, ALL)
         table = music.array_response_c64()
         music.close()
         for kind, loading in kinds_loadings():
             ctx = (m, geometry, kind, loading)
             blk = handle(m, n, K, pos, snaps, kind, loading)
-            out, launches = dev_call(blk, x, n, K)
+            out, launches = gh.device_call(blk, x, ALL)
             assert launches == l_music - (1 if kind == "bartlett" else 0), (ctx, launches, l_music)
             for w in range(W):
                 P = eo.spectrum(out["R"][w], table, kind, loading)
@@ -149,7 +90,7 @@ def test_branches(kind, loading, m):
         x, _ = windows(pos, n_of, 7 * m + n, snaps)
         blk = handle(m, n, K, pos, snaps, kind, loading)
         table = blk.array_response_c64()
-        ref, _ = dev_call(blk, x, n, K)
+        ref, _ = gh.device_call(blk, x, ALL)
         Ps = [eo.spectrum(ref["R"][w], table, kind, loading) for w in range(W)]
         for rule in ("fixed", "mdl"):
             blk.set_source_rule(rule)
@@ -157,7 +98,7 @@ def test_branches(kind, loading, m):
                 ctx = (kind, loading, m, n, rule, peak)
                 blk.set_peak_mode("top_bins" if peak == "top" else "local_maxima", EXCL)
                 for spectrum in (False, True):
-                    out, launches = dev_call(blk, x, n, K, spectrum=spectrum, p64=False, R=False)
+                    out, launches = gh.device_call(blk, x, PEAKS + (("spectrum",) if spectrum else ()))
                     eig = 1 if rule == "mdl" else 0  # the eigensolver runs only to count
                     cnt = 1 if rule == "mdl" else 0
                     prep = 1 if kind == "mvdr" else 0
@@ -203,9 +144,9 @@ def test_refine_1d(kind, loading, m):
     x, truth = windows(pos, [n] * W, 31 * m, snaps)
     blk = handle(m, n, K, pos, snaps, kind, loading)
     blk.set_peak_mode("local_maxima", EXCL)
-    off, _ = dev_call(blk, x, n, K)
+    off, _ = gh.device_call(blk, x, ALL)
     blk.set_refine(True)
-    on, _ = dev_call(blk, x, n, K)
+    on, _ = gh.device_call(blk, x, ALL)
     for k in ("bins", "spectrum", "P64"):
         assert np.array_equal(on[k], off[k]), k
     moved = 0
@@ -268,7 +209,7 @@ def test_mvdr_non_pd_windows():
     x[0, 5] = np.complex64(np.nan)
     x[1] = 0
     for spectrum in (False, True):
-        out, _ = dev_call(blk, x, n, K, spectrum=spectrum, p64=spectrum, R=False)
+        out, _ = gh.device_call(blk, x, PEAKS + (("spectrum", "P64") if spectrum else ()))
         for w in (0, 1):
             assert out["bins"][w, 0] == -1 and out["angles"][w, 0] == 0.0 and out["levels"][w, 0] == 0.0
             if spectrum:
@@ -341,9 +282,9 @@ def test_music_restored_byte_identical(base):
         blk = music_doa(m, n, cfg["nsamples"], table, K)
         if switch:
             blk.set_estimator("mvdr", 0.01)
-            dev_call(blk, x, n, K, spectrum=False, p64=False, R=False)
+            gh.device_call(blk, x, PEAKS)
             blk.set_estimator("music")
-        out, launches = dev_call(blk, x, n, K, spectrum=False, p64=False, R=False)
+        out, launches = gh.device_call(blk, x, PEAKS)
         res.append((out, launches))
         blk.close()
     (a, la), (b, lb) = res
@@ -405,45 +346,23 @@ def test_multi_device_and_sharded_gather():
     assert np.array_equal(a1, a2) and np.array_equal(l1, l2)
     assert np.array_equal(single.last_bins(), multi.last_bins())
     # sharded entry with the fused all-gather of the bins
-    G = 2
-    d_in, d_ang, d_bins = [], [], []
-    for g in range(G):
-        dev = torch.device("cuda:%d" % g)
-        d_in.append(torch.from_numpy(np.ascontiguousarray(x[g::G]).view(np.float32)).to(dev))
-        d_ang.append(torch.zeros((x[g::G].shape[0], n), dtype=torch.float32, device=dev))
-        d_bins.append(torch.full((W, n), SENTINEL, dtype=torch.int32, device=dev))
-    multi.process_device_sharded([t.data_ptr() for t in d_in], W, [t.data_ptr() for t in d_ang],
-                                 d_bins_all=[t.data_ptr() for t in d_bins])
-    for g in range(G):
-        torch.cuda.synchronize(g)
-        assert np.array_equal(d_bins[g].cpu().numpy(), single.last_bins())
+    for sh in gh.sharded_call(multi, x):
+        assert np.array_equal(sh["bins"], single.last_bins())
     single.close()
     multi.close()
 
 
 # ---- the C++ block ------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("kind,loading,refine", [("mvdr", 0.01, 0), ("bartlett", 0.0, 1)])
-def test_cpp_block_estimator(tmp_path, kind, loading, refine):
-    build.build_cuda()
-    subprocess.check_call(["make", "-C", os.path.join(ROOT, "lib"), "-s"])
+def test_cpp_block_estimator(kind, loading, refine):
     m, n, K, snaps, Wn = 8, 2, 360, 128, 10
     pos = positions("uca", m)
     x, _ = windows(pos, [2] * Wn, 99, snaps)
     est = music_doa.ESTIMATORS[kind]
-    fin, fout = tmp_path / "in.bin", tmp_path / "out.bin"
-    with open(fin, "wb") as f:
-        f.write(struct.pack("<10I", m, n, m * snaps, K, Wn, est, 1, EXCL, 0, refine))
-        f.write(struct.pack("<2d", loading, LAM))
-        f.write(np.ascontiguousarray(pos).tobytes())
-        f.write(x.view(np.float32).tobytes())
-    r = subprocess.run([os.path.join(ROOT, "lib", "_build", "test_block_estimator"), str(fin), str(fout)], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    raw = np.fromfile(fout, dtype=np.float32)
-    o = 0
-    got = {}
-    for k, size in (("angles", Wn * n), ("levels", Wn * n), ("spectrum", Wn * K), ("bins", Wn * n), ("counts", Wn)):
-        got[k] = raw[o:o + size]
-        o += size
+    got = gh.run_cpp_block("test_block_estimator", struct.pack("<10I", m, n, m * snaps, K, Wn, est, 1, EXCL, 0, refine) +
+                           struct.pack("<2d", loading, LAM), [np.ascontiguousarray(pos), x],
+                           [("angles", np.float32, Wn * n), ("levels", np.float32, Wn * n), ("spectrum", np.float32, Wn * K),
+                            ("bins", np.float32, Wn * n), ("counts", np.float32, Wn)])
     blk = handle(m, n, K, pos, snaps, kind, loading)
     blk.set_peak_mode("local_maxima", EXCL)
     blk.set_refine(bool(refine))

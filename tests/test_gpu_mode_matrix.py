@@ -12,26 +12,25 @@ import numpy as np
 import pytest
 import torch
 
-from gr_baz_b200 import _capi, synth
+from gr_baz_b200 import _capi
 from gr_baz_b200.music_doa import music_doa
 from gr_baz_b200.music_doa_azel import music_doa_azel
-from oracle import music_oracle as mo
 
 import azel_oracle as ao
 import beams_oracle as bo
 import calibration_oracle as co
 import composed_oracle as cmp
 import estimator_oracle as eo
+import gpu_harness as gh
 import helpers
 import refine_oracle as ro
 import source_count_oracle as so
+from helpers import LAM, check_beams, check_weights, circ, corrupt, near_half, positions, random_gains
 
 pytestmark = pytest.mark.gpu
 
-LAM = synth.C_LIGHT / synth.FREQUENCY
-SENTINEL = -7
-DEV = torch.device("cuda:0")
-STREAM = lambda: torch.cuda.current_stream().cuda_stream
+DEV = gh.DEV
+STREAM = gh.stream
 FLIP = 1e-9          # decisions the oracle sees this close to flipping may go either way (the feature tests' bound)
 COUNT_MARGIN = 1e-6  # counts must be exact wherever the MDL / AIC criterion margin exceeds this
 L_RTOL = 1e-5
@@ -118,13 +117,13 @@ def row_id(r):
 # ---- the Python restatement of the planner (plan_call + launch_cov + launch_eig_scan + enqueue_device) ---------------------
 def plan(m, n, N, K, r, outs, planar=False, hop=0, beams=False, azel=False):
     """(path, scan, peaks) and the launches per sub-batch of one call; outs: the set of outputs the call asks for among
-    spectrum, P64, R, ev, bins, counts (angles always), beams (+ weights)"""
+    spectrum, P64, R, eigvals, bins, counts (angles always), beams (+ weights)"""
     fixed, music = r["rule"] == "fixed", r["est"] == "music"
     local, gridless, dml = r["peak"] == "local", r["peak"] in ("roots", "esprit"), r["peak"] == "dml"
     spec, p64o = "spectrum" in outs, "P64" in outs
     planar_fusable = not planar or (hop % 2 == 0 and N % 2 == 0)
     fusable = (not azel and music and fixed and not r["refine"] and r["peak"] == "top" and n == 1 and not p64o and
-               "R" not in outs and "ev" not in outs and not beams and not r["calib"])
+               "R" not in outs and "eigvals" not in outs and not beams and not r["calib"])
     fill = 1 if fixed and "counts" in outs else 0
     if fusable and m == 4 and planar_fusable:
         return ("fused4", None, None), fill + 1, 0
@@ -138,7 +137,7 @@ def plan(m, n, N, K, r, outs, planar=False, hop=0, beams=False, azel=False):
         cov = 1 + (m // 4 > 1)
     else:
         cov = 1
-    eig = (music and (not dml or spec or p64o)) or not fixed or "ev" in outs
+    eig = (music and (not dml or spec or p64o)) or not fixed or "eigvals" in outs
     argmax = n == 1 and not local and not gridless and not dml
     if music and (gridless or dml):
         scan = "grid" if spec or p64o else None
@@ -177,10 +176,6 @@ def sub_windows(m, n, K, ws, W):
 
 
 # ---- fixtures ----------------------------------------------------------------------------------------------------------
-def uca(m):
-    return np.asarray(mo.scaled_antenna_array(synth.SPACING, synth.antenna_array("uca", m)), np.float64)
-
-
 def ula(m):
     return np.array([[0.5 * LAM * i, 0.0] for i in range(m)])
 
@@ -200,16 +195,6 @@ def ula_windows(pos, N, seed, counts=(0, 1, 2, 3), per=2):
     return np.ascontiguousarray(np.array(xs).astype(np.complex64))
 
 
-def random_gains(rng, m):
-    return 10.0 ** (rng.uniform(-3.0, 3.0, m) / 20.0) * np.exp(1j * rng.uniform(-math.pi, math.pi, m))
-
-
-def corrupt(x, g):
-    m = len(g)
-    X = x.astype(np.complex128).reshape(x.shape[0], -1, m) * np.asarray(g)[None, None, :]
-    return np.ascontiguousarray(X.reshape(x.shape[0], -1).astype(np.complex64))
-
-
 def setup(r, seed, W_per=2):
     """(handle, raw input windows, gains or None, geometry or None) of one matrix row"""
     m, n, N = r["shape"]
@@ -221,7 +206,7 @@ def setup(r, seed, W_per=2):
         pos = ula(m)
         x = ula_windows(pos, N, seed, per=W_per)
     else:
-        pos = uca(m)
+        pos = positions("uca", m)
         _, x, _ = so.mixed_windows(m, N, K, seed, per=W_per)
     if r["table"] == "table":
         blk.set_array_response(helpers.planar_table(m, K, seed))
@@ -243,44 +228,8 @@ def apply(blk, r):
     blk.set_refine(r["refine"])
 
 
-def call(blk, x, K, outs, counts_entry=False):
-    """one process_device_ex call (process_device_counts with counts_entry) asking for angles and `outs`; returns
-    (outputs as numpy, kernel launches)"""
-    W, m, n = x.shape[0], blk.m, blk.n
-    d_in = torch.from_numpy(x.view(np.float32)).to(DEV)
-    shapes = {"levels": ((W, n), torch.float32), "spectrum": ((W, K), torch.float32), "bins": ((W, n), torch.int32),
-              "P64": ((W, K), torch.float64), "R": ((W, m, m, 2), torch.float64), "ev": ((W, m), torch.float64),
-              "counts": ((W,), torch.int32)}
-    o = {"angles": torch.full((W, n), SENTINEL, dtype=torch.float32, device=DEV)}
-    for k in outs:
-        o[k] = torch.full(shapes[k][0], SENTINEL, dtype=shapes[k][1], device=DEV)
-    p = lambda k: o[k].data_ptr() if k in o else None
-    l0 = blk.launch_count()
-    if counts_entry:
-        blk.process_device(d_in.data_ptr(), W, p("angles"), p("levels"), p("spectrum"), p("bins"), stream=STREAM(),
-                           d_counts=p("counts"))
-    else:
-        blk.process_device(d_in.data_ptr(), W, p("angles"), p("levels"), p("spectrum"), p("bins"), stream=STREAM(),
-                           d_P64=p("P64"), d_R=p("R"), d_eigvals=p("ev"))
-    torch.cuda.synchronize()
-    out = {k: v.cpu().numpy() for k, v in o.items()}
-    if "R" in out:
-        out["R"] = out["R"][..., 0] + 1j * out["R"][..., 1]
-    return out, blk.launch_count() - l0
-
-
-def circ(a, b):
-    d = abs(float(a) - float(b)) % 360.0
-    return min(d, 360.0 - d)
-
-
 def ulps(a, b):
     return circ(a, b) / float(np.spacing(np.float32(max(abs(float(a)), abs(float(b)), 1e-3))))
-
-
-def near_half(tdeg, K):
-    f = float(tdeg) * K / 360.0
-    return abs(f - math.floor(f) - 0.5) <= 1e-6
 
 
 # ---- the comparison with the composed oracle ------------------------------------------------------------------------------
@@ -345,7 +294,7 @@ def close_nan(a, b, rtol):
     return not np.any(~nan) or float(np.max(np.abs(a[~nan] - b[~nan]) / np.abs(b[~nan]))) <= rtol
 
 
-OUTPUT_SETS = {"all": ("levels", "spectrum", "bins", "P64", "R", "ev"), "angles": (), "levels": ("levels",), "bins": ("bins",)}
+OUTPUT_SETS = {"all": ("levels", "spectrum", "bins", "P64", "R", "eigvals"), "angles": (), "levels": ("levels",), "bins": ("bins",)}
 
 
 def same_or_close(a, b, same_kernel, ctx):
@@ -374,11 +323,11 @@ def test_matrix_row(r):
     ctx = row_id(r)
     res = {}
     for name, outs in OUTPUT_SETS.items():
-        res[name] = call(blk, x, K, outs)
+        res[name] = gh.device_call(blk, x, outs)
         key, want = launches(m, n, N, K, r, set(outs), W)
         assert res[name][1] == want, (ctx, name, res[name][1], want)
     co_outs = ("levels", "bins", "counts")
-    res["counts"] = call(blk, x, K, co_outs, counts_entry=True)
+    res["counts"] = gh.device_call(blk, x, co_outs)
     key_c, want = launches(m, n, N, K, r, set(co_outs), W)
     assert res["counts"][1] == want, (ctx, "counts", res["counts"][1], want)
     full = res["all"][0]
@@ -386,7 +335,7 @@ def test_matrix_row(r):
     R = full["R"]
     if g is not None:
         blk.set_calibration(None)
-        raw = call(blk, x, K, ("R",))[0]["R"]
+        raw = gh.device_call(blk, x, ("R",))[0]["R"]
         blk.set_calibration(g)
         want_R = np.array([co.correct(Rw, g) for Rw in raw])
         assert np.all(np.abs(R - want_R) <= 1e-15 * np.abs(want_R)), ctx
@@ -433,7 +382,7 @@ def test_check_modes_restatement():
     x = ula_windows(ula(m), N, 3, counts=(2,), per=2)
     d_in = torch.from_numpy(x.view(np.float32)).to(DEV)
     d_ang = torch.zeros((2, n), dtype=torch.float32, device=DEV)
-    tables = {"uca": lambda: blk.set_array_geometry(uca(m), LAM), "ula": lambda: blk.set_array_geometry(ula(m), LAM),
+    tables = {"uca": lambda: blk.set_array_geometry(positions("uca", m), LAM), "ula": lambda: blk.set_array_geometry(ula(m), LAM),
               "table": lambda: blk.set_array_response(helpers.planar_table(m, K, 5))}
     n_acc = n_ref = 0
     for peak in PEAK_CODES:
@@ -518,7 +467,7 @@ def test_entries(r):
     table = blk.array_response_c64()
     md = cmp.modes(r["peak"], r["excl"], r["est"], r["loading"], r["rule"], r["refine"])
     ctx = row_id(r)
-    dev, _ = call(blk, x, K, ("levels", "bins", "counts"), counts_entry=True)
+    dev, _ = gh.device_call(blk, x, ("levels", "bins", "counts"))
     # host
     ang, lvl = np.zeros((W, n), np.float32), np.zeros((W, n), np.float32)
     assert blk.work(W, [x], [ang, lvl]) == W
@@ -526,22 +475,14 @@ def test_entries(r):
     # planar, hop = N and an overlapping hop
     for hop in (N, N // 2 + 1):
         streams, xw = planar_streams(x, m, N, hop, W)
-        devw, _ = call(blk, xw, K, ("levels", "bins"))
+        devw, _ = gh.device_call(blk, xw, ("levels", "bins"))
         key_dev = launches(m, n, N, K, r, {"levels", "bins"}, W)[0]
         ang, lvl = np.zeros((W, n), np.float32), np.zeros((W, n), np.float32)
         assert blk.work_planar(W, streams, [ang, lvl], hop=hop) == W
         ph = {"angles": ang, "levels": lvl, "bins": blk.last_bins().copy()}
-        d_streams = [torch.from_numpy(s.view(np.float32)).to(DEV) for s in streams]
-        o = {"angles": torch.full((W, n), SENTINEL, dtype=torch.float32, device=DEV),
-             "levels": torch.full((W, n), SENTINEL, dtype=torch.float32, device=DEV),
-             "bins": torch.full((W, n), SENTINEL, dtype=torch.int32, device=DEV)}
-        l0 = blk.launch_count()
-        blk.process_planar_device([s.data_ptr() for s in d_streams], hop, W, o["angles"].data_ptr(), o["levels"].data_ptr(), None,
-                                  o["bins"].data_ptr(), stream=STREAM())
-        torch.cuda.synchronize()
+        pd, nl = gh.planar_device_call(blk, streams, hop, W, ("levels", "bins"))
         key_p, want = launches(m, n, N, K, r, {"levels", "bins"}, W, planar=True, hop=hop)
-        assert blk.launch_count() - l0 == want, (ctx, hop, blk.launch_count() - l0, want)
-        pd = {k: v.cpu().numpy() for k, v in o.items()}
+        assert nl == want, (ctx, hop, nl, want)
         same_or_close(ph, pd, True, (ctx, "planar host/device", hop))
         if m <= 4:
             same_or_close(pd, devw, key_p == key_dev, (ctx, "planar", hop))
@@ -558,9 +499,8 @@ def test_entries(r):
     # beams, device and host
     rule, loading = BEAM_RULES[ENTRY_ROWS.index(r) % len(BEAM_RULES)]
     blk.set_beamformer(rule, loading)
-    from test_gpu_beams import beams_call, check_beams, check_weights
-    ex, _ = call(blk, x, K, ("levels", "bins", "R"))
-    bd, nl = beams_call(blk, x, n, K)
+    ex, _ = gh.device_call(blk, x, ("levels", "bins", "R"))
+    bd, nl = gh.device_call(blk, x, ("levels", "bins", "counts", "weights", "beams"))
     key, want = launches(m, n, N, K, r, {"levels", "bins", "counts", "weights", "beams"}, W, beams=True)
     assert nl == want, (ctx, "beams", nl, want)
     same_or_close(bd, ex, True, (ctx, "beams vs ex"))
@@ -589,21 +529,10 @@ def test_entries(r):
         ang, lvl = np.zeros((W, n), np.float32), np.zeros((W, n), np.float32)
         assert mb.work(W, [x], [ang, lvl]) == W
         same_or_close({"angles": ang, "levels": lvl, "bins": mb.last_bins(), "counts": mb.last_counts()}, dev, True, (ctx, "multi"))
-        ins, angs, lvls, bins_all = [], [], [], []
-        for d in range(G):
-            dd = torch.device("cuda:%d" % d)
-            ins.append(torch.from_numpy(np.ascontiguousarray(x[d::G]).view(np.float32)).to(dd))
-            angs.append(torch.full((len(x[d::G]), n), SENTINEL, dtype=torch.float32, device=dd))
-            lvls.append(torch.full((len(x[d::G]), n), SENTINEL, dtype=torch.float32, device=dd))
-            bins_all.append(torch.full((W, n), SENTINEL, dtype=torch.int32, device=dd))
-        mb.process_device_sharded([t.data_ptr() for t in ins], W, [t.data_ptr() for t in angs], [t.data_ptr() for t in lvls],
-                                  [t.data_ptr() for t in bins_all])
-        for d in range(G):
-            torch.cuda.synchronize(d)
-        for d in range(G):
-            assert angs[d].cpu().numpy().tobytes() == dev["angles"][d::G].tobytes(), (ctx, "sharded", d)
-            assert lvls[d].cpu().numpy().tobytes() == dev["levels"][d::G].tobytes(), (ctx, "sharded", d)
-            assert bins_all[d].cpu().numpy().tobytes() == dev["bins"].tobytes(), (ctx, "sharded bins", d)
+        for d, sh in enumerate(gh.sharded_call(mb, x, levels=True)):
+            assert sh["angles"].tobytes() == dev["angles"][d::G].tobytes(), (ctx, "sharded", d)
+            assert sh["levels"].tobytes() == dev["levels"][d::G].tobytes(), (ctx, "sharded", d)
+            assert sh["bins"].tobytes() == dev["bins"].tobytes(), (ctx, "sharded bins", d)
         mb.close()
     blk.close()
 
@@ -635,18 +564,11 @@ def test_azel_matrix():
         blk.set_calibration(g if r["calib"] else None)
         x = corrupt(x0, g) if r["calib"] else x0
         W = len(x)
-        d_in = torch.from_numpy(x.view(np.float32)).to(DEV)
-        o = {k: torch.full((W, n), SENTINEL, dtype=torch.float32, device=DEV) for k in ("az", "el", "lv")}
-        o["sp"] = torch.full((W, grid.K), SENTINEL, dtype=torch.float32, device=DEV)
-        o["b"] = torch.full((W, n), SENTINEL, dtype=torch.int32, device=DEV)
-        o["c"] = torch.full((W,), SENTINEL, dtype=torch.int32, device=DEV)
-        l0 = blk.launch_count()
-        blk.process_device(d_in.data_ptr(), W, o["az"].data_ptr(), o["el"].data_ptr(), o["lv"].data_ptr(), o["sp"].data_ptr(),
-                           o["b"].data_ptr(), o["c"].data_ptr(), stream=STREAM())
-        torch.cuda.synchronize()
+        o, nl = gh.device_call(blk, x, ("levels", "spectrum", "bins", "counts"))
         key, want = launches(m, n, snaps, grid.K, dict(r, peak=r["peak"]), {"levels", "spectrum", "bins", "counts"}, W, azel=True)
-        assert blk.launch_count() - l0 == want, (ctx, blk.launch_count() - l0, want)
-        got = {k: v.cpu().numpy() for k, v in o.items()}
+        assert nl == want, (ctx, nl, want)
+        got = {k: o[key] for k, key in (("az", "azimuth"), ("el", "elevation"), ("lv", "levels"), ("sp", "spectrum"), ("b", "bins"),
+                                         ("c", "counts"))}
         R = cmp.covariance(x, m, g if r["calib"] else None)
         for w in range(W):
             d, margin = cmp.count(R[w], snaps, n, r["rule"])
@@ -704,7 +626,7 @@ def test_sub_batches(name, r, shape, K, W, outs, beams):
     holds on both sides of every boundary"""
     m, n, N = shape
     rng = np.random.default_rng(77)
-    pos = uca(m)
+    pos = positions("uca", m)
     blk = music_doa(m, n, m * N, np.ones((K, m), np.complex64), K)
     blk.set_array_geometry(pos, LAM)
     apply(blk, r)
@@ -734,9 +656,9 @@ def test_sub_batches(name, r, shape, K, W, outs, beams):
         return blk.launch_count() - l0
 
     def buffers():
-        o = {"angles": torch.full((W, n), SENTINEL, dtype=torch.float32, device=DEV)}
+        o = {"angles": torch.full((W, n), gh.SENTINEL, dtype=torch.float32, device=DEV)}
         for k in outs:
-            o[k] = torch.full((W,) + shapes[k][0], SENTINEL, dtype=shapes[k][1], device=DEV)
+            o[k] = torch.full((W,) + shapes[k][0], gh.SENTINEL, dtype=shapes[k][1], device=DEV)
         return o
 
     whole = buffers()
@@ -757,7 +679,7 @@ def test_sub_batches(name, r, shape, K, W, outs, beams):
     xs = np.ascontiguousarray(x[idx])
     sel = {k: v.cpu().numpy()[idx] for k, v in whole.items()}
     blk.set_beamformer("off", 0.0)
-    ex, _ = call(blk, xs, K, ("levels", "bins", "R"))
+    ex, _ = gh.device_call(blk, xs, ("levels", "bins", "R"))
     table = blk.array_response_c64()
     md = cmp.modes(r["peak"], r["excl"], r["est"], r["loading"], r["rule"], r["refine"])
     tally = Tally()
@@ -774,8 +696,7 @@ def test_sub_batches(name, r, shape, K, W, outs, beams):
     if beams:
         # the beams of the boundary windows equal a call that also returns the weights, which match the oracle
         blk.set_beamformer("mvdr", 0.01)
-        from test_gpu_beams import beams_call, check_weights
-        bd, _ = beams_call(blk, xs, n, K)
+        bd, _ = gh.device_call(blk, xs, ("levels", "bins", "counts", "weights", "beams"))
         bw = np.ascontiguousarray(sel["beams"]).view(np.float32)
         assert np.ascontiguousarray(bd["beams"]).view(np.float32).tobytes() == bw.tobytes(), name
         check_weights(bd["weights"], ex["R"], bd, bo.MVDR, 0.01, table, pos, name)
@@ -792,7 +713,7 @@ def test_calibration_accumulator_sizes(m):
     test_gpu_calibration.test_estimator); a repeated call sequence gives bit-identical gains (the CTA counter re-arms);
     host and device accumulation over the same split agree bit for bit.  At m = 16 the largest W run in two sub-batches."""
     N, az = 16, 40.0
-    pos = ula(2) if m == 2 else uca(m)
+    pos = ula(2) if m == 2 else positions("uca", m)
     kind = "phase" if m == 2 else "gain_phase"
     rng = np.random.default_rng(300 + m)
     g = random_gains(rng, m)

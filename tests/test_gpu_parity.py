@@ -15,6 +15,7 @@ from gr_baz_b200.music_doa_helper import music_doa_helper
 from oracle import c_oracle as co
 from oracle import music_oracle as mo
 
+import gpu_harness as gh
 import helpers
 
 pytestmark = pytest.mark.gpu
@@ -38,25 +39,13 @@ def run_block(cfg, table, x, spectrum=True, device_path=False, want_internals=Fa
         assert blk.work(W, [x], outs) == W
         out.update(angles=ang, levels=lvl, bins=blk.last_bins().copy())
     else:
-        dev = torch.device("cuda:0")
-        d_in = torch.from_numpy(x.view(np.float32)).to(dev)
-        d_ang = torch.empty((W, cfg["n"]), dtype=torch.float32, device=dev)
-        d_lvl = torch.empty_like(d_ang)
-        d_bins = torch.empty((W, cfg["n"]), dtype=torch.int32, device=dev)
-        d_spec = torch.empty((W, cfg["resolution"]), dtype=torch.float32, device=dev) if spectrum else None
-        d_P = torch.empty((W, cfg["resolution"]), dtype=torch.float64, device=dev) if want_internals else None
-        d_R = torch.empty((W, cfg["m"], cfg["m"], 2), dtype=torch.float64, device=dev) if want_internals else None
-        d_ev = torch.empty((W, cfg["m"]), dtype=torch.float64, device=dev) if want_internals else None
-        ptr = lambda t: t.data_ptr() if t is not None else None
-        blk.process_device(ptr(d_in), W, ptr(d_ang), ptr(d_lvl), ptr(d_spec), ptr(d_bins),
-                           stream=torch.cuda.current_stream().cuda_stream, d_P64=ptr(d_P), d_R=ptr(d_R), d_eigvals=ptr(d_ev))
-        torch.cuda.synchronize()
-        out.update(angles=d_ang.cpu().numpy(), levels=d_lvl.cpu().numpy(), bins=d_bins.cpu().numpy())
+        internals = ("P64", "R", "eigvals") if want_internals else ()
+        o, _ = gh.device_call(blk, x, ("levels", "bins") + (("spectrum",) if spectrum else ()) + internals)
+        out.update(angles=o["angles"], levels=o["levels"], bins=o["bins"])
         if spectrum:
-            out["spectrum"] = d_spec.cpu().numpy()
+            out["spectrum"] = o["spectrum"]
         if want_internals:
-            R = d_R.cpu().numpy()
-            out.update(P=d_P.cpu().numpy(), R=R[..., 0] + 1j * R[..., 1], eigvals=d_ev.cpu().numpy())
+            out.update(P=o["P64"], R=o["R"], eigvals=o["eigvals"])
     out["launches"] = blk.launch_count()
     blk.close()
     return out

@@ -12,28 +12,11 @@ from gr_baz_b200.music_doa import music_doa
 from oracle import c_oracle as co
 
 import helpers
+from helpers import form_windows, streams_for
 
 pytestmark = pytest.mark.gpu
 
 P_RTOL = 1e-5
-
-
-def streams_for(cfg, seed, total_snapshots):
-    """m planar streams cut out of the synthetic generator: consecutive generator windows laid end to end."""
-    N = cfg["snapshots"]
-    nwin = (total_snapshots + N - 1) // N
-    x = synth.gen_windows_numpy(cfg, seed, 0, nwin).reshape(nwin * N, cfg["m"])  # [snapshot][antenna]
-    return [np.ascontiguousarray(x[:total_snapshots, r]) for r in range(cfg["m"])]
-
-
-def form_windows(streams, hop, W, N):
-    """what interleave + stream_to_vector (+ overlap) hand to the reference block"""
-    m = len(streams)
-    out = np.empty((W, N * m), np.complex64)
-    for w in range(W):
-        seg = np.stack([s[w * hop:w * hop + N] for s in streams], axis=1)  # (N, m): sample-interleaved
-        out[w] = seg.reshape(-1)
-    return out
 
 
 CASES = [  # base config, overrides, hop (None = N), windows

@@ -4,79 +4,38 @@ a 1000x finer grid, and through every entry point.
 The oracle refines the GPU's own grid bins with LAPACK noise eigenvectors, so what is compared here is the refinement
 itself; the grid bins are compared with the same handle with refinement off (byte for byte) and, elsewhere in the
 suite, with the C oracle."""
-import os
 import struct
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
-from gr_baz_b200 import _capi, build, synth
+from gr_baz_b200 import _capi, synth
 from gr_baz_b200.music_doa import music_doa
 from gr_baz_b200.music_doa_helper import music_doa_helper
 from oracle import music_oracle as mo
 
+import gpu_harness as gh
 import refine_oracle as ro
+from helpers import LAM, offgrid_windows, positions
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-LAM = synth.C_LIGHT / synth.FREQUENCY
-SENTINEL = -7
 N = 256
 W = 6
 EXCL = 3
 FLIP = 1e-9      # decisions the oracle sees this close to flipping may go either way
 L_RTOL = 1e-5
+ALL = ("levels", "bins", "spectrum", "counts")
+PEAKS = ("levels", "bins")
 
 
-def positions(geometry, m):
-    return np.asarray(mo.scaled_antenna_array(synth.SPACING, synth.antenna_array(geometry, m)), np.float64)
-
-
-def windows(pos, n_of, seed, snaps=N, noise=0.1):
-    """complex64 (len(n_of), m * snaps) windows; window w holds n_of[w] unit-power sources at random off-grid angles
-    plus complex white noise of power noise^2 (20 dB at the default); returns (x, true angles per window)"""
-    rng = np.random.default_rng(seed)
-    m = pos.shape[0]
-    xs, truth = [], []
-    for S in n_of:
-        X = noise * (rng.standard_normal((m, snaps)) + 1j * rng.standard_normal((m, snaps))) / np.sqrt(2.0)
-        angs = rng.uniform(0.0, 360.0, S)
-        for t in angs:
-            a = ro.steering(pos, LAM, np.deg2rad(t))[0]
-            X += a[:, None] * np.exp(2j * np.pi * rng.uniform(0.0, 1.0, snaps))[None, :]
-        xs.append(X.T.reshape(-1))  # x(r, c) = in[c * m + r]
-        truth.append(angs)
-    return np.ascontiguousarray(np.array(xs).astype(np.complex64)), truth
+def windows(pos, n_of, seed, snaps=N):
+    return offgrid_windows(pos, n_of, seed, snaps)
 
 
 def handle(m, n, K, pos, snaps=N, devices=None):
-    blk = music_doa(m, n, m * snaps, np.ones((K, m), np.complex64), K, devices=devices)
-    blk.set_array_geometry(pos, LAM)
-    return blk
-
-
-def dev_call(blk, x, n, K, spectrum=True, counts=True, bins=True, levels=True):
-    dev = torch.device("cuda:0")
-    Wn = x.shape[0]
-    d_in = torch.from_numpy(x.view(np.float32)).to(dev)
-    o = {"angles": torch.full((Wn, n), SENTINEL, dtype=torch.float32, device=dev)}
-    if levels:
-        o["levels"] = torch.full((Wn, n), SENTINEL, dtype=torch.float32, device=dev)
-    if bins:
-        o["bins"] = torch.full((Wn, n), SENTINEL, dtype=torch.int32, device=dev)
-    if spectrum:
-        o["spectrum"] = torch.full((Wn, K), SENTINEL, dtype=torch.float32, device=dev)
-    if counts:
-        o["counts"] = torch.full((Wn,), SENTINEL, dtype=torch.int32, device=dev)
-    p = lambda k: o[k].data_ptr() if k in o else None
-    l0 = blk.launch_count()
-    blk.process_device(d_in.data_ptr(), Wn, p("angles"), p("levels"), p("spectrum"), p("bins"),
-                       stream=torch.cuda.current_stream().cuda_stream, d_counts=p("counts"))
-    torch.cuda.synchronize()
-    return {k: v.cpu().numpy() for k, v in o.items()}, blk.launch_count() - l0
+    return gh.make_block(m, n, snaps, K, pos=pos, devices=devices)
 
 
 def ulps_apart(a, b):
@@ -106,9 +65,9 @@ def test_parity_with_oracle(m, n):
                     ctx = (m, n, geometry, K, rule, peak)
                     blk.set_peak_mode("top_bins" if peak == "top" else "local_maxima", EXCL)
                     blk.set_refine(False)
-                    off, _ = dev_call(blk, x, n, K)
+                    off, _ = gh.device_call(blk, x, ALL)
                     blk.set_refine(True)
-                    on, _ = dev_call(blk, x, n, K)
+                    on, _ = gh.device_call(blk, x, ALL)
                     for k in ("bins", "spectrum", "counts"):
                         assert np.array_equal(on[k].view(np.int32), off[k].view(np.int32)), (ctx, k)
                     for w in range(W):
@@ -146,11 +105,11 @@ def test_off_means_off_on_every_entry():
         x, _ = windows(pos, [n] * 16, 77 + m)
         fresh, used = handle(m, n, K, pos), handle(m, n, K, pos)
         used.set_refine(True)
-        dev_call(used, x, n, K)
+        gh.device_call(used, x, ALL)
         used.set_refine(False)
         assert not used.refine
-        a, la = dev_call(fresh, x, n, K, spectrum=False, counts=False)
-        b, lb = dev_call(used, x, n, K, spectrum=False, counts=False)
+        a, la = gh.device_call(fresh, x, PEAKS)
+        b, lb = gh.device_call(used, x, PEAKS)
         assert la == lb and (m != 4 or la == 1), (la, lb)
         for k in a:
             assert np.array_equal(a[k].view(np.int32), b[k].view(np.int32)), (m, k)
@@ -181,9 +140,9 @@ def test_against_a_1000x_finer_grid(cid):
     x = synth.gen_windows_numpy(cfg, 2718 + cid, 0, Wc)
     coarse = handle(m, 1, Kc, pos, snaps=1024)
     coarse.set_refine(True)
-    rc, _ = dev_call(coarse, x, 1, Kc, spectrum=False)
+    rc, _ = gh.device_call(coarse, x, ("levels", "bins", "counts"))
     fine = handle(m, 1, Kf, pos, snaps=1024)
-    rf, _ = dev_call(fine, x, 1, Kf, spectrum=False)
+    rf, _ = gh.device_call(fine, x, ("levels", "bins", "counts"))
     table_f = fine.array_response_c64().astype(np.complex128)
     coarse.close()
     fine.close()
@@ -217,7 +176,7 @@ def test_edges():
         X += 0.01 * (rng.standard_normal((m, N)) + 1j * rng.standard_normal((m, N)))
         xs.append(X.T.reshape(-1))
     x = np.array(xs).astype(np.complex64)
-    got, _ = dev_call(blk, x, n, K)
+    got, _ = gh.device_call(blk, x, ALL)
     assert np.all(got["angles"] >= 0.0) and np.all(got["angles"] < 360.0), got["angles"]
     err = ro.angle_error(got["angles"][:, 0], np.array([0.05, 359.95, 0.05, 359.95]), "uca")
     assert np.all(err < 0.02), err
@@ -227,7 +186,7 @@ def test_edges():
     xe[1, 5] = np.nan
     for rule in ("fixed", "mdl"):
         blk.set_source_rule(rule)
-        got, _ = dev_call(blk, xe, n, K)
+        got, _ = gh.device_call(blk, xe, ALL)
         empty = [1] if rule == "fixed" else [0, 1, 2]
         for w in empty:
             assert got["bins"][w, 0] == -1 and got["angles"][w, 0] == 0.0 and got["levels"][w, 0] == 0.0, (rule, w)
@@ -244,38 +203,32 @@ def test_entries_agree():
     blk.set_peak_mode("local_maxima", EXCL)
     blk.set_refine(True)
     assert blk.refine
-    ref, _ = dev_call(blk, x, n, K, spectrum=False, counts=False)
-    ang, lvl = np.zeros((Wn, n), np.float32), np.zeros((Wn, n), np.float32)
-    blk.work(Wn, [x], [ang, lvl])
-    assert np.array_equal(ang, ref["angles"]) and np.array_equal(lvl, ref["levels"]) and np.array_equal(blk.last_bins(), ref["bins"])
-    assert not np.array_equal(ang, (ref["bins"] * (360.0 / K)).astype(np.float32))  # refined, not grid angles
-    xs = x.reshape(Wn, N, m)
-    streams = [np.ascontiguousarray(xs[:, :, r].reshape(-1)) for r in range(m)]
-    pa, pl = np.zeros((Wn, n), np.float32), np.zeros((Wn, n), np.float32)
-    blk.work_planar(Wn, streams, [pa, pl])
-    assert np.array_equal(pa, ref["angles"]) and np.array_equal(pl, ref["levels"])
-    dev = torch.device("cuda:0")
-    d_streams = [torch.from_numpy(s.view(np.float32)).to(dev) for s in streams]
-    da = torch.zeros((Wn, n), dtype=torch.float32, device=dev)
-    dl = torch.zeros((Wn, n), dtype=torch.float32, device=dev)
-    blk.process_planar_device([s.data_ptr() for s in d_streams], N, Wn, da.data_ptr(), dl.data_ptr(),
-                              stream=torch.cuda.current_stream().cuda_stream)  # no bins: the workspace holds them
-    torch.cuda.synchronize()
-    assert np.array_equal(da.cpu().numpy(), ref["angles"]) and np.array_equal(dl.cpu().numpy(), ref["levels"])
+    ref, _ = gh.device_call(blk, x, PEAKS)
     # the device entry without bins, angles only
-    nb, _ = dev_call(blk, x, n, K, spectrum=False, counts=False, bins=False, levels=False)
+    nb, _ = gh.device_call(blk, x)
     assert np.array_equal(nb["angles"], ref["angles"])
     blk.close()
+
+    def make(devices=None):
+        b = handle(m, n, K, pos, devices=devices)
+        b.set_peak_mode("local_maxima", EXCL)
+        b.set_refine(True)
+        return b
+
+    # planar device without bins: the workspace holds them
+    e = gh.entry_outputs(make, x, planar_outputs=("levels",))
+    ang, lvl = e["host"]["angles"], e["host"]["levels"]
+    assert np.array_equal(ang, ref["angles"]) and np.array_equal(lvl, ref["levels"]) and np.array_equal(e["host"]["bins"], ref["bins"])
+    assert not np.array_equal(ang, (ref["bins"] * (360.0 / K)).astype(np.float32))  # refined, not grid angles
+    pa, pl = e["planar_host"]["angles"], e["planar_host"]["levels"]
+    assert np.array_equal(pa, ref["angles"]) and np.array_equal(pl, ref["levels"])
+    da, dl = e["planar_device"]["angles"], e["planar_device"]["levels"]
+    assert np.array_equal(da, ref["angles"]) and np.array_equal(dl, ref["levels"])
     for devices in ([0], list(range(torch.cuda.device_count()))):
-        mb = handle(m, n, K, pos, devices=devices)
-        mb.set_peak_mode("local_maxima", EXCL)
-        mb.set_refine(True)
-        a2, l2 = np.zeros((Wn, n), np.float32), np.zeros((Wn, n), np.float32)
-        mb.work(Wn, [x], [a2, l2])
+        a2, l2 = e["multi_host%s" % devices]["angles"], e["multi_host%s" % devices]["levels"]
         assert np.array_equal(a2, ref["angles"]) and np.array_equal(l2, ref["levels"]), devices
-        g, _ = dev_call(mb, x, n, K, spectrum=False, counts=False)
+        g = e["multi_device%s" % devices]
         assert np.array_equal(g["angles"], ref["angles"]) and np.array_equal(g["bins"], ref["bins"]), devices
-        mb.close()
     # the helper installs the geometry and keeps refining across a retune
     cfg = synth.config(4, snapshots=N, resolution=K)
     hx = synth.gen_windows_numpy(cfg, 99, 0, 8)
@@ -283,7 +236,7 @@ def test_entries_agree():
     assert hp.impl.refine
     plain = handle(m, 1, K, positions("uca", m))
     plain.set_refine(True)
-    pr, _ = dev_call(plain, hx, 1, K, spectrum=False, counts=False)
+    pr, _ = gh.device_call(plain, hx, PEAKS)
     plain.close()
     ha, hl = np.zeros((8, 1), np.float32), np.zeros((8, 1), np.float32)
     hp.work(8, [hx], [ha, hl])
@@ -303,22 +256,13 @@ def test_sharded_entry():
     x, _ = windows(pos, [n] * Wn, 41)
     blk = handle(m, n, K, pos)
     blk.set_refine(True)
-    ref, _ = dev_call(blk, x, n, K, spectrum=False, counts=False)
+    ref, _ = gh.device_call(blk, x, PEAKS)
     blk.close()
     mb = handle(m, n, K, pos, devices=list(range(G)))
     mb.set_refine(True)
-    ins, angs, bins_all = [], [], []
-    for g in range(G):
-        d = torch.device("cuda", g)
-        ins.append(torch.from_numpy(np.ascontiguousarray(x[g::G]).view(np.float32)).to(d))
-        angs.append(torch.zeros((len(x[g::G]), n), dtype=torch.float32, device=d))
-        bins_all.append(torch.full((Wn, n), SENTINEL, dtype=torch.int32, device=d))
-    mb.process_device_sharded([t.data_ptr() for t in ins], Wn, [t.data_ptr() for t in angs], None, [t.data_ptr() for t in bins_all])
-    for g in range(G):
-        torch.cuda.synchronize(g)
-    for g in range(G):
-        assert np.array_equal(angs[g].cpu().numpy(), ref["angles"][g::G]), g
-        assert np.array_equal(bins_all[g].cpu().numpy(), ref["bins"]), g
+    for g, sh in enumerate(gh.sharded_call(mb, x)):
+        assert np.array_equal(sh["angles"], ref["angles"][g::G]), g
+        assert np.array_equal(sh["bins"], ref["bins"]), g
     mb.close()
 
 
@@ -327,9 +271,9 @@ def test_launch_counts_and_sub_batches():
     pos = positions("ula_x", 4)
     x, _ = windows(pos, [1] * 8, 3)
     blk = handle(4, 1, 3600, pos)
-    _, l_off = dev_call(blk, x, 1, 3600, spectrum=False, counts=False)
+    _, l_off = gh.device_call(blk, x, PEAKS)
     blk.set_refine(True)
-    _, l_on = dev_call(blk, x, 1, 3600, spectrum=False, counts=False)
+    _, l_on = gh.device_call(blk, x, PEAKS)
     assert (l_off, l_on) == (1, 4)
     blk.close()
     # several sub-batches: one extra launch in each, and the whole call equals two calls over its halves
@@ -347,8 +291,8 @@ def test_launch_counts_and_sub_batches():
         torch.cuda.synchronize()
         return blk.launch_count() - l0
 
-    outs = lambda: [torch.full((Wb, n), SENTINEL, dtype=torch.float32, device=dev), torch.full((Wb, n), SENTINEL, dtype=torch.float32, device=dev),
-                    torch.full((Wb, n), SENTINEL, dtype=torch.int32, device=dev)]
+    outs = lambda: [torch.full((Wb, n), gh.SENTINEL, dtype=torch.float32, device=dev), torch.full((Wb, n), gh.SENTINEL, dtype=torch.float32, device=dev),
+                    torch.full((Wb, n), gh.SENTINEL, dtype=torch.int32, device=dev)]
     per_sub = 4  # cov4_tma + eig + scan + top-n
     l_off = run(0, Wb, outs())
     assert l_off % per_sub == 0 and l_off // per_sub >= 2
@@ -379,45 +323,31 @@ def test_errors():
     blk.set_array_geometry(pos, LAM)
     blk.set_refine(True)
     x, _ = windows(pos, [1] * 4, 13)
-    dev_call(blk, x, 1, K)
+    gh.device_call(blk, x, ALL)
     blk.set_array_response(np.ones((K, m), np.complex64))  # a table without geometry: the next call must fail
     with pytest.raises(_capi.MusicB200Error) as e:
-        dev_call(blk, x, 1, K)
+        gh.device_call(blk, x, ALL)
     assert e.value.code == _capi.EINVAL
     with pytest.raises(_capi.MusicB200Error) as e:
         blk.work(4, [x], [np.zeros((4, 1), np.float32)])
     assert e.value.code == _capi.EINVAL
     blk.set_refine(False)
-    dev_call(blk, x, 1, K)
+    gh.device_call(blk, x, ALL)
     blk.close()
 
 
-def test_cpp_block_refine(tmp_path):
-    build.build_cuda()
-    subprocess.check_call(["make", "-C", os.path.join(ROOT, "lib"), "-s"])
+def test_cpp_block_refine():
     m, n, K, Wn = 8, 2, 720, 12
     pos = positions("uca", m)
     x, _ = windows(pos, [n] * Wn, 55)
     table = np.ones((K, m), np.complex64)
-    fin, fout, fgeo = tmp_path / "in.bin", tmp_path / "out.bin", tmp_path / "geom.bin"
-    with open(fin, "wb") as f:
-        f.write(struct.pack("<5I", m, n, m * N, K, Wn))
-        f.write(table.view(np.float32).tobytes())
-        f.write(table.view(np.float32).tobytes())
-        f.write(x.view(np.float32).tobytes())
-    with open(fgeo, "wb") as f:
-        f.write(np.ascontiguousarray(pos).tobytes())
-        f.write(struct.pack("<d", LAM))
-    r = subprocess.run([os.path.join(ROOT, "lib", "_build", "test_block"), str(fin), str(fout), "0", str(fgeo)], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    raw = np.fromfile(fout, dtype=np.float32)
-    o = 0
-    ang = raw[o:o + Wn * n].reshape(Wn, n); o += Wn * n
-    lvl = raw[o:o + Wn * n].reshape(Wn, n); o += Wn * n
-    spec = raw[o:o + Wn * K].reshape(Wn, K); o += Wn * K
-    bins = raw[o:o + Wn * n].view(np.int32).reshape(Wn, n); o += Wn * n
-    counts = raw[o:o + Wn].view(np.int32); o += Wn
-    assert o == raw.size and np.all(counts == n)
+    geometry = np.ascontiguousarray(pos).tobytes() + struct.pack("<d", LAM)
+    c = gh.run_cpp_block("test_block", struct.pack("<5I", m, n, m * N, K, Wn), [table, table, x],
+                         [("a", np.float32, Wn * n), ("l", np.float32, Wn * n), ("s", np.float32, Wn * K),
+                          ("b", np.int32, Wn * n), ("c", np.int32, Wn)], args=("0", geometry))
+    ang, lvl, spec = c["a"].reshape(Wn, n), c["l"].reshape(Wn, n), c["s"].reshape(Wn, K)
+    bins, counts = c["b"].reshape(Wn, n), c["c"]
+    assert np.all(counts == n)
     py = handle(m, n, K, pos)
     py.set_refine(True)
     pa, pl, ps = np.zeros((Wn, n), np.float32), np.zeros((Wn, n), np.float32), np.zeros((Wn, K), np.float32)

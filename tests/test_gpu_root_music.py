@@ -3,9 +3,7 @@ numpy.roots on LAPACK eigenvectors), through every entry point, and the other pe
 
 The oracle runs on the GPU's own covariance (d_R), so what is compared is the root stage itself."""
 import math
-import os
 import struct
-import subprocess
 
 import numpy as np
 import pytest
@@ -15,112 +13,22 @@ from gr_baz_b200 import _capi, synth
 from gr_baz_b200.music_doa import music_doa
 from gr_baz_b200.music_doa_azel import music_doa_azel
 
-import refine_oracle as ro
+import gpu_harness as gh
 import root_music_oracle as rm
+from helpers import LAM, PLAN, axis_deg, circ, near_half, plan_windows as windows, two_source_windows, ula
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-LAM = synth.C_LIGHT / synth.FREQUENCY
-SENTINEL = -7
 FLIP = 1e-9     # selections the oracle sees this close to flipping may go either way
 L_RTOL = 1e-5
-
-
-def ula(m, kind):
-    """x-axis, y-axis, an oblique offset ULA and the x-axis ULA in reversed order, lambda / 2 apart"""
-    axis, p0, rev = {"x": (0.0, (0.0, 0.0), False), "y": (90.0, (0.0, 0.0), False),
-                     "oblique": (30.0, (0.7, -1.3), False), "reversed": (0.0, (0.0, 0.0), True)}[kind]
-    a = math.radians(axis)
-    pos = np.array([[p0[0] + 0.5 * i * math.cos(a), p0[1] + 0.5 * i * math.sin(a)] for i in range(m)])
-    return pos[::-1].copy() if rev else pos
-
-
-def axis_deg(pos):
-    s = rm.ula_geometry(pos, LAM)[2]
-    return math.degrees(math.atan2(s[1], s[0]))
-
-
-def source_angles(rng, S, alpha, min_cos=0.05):
-    """S angles over [0, 360), at least 2 degrees from end-fire, with distinct cos(t - alpha)"""
-    while True:
-        t = rng.uniform(0.0, 360.0, S)
-        off = (t - alpha) % 180.0
-        if np.any(np.minimum(off, 180.0 - off) < 2.0):
-            continue
-        cs = np.cos(np.radians(t - alpha))
-        if S < 2 or np.min(np.abs(np.subtract.outer(cs, cs))[np.triu_indices(S, 1)]) >= min_cos:
-            return t
-
-
-def windows(pos, plan, seed, snaps):
-    """complex64 windows; plan[w] = (sources, snr_db or None for noiseless); returns (x, truth per window)"""
-    rng = np.random.default_rng(seed)
-    m = pos.shape[0]
-    alpha = axis_deg(pos)
-    xs, truth = [], []
-    for S, snr in plan:
-        X = np.zeros((m, snaps), np.complex128)
-        if snr is not None:
-            X += (rng.standard_normal((m, snaps)) + 1j * rng.standard_normal((m, snaps))) / np.sqrt(2.0)
-        angs = source_angles(rng, S, alpha) if S else np.zeros(0)
-        amp = 1.0 if snr is None else 10.0 ** (snr / 20.0)
-        for t in angs:
-            a = ro.steering(pos, LAM, math.radians(t))[0]
-            X += amp * a[:, None] * (rng.standard_normal(snaps) + 1j * rng.standard_normal(snaps))[None, :] / np.sqrt(2.0)
-        xs.append(X.T.reshape(-1))
-        truth.append(angs)
-    return np.ascontiguousarray(np.array(xs).astype(np.complex64)), truth
+PEAKS = ("levels", "bins")
 
 
 def handle(m, n, K, pos, snaps, mode="roots", rule="fixed", devices=None):
-    blk = music_doa(m, n, m * snaps, np.ones((K, m), np.complex64), K, devices=devices)
-    blk.set_array_geometry(pos, LAM)
-    blk.set_source_rule(rule)
-    blk.set_peak_mode(mode, 0)
-    return blk
-
-
-def dev_call(blk, x, n, K, spectrum=False, p64=False, R=False, counts=False):
-    """one process_device_ex call (or process_device_counts with counts); returns (outputs, kernel launches)"""
-    dev = torch.device("cuda:0")
-    Wn, m = x.shape[0], blk.m
-    d_in = torch.from_numpy(x.view(np.float32)).to(dev)
-    o = {"angles": torch.full((Wn, n), SENTINEL, dtype=torch.float32, device=dev),
-         "levels": torch.full((Wn, n), SENTINEL, dtype=torch.float32, device=dev),
-         "bins": torch.full((Wn, n), SENTINEL, dtype=torch.int32, device=dev)}
-    if spectrum:
-        o["spectrum"] = torch.full((Wn, K), SENTINEL, dtype=torch.float32, device=dev)
-    if p64:
-        o["P64"] = torch.full((Wn, K), SENTINEL, dtype=torch.float64, device=dev)
-    if R:
-        o["R"] = torch.zeros((Wn, m, m, 2), dtype=torch.float64, device=dev)
-    if counts:
-        o["counts"] = torch.full((Wn,), SENTINEL, dtype=torch.int32, device=dev)
-    p = lambda k: o[k].data_ptr() if k in o else None
-    l0 = blk.launch_count()
-    blk.process_device(d_in.data_ptr(), Wn, p("angles"), p("levels"), p("spectrum"), p("bins"),
-                       stream=torch.cuda.current_stream().cuda_stream, d_P64=p("P64"), d_R=p("R"), d_counts=p("counts"))
-    torch.cuda.synchronize()
-    out = {k: v.cpu().numpy() for k, v in o.items()}
-    if "R" in out:
-        out["R"] = out["R"][..., 0] + 1j * out["R"][..., 1]
-    return out, blk.launch_count() - l0
-
-
-def circ(a, b):
-    d = abs(float(a) - float(b)) % 360.0
-    return min(d, 360.0 - d)
-
-
-def near_half(tdeg, K):
-    f = tdeg * K / 360.0
-    return abs(f - math.floor(f) - 0.5) <= 1e-6
+    return gh.make_block(m, n, snaps, K, pos=pos, rule=rule, mode=mode, devices=devices)
 
 
 # ---- parity with the oracle ------------------------------------------------------------------------------------------
-PLAN = [(0, 0.0), (1, 40.0), (2, 40.0), (1, 20.0), (2, 20.0), (3, 20.0), (1, 0.0), (2, 0.0), (3, 0.0), (1, None),
-        (2, None), (3, 10.0)]
 
 
 @pytest.mark.parametrize("m", [2, 3, 4, 5, 8, 12, 16])
@@ -139,12 +47,12 @@ def test_parity_with_oracle(m):
             for rule in ("fixed", "mdl"):
                 K = 3600 if (gi + n) % 2 else 360
                 blk = handle(m, n, K, pos, snaps, rule=rule)
-                out, _ = dev_call(blk, x, n, K, R=True)
+                out, _ = gh.device_call(blk, x, PEAKS + ("R",))
                 counts = None
                 if rule == "mdl":
-                    cnt, _ = dev_call(blk, x, n, K, counts=True)
+                    cnt, _ = gh.device_call(blk, x, PEAKS + ("counts",))
                     top = handle(m, n, K, pos, snaps, mode="top_bins", rule=rule)
-                    tc, _ = dev_call(top, x, n, K, counts=True)
+                    tc, _ = gh.device_call(top, x, PEAKS + ("counts",))
                     top.close()
                     assert np.array_equal(cnt["counts"], tc["counts"]), (m, n, kind)
                     assert np.array_equal(cnt["angles"], out["angles"]) and np.array_equal(cnt["bins"], out["bins"])
@@ -186,7 +94,7 @@ def test_degenerate_windows():
     x[1, 17] = np.nan
     for rule in ("fixed", "mdl"):
         blk = handle(m, n, K, pos, snaps, rule=rule)
-        out, _ = dev_call(blk, x, n, K)
+        out, _ = gh.device_call(blk, x, PEAKS)
         empty = [0, 1] if rule == "fixed" else [0, 1, 2]
         for w in empty:
             assert np.all(out["bins"][w] == -1) and np.all(out["angles"][w] == 0.0) and np.all(out["levels"][w] == 0.0), (rule, w, out)
@@ -202,59 +110,37 @@ def test_entries_agree():
     pos = ula(m, "x")
     x, _ = windows(pos, [(1, 20.0)] * Wn, 31, snaps)
     blk = handle(m, n, K, pos, snaps)
-    ref, _ = dev_call(blk, x, n, K)
+    ref, _ = gh.device_call(blk, x, PEAKS)
     assert np.all(ref["bins"] >= 0)
-    ex, _ = dev_call(blk, x, n, K, spectrum=True, p64=True, R=True)
-    cn, _ = dev_call(blk, x, n, K, counts=True)
+    ex, _ = gh.device_call(blk, x, PEAKS + ("spectrum", "P64", "R"))
+    cn, _ = gh.device_call(blk, x, PEAKS + ("counts",))
     for o in (ex, cn):
         assert all(np.array_equal(o[k], ref[k]) for k in ("angles", "levels", "bins"))
     assert np.all(cn["counts"] == n)
     loc = handle(m, n, K, pos, snaps, mode="local_maxima")
-    lo, _ = dev_call(loc, x, n, K, spectrum=True, p64=True)
+    lo, _ = gh.device_call(loc, x, PEAKS + ("spectrum", "P64"))
     loc.close()
     assert np.array_equal(lo["spectrum"], ex["spectrum"]) and np.array_equal(lo["P64"], ex["P64"])
-    ang, lvl, spec = np.zeros((Wn, n), np.float32), np.zeros((Wn, n), np.float32), np.zeros((Wn, K), np.float32)
-    blk.work(Wn, [x], [ang, lvl, spec])
-    assert np.array_equal(ang, ref["angles"]) and np.array_equal(lvl, ref["levels"]) and np.array_equal(blk.last_bins(), ref["bins"])
-    assert np.array_equal(spec, ex["spectrum"])
-    streams = [np.ascontiguousarray(x.reshape(Wn, snaps, m)[:, :, r].reshape(-1)) for r in range(m)]
-    pa, pl = np.zeros((Wn, n), np.float32), np.zeros((Wn, n), np.float32)
-    blk.work_planar(Wn, streams, [pa, pl])
-    assert np.array_equal(pa, ref["angles"]) and np.array_equal(pl, ref["levels"]) and np.array_equal(blk.last_bins(), ref["bins"])
-    dev = torch.device("cuda:0")
-    d_streams = [torch.from_numpy(s.view(np.float32)).to(dev) for s in streams]
-    da = torch.zeros((Wn, n), dtype=torch.float32, device=dev)
-    l0 = blk.launch_count()
-    blk.process_planar_device([t.data_ptr() for t in d_streams], snaps, Wn, da.data_ptr(), stream=torch.cuda.current_stream().cuda_stream)
-    torch.cuda.synchronize()
-    assert blk.launch_count() - l0 == 3  # the planar covariance, eig, roots: never the fused kernel
-    assert np.array_equal(da.cpu().numpy(), ref["angles"])
     blk.close()
+    e = gh.entry_outputs(lambda devices=None: handle(m, n, K, pos, snaps, devices=devices), x, spectrum=True)
+    h = e["host"]
+    assert np.array_equal(h["angles"], ref["angles"]) and np.array_equal(h["levels"], ref["levels"]) and np.array_equal(h["bins"], ref["bins"])
+    assert np.array_equal(h["spectrum"], ex["spectrum"])
+    ph = e["planar_host"]
+    assert np.array_equal(ph["angles"], ref["angles"]) and np.array_equal(ph["levels"], ref["levels"]) and np.array_equal(ph["bins"], ref["bins"])
+    assert e["planar_launches"] == 3  # the planar covariance, eig, roots: never the fused kernel
+    assert np.array_equal(e["planar_device"]["angles"], ref["angles"])
     G = torch.cuda.device_count()
     for devices in ([0], list(range(G))):
-        mb = handle(m, n, K, pos, snaps, devices=devices)
-        a2, l2 = np.zeros((Wn, n), np.float32), np.zeros((Wn, n), np.float32)
-        mb.work(Wn, [x], [a2, l2])
-        assert np.array_equal(a2, ref["angles"]) and np.array_equal(l2, ref["levels"]), devices
-        g, _ = dev_call(mb, x, n, K)
+        a2 = e["multi_host%s" % devices]
+        assert np.array_equal(a2["angles"], ref["angles"]) and np.array_equal(a2["levels"], ref["levels"]), devices
+        g = e["multi_device%s" % devices]
         assert np.array_equal(g["angles"], ref["angles"]) and np.array_equal(g["bins"], ref["bins"]), devices
-        mb.close()
     if G < 2:
         return
-    mb = handle(m, n, K, pos, snaps, devices=list(range(G)))
-    ins, angs, bins_all = [], [], []
-    for g in range(G):
-        d = torch.device("cuda", g)
-        ins.append(torch.from_numpy(np.ascontiguousarray(x[g::G]).view(np.float32)).to(d))
-        angs.append(torch.zeros((len(x[g::G]), n), dtype=torch.float32, device=d))
-        bins_all.append(torch.full((Wn, n), SENTINEL, dtype=torch.int32, device=d))
-    mb.process_device_sharded([t.data_ptr() for t in ins], Wn, [t.data_ptr() for t in angs], None, [t.data_ptr() for t in bins_all])
-    for g in range(G):
-        torch.cuda.synchronize(g)
-    for g in range(G):
-        assert np.array_equal(angs[g].cpu().numpy(), ref["angles"][g::G]), g
-        assert np.array_equal(bins_all[g].cpu().numpy(), ref["bins"]), g
-    mb.close()
+    for g, sh in enumerate(e["sharded"]):
+        assert np.array_equal(sh["angles"], ref["angles"][g::G]), g
+        assert np.array_equal(sh["bins"], ref["bins"]), g
 
 
 def test_launch_counts_and_sub_batches():
@@ -264,17 +150,17 @@ def test_launch_counts_and_sub_batches():
     x, _ = windows(pos, [(1, 20.0)], 3, snaps)
     for rule, spectrum, want in (("fixed", False, 3), ("mdl", False, 4), ("fixed", True, 4), ("mdl", True, 5)):
         blk = handle(m, n, K, pos, snaps, rule=rule)
-        _, launches = dev_call(blk, x, n, K, spectrum=spectrum)
+        _, launches = gh.device_call(blk, x, PEAKS + (("spectrum",) if spectrum else ()))
         assert launches == want, (rule, spectrum, launches)
         blk.close()
     # several sub-batches (the internal fp64 spectrum of K bins per window bounds one); the whole call equals its halves
     Kb, Wb, Nb = 36000, 3000, 64
     xb, _ = windows(pos, [(1, 20.0)] * Wb, 808, Nb)
     blk = handle(m, n, Kb, pos, Nb)
-    whole, launches = dev_call(blk, xb, n, Kb, spectrum=True)
+    whole, launches = gh.device_call(blk, xb, PEAKS + ("spectrum",))
     assert launches % 4 == 0 and launches // 4 >= 2, launches
-    first, _ = dev_call(blk, xb[: Wb // 2], n, Kb, spectrum=True)
-    second, _ = dev_call(blk, xb[Wb // 2:], n, Kb, spectrum=True)
+    first, _ = gh.device_call(blk, xb[: Wb // 2], PEAKS + ("spectrum",))
+    second, _ = gh.device_call(blk, xb[Wb // 2:], PEAKS + ("spectrum",))
     for k in ("angles", "levels", "bins", "spectrum"):
         assert np.array_equal(whole[k], np.concatenate([first[k], second[k]])), k
     blk.close()
@@ -286,13 +172,13 @@ def test_switching_back_to_top_bins():
     x = synth.gen_windows_numpy(cfg, 11, 0, 64)
     pos = ula(4, "x")
     fresh = handle(4, 1, cfg["resolution"], pos, cfg["snapshots"], mode="top_bins")
-    ref, l_ref = dev_call(fresh, x, 1, cfg["resolution"])
+    ref, l_ref = gh.device_call(fresh, x, PEAKS)
     fresh.close()
     blk = handle(4, 1, cfg["resolution"], pos, cfg["snapshots"])
-    _, l_roots = dev_call(blk, x, 1, cfg["resolution"])
+    _, l_roots = gh.device_call(blk, x, PEAKS)
     assert l_roots == 3
     blk.set_peak_mode("top_bins", 0)
-    got, l_top = dev_call(blk, x, 1, cfg["resolution"])
+    got, l_top = gh.device_call(blk, x, PEAKS)
     assert l_ref == l_top == 1
     assert all(np.array_equal(got[k], ref[k]) for k in ("angles", "levels", "bins"))
     blk.close()
@@ -304,17 +190,9 @@ def test_mirror_case():
     maximum rule spends its second slot on the mirror of the first)"""
     m, n, K, snaps, Wn = 4, 2, 3600, 4096, 100
     pos = ula(m, "x")
-    rng = np.random.default_rng(40)
-    xs = []
-    for _ in range(Wn):
-        X = (rng.standard_normal((m, snaps)) + 1j * rng.standard_normal((m, snaps))) / np.sqrt(2.0)
-        for t in (40.0, 110.0):
-            a = ro.steering(pos, LAM, math.radians(t))[0]
-            X += 10.0 * a[:, None] * (rng.standard_normal(snaps) + 1j * rng.standard_normal(snaps))[None, :] / np.sqrt(2.0)
-        xs.append(X.T.reshape(-1))
-    x = np.array(xs).astype(np.complex64)
+    x = two_source_windows(pos, (40.0, 110.0), 20.0, snaps, Wn, 40)
     blk = handle(m, n, K, pos, snaps)
-    out, _ = dev_call(blk, x, n, K)
+    out, _ = gh.device_call(blk, x, PEAKS)
     blk.close()
     got = np.sort(out["angles"], axis=1)
     assert np.all(np.abs(got[:, 0] - 40.0) < 1.0) and np.all(np.abs(got[:, 1] - 110.0) < 1.0), got
@@ -325,17 +203,9 @@ def test_resolution(m, th):
     """0 dB, 1024 snapshots: both sources within half their separation in at least 90 % of windows"""
     n, K, snaps, Wn = 2, 3600, 1024, 200
     pos = ula(m, "x")
-    rng = np.random.default_rng(7 * m)
-    xs = []
-    for _ in range(Wn):
-        X = (rng.standard_normal((m, snaps)) + 1j * rng.standard_normal((m, snaps))) / np.sqrt(2.0)
-        for t in th:
-            a = ro.steering(pos, LAM, math.radians(t))[0]
-            X += a[:, None] * (rng.standard_normal(snaps) + 1j * rng.standard_normal(snaps))[None, :] / np.sqrt(2.0)
-        xs.append(X.T.reshape(-1))
-    x = np.array(xs).astype(np.complex64)
+    x = two_source_windows(pos, th, 0.0, snaps, Wn, 7 * m)
     blk = handle(m, n, K, pos, snaps)
-    out, _ = dev_call(blk, x, n, K)
+    out, _ = gh.device_call(blk, x, PEAKS)
     blk.close()
     got = np.sort(out["angles"], axis=1)
     ok = np.all(np.abs(got - np.array(th)[None, :]) < (th[1] - th[0]) / 2.0, axis=1)
@@ -374,14 +244,14 @@ def test_invalid_combinations():
     for bad in (uca, bent, ula(m, "x") * 1.2):
         blk.set_array_geometry(bad, LAM)  # set_geometry() itself keeps its behaviour
         with pytest.raises(_capi.MusicB200Error):
-            dev_call(blk, x, n, K)
+            gh.device_call(blk, x, PEAKS)
         assert L.music_b200_set_peak_mode(blk._h, 2, 0) == EINVAL
         blk.set_array_geometry(pos, LAM)
         assert L.music_b200_set_peak_mode(blk._h, 2, 0) == _capi.OK
     # set_table() after set_peak_mode(ROOTS): the call fails, no fall-back to grid peaks
     blk.set_array_response(np.ones((K, m), np.complex64))
     with pytest.raises(_capi.MusicB200Error):
-        dev_call(blk, x, n, K)
+        gh.device_call(blk, x, PEAKS)
     ang = np.zeros((1, n), np.float32)
     with pytest.raises(_capi.MusicB200Error):
         blk.work(1, [x], [ang])
@@ -398,28 +268,14 @@ def test_invalid_combinations():
 
 def test_cpp_block():
     """the C++ block through set_peak_mode(2, 0) equals the Python block"""
-    exe = os.path.join(ROOT, "lib", "_build", "test_block_roots")
     m, n, K, snaps, Wn = 8, 2, 720, 256, 16
     pos = ula(m, "oblique")
     x, _ = windows(pos, [(2, 20.0)] * Wn, 77, snaps)
-    import tempfile
-    with tempfile.TemporaryDirectory() as td:
-        fin, fout = os.path.join(td, "in.bin"), os.path.join(td, "out.bin")
-        with open(fin, "wb") as f:
-            f.write(struct.pack("<6I", m, n, m * snaps, K, Wn, 1))
-            f.write(struct.pack("<d", LAM))
-            f.write(np.ascontiguousarray(pos, np.float64).tobytes())
-            f.write(x.view(np.float32).tobytes())
-        r = subprocess.run([exe, fin, fout], capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr
-        raw = open(fout, "rb").read()
-    o = 0
-    take = lambda cnt, dt: np.frombuffer(raw[o:o + 4 * cnt], dt)
-    ca = take(Wn * n, np.float32); o += 4 * Wn * n
-    cl = take(Wn * n, np.float32); o += 4 * Wn * n
-    cs = take(Wn * K, np.float32); o += 4 * Wn * K
-    cb = take(Wn * n, np.int32); o += 4 * Wn * n
-    cc = take(Wn, np.int32)
+    c = gh.run_cpp_block("test_block_roots", struct.pack("<6I", m, n, m * snaps, K, Wn, 1) + struct.pack("<d", LAM),
+                         [np.ascontiguousarray(pos, np.float64), x],
+                         [("a", np.float32, Wn * n), ("l", np.float32, Wn * n), ("s", np.float32, Wn * K),
+                          ("b", np.int32, Wn * n), ("c", np.int32, Wn)])
+    ca, cl, cs, cb, cc = c["a"], c["l"], c["s"], c["b"], c["c"]
     blk = handle(m, n, K, pos, snaps, rule="mdl")
     ang, lvl, spec = np.zeros((Wn, n), np.float32), np.zeros((Wn, n), np.float32), np.zeros((Wn, K), np.float32)
     blk.work(Wn, [x], [ang, lvl, spec])

@@ -4,55 +4,31 @@ Windows of one shape mix 0, 1, 2 and 3 sources (tests/source_count_oracle.py::mi
 counts equal the fp64 definition on LAPACK eigenvalues and on the GPU's own; bins and angles are bit-identical to the
 C oracle run at n = count, and to a FIXED handle created with n = count; levels and spectrum agree to 1e-5, and the
 slots at and beyond the count are exactly (0, 0, -1)."""
-import os
 import struct
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
-from gr_baz_b200 import _capi, build
+from gr_baz_b200 import _capi
 from gr_baz_b200.music_doa import music_doa
 from oracle import c_oracle as co
 from oracle import music_oracle as mo
 
+import gpu_harness as gh
 import helpers
 import source_count_oracle as so
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 P_RTOL = 1e-5
 MARGIN = 1e-6
-SENTINEL = -7
 K = 720
 NMAX = 3
 EXCL = 3
 SEED = 100
-
-
-def dev_call(blk, x, n, spectrum=False, counts=True, eigvals=False):
-    """process_device on every window of x; returns host arrays (and the launch count of the call)"""
-    dev = torch.device("cuda:0")
-    W = x.shape[0]
-    d_in = torch.from_numpy(x.view(np.float32)).to(dev)
-    o = {"angles": torch.full((W, n), SENTINEL, dtype=torch.float32, device=dev),
-         "levels": torch.full((W, n), SENTINEL, dtype=torch.float32, device=dev),
-         "bins": torch.full((W, n), SENTINEL, dtype=torch.int32, device=dev)}
-    if spectrum:
-        o["spectrum"] = torch.full((W, K), SENTINEL, dtype=torch.float32, device=dev)
-    if counts:
-        o["counts"] = torch.full((W,), SENTINEL, dtype=torch.int32, device=dev)
-    if eigvals:
-        o["eigvals"] = torch.full((W, blk.m), SENTINEL, dtype=torch.float64, device=dev)
-    p = lambda k: o[k].data_ptr() if k in o else None
-    l0 = blk.launch_count()
-    blk.process_device(d_in.data_ptr(), W, p("angles"), p("levels"), p("spectrum"), p("bins"),
-                       stream=torch.cuda.current_stream().cuda_stream, d_eigvals=p("eigvals"), d_counts=p("counts"))
-    torch.cuda.synchronize()
-    launches = blk.launch_count() - l0
-    return {k: v.cpu().numpy() for k, v in o.items()}, launches
+PEAKS = ("levels", "bins")
+COUNTS = PEAKS + ("counts",)
 
 
 def inv_norm2(table):
@@ -106,10 +82,10 @@ def test_counts_and_peaks_match_oracle(m, N, rule, peak, spectrum):
     if peak == "local":
         blk.set_peak_mode("local_maxima", EXCL)
     blk.set_source_rule(rule)
-    got, _ = dev_call(blk, x, NMAX, spectrum=spectrum)
+    got, _ = gh.device_call(blk, x, COUNTS + (("spectrum",) if spectrum else ()))
     check_against_oracles(got, x, m, N, table, rule, peak, NMAX, counts_ref, ctx)
     # the same definition applied to the GPU's own eigenvalues
-    internals, _ = dev_call(blk, x, NMAX, counts=False, eigvals=True)
+    internals, _ = gh.device_call(blk, x, PEAKS + ("eigvals",))
     gpu_counts = [so.estimate_source_count(internals["eigvals"][w], N, NMAX, rule)[0] for w in range(len(x))]
     assert np.array_equal(gpu_counts, counts_ref), ctx
     blk.close()
@@ -119,7 +95,7 @@ def test_counts_and_peaks_match_oracle(m, N, rule, peak, spectrum):
         fx = music_doa(m, d, m * N, table.tolist(), K)
         if peak == "local":
             fx.set_peak_mode("local_maxima", EXCL)
-        ref, _ = dev_call(fx, x[idx], d, spectrum=spectrum, counts=False)
+        ref, _ = gh.device_call(fx, x[idx], PEAKS + (("spectrum",) if spectrum else ()))
         fx.close()
         assert np.array_equal(got["bins"][idx, :d], ref["bins"]), (ctx, d)
         assert np.array_equal(got["angles"][idx, :d], ref["angles"]), (ctx, d)
@@ -137,7 +113,7 @@ def test_single_source_handle(m, spectrum):
     assert min(so.margin(e[1]) for e in est) > MARGIN and set(counts_ref.tolist()) == {0, 1}
     blk = music_doa(m, 1, m * N, table.tolist(), K)
     blk.set_source_rule("mdl")
-    got, launches = dev_call(blk, x, 1, spectrum=spectrum)
+    got, launches = gh.device_call(blk, x, COUNTS + (("spectrum",) if spectrum else ()))
     blk.close()
     assert launches == 4, launches  # covariance + eig + count + scan
     check_against_oracles(got, x, m, N, table, "mdl", "top", 1, counts_ref, (m, spectrum))
@@ -147,16 +123,16 @@ def test_launches_m4_peak_only_and_back_to_fixed():
     m, N = 4, 1024
     table, x, _ = so.mixed_windows(m, N, K, SEED, counts=(0, 1))
     blk = music_doa(m, 1, m * N, table.tolist(), K)
-    _, l_fixed = dev_call(blk, x, 1, counts=False)
+    _, l_fixed = gh.device_call(blk, x, PEAKS)
     assert l_fixed == 1  # the fused kernel
     blk.set_source_rule("mdl")
-    got, l_mdl = dev_call(blk, x, 1, counts=True)
+    got, l_mdl = gh.device_call(blk, x, COUNTS)
     assert l_mdl == 4  # cov4_tma + eig + source count + scan_peak1, no top-n
     assert np.array_equal(got["counts"], [0] * 3 + [1] * 3)
     blk.set_source_rule("fixed")
-    _, l_back = dev_call(blk, x, 1, counts=False)
+    _, l_back = gh.device_call(blk, x, PEAKS)
     assert l_back == 1
-    got, l_cnt = dev_call(blk, x, 1, counts=True)
+    got, l_cnt = gh.device_call(blk, x, COUNTS)
     assert np.all(got["counts"] == 1) and l_cnt == 2  # the fused kernel plus the fill of the counts
     blk.close()
 
@@ -180,8 +156,8 @@ def test_sub_batches_match_per_range_calls():
     d_in = torch.from_numpy(x.view(np.float32)).to(dev)
 
     def outs():
-        return [torch.full((W, n), SENTINEL, dtype=torch.float32, device=dev), torch.full((W, n), SENTINEL, dtype=torch.float32, device=dev),
-                torch.full((W, n), SENTINEL, dtype=torch.int32, device=dev), torch.full((W,), SENTINEL, dtype=torch.int32, device=dev)]
+        return [torch.full((W, n), gh.SENTINEL, dtype=torch.float32, device=dev), torch.full((W, n), gh.SENTINEL, dtype=torch.float32, device=dev),
+                torch.full((W, n), gh.SENTINEL, dtype=torch.int32, device=dev), torch.full((W,), gh.SENTINEL, dtype=torch.int32, device=dev)]
 
     def run(o, w0, nw):
         l0 = blk.launch_count()
@@ -231,7 +207,7 @@ def test_zero_and_nan_windows_have_no_sources():
     for rule in ("mdl", "aic"):
         blk = music_doa(m, NMAX, m * N, table.tolist(), K)
         blk.set_source_rule(rule)
-        got, _ = dev_call(blk, x, NMAX, spectrum=True)
+        got, _ = gh.device_call(blk, x, COUNTS + ("spectrum",))
         blk.close()
         assert got["counts"][0] == 0 and got["counts"][2] == 0, rule
         for w in (0, 2):
@@ -255,16 +231,14 @@ def test_host_device_multi_device_and_planar_entries():
     ang, lvl, bins, cnt = run_entries(blk, x, m, N)
     assert np.all(cnt == NMAX)  # FIXED: every count is n
     blk.set_source_rule("mdl")
-    dref, _ = dev_call(blk, x, NMAX)
+    dref, _ = gh.device_call(blk, x, COUNTS)
     ang, lvl, bins, cnt = run_entries(blk, x, m, N)
     assert np.array_equal(cnt, dref["counts"]) and np.array_equal(bins, dref["bins"]) and np.array_equal(ang, dref["angles"])
     assert np.array_equal(lvl.view(np.int32), dref["levels"].view(np.int32))
     assert set(cnt.tolist()) >= {0, 1, 2, 3}
     # planar streams honour the rule (no counts returned)
-    xs = x.reshape(W, N, m)
-    streams = [np.ascontiguousarray(xs[:, :, r].reshape(-1)) for r in range(m)]
     pa = np.zeros((W, NMAX), np.float32)
-    blk.work_planar(W, streams, [pa])
+    blk.work_planar(W, helpers.antenna_streams(x, m), [pa])
     assert np.array_equal(blk.last_bins(), dref["bins"]) and np.array_equal(pa, dref["angles"])
     blk.close()
     # multi-device handles: "0" and every GPU, windows dealt round-robin, counts in stream order
@@ -273,7 +247,7 @@ def test_host_device_multi_device_and_planar_entries():
         mb.set_source_rule("mdl")
         a2, l2, b2, c2 = run_entries(mb, x, m, N)
         assert np.array_equal(c2, dref["counts"]) and np.array_equal(b2, dref["bins"]) and np.array_equal(a2, dref["angles"]), devices
-        g, _ = dev_call(mb, x, NMAX)
+        g, _ = gh.device_call(mb, x, COUNTS)
         assert np.array_equal(g["counts"], dref["counts"]) and np.array_equal(g["bins"], dref["bins"]), devices
         mb.close()
 
@@ -299,28 +273,15 @@ def test_invalid_rules_are_rejected():
 
 
 @pytest.mark.parametrize("rule", [1, 2])
-def test_cpp_block_source_rule(tmp_path, rule):
-    build.build_cuda()
-    subprocess.check_call(["make", "-C", os.path.join(ROOT, "lib"), "-s"])
+def test_cpp_block_source_rule(rule):
     m, N = 8, 4096
     table, x, _ = so.mixed_windows(m, N, K, SEED + 8)
     W = x.shape[0]
-    fin, fout = tmp_path / "in.bin", tmp_path / "out.bin"
-    with open(fin, "wb") as f:
-        f.write(struct.pack("<5I", m, NMAX, m * N, K, W))
-        f.write(table.view(np.float32).tobytes())
-        f.write(table.view(np.float32).tobytes())
-        f.write(x.view(np.float32).tobytes())
-    r = subprocess.run([os.path.join(ROOT, "lib", "_build", "test_block"), str(fin), str(fout), str(rule)], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    raw = np.fromfile(fout, dtype=np.float32)
-    o = 0
-    ang = raw[o:o + W * NMAX].reshape(W, NMAX); o += W * NMAX
-    lvl = raw[o:o + W * NMAX].reshape(W, NMAX); o += W * NMAX
-    spec = raw[o:o + W * K].reshape(W, K); o += W * K
-    bins = raw[o:o + W * NMAX].view(np.int32).reshape(W, NMAX); o += W * NMAX
-    counts = raw[o:o + W].view(np.int32); o += W
-    assert o == raw.size
+    c = gh.run_cpp_block("test_block", struct.pack("<5I", m, NMAX, m * N, K, W), [table, table, x],
+                         [("a", np.float32, W * NMAX), ("l", np.float32, W * NMAX), ("s", np.float32, W * K),
+                          ("b", np.int32, W * NMAX), ("c", np.int32, W)], args=(rule,))
+    ang, lvl, spec = c["a"].reshape(W, NMAX), c["l"].reshape(W, NMAX), c["s"].reshape(W, K)
+    bins, counts = c["b"].reshape(W, NMAX), c["c"]
     name = {1: "mdl", 2: "aic"}[rule]
     ref = [so.estimate_source_count(np.linalg.eigvalsh(mo.covariance(x[w], m)), N, NMAX, name)[0] for w in range(W)]
     got = {"angles": ang, "levels": lvl, "spectrum": spec, "bins": bins, "counts": counts}

@@ -22,7 +22,6 @@ counts its passes: test_fused4_screen_on_scaled_and_calibrated_tables (scaling, 
 test_fused_kernels_at_table_edges (the screen's 192-row tiles and decimated subsample)."""
 import numpy as np
 import pytest
-import torch
 
 from gr_baz_b200.music_doa import music_doa
 from gr_baz_b200.music_doa_azel import music_doa_azel
@@ -31,11 +30,11 @@ from oracle import music_oracle as mo
 
 import azel_oracle as ao
 import estimator_oracle as eo
+import gpu_harness as gh
 import helpers
 
 pytestmark = pytest.mark.gpu
 
-SENTINEL = -7
 EXCL = 3        # exclusion_bins of the local-maxima paths
 P_RTOL = 1e-5
 K0 = 3600
@@ -70,56 +69,25 @@ PATHS = {
 }
 
 
-def make_handle(path, table, monkeypatch):
+def make_handle(path, table):
     m, n, N, _, o = PATHS[path]
-    with monkeypatch.context() as mp:
-        for k, v in o.get("env", {}).items():
-            mp.setenv(k, v)
-        blk = music_doa(m, n, N * m, table, table.shape[0])
-    if o.get("peak") == "local":
-        blk.set_peak_mode("local_maxima", EXCL)
-    if "est" in o:
-        blk.set_estimator(*o["est"])
-    if "rule" in o:
-        blk.set_source_rule(o["rule"])
-    return blk
+    return gh.make_block(m, n, N, table=table, est=o.get("est"), rule=o.get("rule"),
+                         mode="local_maxima" if o.get("peak") == "local" else None, excl=EXCL, env=o.get("env"))
 
 
 def call(blk, path, x, spectrum=None, p64=None):
     """the path's call on windows x; returns (outputs as numpy, kernel launches).  spectrum / p64 override the
     path's own choice of outputs (p64 = True: the unfused fp64 scan with P64 and R)."""
     m, n, N, _, o = PATHS[path]
-    K = blk.resolution
     spectrum = o.get("spectrum", False) if spectrum is None else spectrum
     p64 = o.get("p64", False) if p64 is None else p64
-    dev = torch.device("cuda:0")
-    W = x.shape[0]
-    out = {"angles": torch.full((W, n), SENTINEL, dtype=torch.float32, device=dev),
-           "levels": torch.full((W, n), SENTINEL, dtype=torch.float32, device=dev),
-           "bins": torch.full((W, n), SENTINEL, dtype=torch.int32, device=dev)}
-    if spectrum:
-        out["spectrum"] = torch.full((W, K), SENTINEL, dtype=torch.float32, device=dev)
-    if p64:
-        out["P64"] = torch.full((W, K), SENTINEL, dtype=torch.float64, device=dev)
-        out["R"] = torch.zeros((W, m, m, 2), dtype=torch.float64, device=dev)
-    p = lambda k: out[k].data_ptr() if k in out else None
-    stream = torch.cuda.current_stream().cuda_stream
-    l0 = blk.launch_count()
+    outs = ("levels", "bins") + (("spectrum",) if spectrum else ())
     if o.get("planar") and not p64:
-        xs = torch.from_numpy(np.ascontiguousarray(x.reshape(W, N, m).transpose(2, 0, 1).reshape(m, W * N))).to(dev)
-        blk.process_planar_device([xs[r].data_ptr() for r in range(m)], N, W, p("angles"), p("levels"), p("spectrum"),
-                                  p("bins"), stream=stream)
+        res, launches = gh.planar_device_call(blk, helpers.antenna_streams(x, m), N, x.shape[0], outs)
     else:
-        d_in = torch.from_numpy(x.view(np.float32)).to(dev)
-        blk.process_device(d_in.data_ptr(), W, p("angles"), p("levels"), p("spectrum"), p("bins"), stream=stream,
-                           d_P64=p("P64"), d_R=p("R"))
-    torch.cuda.synchronize()
-    launches = blk.launch_count() - l0
-    res = {k: v.cpu().numpy() for k, v in out.items()}
-    if "R" in res:
-        res["R"] = res["R"][..., 0] + 1j * res["R"][..., 1]
-    for k in ("angles", "levels", "bins") + (("spectrum",) if spectrum else ()):
-        assert not np.any(res[k] == SENTINEL), (path, k, "unwritten slot")
+        res, launches = gh.device_call(blk, x, outs + (("P64", "R") if p64 else ()))
+    for k in ("angles",) + outs:
+        assert not np.any(res[k] == gh.SENTINEL), (path, k, "unwritten slot")
     return res, launches
 
 
@@ -192,7 +160,7 @@ def test_power_of_two_table_scaling_is_exact(path, monkeypatch):
     m, n, N, _, o = PATHS[path]
     table = helpers.planar_table(m, K0, 10 + m)
     x = mixed_windows(table, N, 20 + m)
-    blk = make_handle(path, table, monkeypatch)
+    blk = make_handle(path, table)
     base = run_path(blk, path, x)
     bfull, _ = call(blk, path, x, spectrum=True, p64=True)
     P0 = bfull["P64"]
@@ -331,7 +299,7 @@ def test_calibrated_table_against_oracle(path, monkeypatch):
     rng = np.random.default_rng(32 + m)
     x = helpers.source_windows(rng, [[table[int(rng.integers(0, K0))] for _ in range(n)] if w % 4 else None
                                      for w in range(W0)], m, N)
-    blk = make_handle(path, table, monkeypatch)
+    blk = make_handle(path, table)
     check_against_oracle(blk, path, x, table, path)
     blk.close()
 
@@ -366,7 +334,7 @@ def test_duplicated_rows_tie_to_the_lowest_bin(path, monkeypatch):
     rule applied to the bit-equal strengths: the lowest bin for n = 1, the tied bins in ascending order with equal
     levels for n = 2, both maxima (lower first) for local maxima when they are farther apart than the exclusion"""
     m, n, N, _, o = PATHS[path]
-    blk = make_handle(path, helpers.planar_table(m, K0, 40 + m), monkeypatch)
+    blk = make_handle(path, helpers.planar_table(m, K0, 40 + m))
     rng = np.random.default_rng(50 + m)
     for rows, what in DUPLICATES:
         for src in (rows[0], rows[-1]):  # the lower row copied upwards, and the upper one downwards
@@ -404,7 +372,7 @@ def test_zero_rows(path, monkeypatch):
     m, n, N, _, o = PATHS[path]
     geo = helpers.planar_table(m, K0, 60 + m)
     x = mixed_windows(geo, N, 61 + m, W=4)
-    blk = make_handle(path, geo, monkeypatch)
+    blk = make_handle(path, geo)
     bartlett = o.get("est", ("",))[0] == "bartlett"
     for zeros in ((777,), (5, 1000, K0 - 1), (3, 4)):
         table = geo.copy()
@@ -485,7 +453,7 @@ def test_fused_kernels_at_table_edges(path, K, monkeypatch):
             x, got = x[:64], {k: v[:64] for k, v in got.items()}
         else:
             x = mixed_windows(table, N, 72 + K, W=16)
-            blk = make_handle(path, table, monkeypatch)
+            blk = make_handle(path, table)
             got = run_path(blk, path, x)
             blk.close()
         ref = co.work_batch(x, m, n, table)
@@ -499,7 +467,7 @@ def test_random_table_rough_spectrum(path, monkeypatch):
     m, n, N, _, _ = PATHS[path]
     table = helpers.random_table(m, K0, 80 + m)
     x = mixed_windows(table, N, 81 + m)
-    blk = make_handle(path, table, monkeypatch)
+    blk = make_handle(path, table)
     _, P = check_against_oracle(blk, path, x, table, path)
     blk.close()
     nmax = [int(np.sum((P[w] > np.roll(P[w], 1)) & (P[w] > np.roll(P[w], -1)))) for w in range(P.shape[0])]
@@ -517,18 +485,10 @@ def test_azel_random_table(peak):
     blk = music_doa_azel(m, n, m * snaps, grid.n_az, grid.n_el, (grid.el_lo, grid.el_hi), ao.uca_xyz(m, 1.0), 1.0)
     blk.set_array_response(table.reshape(grid.n_el, grid.n_az, m))
     blk.set_peak_mode("top_bins" if peak == "top" else "local_maxima", 2)
-    dev = torch.device("cuda:0")
-    d_in = torch.from_numpy(x.view(np.float32)).to(dev)
-    o = {k: torch.full((W, n), SENTINEL, dtype=torch.float32, device=dev) for k in ("az", "el", "lv")}
-    spec = torch.full((W, grid.K), SENTINEL, dtype=torch.float32, device=dev)
-    bins = torch.full((W, n), SENTINEL, dtype=torch.int32, device=dev)
-    l0 = blk.launch_count()
-    blk.process_device(d_in.data_ptr(), W, o["az"].data_ptr(), o["el"].data_ptr(), o["lv"].data_ptr(), spec.data_ptr(),
-                       bins.data_ptr(), stream=torch.cuda.current_stream().cuda_stream)
-    torch.cuda.synchronize()
-    assert blk.launch_count() - l0 == 5  # cov4_tma, eig, scan, top-n / 2-D local maxima, decode
+    o, launches = gh.device_call(blk, x, ("levels", "spectrum", "bins"))
+    assert launches == 5  # cov4_tma, eig, scan, top-n / 2-D local maxima, decode
     blk.close()
-    gb, gl, gs = bins.cpu().numpy(), o["lv"].cpu().numpy(), spec.cpu().numpy()
+    gb, gl, gs = o["bins"], o["levels"], o["spectrum"]
     for w in range(W):
         r = ao.work(x[w], m, n, table, grid, peak, 2)
         P = r["P"]

@@ -31,7 +31,7 @@ import torch  # noqa: E402
 
 import bench  # noqa: E402  (the workload and table of bench.py, unchanged)
 import dml_oracle as dm  # noqa: E402
-import test_dml_oracle as td  # noqa: E402
+import helpers  # noqa: E402
 from gr_baz_b200 import synth  # noqa: E402
 from gr_baz_b200.music_doa import music_doa  # noqa: E402
 
@@ -107,13 +107,13 @@ def run(cfg, W, variants, args, dev, stream):
 
 def coherent_uca16(dev):
     """resolved windows of a seeded coherent UCA 16 stream (two sources 20 degrees apart, 20 dB, 1024 snapshots)"""
-    W, m, n, snaps = 500, 16, 2, td.SNAPS
+    W, m, n, snaps = 500, 16, 2, helpers.SNAPS
     rng = np.random.default_rng(16)
     th = rng.uniform(0.0, 360.0, W)
     th = np.stack([th, (th + 20.0) % 360.0], axis=1)
-    pos = td.array("uca", m)
-    tab = td.table(pos)
-    x = td.source_windows(pos, th, True, W, 17)
+    pos = helpers.array_wl("uca", m)
+    tab = helpers.table_wl(pos)
+    x = helpers.angle_windows(pos, th, True, W, 17)
     res = {}
     for mode in ("dml", "local_maxima"):
         b = music_doa(m, n, m * snaps, tab, tab.shape[0])
@@ -122,7 +122,7 @@ def coherent_uca16(dev):
         b.work(W, [x], [ang, lvl])
         bins = b.last_bins()
         b.close()
-        res[mode] = int(sum(td.resolved([a for a, k in zip(ang[w], bins[w]) if k >= 0], th[w]) for w in range(W)))
+        res[mode] = int(sum(helpers.resolved([a for a, k in zip(ang[w], bins[w]) if k >= 0], th[w]) for w in range(W)))
     res["windows"] = W
     return res
 

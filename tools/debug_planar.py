@@ -6,7 +6,7 @@ from gr_baz_b200 import synth
 from gr_baz_b200.music_doa import music_doa
 from oracle import c_oracle as co
 import helpers
-from test_gpu_planar import streams_for, form_windows
+from helpers import streams_for, form_windows
 cfg = synth.config(2, snapshots=1024)
 N, hop, W = 1024, 512, 1500
 table = helpers.table_for(cfg)
