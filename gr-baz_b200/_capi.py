@@ -122,6 +122,18 @@ def load():
         L.music_b200_process_azel_host.restype = ctypes.c_int
         L.music_b200_process_azel_device.argtypes = [vp, fp, u32, fp, fp, fp, fp, fp, fp, vp]
         L.music_b200_process_azel_device.restype = ctypes.c_int
+        L.music_b200_create_channels.argtypes = [ctypes.POINTER(vp), u32, u32, u32, u32, u32, u32, u32, ctypes.c_int, ctypes.c_int, ctypes.c_int]
+        L.music_b200_create_channels.restype = ctypes.c_int
+        L.music_b200_set_geometry_channels.argtypes = [vp, fp, dbl, dbl]
+        L.music_b200_set_geometry_channels.restype = ctypes.c_int
+        L.music_b200_channel_frequencies.argtypes = [vp, fp]
+        L.music_b200_channel_frequencies.restype = ctypes.c_int
+        L.music_b200_get_table_channel.argtypes = [vp, u32, fp]
+        L.music_b200_get_table_channel.restype = ctypes.c_int
+        L.music_b200_process_channels_device.argtypes = [vp, fp, u32, fp, fp, fp, fp, fp, fp, vp]
+        L.music_b200_process_channels_device.restype = ctypes.c_int
+        L.music_b200_process_channels_host.argtypes = [vp, fp, u32, fp, fp, fp, fp, fp, fp]
+        L.music_b200_process_channels_host.restype = ctypes.c_int
         L.music_b200_launch_count.argtypes = [vp]
         L.music_b200_launch_count.restype = ctypes.c_uint64
         L.music_b200_set_stage_timing.argtypes = [vp, ctypes.c_int]
@@ -155,6 +167,8 @@ EXPORTS = [
     "music_b200_set_beamformer", "music_b200_process_device_beams", "music_b200_process_host_beams",
     "music_b200_set_calibration", "music_b200_get_calibration", "music_b200_calib_reset", "music_b200_calib_accumulate_device",
     "music_b200_calib_accumulate_host", "music_b200_calib_solve",
+    "music_b200_create_channels", "music_b200_set_geometry_channels", "music_b200_channel_frequencies",
+    "music_b200_get_table_channel", "music_b200_process_channels_device", "music_b200_process_channels_host",
 ]
 
 

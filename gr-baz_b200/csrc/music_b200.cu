@@ -37,6 +37,7 @@
 #include "music_dml.cuh"
 #include "music_beams.cuh"
 #include "music_calib.cuh"
+#include "music_channels.cuh"
 
 using namespace music;
 
@@ -179,6 +180,23 @@ struct music_b200 {
     unsigned steer_guarded = 0;    // entries of the last built table re-evaluated with the host libm
     bool azel = false;             // music_b200_create_azel(): K = n_az * n_el rows, elevation-major (music_azel.cuh)
     AzelGrid grid = {};
+    // channel handle (music_b200_create_channels, music_channels.cuh): the filter bank's shape, its twiddle and taper
+    // tables, and per table slot the C per-channel tables (views into one c64 and one soa allocation per slot; a table
+    // from set_table() sits in entry 0 and serves every channel)
+    bool chan = false;
+    ChanShape cshape = {};
+    int chan_taper = MUSIC_B200_TAPER_RECT, chan_combine = MUSIC_B200_CHANNELS_SEPARATE;
+    double2 *chan_tw = nullptr;
+    double *chan_taper_d = nullptr;
+    int chan_ctas = 1;             // resident CTAs of chan_cov_kernel per SM at this shape
+    std::vector<DeviceTable> ctab[2];
+    float *ctab_c64[2] = {nullptr, nullptr};
+    double *ctab_soa[2] = {nullptr, nullptr};
+    bool ctab_shared[2] = {false, false};
+    bool ctab_set = false;         // a table has been installed (create_channels() takes none)
+    double chan_fs = 0.0;          // sample rate of the last set_geometry_channels() (0: none yet)
+    unsigned char *chan_arena = nullptr;  // device staging of the channel host entry
+    size_t chan_arena_cap = 0;
 
     // fp64 workspace slots (R, eigenvalues, sorted eigenvectors, optional strengths) of the unfused path: one per
     // staging stream of the host entry points (slot 0 also serves the device entry points)
@@ -269,9 +287,8 @@ uint32_t table_tiles(uint32_t K) { return (uint32_t)((K + TILE - 1) / TILE); }
 size_t soa_doubles(uint32_t K, uint32_t M) { return (size_t)table_tiles(K) * (2 * M + 1) * TILE; }
 
 // derived layouts (fp64 SoA tiles, TF32 hi/lo MMA fragments) of the c64 table already in t.c64
-int finish_table(music_b200 *h, int slot, cudaStream_t st)
+int finish_table(music_b200 *h, DeviceTable &t, cudaStream_t st)
 {
-    DeviceTable &t = h->table[slot];
     const int ntiles = (int)table_tiles(h->K);
     prep_table_kernel<<<ntiles, TILE, 0, st>>>(reinterpret_cast<const float2 *>(t.c64), t.soa, (int)h->K, (int)h->m);
     h->launches++;
@@ -308,12 +325,12 @@ bool screen_bounds_table(const float *tab, uint32_t K)
     return true;
 }
 
-int upload_table(music_b200 *h, int slot, const float *table_c64, cudaStream_t st)
+int upload_table(music_b200 *h, DeviceTable &t, const float *table_c64, cudaStream_t st)
 {
-    h->table[slot].geometric = false;
-    h->table[slot].screen_ok = h->m != 4 || screen_bounds_table(table_c64, h->K);
-    CU(h, cudaMemcpyAsync(h->table[slot].c64, table_c64, (size_t)h->K * h->m * 2 * sizeof(float), cudaMemcpyHostToDevice, st));
-    return finish_table(h, slot, st);
+    t.geometric = false;
+    t.screen_ok = h->m != 4 || screen_bounds_table(table_c64, h->K);
+    CU(h, cudaMemcpyAsync(t.c64, table_c64, (size_t)h->K * h->m * 2 * sizeof(float), cudaMemcpyHostToDevice, st));
+    return finish_table(h, t, st);
 }
 
 // The root mode's ULA condition (include/music_b200.h) on positions [M][x, y]: s = (p_{M-1} - p_0) / (M - 1), |s| > 0,
@@ -336,6 +353,9 @@ UlaGeom ula_geometry(const double *pos, int M, double lambda)
 // The peak modes that take their angles from the ULA geometry instead of the table: ROOTS and ESPRIT
 bool gridless_ula(int peak) { return peak == MUSIC_B200_PEAKS_ROOTS || peak == MUSIC_B200_PEAKS_ESPRIT; }
 
+// The independent looks behind each covariance: the N snapshots of a window, on a channel handle its J segments.
+uint32_t snapshots(const music_b200 *h) { return h->chan ? (uint32_t)h->cshape.J : h->N; }
+
 // Whether handle h can run with modes p; if not, records why and returns EINVAL.  With a table t, also whether p can run
 // on it: the gridless ULA peak modes need a ULA geometry, the refinement a geometric table.  Tables are checked on handles that
 // hold one (single-device handles, and the children of a multi-device handle).
@@ -351,9 +371,18 @@ int check_modes(music_b200 *h, const Modes &p, const DeviceTable *t)
     if (!std::isfinite(p.loading) || p.loading < 0.0) return fail(h, MUSIC_B200_EINVAL, "loading must be finite and >= 0 (got %g)", p.loading);
     if (p.est != MUSIC_B200_ESTIMATOR_MVDR && p.loading != 0.0)
         return fail(h, MUSIC_B200_EINVAL, "diagonal loading applies to MVDR only (got %g)", p.loading);
-    if (p.est == MUSIC_B200_ESTIMATOR_MVDR && p.loading == 0.0 && h->N <= h->m)
+    if (p.est == MUSIC_B200_ESTIMATOR_MVDR && p.loading == 0.0 && snapshots(h) <= h->m)
         return fail(h, MUSIC_B200_EINVAL, "MVDR without diagonal loading needs more snapshots than antennas (N = %u, m = %u): R is singular",
-                    h->N, h->m);
+                    snapshots(h), h->m);
+    if (h->chan) {
+        // per channel only the grid modes are built (include/music_b200.h lists the rest as not built)
+        if (p.peak != MUSIC_B200_PEAKS_TOP_BINS && p.peak != MUSIC_B200_PEAKS_LOCAL_MAXIMA)
+            return fail(h, MUSIC_B200_EINVAL, "a channel handle takes the TOP_BINS and LOCAL_MAXIMA peak modes only (ROOTS, ESPRIT and DML "
+                                              "per channel are not built)");
+        if (p.refine != MUSIC_B200_REFINE_OFF) return fail(h, MUSIC_B200_EINVAL, "peak refinement is not built for channel handles");
+        if (h->chan_combine == MUSIC_B200_CHANNELS_INCOHERENT && p.est != MUSIC_B200_ESTIMATOR_MUSIC)
+            return fail(h, MUSIC_B200_EINVAL, "the INCOHERENT combine is defined for the MUSIC estimator only");
+    }
     if (gridless_ula(p.peak)) {
         const char *name = p.peak == MUSIC_B200_PEAKS_ROOTS ? "root" : "ESPRIT";
         if (p.excl != 0) return fail(h, MUSIC_B200_EINVAL, "the %s peak mode takes exclusion_bins = 0", name);
@@ -396,9 +425,8 @@ int for_each_child(music_b200 *h, F apply)
 
 // Steering table built on the device from the element positions (music_steer.cuh), then patched at the
 // few entries whose float32 rounding could depend on the libm in use.
-int build_table(music_b200 *h, int slot, const double *pos_xy, double lambda, cudaStream_t st)
+int build_table(music_b200 *h, DeviceTable &t, const double *pos_xy, double lambda, cudaStream_t st)
 {
-    DeviceTable &t = h->table[slot];
     const int K = (int)h->K, M = (int)h->m;
     t.geometric = false;
     t.screen_ok = true;  // unit-modulus rows: ||a||^2 = M
@@ -439,7 +467,7 @@ int build_table(music_b200 *h, int slot, const double *pos_xy, double lambda, cu
         CU(h, cudaGetLastError());
         CU(h, cudaStreamSynchronize(st));  // vals is a local
     }
-    const int rc = finish_table(h, slot, st);
+    const int rc = finish_table(h, t, st);
     if (rc) return rc;
     t.geometric = true;
     for (int i = 0; i < 2 * M; ++i) t.geo.pos[i] = pos_xy[i];
@@ -462,7 +490,7 @@ int build_table_azel(music_b200 *h, int slot, const double *pos_xyz, double lamb
     azel_table_kernel<<<(K * M + 255) / 256, 256, 0, st>>>(g, M, reinterpret_cast<float2 *>(t.c64));
     h->launches++;
     CU(h, cudaGetLastError());
-    const int rc = finish_table(h, slot, st);
+    const int rc = finish_table(h, t, st);
     if (rc) return rc;
     t.geometric = true;
     t.ageo = g;
@@ -517,6 +545,7 @@ struct Plan {
     bool beams = false;                              // beam weights (+ beams) after the peaks: the beams entry points
     bool calib = false;                              // correct R after the covariance (and the beam weights) by the calibration
     bool ws_p64 = false, ws_counts = false, ws_bins = false, ws_wts = false;  // workspace buffers the kernels write
+    bool combine = false;                            // channel handle, INCOHERENT: one spectrum per window from all channels
 };
 
 Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *planar, unsigned hop)
@@ -535,7 +564,7 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
     for (uint32_t r = 0; planar && r < h->m; ++r) planar_fusable = planar_fusable && (reinterpret_cast<uintptr_t>(planar->p[r]) & 15u) == 0;
     // A beams call needs R, which the fused kernels keep in registers: it runs the unfused plan of a call that asks for R.
     const bool beams = o.wts || o.beams;
-    const bool fusable = h->fused && !h->azel && music_est && fixed_n && md.refine == MUSIC_B200_REFINE_OFF &&
+    const bool fusable = h->fused && !h->chan && !h->azel && music_est && fixed_n && md.refine == MUSIC_B200_REFINE_OFF &&
                          md.peak == MUSIC_B200_PEAKS_TOP_BINS && h->n == 1 && !o.P64 && !o.R && !o.ev && !beams && !h->calib;
     if (fusable && h->m == 4 && planar_fusable && (!o.spec || h->fused_spec)) p.path = Path::Fused4;
     else if (fusable && h->m == 8 && !planar && !o.spec && h->N >= 128 && h->N % 2 == 0) p.path = Path::Fused8;
@@ -569,6 +598,16 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
     p.calib = h->calib;
     p.ws_bins = p.decode || p.refine || (beams && !o.bins);
     p.ws_wts = beams && !o.wts;
+    if (h->chan && h->chan_combine == MUSIC_B200_CHANNELS_INCOHERENT) {
+        // every channel's scan writes its fp64 strengths into the workspace; the combine kernel writes the spectrum and
+        // the peak rule (also for n = 1) reads the combined strengths
+        p.combine = true;
+        p.scan = Scan::Grid;
+        p.argmax = false;
+        p.p64 = p.ws_p64 = true;
+        p.spec = false;
+        p.peaks = local ? Peaks::Local : Peaks::TopN;
+    }
     return p;
 }
 
@@ -578,7 +617,8 @@ uint32_t max_sub_windows(const music_b200 *h, const Plan &p)
     const size_t per_win = (size_t)h->m * h->m * 2 * 8 * 2 + h->m * 8 + (p.ws_p64 ? (size_t)h->K * 8 : 0) +
                            (p.ws_counts ? sizeof(int32_t) : 0) + (p.ws_bins ? h->n * sizeof(int32_t) : 0) +
                            (p.ws_wts ? (size_t)h->n * h->m * 2 * sizeof(double) : 0);
-    size_t c = ((size_t)384 << 20) / per_win;
+    // a channel handle's workspace holds C pseudo-windows per window
+    size_t c = ((size_t)384 << 20) / (per_win * (h->chan ? (size_t)h->cshape.C : 1));
     c = std::max<size_t>(SCAN_B, std::min<size_t>(c, 1u << 20));
     return (uint32_t)(c / SCAN_B * SCAN_B);
 }
@@ -671,14 +711,14 @@ void with_scan_form(const Plan &p, const int32_t *cnt, F f)
     else f(ScanForm<EST_MUSIC, false>());
 }
 
-// K3, the grid scan of W windows the plan chose, into the outputs o of these windows.  cnt: the per-window source counts
-// (NULL under the FIXED rule).  scan_kernel stages per window the eigenvectors (MUSIC), the g_j of mvdr_prep_kernel
+// K3, the grid scan of W windows the plan chose against table tb, into the outputs o of these windows.  cnt: the
+// per-window source counts (NULL under the FIXED rule).  scan_kernel stages per window the eigenvectors (MUSIC), the g_j of mvdr_prep_kernel
 // (MVDR) or R (Bartlett).
 void launch_scan(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t W, const Outputs &o, const PeakOut &po,
-                 const int32_t *cnt, cudaStream_t st)
+                 const int32_t *cnt, const DeviceTable &tb, cudaStream_t st)
 {
     if (p.scan == Scan::None) return;
-    const double *soa = h->table[h->cur_table].soa;
+    const double *soa = tb.soa;
     const double *V = p.est == MUSIC_B200_ESTIMATOR_BARTLETT ? ws.R : ws.Vt;
     float *d_spec = o.spec;
     double *d_p64 = o.P64 ? o.P64 : ws.P64;
@@ -866,18 +906,12 @@ void launch_beams(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t W,
     h->launches++;
 }
 
-// K2 (+ source count) + K3 (+ peak rule) of W windows from ws.R into the outputs o (of these W windows), on `st`, as
-// planned.  tev (optional) = timing events [1..4].  An az-el handle's peak bins are decoded into (azimuth, elevation)
-// after the peak rule.  With refinement on, the refine kernel follows (timed with the peak rule) and reads the bins
-// written before it: from the caller's array, or from the workspace when the caller asked for none.  A beams call
-// then forms the weights and beams of the windows at d_in (timed with the peak rule as well).
-int launch_eig_scan(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t W, const Outputs &o, cudaStream_t st, cudaEvent_t *tev,
-                    const float *d_in = nullptr)
+// K2 of W windows from ws.R as planned: the eigensolver, the source count from `nsnap` snapshots (into ws.cnt and, when
+// given, counts_out) and the MVDR preparation.  Returns the per-window counts the later stages read (NULL under FIXED).
+const int32_t *launch_eig_stage(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t W, int32_t *counts_out, uint32_t nsnap,
+                                cudaStream_t st)
 {
     const int M = (int)h->m;
-    const DeviceTable &tb = h->table[h->cur_table];
-    PeakOut po = make_peak_out(o);
-    if (p.ws_bins && !po.bins) po.bins = ws.bins;
     if (p.eig) {
         const int grid = (W + 127) / 128;
         switch (M) {
@@ -895,7 +929,7 @@ int launch_eig_scan(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t 
     // per-window model order from the eigenvalues just written (timed with the eigensolver)
     const int32_t *cnt = nullptr;
     if (p.count) {
-        source_count_kernel<<<(W + 127) / 128, 128, 0, st>>>(ws.ev, M, (int)h->n, (int)h->N, h->source_rule, (int)W, ws.cnt, o.counts);
+        source_count_kernel<<<(W + 127) / 128, 128, 0, st>>>(ws.ev, M, (int)h->n, (int)nsnap, h->source_rule, (int)W, ws.cnt, counts_out);
         h->launches++;
         cnt = ws.cnt;
     }
@@ -904,8 +938,31 @@ int launch_eig_scan(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t 
         mvdr_prep_kernel<<<(W + PREP_WARPS - 1) / PREP_WARPS, PREP_WARPS * 32, 0, st>>>(ws.R, ws.Vt, M, (int)W, h->modes.loading);
         h->launches++;
     }
+    return cnt;
+}
+
+// The 1-D grid peak rules (TopN, Local) of W windows on the fp64 strengths p64
+void launch_grid_peaks(music_b200 *h, Peaks peaks, const double *p64, uint32_t W, const PeakOut &po, const int32_t *cnt, cudaStream_t st)
+{
+    if (peaks == Peaks::Local) topn_local_kernel<<<(W + 7) / 8, 256, 0, st>>>(p64, (int)h->n, (int)h->K, (int)W, (int)h->modes.excl, po, cnt);
+    else topn_kernel<<<(W + 7) / 8, 256, 0, st>>>(p64, (int)h->n, (int)h->K, (int)W, po, cnt);
+}
+
+// K2 (+ source count) + K3 (+ peak rule) of W windows from ws.R into the outputs o (of these W windows), on `st`, as
+// planned.  tev (optional) = timing events [1..4].  An az-el handle's peak bins are decoded into (azimuth, elevation)
+// after the peak rule.  With refinement on, the refine kernel follows (timed with the peak rule) and reads the bins
+// written before it: from the caller's array, or from the workspace when the caller asked for none.  A beams call
+// then forms the weights and beams of the windows at d_in (timed with the peak rule as well).
+int launch_eig_scan(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t W, const Outputs &o, cudaStream_t st, cudaEvent_t *tev,
+                    const float *d_in = nullptr)
+{
+    const int M = (int)h->m;
+    const DeviceTable &tb = h->table[h->cur_table];
+    PeakOut po = make_peak_out(o);
+    if (p.ws_bins && !po.bins) po.bins = ws.bins;
+    const int32_t *cnt = launch_eig_stage(h, p, ws, W, o.counts, h->N, st);
     if (tev) cudaEventRecord(tev[2], st);
-    launch_scan(h, p, ws, W, o, po, cnt, st);
+    launch_scan(h, p, ws, W, o, po, cnt, tb, st);
     double *p64 = o.P64 ? o.P64 : ws.P64;  // what the peak rules read
     if (tev) cudaEventRecord(tev[3], st);
     const int excl = (int)h->modes.excl;
@@ -926,8 +983,8 @@ int launch_eig_scan(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t 
         });
         break;
     case Peaks::Local2D: topn_local2d_kernel<<<W, AZEL_LM_THREADS, 0, st>>>(p64, (int)h->n, h->grid.n_az, h->grid.n_el, excl, po, cnt); break;
-    case Peaks::Local: topn_local_kernel<<<(W + 7) / 8, 256, 0, st>>>(p64, (int)h->n, (int)h->K, (int)W, excl, po, cnt); break;
-    case Peaks::TopN: topn_kernel<<<(W + 7) / 8, 256, 0, st>>>(p64, (int)h->n, (int)h->K, (int)W, po, cnt); break;
+    case Peaks::Local:
+    case Peaks::TopN: launch_grid_peaks(h, p.peaks, p64, W, po, cnt, st); break;
     case Peaks::None: break;
     }
     if (p.peaks != Peaks::None) h->launches++;
@@ -1087,6 +1144,89 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, const Ou
     if (gf.epoch) {
         gather_signal_kernel<<<1, 32, 0, st>>>(gf, out.gather.G, out.gather.rank);
         h->launches++;
+    }
+    return MUSIC_B200_OK;
+}
+
+// the table channel c of a channel handle scans with
+const DeviceTable &channel_table(const music_b200 *h, int c) { return h->ctab[h->cur_table][h->ctab_shared[h->cur_table] ? 0 : c]; }
+
+// A channel handle's call (music_channels.cuh): `nwindows` windows on `st` in sub-batches through workspace slot 0, which
+// holds a sub-batch of W windows as C * W pseudo-windows, channel-major [C][W].  The filter bank writes every channel's
+// R in one launch; eigensolver, source count (from the J segments) and MVDR preparation run once over all C * W
+// pseudo-windows; scan and peak rule run once per channel on that channel's contiguous run, with that channel's table,
+// straight into the channel's block of the caller's channel-major outputs `out` ([C][nwindows] rows under SEPARATE,
+// [nwindows] rows under INCOHERENT).  R_out (may be NULL): [C][nwindows][m][m] complex fp64.
+int enqueue_channels(music_b200 *h, const float *d_in, uint32_t nwindows, const Outputs &out, double *R_out, cudaStream_t st)
+{
+    if (nwindows == 0) return MUSIC_B200_OK;
+    if (!d_in || !out.angles) return fail(h, MUSIC_B200_EINVAL, "d_in_c64 and d_angles must not be NULL");
+    if ((reinterpret_cast<uintptr_t>(d_in) & 15u) != 0) return fail(h, MUSIC_B200_EINVAL, "d_in_c64 must be 16-byte aligned");
+    if (!h->ctab_set) return fail(h, MUSIC_B200_EINVAL, "no array response yet: call music_b200_set_geometry_channels() or music_b200_set_table()");
+    if (const int rc = check_modes(h, h->modes, nullptr)) return rc;
+    const bool separate = h->chan_combine == MUSIC_B200_CHANNELS_SEPARATE;
+    if (!separate && out.counts) return fail(h, MUSIC_B200_EINVAL, "the INCOHERENT combine reports no counts: counts must be NULL");
+    const ChanShape &cs = h->cshape;
+    const uint32_t C = (uint32_t)cs.C;
+    if (h->source_rule == MUSIC_B200_SOURCES_FIXED && out.counts) {
+        const size_t e = (size_t)C * nwindows;
+        fill_counts_kernel<<<(unsigned)((e + 255) / 256), 256, 0, st>>>(out.counts, (int)h->n, (int)e);
+        h->launches++;
+        CU(h, cudaGetLastError());
+    }
+    const Plan plan = plan_call(h, out, nullptr, 0);
+    const uint32_t sub = std::min((nwindows + SCAN_B - 1) / SCAN_B * SCAN_B, max_sub_windows(h, plan));
+    Workspace &ws = h->ws[0];
+    if (const int rc = ensure_slot(h, ws, sub * C, plan)) return rc;
+    if (ws.used) CU(h, cudaStreamWaitEvent(st, ws.scan_done, 0));
+    const size_t mm2 = (size_t)h->m * h->m * 2, K = h->K;
+    const size_t smem = chan_smem(cs.M, cs.F, cs.B, cs.Cg).total;
+    for (uint32_t w0 = 0; w0 < nwindows; w0 += sub) {
+        const uint32_t W = std::min(sub, nwindows - w0);
+        cudaEvent_t *tev = timing_events(h);
+        if (tev) cudaEventRecord(tev[0], st);
+        const int grid = (int)std::min<uint32_t>(W, (uint32_t)(h->sm_count * h->chan_ctas));
+        chan_cov_kernel<<<grid, CHAN_THREADS, smem, st>>>(d_in + (size_t)w0 * h->nsamples * 2, ws.R, (int)W, cs, h->chan_tw, h->chan_taper_d);
+        h->launches++;
+        if (tev) cudaEventRecord(tev[1], st);
+        const int32_t *cnt = launch_eig_stage(h, plan, ws, C * W, nullptr, (uint32_t)cs.J, st);
+        if (cnt && out.counts)
+            CU(h, cudaMemcpy2DAsync(out.counts + w0, (size_t)nwindows * sizeof(int32_t), cnt, (size_t)W * sizeof(int32_t), (size_t)W * sizeof(int32_t), C,
+                                    cudaMemcpyDeviceToDevice, st));
+        if (tev) cudaEventRecord(tev[2], st);
+        // channel c's run of the workspace, and its block of the outputs from window w0 on
+        const auto run = [&](uint32_t c) {
+            Workspace v = ws;
+            v.R += (size_t)c * W * mm2;
+            v.Vt += (size_t)c * W * mm2;
+            if (v.P64) v.P64 += (size_t)c * W * K;
+            return v;
+        };
+        const auto block = [&](uint32_t c) { return separate ? out.at((size_t)c * nwindows + w0) : Outputs().shaped(h); };
+        for (uint32_t c = 0; c < C; ++c) {
+            const Outputs o = block(c);
+            launch_scan(h, plan, run(c), W, o, make_peak_out(o), cnt ? cnt + (size_t)c * W : nullptr, channel_table(h, (int)c), st);
+        }
+        if (tev) cudaEventRecord(tev[3], st);
+        if (plan.combine) {
+            const size_t WK = (size_t)W * K;
+            chan_combine_kernel<<<(unsigned)((WK + 255) / 256), 256, 0, st>>>(ws.P64, (int)C, WK, out.spec ? out.spec + (size_t)w0 * K : nullptr);
+            launch_grid_peaks(h, plan.peaks, ws.P64, W, make_peak_out(out.at(w0)), nullptr, st);
+            h->launches += 2;
+        } else if (plan.peaks != Peaks::None) {
+            for (uint32_t c = 0; c < C; ++c) {
+                const Outputs o = block(c);
+                launch_grid_peaks(h, plan.peaks, o.P64 ? o.P64 : run(c).P64, W, make_peak_out(o), cnt ? cnt + (size_t)c * W : nullptr, st);
+                h->launches++;
+            }
+        }
+        if (tev) cudaEventRecord(tev[4], st);
+        if (R_out)
+            CU(h, cudaMemcpy2DAsync(R_out + (size_t)w0 * mm2, (size_t)nwindows * mm2 * sizeof(double), ws.R, (size_t)W * mm2 * sizeof(double),
+                                    (size_t)W * mm2 * sizeof(double), C, cudaMemcpyDeviceToDevice, st));
+        CU(h, cudaGetLastError());
+        CU(h, cudaEventRecord(ws.scan_done, st));
+        ws.used = true;
     }
     return MUSIC_B200_OK;
 }
@@ -1380,8 +1520,44 @@ int stage_host(music_b200 *h, const HostInput &in, uint32_t nwindows, const Outp
 
 // The device part of create() / create_azel(), after their argument checks: device checks, buffers, the first table
 // (uploaded, or for an az-el handle (azel != NULL) built from its element positions, wavelength and grid).
+// The filter bank of a channel handle: twiddles and taper on the device, the group split, the kernel's shared memory.
+int init_channels(music_b200 *h)
+{
+    ChanShape &cs = h->cshape;
+    std::vector<double2> tw(cs.F / 2);
+    std::vector<double> taper(cs.F);
+    cs.denom = (double)cs.J * chan_tables_host(cs.F, h->chan_taper, tw.data(), taper.data());
+    cs.B = chan_batch(cs.M, cs.F, cs.J);
+    cs.Cg = chan_group_size(cs.M, cs.F, cs.B, cs.C);
+    cs.groups = (cs.C + cs.Cg - 1) / cs.Cg;
+    CU(h, cudaMalloc(&h->chan_tw, tw.size() * sizeof(double2)));
+    CU(h, cudaMalloc(&h->chan_taper_d, taper.size() * sizeof(double)));
+    CU(h, cudaMemcpy(h->chan_tw, tw.data(), tw.size() * sizeof(double2), cudaMemcpyHostToDevice));
+    CU(h, cudaMemcpy(h->chan_taper_d, taper.data(), taper.size() * sizeof(double), cudaMemcpyHostToDevice));
+    const size_t smem = chan_smem(cs.M, cs.F, cs.B, cs.Cg).total;
+    CU(h, cudaFuncSetAttribute(chan_cov_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CHAN_SMEM_MAX));
+    CU(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&h->chan_ctas, chan_cov_kernel, CHAN_THREADS, smem));
+    if (h->chan_ctas < 1) return fail(h, MUSIC_B200_ECUDA, "chan_cov_kernel does not fit an SM with %zu bytes of shared memory", smem);
+    return MUSIC_B200_OK;
+}
+
+// the per-channel tables of slot `slot` (allocated the first time the slot is filled)
+int ensure_channel_tables(music_b200 *h, int slot)
+{
+    if (!h->ctab[slot].empty()) return MUSIC_B200_OK;
+    const size_t C = (size_t)h->cshape.C, c64 = (size_t)h->K * h->m * 2, soa = soa_doubles(h->K, h->m);
+    CU(h, cudaMalloc(&h->ctab_c64[slot], C * c64 * sizeof(float)));
+    CU(h, cudaMalloc(&h->ctab_soa[slot], C * soa * sizeof(double)));
+    h->ctab[slot].resize(C);
+    for (size_t c = 0; c < C; ++c) {
+        h->ctab[slot][c].c64 = h->ctab_c64[slot] + c * c64;
+        h->ctab[slot][c].soa = h->ctab_soa[slot] + c * soa;
+    }
+    return MUSIC_B200_OK;
+}
+
 int create_on_device(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples, uint32_t resolution, const float *table_c64,
-                     int device, const AzelGeom *azel)
+                     int device, const AzelGeom *azel, const music_b200 *chan = nullptr)
 {
     int ndev = 0;
     cudaError_t e = cudaGetDeviceCount(&ndev);
@@ -1402,6 +1578,12 @@ int create_on_device(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples
         h->azel = true;
         h->grid = azel->grid;
     }
+    if (chan) {  // the channel settings create_channels() checked
+        h->chan = true;
+        h->cshape = chan->cshape;
+        h->chan_taper = chan->chan_taper;
+        h->chan_combine = chan->chan_combine;
+    }
 
     int rc = MUSIC_B200_OK;
     auto init = [&]() -> int {
@@ -1409,6 +1591,7 @@ int create_on_device(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples
         for (int i = 0; i < 2; ++i) {
             CU(h, cudaStreamCreateWithFlags(&h->streams[i], cudaStreamNonBlocking));
             CU(h, cudaEventCreateWithFlags(&h->ws[i].scan_done, cudaEventDisableTiming));
+            if (chan) continue;  // a channel handle's tables are per channel (ensure_channel_tables)
             CU(h, cudaMalloc(&h->table[i].c64, (size_t)resolution * m * 2 * sizeof(float)));
             CU(h, cudaMalloc(&h->table[i].soa, soa_doubles(resolution, m) * sizeof(double)));
             if (m == 4 && !azel) {  // the fused M = 4 kernel's screen layout; an az-el handle never runs that kernel
@@ -1443,7 +1626,8 @@ int create_on_device(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples
             CU(h, cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
         }
         CU(h, cudaFuncSetAttribute(cov4_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)COV_SMEM));
-        return azel ? build_table_azel(h, 0, azel->pos, azel->lambda, h->streams[0]) : upload_table(h, 0, table_c64, h->streams[0]);
+        if (chan) return init_channels(h);
+        return azel ? build_table_azel(h, 0, azel->pos, azel->lambda, h->streams[0]) : upload_table(h, h->table[0], table_c64, h->streams[0]);
     };
     rc = init();
     if (rc != MUSIC_B200_OK) {
@@ -1564,12 +1748,23 @@ int music_b200_set_table(music_b200 *h, const float *table_c64)
     if (!h->kids.empty())  // multi-device handle: every device holds a full copy of the table (SURVEY.md section 8e)
         return for_each_child(h, [&](music_b200 *c) { return music_b200_set_table(c, table_c64); });
     CU(h, cudaSetDevice(h->device));
+    if (h->chan) {
+        // one measured table for every channel (the narrowband assumption): entry 0 of the idle slot
+        CU(h, cudaDeviceSynchronize());
+        const int slot = h->cur_table ^ 1;
+        if (const int rc = ensure_channel_tables(h, slot)) return rc;
+        if (const int rc = upload_table(h, h->ctab[slot][0], table_c64, h->streams[0])) return rc;
+        h->ctab_shared[slot] = true;
+        h->cur_table = slot;
+        h->ctab_set = true;
+        return MUSIC_B200_OK;
+    }
     // Work enqueued by earlier process_device() calls may still be reading the current slot on
     // a caller stream; fill the other slot and flip.  (The slot being overwritten was retired
     // two set_table() calls ago; synchronise the device once to be safe - retunes are rare.)
     CU(h, cudaDeviceSynchronize());
     const int slot = h->cur_table ^ 1;
-    int rc = upload_table(h, slot, table_c64, h->streams[0]);
+    int rc = upload_table(h, h->table[slot], table_c64, h->streams[0]);
     if (rc) return rc;
     h->cur_table = slot;
     return MUSIC_B200_OK;
@@ -1581,6 +1776,7 @@ int music_b200_process_planar_device(music_b200 *h, const float *const *d_stream
     h = served(h);
     if (!h) return MUSIC_B200_EINVAL;
     if (h->azel) return fail(h, MUSIC_B200_EINVAL, "planar input is not supported on an az-el handle");
+    if (h->chan) return fail(h, MUSIC_B200_EINVAL, "planar input is not built for channel handles");
     if (nwindows == 0) return MUSIC_B200_OK;
     if (!d_streams) return fail(h, MUSIC_B200_EINVAL, "d_streams must not be NULL");
     if (hop == 0) return fail(h, MUSIC_B200_EINVAL, "hop must be >= 1 snapshot");
@@ -1602,6 +1798,7 @@ int music_b200_process_planar_host(music_b200 *h, const float *const *streams, u
     h = served(h);
     if (!h) return MUSIC_B200_EINVAL;
     if (h->azel) return fail(h, MUSIC_B200_EINVAL, "planar input is not supported on an az-el handle");
+    if (h->chan) return fail(h, MUSIC_B200_EINVAL, "planar input is not built for channel handles");
     if (nwindows == 0) return MUSIC_B200_OK;
     if (!streams || !angles) return fail(h, MUSIC_B200_EINVAL, "streams and angles must not be NULL");
     if (hop == 0) return fail(h, MUSIC_B200_EINVAL, "hop must be >= 1 snapshot");
@@ -1728,6 +1925,7 @@ int music_b200_set_geometry(music_b200 *h, const double *positions_xy, double wa
 {
     if (!h) return MUSIC_B200_EINVAL;
     if (h->azel) return fail(h, MUSIC_B200_EINVAL, "an az-el handle takes music_b200_set_geometry_azel()");
+    if (h->chan) return fail(h, MUSIC_B200_EINVAL, "a channel handle takes music_b200_set_geometry_channels()");
     if (!positions_xy) return fail(h, MUSIC_B200_EINVAL, "element positions must not be NULL");
     if (!(wavelength > 0.0) || !std::isfinite(wavelength)) return fail(h, MUSIC_B200_EINVAL, "wavelength must be positive and finite");
     for (uint32_t i = 0; i < 2 * h->m; ++i)
@@ -1738,7 +1936,7 @@ int music_b200_set_geometry(music_b200 *h, const double *positions_xy, double wa
     CU(h, cudaSetDevice(h->device));
     CU(h, cudaDeviceSynchronize());  // as in set_table(): the slot being rebuilt must be idle
     const int slot = h->cur_table ^ 1;
-    int rc = build_table(h, slot, positions_xy, wavelength, h->streams[0]);
+    int rc = build_table(h, h->table[slot], positions_xy, wavelength, h->streams[0]);
     if (rc) return rc;
     h->cur_table = slot;
     if (guarded) *guarded = h->steer_guarded;
@@ -1755,6 +1953,7 @@ int music_b200_get_table(music_b200 *h, float *table_c64)
 {
     if (!h) return MUSIC_B200_EINVAL;
     if (!table_c64) return fail(h, MUSIC_B200_EINVAL, "output table must not be NULL");
+    if (h->chan) return fail(h, MUSIC_B200_EINVAL, "a channel handle has one table per channel: music_b200_get_table_channel()");
     h = served(h);
     std::lock_guard<std::mutex> g(h->mutex);
     CU(h, cudaSetDevice(h->device));
@@ -1786,6 +1985,7 @@ int process_device_impl(music_b200 *h, const float *d_in_c64, uint32_t nwindows,
         return fail(h, MUSIC_B200_EINVAL, "d_in_c64 lives on device %d, which this handle does not own", at.device);
     }
     if (h->azel) return fail(h, MUSIC_B200_EINVAL, "an az-el handle takes music_b200_process_azel_device()");
+    if (h->chan) return fail(h, MUSIC_B200_EINVAL, "a channel handle takes music_b200_process_channels_device()");
     std::lock_guard<std::mutex> g(h->mutex);
     NvtxRange range("music_b200_process_device");
     CU(h, cudaSetDevice(h->device));
@@ -1801,6 +2001,7 @@ int process_host_impl(music_b200 *h, const float *in_c64, uint32_t nwindows, Out
 {
     if (!h) return MUSIC_B200_EINVAL;
     if (h->azel && !dst.elev) return fail(h, MUSIC_B200_EINVAL, "an az-el handle takes music_b200_process_azel_host()");
+    if (h->chan) return fail(h, MUSIC_B200_EINVAL, "a channel handle takes music_b200_process_channels_host()");
     if (nwindows == 0) return MUSIC_B200_OK;
     if (!in_c64 || !dst.angles) return fail(h, MUSIC_B200_EINVAL, "in_c64 and angles must not be NULL");
     std::lock_guard<std::mutex> g(h->mutex);
@@ -1882,6 +2083,7 @@ int music_b200_set_beamformer(music_b200 *h, int rule, double loading)
 {
     if (!h) return MUSIC_B200_EINVAL;
     if (h->azel) return fail(h, MUSIC_B200_EINVAL, "the beamformer is not supported on an az-el handle");
+    if (h->chan) return fail(h, MUSIC_B200_EINVAL, "wideband beams are not built: a channel handle takes no beamformer");
     if (rule != MUSIC_B200_BEAMS_OFF && rule != MUSIC_B200_BEAMS_DAS && rule != MUSIC_B200_BEAMS_MVDR && rule != MUSIC_B200_BEAMS_LCMV)
         return fail(h, MUSIC_B200_EINVAL, "unknown beamformer %d", rule);
     if (!std::isfinite(loading) || loading < 0.0) return fail(h, MUSIC_B200_EINVAL, "loading must be finite and >= 0 (got %g)", loading);
@@ -1925,6 +2127,7 @@ int music_b200_process_host_beams(music_b200 *h, const float *in_c64, uint32_t n
 int music_b200_set_calibration(music_b200 *h, const double *gains)
 {
     if (!h) return MUSIC_B200_EINVAL;
+    if (h->chan) return fail(h, MUSIC_B200_EINVAL, "per-channel calibration is not built: a channel handle takes no calibration");
     CalibVec cv = {};
     if (gains) {
         for (uint32_t m = 0; m < h->m; ++m) {
@@ -2007,6 +2210,7 @@ int music_b200_calib_reset(music_b200 *h)
 {
     h = served(h);
     if (!h) return MUSIC_B200_EINVAL;
+    if (h->chan) return fail(h, MUSIC_B200_EINVAL, "per-channel calibration is not built: a channel handle takes no calibration");
     std::lock_guard<std::mutex> g(h->mutex);
     CU(h, cudaSetDevice(h->device));
     if (const int rc = ensure_calib_buffers(h)) return rc;
@@ -2021,6 +2225,7 @@ int music_b200_calib_accumulate_device(music_b200 *h, const float *d_in_c64, uin
 {
     h = served(h);
     if (!h) return MUSIC_B200_EINVAL;
+    if (h->chan) return fail(h, MUSIC_B200_EINVAL, "per-channel calibration is not built: a channel handle takes no calibration");
     if (nwindows == 0) return MUSIC_B200_OK;
     if (!d_in_c64) return fail(h, MUSIC_B200_EINVAL, "d_in_c64 must not be NULL");
     if ((reinterpret_cast<uintptr_t>(d_in_c64) & 15u) != 0) return fail(h, MUSIC_B200_EINVAL, "d_in_c64 must be 16-byte aligned");
@@ -2033,6 +2238,7 @@ int music_b200_calib_accumulate_host(music_b200 *h, const float *in_c64, uint32_
 {
     h = served(h);
     if (!h) return MUSIC_B200_EINVAL;
+    if (h->chan) return fail(h, MUSIC_B200_EINVAL, "per-channel calibration is not built: a channel handle takes no calibration");
     if (nwindows == 0) return MUSIC_B200_OK;
     if (!in_c64) return fail(h, MUSIC_B200_EINVAL, "in_c64 must not be NULL");
     std::lock_guard<std::mutex> g(h->mutex);
@@ -2064,6 +2270,7 @@ int music_b200_calib_solve(music_b200 *h, double az_deg, double el_deg, int kind
 {
     h = served(h);
     if (!h) return MUSIC_B200_EINVAL;
+    if (h->chan) return fail(h, MUSIC_B200_EINVAL, "per-channel calibration is not built: a channel handle takes no calibration");
     if (!gains) return fail(h, MUSIC_B200_EINVAL, "gains must not be NULL");
     if (kind != MUSIC_B200_CALIB_PHASE && kind != MUSIC_B200_CALIB_GAIN_PHASE) return fail(h, MUSIC_B200_EINVAL, "unknown calibration kind %d", kind);
     if (kind == MUSIC_B200_CALIB_GAIN_PHASE && h->m < 3)
@@ -2115,8 +2322,10 @@ int music_b200_set_source_rule(music_b200 *h, int rule)
     if (!h) return MUSIC_B200_EINVAL;
     if (rule != MUSIC_B200_SOURCES_FIXED && rule != MUSIC_B200_SOURCES_MDL && rule != MUSIC_B200_SOURCES_AIC)
         return fail(h, MUSIC_B200_EINVAL, "unknown source rule %d", rule);
-    if (rule != MUSIC_B200_SOURCES_FIXED && h->N <= h->m)
-        return fail(h, MUSIC_B200_EINVAL, "MDL / AIC need more snapshots than antennas (N = %u, m = %u)", h->N, h->m);
+    if (rule != MUSIC_B200_SOURCES_FIXED && snapshots(h) <= h->m)
+        return fail(h, MUSIC_B200_EINVAL, "MDL / AIC need more snapshots than antennas (N = %u, m = %u)", snapshots(h), h->m);
+    if (rule != MUSIC_B200_SOURCES_FIXED && h->chan && h->chan_combine == MUSIC_B200_CHANNELS_INCOHERENT)
+        return fail(h, MUSIC_B200_EINVAL, "the INCOHERENT combine is defined for the FIXED source rule only");
     std::lock_guard<std::mutex> g(h->mutex);
     if (const int rc = for_each_child(h, [&](music_b200 *c) { return music_b200_set_source_rule(c, rule); })) return rc;
     h->source_rule = rule;
@@ -2195,6 +2404,7 @@ int music_b200_gather_create(music_b200 *h, uint32_t total_windows, unsigned cha
     if (!h || !ipc_handles) return MUSIC_B200_EINVAL;
     if (!h->kids.empty()) return fail(h, MUSIC_B200_EINVAL, "gather_create applies to single-device handles (a multi-device handle gathers in process_device_sharded)");
     if (h->azel) return fail(h, MUSIC_B200_EINVAL, "the bins all-gather is not supported on an az-el handle");
+    if (h->chan) return fail(h, MUSIC_B200_EINVAL, "the bins all-gather is not built for channel handles");
     std::lock_guard<std::mutex> g(h->mutex);
     CU(h, cudaSetDevice(h->device));
     if (h->gather_buf) return fail(h, MUSIC_B200_EINVAL, "gather buffer already created");
@@ -2218,6 +2428,7 @@ int music_b200_gather_attach(music_b200 *h, int nranks, int rank, const unsigned
     if (!h || !all_handles) return MUSIC_B200_EINVAL;
     if (nranks < 1 || nranks > MAX_PEERS || rank < 0 || rank >= nranks) return fail(h, MUSIC_B200_EINVAL, "need 1 <= nranks <= %d and 0 <= rank < nranks", MAX_PEERS);
     if (h->azel) return fail(h, MUSIC_B200_EINVAL, "the bins all-gather is not supported on an az-el handle");
+    if (h->chan) return fail(h, MUSIC_B200_EINVAL, "the bins all-gather is not built for channel handles");
     std::lock_guard<std::mutex> g(h->mutex);
     if (!h->gather_buf) return fail(h, MUSIC_B200_EINVAL, "call gather_create first");
     CU(h, cudaSetDevice(h->device));
@@ -2378,6 +2589,175 @@ int music_b200_process_azel_host(music_b200 *h, const float *in_c64, uint32_t nw
     return process_host_impl(h, in_c64, nwindows, o);
 }
 
+/* ---- frequency-channelised direction finding (music_channels.cuh) ---- */
+int music_b200_create_channels(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples, uint32_t resolution, uint32_t nfft,
+                               uint32_t chan_first, uint32_t chan_count, int taper, int combine, int device)
+{
+    if (!out) return fail(nullptr, MUSIC_B200_EINVAL, "out must not be NULL");
+    *out = nullptr;
+    if (m == 0 || m > MUSIC_B200_MAX_M) return fail(nullptr, MUSIC_B200_EINVAL, "m must be in 1..%d (got %u)", MUSIC_B200_MAX_M, m);
+    if (n == 0 || n >= m) return fail(nullptr, MUSIC_B200_EINVAL, "need 1 <= n < m (got n=%u, m=%u)", n, m);
+    if (nsamples == 0 || nsamples % m != 0) return fail(nullptr, MUSIC_B200_EINVAL, "nsamples must be a positive multiple of m (got %u)", nsamples);
+    if (resolution == 0) return fail(nullptr, MUSIC_B200_EINVAL, "resolution must be > 0");
+    if (nfft < (uint32_t)CHAN_MIN_F || nfft > (uint32_t)CHAN_MAX_F || (nfft & (nfft - 1)) != 0)
+        return fail(nullptr, MUSIC_B200_EINVAL, "nfft must be a power of two in %d..%d (got %u)", CHAN_MIN_F, CHAN_MAX_F, nfft);
+    if ((nsamples / m) % nfft != 0)
+        return fail(nullptr, MUSIC_B200_EINVAL, "nfft must divide the %u snapshots of a window (got %u)", nsamples / m, nfft);
+    if (chan_count == 0 || chan_count > nfft || chan_first >= nfft)
+        return fail(nullptr, MUSIC_B200_EINVAL, "need 1 <= chan_count <= nfft and chan_first < nfft (got first=%u, count=%u)", chan_first, chan_count);
+    if (taper != MUSIC_B200_TAPER_RECT && taper != MUSIC_B200_TAPER_HANN) return fail(nullptr, MUSIC_B200_EINVAL, "unknown taper %d", taper);
+    if (combine != MUSIC_B200_CHANNELS_SEPARATE && combine != MUSIC_B200_CHANNELS_INCOHERENT)
+        return fail(nullptr, MUSIC_B200_EINVAL, "unknown combine rule %d", combine);
+    music_b200 spec;
+    ChanShape &cs = spec.cshape;
+    cs.M = (int)m;
+    cs.N = (int)(nsamples / m);
+    cs.F = (int)nfft;
+    for (cs.logF = 0; (1u << cs.logF) < nfft; ++cs.logF) {}
+    cs.J = cs.N / cs.F;
+    cs.first = (int)chan_first;
+    cs.C = (int)chan_count;
+    spec.chan_taper = taper;
+    spec.chan_combine = combine;
+    return create_on_device(out, m, n, nsamples, resolution, nullptr, device, nullptr, &spec);
+}
+
+namespace {
+
+// frequency offset of channel c in units of the sample rate: s(b_c) / F
+double channel_offset(const ChanShape &cs, int c)
+{
+    const int b = (cs.first + c) & (cs.F - 1);
+    return (double)(b < cs.F / 2 ? b : b - cs.F) / (double)cs.F;
+}
+
+}  // namespace
+
+int music_b200_set_geometry_channels(music_b200 *h, const double *positions_xy, double centre_frequency_hz, double sample_rate_hz)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (!h->chan) return fail(h, MUSIC_B200_EINVAL, "set_geometry_channels needs a handle from music_b200_create_channels");
+    if (!positions_xy) return fail(h, MUSIC_B200_EINVAL, "element positions must not be NULL");
+    for (uint32_t i = 0; i < 2 * h->m; ++i)
+        if (!std::isfinite(positions_xy[i])) return fail(h, MUSIC_B200_EINVAL, "element positions must be finite");
+    if (!(sample_rate_hz > 0.0) || !std::isfinite(sample_rate_hz)) return fail(h, MUSIC_B200_EINVAL, "the sample rate must be positive and finite");
+    if (!std::isfinite(centre_frequency_hz) || !(centre_frequency_hz > 0.5 * sample_rate_hz))
+        return fail(h, MUSIC_B200_EINVAL, "the centre frequency must be finite and above half the sample rate (every channel frequency must be > 0)");
+    std::lock_guard<std::mutex> g(h->mutex);
+    CU(h, cudaSetDevice(h->device));
+    CU(h, cudaDeviceSynchronize());  // as in set_table(): the slot being rebuilt must be idle
+    const int slot = h->cur_table ^ 1;
+    if (const int rc = ensure_channel_tables(h, slot)) return rc;
+    for (int c = 0; c < h->cshape.C; ++c) {
+        const double f_c = sample_rate_hz * channel_offset(h->cshape, c);
+        const double lambda = 299792458.0 / (centre_frequency_hz + f_c);
+        if (const int rc = build_table(h, h->ctab[slot][c], positions_xy, lambda, h->streams[0])) return rc;
+    }
+    h->ctab_shared[slot] = false;
+    h->cur_table = slot;
+    h->ctab_set = true;
+    h->chan_fs = sample_rate_hz;
+    return MUSIC_B200_OK;
+}
+
+int music_b200_channel_frequencies(music_b200 *h, double *offsets_hz)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (!h->chan) return fail(h, MUSIC_B200_EINVAL, "channel_frequencies needs a handle from music_b200_create_channels");
+    if (!offsets_hz) return fail(h, MUSIC_B200_EINVAL, "offsets_hz must not be NULL");
+    std::lock_guard<std::mutex> g(h->mutex);
+    if (h->chan_fs == 0.0) return fail(h, MUSIC_B200_EINVAL, "no sample rate yet: call music_b200_set_geometry_channels()");
+    for (int c = 0; c < h->cshape.C; ++c) offsets_hz[c] = h->chan_fs * channel_offset(h->cshape, c);
+    return MUSIC_B200_OK;
+}
+
+int music_b200_get_table_channel(music_b200 *h, uint32_t channel, float *table_c64)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (!h->chan) return fail(h, MUSIC_B200_EINVAL, "get_table_channel needs a handle from music_b200_create_channels");
+    if (!table_c64) return fail(h, MUSIC_B200_EINVAL, "output table must not be NULL");
+    if (channel >= (uint32_t)h->cshape.C) return fail(h, MUSIC_B200_EINVAL, "channel %u out of range (0..%d)", channel, h->cshape.C - 1);
+    std::lock_guard<std::mutex> g(h->mutex);
+    if (!h->ctab_set) return fail(h, MUSIC_B200_EINVAL, "no array response yet: call music_b200_set_geometry_channels() or music_b200_set_table()");
+    CU(h, cudaSetDevice(h->device));
+    CU(h, cudaMemcpy(table_c64, channel_table(h, (int)channel).c64, (size_t)h->K * h->m * 2 * sizeof(float), cudaMemcpyDeviceToHost));
+    return MUSIC_B200_OK;
+}
+
+int music_b200_process_channels_device(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_angles, float *d_levels,
+                                       float *d_spectrum, int32_t *d_bins, int32_t *d_counts, double *d_R, void *stream)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (!h->chan) return fail(h, MUSIC_B200_EINVAL, "process_channels_device needs a handle from music_b200_create_channels");
+    std::lock_guard<std::mutex> g(h->mutex);
+    NvtxRange range("music_b200_process_channels_device");
+    CU(h, cudaSetDevice(h->device));
+    Outputs o = caller_outputs(d_angles, d_levels, d_spectrum, d_bins);
+    o.counts = d_counts;
+    return enqueue_channels(h, d_in_c64, nwindows, o.shaped(h), d_R, static_cast<cudaStream_t>(stream));
+}
+
+int music_b200_process_channels_host(music_b200 *h, const float *in_c64, uint32_t nwindows, float *angles, float *levels, float *spectrum,
+                                     int32_t *bins, int32_t *counts, double *R)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (!h->chan) return fail(h, MUSIC_B200_EINVAL, "process_channels_host needs a handle from music_b200_create_channels");
+    if (nwindows == 0) return MUSIC_B200_OK;
+    if (!in_c64 || !angles) return fail(h, MUSIC_B200_EINVAL, "in_c64 and angles must not be NULL");
+    std::lock_guard<std::mutex> g(h->mutex);
+    NvtxRange range("music_b200_process_channels_host");
+    CU(h, cudaSetDevice(h->device));
+    // Chunks of windows through one device arena on the handle's first stream: the input, then each output in the
+    // chunk's own channel-major layout [rows][chunk], copied into the caller's [rows][nwindows] arrays row by row.
+    const size_t C = (size_t)h->cshape.C, rows = h->chan_combine == MUSIC_B200_CHANNELS_SEPARATE ? C : 1;
+    const size_t n = h->n, K = h->K, mm2 = (size_t)h->m * h->m * 2, win_bytes = (size_t)h->nsamples * 2 * sizeof(float);
+    struct Piece { void *host; size_t nrows, row_bytes; bool want; size_t off; };  // row_bytes: of one window
+    Piece pc[6] = {{angles, rows, n * sizeof(float), true, 0},      {levels, rows, n * sizeof(float), levels != nullptr, 0},
+                   {bins, rows, n * sizeof(int32_t), bins != nullptr, 0}, {counts, rows, sizeof(int32_t), counts != nullptr, 0},
+                   {spectrum, rows, K * sizeof(float), spectrum != nullptr, 0}, {R, C, mm2 * sizeof(double), R != nullptr, 0}};
+    size_t per_win = win_bytes;
+    for (const Piece &p : pc) per_win += p.want ? p.nrows * p.row_bytes : 0;
+    const uint32_t chunk = (uint32_t)std::max<size_t>(1, std::min<size_t>(nwindows, ((size_t)64 << 20) / per_win));
+    const auto align = [](size_t b) { return (b + 255) / 256 * 256; };
+    size_t need = align((size_t)chunk * win_bytes);
+    for (Piece &p : pc) {
+        p.off = need;
+        if (p.want) need += align(p.nrows * p.row_bytes * chunk);
+    }
+    if (need > h->chan_arena_cap) {
+        CU(h, cudaDeviceSynchronize());
+        cudaFree(h->chan_arena);
+        h->chan_arena = nullptr;
+        h->chan_arena_cap = 0;
+        CU(h, cudaMalloc(&h->chan_arena, need));
+        h->chan_arena_cap = need;
+    }
+    cudaStream_t st = h->streams[0];
+    int rc = MUSIC_B200_OK;
+    for (uint32_t w0 = 0; w0 < nwindows && rc == MUSIC_B200_OK; w0 += chunk) {
+        const uint32_t W = std::min(chunk, nwindows - w0);
+        float *d_in = reinterpret_cast<float *>(h->chan_arena);
+        CU_BREAK(h, rc, cudaMemcpyAsync(d_in, in_c64 + (size_t)w0 * h->nsamples * 2, (size_t)W * win_bytes, cudaMemcpyHostToDevice, st));
+        const auto dev = [&](int i) { return pc[i].want ? h->chan_arena + pc[i].off : nullptr; };
+        Outputs o = caller_outputs(reinterpret_cast<float *>(dev(0)), reinterpret_cast<float *>(dev(1)), reinterpret_cast<float *>(dev(4)),
+                                   reinterpret_cast<int32_t *>(dev(2)));
+        o.counts = reinterpret_cast<int32_t *>(dev(3));
+        rc = enqueue_channels(h, d_in, W, o.shaped(h), reinterpret_cast<double *>(dev(5)), st);
+        if (rc) break;
+        for (int i = 0; i < 6 && rc == MUSIC_B200_OK; ++i) {
+            const Piece &p = pc[i];
+            if (!p.want) continue;
+            CU_BREAK(h, rc, cudaMemcpy2DAsync(static_cast<char *>(p.host) + (size_t)w0 * p.row_bytes, (size_t)nwindows * p.row_bytes, dev(i),
+                                              (size_t)W * p.row_bytes, (size_t)W * p.row_bytes, p.nrows, cudaMemcpyDeviceToHost, st));
+        }
+        if (rc) break;
+        CU_BREAK(h, rc, cudaStreamSynchronize(st));  // the arena is free for the next chunk
+    }
+    const cudaError_t e = cudaStreamSynchronize(st);
+    if (rc == MUSIC_B200_OK && e != cudaSuccess) rc = fail(h, MUSIC_B200_ECUDA, "stream sync failed: %s", cudaGetErrorString(e));
+    return rc;
+}
+
 void music_b200_destroy(music_b200 *h)
 {
     if (!h) return;
@@ -2397,6 +2777,8 @@ void music_b200_destroy(music_b200 *h)
     cudaFree(h->f8_stats);
     cudaFree(h->work_ctr);
     cudaFree(h->cal_acc); cudaFree(h->cal_part); cudaFree(h->cal_ctr); cudaFree(h->cal_out);
+    cudaFree(h->chan_tw); cudaFree(h->chan_taper_d); cudaFree(h->chan_arena);
+    for (int i = 0; i < 2; ++i) { cudaFree(h->ctab_c64[i]); cudaFree(h->ctab_soa[i]); }
     cudaFree(h->steer_pos); cudaFree(h->steer_count); cudaFree(h->steer_list); cudaFree(h->steer_vals);
     if (h->fused_done) cudaEventDestroy(h->fused_done);
     for (int i = 0; i < 2; ++i) {

@@ -523,6 +523,68 @@ int music_b200_process_azel_host(music_b200 *h, const float *in_c64, uint32_t nw
 int music_b200_process_azel_device(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_azimuth, float *d_elevation,
                                    float *d_levels, float *d_spectrum, int32_t *d_bins, int32_t *d_counts, void *stream);
 
+/*
+ * Frequency-channelised direction finding (extension, no reference counterpart): an FFT filter bank fused into the
+ * covariance, one direction-finding problem per frequency channel, and the incoherent wideband MUSIC spectrum.  Every
+ * other mode starts from one covariance over the whole sampled bandwidth; a channel handle separates emitters at
+ * different frequencies and matches each channel against a table built for that channel's own wavelength.
+ * A channel handle has, besides m, n, nsamples (N = nsamples / m snapshots) and resolution (K): an FFT length F = nfft
+ * (a power of two, 8 <= F <= 256, F | N), a channel range (chan_first < F, 1 <= chan_count = C <= F), a taper and a
+ * combine rule.
+ *   segments   window w is cut into J = N / F consecutive, non-overlapping segments of F snapshots.
+ *   filter bank  X_j[b] = sum_{t<F} h[t] x[jF + t] exp(-2 pi i b t / F) (an m-vector), h = 1 (MUSIC_B200_TAPER_RECT) or the
+ *              periodic Hann h[t] = 1/2 - 1/2 cos(2 pi t / F) (MUSIC_B200_TAPER_HANN).
+ *   channels   channel c in [0, C) is FFT bin b_c = (chan_first + c) mod F, so a range may wrap through the negative
+ *              frequencies, at frequency offset f_c = fs * (s(b_c) / F), s(b) = b for b < F / 2 and b - F otherwise
+ *              (evaluated in fp64 in exactly this order; music_b200_channel_frequencies returns f_c).
+ *   covariance R_c = sum_j X_j[b_c] X_j[b_c]^H / (J sum_t h[t]^2), fp64 throughout (the inputs widen exactly).  White
+ *              noise of power s2 gives R_c ~ s2 I in every channel; for RECT (1 / F) sum_b R_b is the plain handle's R.
+ *              R_c does not depend on which other channels the handle has.
+ *   tables     set_geometry_channels(positions_xy, f_centre, fs) builds one table per channel with the device builder of
+ *              music_b200_set_geometry(): a_c(theta)[r] = exp(-j 2 pi <p_r, u(theta)> / lambda_c),
+ *              lambda_c = 299792458.0 / (f_centre + f_c), bit-identical to set_geometry(positions_xy, lambda_c) on a plain
+ *              handle.  f_centre must exceed fs / 2.  music_b200_set_table() on a channel handle installs ONE measured
+ *              table for all channels: that is the narrowband assumption, and the caller's choice.  create_channels()
+ *              installs no table: a process call before either returns EINVAL.  music_b200_get_table_channel() returns
+ *              channel c's table; music_b200_get_table() returns EINVAL on a channel handle.
+ *   SEPARATE   every (window, channel) is an ordinary problem on (R_c, table_c): estimator MUSIC / MVDR / BARTLETT, peak
+ *              mode TOP_BINS / LOCAL_MAXIMA, source rule FIXED / MDL / AIC with their definitions above, except that MDL,
+ *              AIC and the N <= m conditions use J, the number of segments (the independent looks), in place of N.  Under
+ *              MDL a count of 0 is how an empty channel shows.
+ *              Outputs are channel-major: angles / levels / bins [C][W][n], counts [C][W], spectrum [C][W][K]; channel
+ *              c's block is what a plain handle would have written for (R_c, table_c).
+ *   INCOHERENT (Wax, Shan and Kailath 1984) one problem per window: P(theta_k) = 1 / sum_c (1 / P_c(theta_k)), P_c channel
+ *              c's MUSIC strength with its own table, i.e. 1 / sum_c ||G_c^H a_c(theta_k)||^2, summed in channel order;
+ *              then the peak mode on P.  MUSIC estimator and FIXED rule only.  angles / levels / bins [W][n],
+ *              spectrum [W][K], counts must be NULL.
+ *   R          (either rule, may be NULL) [C][W][m][m] complex fp64.
+ * Not built, and refused with EINVAL rather than ignored: the ROOTS, ESPRIT and DML peak modes, refinement, beams
+ * (set_beamformer), calibration (set_calibration and the calib entries), the planar, sharded, gather and az-el entries and
+ * set_geometry() on a channel handle; create_multi() makes no channel handle.  The plain process entries on a channel
+ * handle and the channel entries on a plain handle return EINVAL.  Segments do not overlap.
+ * A call runs, per sub-batch: chan_cov_kernel (the filter bank and all C covariances, one read of the input per channel
+ * group; timed in the covariance slot of the stage timing), then the eigensolver, source count and MVDR preparation of the
+ * plain unfused path once over all C * W (window, channel) pairs, then one scan and one peak-rule launch per channel on
+ * that channel's table, and under INCOHERENT one combine kernel and one peak-rule launch.  set_estimator, set_peak_mode,
+ * set_source_rule, stage timing, the reducers and launch_count work as on any handle.
+ * The device entry is enqueued on `stream` and does not synchronise; d_in must be 16-byte aligned.  The host entry copies
+ * in chunks and returns when done.
+ */
+#define MUSIC_B200_TAPER_RECT 0
+#define MUSIC_B200_TAPER_HANN 1
+#define MUSIC_B200_CHANNELS_SEPARATE 0
+#define MUSIC_B200_CHANNELS_INCOHERENT 1
+int music_b200_create_channels(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples, uint32_t resolution, uint32_t nfft,
+                               uint32_t chan_first, uint32_t chan_count, int taper, int combine, int device);
+int music_b200_set_geometry_channels(music_b200 *h, const double *positions_xy /* [m][2] */, double centre_frequency_hz,
+                                     double sample_rate_hz);
+int music_b200_channel_frequencies(music_b200 *h, double *offsets_hz /* [C] */);
+int music_b200_get_table_channel(music_b200 *h, uint32_t channel, float *table_c64);
+int music_b200_process_channels_device(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_angles, float *d_levels,
+                                       float *d_spectrum, int32_t *d_bins, int32_t *d_counts, double *d_R, void *stream);
+int music_b200_process_channels_host(music_b200 *h, const float *in_c64, uint32_t nwindows, float *angles, float *levels,
+                                     float *spectrum, int32_t *bins, int32_t *counts, double *R);
+
 /* Copies the table currently in use (float[resolution][m][2]) back to host memory. */
 int music_b200_get_table(music_b200 *h, float *table_c64);
 
