@@ -207,7 +207,7 @@ struct music_b200 {
     bool pdl = true;                   // fused M = 4 kernel: programmatic dependent launch (MUSIC_B200_PDL=0 turns it off)
     cudaEvent_t fused_done = nullptr;  // orders persistent launches that share a ticket counter but not a stream
     bool fused_used[2] = {false, false};
-    int eig_mode = 0;                 // fused kernel: 0 principal eigenvector by squaring (default), 1 / 2 Jacobi with four lanes / one lane per window (MUSIC_B200_EIG=jacobi|jacobi1)
+    int eig_mode = 0;                 // fused kernels: 0 principal eigenvector by squaring (default), otherwise their Jacobi solver for every window (four lanes per window at M = 4, one warp at M = 8); MUSIC_B200_EIG=jacobi and the older spelling jacobi1 (2) both select it
     unsigned *f8_stats = nullptr;     // fused M = 8 kernel: windows solved by squaring / by the Jacobi fallback
     int mma_fin_max = 2;              // fused kernel: no tensor-core pass starts once the tickets have run out and this many covariance warps are done (MUSIC_B200_MMA_FIN; 0: at ticket exhaustion, -1: fp64 drain only)
     long long *fused_trace = nullptr;  // MUSIC_B200_TRACE=1: per-CTA clock64 trace of the fused kernel (tools/fused_trace.py)
