@@ -130,6 +130,10 @@ def load():
         L.music_b200_channel_frequencies.restype = ctypes.c_int
         L.music_b200_get_table_channel.argtypes = [vp, u32, fp]
         L.music_b200_get_table_channel.restype = ctypes.c_int
+        L.music_b200_set_focusing.argtypes = [vp, u32, u32]
+        L.music_b200_set_focusing.restype = ctypes.c_int
+        L.music_b200_get_focusing.argtypes = [vp, fp, fp]
+        L.music_b200_get_focusing.restype = ctypes.c_int
         L.music_b200_process_channels_device.argtypes = [vp, fp, u32, fp, fp, fp, fp, fp, fp, vp]
         L.music_b200_process_channels_device.restype = ctypes.c_int
         L.music_b200_process_channels_host.argtypes = [vp, fp, u32, fp, fp, fp, fp, fp, fp]
@@ -169,6 +173,7 @@ EXPORTS = [
     "music_b200_calib_accumulate_host", "music_b200_calib_solve",
     "music_b200_create_channels", "music_b200_set_geometry_channels", "music_b200_channel_frequencies",
     "music_b200_get_table_channel", "music_b200_process_channels_device", "music_b200_process_channels_host",
+    "music_b200_set_focusing", "music_b200_get_focusing",
 ]
 
 

@@ -38,6 +38,7 @@
 #include "music_beams.cuh"
 #include "music_calib.cuh"
 #include "music_channels.cuh"
+#include "music_focus.cuh"
 
 using namespace music;
 
@@ -197,6 +198,16 @@ struct music_b200 {
     double chan_fs = 0.0;          // sample rate of the last set_geometry_channels() (0: none yet)
     unsigned char *chan_arena = nullptr;  // device staging of the channel host entry
     size_t chan_arena_cap = 0;
+    // COHERENT combine (music_focus.cuh): the focusing sector (count 0: the whole grid), per table slot the focusing
+    // matrices T_c [C][m][m] on the device and the focusing errors e_c, and the set-up scratch
+    uint32_t foc_first = 0, foc_count = 0;
+    double2 *foc_T[2] = {nullptr, nullptr};
+    std::vector<double> foc_err[2];
+    double *foc_lam = nullptr;   // [C] the wavelengths of the slot being focused
+    double2 *foc_B = nullptr;    // [C][m][m] B_c
+    double *foc_e2 = nullptr;    // [C] squared focusing errors
+    double2 *foc_Rc = nullptr;   // the filter bank's [C][W][m][m] covariances of a sub-batch (the workspace holds W windows)
+    size_t foc_Rc_cap = 0;       // its capacity in C * W matrices
 
     // fp64 workspace slots (R, eigenvalues, sorted eigenvectors, optional strengths) of the unfused path: one per
     // staging stream of the host entry points (slot 0 also serves the device entry points)
@@ -353,8 +364,14 @@ UlaGeom ula_geometry(const double *pos, int M, double lambda)
 // The peak modes that take their angles from the ULA geometry instead of the table: ROOTS and ESPRIT
 bool gridless_ula(int peak) { return peak == MUSIC_B200_PEAKS_ROOTS || peak == MUSIC_B200_PEAKS_ESPRIT; }
 
-// The independent looks behind each covariance: the N snapshots of a window, on a channel handle its J segments.
-uint32_t snapshots(const music_b200 *h) { return h->chan ? (uint32_t)h->cshape.J : h->N; }
+bool coherent(const music_b200 *h) { return h->chan && h->chan_combine == MUSIC_B200_CHANNELS_COHERENT; }
+
+// The independent looks behind each covariance: the N snapshots of a window, on a channel handle its J segments, and
+// behind a focused covariance the J segments of all C channels.
+uint32_t snapshots(const music_b200 *h)
+{
+    return !h->chan ? h->N : coherent(h) ? (uint32_t)(h->cshape.J * h->cshape.C) : (uint32_t)h->cshape.J;
+}
 
 // Whether handle h can run with modes p; if not, records why and returns EINVAL.  With a table t, also whether p can run
 // on it: the gridless ULA peak modes need a ULA geometry, the refinement a geometric table.  Tables are checked on handles that
@@ -374,7 +391,7 @@ int check_modes(music_b200 *h, const Modes &p, const DeviceTable *t)
     if (p.est == MUSIC_B200_ESTIMATOR_MVDR && p.loading == 0.0 && snapshots(h) <= h->m)
         return fail(h, MUSIC_B200_EINVAL, "MVDR without diagonal loading needs more snapshots than antennas (N = %u, m = %u): R is singular",
                     snapshots(h), h->m);
-    if (h->chan) {
+    if (h->chan && !coherent(h)) {
         // per channel only the grid modes are built (include/music_b200.h lists the rest as not built)
         if (p.peak != MUSIC_B200_PEAKS_TOP_BINS && p.peak != MUSIC_B200_PEAKS_LOCAL_MAXIMA)
             return fail(h, MUSIC_B200_EINVAL, "a channel handle takes the TOP_BINS and LOCAL_MAXIMA peak modes only (ROOTS, ESPRIT and DML "
@@ -407,8 +424,16 @@ int check_modes(music_b200 *h, const Modes &p, const DeviceTable *t)
     return MUSIC_B200_OK;
 }
 
-// the current table of a handle that holds one (a multi-device handle's children hold the copies)
-const DeviceTable *own_table(const music_b200 *h) { return h->kids.empty() ? &h->table[h->cur_table] : nullptr; }
+// the table channel c of a channel handle scans with
+const DeviceTable &channel_table(const music_b200 *h, int c) { return h->ctab[h->cur_table][h->ctab_shared[h->cur_table] ? 0 : c]; }
+
+// The current table of a handle that holds one (a multi-device handle's children hold the copies).  On a channel handle:
+// the reference channel's (what a focused covariance is matched against), once there is one.
+const DeviceTable *own_table(const music_b200 *h)
+{
+    if (h->chan) return h->ctab_set ? &channel_table(h, h->cshape.C / 2) : nullptr;
+    return h->kids.empty() ? &h->table[h->cur_table] : nullptr;
+}
 
 // The handle that serves an entry point which a multi-device handle does not spread over its devices: device 0.
 music_b200 *served(music_b200 *h) { return h && !h->kids.empty() ? h->kids[0] : h; }
@@ -617,8 +642,10 @@ uint32_t max_sub_windows(const music_b200 *h, const Plan &p)
     const size_t per_win = (size_t)h->m * h->m * 2 * 8 * 2 + h->m * 8 + (p.ws_p64 ? (size_t)h->K * 8 : 0) +
                            (p.ws_counts ? sizeof(int32_t) : 0) + (p.ws_bins ? h->n * sizeof(int32_t) : 0) +
                            (p.ws_wts ? (size_t)h->n * h->m * 2 * sizeof(double) : 0);
-    // a channel handle's workspace holds C pseudo-windows per window
-    size_t c = ((size_t)384 << 20) / (per_win * (h->chan ? (size_t)h->cshape.C : 1));
+    // A SEPARATE / INCOHERENT channel handle's workspace holds C pseudo-windows per window; a COHERENT one holds the
+    // windows, and the channel buffer beside it the C covariances of each.
+    const size_t C = h->chan ? (size_t)h->cshape.C : 1;
+    size_t c = coherent(h) ? ((size_t)384 << 20) / (per_win + C * h->m * h->m * sizeof(double2)) : ((size_t)384 << 20) / (per_win * C);
     c = std::max<size_t>(SCAN_B, std::min<size_t>(c, 1u << 20));
     return (uint32_t)(c / SCAN_B * SCAN_B);
 }
@@ -948,19 +975,18 @@ void launch_grid_peaks(music_b200 *h, Peaks peaks, const double *p64, uint32_t W
     else topn_kernel<<<(W + 7) / 8, 256, 0, st>>>(p64, (int)h->n, (int)h->K, (int)W, po, cnt);
 }
 
-// K2 (+ source count) + K3 (+ peak rule) of W windows from ws.R into the outputs o (of these W windows), on `st`, as
-// planned.  tev (optional) = timing events [1..4].  An az-el handle's peak bins are decoded into (azimuth, elevation)
+// K2 (+ source count from `nsnap` looks) + K3 (+ peak rule) of W windows from ws.R against table tb into the outputs o
+// (of these W windows), on `st`, as planned.  tev (optional) = timing events [1..4].  An az-el handle's peak bins are decoded into (azimuth, elevation)
 // after the peak rule.  With refinement on, the refine kernel follows (timed with the peak rule) and reads the bins
 // written before it: from the caller's array, or from the workspace when the caller asked for none.  A beams call
 // then forms the weights and beams of the windows at d_in (timed with the peak rule as well).
-int launch_eig_scan(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t W, const Outputs &o, cudaStream_t st, cudaEvent_t *tev,
-                    const float *d_in = nullptr)
+int launch_eig_scan(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t W, const Outputs &o, const DeviceTable &tb, uint32_t nsnap,
+                    cudaStream_t st, cudaEvent_t *tev, const float *d_in = nullptr)
 {
     const int M = (int)h->m;
-    const DeviceTable &tb = h->table[h->cur_table];
     PeakOut po = make_peak_out(o);
     if (p.ws_bins && !po.bins) po.bins = ws.bins;
-    const int32_t *cnt = launch_eig_stage(h, p, ws, W, o.counts, h->N, st);
+    const int32_t *cnt = launch_eig_stage(h, p, ws, W, o.counts, nsnap, st);
     if (tev) cudaEventRecord(tev[2], st);
     launch_scan(h, p, ws, W, o, po, cnt, tb, st);
     double *p64 = o.P64 ? o.P64 : ws.P64;  // what the peak rules read
@@ -1135,7 +1161,8 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, const Ou
             h->launches++;
         }
         if (tev) cudaEventRecord(tev[1], st);
-        rc = launch_eig_scan(h, plan, ws, W, out.at(w0), st, tev, planar ? nullptr : d_in + (size_t)w0 * h->nsamples * 2);
+        rc = launch_eig_scan(h, plan, ws, W, out.at(w0), h->table[h->cur_table], h->N, st, tev,
+                             planar ? nullptr : d_in + (size_t)w0 * h->nsamples * 2);
         if (rc) return rc;
         CU(h, cudaEventRecord(ws.scan_done, st));
         ws.used = true;
@@ -1148,28 +1175,31 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, const Ou
     return MUSIC_B200_OK;
 }
 
-// the table channel c of a channel handle scans with
-const DeviceTable &channel_table(const music_b200 *h, int c) { return h->ctab[h->cur_table][h->ctab_shared[h->cur_table] ? 0 : c]; }
-
 // A channel handle's call (music_channels.cuh): `nwindows` windows on `st` in sub-batches through workspace slot 0, which
 // holds a sub-batch of W windows as C * W pseudo-windows, channel-major [C][W].  The filter bank writes every channel's
 // R in one launch; eigensolver, source count (from the J segments) and MVDR preparation run once over all C * W
 // pseudo-windows; scan and peak rule run once per channel on that channel's contiguous run, with that channel's table,
 // straight into the channel's block of the caller's channel-major outputs `out` ([C][nwindows] rows under SEPARATE,
 // [nwindows] rows under INCOHERENT).  R_out (may be NULL): [C][nwindows][m][m] complex fp64.
+// Under COHERENT the filter bank writes the C * W covariances into the handle's channel buffer (foc_Rc), the focus kernel
+// folds them into W focused ones in the workspace, which is sized for W windows, and the plain unfused stages run once
+// over them, on the reference channel's table, with J * C looks; outputs and R_out have
+// [nwindows] rows.
 int enqueue_channels(music_b200 *h, const float *d_in, uint32_t nwindows, const Outputs &out, double *R_out, cudaStream_t st)
 {
     if (nwindows == 0) return MUSIC_B200_OK;
     if (!d_in || !out.angles) return fail(h, MUSIC_B200_EINVAL, "d_in_c64 and d_angles must not be NULL");
     if ((reinterpret_cast<uintptr_t>(d_in) & 15u) != 0) return fail(h, MUSIC_B200_EINVAL, "d_in_c64 must be 16-byte aligned");
     if (!h->ctab_set) return fail(h, MUSIC_B200_EINVAL, "no array response yet: call music_b200_set_geometry_channels() or music_b200_set_table()");
-    if (const int rc = check_modes(h, h->modes, nullptr)) return rc;
-    const bool separate = h->chan_combine == MUSIC_B200_CHANNELS_SEPARATE;
-    if (!separate && out.counts) return fail(h, MUSIC_B200_EINVAL, "the INCOHERENT combine reports no counts: counts must be NULL");
+    const bool separate = h->chan_combine == MUSIC_B200_CHANNELS_SEPARATE, focus = coherent(h);
     const ChanShape &cs = h->cshape;
+    const int ref = cs.C / 2;
+    if (const int rc = check_modes(h, h->modes, focus ? &channel_table(h, ref) : nullptr)) return rc;
+    if (h->chan_combine == MUSIC_B200_CHANNELS_INCOHERENT && out.counts)
+        return fail(h, MUSIC_B200_EINVAL, "the INCOHERENT combine reports no counts: counts must be NULL");
     const uint32_t C = (uint32_t)cs.C;
     if (h->source_rule == MUSIC_B200_SOURCES_FIXED && out.counts) {
-        const size_t e = (size_t)C * nwindows;
+        const size_t e = (size_t)(separate ? C : 1) * nwindows;
         fill_counts_kernel<<<(unsigned)((e + 255) / 256), 256, 0, st>>>(out.counts, (int)h->n, (int)e);
         h->launches++;
         CU(h, cudaGetLastError());
@@ -1177,7 +1207,15 @@ int enqueue_channels(music_b200 *h, const float *d_in, uint32_t nwindows, const 
     const Plan plan = plan_call(h, out, nullptr, 0);
     const uint32_t sub = std::min((nwindows + SCAN_B - 1) / SCAN_B * SCAN_B, max_sub_windows(h, plan));
     Workspace &ws = h->ws[0];
-    if (const int rc = ensure_slot(h, ws, sub * C, plan)) return rc;
+    if (const int rc = ensure_slot(h, ws, focus ? sub : sub * C, plan)) return rc;
+    if (focus && (size_t)sub * C > h->foc_Rc_cap) {
+        if (ws.used) CU(h, cudaEventSynchronize(ws.scan_done));  // the last call may still read it on another stream
+        cudaFree(h->foc_Rc);
+        h->foc_Rc = nullptr;
+        h->foc_Rc_cap = 0;
+        CU(h, cudaMalloc(&h->foc_Rc, (size_t)sub * C * h->m * h->m * sizeof(double2)));
+        h->foc_Rc_cap = (size_t)sub * C;
+    }
     if (ws.used) CU(h, cudaStreamWaitEvent(st, ws.scan_done, 0));
     const size_t mm2 = (size_t)h->m * h->m * 2, K = h->K;
     const size_t smem = chan_smem(cs.M, cs.F, cs.B, cs.Cg).total;
@@ -1186,8 +1224,23 @@ int enqueue_channels(music_b200 *h, const float *d_in, uint32_t nwindows, const 
         cudaEvent_t *tev = timing_events(h);
         if (tev) cudaEventRecord(tev[0], st);
         const int grid = (int)std::min<uint32_t>(W, (uint32_t)(h->sm_count * h->chan_ctas));
-        chan_cov_kernel<<<grid, CHAN_THREADS, smem, st>>>(d_in + (size_t)w0 * h->nsamples * 2, ws.R, (int)W, cs, h->chan_tw, h->chan_taper_d);
+        double *Rc = focus ? reinterpret_cast<double *>(h->foc_Rc) : ws.R;
+        chan_cov_kernel<<<grid, CHAN_THREADS, smem, st>>>(d_in + (size_t)w0 * h->nsamples * 2, Rc, (int)W, cs, h->chan_tw, h->chan_taper_d);
         h->launches++;
+        if (focus) {
+            // R_foc into the workspace, inside the covariance slot of the stage timing; then one plain problem per window
+            const int M = (int)h->m, wt = focus_windows(M);
+            chan_focus_kernel<<<(W + wt - 1) / wt, focus_threads(M), 0, st>>>(h->foc_Rc, reinterpret_cast<double2 *>(ws.R), (int)W, (int)C,
+                                                                            M, ref, h->foc_T[h->cur_table]);
+            h->launches++;
+            if (tev) cudaEventRecord(tev[1], st);
+            Outputs o = out.at(w0);
+            o.R = R_out ? R_out + (size_t)w0 * mm2 : nullptr;
+            if (const int rc = launch_eig_scan(h, plan, ws, W, o, channel_table(h, ref), snapshots(h), st, tev)) return rc;
+            CU(h, cudaEventRecord(ws.scan_done, st));
+            ws.used = true;
+            continue;
+        }
         if (tev) cudaEventRecord(tev[1], st);
         const int32_t *cnt = launch_eig_stage(h, plan, ws, C * W, nullptr, (uint32_t)cs.J, st);
         if (cnt && out.counts)
@@ -1748,6 +1801,9 @@ int music_b200_set_table(music_b200 *h, const float *table_c64)
     if (!h->kids.empty())  // multi-device handle: every device holds a full copy of the table (SURVEY.md section 8e)
         return for_each_child(h, [&](music_b200 *c) { return music_b200_set_table(c, table_c64); });
     CU(h, cudaSetDevice(h->device));
+    if (coherent(h))
+        return fail(h, MUSIC_B200_EINVAL, "the COHERENT combine focuses geometric tables: one measured table gives no focusing "
+                                          "(call music_b200_set_geometry_channels())");
     if (h->chan) {
         // one measured table for every channel (the narrowband assumption): entry 0 of the idle slot
         CU(h, cudaDeviceSynchronize());
@@ -2606,7 +2662,7 @@ int music_b200_create_channels(music_b200 **out, uint32_t m, uint32_t n, uint32_
     if (chan_count == 0 || chan_count > nfft || chan_first >= nfft)
         return fail(nullptr, MUSIC_B200_EINVAL, "need 1 <= chan_count <= nfft and chan_first < nfft (got first=%u, count=%u)", chan_first, chan_count);
     if (taper != MUSIC_B200_TAPER_RECT && taper != MUSIC_B200_TAPER_HANN) return fail(nullptr, MUSIC_B200_EINVAL, "unknown taper %d", taper);
-    if (combine != MUSIC_B200_CHANNELS_SEPARATE && combine != MUSIC_B200_CHANNELS_INCOHERENT)
+    if (combine != MUSIC_B200_CHANNELS_SEPARATE && combine != MUSIC_B200_CHANNELS_INCOHERENT && combine != MUSIC_B200_CHANNELS_COHERENT)
         return fail(nullptr, MUSIC_B200_EINVAL, "unknown combine rule %d", combine);
     music_b200 spec;
     ChanShape &cs = spec.cshape;
@@ -2631,6 +2687,53 @@ double channel_offset(const ChanShape &cs, int c)
     return (double)(b < cs.F / 2 ? b : b - cs.F) / (double)cs.F;
 }
 
+// The focusing matrices and errors of table slot `slot` (music_focus.cuh) from its channel tables' geometry and the
+// handle's sector: B_c on the device, the polar factors on the host, then the errors on the device.  On EINVAL (a
+// singular B_c) the slot's matrices are left as they were.
+int build_focusing(music_b200 *h, int slot, cudaStream_t st)
+{
+    const int C = h->cshape.C, M = (int)h->m, ref = C / 2;
+    const size_t MM = (size_t)M * M;
+    if (!h->foc_T[slot]) CU(h, cudaMalloc(&h->foc_T[slot], (size_t)C * MM * sizeof(double2)));
+    if (!h->foc_B) CU(h, cudaMalloc(&h->foc_B, (size_t)C * MM * sizeof(double2)));
+    if (!h->foc_lam) CU(h, cudaMalloc(&h->foc_lam, (size_t)C * sizeof(double)));
+    if (!h->foc_e2) CU(h, cudaMalloc(&h->foc_e2, (size_t)C * sizeof(double)));
+    FocusGeom g = {};
+    for (int i = 0; i < 2 * M; ++i) g.pos[i] = h->ctab[slot][0].geo.pos[i];
+    g.M = M; g.K = (int)h->K; g.C = C; g.ref = ref;
+    g.first = (int)h->foc_first;
+    g.count = h->foc_count ? (int)h->foc_count : (int)h->K;
+    std::vector<double> lam(C);
+    for (int c = 0; c < C; ++c) lam[c] = h->ctab[slot][c].geo.lambda;
+    CU(h, cudaMemcpyAsync(h->foc_lam, lam.data(), C * sizeof(double), cudaMemcpyHostToDevice, st));
+    focus_setup_kernel<<<C, FOCUS_THREADS, 0, st>>>(g, h->foc_lam, nullptr, h->foc_B, nullptr);
+    h->launches++;
+    CU(h, cudaGetLastError());
+    std::vector<std::complex<double>> B((size_t)C * MM), T((size_t)C * MM, std::complex<double>(0.0, 0.0));
+    CU(h, cudaMemcpyAsync(B.data(), h->foc_B, B.size() * sizeof(double2), cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    for (int c = 0; c < C; ++c) {
+        if (c == ref) {
+            for (int i = 0; i < M; ++i) T[(size_t)c * MM + (size_t)i * M + i] = 1.0;
+            continue;
+        }
+        if (!focus_polar(M, B.data() + (size_t)c * MM, T.data() + (size_t)c * MM))
+            return fail(h, MUSIC_B200_EINVAL, "the focusing matrix of channel %d is singular on this sector (sigma_min <= %g sigma_max): "
+                                              "widen the sector", c, FOCUS_SINGULAR);
+    }
+    CU(h, cudaMemcpyAsync(h->foc_T[slot], T.data(), T.size() * sizeof(double2), cudaMemcpyHostToDevice, st));
+    focus_setup_kernel<<<C, FOCUS_THREADS, 0, st>>>(g, h->foc_lam, h->foc_T[slot], nullptr, h->foc_e2);
+    h->launches++;
+    CU(h, cudaGetLastError());
+    std::vector<double> e2(C);
+    CU(h, cudaMemcpyAsync(e2.data(), h->foc_e2, C * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));  // T and e2 are locals
+    h->foc_err[slot].assign(C, 0.0);
+    for (int c = 0; c < C; ++c)
+        if (c != ref) h->foc_err[slot][c] = std::sqrt(e2[c]) / std::sqrt((double)M * g.count);
+    return MUSIC_B200_OK;
+}
+
 }  // namespace
 
 int music_b200_set_geometry_channels(music_b200 *h, const double *positions_xy, double centre_frequency_hz, double sample_rate_hz)
@@ -2653,6 +2756,8 @@ int music_b200_set_geometry_channels(music_b200 *h, const double *positions_xy, 
         const double lambda = 299792458.0 / (centre_frequency_hz + f_c);
         if (const int rc = build_table(h, h->ctab[slot][c], positions_xy, lambda, h->streams[0])) return rc;
     }
+    if (coherent(h))
+        if (const int rc = build_focusing(h, slot, h->streams[0])) return rc;
     h->ctab_shared[slot] = false;
     h->cur_table = slot;
     h->ctab_set = true;
@@ -2684,6 +2789,57 @@ int music_b200_get_table_channel(music_b200 *h, uint32_t channel, float *table_c
     return MUSIC_B200_OK;
 }
 
+int music_b200_set_focusing(music_b200 *h, uint32_t first_bin, uint32_t bin_count)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (!coherent(h)) return fail(h, MUSIC_B200_EINVAL, "set_focusing needs a channel handle with the COHERENT combine");
+    if (bin_count == 0 || bin_count > h->K || first_bin >= h->K)
+        return fail(h, MUSIC_B200_EINVAL, "need 1 <= bin_count <= resolution and first_bin < resolution (got first=%u, count=%u)", first_bin,
+                    bin_count);
+    std::lock_guard<std::mutex> g(h->mutex);
+    const uint32_t first0 = h->foc_first, count0 = h->foc_count;
+    h->foc_first = first_bin;
+    h->foc_count = bin_count;
+    if (!h->ctab_set) return MUSIC_B200_OK;  // the next set_geometry_channels() focuses on this sector
+    // As a retune does: fill the idle table slot (the current slot's channel tables, new matrices) and switch to it, so
+    // the current slot is never rewritten under a call; the slot being refilled must be idle, as in set_table().
+    CU(h, cudaSetDevice(h->device));
+    CU(h, cudaDeviceSynchronize());
+    const int cur = h->cur_table, slot = cur ^ 1;
+    if (const int rc = ensure_channel_tables(h, slot)) return rc;
+    const size_t C = (size_t)h->cshape.C;
+    CU(h, cudaMemcpy(h->ctab_c64[slot], h->ctab_c64[cur], C * h->K * h->m * 2 * sizeof(float), cudaMemcpyDeviceToDevice));
+    CU(h, cudaMemcpy(h->ctab_soa[slot], h->ctab_soa[cur], C * soa_doubles(h->K, h->m) * sizeof(double), cudaMemcpyDeviceToDevice));
+    for (size_t c = 0; c < C; ++c) {
+        DeviceTable t = h->ctab[cur][c];  // geometry, ULA test and flags; the slot's own buffers
+        t.c64 = h->ctab[slot][c].c64;
+        t.soa = h->ctab[slot][c].soa;
+        h->ctab[slot][c] = t;
+    }
+    if (const int rc = build_focusing(h, slot, h->streams[0])) {
+        h->foc_first = first0;
+        h->foc_count = count0;
+        return rc;
+    }
+    h->ctab_shared[slot] = false;
+    h->cur_table = slot;
+    return MUSIC_B200_OK;
+}
+
+int music_b200_get_focusing(music_b200 *h, double *T, double *err)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (!coherent(h)) return fail(h, MUSIC_B200_EINVAL, "get_focusing needs a channel handle with the COHERENT combine");
+    std::lock_guard<std::mutex> g(h->mutex);
+    if (!h->ctab_set) return fail(h, MUSIC_B200_EINVAL, "no focusing yet: call music_b200_set_geometry_channels()");
+    CU(h, cudaSetDevice(h->device));
+    const size_t C = (size_t)h->cshape.C;
+    if (T) CU(h, cudaMemcpy(T, h->foc_T[h->cur_table], C * h->m * h->m * sizeof(double2), cudaMemcpyDeviceToHost));
+    if (err)
+        for (size_t c = 0; c < C; ++c) err[c] = h->foc_err[h->cur_table][c];
+    return MUSIC_B200_OK;
+}
+
 int music_b200_process_channels_device(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_angles, float *d_levels,
                                        float *d_spectrum, int32_t *d_bins, int32_t *d_counts, double *d_R, void *stream)
 {
@@ -2710,11 +2866,12 @@ int music_b200_process_channels_host(music_b200 *h, const float *in_c64, uint32_
     // Chunks of windows through one device arena on the handle's first stream: the input, then each output in the
     // chunk's own channel-major layout [rows][chunk], copied into the caller's [rows][nwindows] arrays row by row.
     const size_t C = (size_t)h->cshape.C, rows = h->chan_combine == MUSIC_B200_CHANNELS_SEPARATE ? C : 1;
+    const size_t r_rows = coherent(h) ? 1 : C;  // R: the focused covariance of each window, or every channel's
     const size_t n = h->n, K = h->K, mm2 = (size_t)h->m * h->m * 2, win_bytes = (size_t)h->nsamples * 2 * sizeof(float);
     struct Piece { void *host; size_t nrows, row_bytes; bool want; size_t off; };  // row_bytes: of one window
     Piece pc[6] = {{angles, rows, n * sizeof(float), true, 0},      {levels, rows, n * sizeof(float), levels != nullptr, 0},
                    {bins, rows, n * sizeof(int32_t), bins != nullptr, 0}, {counts, rows, sizeof(int32_t), counts != nullptr, 0},
-                   {spectrum, rows, K * sizeof(float), spectrum != nullptr, 0}, {R, C, mm2 * sizeof(double), R != nullptr, 0}};
+                   {spectrum, rows, K * sizeof(float), spectrum != nullptr, 0}, {R, r_rows, mm2 * sizeof(double), R != nullptr, 0}};
     size_t per_win = win_bytes;
     for (const Piece &p : pc) per_win += p.want ? p.nrows * p.row_bytes : 0;
     const uint32_t chunk = (uint32_t)std::max<size_t>(1, std::min<size_t>(nwindows, ((size_t)64 << 20) / per_win));
@@ -2778,6 +2935,7 @@ void music_b200_destroy(music_b200 *h)
     cudaFree(h->work_ctr);
     cudaFree(h->cal_acc); cudaFree(h->cal_part); cudaFree(h->cal_ctr); cudaFree(h->cal_out);
     cudaFree(h->chan_tw); cudaFree(h->chan_taper_d); cudaFree(h->chan_arena);
+    cudaFree(h->foc_T[0]); cudaFree(h->foc_T[1]); cudaFree(h->foc_lam); cudaFree(h->foc_B); cudaFree(h->foc_e2); cudaFree(h->foc_Rc);
     for (int i = 0; i < 2; ++i) { cudaFree(h->ctab_c64[i]); cudaFree(h->ctab_soa[i]); }
     cudaFree(h->steer_pos); cudaFree(h->steer_count); cudaFree(h->steer_list); cudaFree(h->steer_vals);
     if (h->fused_done) cudaEventDestroy(h->fused_done);

@@ -10,9 +10,14 @@ Each window is cut into nsamples / m / nfft segments, an nfft-point FFT filter b
 wavelength.  ``combine="separate"``: one direction-finding problem per channel; an output item holds the channels of one
 window, ``count * n`` angles, ``count * n`` levels and optionally ``count * resolution`` spectrum floats, channel by
 channel.  ``combine="incoherent"``: one incoherent wideband MUSIC spectrum per window; items as for :class:`music_doa`.
+``combine="coherent"``: every channel's covariance is focused onto the centre channel's frequency and summed, and each
+window is one ordinary problem on that sum and the centre channel's table; items as for :class:`music_doa`, and the
+root-MUSIC, ESPRIT, DML and refinement setters work.  ``set_focusing`` chooses the sector of grid bins the focusing
+matrices fit, ``focusing`` returns them and their errors.
 ``antenna_array`` holds m [x, y] positions in units of ``spacing`` metres.  Peak mode, estimator and source rule setters,
 the reducers, ``last_bins`` / ``last_counts`` and ``close`` are those of :class:`music_doa`; the modes that are not
-built for channels (root-MUSIC, ESPRIT, DML, refinement, beams, calibration, planar input) raise.
+built for channels (beams, calibration, planar input, and under "separate" / "incoherent" root-MUSIC, ESPRIT, DML and
+refinement) raise.
 """
 from __future__ import annotations
 
@@ -25,7 +30,7 @@ from . import _capi
 from .music_doa import _table_c64, _uid, _uid_lock, music_doa
 
 TAPERS = {"rect": 0, "hann": 1}
-COMBINES = {"separate": 0, "incoherent": 1}
+COMBINES = {"separate": 0, "incoherent": 1, "coherent": 2}
 
 
 class music_doa_channels(music_doa):
@@ -59,7 +64,7 @@ class music_doa_channels(music_doa):
 
     @property
     def rows(self):
-        """channel blocks per output item: the channel count under "separate", 1 under "incoherent" """
+        """channel blocks per output item: the channel count under "separate", 1 under "incoherent" and "coherent" """
         return self.chan_count if self.combine == "separate" else 1
 
     def output_signature(self):
@@ -80,6 +85,17 @@ class music_doa_channels(music_doa):
         table = _table_c64(array_response, self.resolution, self.m)
         _capi.check(self._lib.music_b200_set_table(self._h, table.ctypes.data), self._h)
 
+    def set_focusing(self, first_bin, bin_count):
+        """coherent: fit the focusing matrices on grid bins (first_bin + i) mod resolution, i < bin_count"""
+        _capi.check(self._lib.music_b200_set_focusing(self._h, int(first_bin), int(bin_count)), self._h)
+
+    def focusing(self):
+        """coherent: (T complex128 (count, m, m), err float64 (count,)), the focusing matrices and their errors"""
+        T = np.empty((self.chan_count, self.m, self.m), np.complex128)
+        err = np.empty(self.chan_count, np.float64)
+        _capi.check(self._lib.music_b200_get_focusing(self._h, T.ctypes.data, err.ctypes.data), self._h)
+        return T, err
+
     def channel_frequencies(self):
         """float64 (count,): each channel's frequency offset from the centre frequency in Hz"""
         f = np.empty(self.chan_count, np.float64)
@@ -96,7 +112,8 @@ class music_doa_channels(music_doa):
 
     def process_host(self, x, nwindows, levels=True, spectrum=False, bins=True, counts=False, R=False):
         """The host entry on complex64 windows x, results in the C ABI's channel-major layout: a dict of angles / levels /
-        bins (rows, W, n), counts (rows, W), spectrum (rows, W, resolution), R (count, W, m, m) complex128."""
+        bins (rows, W, n), counts (rows, W), spectrum (rows, W, resolution), R (count, W, m, m) complex128, under
+        "coherent" the focused covariances (W, m, m)."""
         W, r, n, m = int(nwindows), self.rows, self.n, self.m
         if x.dtype != np.complex64 or not x.flags["C_CONTIGUOUS"] or x.size < W * self.nsamples:
             raise ValueError("x must be C-contiguous complex64 with >= nwindows*nsamples elements")
@@ -110,7 +127,7 @@ class music_doa_channels(music_doa):
         if counts:
             out["counts"] = np.zeros((r, W), np.int32)
         if R:
-            out["R"] = np.zeros((self.chan_count, W, m, m), np.complex128)
+            out["R"] = np.zeros((W, m, m) if self.combine == "coherent" else (self.chan_count, W, m, m), np.complex128)
         p = lambda k: out[k].ctypes.data if k in out else None
         rc = self._lib.music_b200_process_channels_host(self._h, x.ctypes.data, W, p("angles"), p("levels"), p("spectrum"), p("bins"),
                                                         p("counts"), p("R"))
@@ -131,12 +148,12 @@ class music_doa_channels(music_doa):
         for o, s in zip(outs, [r * self.n, r * self.n, r * self.resolution]):
             if o.dtype != np.float32 or not o.flags["C_CONTIGUOUS"] or o.size < W * s:
                 raise ValueError("output buffers must be C-contiguous float32 of the port's item size")
-        res = self.process_host(input_items[0], W, levels=len(outs) > 1, spectrum=len(outs) > 2, counts=self.combine == "separate")
+        res = self.process_host(input_items[0], W, levels=len(outs) > 1, spectrum=len(outs) > 2, counts=self.combine != "incoherent")
         for o, k in zip(outs, ["angles", "levels", "spectrum"]):
             a = res[k]
             o.reshape(-1)[: a.size].reshape(W, r, a.shape[2])[...] = a.transpose(1, 0, 2)
         self._last_bins = np.ascontiguousarray(res["bins"].transpose(1, 0, 2))          # (W, rows, n)
-        self._last_counts = np.ascontiguousarray(res["counts"].T) if "counts" in res else None  # (W, count)
+        self._last_counts = np.ascontiguousarray(res["counts"].T) if "counts" in res else None  # (W, rows)
         return W
 
     def process_device(self, d_in, nwindows, d_angles, d_levels=None, d_spectrum=None, d_bins=None, d_counts=None, d_R=None,

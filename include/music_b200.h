@@ -557,15 +557,42 @@ int music_b200_process_azel_device(music_b200 *h, const float *d_in_c64, uint32_
  *              c's MUSIC strength with its own table, i.e. 1 / sum_c ||G_c^H a_c(theta_k)||^2, summed in channel order;
  *              then the peak mode on P.  MUSIC estimator and FIXED rule only.  angles / levels / bins [W][n],
  *              spectrum [W][K], counts must be NULL.
- *   R          (either rule, may be NULL) [C][W][m][m] complex fp64.
- * Not built, and refused with EINVAL rather than ignored: the ROOTS, ESPRIT and DML peak modes, refinement, beams
+ *   COHERENT   (the coherent signal-subspace method, Wang and Kaveh 1985, with the rotational focusing matrices of Hung and
+ *              Kaveh 1988) one ordinary problem per window on a focused covariance:
+ *     reference  channel c_ref = C / 2 (integer division) at lambda_ref = lambda_{c_ref}; its table is the reference table.
+ *     sector     grid bins S = {(first + i) mod K : i < count}, the whole grid (0, K) unless music_b200_set_focusing()
+ *                chose another; the sector persists across set_geometry_channels() retunes.
+ *     steering   fp64 vectors from the geometry (not the float tables): a_c(theta)[r] = exp(-j 2 pi <p_r, u(theta)> / lambda_c).
+ *     focusing   B_c = sum_{k in S} a_ref(theta_k) a_c(theta_k)^H + beta |S| I, beta = 1e-3; T_c = U V^H from the SVD
+ *                B_c = U S V^H, the unitary minimiser of sum_k ||a_ref - T a_c||^2; T_{c_ref} = I exactly (not computed).
+ *                beta keeps T_c unique on sectors narrower than the array's degrees of freedom.  When
+ *                sigma_min(B_c) <= 1e-12 sigma_max(B_c) for some c, set_geometry_channels() / set_focusing() return EINVAL
+ *                and name the channel; the handle keeps its previous matrices.  The matrices are built on every
+ *                set_geometry_channels() and set_focusing(), in the idle table slot beside its channel tables, which then
+ *                becomes current (set_focusing() copies the current tables into it), after a device synchronise as in
+ *                every table setter.
+ *     error      e_c = ||T_c A_c - A_ref||_F / ||A_ref||_F over the columns a(theta_k), k in S (music_b200_get_focusing).
+ *     covariance R_foc = (1 / C) sum_c T_c R_c T_c^H in fp64, summed in channel order, the c_ref term R_ref itself (added
+ *                without multiplication); upper triangle as summed, lower triangle its mirror, diagonal real.
+ *     problem    (R_foc, reference table) with J * C looks in place of N (MDL, AIC and the N <= m conditions): estimator
+ *                MUSIC / MVDR / BARTLETT, peak mode TOP_BINS / LOCAL_MAXIMA / ROOTS / ESPRIT / DML (ROOTS and ESPRIT need
+ *                a ULA with spacing <= lambda_ref / 2), source rule FIXED / MDL / AIC, refinement OFF / NEWTON on the
+ *                reference geometry.  With C = 1 every output equals SEPARATE's.
+ *     outputs    angles / levels / bins [W][n], spectrum [W][K], counts [W], R [W][m][m] holding R_foc.
+ *     caveat     the focusing error moves signal power into the noise eigenvalues, so MDL and AIC over-count at high
+ *                SNR (in a two-path UCA-8 case at 20 dB per element, MDL gave 4 for 2).
+ *              music_b200_set_table() is refused on a COHERENT handle (one shared table gives no focusing).
+ *   R          (SEPARATE, INCOHERENT, may be NULL) [C][W][m][m] complex fp64.
+ * Not built, and refused with EINVAL rather than ignored: under SEPARATE and INCOHERENT the ROOTS, ESPRIT and DML peak modes and refinement; on every channel handle beams
  * (set_beamformer), calibration (set_calibration and the calib entries), the planar, sharded, gather and az-el entries and
  * set_geometry() on a channel handle; create_multi() makes no channel handle.  The plain process entries on a channel
  * handle and the channel entries on a plain handle return EINVAL.  Segments do not overlap.
  * A call runs, per sub-batch: chan_cov_kernel (the filter bank and all C covariances, one read of the input per channel
  * group; timed in the covariance slot of the stage timing), then the eigensolver, source count and MVDR preparation of the
  * plain unfused path once over all C * W (window, channel) pairs, then one scan and one peak-rule launch per channel on
- * that channel's table, and under INCOHERENT one combine kernel and one peak-rule launch.  set_estimator, set_peak_mode,
+ * that channel's table, and under INCOHERENT one combine kernel and one peak-rule launch.  Under COHERENT a sub-batch runs
+ * chan_cov_kernel, chan_focus_kernel (timed in the covariance slot) and the plain unfused stages once over its W focused
+ * covariances, whatever C is.  set_estimator, set_peak_mode,
  * set_source_rule, stage timing, the reducers and launch_count work as on any handle.
  * The device entry is enqueued on `stream` and does not synchronise; d_in must be 16-byte aligned.  The host entry copies
  * in chunks and returns when done.
@@ -574,12 +601,18 @@ int music_b200_process_azel_device(music_b200 *h, const float *d_in_c64, uint32_
 #define MUSIC_B200_TAPER_HANN 1
 #define MUSIC_B200_CHANNELS_SEPARATE 0
 #define MUSIC_B200_CHANNELS_INCOHERENT 1
+#define MUSIC_B200_CHANNELS_COHERENT 2
 int music_b200_create_channels(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples, uint32_t resolution, uint32_t nfft,
                                uint32_t chan_first, uint32_t chan_count, int taper, int combine, int device);
 int music_b200_set_geometry_channels(music_b200 *h, const double *positions_xy /* [m][2] */, double centre_frequency_hz,
                                      double sample_rate_hz);
 int music_b200_channel_frequencies(music_b200 *h, double *offsets_hz /* [C] */);
 int music_b200_get_table_channel(music_b200 *h, uint32_t channel, float *table_c64);
+/* COHERENT handles only (EINVAL otherwise).  set_focusing: the sector (1 <= bin_count <= K, first_bin < K), rebuilding the
+ * matrices when a geometry exists.  get_focusing: T [C][m][m] complex fp64 and e_c [C] (either may be NULL); EINVAL
+ * before set_geometry_channels(). */
+int music_b200_set_focusing(music_b200 *h, uint32_t first_bin, uint32_t bin_count);
+int music_b200_get_focusing(music_b200 *h, double *T, double *err);
 int music_b200_process_channels_device(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_angles, float *d_levels,
                                        float *d_spectrum, int32_t *d_bins, int32_t *d_counts, double *d_R, void *stream);
 int music_b200_process_channels_host(music_b200 *h, const float *in_c64, uint32_t nwindows, float *angles, float *levels,

@@ -51,7 +51,7 @@ baz_music_doa_channels::baz_music_doa_channels(unsigned int m, unsigned int n, u
     : gr::sync_block("music_doa_channels", gr::io_signature::make(1, 1, nsamples * sizeof(gr_complex)),
                      gr::io_signature::makev(1, 3, output_sizes(rows_of(chan_count, combine), n, resolution))),
       d_m(m), d_n(n), d_resolution(resolution), d_chan_count(chan_count), d_rows(rows_of(chan_count, combine)),
-      d_separate(combine == MUSIC_B200_CHANNELS_SEPARATE), d_handle(NULL)
+      d_counted(combine != MUSIC_B200_CHANNELS_INCOHERENT), d_handle(NULL)
 {
     const int rc = music_b200_create_channels(&d_handle, m, n, nsamples, resolution, nfft, chan_first, chan_count, taper, combine,
                                               device_from_env());
@@ -111,6 +111,22 @@ void baz_music_doa_channels::set_estimator(int estimator, double loading)
     if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa_channels: ") + music_b200_last_error(d_handle));
 }
 
+void baz_music_doa_channels::set_focusing(unsigned int first_bin, unsigned int bin_count)
+{
+    gr::thread::scoped_lock guard(d_mutex);
+    const int rc = music_b200_set_focusing(d_handle, first_bin, bin_count);
+    if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa_channels: ") + music_b200_last_error(d_handle));
+}
+
+std::vector<double> baz_music_doa_channels::focusing_error()
+{
+    std::vector<double> e(d_chan_count);
+    gr::thread::scoped_lock guard(d_mutex);
+    const int rc = music_b200_get_focusing(d_handle, NULL, e.data());
+    if (rc != MUSIC_B200_OK) throw std::runtime_error(std::string("music_doa_channels: ") + music_b200_last_error(d_handle));
+    return e;
+}
+
 std::vector<double> baz_music_doa_channels::channel_frequencies()
 {
     std::vector<double> f(d_chan_count);
@@ -138,13 +154,13 @@ int baz_music_doa_channels::work(int noutput_items, gr_vector_const_void_star &i
     const bool lvl = output_items.size() > 1, spec = output_items.size() > 2;
 
     gr::thread::scoped_lock guard(d_mutex);
-    /* staging: angles, levels, then the spectrum rows; bins, then the counts (the separate rule only) */
+    /* staging: angles, levels, then the spectrum rows; bins, then the counts (not under the incoherent rule) */
     d_stage.resize(W * (2 * rn + (spec ? rk : 0)));
     d_istage.resize(W * (rn + d_rows));
     float *s_ang = d_stage.data(), *s_lvl = s_ang + W * rn, *s_spec = s_lvl + W * rn;
     int *s_bins = d_istage.data(), *s_cnt = s_bins + W * rn;
     const int rc = music_b200_process_channels_host(d_handle, in, (uint32_t)W, s_ang, lvl ? s_lvl : NULL, spec ? s_spec : NULL, s_bins,
-                                                    d_separate ? s_cnt : NULL, NULL);
+                                                    d_counted ? s_cnt : NULL, NULL);
     if (rc != MUSIC_B200_OK) throw std::runtime_error(std::string("music_doa_channels: ") + music_b200_last_error(d_handle));
     to_items(s_ang, static_cast<float *>(output_items[0]), d_rows, W, d_n);
     if (lvl) to_items(s_lvl, static_cast<float *>(output_items[1]), d_rows, W, d_n);
@@ -152,7 +168,7 @@ int baz_music_doa_channels::work(int noutput_items, gr_vector_const_void_star &i
     d_bins.resize(W * rn);
     to_items(s_bins, d_bins.data(), d_rows, W, d_n);
     d_counts.clear();
-    if (d_separate) {
+    if (d_counted) {
         d_counts.resize(W * d_rows);
         to_items(s_cnt, d_counts.data(), d_rows, W, 1);
     }
