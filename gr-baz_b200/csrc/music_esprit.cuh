@@ -5,9 +5,9 @@
 // same row blocks of E_s, Psi = (E1^H E1)^-1 E1^H E2 is similar to diag(z0_k): its d eigenvalues give the d directions
 // with no grid, no polynomial and no root selection.  E_s is orthonormal, so E1^H E1 = I - r^H r with r = the last row
 // of E_s, and Sherman-Morrison gives the inverse I + r^H r / (1 - |r|^2) without a factorisation.  The eigenvalues of
-// Psi come from a Householder reduction to Hessenberg form and single-shift complex QR steps (Wilkinson shifts,
-// deflation on a negligible subdiagonal).  The full definition (angles, levels, bins, slot order) is in
-// include/music_b200.h and is restated by tests/esprit_oracle.py.
+// Psi come from a Householder reduction to Hessenberg form and single-shift complex QR steps (Wilkinson shifts, an
+// exceptional shift at the 10th and 20th step without a deflation, deflation on a negligible subdiagonal).  The full
+// definition (angles, levels, bins, slot order) is in include/music_b200.h and is restated by tests/esprit_oracle.py.
 //
 // One warp per window; Psi (d x d, d <= 15) lives in the warp's shared memory, lane j <-> column j (or row j) in each
 // update.  Everything is fp64.
@@ -20,6 +20,12 @@ constexpr int ESPRIT_WARPS = 4;
 constexpr int ESPRIT_LD = MAXM;                       // row stride of the per-warp matrix
 constexpr int ESPRIT_MAX_IT = 30;                     // QR steps allowed between two deflations
 constexpr double ESPRIT_EPS = 2.220446049250313e-16;  // 2^-52: a subdiagonal this small (relative) is negligible
+constexpr int ESPRIT_EXC_EVERY = 10;                  // exceptional shifts at the 10th and 20th step without a deflation
+constexpr double ESPRIT_EXC_SCALE = 0.75;             // their size, in units of the subdiagonal (zlahqr's dat1);
+                                                      // anchored at h_hi,hi at step 10 and at h_l,l at step 20
+// their direction: the unit vector (0.6, 0.8), whose angle is no rational multiple of pi, so that no arrangement of
+// roots of unity around the diagonal entry is equally far from it
+constexpr double ESPRIT_EXC_RE = 0.6, ESPRIT_EXC_IM = 0.8;
 
 __device__ __forceinline__ double cabs2(double2 a) { return a.x * a.x + a.y * a.y; }
 __device__ __forceinline__ double2 cconj(double2 a) { return make_double2(a.x, -a.y); }
@@ -75,17 +81,27 @@ __device__ bool esprit_eigvals(double2 *A, double2 *v, double2 *g, double2 *ev, 
             continue;
         }
         if (++its > ESPRIT_MAX_IT) return false;
-        // Wilkinson shift: the eigenvalue of the trailing 2 x 2 block [a b; c e] nearer to e, e - bc / (p +- sqrt(p^2 + bc))
-        const double2 a = A[(hi - 1) * ESPRIT_LD + hi - 1], b = A[(hi - 1) * ESPRIT_LD + hi];
-        const double2 c = A[hi * ESPRIT_LD + hi - 1], e = A[hi * ESPRIT_LD + hi];
-        const double2 p = cscale(csub(a, e), 0.5), bc = cmul(b, c), q = cadd(cmul(p, p), bc);
-        const double qa = sqrt(cabs2(q)), ar = atan2(q.y, q.x) * 0.5;
-        double sr, cr;
-        sincos(ar, &sr, &cr);
-        double2 sq = make_double2(sqrt(qa) * cr, sqrt(qa) * sr);
-        if (p.x * sq.x + p.y * sq.y < 0.0) sq = cscale(sq, -1.0);
-        const double2 den = cadd(p, sq);
-        const double2 mu = cabs2(den) > 0.0 ? csub(e, cdiv(bc, den)) : e;
+        double2 mu;
+        if (its % ESPRIT_EXC_EVERY == 0 && its < ESPRIT_MAX_IT) {
+            // exceptional shift (after LAPACK zlahqr, which anchors them the other way round): Wilkinson shifts stall on
+            // a Psi whose trailing eigenvalues are all equally far from the shift, e.g. the phase-weighted cyclic
+            // permutation of equally spaced sources
+            const int k = its == ESPRIT_EXC_EVERY ? hi : l;
+            const double h = sqrt(cabs2(k == hi ? A[hi * ESPRIT_LD + hi - 1] : A[(l + 1) * ESPRIT_LD + l]));
+            mu = cadd(A[k * ESPRIT_LD + k], cscale(make_double2(ESPRIT_EXC_RE, ESPRIT_EXC_IM), ESPRIT_EXC_SCALE * h));
+        } else {
+            // Wilkinson shift: the eigenvalue of the trailing 2 x 2 block [a b; c e] nearer to e, e - bc / (p +- sqrt(p^2 + bc))
+            const double2 a = A[(hi - 1) * ESPRIT_LD + hi - 1], b = A[(hi - 1) * ESPRIT_LD + hi];
+            const double2 c = A[hi * ESPRIT_LD + hi - 1], e = A[hi * ESPRIT_LD + hi];
+            const double2 p = cscale(csub(a, e), 0.5), bc = cmul(b, c), q = cadd(cmul(p, p), bc);
+            const double qa = sqrt(cabs2(q)), ar = atan2(q.y, q.x) * 0.5;
+            double sr, cr;
+            sincos(ar, &sr, &cr);
+            double2 sq = make_double2(sqrt(qa) * cr, sqrt(qa) * sr);
+            if (p.x * sq.x + p.y * sq.y < 0.0) sq = cscale(sq, -1.0);
+            const double2 den = cadd(p, sq);
+            mu = cabs2(den) > 0.0 ? csub(e, cdiv(bc, den)) : e;
+        }
         __syncwarp();
         if (lane >= l && lane <= hi) A[lane * ESPRIT_LD + lane] = csub(A[lane * ESPRIT_LD + lane], mu);
         __syncwarp();

@@ -25,7 +25,8 @@ struct UlaGeom {
 constexpr int ROOTS_WARPS = 4;
 constexpr int ROOTS_MAX_IT = 100;
 constexpr double ROOTS_EPS = 2.220446049250313e-16;  // 2^-52
-constexpr double ROOTS_STOP = 4.0 * ROOTS_EPS;        // stop once every correction is <= 4 ulps of |z|
+constexpr double ROOTS_STOP = 4.0 * ROOTS_EPS;        // a lane stops once its correction is <= 4 ulps of |z|,
+constexpr double ROOTS_BACK = 8.0;                    // or once |Q(z)| <= ROOTS_BACK P eps sum_k |b_k| |z|^k
 constexpr double ROOTS_MERGE = 1e-6;                  // two roots this close (relative) are one double root
 
 __device__ __forceinline__ double2 cdiv(double2 a, double2 b)
@@ -97,21 +98,55 @@ __global__ void __launch_bounds__(ROOTS_WARPS * 32) roots_kernel(const double *_
     double2 z = make_double2(0.0, 0.0);
     bool ok = finite && d > 0 && P > 0;
     if (ok) {
+        // starting points on the circles of the Newton polygon (Bini): the upper convex hull of (k, log2 |b_k|), with
+        // |b_k| = |c_{|k - H|}|, every lane building the same hull; the roots of hull segment [i, j) start on the circle
+        // of radius (|b_i| / |b_j|)^(1 / (j - i)), so that roots decades away from the unit circle start near it
+        const double lgc = (lane < M && (c.x != 0.0 || c.y != 0.0)) ? log2(hypot(c.x, c.y)) : -INFINITY;
+        int hull[32], nh = 1;
+        hull[0] = 0;
+        for (int k = 1; k <= P; ++k) {
+            const double lk = __shfl_sync(0xffffffffu, lgc, k >= H ? k - H : H - k);
+            if (lk == -INFINITY) continue;
+            while (nh >= 2) {
+                const int i = hull[nh - 2], j = hull[nh - 1];
+                const double li = __shfl_sync(0xffffffffu, lgc, i >= H ? i - H : H - i);
+                const double lj = __shfl_sync(0xffffffffu, lgc, j >= H ? j - H : H - j);
+                if ((lj - li) * (k - i) <= (lk - li) * (j - i)) --nh;  // j on or below the chord i -> k
+                else break;
+            }
+            hull[nh++] = k;
+        }
+        int si = 0;
+        while (si + 2 < nh && hull[si + 1] <= lane) ++si;
+        const int i0 = hull[si], j0 = hull[si + 1];
+        const double li = __shfl_sync(0xffffffffu, lgc, i0 >= H ? i0 - H : H - i0);
+        const double lj = __shfl_sync(0xffffffffu, lgc, j0 >= H ? j0 - H : H - j0);
+        const double u = exp2((li - lj) / (j0 - i0));
         double sn, cs;
-        sincospi(2.0 * lane / P + 0.5 / P, &sn, &cs);
-        z = make_double2(cs, sn);
+        sincospi(2.0 * (lane - i0) / (j0 - i0) + 2.0 * i0 / P + 0.5 / P, &sn, &cs);
+        z = make_double2(u * cs, u * sn);
+        bool done = lane >= P, conv = false;
         for (int it = 0; it < ROOTS_MAX_IT; ++it) {
-            // Horner for Q and Q' (coefficients broadcast from the lanes that built them)
-            double2 q = shfl2(c, H), dq = make_double2(0.0, 0.0);  // b_P = c_H
-            for (int k = P - 1; k >= 0; --k) {
-                const int l = k - H;
+            // Horner for Q and Q' (coefficients broadcast from the lanes that built them); outside the unit circle for
+            // R(w) = w^P Q(1 / w) and R' at w = 1 / z instead, so that no power of z overflows.  acc = sum_k |b_k| |w|^k
+            const bool outside = z.x * z.x + z.y * z.y > 1.0;
+            const double2 w = outside ? cdiv(make_double2(1.0, 0.0), z) : z;
+            const double aw = hypot(w.x, w.y);
+            double2 q = shfl2(c, H), dq = make_double2(0.0, 0.0);  // b_0 = conj(c_H), b_P = c_H: equal modulus
+            if (outside) q.y = -q.y;
+            double acc = hypot(q.x, q.y);
+            for (int k = 1; k <= P; ++k) {
+                const int l = (outside ? k : P - k) - H;
                 double2 b = shfl2(c, l >= 0 ? l : -l);
                 if (l < 0) b.y = -b.y;
-                dq = cmul(dq, z);
+                dq = cmul(dq, w);
                 dq.x += q.x; dq.y += q.y;
-                q = cmul(q, z);
+                q = cmul(q, w);
                 q.x += b.x; q.y += b.y;
+                acc = acc * aw + hypot(b.x, b.y);
             }
+            // a lane whose residual is at rounding level holds an exact root of a polynomial within that rounding
+            if (hypot(q.x, q.y) <= ROOTS_BACK * P * ROOTS_EPS * acc) done = true;
             // Aberth term sum_{s != r} 1 / (z_r - z_s)
             double2 S = make_double2(0.0, 0.0);
             for (int s = 0; s < P; ++s) {
@@ -122,15 +157,28 @@ __global__ void __launch_bounds__(ROOTS_WARPS * 32) roots_kernel(const double *_
                     S.y -= dy * r;
                 }
             }
-            // Aberth correction N / (1 - N S) with N = Q / Q', as one division: Q / (Q' - Q S)
-            const double2 qS = cmul(q, S);
-            const double2 wc = cdiv(q, make_double2(dq.x - qS.x, dq.y - qS.y));
-            z.x -= wc.x;
-            z.y -= wc.y;
-            const bool conv = lane >= P || wc.x * wc.x + wc.y * wc.y <= ROOTS_STOP * ROOTS_STOP * (z.x * z.x + z.y * z.y);
-            if (__all_sync(0xffffffffu, conv)) break;
+            // Aberth correction N / (1 - N S) with N = Q / Q', as one division: Q / (Q' - Q S); outside, N = z R / (P R -
+            // w R'), so z R / (P R - w R' - z R S)
+            double2 wc;
+            if (outside) {
+                const double2 num = cmul(z, q), nS = cmul(num, S), wd = cmul(w, dq);
+                wc = cdiv(num, make_double2(P * q.x - wd.x - nS.x, P * q.y - wd.y - nS.y));
+            } else {
+                const double2 qS = cmul(q, S);
+                wc = cdiv(q, make_double2(dq.x - qS.x, dq.y - qS.y));
+            }
+            if (!done) {  // a converged lane stays put
+                z.x -= wc.x;
+                z.y -= wc.y;
+                done = wc.x * wc.x + wc.y * wc.y <= ROOTS_STOP * ROOTS_STOP * (z.x * z.x + z.y * z.y);
+            }
+            if (__all_sync(0xffffffffu, done)) {
+                conv = true;
+                break;
+            }
         }
-        ok = __all_sync(0xffffffffu, lane >= P || (isfinite(z.x) && isfinite(z.y)));
+        // a window whose iteration has not converged in ROOTS_MAX_IT steps reports no peaks
+        ok = conv && __all_sync(0xffffffffu, lane >= P || (isfinite(z.x) && isfinite(z.y)));
     }
 
     // a double root on the unit circle (the two approximants are each other's nearest root, closer than

@@ -125,7 +125,10 @@ int music_b200_set_table(music_b200 *h, const float *table_c64);
  *              c_l = sum_{j - i = l} C_ij (l = -(M-1) .. M-1, c_{-l} = conj(c_l)), Q(z) = sum_l c_l z^(l + M - 1), so that
  *              D(t) = sum_l c_l z0^l with z0 = exp(-j 2 pi (s . u(t)) / lambda), all fp64.  Each outermost pair
  *              c_{+-l} that is exactly zero contributes a root at 0 and one at infinity.
- *   roots      Aberth-Ehrlich iteration in fp64 (starting points on the unit circle, at most 100 steps).  Two roots that
+ *   roots      Aberth-Ehrlich iteration in fp64: starting points on the circles of the Newton polygon of |b_k| (Bini),
+ *              evaluation in 1 / z outside the unit circle (no power of z overflows), a root done once its correction is
+ *              within 4 ulps of |z| or |Q(z)| <= 8 (2M - 2) 2^-52 sum_k |b_k| |z|^k; a window whose roots are not all done
+ *              after 100 steps reports no peaks.  Two roots that
  *              are each other's nearest and closer than 1e-6 max(|z_a|, |z_b|) are one double root on the unit circle
  *              (D >= 0 there, so a root on the circle has even multiplicity): both become their midpoint, with modulus
  *              taken as 1, and the copy of the higher index sorts after every other root of modulus 1.
@@ -156,7 +159,8 @@ int music_b200_set_table(music_b200 *h, const float *table_c64);
  *              finite report no peaks.  (E1^H E1 = I - r^H r with r = the last row of E_s, so the condition is
  *              |r|^2 < 1, and the inverse is I + r^H r / (1 - |r|^2).)
  *   eigenvalues  phi_1 .. phi_d of Psi in fp64: Householder reduction to Hessenberg form, then single-shift complex QR
- *              with Wilkinson shifts, deflating a subdiagonal h_{l,l-1} once |h_{l,l-1}| <= 2^-52 (|h_{l-1,l-1}| +
+ *              with Wilkinson shifts (exceptional shifts h + 0.75 |h_sub| (0.6 + 0.8 j) at the 10th and 20th step
+ *              without a deflation, after LAPACK zlahqr), deflating a subdiagonal h_{l,l-1} once |h_{l,l-1}| <= 2^-52 (|h_{l-1,l-1}| +
  *              |h_{l,l}|); a window that needs more than 30 QR steps between two deflations reports no peaks.  On a ULA
  *              each phi is z0 = exp(-j 2 pi (s . u) / lambda) of one source, the z of ROOTS.
  *   outputs    each eigenvalue phi gives t* by ROOTS's angle rule (z = phi), level = (float)(1 / D(t*)) with D the direct
