@@ -47,6 +47,52 @@ namespace {
 std::mutex g_err_mutex;
 std::string g_create_error;
 
+cudaError_t pinned_alloc(void **p, size_t bytes) { return cudaHostAlloc(p, bytes, cudaHostAllocDefault); }
+
+// The owner of one allocation of T elements made by Alloc and released by Free.  Every owner of a handle is destroyed
+// while the handle's device is current (music_b200_destroy).
+template <class T, cudaError_t (*Alloc)(void **, size_t), cudaError_t (*Free)(void *)>
+class Owned {
+public:
+    Owned() = default;
+    Owned(Owned &&o) noexcept { *this = std::move(o); }
+    Owned &operator=(Owned &&o) noexcept
+    {
+        reset();
+        std::swap(p_, o.p_);
+        std::swap(n_, o.n_);
+        return *this;
+    }
+    ~Owned() { reset(); }
+    // Holds at least n elements afterwards; the old block is freed before the new one is allocated, so a grow never
+    // holds both.  The contents are not kept.  On failure the owner is empty.
+    cudaError_t grow(size_t n)
+    {
+        if (n <= n_) return cudaSuccess;
+        reset();
+        void *p = nullptr;
+        const cudaError_t e = Alloc(&p, n * sizeof(T));
+        if (e == cudaSuccess) { p_ = static_cast<T *>(p); n_ = n; }
+        return e;
+    }
+    size_t size() const { return n_; }
+    T *get() const { return p_; }
+    operator T *() const { return p_; }
+private:
+    void reset()
+    {
+        if (p_) Free(p_);
+        p_ = nullptr;
+        n_ = 0;
+    }
+    T *p_ = nullptr;
+    size_t n_ = 0;
+};
+
+template <class T> using DevBuf = Owned<T, cudaMalloc, cudaFree>;
+template <class T> using PinBuf = Owned<T, pinned_alloc, cudaFreeHost>;
+
+// A view of one steering table; the buffers belong to its TableSlot.
 struct DeviceTable {
     float *c64 = nullptr;   // [K][M] (re, im)
     double *soa = nullptr;  // [ntiles][2M+1][TILE]
@@ -59,14 +105,31 @@ struct DeviceTable {
     UlaGeom ula = {};             // whether `geo` is a uniform linear array the root mode accepts, and its p_0 and step
 };
 
+// One slot of the steering-table double buffer (retune()).  `tabs` holds C tables (C: the channel count on a channel
+// handle, 1 on every other handle) as views into one c64 and one SoA allocation; it is empty until the slot is first
+// used (alloc_slot).
+struct TableSlot {
+    std::vector<DeviceTable> tabs;
+    DevBuf<float> c64;
+    DevBuf<double> soa;
+    DevBuf<unsigned char> fz;  // the fused M = 4 kernel's screen layout of tabs[0], on the handles that run that kernel
+    DevBuf<float> na_max;
+    bool shared = false;       // one table from set_table() (tabs[0]) serves every channel
+    DevBuf<double2> foc_T;     // COHERENT channel handle: the focusing matrices T_c [C][m][m] of these tables
+    std::vector<double> foc_err;  // and their focusing errors e_c
+};
+
+// A non-owning view of a workspace slot's buffers, or of one channel's run of them (enqueue_channels)
+struct WsView { double *R, *ev, *Vt, *P64; int32_t *cnt, *bins; double *wts; };
+
 struct Workspace {
-    double *R = nullptr, *ev = nullptr, *Vt = nullptr, *P64 = nullptr;
-    int32_t *cnt = nullptr;  // per-window source counts (source rule other than FIXED)
-    int32_t *bins = nullptr; // [cap][n] peak bins for the refinement and the beams when the caller asked for none
-    double *wts = nullptr;   // [cap][n][m] complex beam weights when a beams call asked for none
-    uint32_t cap = 0, p64_cap = 0, cnt_cap = 0, bins_cap = 0, wts_cap = 0;
+    DevBuf<double> R, ev, Vt, P64;
+    DevBuf<int32_t> cnt;   // per-window source counts (source rule other than FIXED)
+    DevBuf<int32_t> bins;  // [windows][n] peak bins for the refinement and the beams when the caller asked for none
+    DevBuf<double> wts;    // [windows][n][m] complex beam weights when a beams call asked for none
     cudaEvent_t scan_done = nullptr;
     bool used = false;
+    WsView view() const { return {R, ev, Vt, P64, cnt, bins, wts}; }
 };
 
 // The modes set by set_peak_mode(), set_refine() and set_estimator(); check_modes() says which combine.
@@ -137,13 +200,31 @@ struct Outputs {
     }
 };
 
+// the buffers behind a staging slot's outputs, on the device or pinned (the spectrum is staged on the device only)
+template <template <class> class Buf>
+struct StagedOutputs {
+    Buf<float> angles, elev, levels, spec, beams;
+    Buf<int32_t> bins, counts;
+    Buf<double> wts;
+
+    Outputs view(const music_b200 *h) const
+    {
+        Outputs o;
+        o.angles = angles; o.elev = elev; o.levels = levels; o.spec = spec;
+        o.beams = beams; o.bins = bins; o.counts = counts; o.wts = wts;
+        return o.shaped(h);
+    }
+};
+
 // One staging stream of the host entry points: the input and output buffers of a chunk, and which windows of the call
 // the pinned mirrors hold.  Device->host copies into caller memory would be synchronous when that memory is pageable
 // (numpy arrays, GNU Radio buffers) and stall the enqueue of the next chunk's upload, hence the pinned mirrors.
 struct HostSlot {
-    float *in = nullptr;
-    Outputs dev;   // device outputs (the spectrum only when a call asked for it)
-    Outputs pin;   // pinned host mirrors of dev's per-window outputs and of its beam and weight rows
+    DevBuf<float> in;
+    StagedOutputs<DevBuf> dbuf;
+    StagedOutputs<PinBuf> pbuf;
+    Outputs dev;   // views of dbuf: device outputs (the spectrum only when a call asked for it)
+    Outputs pin;   // views of pbuf: pinned host mirrors of dev's per-window outputs and of its beam and weight rows
     uint32_t w0 = 0, W = 0;  // W = 0: nothing pending
 };
 
@@ -158,12 +239,12 @@ struct music_b200 {
     std::string error;
     std::atomic<uint64_t> launches{0};
 
-    DeviceTable table[2];
+    TableSlot tables[2];
     int cur_table = 0;
-    double *steer_pos = nullptr;   // device copy of the element positions (set_geometry)
-    unsigned *steer_count = nullptr;
-    int *steer_list = nullptr;
-    float *steer_vals = nullptr;
+    DevBuf<double> steer_pos;      // device copy of the element positions (set_geometry)
+    DevBuf<unsigned> steer_count;
+    DevBuf<int> steer_list;
+    DevBuf<float> steer_vals;
     Modes modes;
     int source_rule = MUSIC_B200_SOURCES_FIXED;  // set_source_rule()
     int beam_rule = MUSIC_B200_BEAMS_OFF;        // set_beamformer(): read by the beams entry points only
@@ -174,54 +255,44 @@ struct music_b200 {
     double cal_g[2 * MUSIC_B200_MAX_M] = {};  // the gains as set
     // the calibration accumulator (music_b200_calib_*; the served device of a multi-device handle): sum of the raw R
     // over cal_windows windows, the accumulate kernel's per-CTA partial sums and counter, the solve kernel's result
-    double2 *cal_acc = nullptr, *cal_part = nullptr;
-    unsigned *cal_ctr = nullptr;
-    double *cal_out = nullptr;
+    DevBuf<double2> cal_acc, cal_part;
+    DevBuf<unsigned> cal_ctr;
+    DevBuf<double> cal_out;
     uint64_t cal_windows = 0;
     unsigned steer_guarded = 0;    // entries of the last built table re-evaluated with the host libm
     bool azel = false;             // music_b200_create_azel(): K = n_az * n_el rows, elevation-major (music_azel.cuh)
     AzelGrid grid = {};
-    // channel handle (music_b200_create_channels, music_channels.cuh): the filter bank's shape, its twiddle and taper
-    // tables, and per table slot the C per-channel tables (views into one c64 and one soa allocation per slot; a table
-    // from set_table() sits in entry 0 and serves every channel)
+    // channel handle (music_b200_create_channels, music_channels.cuh): the filter bank's shape and its twiddle and taper
+    // tables; the C per-channel tables are in the table slots, and create_channels() installs none
     bool chan = false;
     ChanShape cshape = {};
     int chan_taper = MUSIC_B200_TAPER_RECT, chan_combine = MUSIC_B200_CHANNELS_SEPARATE;
-    double2 *chan_tw = nullptr;
-    double *chan_taper_d = nullptr;
+    DevBuf<double2> chan_tw;
+    DevBuf<double> chan_taper_d;
     int chan_ctas = 1;             // resident CTAs of chan_cov_kernel per SM at this shape
-    std::vector<DeviceTable> ctab[2];
-    float *ctab_c64[2] = {nullptr, nullptr};
-    double *ctab_soa[2] = {nullptr, nullptr};
-    bool ctab_shared[2] = {false, false};
-    bool ctab_set = false;         // a table has been installed (create_channels() takes none)
     double chan_fs = 0.0;          // sample rate of the last set_geometry_channels() (0: none yet)
-    unsigned char *chan_arena = nullptr;  // device staging of the channel host entry
-    size_t chan_arena_cap = 0;
-    // COHERENT combine (music_focus.cuh): the focusing sector (count 0: the whole grid), per table slot the focusing
-    // matrices T_c [C][m][m] on the device and the focusing errors e_c, and the set-up scratch
+    DevBuf<unsigned char> chan_arena;  // device staging of the channel host entry
+    // COHERENT combine (music_focus.cuh): the focusing sector (count 0: the whole grid) and the set-up scratch; the
+    // focusing matrices and errors are in the table slots
     uint32_t foc_first = 0, foc_count = 0;
-    double2 *foc_T[2] = {nullptr, nullptr};
-    std::vector<double> foc_err[2];
-    double *foc_lam = nullptr;   // [C] the wavelengths of the slot being focused
-    double2 *foc_B = nullptr;    // [C][m][m] B_c
-    double *foc_e2 = nullptr;    // [C] squared focusing errors
-    double2 *foc_Rc = nullptr;   // the filter bank's [C][W][m][m] covariances of a sub-batch (the workspace holds W windows)
-    size_t foc_Rc_cap = 0;       // its capacity in C * W matrices
+    DevBuf<double> foc_lam;      // [C] the wavelengths of the slot being focused
+    DevBuf<double2> foc_B;       // [C][m][m] B_c
+    DevBuf<double> foc_e2;       // [C] squared focusing errors
+    DevBuf<double2> foc_Rc;      // the filter bank's [C][W][m][m] covariances of a sub-batch (the workspace holds W windows)
 
     // fp64 workspace slots (R, eigenvalues, sorted eigenvectors, optional strengths) of the unfused path: one per
     // staging stream of the host entry points (slot 0 also serves the device entry points)
     Workspace ws[2];
-    unsigned *work_ctr = nullptr;      // persistent kernels: ring of self-resetting (window tickets, finished CTAs) pairs, CTR_RING per slot
+    DevBuf<unsigned> work_ctr;         // persistent kernels: ring of self-resetting (window tickets, finished CTAs) pairs, CTR_RING per slot
     unsigned ctr_seq[2] = {0, 0};      // next ring entry per slot
     bool fused_spec = true;            // the spectrum port on the fused M = 4 kernel (MUSIC_B200_FUSED_SPEC=0: three-kernel path)
     bool pdl = true;                   // fused M = 4 kernel: programmatic dependent launch (MUSIC_B200_PDL=0 turns it off)
     cudaEvent_t fused_done = nullptr;  // orders persistent launches that share a ticket counter but not a stream
     bool fused_used[2] = {false, false};
     int eig_mode = 0;                 // fused kernels: 0 principal eigenvector by squaring (default), otherwise their Jacobi solver for every window (four lanes per window at M = 4, one warp at M = 8); MUSIC_B200_EIG=jacobi and the older spelling jacobi1 (2) both select it
-    unsigned *f8_stats = nullptr;     // fused M = 8 kernel: windows solved by squaring / by the Jacobi fallback
+    DevBuf<unsigned> f8_stats;        // fused M = 8 kernel: windows solved by squaring / by the Jacobi fallback
     int mma_fin_max = 2;              // fused kernel: no tensor-core pass starts once the tickets have run out and this many covariance warps are done (MUSIC_B200_MMA_FIN; 0: at ticket exhaustion, -1: fp64 drain only)
-    long long *fused_trace = nullptr;  // MUSIC_B200_TRACE=1: per-CTA clock64 trace of the fused kernel (tools/fused_trace.py)
+    DevBuf<long long> fused_trace;     // MUSIC_B200_TRACE=1: per-CTA clock64 trace of the fused kernel (tools/fused_trace.py)
     unsigned trace_seq = 0;            // next launch's slot in the trace ring (FZ_TRACE_LAUNCHES launches of FZ_TRACE_CTAS rows)
     bool fused = true;       // MUSIC_B200_FUSED=0 forces the three-kernel path
     // optional per-stage timing (bench.py's roofline leg): events around K1/K2/K3/top-n per chunk
@@ -246,14 +317,25 @@ struct music_b200 {
     // multi-device handle (music_b200_create_multi): one child per device, windows dealt w -> child w mod G
     std::vector<music_b200 *> kids;
 
-    // fused all-gather of the peak bins (music_b200_gather_*): peer-mapped buffers, epoch flags
-    int32_t *gather_buf = nullptr;
-    unsigned *gather_flags = nullptr;
+    // fused all-gather of the peak bins (music_b200_gather_*): peer-mapped buffers, epoch flags, and every IPC mapping of
+    // a peer's buffer or flags this handle has opened
+    DevBuf<int32_t> gather_buf;
+    DevBuf<unsigned> gather_flags;
     size_t gather_cap = 0;
     Gather gather;
     unsigned *peer_flags[MAX_PEERS] = {};
-    bool peer_ipc[MAX_PEERS] = {};
+    std::vector<void *> ipc_maps;
     unsigned gather_epoch = 0;
+
+    ~music_b200()
+    {
+        for (int i = 0; i < 2; ++i) {
+            if (streams[i]) cudaStreamDestroy(streams[i]);
+            if (ws[i].scan_done) cudaEventDestroy(ws[i].scan_done);
+        }
+        if (fused_done) cudaEventDestroy(fused_done);
+        for (cudaEvent_t e : tev) cudaEventDestroy(e);
+    }
 };
 
 namespace {
@@ -424,16 +506,22 @@ int check_modes(music_b200 *h, const Modes &p, const DeviceTable *t)
     return MUSIC_B200_OK;
 }
 
-// the table channel c of a channel handle scans with
-const DeviceTable &channel_table(const music_b200 *h, int c) { return h->ctab[h->cur_table][h->ctab_shared[h->cur_table] ? 0 : c]; }
+const TableSlot &cur_slot(const music_b200 *h) { return h->tables[h->cur_table]; }
 
-// The current table of a handle that holds one (a multi-device handle's children hold the copies).  On a channel handle:
-// the reference channel's (what a focused covariance is matched against), once there is one.
-const DeviceTable *own_table(const music_b200 *h)
+// Whether the current slot holds a table.  A channel handle has none until its first retune, a multi-device handle none
+// at all (its children hold the copies).
+bool has_table(const music_b200 *h) { return !cur_slot(h).tabs.empty(); }
+
+// the current table channel c scans with (c = 0 on a handle without channels)
+const DeviceTable &table(const music_b200 *h, int c = 0)
 {
-    if (h->chan) return h->ctab_set ? &channel_table(h, h->cshape.C / 2) : nullptr;
-    return h->kids.empty() ? &h->table[h->cur_table] : nullptr;
+    const TableSlot &s = cur_slot(h);
+    return s.tabs[s.shared ? 0 : c];
 }
+
+// The current table of a handle that holds one.  On a channel handle: the reference channel's (what a focused covariance
+// is matched against).
+const DeviceTable *own_table(const music_b200 *h) { return has_table(h) ? &table(h, h->chan ? h->cshape.C / 2 : 0) : nullptr; }
 
 // The handle that serves an entry point which a multi-device handle does not spread over its devices: device 0.
 music_b200 *served(music_b200 *h) { return h && !h->kids.empty() ? h->kids[0] : h; }
@@ -455,12 +543,10 @@ int build_table(music_b200 *h, DeviceTable &t, const double *pos_xy, double lamb
     const int K = (int)h->K, M = (int)h->m;
     t.geometric = false;
     t.screen_ok = true;  // unit-modulus rows: ||a||^2 = M
-    if (!h->steer_pos) {
-        CU(h, cudaMalloc(&h->steer_pos, sizeof(double) * 2 * MUSIC_B200_MAX_M));
-        CU(h, cudaMalloc(&h->steer_count, sizeof(unsigned)));
-        CU(h, cudaMalloc(&h->steer_list, sizeof(int) * STEER_GUARD_CAP));
-        CU(h, cudaMalloc(&h->steer_vals, sizeof(float) * 2 * STEER_GUARD_CAP));
-    }
+    CU(h, h->steer_pos.grow(2 * MUSIC_B200_MAX_M));
+    CU(h, h->steer_count.grow(1));
+    CU(h, h->steer_list.grow(STEER_GUARD_CAP));
+    CU(h, h->steer_vals.grow(2 * STEER_GUARD_CAP));
     CU(h, cudaMemcpyAsync(h->steer_pos, pos_xy, sizeof(double) * 2 * M, cudaMemcpyHostToDevice, st));
     CU(h, cudaMemsetAsync(h->steer_count, 0, sizeof(unsigned), st));
     steer_table_kernel<<<(K * M + 255) / 256, 256, 0, st>>>(h->steer_pos, lambda, K, M, reinterpret_cast<float2 *>(t.c64),
@@ -487,7 +573,7 @@ int build_table(music_b200 *h, DeviceTable &t, const double *pos_xy, double lamb
         for (unsigned i = 0; i < cnt; ++i) steer_entry_host(pos_xy, lambda, K, list[i] / M, list[i] % M, &vals[2 * i], &vals[2 * i + 1]);
         CU(h, cudaMemcpyAsync(h->steer_vals, vals.data(), vals.size() * sizeof(float), cudaMemcpyHostToDevice, st));
         steer_patch_kernel<<<(cnt + 255) / 256, 256, 0, st>>>(reinterpret_cast<float2 *>(t.c64), h->steer_list,
-                                                            reinterpret_cast<const float2 *>(h->steer_vals), (int)cnt);
+                                                            reinterpret_cast<const float2 *>(h->steer_vals.get()), (int)cnt);
         h->launches++;
         CU(h, cudaGetLastError());
         CU(h, cudaStreamSynchronize(st));  // vals is a local
@@ -503,9 +589,8 @@ int build_table(music_b200 *h, DeviceTable &t, const double *pos_xy, double lamb
 
 // Steering table of an az-el handle, built on the device from the element positions [M][x, y, z] (music_azel.cuh).
 // No host patching: the table is defined to within one float32 ulp, not bit for bit.
-int build_table_azel(music_b200 *h, int slot, const double *pos_xyz, double lambda, cudaStream_t st)
+int build_table_azel(music_b200 *h, DeviceTable &t, const double *pos_xyz, double lambda, cudaStream_t st)
 {
-    DeviceTable &t = h->table[slot];
     const int K = (int)h->K, M = (int)h->m;
     t.geometric = false;
     AzelGeom g = {};
@@ -652,42 +737,23 @@ uint32_t max_sub_windows(const music_b200 *h, const Plan &p)
 
 int ensure_slot(music_b200 *h, Workspace &ws, uint32_t windows, const Plan &p)
 {
-    if (windows > ws.cap) {
+    bool idle = !ws.used;
+    const auto grow = [&](auto &buf, size_t elems) -> int {
+        if (elems <= buf.size()) return MUSIC_B200_OK;
         // the slot may still be in use by an earlier call on another stream
-        if (ws.used) CU(h, cudaEventSynchronize(ws.scan_done));
-        cudaFree(ws.R); cudaFree(ws.ev); cudaFree(ws.Vt);
-        ws.R = ws.ev = ws.Vt = nullptr; ws.cap = 0;
-        const size_t mm = (size_t)h->m * h->m * 2;
-        CU(h, cudaMalloc(&ws.R, windows * mm * sizeof(double)));
-        CU(h, cudaMalloc(&ws.Vt, windows * mm * sizeof(double)));
-        CU(h, cudaMalloc(&ws.ev, (size_t)windows * h->m * sizeof(double)));
-        ws.cap = windows;
-    }
-    if (p.ws_p64 && windows > ws.p64_cap) {
-        if (ws.used) CU(h, cudaEventSynchronize(ws.scan_done));
-        cudaFree(ws.P64); ws.P64 = nullptr; ws.p64_cap = 0;
-        CU(h, cudaMalloc(&ws.P64, (size_t)windows * h->K * sizeof(double)));
-        ws.p64_cap = windows;
-    }
-    if (p.ws_counts && windows > ws.cnt_cap) {
-        if (ws.used) CU(h, cudaEventSynchronize(ws.scan_done));
-        cudaFree(ws.cnt); ws.cnt = nullptr; ws.cnt_cap = 0;
-        CU(h, cudaMalloc(&ws.cnt, (size_t)windows * sizeof(int32_t)));
-        ws.cnt_cap = windows;
-    }
-    if (p.ws_bins && windows > ws.bins_cap) {
-        if (ws.used) CU(h, cudaEventSynchronize(ws.scan_done));
-        cudaFree(ws.bins); ws.bins = nullptr; ws.bins_cap = 0;
-        CU(h, cudaMalloc(&ws.bins, (size_t)windows * h->n * sizeof(int32_t)));
-        ws.bins_cap = windows;
-    }
-    if (p.ws_wts && windows > ws.wts_cap) {
-        if (ws.used) CU(h, cudaEventSynchronize(ws.scan_done));
-        cudaFree(ws.wts); ws.wts = nullptr; ws.wts_cap = 0;
-        CU(h, cudaMalloc(&ws.wts, (size_t)windows * h->n * h->m * 2 * sizeof(double)));
-        ws.wts_cap = windows;
-    }
-    return MUSIC_B200_OK;
+        if (!idle) CU(h, cudaEventSynchronize(ws.scan_done));
+        idle = true;
+        CU(h, buf.grow(elems));
+        return MUSIC_B200_OK;
+    };
+    const size_t w = windows, mm = (size_t)h->m * h->m * 2;
+    if (const int rc = grow(ws.R, w * mm)) return rc;
+    if (const int rc = grow(ws.Vt, w * mm)) return rc;
+    if (const int rc = grow(ws.ev, w * h->m)) return rc;
+    if (const int rc = grow(ws.P64, p.ws_p64 ? w * h->K : 0)) return rc;
+    if (const int rc = grow(ws.cnt, p.ws_counts ? w : 0)) return rc;
+    if (const int rc = grow(ws.bins, p.ws_bins ? w * h->n : 0)) return rc;
+    return grow(ws.wts, p.ws_wts ? w * h->n * h->m * 2 : 0);
 }
 
 // Runtime M -> the M template argument of the scan kernels: 4, 8 and 16 are specialised, every other M runs the
@@ -741,7 +807,7 @@ void with_scan_form(const Plan &p, const int32_t *cnt, F f)
 // K3, the grid scan of W windows the plan chose against table tb, into the outputs o of these windows.  cnt: the
 // per-window source counts (NULL under the FIXED rule).  scan_kernel stages per window the eigenvectors (MUSIC), the g_j of mvdr_prep_kernel
 // (MVDR) or R (Bartlett).
-void launch_scan(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t W, const Outputs &o, const PeakOut &po,
+void launch_scan(music_b200 *h, const Plan &p, const WsView &ws, uint32_t W, const Outputs &o, const PeakOut &po,
                  const int32_t *cnt, const DeviceTable &tb, cudaStream_t st)
 {
     if (p.scan == Scan::None) return;
@@ -808,7 +874,7 @@ unsigned *ticket_counter(music_b200 *h, int slot, cudaStream_t st)
 }
 
 // K1: covariance of W windows into ws.R, on `st`.
-void launch_cov(music_b200 *h, const Workspace &ws, const float *d_in, uint32_t W, cudaStream_t st, int ctr_slot)
+void launch_cov(music_b200 *h, const WsView &ws, const float *d_in, uint32_t W, cudaStream_t st, int ctr_slot)
 {
     const int M = (int)h->m, N = (int)h->N;
     if (M == 4) {
@@ -908,10 +974,10 @@ __global__ void gather_wait_kernel(const unsigned *flags, int npeer, unsigned ep
 // The beam weights of W windows from ws.R, the angles and bins po holds, into o.wts (or the workspace), then the beams
 // of the W windows at d_in into o.beams when the caller asked for them (music_beams.cuh).  With a calibration set the
 // weights are taken back to raw-input coordinates before the beams are formed (music_calib.cuh).
-void launch_beams(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t W, const Outputs &o, const PeakOut &po, const float *d_in,
+void launch_beams(music_b200 *h, const Plan &p, const WsView &ws, uint32_t W, const Outputs &o, const PeakOut &po, const float *d_in,
                   cudaStream_t st)
 {
-    const DeviceTable &tb = h->table[h->cur_table];
+    const DeviceTable &tb = table(h);
     const int M = (int)h->m, n = (int)h->n, N = (int)h->N;
     double *wts = o.wts ? o.wts : ws.wts;
     beam_weights_kernel<<<(W + BEAM_WARPS - 1) / BEAM_WARPS, BEAM_WARPS * 32, 0, st>>>(
@@ -935,7 +1001,7 @@ void launch_beams(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t W,
 
 // K2 of W windows from ws.R as planned: the eigensolver, the source count from `nsnap` snapshots (into ws.cnt and, when
 // given, counts_out) and the MVDR preparation.  Returns the per-window counts the later stages read (NULL under FIXED).
-const int32_t *launch_eig_stage(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t W, int32_t *counts_out, uint32_t nsnap,
+const int32_t *launch_eig_stage(music_b200 *h, const Plan &p, const WsView &ws, uint32_t W, int32_t *counts_out, uint32_t nsnap,
                                 cudaStream_t st)
 {
     const int M = (int)h->m;
@@ -980,7 +1046,7 @@ void launch_grid_peaks(music_b200 *h, Peaks peaks, const double *p64, uint32_t W
 // after the peak rule.  With refinement on, the refine kernel follows (timed with the peak rule) and reads the bins
 // written before it: from the caller's array, or from the workspace when the caller asked for none.  A beams call
 // then forms the weights and beams of the windows at d_in (timed with the peak rule as well).
-int launch_eig_scan(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t W, const Outputs &o, const DeviceTable &tb, uint32_t nsnap,
+int launch_eig_scan(music_b200 *h, const Plan &p, const WsView &ws, uint32_t W, const Outputs &o, const DeviceTable &tb, uint32_t nsnap,
                     cudaStream_t st, cudaEvent_t *tev, const float *d_in = nullptr)
 {
     const int M = (int)h->m;
@@ -1047,7 +1113,7 @@ int launch_eig_scan(music_b200 *h, const Plan &p, const Workspace &ws, uint32_t 
 }
 
 // K1 on planar streams (music_planar.cuh): windows first .. first + W - 1 of the call
-void launch_cov_planar(music_b200 *h, const Workspace &ws, const PlanarStreams &S, unsigned long long first_snapshot,
+void launch_cov_planar(music_b200 *h, const WsView &ws, const PlanarStreams &S, unsigned long long first_snapshot,
                        unsigned hop, uint32_t W, cudaStream_t st)
 {
     const int M = (int)h->m, N = (int)h->N, T = (M + 3) / 4, wpb = 8;
@@ -1070,7 +1136,7 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, const Ou
     if ((!planar && !d_in) || !out.angles) return fail(h, MUSIC_B200_EINVAL, "d_in_c64 and d_angles must not be NULL");
     if (h->azel && !out.elev) return fail(h, MUSIC_B200_EINVAL, "an az-el handle needs the elevation output");
     if (!planar && (reinterpret_cast<uintptr_t>(d_in) & 15u) != 0) return fail(h, MUSIC_B200_EINVAL, "d_in_c64 must be 16-byte aligned");
-    if (const int rc = check_modes(h, h->modes, &h->table[h->cur_table])) return rc;
+    if (const int rc = check_modes(h, h->modes, &table(h))) return rc;
     if (h->source_rule == MUSIC_B200_SOURCES_FIXED && out.counts) {
         fill_counts_kernel<<<(nwindows + 255) / 256, 256, 0, st>>>(out.counts, (int)h->n, (int)nwindows);
         h->launches++;
@@ -1083,7 +1149,7 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, const Ou
         if (tev) cudaEventRecord(tev[0], st);
         const int grid = std::min<int>(h->sm_count, (int)((nwindows + FZ_COV_WARPS - 1) / FZ_COV_WARPS));
         unsigned *ctr = ticket_counter(h, slot, st);
-        const DeviceTable &tb = h->table[h->cur_table];
+        const DeviceTable &tb = table(h);
         const PeakOut po = make_peak_out(out);
         const GatherFlags gf = make_gather_flags(h, out.gather);
         // Programmatic dependent launch: when the previous operation on `st` is another launch of this kernel, the new
@@ -1133,7 +1199,7 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, const Ou
             if (tev) cudaEventRecord(tev[0], st);
             const int grid = std::min<int>(h->sm_count, (int)((nwindows + F8_WARPS - 1) / F8_WARPS));
             unsigned *ctr = ticket_counter(h, slot, st);
-            music8_fused_kernel<<<grid, F8_WARPS * 32, F8_SMEM, st>>>(tm, h->table[h->cur_table].soa, (int)nwindows, (int)h->N, (int)h->K,
+            music8_fused_kernel<<<grid, F8_WARPS * 32, F8_SMEM, st>>>(tm, table(h).soa, (int)nwindows, (int)h->N, (int)h->K,
                                                                      make_peak_out(out), ctr, make_gather_flags(h, out.gather),
                                                                      h->eig_mode ? 1 : 0, h->f8_stats);
             h->launches++;
@@ -1148,20 +1214,21 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, const Ou
     int rc = ensure_slot(h, ws, sub, plan);
     if (rc) return rc;
     if (ws.used) CU(h, cudaStreamWaitEvent(st, ws.scan_done, 0));  // the slot's last user may have run on another stream
+    const WsView v = ws.view();
     for (uint32_t w0 = 0; w0 < nwindows; w0 += sub) {
         const uint32_t W = std::min(sub, nwindows - w0);
         cudaEvent_t *tev = timing_events(h);
         if (tev) cudaEventRecord(tev[0], st);
-        if (planar) launch_cov_planar(h, ws, *planar, (unsigned long long)w0 * hop, hop, W, st);
-        else launch_cov(h, ws, d_in + (size_t)w0 * h->nsamples * 2, W, st, slot);
+        if (planar) launch_cov_planar(h, v, *planar, (unsigned long long)w0 * hop, hop, W, st);
+        else launch_cov(h, v, d_in + (size_t)w0 * h->nsamples * 2, W, st, slot);
         if (plan.calib) {
             // the receiver correction of R, inside the covariance slot of the stage timing
             const size_t e = (size_t)W * h->m * h->m;
-            calib_apply_kernel<<<(unsigned)((e + CALIB_THREADS - 1) / CALIB_THREADS), CALIB_THREADS, 0, st>>>(ws.R, (int)h->m, (int)W, h->cal_c);
+            calib_apply_kernel<<<(unsigned)((e + CALIB_THREADS - 1) / CALIB_THREADS), CALIB_THREADS, 0, st>>>(v.R, (int)h->m, (int)W, h->cal_c);
             h->launches++;
         }
         if (tev) cudaEventRecord(tev[1], st);
-        rc = launch_eig_scan(h, plan, ws, W, out.at(w0), h->table[h->cur_table], h->N, st, tev,
+        rc = launch_eig_scan(h, plan, v, W, out.at(w0), table(h), h->N, st, tev,
                              planar ? nullptr : d_in + (size_t)w0 * h->nsamples * 2);
         if (rc) return rc;
         CU(h, cudaEventRecord(ws.scan_done, st));
@@ -1190,11 +1257,11 @@ int enqueue_channels(music_b200 *h, const float *d_in, uint32_t nwindows, const 
     if (nwindows == 0) return MUSIC_B200_OK;
     if (!d_in || !out.angles) return fail(h, MUSIC_B200_EINVAL, "d_in_c64 and d_angles must not be NULL");
     if ((reinterpret_cast<uintptr_t>(d_in) & 15u) != 0) return fail(h, MUSIC_B200_EINVAL, "d_in_c64 must be 16-byte aligned");
-    if (!h->ctab_set) return fail(h, MUSIC_B200_EINVAL, "no array response yet: call music_b200_set_geometry_channels() or music_b200_set_table()");
+    if (!has_table(h)) return fail(h, MUSIC_B200_EINVAL, "no array response yet: call music_b200_set_geometry_channels() or music_b200_set_table()");
     const bool separate = h->chan_combine == MUSIC_B200_CHANNELS_SEPARATE, focus = coherent(h);
     const ChanShape &cs = h->cshape;
     const int ref = cs.C / 2;
-    if (const int rc = check_modes(h, h->modes, focus ? &channel_table(h, ref) : nullptr)) return rc;
+    if (const int rc = check_modes(h, h->modes, focus ? &table(h, ref) : nullptr)) return rc;
     if (h->chan_combine == MUSIC_B200_CHANNELS_INCOHERENT && out.counts)
         return fail(h, MUSIC_B200_EINVAL, "the INCOHERENT combine reports no counts: counts must be NULL");
     const uint32_t C = (uint32_t)cs.C;
@@ -1208,15 +1275,13 @@ int enqueue_channels(music_b200 *h, const float *d_in, uint32_t nwindows, const 
     const uint32_t sub = std::min((nwindows + SCAN_B - 1) / SCAN_B * SCAN_B, max_sub_windows(h, plan));
     Workspace &ws = h->ws[0];
     if (const int rc = ensure_slot(h, ws, focus ? sub : sub * C, plan)) return rc;
-    if (focus && (size_t)sub * C > h->foc_Rc_cap) {
+    const size_t foc_elems = (size_t)sub * C * h->m * h->m;
+    if (focus && foc_elems > h->foc_Rc.size()) {
         if (ws.used) CU(h, cudaEventSynchronize(ws.scan_done));  // the last call may still read it on another stream
-        cudaFree(h->foc_Rc);
-        h->foc_Rc = nullptr;
-        h->foc_Rc_cap = 0;
-        CU(h, cudaMalloc(&h->foc_Rc, (size_t)sub * C * h->m * h->m * sizeof(double2)));
-        h->foc_Rc_cap = (size_t)sub * C;
+        CU(h, h->foc_Rc.grow(foc_elems));
     }
     if (ws.used) CU(h, cudaStreamWaitEvent(st, ws.scan_done, 0));
+    const WsView v = ws.view();
     const size_t mm2 = (size_t)h->m * h->m * 2, K = h->K;
     const size_t smem = chan_smem(cs.M, cs.F, cs.B, cs.Cg).total;
     for (uint32_t w0 = 0; w0 < nwindows; w0 += sub) {
@@ -1224,47 +1289,47 @@ int enqueue_channels(music_b200 *h, const float *d_in, uint32_t nwindows, const 
         cudaEvent_t *tev = timing_events(h);
         if (tev) cudaEventRecord(tev[0], st);
         const int grid = (int)std::min<uint32_t>(W, (uint32_t)(h->sm_count * h->chan_ctas));
-        double *Rc = focus ? reinterpret_cast<double *>(h->foc_Rc) : ws.R;
+        double *Rc = focus ? reinterpret_cast<double *>(h->foc_Rc.get()) : v.R;
         chan_cov_kernel<<<grid, CHAN_THREADS, smem, st>>>(d_in + (size_t)w0 * h->nsamples * 2, Rc, (int)W, cs, h->chan_tw, h->chan_taper_d);
         h->launches++;
         if (focus) {
             // R_foc into the workspace, inside the covariance slot of the stage timing; then one plain problem per window
             const int M = (int)h->m, wt = focus_windows(M);
-            chan_focus_kernel<<<(W + wt - 1) / wt, focus_threads(M), 0, st>>>(h->foc_Rc, reinterpret_cast<double2 *>(ws.R), (int)W, (int)C,
-                                                                            M, ref, h->foc_T[h->cur_table]);
+            chan_focus_kernel<<<(W + wt - 1) / wt, focus_threads(M), 0, st>>>(h->foc_Rc, reinterpret_cast<double2 *>(v.R), (int)W, (int)C,
+                                                                            M, ref, cur_slot(h).foc_T);
             h->launches++;
             if (tev) cudaEventRecord(tev[1], st);
             Outputs o = out.at(w0);
             o.R = R_out ? R_out + (size_t)w0 * mm2 : nullptr;
-            if (const int rc = launch_eig_scan(h, plan, ws, W, o, channel_table(h, ref), snapshots(h), st, tev)) return rc;
+            if (const int rc = launch_eig_scan(h, plan, v, W, o, table(h, ref), snapshots(h), st, tev)) return rc;
             CU(h, cudaEventRecord(ws.scan_done, st));
             ws.used = true;
             continue;
         }
         if (tev) cudaEventRecord(tev[1], st);
-        const int32_t *cnt = launch_eig_stage(h, plan, ws, C * W, nullptr, (uint32_t)cs.J, st);
+        const int32_t *cnt = launch_eig_stage(h, plan, v, C * W, nullptr, (uint32_t)cs.J, st);
         if (cnt && out.counts)
             CU(h, cudaMemcpy2DAsync(out.counts + w0, (size_t)nwindows * sizeof(int32_t), cnt, (size_t)W * sizeof(int32_t), (size_t)W * sizeof(int32_t), C,
                                     cudaMemcpyDeviceToDevice, st));
         if (tev) cudaEventRecord(tev[2], st);
         // channel c's run of the workspace, and its block of the outputs from window w0 on
         const auto run = [&](uint32_t c) {
-            Workspace v = ws;
-            v.R += (size_t)c * W * mm2;
-            v.Vt += (size_t)c * W * mm2;
-            if (v.P64) v.P64 += (size_t)c * W * K;
-            return v;
+            WsView r = v;
+            r.R += (size_t)c * W * mm2;
+            r.Vt += (size_t)c * W * mm2;
+            if (r.P64) r.P64 += (size_t)c * W * K;
+            return r;
         };
         const auto block = [&](uint32_t c) { return separate ? out.at((size_t)c * nwindows + w0) : Outputs().shaped(h); };
         for (uint32_t c = 0; c < C; ++c) {
             const Outputs o = block(c);
-            launch_scan(h, plan, run(c), W, o, make_peak_out(o), cnt ? cnt + (size_t)c * W : nullptr, channel_table(h, (int)c), st);
+            launch_scan(h, plan, run(c), W, o, make_peak_out(o), cnt ? cnt + (size_t)c * W : nullptr, table(h, (int)c), st);
         }
         if (tev) cudaEventRecord(tev[3], st);
         if (plan.combine) {
             const size_t WK = (size_t)W * K;
-            chan_combine_kernel<<<(unsigned)((WK + 255) / 256), 256, 0, st>>>(ws.P64, (int)C, WK, out.spec ? out.spec + (size_t)w0 * K : nullptr);
-            launch_grid_peaks(h, plan.peaks, ws.P64, W, make_peak_out(out.at(w0)), nullptr, st);
+            chan_combine_kernel<<<(unsigned)((WK + 255) / 256), 256, 0, st>>>(v.P64, (int)C, WK, out.spec ? out.spec + (size_t)w0 * K : nullptr);
+            launch_grid_peaks(h, plan.peaks, v.P64, W, make_peak_out(out.at(w0)), nullptr, st);
             h->launches += 2;
         } else if (plan.peaks != Peaks::None) {
             for (uint32_t c = 0; c < C; ++c) {
@@ -1275,7 +1340,7 @@ int enqueue_channels(music_b200 *h, const float *d_in, uint32_t nwindows, const 
         }
         if (tev) cudaEventRecord(tev[4], st);
         if (R_out)
-            CU(h, cudaMemcpy2DAsync(R_out + (size_t)w0 * mm2, (size_t)nwindows * mm2 * sizeof(double), ws.R, (size_t)W * mm2 * sizeof(double),
+            CU(h, cudaMemcpy2DAsync(R_out + (size_t)w0 * mm2, (size_t)nwindows * mm2 * sizeof(double), v.R, (size_t)W * mm2 * sizeof(double),
                                     (size_t)W * mm2 * sizeof(double), C, cudaMemcpyDeviceToDevice, st));
         CU(h, cudaGetLastError());
         CU(h, cudaEventRecord(ws.scan_done, st));
@@ -1332,58 +1397,36 @@ void host_register(music_b200 *h, const void *ptr, size_t bytes, bool read_only)
     h->hostregs.push_back(music_b200::HostReg{lo, (size_t)(hi - lo)});
 }
 
-void free_host_staging(music_b200 *h)
-{
-    for (HostSlot &sl : h->stage) {
-        cudaFree(sl.in);
-        cudaFree(sl.dev.spec);
-        cudaFree(sl.dev.wts);
-        cudaFree(sl.dev.beams);
-        cudaFreeHost(sl.pin.wts);
-        cudaFreeHost(sl.pin.beams);
-        const auto dev = sl.dev.window_fields(), pin = sl.pin.window_fields();
-        for (size_t f = 0; f < dev.size(); ++f) {
-            cudaFree(dev[f].p);
-            cudaFreeHost(pin[f].p);
-        }
-        sl = HostSlot();
-    }
-    h->host_chunk = 0;
-    h->host_spec_alloc = false;
-    h->host_beam_alloc = false;
-}
-
 int ensure_host_staging(music_b200 *h, uint32_t chunk, bool spec, bool beams)
 {
     if (chunk <= h->host_chunk && (!spec || h->host_spec_alloc) && (!beams || h->host_beam_alloc)) return MUSIC_B200_OK;
     spec = spec || h->host_spec_alloc;
     beams = beams || h->host_beam_alloc;
     const uint32_t cap = std::max(chunk, h->host_chunk);
-    free_host_staging(h);
+    // every old buffer is freed before the first new one is allocated
+    for (HostSlot &sl : h->stage) sl = HostSlot();
+    h->host_chunk = 0;
+    h->host_spec_alloc = h->host_beam_alloc = false;
     const size_t wn = (size_t)cap * h->n;
-    for (HostSlot &sl : h->stage) {
-        sl.dev.shaped(h);
-        sl.pin.shaped(h);
-        CU(h, cudaMalloc(&sl.in, (size_t)cap * h->nsamples * 2 * sizeof(float)));
-        CU(h, cudaMalloc(&sl.dev.angles, wn * sizeof(float)));
-        CU(h, cudaMalloc(&sl.dev.levels, wn * sizeof(float)));
-        CU(h, cudaMalloc(&sl.dev.bins, wn * sizeof(int32_t)));
-        CU(h, cudaHostAlloc(&sl.pin.angles, wn * sizeof(float), cudaHostAllocDefault));
-        CU(h, cudaHostAlloc(&sl.pin.levels, wn * sizeof(float), cudaHostAllocDefault));
-        CU(h, cudaHostAlloc(&sl.pin.bins, wn * sizeof(int32_t), cudaHostAllocDefault));
-        CU(h, cudaMalloc(&sl.dev.counts, (size_t)cap * sizeof(int32_t)));
-        CU(h, cudaHostAlloc(&sl.pin.counts, (size_t)cap * sizeof(int32_t), cudaHostAllocDefault));
-        if (spec) CU(h, cudaMalloc(&sl.dev.spec, (size_t)cap * h->K * sizeof(float)));
+    const auto alloc = [&](auto &b) -> int {
+        CU(h, b.angles.grow(wn));
+        CU(h, b.levels.grow(wn));
+        CU(h, b.bins.grow(wn));
+        CU(h, b.counts.grow(cap));
         if (beams) {
-            CU(h, cudaMalloc(&sl.dev.wts, wn * h->m * 2 * sizeof(double)));
-            CU(h, cudaMalloc(&sl.dev.beams, wn * h->N * 2 * sizeof(float)));
-            CU(h, cudaHostAlloc(&sl.pin.wts, wn * h->m * 2 * sizeof(double), cudaHostAllocDefault));
-            CU(h, cudaHostAlloc(&sl.pin.beams, wn * h->N * 2 * sizeof(float), cudaHostAllocDefault));
+            CU(h, b.wts.grow(wn * h->m * 2));
+            CU(h, b.beams.grow(wn * h->N * 2));
         }
-        if (h->azel) {
-            CU(h, cudaMalloc(&sl.dev.elev, wn * sizeof(float)));
-            CU(h, cudaHostAlloc(&sl.pin.elev, wn * sizeof(float), cudaHostAllocDefault));
-        }
+        if (h->azel) CU(h, b.elev.grow(wn));
+        return MUSIC_B200_OK;
+    };
+    for (HostSlot &sl : h->stage) {
+        CU(h, sl.in.grow((size_t)cap * h->nsamples * 2));
+        if (spec) CU(h, sl.dbuf.spec.grow((size_t)cap * h->K));
+        if (const int rc = alloc(sl.dbuf)) return rc;
+        if (const int rc = alloc(sl.pbuf)) return rc;
+        sl.dev = sl.dbuf.view(h);
+        sl.pin = sl.pbuf.view(h);
     }
     h->host_chunk = cap;
     h->host_spec_alloc = spec;
@@ -1531,7 +1574,7 @@ int stage_host(music_b200 *h, const HostInput &in, uint32_t nwindows, const Outp
                 if (!dst.counts) o.counts = nullptr;
                 if (!dst.wts) o.wts = nullptr;
                 if (!dst.beams) o.beams = nullptr;
-                rc = enqueue_device(c, in.streams ? nullptr : sl.in, W, o, st, s, in.streams ? &S : nullptr, in.hop);
+                rc = enqueue_device(c, in.streams ? nullptr : sl.in.get(), W, o, st, s, in.streams ? &S : nullptr, in.hop);
                 if (rc && c != h) fail(h, rc, "%s", std::string(c->error).c_str());
                 if (rc) break;
             }
@@ -1583,8 +1626,8 @@ int init_channels(music_b200 *h)
     cs.B = chan_batch(cs.M, cs.F, cs.J);
     cs.Cg = chan_group_size(cs.M, cs.F, cs.B, cs.C);
     cs.groups = (cs.C + cs.Cg - 1) / cs.Cg;
-    CU(h, cudaMalloc(&h->chan_tw, tw.size() * sizeof(double2)));
-    CU(h, cudaMalloc(&h->chan_taper_d, taper.size() * sizeof(double)));
+    CU(h, h->chan_tw.grow(tw.size()));
+    CU(h, h->chan_taper_d.grow(taper.size()));
     CU(h, cudaMemcpy(h->chan_tw, tw.data(), tw.size() * sizeof(double2), cudaMemcpyHostToDevice));
     CU(h, cudaMemcpy(h->chan_taper_d, taper.data(), taper.size() * sizeof(double), cudaMemcpyHostToDevice));
     const size_t smem = chan_smem(cs.M, cs.F, cs.B, cs.Cg).total;
@@ -1594,18 +1637,52 @@ int init_channels(music_b200 *h)
     return MUSIC_B200_OK;
 }
 
-// the per-channel tables of slot `slot` (allocated the first time the slot is filled)
-int ensure_channel_tables(music_b200 *h, int slot)
+// The buffers of table slot s, allocated the first time the slot is filled
+int alloc_slot(music_b200 *h, TableSlot &s)
 {
-    if (!h->ctab[slot].empty()) return MUSIC_B200_OK;
-    const size_t C = (size_t)h->cshape.C, c64 = (size_t)h->K * h->m * 2, soa = soa_doubles(h->K, h->m);
-    CU(h, cudaMalloc(&h->ctab_c64[slot], C * c64 * sizeof(float)));
-    CU(h, cudaMalloc(&h->ctab_soa[slot], C * soa * sizeof(double)));
-    h->ctab[slot].resize(C);
-    for (size_t c = 0; c < C; ++c) {
-        h->ctab[slot][c].c64 = h->ctab_c64[slot] + c * c64;
-        h->ctab[slot][c].soa = h->ctab_soa[slot] + c * soa;
+    if (!s.tabs.empty()) return MUSIC_B200_OK;
+    const size_t C = h->chan ? (size_t)h->cshape.C : 1, c64 = (size_t)h->K * h->m * 2, soa = soa_doubles(h->K, h->m);
+    CU(h, s.c64.grow(C * c64));
+    CU(h, s.soa.grow(C * soa));
+    if (h->m == 4 && !h->azel && !h->chan) {  // the fused M = 4 kernel's screen layout; no other handle runs that kernel
+        CU(h, s.fz.grow(fused_table_bytes((int)h->K)));
+        CU(h, s.na_max.grow(1));
     }
+    if (coherent(h)) CU(h, s.foc_T.grow(C * h->m * h->m));
+    s.tabs.resize(C);
+    for (size_t c = 0; c < C; ++c) {
+        s.tabs[c].c64 = s.c64 + c * c64;
+        s.tabs[c].soa = s.soa + c * soa;
+    }
+    s.tabs[0].fz = s.fz;
+    s.tabs[0].na_max = s.na_max;
+    return MUSIC_B200_OK;
+}
+
+// A retune: fills the idle table slot and makes it current only when `fill` succeeded.  Work enqueued by earlier calls
+// may still read the current slot on a caller stream, so it is never rewritten; the idle slot was current before the
+// last retune, and the device is synchronised once to be sure it is idle - retunes are rare.
+template <class F>
+int retune(music_b200 *h, F fill)
+{
+    CU(h, cudaSetDevice(h->device));
+    CU(h, cudaDeviceSynchronize());
+    const int idle = h->cur_table ^ 1;
+    if (const int rc = alloc_slot(h, h->tables[idle])) return rc;
+    if (const int rc = fill(h->tables[idle])) return rc;
+    h->cur_table = idle;
+    return MUSIC_B200_OK;
+}
+
+// The checks every create entry point makes first, the reference's constructor asserts (lib/baz_music_doa.cc:45-50,
+// + n >= 1, n < m, see header)
+int check_create(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples)
+{
+    if (!out) return fail(nullptr, MUSIC_B200_EINVAL, "out must not be NULL");
+    *out = nullptr;
+    if (m == 0 || m > MUSIC_B200_MAX_M) return fail(nullptr, MUSIC_B200_EINVAL, "m must be in 1..%d (got %u)", MUSIC_B200_MAX_M, m);
+    if (n == 0 || n >= m) return fail(nullptr, MUSIC_B200_EINVAL, "need 1 <= n < m (got n=%u, m=%u)", n, m);
+    if (nsamples == 0 || nsamples % m != 0) return fail(nullptr, MUSIC_B200_EINVAL, "nsamples must be a positive multiple of m (got %u)", nsamples);
     return MUSIC_B200_OK;
 }
 
@@ -1644,13 +1721,6 @@ int create_on_device(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples
         for (int i = 0; i < 2; ++i) {
             CU(h, cudaStreamCreateWithFlags(&h->streams[i], cudaStreamNonBlocking));
             CU(h, cudaEventCreateWithFlags(&h->ws[i].scan_done, cudaEventDisableTiming));
-            if (chan) continue;  // a channel handle's tables are per channel (ensure_channel_tables)
-            CU(h, cudaMalloc(&h->table[i].c64, (size_t)resolution * m * 2 * sizeof(float)));
-            CU(h, cudaMalloc(&h->table[i].soa, soa_doubles(resolution, m) * sizeof(double)));
-            if (m == 4 && !azel) {  // the fused M = 4 kernel's screen layout; an az-el handle never runs that kernel
-                CU(h, cudaMalloc(&h->table[i].fz, fused_table_bytes((int)resolution)));
-                CU(h, cudaMalloc(&h->table[i].na_max, sizeof(float)));
-            }
         }
         // scan kernels with M = 16 need 32 KiB dynamic smem (< 48 KiB default), nothing to opt in.
         if (const char *e = getenv("MUSIC_B200_FUSED")) h->fused = atoi(e) != 0;
@@ -1661,16 +1731,16 @@ int create_on_device(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples
         CU(h, cudaFuncSetAttribute(covN_tma_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CN_SMEM));
         CU(h, cudaFuncSetAttribute(covN_tma_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CN_SMEM));
         CU(h, cudaFuncSetAttribute(music8_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)F8_SMEM));
-        CU(h, cudaMalloc(&h->f8_stats, 2 * sizeof(unsigned)));
+        CU(h, h->f8_stats.grow(2));
         CU(h, cudaMemset(h->f8_stats, 0, 2 * sizeof(unsigned)));
         CU(h, cudaEventCreateWithFlags(&h->fused_done, cudaEventDisableTiming));
-        CU(h, cudaMalloc(&h->work_ctr, 2 * CTR_RING * 2 * sizeof(unsigned)));  // self-resetting (tickets, finished CTAs) pairs
+        CU(h, h->work_ctr.grow(2 * CTR_RING * 2));  // self-resetting (tickets, finished CTAs) pairs
         CU(h, cudaMemset(h->work_ctr, 0, 2 * CTR_RING * 2 * sizeof(unsigned)));
         if (const char *e = getenv("MUSIC_B200_HOSTREG")) h->hostreg = atoi(e) != 0;
         if (getenv("MUSIC_B200_TRACE")) {
-            const size_t tb = (size_t)FZ_TRACE_LAUNCHES * FZ_TRACE_CTAS * FZ_TRACE * sizeof(long long);
-            CU(h, cudaMalloc(&h->fused_trace, tb));
-            CU(h, cudaMemset(h->fused_trace, 0, tb));
+            const size_t tb = (size_t)FZ_TRACE_LAUNCHES * FZ_TRACE_CTAS * FZ_TRACE;
+            CU(h, h->fused_trace.grow(tb));
+            CU(h, cudaMemset(h->fused_trace, 0, tb * sizeof(long long)));
         }
         // the fused M = 4 kernel runs two CTAs per SM: all of the SM's unified L1 / shared memory goes to shared memory
         for (const void *k : {(const void *)music4_fused_kernel<false, false>, (const void *)music4_fused_kernel<true, false>,
@@ -1679,8 +1749,10 @@ int create_on_device(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples
             CU(h, cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
         }
         CU(h, cudaFuncSetAttribute(cov4_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)COV_SMEM));
-        if (chan) return init_channels(h);
-        return azel ? build_table_azel(h, 0, azel->pos, azel->lambda, h->streams[0]) : upload_table(h, h->table[0], table_c64, h->streams[0]);
+        if (chan) return init_channels(h);  // a channel handle takes its first tables at its first retune
+        if (const int rc = alloc_slot(h, h->tables[0])) return rc;
+        DeviceTable &t = h->tables[0].tabs[0];
+        return azel ? build_table_azel(h, t, azel->pos, azel->lambda, h->streams[0]) : upload_table(h, t, table_c64, h->streams[0]);
     };
     rc = init();
     if (rc != MUSIC_B200_OK) {
@@ -1688,7 +1760,6 @@ int create_on_device(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples
         music_b200_destroy(h);
         return rc;
     }
-    h->cur_table = 0;
     *out = h;
     return MUSIC_B200_OK;
 }
@@ -1781,12 +1852,7 @@ int music_b200_get_stage_times(music_b200 *h, double *ms4, uint64_t *chunks)
 int music_b200_create(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples, uint32_t resolution,
                       const float *table_c64, int device)
 {
-    if (!out) return fail(nullptr, MUSIC_B200_EINVAL, "out must not be NULL");
-    *out = nullptr;
-    // reference asserts, lib/baz_music_doa.cc:45-50 (+ n >= 1, n < m, see header)
-    if (m == 0 || m > MUSIC_B200_MAX_M) return fail(nullptr, MUSIC_B200_EINVAL, "m must be in 1..%d (got %u)", MUSIC_B200_MAX_M, m);
-    if (n == 0 || n >= m) return fail(nullptr, MUSIC_B200_EINVAL, "need 1 <= n < m (got n=%u, m=%u)", n, m);
-    if (nsamples == 0 || nsamples % m != 0) return fail(nullptr, MUSIC_B200_EINVAL, "nsamples must be a positive multiple of m (got %u)", nsamples);
+    if (const int rc = check_create(out, m, n, nsamples)) return rc;
     if (resolution == 0) return fail(nullptr, MUSIC_B200_EINVAL, "resolution must be > 0");
     if (!table_c64) return fail(nullptr, MUSIC_B200_EINVAL, "array response table must not be NULL");
 
@@ -1800,30 +1866,14 @@ int music_b200_set_table(music_b200 *h, const float *table_c64)
     std::lock_guard<std::mutex> g(h->mutex);
     if (!h->kids.empty())  // multi-device handle: every device holds a full copy of the table (SURVEY.md section 8e)
         return for_each_child(h, [&](music_b200 *c) { return music_b200_set_table(c, table_c64); });
-    CU(h, cudaSetDevice(h->device));
     if (coherent(h))
         return fail(h, MUSIC_B200_EINVAL, "the COHERENT combine focuses geometric tables: one measured table gives no focusing "
                                           "(call music_b200_set_geometry_channels())");
-    if (h->chan) {
-        // one measured table for every channel (the narrowband assumption): entry 0 of the idle slot
-        CU(h, cudaDeviceSynchronize());
-        const int slot = h->cur_table ^ 1;
-        if (const int rc = ensure_channel_tables(h, slot)) return rc;
-        if (const int rc = upload_table(h, h->ctab[slot][0], table_c64, h->streams[0])) return rc;
-        h->ctab_shared[slot] = true;
-        h->cur_table = slot;
-        h->ctab_set = true;
-        return MUSIC_B200_OK;
-    }
-    // Work enqueued by earlier process_device() calls may still be reading the current slot on
-    // a caller stream; fill the other slot and flip.  (The slot being overwritten was retired
-    // two set_table() calls ago; synchronise the device once to be safe - retunes are rare.)
-    CU(h, cudaDeviceSynchronize());
-    const int slot = h->cur_table ^ 1;
-    int rc = upload_table(h, h->table[slot], table_c64, h->streams[0]);
-    if (rc) return rc;
-    h->cur_table = slot;
-    return MUSIC_B200_OK;
+    // on a channel handle one measured table serves every channel (the narrowband assumption)
+    return retune(h, [&](TableSlot &s) {
+        s.shared = true;
+        return upload_table(h, s.tabs[0], table_c64, h->streams[0]);
+    });
 }
 
 int music_b200_process_planar_device(music_b200 *h, const float *const *d_streams, uint32_t hop, uint32_t nwindows,
@@ -1907,21 +1957,18 @@ int music_b200_reduce_angles_host(music_b200 *h, const float *angles, const floa
     if (!h) return MUSIC_B200_EINVAL;
     if (!angles || !mean_deg) return fail(h, MUSIC_B200_EINVAL, "angles and mean_deg must not be NULL");
     if (weighted && !levels) return fail(h, MUSIC_B200_EINVAL, "level weighting needs levels");
-    float *d_a = nullptr, *d_l = nullptr, *d_o = nullptr;
-    const size_t nb = (size_t)nwindows * h->n * sizeof(float);
-    int rc = MUSIC_B200_OK;
+    DevBuf<float> d_a, d_l, d_o;
+    const size_t ne = (size_t)nwindows * h->n, nb = ne * sizeof(float);
     {
         std::lock_guard<std::mutex> g(h->mutex);
         CU(h, cudaSetDevice(h->device));
-        if (cudaMalloc(&d_a, std::max<size_t>(nb, 4)) != cudaSuccess || cudaMalloc(&d_o, 3 * h->n * sizeof(float)) != cudaSuccess ||
-            (levels && cudaMalloc(&d_l, std::max<size_t>(nb, 4)) != cudaSuccess)) {
-            cudaFree(d_a); cudaFree(d_o); cudaFree(d_l);
+        if (d_a.grow(std::max<size_t>(ne, 1)) != cudaSuccess || d_o.grow(3 * h->n) != cudaSuccess ||
+            (levels && d_l.grow(std::max<size_t>(ne, 1)) != cudaSuccess))
             return fail(h, MUSIC_B200_ENOMEM, "cudaMalloc failed for the reducer buffers");
-        }
         cudaMemcpy(d_a, angles, nb, cudaMemcpyHostToDevice);
         if (levels) cudaMemcpy(d_l, levels, nb, cudaMemcpyHostToDevice);
     }
-    rc = music_b200_reduce_angles_device(h, d_a, d_l, nwindows, weighted, d_o, d_o + h->n, d_o + 2 * h->n, nullptr);
+    int rc = music_b200_reduce_angles_device(h, d_a, d_l, nwindows, weighted, d_o, d_o + h->n, d_o + 2 * h->n, nullptr);
     if (rc == MUSIC_B200_OK) {
         std::vector<float> out(3 * h->n);
         const cudaError_t e = cudaMemcpy(out.data(), d_o, out.size() * sizeof(float), cudaMemcpyDeviceToHost);
@@ -1934,7 +1981,6 @@ int music_b200_reduce_angles_host(music_b200 *h, const float *angles, const floa
             }
         }
     }
-    cudaFree(d_a); cudaFree(d_o); cudaFree(d_l);
     return rc;
 }
 
@@ -1944,23 +1990,20 @@ int music_b200_reduce_spectrum_host(music_b200 *h, const float *spectrum, uint32
     if (!h) return MUSIC_B200_EINVAL;
     if (!spectrum || !mean) return fail(h, MUSIC_B200_EINVAL, "spectrum and mean must not be NULL");
     if (nwindows == 0) return fail(h, MUSIC_B200_EINVAL, "nwindows must be >= 1");
-    float *d_s = nullptr, *d_m = nullptr;
-    const size_t nb = (size_t)nwindows * h->K * sizeof(float);
+    DevBuf<float> d_s, d_m;
+    const size_t ne = (size_t)nwindows * h->K;
     {
         std::lock_guard<std::mutex> g(h->mutex);
         CU(h, cudaSetDevice(h->device));
-        if (cudaMalloc(&d_s, nb) != cudaSuccess || cudaMalloc(&d_m, h->K * sizeof(float)) != cudaSuccess) {
-            cudaFree(d_s); cudaFree(d_m);
+        if (d_s.grow(ne) != cudaSuccess || d_m.grow(h->K) != cudaSuccess)
             return fail(h, MUSIC_B200_ENOMEM, "cudaMalloc failed for the reducer buffers");
-        }
-        cudaMemcpy(d_s, spectrum, nb, cudaMemcpyHostToDevice);
+        cudaMemcpy(d_s, spectrum, ne * sizeof(float), cudaMemcpyHostToDevice);
     }
     int rc = music_b200_reduce_spectrum_device(h, d_s, nwindows, d_m, nullptr);
     if (rc == MUSIC_B200_OK) {
         const cudaError_t e = cudaMemcpy(mean, d_m, h->K * sizeof(float), cudaMemcpyDeviceToHost);
         if (e != cudaSuccess) rc = fail(h, MUSIC_B200_ECUDA, "reducer failed: %s", cudaGetErrorString(e));
     }
-    cudaFree(d_s); cudaFree(d_m);
     return rc;
 }
 
@@ -1989,12 +2032,8 @@ int music_b200_set_geometry(music_b200 *h, const double *positions_xy, double wa
     std::lock_guard<std::mutex> g(h->mutex);
     if (!h->kids.empty())
         return for_each_child(h, [&](music_b200 *c) { return music_b200_set_geometry(c, positions_xy, wavelength, guarded); });
-    CU(h, cudaSetDevice(h->device));
-    CU(h, cudaDeviceSynchronize());  // as in set_table(): the slot being rebuilt must be idle
-    const int slot = h->cur_table ^ 1;
-    int rc = build_table(h, h->table[slot], positions_xy, wavelength, h->streams[0]);
-    if (rc) return rc;
-    h->cur_table = slot;
+    if (const int rc = retune(h, [&](TableSlot &s) { return build_table(h, s.tabs[0], positions_xy, wavelength, h->streams[0]); }))
+        return rc;
     if (guarded) *guarded = h->steer_guarded;
     return MUSIC_B200_OK;
 }
@@ -2013,7 +2052,7 @@ int music_b200_get_table(music_b200 *h, float *table_c64)
     h = served(h);
     std::lock_guard<std::mutex> g(h->mutex);
     CU(h, cudaSetDevice(h->device));
-    CU(h, cudaMemcpy(table_c64, h->table[h->cur_table].c64, (size_t)h->K * h->m * 2 * sizeof(float), cudaMemcpyDeviceToHost));
+    CU(h, cudaMemcpy(table_c64, table(h).c64, (size_t)h->K * h->m * 2 * sizeof(float), cudaMemcpyDeviceToHost));
     return MUSIC_B200_OK;
 }
 
@@ -2220,12 +2259,12 @@ namespace {
 // the accumulator, partial sums, counter and result buffer of a served handle (zeroed on first use)
 int ensure_calib_buffers(music_b200 *h)
 {
-    if (h->cal_acc) return MUSIC_B200_OK;
+    if (h->cal_out) return MUSIC_B200_OK;  // (allocated last)
     const size_t mm = (size_t)h->m * h->m;
-    CU(h, cudaMalloc(&h->cal_acc, mm * sizeof(double2)));
-    CU(h, cudaMalloc(&h->cal_part, (size_t)CALIB_ACC_MAX_CTAS * mm * sizeof(double2)));
-    CU(h, cudaMalloc(&h->cal_ctr, sizeof(unsigned)));
-    CU(h, cudaMalloc(&h->cal_out, CALIB_OUT * sizeof(double)));
+    CU(h, h->cal_acc.grow(mm));
+    CU(h, h->cal_part.grow((size_t)CALIB_ACC_MAX_CTAS * mm));
+    CU(h, h->cal_ctr.grow(1));
+    CU(h, h->cal_out.grow(CALIB_OUT));
     CU(h, cudaMemset(h->cal_acc, 0, mm * sizeof(double2)));
     CU(h, cudaMemset(h->cal_ctr, 0, sizeof(unsigned)));
     CU(h, cudaDeviceSynchronize());  // the memsets ran on the legacy stream; the kernels run on non-blocking ones
@@ -2246,7 +2285,7 @@ int calib_accumulate(music_b200 *h, const float *d_in, uint32_t nwindows, cudaSt
     if (ws.used) CU(h, cudaStreamWaitEvent(st, ws.scan_done, 0));
     for (uint32_t w0 = 0; w0 < nwindows; w0 += sub) {
         const uint32_t W = std::min(sub, nwindows - w0);
-        launch_cov(h, ws, d_in + (size_t)w0 * h->nsamples * 2, W, st, 0);
+        launch_cov(h, ws.view(), d_in + (size_t)w0 * h->nsamples * 2, W, st, 0);
         const int wpc = calib_acc_wpc((int)W);
         calib_accum_kernel<<<(W + wpc - 1) / wpc, CALIB_THREADS, 0, st>>>(ws.R, (int)h->m, (int)W, wpc, h->cal_part, h->cal_ctr, h->cal_acc);
         h->launches++;
@@ -2303,10 +2342,12 @@ int music_b200_calib_accumulate_host(music_b200 *h, const float *in_c64, uint32_
     // pinned copy makes the transfer independent of how the caller's memory is, or partly is, registered)
     const size_t win_bytes = (size_t)h->nsamples * 2 * sizeof(float);
     const uint32_t chunk = (uint32_t)std::max<size_t>(1, std::min<size_t>(nwindows, ((size_t)32 << 20) / win_bytes));
-    float *d = nullptr, *pin = nullptr;
+    const size_t chunk_floats = (size_t)chunk * h->nsamples * 2;
+    DevBuf<float> d;
+    PinBuf<float> pin;
     cudaStream_t st = h->streams[0];
     int rc = MUSIC_B200_OK;
-    if (cudaMalloc(&d, chunk * win_bytes) != cudaSuccess || cudaHostAlloc(&pin, chunk * win_bytes, cudaHostAllocDefault) != cudaSuccess)
+    if (d.grow(chunk_floats) != cudaSuccess || pin.grow(chunk_floats) != cudaSuccess)
         rc = fail(h, MUSIC_B200_ENOMEM, "cannot allocate the calibration staging buffers");
     for (uint32_t w0 = 0; w0 < nwindows && rc == MUSIC_B200_OK; w0 += chunk) {
         const uint32_t W = std::min(chunk, nwindows - w0);
@@ -2316,8 +2357,6 @@ int music_b200_calib_accumulate_host(music_b200 *h, const float *in_c64, uint32_
         rc = calib_accumulate(h, d, W, st);
     }
     const cudaError_t e = cudaStreamSynchronize(st);
-    cudaFree(d);
-    cudaFreeHost(pin);
     if (rc == MUSIC_B200_OK && e != cudaSuccess) rc = fail(h, MUSIC_B200_ECUDA, "stream sync failed: %s", cudaGetErrorString(e));
     return rc;
 }
@@ -2335,7 +2374,7 @@ int music_b200_calib_solve(music_b200 *h, double az_deg, double el_deg, int kind
     if (!std::isfinite(az_deg) || !std::isfinite(el_deg)) return fail(h, MUSIC_B200_EINVAL, "the source direction must be finite");
     if (!h->azel && el_deg != 0.0) return fail(h, MUSIC_B200_EINVAL, "a 1-D handle takes el_deg = 0 (got %g)", el_deg);
     std::lock_guard<std::mutex> g(h->mutex);
-    const DeviceTable &tb = h->table[h->cur_table];
+    const DeviceTable &tb = table(h);
     if (!tb.geometric)
         return fail(h, MUSIC_B200_EINVAL, "calibration needs a table built from the array geometry (set_geometry / set_geometry_azel); "
                                           "the current one came from set_table()");
@@ -2466,16 +2505,21 @@ int music_b200_gather_create(music_b200 *h, uint32_t total_windows, unsigned cha
     if (h->gather_buf) return fail(h, MUSIC_B200_EINVAL, "gather buffer already created");
     static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
     const size_t elems = (size_t)total_windows * h->n;
-    CU(h, cudaMalloc(&h->gather_buf, std::max<size_t>(elems, 1) * sizeof(int32_t)));
-    CU(h, cudaMalloc(&h->gather_flags, MAX_PEERS * sizeof(unsigned)));
-    CU(h, cudaMemset(h->gather_buf, 0xff, std::max<size_t>(elems, 1) * sizeof(int32_t)));
-    CU(h, cudaMemset(h->gather_flags, 0, MAX_PEERS * sizeof(unsigned)));
-    h->gather_cap = elems;
+    // the handle takes the buffers once both exist and are shared: a failure leaves it without a gather buffer
+    DevBuf<int32_t> buf;
+    DevBuf<unsigned> flags;
+    CU(h, buf.grow(std::max<size_t>(elems, 1)));
+    CU(h, flags.grow(MAX_PEERS));
+    CU(h, cudaMemset(buf, 0xff, buf.size() * sizeof(int32_t)));
+    CU(h, cudaMemset(flags, 0, MAX_PEERS * sizeof(unsigned)));
     cudaIpcMemHandle_t hb, hf;
-    CU(h, cudaIpcGetMemHandle(&hb, h->gather_buf));
-    CU(h, cudaIpcGetMemHandle(&hf, h->gather_flags));
+    CU(h, cudaIpcGetMemHandle(&hb, buf));
+    CU(h, cudaIpcGetMemHandle(&hf, flags));
     memcpy(ipc_handles, &hb, 64);
     memcpy(ipc_handles + 64, &hf, 64);
+    h->gather_buf = std::move(buf);
+    h->gather_flags = std::move(flags);
+    h->gather_cap = elems;
     return MUSIC_B200_OK;
 }
 
@@ -2497,12 +2541,14 @@ int music_b200_gather_attach(music_b200 *h, int nranks, int rank, const unsigned
         cudaIpcMemHandle_t hb, hf;
         memcpy(&hb, all_handles + (size_t)p * 128, 64);
         memcpy(&hf, all_handles + (size_t)p * 128 + 64, 64);
+        // each mapping is recorded as soon as it is open, so that music_b200_destroy() closes it whatever fails next
         void *pb = nullptr, *pf = nullptr;
         CU(h, cudaIpcOpenMemHandle(&pb, hb, cudaIpcMemLazyEnablePeerAccess));
+        h->ipc_maps.push_back(pb);
         CU(h, cudaIpcOpenMemHandle(&pf, hf, cudaIpcMemLazyEnablePeerAccess));
+        h->ipc_maps.push_back(pf);
         h->gather.peer[p] = static_cast<int32_t *>(pb);
         h->peer_flags[p] = static_cast<unsigned *>(pf);
-        h->peer_ipc[p] = true;
     }
     h->gather.G = nranks;
     h->gather.rank = rank;
@@ -2522,7 +2568,7 @@ int music_b200_gather_wait(music_b200 *h, void *stream)
     return MUSIC_B200_OK;
 }
 
-const int32_t *music_b200_gather_buffer(const music_b200 *h) { return h ? h->gather_buf : nullptr; }
+const int32_t *music_b200_gather_buffer(const music_b200 *h) { return h ? h->gather_buf.get() : nullptr; }
 
 int music_b200_gather_read(music_b200 *h, int32_t *host_out, uint32_t count)
 {
@@ -2582,11 +2628,7 @@ int check_azel_geometry(music_b200 *h, uint32_t m, const double *positions_xyz, 
 int music_b200_create_azel(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples, uint32_t n_az, uint32_t n_el,
                            double el_lo_deg, double el_hi_deg, const double *positions_xyz, double wavelength, int device)
 {
-    if (!out) return fail(nullptr, MUSIC_B200_EINVAL, "out must not be NULL");
-    *out = nullptr;
-    if (m == 0 || m > MUSIC_B200_MAX_M) return fail(nullptr, MUSIC_B200_EINVAL, "m must be in 1..%d (got %u)", MUSIC_B200_MAX_M, m);
-    if (n == 0 || n >= m) return fail(nullptr, MUSIC_B200_EINVAL, "need 1 <= n < m (got n=%u, m=%u)", n, m);
-    if (nsamples == 0 || nsamples % m != 0) return fail(nullptr, MUSIC_B200_EINVAL, "nsamples must be a positive multiple of m (got %u)", nsamples);
+    if (const int rc = check_create(out, m, n, nsamples)) return rc;
     if (n_az == 0 || n_el == 0) return fail(nullptr, MUSIC_B200_EINVAL, "n_az and n_el must be > 0");
     if ((uint64_t)n_az * n_el > MUSIC_B200_AZEL_MAX_BINS)
         return fail(nullptr, MUSIC_B200_EINVAL, "n_az * n_el must be at most %u (got %llu)", (unsigned)MUSIC_B200_AZEL_MAX_BINS, (unsigned long long)n_az * n_el);
@@ -2609,13 +2651,7 @@ int music_b200_set_geometry_azel(music_b200 *h, const double *positions_xyz, dou
     const int rc = check_azel_geometry(h, h->m, positions_xyz, wavelength);
     if (rc) return rc;
     std::lock_guard<std::mutex> g(h->mutex);
-    CU(h, cudaSetDevice(h->device));
-    CU(h, cudaDeviceSynchronize());  // as in set_table(): the slot being rebuilt must be idle
-    const int slot = h->cur_table ^ 1;
-    const int rb = build_table_azel(h, slot, positions_xyz, wavelength, h->streams[0]);
-    if (rb) return rb;
-    h->cur_table = slot;
-    return MUSIC_B200_OK;
+    return retune(h, [&](TableSlot &s) { return build_table_azel(h, s.tabs[0], positions_xyz, wavelength, h->streams[0]); });
 }
 
 int music_b200_process_azel_device(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_azimuth, float *d_elevation,
@@ -2649,11 +2685,7 @@ int music_b200_process_azel_host(music_b200 *h, const float *in_c64, uint32_t nw
 int music_b200_create_channels(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples, uint32_t resolution, uint32_t nfft,
                                uint32_t chan_first, uint32_t chan_count, int taper, int combine, int device)
 {
-    if (!out) return fail(nullptr, MUSIC_B200_EINVAL, "out must not be NULL");
-    *out = nullptr;
-    if (m == 0 || m > MUSIC_B200_MAX_M) return fail(nullptr, MUSIC_B200_EINVAL, "m must be in 1..%d (got %u)", MUSIC_B200_MAX_M, m);
-    if (n == 0 || n >= m) return fail(nullptr, MUSIC_B200_EINVAL, "need 1 <= n < m (got n=%u, m=%u)", n, m);
-    if (nsamples == 0 || nsamples % m != 0) return fail(nullptr, MUSIC_B200_EINVAL, "nsamples must be a positive multiple of m (got %u)", nsamples);
+    if (const int rc = check_create(out, m, n, nsamples)) return rc;
     if (resolution == 0) return fail(nullptr, MUSIC_B200_EINVAL, "resolution must be > 0");
     if (nfft < (uint32_t)CHAN_MIN_F || nfft > (uint32_t)CHAN_MAX_F || (nfft & (nfft - 1)) != 0)
         return fail(nullptr, MUSIC_B200_EINVAL, "nfft must be a power of two in %d..%d (got %u)", CHAN_MIN_F, CHAN_MAX_F, nfft);
@@ -2687,24 +2719,23 @@ double channel_offset(const ChanShape &cs, int c)
     return (double)(b < cs.F / 2 ? b : b - cs.F) / (double)cs.F;
 }
 
-// The focusing matrices and errors of table slot `slot` (music_focus.cuh) from its channel tables' geometry and the
+// The focusing matrices and errors of table slot s (music_focus.cuh) from its channel tables' geometry and the
 // handle's sector: B_c on the device, the polar factors on the host, then the errors on the device.  On EINVAL (a
 // singular B_c) the slot's matrices are left as they were.
-int build_focusing(music_b200 *h, int slot, cudaStream_t st)
+int build_focusing(music_b200 *h, TableSlot &s, cudaStream_t st)
 {
     const int C = h->cshape.C, M = (int)h->m, ref = C / 2;
     const size_t MM = (size_t)M * M;
-    if (!h->foc_T[slot]) CU(h, cudaMalloc(&h->foc_T[slot], (size_t)C * MM * sizeof(double2)));
-    if (!h->foc_B) CU(h, cudaMalloc(&h->foc_B, (size_t)C * MM * sizeof(double2)));
-    if (!h->foc_lam) CU(h, cudaMalloc(&h->foc_lam, (size_t)C * sizeof(double)));
-    if (!h->foc_e2) CU(h, cudaMalloc(&h->foc_e2, (size_t)C * sizeof(double)));
+    CU(h, h->foc_B.grow((size_t)C * MM));
+    CU(h, h->foc_lam.grow(C));
+    CU(h, h->foc_e2.grow(C));
     FocusGeom g = {};
-    for (int i = 0; i < 2 * M; ++i) g.pos[i] = h->ctab[slot][0].geo.pos[i];
+    for (int i = 0; i < 2 * M; ++i) g.pos[i] = s.tabs[0].geo.pos[i];
     g.M = M; g.K = (int)h->K; g.C = C; g.ref = ref;
     g.first = (int)h->foc_first;
     g.count = h->foc_count ? (int)h->foc_count : (int)h->K;
     std::vector<double> lam(C);
-    for (int c = 0; c < C; ++c) lam[c] = h->ctab[slot][c].geo.lambda;
+    for (int c = 0; c < C; ++c) lam[c] = s.tabs[c].geo.lambda;
     CU(h, cudaMemcpyAsync(h->foc_lam, lam.data(), C * sizeof(double), cudaMemcpyHostToDevice, st));
     focus_setup_kernel<<<C, FOCUS_THREADS, 0, st>>>(g, h->foc_lam, nullptr, h->foc_B, nullptr);
     h->launches++;
@@ -2721,16 +2752,16 @@ int build_focusing(music_b200 *h, int slot, cudaStream_t st)
             return fail(h, MUSIC_B200_EINVAL, "the focusing matrix of channel %d is singular on this sector (sigma_min <= %g sigma_max): "
                                               "widen the sector", c, FOCUS_SINGULAR);
     }
-    CU(h, cudaMemcpyAsync(h->foc_T[slot], T.data(), T.size() * sizeof(double2), cudaMemcpyHostToDevice, st));
-    focus_setup_kernel<<<C, FOCUS_THREADS, 0, st>>>(g, h->foc_lam, h->foc_T[slot], nullptr, h->foc_e2);
+    CU(h, cudaMemcpyAsync(s.foc_T, T.data(), T.size() * sizeof(double2), cudaMemcpyHostToDevice, st));
+    focus_setup_kernel<<<C, FOCUS_THREADS, 0, st>>>(g, h->foc_lam, s.foc_T, nullptr, h->foc_e2);
     h->launches++;
     CU(h, cudaGetLastError());
     std::vector<double> e2(C);
     CU(h, cudaMemcpyAsync(e2.data(), h->foc_e2, C * sizeof(double), cudaMemcpyDeviceToHost, st));
     CU(h, cudaStreamSynchronize(st));  // T and e2 are locals
-    h->foc_err[slot].assign(C, 0.0);
+    s.foc_err.assign(C, 0.0);
     for (int c = 0; c < C; ++c)
-        if (c != ref) h->foc_err[slot][c] = std::sqrt(e2[c]) / std::sqrt((double)M * g.count);
+        if (c != ref) s.foc_err[c] = std::sqrt(e2[c]) / std::sqrt((double)M * g.count);
     return MUSIC_B200_OK;
 }
 
@@ -2747,22 +2778,17 @@ int music_b200_set_geometry_channels(music_b200 *h, const double *positions_xy, 
     if (!std::isfinite(centre_frequency_hz) || !(centre_frequency_hz > 0.5 * sample_rate_hz))
         return fail(h, MUSIC_B200_EINVAL, "the centre frequency must be finite and above half the sample rate (every channel frequency must be > 0)");
     std::lock_guard<std::mutex> g(h->mutex);
-    CU(h, cudaSetDevice(h->device));
-    CU(h, cudaDeviceSynchronize());  // as in set_table(): the slot being rebuilt must be idle
-    const int slot = h->cur_table ^ 1;
-    if (const int rc = ensure_channel_tables(h, slot)) return rc;
-    for (int c = 0; c < h->cshape.C; ++c) {
-        const double f_c = sample_rate_hz * channel_offset(h->cshape, c);
-        const double lambda = 299792458.0 / (centre_frequency_hz + f_c);
-        if (const int rc = build_table(h, h->ctab[slot][c], positions_xy, lambda, h->streams[0])) return rc;
-    }
-    if (coherent(h))
-        if (const int rc = build_focusing(h, slot, h->streams[0])) return rc;
-    h->ctab_shared[slot] = false;
-    h->cur_table = slot;
-    h->ctab_set = true;
-    h->chan_fs = sample_rate_hz;
-    return MUSIC_B200_OK;
+    const int rc = retune(h, [&](TableSlot &s) {
+        for (int c = 0; c < h->cshape.C; ++c) {
+            const double f_c = sample_rate_hz * channel_offset(h->cshape, c);
+            const double lambda = 299792458.0 / (centre_frequency_hz + f_c);
+            if (const int rb = build_table(h, s.tabs[c], positions_xy, lambda, h->streams[0])) return rb;
+        }
+        s.shared = false;
+        return coherent(h) ? build_focusing(h, s, h->streams[0]) : MUSIC_B200_OK;
+    });
+    if (rc == MUSIC_B200_OK) h->chan_fs = sample_rate_hz;
+    return rc;
 }
 
 int music_b200_channel_frequencies(music_b200 *h, double *offsets_hz)
@@ -2783,9 +2809,9 @@ int music_b200_get_table_channel(music_b200 *h, uint32_t channel, float *table_c
     if (!table_c64) return fail(h, MUSIC_B200_EINVAL, "output table must not be NULL");
     if (channel >= (uint32_t)h->cshape.C) return fail(h, MUSIC_B200_EINVAL, "channel %u out of range (0..%d)", channel, h->cshape.C - 1);
     std::lock_guard<std::mutex> g(h->mutex);
-    if (!h->ctab_set) return fail(h, MUSIC_B200_EINVAL, "no array response yet: call music_b200_set_geometry_channels() or music_b200_set_table()");
+    if (!has_table(h)) return fail(h, MUSIC_B200_EINVAL, "no array response yet: call music_b200_set_geometry_channels() or music_b200_set_table()");
     CU(h, cudaSetDevice(h->device));
-    CU(h, cudaMemcpy(table_c64, channel_table(h, (int)channel).c64, (size_t)h->K * h->m * 2 * sizeof(float), cudaMemcpyDeviceToHost));
+    CU(h, cudaMemcpy(table_c64, table(h, (int)channel).c64, (size_t)h->K * h->m * 2 * sizeof(float), cudaMemcpyDeviceToHost));
     return MUSIC_B200_OK;
 }
 
@@ -2800,30 +2826,26 @@ int music_b200_set_focusing(music_b200 *h, uint32_t first_bin, uint32_t bin_coun
     const uint32_t first0 = h->foc_first, count0 = h->foc_count;
     h->foc_first = first_bin;
     h->foc_count = bin_count;
-    if (!h->ctab_set) return MUSIC_B200_OK;  // the next set_geometry_channels() focuses on this sector
-    // As a retune does: fill the idle table slot (the current slot's channel tables, new matrices) and switch to it, so
-    // the current slot is never rewritten under a call; the slot being refilled must be idle, as in set_table().
-    CU(h, cudaSetDevice(h->device));
-    CU(h, cudaDeviceSynchronize());
-    const int cur = h->cur_table, slot = cur ^ 1;
-    if (const int rc = ensure_channel_tables(h, slot)) return rc;
-    const size_t C = (size_t)h->cshape.C;
-    CU(h, cudaMemcpy(h->ctab_c64[slot], h->ctab_c64[cur], C * h->K * h->m * 2 * sizeof(float), cudaMemcpyDeviceToDevice));
-    CU(h, cudaMemcpy(h->ctab_soa[slot], h->ctab_soa[cur], C * soa_doubles(h->K, h->m) * sizeof(double), cudaMemcpyDeviceToDevice));
-    for (size_t c = 0; c < C; ++c) {
-        DeviceTable t = h->ctab[cur][c];  // geometry, ULA test and flags; the slot's own buffers
-        t.c64 = h->ctab[slot][c].c64;
-        t.soa = h->ctab[slot][c].soa;
-        h->ctab[slot][c] = t;
-    }
-    if (const int rc = build_focusing(h, slot, h->streams[0])) {
+    if (!has_table(h)) return MUSIC_B200_OK;  // the next set_geometry_channels() focuses on this sector
+    // a retune to the current slot's channel tables with new matrices
+    const TableSlot &cur = cur_slot(h);
+    const int rc = retune(h, [&](TableSlot &s) {
+        CU(h, cudaMemcpy(s.c64, cur.c64, cur.c64.size() * sizeof(float), cudaMemcpyDeviceToDevice));
+        CU(h, cudaMemcpy(s.soa, cur.soa, cur.soa.size() * sizeof(double), cudaMemcpyDeviceToDevice));
+        for (size_t c = 0; c < s.tabs.size(); ++c) {
+            DeviceTable t = cur.tabs[c];  // geometry, ULA test and flags; the slot's own buffers
+            t.c64 = s.tabs[c].c64;
+            t.soa = s.tabs[c].soa;
+            s.tabs[c] = t;
+        }
+        s.shared = false;
+        return build_focusing(h, s, h->streams[0]);
+    });
+    if (rc) {
         h->foc_first = first0;
         h->foc_count = count0;
-        return rc;
     }
-    h->ctab_shared[slot] = false;
-    h->cur_table = slot;
-    return MUSIC_B200_OK;
+    return rc;
 }
 
 int music_b200_get_focusing(music_b200 *h, double *T, double *err)
@@ -2831,12 +2853,13 @@ int music_b200_get_focusing(music_b200 *h, double *T, double *err)
     if (!h) return MUSIC_B200_EINVAL;
     if (!coherent(h)) return fail(h, MUSIC_B200_EINVAL, "get_focusing needs a channel handle with the COHERENT combine");
     std::lock_guard<std::mutex> g(h->mutex);
-    if (!h->ctab_set) return fail(h, MUSIC_B200_EINVAL, "no focusing yet: call music_b200_set_geometry_channels()");
+    if (!has_table(h)) return fail(h, MUSIC_B200_EINVAL, "no focusing yet: call music_b200_set_geometry_channels()");
     CU(h, cudaSetDevice(h->device));
+    const TableSlot &s = cur_slot(h);
     const size_t C = (size_t)h->cshape.C;
-    if (T) CU(h, cudaMemcpy(T, h->foc_T[h->cur_table], C * h->m * h->m * sizeof(double2), cudaMemcpyDeviceToHost));
+    if (T) CU(h, cudaMemcpy(T, s.foc_T, C * h->m * h->m * sizeof(double2), cudaMemcpyDeviceToHost));
     if (err)
-        for (size_t c = 0; c < C; ++c) err[c] = h->foc_err[h->cur_table][c];
+        for (size_t c = 0; c < C; ++c) err[c] = s.foc_err[c];
     return MUSIC_B200_OK;
 }
 
@@ -2881,19 +2904,15 @@ int music_b200_process_channels_host(music_b200 *h, const float *in_c64, uint32_
         p.off = need;
         if (p.want) need += align(p.nrows * p.row_bytes * chunk);
     }
-    if (need > h->chan_arena_cap) {
+    if (need > h->chan_arena.size()) {
         CU(h, cudaDeviceSynchronize());
-        cudaFree(h->chan_arena);
-        h->chan_arena = nullptr;
-        h->chan_arena_cap = 0;
-        CU(h, cudaMalloc(&h->chan_arena, need));
-        h->chan_arena_cap = need;
+        CU(h, h->chan_arena.grow(need));
     }
     cudaStream_t st = h->streams[0];
     int rc = MUSIC_B200_OK;
     for (uint32_t w0 = 0; w0 < nwindows && rc == MUSIC_B200_OK; w0 += chunk) {
         const uint32_t W = std::min(chunk, nwindows - w0);
-        float *d_in = reinterpret_cast<float *>(h->chan_arena);
+        float *d_in = reinterpret_cast<float *>(h->chan_arena.get());
         CU_BREAK(h, rc, cudaMemcpyAsync(d_in, in_c64 + (size_t)w0 * h->nsamples * 2, (size_t)W * win_bytes, cudaMemcpyHostToDevice, st));
         const auto dev = [&](int i) { return pc[i].want ? h->chan_arena + pc[i].off : nullptr; };
         Outputs o = caller_outputs(reinterpret_cast<float *>(dev(0)), reinterpret_cast<float *>(dev(1)), reinterpret_cast<float *>(dev(4)),
@@ -2919,35 +2938,12 @@ void music_b200_destroy(music_b200 *h)
 {
     if (!h) return;
     for (music_b200 *c : h->kids) music_b200_destroy(c);
-    h->kids.clear();
     cudaSetDevice(h->device);
     cudaDeviceSynchronize();
     for (const music_b200::HostReg &r : h->hostregs) cudaHostUnregister(reinterpret_cast<void *>(r.base));
-    h->hostregs.clear();
-    for (int p = 0; p < MAX_PEERS; ++p)
-        if (h->peer_ipc[p]) { cudaIpcCloseMemHandle(h->gather.peer[p]); cudaIpcCloseMemHandle(h->peer_flags[p]); }
-    cudaFree(h->gather_buf);
-    cudaFree(h->gather_flags);
+    for (void *p : h->ipc_maps) cudaIpcCloseMemHandle(p);
     cudaGetLastError();
-    free_host_staging(h);
-    cudaFree(h->fused_trace);
-    cudaFree(h->f8_stats);
-    cudaFree(h->work_ctr);
-    cudaFree(h->cal_acc); cudaFree(h->cal_part); cudaFree(h->cal_ctr); cudaFree(h->cal_out);
-    cudaFree(h->chan_tw); cudaFree(h->chan_taper_d); cudaFree(h->chan_arena);
-    cudaFree(h->foc_T[0]); cudaFree(h->foc_T[1]); cudaFree(h->foc_lam); cudaFree(h->foc_B); cudaFree(h->foc_e2); cudaFree(h->foc_Rc);
-    for (int i = 0; i < 2; ++i) { cudaFree(h->ctab_c64[i]); cudaFree(h->ctab_soa[i]); }
-    cudaFree(h->steer_pos); cudaFree(h->steer_count); cudaFree(h->steer_list); cudaFree(h->steer_vals);
-    if (h->fused_done) cudaEventDestroy(h->fused_done);
-    for (int i = 0; i < 2; ++i) {
-        cudaFree(h->table[i].c64); cudaFree(h->table[i].soa); cudaFree(h->table[i].fz); cudaFree(h->table[i].na_max);
-        if (h->streams[i]) cudaStreamDestroy(h->streams[i]);
-        cudaFree(h->ws[i].R); cudaFree(h->ws[i].ev); cudaFree(h->ws[i].Vt); cudaFree(h->ws[i].P64); cudaFree(h->ws[i].cnt); cudaFree(h->ws[i].bins);
-        cudaFree(h->ws[i].wts);
-        if (h->ws[i].scan_done) cudaEventDestroy(h->ws[i].scan_done);
-    }
-    for (cudaEvent_t e : h->tev) cudaEventDestroy(e);
-    delete h;
+    delete h;  // the streams, events and buffers with it, on the device made current above
 }
 
 }  // extern "C"

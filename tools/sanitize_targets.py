@@ -1,7 +1,9 @@
 #!/usr/bin/env python
 """Small invocations of the kernels compute-sanitizer should look at (SURVEY.md section 5): run as
   compute-sanitizer --tool racecheck|memcheck|synccheck python tools/sanitize_targets.py <target>
-targets: fused (C1-size windows, 2000 of them + a ragged 1187 + a drain-only 9), fused_jacobi, fused8, covn8, covn16, eig16, multi"""
+targets: fused (C1-size windows, 2000 of them + a ragged 1187 + a drain-only 9), fused_jacobi, fused8, covn8, covn16, eig16, multi,
+lifecycle (every handle kind created, retuned, grown and destroyed through the host entry points; run it under
+  compute-sanitizer --tool memcheck --leak-check full, which reports what a handle leaves allocated)"""
 import os
 import sys
 
@@ -54,3 +56,68 @@ elif target == "multi":
     blk.work(W, [x], [ang])
     print("multi ok", ang[:4, 0])
     blk.close()
+elif target == "lifecycle":
+    # Host entry points only: device memory torch allocated would be reported as a leak.  The primary context is reset
+    # at the end, because compute-sanitizer reports the allocations still live when a context is destroyed.  The handles
+    # take turns on the same input arrays, so none registers caller memory (a range stays registered to the handle that
+    # registered it).
+    import ctypes
+
+    os.environ["MUSIC_B200_HOSTREG"] = "0"
+
+    from gr_baz_b200.music_doa_azel import music_doa_azel
+    from gr_baz_b200.music_doa_channels import music_doa_channels
+
+    cfg = synth.config(1)
+    resp, table = bench.table_for(cfg)
+    rng = np.random.default_rng(5)
+    m, n, ns, K = cfg["m"], cfg["n"], cfg["nsamples"], cfg["resolution"]
+    x = synth.gen_windows_numpy(cfg, 9, 0, 600)
+    pos = np.array([[0.5 * i, 0.0] for i in range(m)]) * synth.C_LIGHT / synth.FREQUENCY
+    lam = synth.C_LIGHT / synth.FREQUENCY
+
+    def work(blk, W, ports):
+        outs = [np.zeros((W, s), np.float32) for s in ports]
+        blk.work(W, [x[:W]], outs)
+
+    for devices in (None, [0]):
+        blk = music_doa(m, n, ns, resp, K, devices=devices)
+        work(blk, 16, [n, n])                      # fused path
+        blk.set_array_geometry(pos, lam)           # retunes: every slot refilled after it has been current
+        blk.set_array_response(resp)
+        blk.set_array_geometry(pos[::-1].copy(), lam)
+        blk.set_source_rule("mdl")                 # unfused: workspace and staging grow
+        work(blk, 40, [n, n])
+        work(blk, 600, [n, n, K])
+        blk.set_beamformer("das")
+        work(blk, 300, [n, n])
+        blk.set_source_rule("fixed")
+        blk.set_beamformer("off")
+        if devices is None:
+            blk.calibrate(x[:64], 0.0, kind="phase")
+            blk.reduce_angles(np.zeros((8, n), np.float32), np.ones((8, n), np.float32), weighted=True)
+            blk.reduce_spectrum(np.ones((8, K), np.float32))
+            blk.gather_attach(1, 0, [blk.gather_create(64)])
+        blk.close()
+    az = music_doa_azel(m, n, ns, 36, 4, (0.0, 45.0), np.c_[pos, np.zeros(m)], lam)
+    for i in range(3):
+        az.set_array_geometry(np.c_[pos * (1.0 + 0.1 * i), np.zeros(m)], lam)
+    outs = [np.zeros((100, s), np.float32) for s in (n, n, n, az.resolution)]
+    az.work(100, [x[:100]], outs)
+    az.close()
+    for combine in ("separate", "incoherent", "coherent"):
+        ch = music_doa_channels(m, n, ns, 90, 16, (14, 5), "hann", combine, np.asarray(synth.antenna_array("uca", m)), 0.3, 400e6, 56e6)
+        ch.set_array_geometry(np.asarray(synth.antenna_array("uca", m)) * 0.35, 420e6, 56e6)
+        if combine == "coherent":
+            ch.set_focusing(10, 60)
+        else:
+            ch.set_array_response(rng.standard_normal((90, m)) + 1j * rng.standard_normal((90, m)))
+        ch.set_array_geometry(np.asarray(synth.antenna_array("uca", m)) * 0.3, 380e6, 56e6)
+        for W in (8, 200):
+            ch.process_host(x, W, spectrum=True, counts=combine != "incoherent", R=True)
+        ch.close()
+    libcuda = ctypes.CDLL("libcuda.so.1")
+    dev0 = ctypes.c_int()
+    assert libcuda.cuDeviceGet(ctypes.byref(dev0), 0) == 0
+    assert libcuda.cuDevicePrimaryCtxReset(dev0) == 0
+    print("lifecycle ok")
