@@ -83,6 +83,8 @@ def load():
         L.music_b200_set_geometry.restype = ctypes.c_int
         L.music_b200_steer_entry_host.argtypes = [fp, ctypes.c_double, u32, u32, u32, fp]
         L.music_b200_steer_entry_host.restype = None
+        L.music_b200_manifold_coeffs_host.argtypes = [fp, u32, ctypes.c_double, ctypes.POINTER(u32), fp]
+        L.music_b200_manifold_coeffs_host.restype = ctypes.c_int
         L.music_b200_get_table.argtypes = [vp, fp]
         L.music_b200_get_table.restype = ctypes.c_int
         L.music_b200_process_host.argtypes = [vp, fp, u32, fp, fp, fp, fp]
@@ -161,7 +163,7 @@ EXPORTS = [
     "music_b200_process_device_sharded", "music_b200_gather_create", "music_b200_gather_attach", "music_b200_gather_wait",
     "music_b200_gather_buffer", "music_b200_gather_read", "music_b200_set_table", "music_b200_set_geometry", "music_b200_set_peak_mode", "music_b200_set_source_rule", "music_b200_set_refine", "music_b200_set_estimator", "music_b200_reduce_angles_device",
     "music_b200_reduce_spectrum_device", "music_b200_reduce_angles_host", "music_b200_reduce_spectrum_host",
-    "music_b200_get_table", "music_b200_steer_entry_host", "music_b200_process_host",
+    "music_b200_get_table", "music_b200_steer_entry_host", "music_b200_manifold_coeffs_host", "music_b200_process_host",
     "music_b200_process_device", "music_b200_process_device_ex", "music_b200_process_host_counts",
     "music_b200_process_device_counts", "music_b200_process_planar_host",
     "music_b200_process_planar_device", "music_b200_launch_count",

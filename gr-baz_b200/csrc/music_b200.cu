@@ -33,6 +33,7 @@
 #include "music_azel.cuh"
 #include "music_estimators.cuh"
 #include "music_roots.cuh"
+#include "music_manifold.cuh"
 #include "music_esprit.cuh"
 #include "music_dml.cuh"
 #include "music_beams.cuh"
@@ -103,6 +104,9 @@ struct DeviceTable {
     RefineGeom geo = {};          // element positions and wavelength of a geometric table (peak refinement)
     AzelGeom ageo = {};           // the same for an az-el handle (music_b200_create_azel): [M][x, y, z] and the grid
     UlaGeom ula = {};             // whether `geo` is a uniform linear array the root mode accepts, and its p_0 and step
+    uint32_t mf_L = 0;            // manifold order of `geo` (0: none built); above MF_MAX_L the mode refuses the table
+    double mf_aperture = 0.0;     // largest element distance over lambda (the refusal's message)
+    const double2 *mf_beta = nullptr;  // [pairs][mf_L + 1] manifold coefficients, in the slot's mf_beta
 };
 
 // One slot of the steering-table double buffer (retune()).  `tabs` holds C tables (C: the channel count on a channel
@@ -117,6 +121,7 @@ struct TableSlot {
     bool shared = false;       // one table from set_table() (tabs[0]) serves every channel
     DevBuf<double2> foc_T;     // COHERENT channel handle: the focusing matrices T_c [C][m][m] of these tables
     std::vector<double> foc_err;  // and their focusing errors e_c
+    DevBuf<double2> mf_beta;   // the manifold coefficients of the table the MANIFOLD mode reads (build_manifold)
 };
 
 // A non-owning view of a workspace slot's buffers, or of one channel's run of them (enqueue_channels)
@@ -443,8 +448,12 @@ UlaGeom ula_geometry(const double *pos, int M, double lambda)
     return u;
 }
 
-// The peak modes that take their angles from the ULA geometry instead of the table: ROOTS and ESPRIT
-bool gridless_ula(int peak) { return peak == MUSIC_B200_PEAKS_ROOTS || peak == MUSIC_B200_PEAKS_ESPRIT; }
+// The peak modes that take their angles from the geometry instead of the table: ROOTS and ESPRIT (uniform linear
+// arrays) and MANIFOLD (any planar array)
+bool gridless_mode(int peak)
+{
+    return peak == MUSIC_B200_PEAKS_ROOTS || peak == MUSIC_B200_PEAKS_ESPRIT || peak == MUSIC_B200_PEAKS_MANIFOLD;
+}
 
 bool coherent(const music_b200 *h) { return h->chan && h->chan_combine == MUSIC_B200_CHANNELS_COHERENT; }
 
@@ -456,11 +465,12 @@ uint32_t snapshots(const music_b200 *h)
 }
 
 // Whether handle h can run with modes p; if not, records why and returns EINVAL.  With a table t, also whether p can run
-// on it: the gridless ULA peak modes need a ULA geometry, the refinement a geometric table.  Tables are checked on handles that
+// on it: the gridless ULA peak modes need a ULA geometry, the manifold mode a geometric table of order <= MF_MAX_L, the
+// refinement a geometric table.  Tables are checked on handles that
 // hold one (single-device handles, and the children of a multi-device handle).
 int check_modes(music_b200 *h, const Modes &p, const DeviceTable *t)
 {
-    if (p.peak != MUSIC_B200_PEAKS_TOP_BINS && p.peak != MUSIC_B200_PEAKS_LOCAL_MAXIMA && !gridless_ula(p.peak) &&
+    if (p.peak != MUSIC_B200_PEAKS_TOP_BINS && p.peak != MUSIC_B200_PEAKS_LOCAL_MAXIMA && !gridless_mode(p.peak) &&
         p.peak != MUSIC_B200_PEAKS_DML)
         return fail(h, MUSIC_B200_EINVAL, "unknown peak mode %d", p.peak);
     if (p.excl >= h->K) return fail(h, MUSIC_B200_EINVAL, "exclusion_bins must be < resolution");
@@ -476,19 +486,26 @@ int check_modes(music_b200 *h, const Modes &p, const DeviceTable *t)
     if (h->chan && !coherent(h)) {
         // per channel only the grid modes are built (include/music_b200.h lists the rest as not built)
         if (p.peak != MUSIC_B200_PEAKS_TOP_BINS && p.peak != MUSIC_B200_PEAKS_LOCAL_MAXIMA)
-            return fail(h, MUSIC_B200_EINVAL, "a channel handle takes the TOP_BINS and LOCAL_MAXIMA peak modes only (ROOTS, ESPRIT and DML "
-                                              "per channel are not built)");
+            return fail(h, MUSIC_B200_EINVAL, "a channel handle takes the TOP_BINS and LOCAL_MAXIMA peak modes only (ROOTS, ESPRIT, "
+                                              "MANIFOLD and DML per channel are not built)");
         if (p.refine != MUSIC_B200_REFINE_OFF) return fail(h, MUSIC_B200_EINVAL, "peak refinement is not built for channel handles");
         if (h->chan_combine == MUSIC_B200_CHANNELS_INCOHERENT && p.est != MUSIC_B200_ESTIMATOR_MUSIC)
             return fail(h, MUSIC_B200_EINVAL, "the INCOHERENT combine is defined for the MUSIC estimator only");
     }
-    if (gridless_ula(p.peak)) {
-        const char *name = p.peak == MUSIC_B200_PEAKS_ROOTS ? "root" : "ESPRIT";
+    if (gridless_mode(p.peak)) {
+        const bool mf = p.peak == MUSIC_B200_PEAKS_MANIFOLD;
+        const char *name = p.peak == MUSIC_B200_PEAKS_ROOTS ? "root" : mf ? "manifold" : "ESPRIT";
         if (p.excl != 0) return fail(h, MUSIC_B200_EINVAL, "the %s peak mode takes exclusion_bins = 0", name);
         if (h->azel) return fail(h, MUSIC_B200_EINVAL, "the %s peak mode is not supported on an az-el handle", name);
         if (p.est != MUSIC_B200_ESTIMATOR_MUSIC) return fail(h, MUSIC_B200_EINVAL, "the %s peak mode needs the MUSIC estimator", name);
         if (p.refine != MUSIC_B200_REFINE_OFF) return fail(h, MUSIC_B200_EINVAL, "the %s peak mode needs refinement off", name);
-        if (t && !(t->geometric && t->ula.ula))
+        if (t && mf && !t->geometric)
+            return fail(h, MUSIC_B200_EINVAL, "the manifold peak mode needs a table built by music_b200_set_geometry() (call "
+                                              "set_geometry(), or another peak mode)");
+        if (t && mf && t->mf_L > (uint32_t)MF_MAX_L)
+            return fail(h, MUSIC_B200_EINVAL, "the manifold peak mode needs an aperture of about 4.4 wavelengths or less: this "
+                                              "geometry spans %.4g wavelengths (order %u > %d)", t->mf_aperture, t->mf_L, MF_MAX_L);
+        if (t && !mf && !(t->geometric && t->ula.ula))
             return fail(h, MUSIC_B200_EINVAL, "the %s peak mode needs a table built by music_b200_set_geometry() from a uniform linear "
                                               "array with spacing <= lambda / 2 (call set_geometry(), or another peak mode)", name);
     }
@@ -587,6 +604,23 @@ int build_table(music_b200 *h, DeviceTable &t, const double *pos_xy, double lamb
     return MUSIC_B200_OK;
 }
 
+// The manifold order and coefficients (music_manifold.cuh) of the geometric table t into slot s: the table the MANIFOLD
+// peak mode reads, a plain handle's or a COHERENT channel handle's reference channel's.  Built at every such retune, so
+// a slot's table and coefficients always come from one geometry.  A geometry above the order cap keeps its order (for
+// the refusal) and no coefficients.
+int build_manifold(music_b200 *h, TableSlot &s, DeviceTable &t)
+{
+    const int M = (int)h->m;
+    t.mf_beta = nullptr;
+    if (!manifold_coeffs_host(t.geo.pos, M, t.geo.lambda, &t.mf_L, nullptr, &t.mf_aperture)) return MUSIC_B200_OK;
+    std::vector<double> beta((size_t)M * (M - 1) / 2 * (t.mf_L + 1) * 2);
+    manifold_coeffs_host(t.geo.pos, M, t.geo.lambda, &t.mf_L, beta.data(), nullptr);
+    CU(h, s.mf_beta.grow(beta.size() / 2));
+    CU(h, cudaMemcpy(s.mf_beta, beta.data(), beta.size() * sizeof(double), cudaMemcpyHostToDevice));
+    t.mf_beta = s.mf_beta;
+    return MUSIC_B200_OK;
+}
+
 // Steering table of an az-el handle, built on the device from the element positions [M][x, y, z] (music_azel.cuh).
 // No host patching: the table is defined to within one float32 ulp, not bit for bit.
 int build_table_azel(music_b200 *h, DeviceTable &t, const double *pos_xyz, double lambda, cudaStream_t st)
@@ -640,7 +674,7 @@ constexpr unsigned CTR_RING = 256;  // ticket-counter pairs per slot (see ticket
 
 enum class Path { Unfused, Fused4, Fused8 };
 enum class Scan { None, Peak1, Grid };                     // scan_peak1_kernel, scan_kernel
-enum class Peaks { None, TopN, Local, Local2D, Roots, Esprit, Dml };  // topn, topn_local, topn_local2d, roots, esprit, dml kernels
+enum class Peaks { None, TopN, Local, Local2D, Roots, Esprit, Manifold, Dml };  // topn, topn_local, topn_local2d, roots, esprit, manifold, dml kernels
 
 // What one call runs, from the handle's modes, the requested outputs and the input form (plan_call).
 struct Plan {
@@ -664,7 +698,7 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
     const bool fixed_n = h->source_rule == MUSIC_B200_SOURCES_FIXED;
     const bool music_est = md.est == MUSIC_B200_ESTIMATOR_MUSIC;
     const bool local = md.peak == MUSIC_B200_PEAKS_LOCAL_MAXIMA;
-    const bool gridless = gridless_ula(md.peak);
+    const bool gridless = gridless_mode(md.peak);
     const bool dml = md.peak == MUSIC_B200_PEAKS_DML;
     Plan p;
     // The fused kernels find the principal eigenvector only, not every eigenvalue a source count needs nor the noise
@@ -697,7 +731,7 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
         p.scan = Scan::Grid;
         p.p64 = !p.argmax || o.P64;
     }
-    if (gridless) p.peaks = md.peak == MUSIC_B200_PEAKS_ROOTS ? Peaks::Roots : Peaks::Esprit;
+    if (gridless) p.peaks = md.peak == MUSIC_B200_PEAKS_ROOTS ? Peaks::Roots : md.peak == MUSIC_B200_PEAKS_ESPRIT ? Peaks::Esprit : Peaks::Manifold;
     else if (dml) p.peaks = Peaks::Dml;
     else if (!p.argmax) p.peaks = local && h->azel ? Peaks::Local2D : local ? Peaks::Local : Peaks::TopN;
     p.decode = h->azel;
@@ -1066,6 +1100,10 @@ int launch_eig_scan(music_b200 *h, const Plan &p, const WsView &ws, uint32_t W, 
     case Peaks::Esprit:
         esprit_kernel<<<(W + ESPRIT_WARPS - 1) / ESPRIT_WARPS, ESPRIT_WARPS * 32, 0, st>>>(ws.Vt, cnt, M, (int)h->n, (int)h->K, (int)W,
                                                                                         tb.geo, tb.ula, po);
+        break;
+    case Peaks::Manifold:
+        manifold_kernel<<<W, manifold_threads((int)tb.mf_L), 0, st>>>(ws.Vt, cnt, M, (int)h->n, (int)h->K, tb.geo, tb.mf_beta,
+                                                                       (int)tb.mf_L, po);
         break;
     case Peaks::Dml:
         // M = 16 runs the runtime-M instantiation (its loops have the same 16-entry bound): the fixed-M one spills
@@ -2014,7 +2052,7 @@ int music_b200_set_peak_mode(music_b200 *h, int mode, uint32_t exclusion_bins)
     Modes p = h->modes;
     p.peak = mode;
     p.excl = exclusion_bins;
-    if (const int rc = check_modes(h, p, gridless_ula(mode) ? own_table(h) : nullptr)) return rc;
+    if (const int rc = check_modes(h, p, gridless_mode(mode) ? own_table(h) : nullptr)) return rc;
     if (const int rc = for_each_child(h, [&](music_b200 *c) { return music_b200_set_peak_mode(c, mode, exclusion_bins); })) return rc;
     h->modes = p;
     return MUSIC_B200_OK;
@@ -2032,7 +2070,10 @@ int music_b200_set_geometry(music_b200 *h, const double *positions_xy, double wa
     std::lock_guard<std::mutex> g(h->mutex);
     if (!h->kids.empty())
         return for_each_child(h, [&](music_b200 *c) { return music_b200_set_geometry(c, positions_xy, wavelength, guarded); });
-    if (const int rc = retune(h, [&](TableSlot &s) { return build_table(h, s.tabs[0], positions_xy, wavelength, h->streams[0]); }))
+    if (const int rc = retune(h, [&](TableSlot &s) {
+            const int rb = build_table(h, s.tabs[0], positions_xy, wavelength, h->streams[0]);
+            return rb ? rb : build_manifold(h, s, s.tabs[0]);
+        }))
         return rc;
     if (guarded) *guarded = h->steer_guarded;
     return MUSIC_B200_OK;
@@ -2042,6 +2083,19 @@ void music_b200_steer_entry_host(const double *positions_xy, double wavelength, 
                                  uint32_t antenna, float *re_im)
 {
     steer_entry_host(positions_xy, wavelength, (int)resolution, (int)step, (int)antenna, &re_im[0], &re_im[1]);
+}
+
+int music_b200_manifold_coeffs_host(const double *positions_xy, uint32_t m, double wavelength, uint32_t *L, double *beta)
+{
+    if (!positions_xy || !L) return fail(nullptr, MUSIC_B200_EINVAL, "positions_xy and L must not be NULL");
+    if (m == 0 || m > MUSIC_B200_MAX_M) return fail(nullptr, MUSIC_B200_EINVAL, "m must be in 1..%d (got %u)", MUSIC_B200_MAX_M, m);
+    if (!(wavelength > 0.0) || !std::isfinite(wavelength)) return fail(nullptr, MUSIC_B200_EINVAL, "wavelength must be positive and finite");
+    for (uint32_t i = 0; i < 2 * m; ++i)
+        if (!std::isfinite(positions_xy[i])) return fail(nullptr, MUSIC_B200_EINVAL, "element positions must be finite");
+    double ap = 0.0;
+    if (!manifold_coeffs_host(positions_xy, (int)m, wavelength, L, beta, &ap))
+        return fail(nullptr, MUSIC_B200_EINVAL, "the geometry spans %.4g wavelengths: manifold order %u > %d", ap, *L, MF_MAX_L);
+    return MUSIC_B200_OK;
 }
 
 int music_b200_get_table(music_b200 *h, float *table_c64)
@@ -2785,7 +2839,9 @@ int music_b200_set_geometry_channels(music_b200 *h, const double *positions_xy, 
             if (const int rb = build_table(h, s.tabs[c], positions_xy, lambda, h->streams[0])) return rb;
         }
         s.shared = false;
-        return coherent(h) ? build_focusing(h, s, h->streams[0]) : MUSIC_B200_OK;
+        if (!coherent(h)) return MUSIC_B200_OK;
+        if (const int rb = build_manifold(h, s, s.tabs[h->cshape.C / 2])) return rb;
+        return build_focusing(h, s, h->streams[0]);
     });
     if (rc == MUSIC_B200_OK) h->chan_fs = sample_rate_hz;
     return rc;
@@ -2832,10 +2888,15 @@ int music_b200_set_focusing(music_b200 *h, uint32_t first_bin, uint32_t bin_coun
     const int rc = retune(h, [&](TableSlot &s) {
         CU(h, cudaMemcpy(s.c64, cur.c64, cur.c64.size() * sizeof(float), cudaMemcpyDeviceToDevice));
         CU(h, cudaMemcpy(s.soa, cur.soa, cur.soa.size() * sizeof(double), cudaMemcpyDeviceToDevice));
+        if (cur.mf_beta.size()) {
+            CU(h, s.mf_beta.grow(cur.mf_beta.size()));
+            CU(h, cudaMemcpy(s.mf_beta, cur.mf_beta, cur.mf_beta.size() * sizeof(double2), cudaMemcpyDeviceToDevice));
+        }
         for (size_t c = 0; c < s.tabs.size(); ++c) {
             DeviceTable t = cur.tabs[c];  // geometry, ULA test and flags; the slot's own buffers
             t.c64 = s.tabs[c].c64;
             t.soa = s.tabs[c].soa;
+            if (t.mf_beta) t.mf_beta = s.mf_beta;
             s.tabs[c] = t;
         }
         s.shared = false;

@@ -111,8 +111,12 @@ class music_doa(object):
         ``"dml"`` = deterministic maximum likelihood by alternating projection: the n table rows whose span captures the
         most power of the covariance, so coherent sources (multipath) are resolved, on any table; levels are
         least-squares source powers.  It needs ``exclusion_bins`` = 0, the "music" estimator and refinement off; use the
-        "fixed" source rule for coherent sources."""
-        modes = {"top_bins": 0, "local_maxima": 1, "roots": 2, "esprit": 3, "dml": 4}
+        "fixed" source rule for coherent sources;
+        ``"manifold"`` = root-MUSIC on any planar array by manifold separation: gridless angles over the whole 360
+        degrees from the roots of one polynomial per window, for a geometry installed with ``set_array_geometry``
+        spanning about 4.4 wavelengths or less.  It has the restrictions of ``"roots"``; on a line array every source
+        also has a mirror root, so use ``"roots"`` or ``"esprit"`` there."""
+        modes = {"top_bins": 0, "local_maxima": 1, "roots": 2, "esprit": 3, "dml": 4, "manifold": 5}
         if mode not in modes:
             raise ValueError("mode must be one of %s" % sorted(modes))
         _capi.check(self._lib.music_b200_set_peak_mode(self._h, modes[mode], int(exclusion_bins)), self._h)

@@ -202,13 +202,63 @@ int music_b200_set_table(music_b200 *h, const float *table_c64);
  * set_table() or set_geometry() is accepted.  It runs the unfused kernels: covariance, the eigensolver only for MDL /
  * AIC, the eigenvalues, the spectrum or P64, the MUSIC scan only for the spectrum or P64, then one DML kernel per
  * sub-batch (one CTA per window for all its searches), timed in the top-n slot of the stage timing.
+ *
+ * MUSIC_B200_PEAKS_MANIFOLD (extension, root-MUSIC by manifold separation): gridless angles over the whole 360 degrees
+ * on any planar array, from the roots of one polynomial per window (Belloni, Richter & Koivunen 2007; Rubsamen &
+ * Gershman 2009).  Covariance, eigensolver, source rules and spectrum are unchanged.
+ *   geometry   the positions p_m = (x_m, y_m) and wavelength set_geometry() recorded with the current table (on a
+ *              COHERENT channel handle the reference channel's geometry and lambda_ref).
+ *   order      rho_max = max_{i<j} ||p_j - p_i|| (fp64 hypot), x = 2 pi rho_max / lambda; L = the smallest integer >= 1
+ *              with L + 1 >= x and 4 tau_{L+1} <= 2^-52, tau_0 = 1, tau_l = tau_{l-1} (x / 2) / l (a running fp64
+ *              product).  Since |J_l(y)| <= (y/2)^l / l!, the truncation moves D by at most M^2 2^-52.  L must be <= 64
+ *              (an aperture of about 4.4 lambda); on lambda / 2 UCAs M = 3, 4, 5, 8, 12, 16 give L = 21, 24, 26, 32, 39, 46.
+ *   table      built in fp64 with the geometry, for each pair i < j in the order (0,1), (0,2), .., (M-2, M-1):
+ *              (rho_ij, theta_ij) the polar form of p_j - p_i, beta_ij,l = (-j)^l J_l(2 pi rho_ij / lambda) e^{-j l theta_ij},
+ *              l = 0 .. L (J_l by Miller's backward recurrence normalised by J_0 + 2 sum J_2k = 1);
+ *              music_b200_manifold_coeffs_host() returns it.
+ *   polynomial G = the M - d noise eigenvectors the scan would use (d = n, or the MDL / AIC count), C = G G^H in fp64;
+ *              c_0 = tr C + 2 sum_{i<j} beta_ij,0 Re C_ij, c_l = sum_{i<j} beta_ij,l (2 Re C_ij for even l, 2 j Im C_ij for
+ *              odd l), l = 1 .. L, c_{-l} = conj(c_l).  Then sum_{|l|<=L} c_l e^{j l t} = D(t) = a(t)^H C a(t) with
+ *              a_m(t) = exp(-j 2 pi (x_m cos t + y_m sin t) / lambda), the refinement's steering.  Q(z) = sum_l c_l z^(l+L),
+ *              degree P = 2L, and on |z| = 1 Q(z) = z^L D(arg z).  Each outermost pair c_{+-l} that is exactly zero
+ *              contributes a root at 0 and one at infinity.
+ *   roots      ROOTS's rules word for word: Aberth-Ehrlich from the Newton-polygon circles, evaluation in 1 / z outside
+ *              the unit circle, the two stop tests (with P for 2M - 2), 100 steps and then no peaks, and the double-root
+ *              merge.
+ *   selection  ROOTS's: sort the P roots by ascending modulus and keep the first P / 2; slots 0 .. d-1 take the d kept
+ *              roots of largest modulus, in descending modulus, exact ties to the lower angle; a kept root at 0 leaves
+ *              its slot unfilled.
+ *   angle      t* = atan2(Im z, Re z) in degrees, + 360 if negative; float cast and 360 -> 0 as in refinement.  The map
+ *              is one-to-one: there is no mirror rule.
+ *   outputs    level = (float)(1 / D(t*)), D the direct fp64 form of the refinement; bin = floor(t* K / 360 + 0.5) mod K.
+ *              Slots d .. n-1, windows with d = 0, windows whose C or roots are not finite and windows with P = 0 (every
+ *              element at one point) report (0, 0, bin -1).  Spectrum, P64, R, eigenvalues and counts are unchanged, and
+ *              the grid scan runs only for the spectrum or P64, as under ROOTS.
+ * Caveats: on a collinear array D is symmetric about the array line, so every source has a mirror root of equal modulus
+ * and the slots fill with mirror pairs (ROOTS and ESPRIT are the modes for line arrays; MANIFOLD accepts them).  Elements
+ * more than lambda / 2 apart carry the grid spectrum's ambiguities.
+ * MANIFOLD has ROOTS's restrictions, checked the same way in either order: exclusion_bins = 0, estimator MUSIC,
+ * refinement OFF, no az-el handle and no SEPARATE / INCOHERENT channel handle; a current table from set_geometry() (a
+ * process_*() call on a set_table() table returns EINVAL, with no fall-back) whose order is <= 64 (EINVAL otherwise,
+ * with the aperture in wavelengths in the message).  COHERENT channel handles, multi-device handles, every 1-D entry
+ * point, calibration and MDL / AIC work as under ROOTS.  It runs the unfused kernels: covariance, eigensolver (+ source
+ * count), [scan], then one manifold kernel per sub-batch (one CTA per window), timed in the top-n slot of the stage
+ * timing.
  */
 #define MUSIC_B200_PEAKS_TOP_BINS 0
 #define MUSIC_B200_PEAKS_LOCAL_MAXIMA 1
 #define MUSIC_B200_PEAKS_ROOTS 2
 #define MUSIC_B200_PEAKS_ESPRIT 3
 #define MUSIC_B200_PEAKS_DML 4
+#define MUSIC_B200_PEAKS_MANIFOLD 5
 int music_b200_set_peak_mode(music_b200 *h, int mode, uint32_t exclusion_bins);
+
+/*
+ * Test hook of MUSIC_B200_PEAKS_MANIFOLD (no device needed): the order L of positions [m][x, y] (metres) at `wavelength`
+ * and, when beta is not NULL, the coefficient table beta[m(m-1)/2][L+1][re, im] the peak mode uses (caller-allocated for
+ * that L: call once with beta NULL to learn it).  Returns EINVAL for L > 64, after writing L, and for invalid arguments.
+ */
+int music_b200_manifold_coeffs_host(const double *positions_xy, uint32_t m, double wavelength, uint32_t *L, double *beta);
 
 /*
  * Source-count rule (extension, no reference counterpart).  MUSIC_B200_SOURCES_FIXED (default) uses the n of

@@ -53,7 +53,9 @@ public:
     void set_array_geometry(const std::vector<std::vector<double> > &positions_xy, double wavelength);
     /* extension: 0 = the reference's n largest bins (default), 1 = n largest local maxima > exclusion_bins apart,
      * 2 = root-MUSIC, 3 = LS-ESPRIT, each on a uniform linear array set by set_array_geometry() (exclusion_bins must be 0),
-     * 4 = deterministic maximum likelihood (coherent sources, any table; exclusion_bins must be 0) */
+     * 4 = deterministic maximum likelihood (coherent sources, any table; exclusion_bins must be 0),
+     * 5 = root-MUSIC by manifold separation on any planar array set by set_array_geometry() spanning <= ~4.4 wavelengths
+     * (exclusion_bins must be 0) */
     void set_peak_mode(int mode, unsigned int exclusion_bins);
     /* extension: 0 = n sources in every window (default), 1 = MDL, 2 = AIC estimate of 0..n sources per window */
     void set_source_rule(int rule);
