@@ -85,6 +85,8 @@ def load():
         L.music_b200_steer_entry_host.restype = None
         L.music_b200_manifold_coeffs_host.argtypes = [fp, u32, ctypes.c_double, ctypes.POINTER(u32), fp]
         L.music_b200_manifold_coeffs_host.restype = ctypes.c_int
+        L.music_b200_azel_lattice_host.argtypes = [fp, u32, ctypes.c_double, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int), fp]
+        L.music_b200_azel_lattice_host.restype = ctypes.c_int
         L.music_b200_get_table.argtypes = [vp, fp]
         L.music_b200_get_table.restype = ctypes.c_int
         L.music_b200_process_host.argtypes = [vp, fp, u32, fp, fp, fp, fp]
@@ -170,6 +172,7 @@ EXPORTS = [
     "music_b200_set_stage_timing", "music_b200_get_stage_times", "music_b200_debug_fused_trace", "music_b200_debug_fused8_stats",
     "music_b200_last_error", "music_b200_destroy",
     "music_b200_create_azel", "music_b200_set_geometry_azel", "music_b200_process_azel_host", "music_b200_process_azel_device",
+    "music_b200_azel_lattice_host",
     "music_b200_set_beamformer", "music_b200_process_device_beams", "music_b200_process_host_beams",
     "music_b200_set_calibration", "music_b200_get_calibration", "music_b200_calib_reset", "music_b200_calib_accumulate_device",
     "music_b200_calib_accumulate_host", "music_b200_calib_solve",

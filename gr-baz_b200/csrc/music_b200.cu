@@ -35,6 +35,7 @@
 #include "music_roots.cuh"
 #include "music_manifold.cuh"
 #include "music_esprit.cuh"
+#include "music_esprit2d.cuh"
 #include "music_dml.cuh"
 #include "music_beams.cuh"
 #include "music_calib.cuh"
@@ -104,6 +105,7 @@ struct DeviceTable {
     RefineGeom geo = {};          // element positions and wavelength of a geometric table (peak refinement)
     AzelGeom ageo = {};           // the same for an az-el handle (music_b200_create_azel): [M][x, y, z] and the grid
     UlaGeom ula = {};             // whether `geo` is a uniform linear array the root mode accepts, and its p_0 and step
+    LatticeGeom lat = {};         // whether `ageo` is a planar lattice the az-el ESPRIT mode accepts, and its steps
     uint32_t mf_L = 0;            // manifold order of `geo` (0: none built); above MF_MAX_L the mode refuses the table
     double mf_aperture = 0.0;     // largest element distance over lambda (the refusal's message)
     const double2 *mf_beta = nullptr;  // [pairs][mf_L + 1] manifold coefficients, in the slot's mf_beta
@@ -426,6 +428,7 @@ bool screen_bounds_table(const float *tab, uint32_t K)
 int upload_table(music_b200 *h, DeviceTable &t, const float *table_c64, cudaStream_t st)
 {
     t.geometric = false;
+    t.lat = {};
     t.screen_ok = h->m != 4 || screen_bounds_table(table_c64, h->K);
     CU(h, cudaMemcpyAsync(t.c64, table_c64, (size_t)h->K * h->m * 2 * sizeof(float), cudaMemcpyHostToDevice, st));
     return finish_table(h, t, st);
@@ -466,7 +469,7 @@ uint32_t snapshots(const music_b200 *h)
 
 // Whether handle h can run with modes p; if not, records why and returns EINVAL.  With a table t, also whether p can run
 // on it: the gridless ULA peak modes need a ULA geometry, the manifold mode a geometric table of order <= MF_MAX_L, the
-// refinement a geometric table.  Tables are checked on handles that
+// az-el ESPRIT mode a planar lattice with n <= d_max, the refinement a geometric table.  Tables are checked on handles that
 // hold one (single-device handles, and the children of a multi-device handle).
 int check_modes(music_b200 *h, const Modes &p, const DeviceTable *t)
 {
@@ -496,16 +499,25 @@ int check_modes(music_b200 *h, const Modes &p, const DeviceTable *t)
         const bool mf = p.peak == MUSIC_B200_PEAKS_MANIFOLD;
         const char *name = p.peak == MUSIC_B200_PEAKS_ROOTS ? "root" : mf ? "manifold" : "ESPRIT";
         if (p.excl != 0) return fail(h, MUSIC_B200_EINVAL, "the %s peak mode takes exclusion_bins = 0", name);
-        if (h->azel) return fail(h, MUSIC_B200_EINVAL, "the %s peak mode is not supported on an az-el handle", name);
+        if (h->azel && p.peak != MUSIC_B200_PEAKS_ESPRIT)
+            return fail(h, MUSIC_B200_EINVAL, "the %s peak mode is not supported on an az-el handle", name);
         if (p.est != MUSIC_B200_ESTIMATOR_MUSIC) return fail(h, MUSIC_B200_EINVAL, "the %s peak mode needs the MUSIC estimator", name);
         if (p.refine != MUSIC_B200_REFINE_OFF) return fail(h, MUSIC_B200_EINVAL, "the %s peak mode needs refinement off", name);
+        if (t && h->azel && !(t->geometric && t->lat.ok))
+            return fail(h, MUSIC_B200_EINVAL, "the ESPRIT peak mode on an az-el handle needs a table built by "
+                                              "music_b200_set_geometry_azel() from a planar lattice array (Mx x My elements "
+                                              "in row-major order, one z, steps <= lambda / 2) (call set_geometry_azel(), or "
+                                              "another peak mode)");
+        if (t && h->azel && h->n > (uint32_t)esp2_dmax(t->lat))
+            return fail(h, MUSIC_B200_EINVAL, "the ESPRIT peak mode on this %d x %d lattice resolves at most %d sources (n = %u)",
+                        t->lat.mx, t->lat.my, esp2_dmax(t->lat), h->n);
         if (t && mf && !t->geometric)
             return fail(h, MUSIC_B200_EINVAL, "the manifold peak mode needs a table built by music_b200_set_geometry() (call "
                                               "set_geometry(), or another peak mode)");
         if (t && mf && t->mf_L > (uint32_t)MF_MAX_L)
             return fail(h, MUSIC_B200_EINVAL, "the manifold peak mode needs an aperture of about 4.4 wavelengths or less: this "
                                               "geometry spans %.4g wavelengths (order %u > %d)", t->mf_aperture, t->mf_L, MF_MAX_L);
-        if (t && !mf && !(t->geometric && t->ula.ula))
+        if (t && !mf && !h->azel && !(t->geometric && t->ula.ula))
             return fail(h, MUSIC_B200_EINVAL, "the %s peak mode needs a table built by music_b200_set_geometry() from a uniform linear "
                                               "array with spacing <= lambda / 2 (call set_geometry(), or another peak mode)", name);
     }
@@ -638,6 +650,7 @@ int build_table_azel(music_b200 *h, DeviceTable &t, const double *pos_xyz, doubl
     if (rc) return rc;
     t.geometric = true;
     t.ageo = g;
+    t.lat = azel_lattice(pos_xyz, M, lambda);
     return MUSIC_B200_OK;
 }
 
@@ -674,7 +687,7 @@ constexpr unsigned CTR_RING = 256;  // ticket-counter pairs per slot (see ticket
 
 enum class Path { Unfused, Fused4, Fused8 };
 enum class Scan { None, Peak1, Grid };                     // scan_peak1_kernel, scan_kernel
-enum class Peaks { None, TopN, Local, Local2D, Roots, Esprit, Manifold, Dml };  // topn, topn_local, topn_local2d, roots, esprit, manifold, dml kernels
+enum class Peaks { None, TopN, Local, Local2D, Roots, Esprit, Esprit2D, Manifold, Dml };  // topn, topn_local, topn_local2d, roots, esprit, esprit2d, manifold, dml kernels
 
 // What one call runs, from the handle's modes, the requested outputs and the input form (plan_call).
 struct Plan {
@@ -731,10 +744,11 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
         p.scan = Scan::Grid;
         p.p64 = !p.argmax || o.P64;
     }
-    if (gridless) p.peaks = md.peak == MUSIC_B200_PEAKS_ROOTS ? Peaks::Roots : md.peak == MUSIC_B200_PEAKS_ESPRIT ? Peaks::Esprit : Peaks::Manifold;
+    if (gridless) p.peaks = md.peak == MUSIC_B200_PEAKS_ROOTS ? Peaks::Roots : md.peak != MUSIC_B200_PEAKS_ESPRIT ? Peaks::Manifold
+                            : h->azel ? Peaks::Esprit2D : Peaks::Esprit;
     else if (dml) p.peaks = Peaks::Dml;
     else if (!p.argmax) p.peaks = local && h->azel ? Peaks::Local2D : local ? Peaks::Local : Peaks::TopN;
-    p.decode = h->azel;
+    p.decode = h->azel && p.peaks != Peaks::Esprit2D;  // the 2-D ESPRIT kernel writes both angles itself
     p.refine = md.refine != MUSIC_B200_REFINE_OFF;
     p.ws_p64 = p.p64 && !o.P64;
     p.ws_counts = p.count;
@@ -1100,6 +1114,10 @@ int launch_eig_scan(music_b200 *h, const Plan &p, const WsView &ws, uint32_t W, 
     case Peaks::Esprit:
         esprit_kernel<<<(W + ESPRIT_WARPS - 1) / ESPRIT_WARPS, ESPRIT_WARPS * 32, 0, st>>>(ws.Vt, cnt, M, (int)h->n, (int)h->K, (int)W,
                                                                                         tb.geo, tb.ula, po);
+        break;
+    case Peaks::Esprit2D:
+        esprit2d_kernel<<<(W + ESP2_WARPS - 1) / ESP2_WARPS, ESP2_WARPS * 32, 0, st>>>(ws.Vt, cnt, M, (int)h->n, (int)W, tb.ageo,
+                                                                                    tb.lat, po, o.elev);
         break;
     case Peaks::Manifold:
         manifold_kernel<<<W, manifold_threads((int)tb.mf_L), 0, st>>>(ws.Vt, cnt, M, (int)h->n, (int)h->K, tb.geo, tb.mf_beta,
@@ -2706,6 +2724,19 @@ int music_b200_set_geometry_azel(music_b200 *h, const double *positions_xyz, dou
     if (rc) return rc;
     std::lock_guard<std::mutex> g(h->mutex);
     return retune(h, [&](TableSlot &s) { return build_table_azel(h, s.tabs[0], positions_xyz, wavelength, h->streams[0]); });
+}
+
+int music_b200_azel_lattice_host(const double *positions_xyz, uint32_t m, double wavelength, int *mx, int *my, double s[4])
+{
+    if (!positions_xyz || !mx || !my || !s) return fail(nullptr, MUSIC_B200_EINVAL, "positions_xyz, mx, my and s must not be NULL");
+    if (m == 0 || m > MUSIC_B200_MAX_M) return fail(nullptr, MUSIC_B200_EINVAL, "m must be in 1..%d (got %u)", MUSIC_B200_MAX_M, m);
+    if (const int rc = check_azel_geometry(nullptr, m, positions_xyz, wavelength)) return rc;
+    const LatticeGeom g = azel_lattice(positions_xyz, (int)m, wavelength);
+    if (!g.ok) return fail(nullptr, MUSIC_B200_EINVAL, "the positions are not a planar lattice with steps <= lambda / 2");
+    *mx = g.mx;
+    *my = g.my;
+    s[0] = g.s1[0], s[1] = g.s1[1], s[2] = g.s2[0], s[3] = g.s2[1];
+    return MUSIC_B200_OK;
 }
 
 int music_b200_process_azel_device(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_azimuth, float *d_elevation,

@@ -35,7 +35,12 @@ __device__ __forceinline__ double2 cscale(double2 a, double s) { return make_dou
 
 // Eigenvalues of the d x d matrix A (row stride ESPRIT_LD, overwritten) into ev[0 .. d-1], by the whole warp; v and g
 // (d entries each) are scratch.  Returns false when a QR step count exceeds ESPRIT_MAX_IT between deflations.
-__device__ bool esprit_eigvals(double2 *A, double2 *v, double2 *g, double2 *ev, int d, int lane)
+// SCHUR: also the complex Schur form A = Z S Z^H (LAPACK zlahqr's wantt and wantz): every QR step updates the whole
+// rows l .. hi (columns k .. d-1) and columns l .. hi (rows 0 .. hi), so A ends upper triangular (its entries below the
+// diagonal are the negligible subdiagonals the QR deflated on, not zeroed), and Z (row stride ESPRIT_LD, the identity
+// on entry) accumulates every Householder reflection and Givens rotation.  Without SCHUR only the active block is kept.
+template <bool SCHUR = false>
+__device__ bool esprit_eigvals(double2 *A, double2 *v, double2 *g, double2 *ev, int d, int lane, double2 *Z = nullptr)
 {
     // Householder reduction to upper Hessenberg form: H = I - tau v v^H zeroes column k below row k + 1
     for (int k = 0; k + 2 < d; ++k) {
@@ -62,6 +67,14 @@ __device__ bool esprit_eigvals(double2 *A, double2 *v, double2 *g, double2 *ev, 
             for (int j = k + 1; j < d; ++j) s = cadd(s, cmul(A[lane * ESPRIT_LD + j], v[j]));
             s = cscale(s, tau);
             for (int j = k + 1; j < d; ++j) A[lane * ESPRIT_LD + j] = csub(A[lane * ESPRIT_LD + j], cmul(s, cconj(v[j])));
+        }
+        if constexpr (SCHUR) {
+            if (lane < d) {  // Z H: row `lane`
+                double2 s = make_double2(0.0, 0.0);
+                for (int j = k + 1; j < d; ++j) s = cadd(s, cmul(Z[lane * ESPRIT_LD + j], v[j]));
+                s = cscale(s, tau);
+                for (int j = k + 1; j < d; ++j) Z[lane * ESPRIT_LD + j] = csub(Z[lane * ESPRIT_LD + j], cmul(s, cconj(v[j])));
+            }
         }
         __syncwarp();
     }
@@ -112,7 +125,7 @@ __device__ bool esprit_eigvals(double2 *A, double2 *v, double2 *g, double2 *ev, 
             const double2 gc = nr > 0.0 ? cscale(x, 1.0 / nr) : make_double2(1.0, 0.0);
             const double2 gs = nr > 0.0 ? cscale(y, 1.0 / nr) : make_double2(0.0, 0.0);
             __syncwarp();
-            if (lane >= k && lane <= hi) {
+            if (lane >= k && lane <= (SCHUR ? d - 1 : hi)) {
                 const double2 u = A[k * ESPRIT_LD + lane], w = A[(k + 1) * ESPRIT_LD + lane];
                 A[k * ESPRIT_LD + lane] = cadd(cmul(cconj(gc), u), cmul(cconj(gs), w));
                 A[(k + 1) * ESPRIT_LD + lane] = csub(cmul(gc, w), cmul(gs, u));
@@ -122,10 +135,17 @@ __device__ bool esprit_eigvals(double2 *A, double2 *v, double2 *g, double2 *ev, 
         }
         for (int k = l; k < hi; ++k) {
             const double2 gc = v[k], gs = g[k];
-            if (lane >= l && lane <= hi) {  // columns k, k + 1 times G_k^H = [c -conj(s); s conj(c)]
+            if (lane >= (SCHUR ? 0 : l) && lane <= hi) {  // columns k, k + 1 times G_k^H = [c -conj(s); s conj(c)]
                 const double2 u = A[lane * ESPRIT_LD + k], w = A[lane * ESPRIT_LD + k + 1];
                 A[lane * ESPRIT_LD + k] = cadd(cmul(u, gc), cmul(w, gs));
                 A[lane * ESPRIT_LD + k + 1] = csub(cmul(w, cconj(gc)), cmul(u, cconj(gs)));
+            }
+            if constexpr (SCHUR) {
+                if (lane < d) {  // the same columns of Z
+                    const double2 u = Z[lane * ESPRIT_LD + k], w = Z[lane * ESPRIT_LD + k + 1];
+                    Z[lane * ESPRIT_LD + k] = cadd(cmul(u, gc), cmul(w, gs));
+                    Z[lane * ESPRIT_LD + k + 1] = csub(cmul(w, cconj(gc)), cmul(u, cconj(gs)));
+                }
             }
             __syncwarp();
         }

@@ -107,7 +107,10 @@ class music_doa(object):
         array with spacing <= lambda / 2 installed with ``set_array_geometry`` (include/music_b200.h).  It needs
         ``exclusion_bins`` = 0, the "music" estimator and refinement off;
         ``"esprit"`` = LS-ESPRIT: gridless angles from the eigenvalues of the signal subspace's shift-invariance matrix,
-        for the same arrays and with the same restrictions as ``"roots"``;
+        for the same arrays and with the same restrictions as ``"roots"``.  On a ``music_doa_azel`` block it is 2-D
+        ESPRIT instead: gridless (azimuth, elevation) pairs for a planar lattice array (Mx x My elements in row-major
+        order, one z, steps <= lambda / 2) installed with ``set_array_geometry``, with no grid scan or 2-D peak pick;
+        it needs n <= min((Mx - 1) My, Mx (My - 1)) besides the restrictions of ``"roots"``;
         ``"dml"`` = deterministic maximum likelihood by alternating projection: the n table rows whose span captures the
         most power of the covariance, so coherent sources (multipath) are resolved, on any table; levels are
         least-squares source powers.  It needs ``exclusion_bins`` = 0, the "music" estimator and refinement off; use the

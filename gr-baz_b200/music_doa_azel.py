@@ -8,6 +8,9 @@ The grid has n_az azimuth steps k * 360 / n_az and n_el elevation steps from el_
 from the xy-plane); the spectrum port carries n_el * n_az floats per window, elevation-major.  The setters, reducers,
 ``last_bins`` / ``last_counts`` and ``close`` are those of :class:`music_doa`; ``last_bins`` holds flat bins
 b = i * n_az + k.  For a planar array use el_lo >= 0: +el and -el have identical steering vectors there.
+``set_peak_mode("esprit")`` selects 2-D ESPRIT on a planar lattice array (a uniform rectangular array, or any other
+Mx x My lattice in row-major element order): gridless (azimuth, elevation) pairs with no grid scan (the spectrum port
+still gets the grid spectrum when it is connected).
 """
 from __future__ import annotations
 

@@ -172,8 +172,9 @@ int music_b200_set_table(music_b200 *h, const float *table_c64);
  *              or P64, as under ROOTS.
  * ESPRIT has ROOTS's restrictions, checked the same way in either order: exclusion_bins = 0, estimator MUSIC,
  * refinement OFF, a current table from set_geometry() of a ULA (a process_*() call on any other table returns EINVAL,
- * with no fall-back to grid peaks), and no az-el handle.  It runs the unfused kernels: covariance, eigensolver (+ source
- * count), [scan], then one ESPRIT kernel per sub-batch, timed in the top-n slot of the stage timing.
+ * with no fall-back to grid peaks).  On an az-el handle the mode is 2-D ESPRIT (defined with the az-el entries below).  It
+ * runs the unfused kernels: covariance, eigensolver (+ source count), [scan], then one ESPRIT kernel per sub-batch, timed
+ * in the top-n slot of the stage timing.
  *
  * MUSIC_B200_PEAKS_DML (extension, deterministic maximum likelihood by alternating projection): the d table rows whose
  * span captures the most power of R, tr(P_A R).  It needs no signal-subspace rank, so it resolves coherent sources (a
@@ -566,6 +567,47 @@ void music_b200_steer_entry_host(const double *positions_xy, double wavelength, 
  * set_geometry_azel: retune, with the locking and double buffering of music_b200_set_table().
  * process_azel_host / _device: as process_host_counts / process_device_counts, plus the elevations (n floats per
  * window, required like the azimuths); levels, spectrum, bins and counts may be NULL.
+ *
+ * MUSIC_B200_PEAKS_ESPRIT on an az-el handle (extension, 2-D LS-ESPRIT): gridless (azimuth, elevation) pairs from the two
+ * shift invariances of a planar lattice (uniform rectangular or any other 2-D lattice) array.  Covariance, eigensolver,
+ * source rules and spectrum are unchanged.  (On a 1-D handle the mode keeps the ULA meaning above.)
+ *   lattice    evaluated on the positions p_m = (x, y, z) at create_azel / set_geometry_azel and kept with the table: for
+ *              each divisor Mx of M with 2 <= Mx <= M / 2, ascending, My = M / Mx, s1 = (p_1 - p_0)_xy,
+ *              s2 = (p_Mx - p_0)_xy.  The geometry is the lattice (Mx, My, s1, s2) when |s1|, |s2| > 0,
+ *              |s1 x s2| > 1e-6 |s1| |s2|, every element m = k Mx + i lies within 1e-6 min(|s1|, |s2|) of
+ *              p_0 + i s1 + k s2 in xy with |z_m - z_0| within the same bound, and |s1|, |s2| <= (lambda / 2)(1 + 1e-12).
+ *              At most one Mx passes.  Row-major element order; column-major passes with s1 and s2 swapped; rotated,
+ *              non-orthogonal (e.g. triangular) lattices, any p_0 and z_0 pass.  music_b200_azel_lattice_host() tests it.
+ *   doublets   P1 = {(m(i, k), m(i + 1, k)) : i < Mx - 1}, P2 = {(m(i, k), m(i, k + 1)) : k < My - 1}, both in ascending
+ *              first index; d_max = min((Mx - 1) My, Mx (My - 1)).
+ *   subspace   E_s = the d eigenvectors of largest eigenvalue (d = n, or the MDL / AIC count); A_j = the rows of E_s at
+ *              the first indices of P_j, B_j = the rows at the second indices.
+ *   matrices   G_j = A_j^H A_j, C_j = A_j^H B_j, Psi_j = G_j^-1 C_j in fp64 by Cholesky of G_j (lower, row by row).  G_j =
+ *              I - (excluded rows)^H (excluded rows) has its eigenvalues in [0, 1]: a pivot <= 2^-40 before its square
+ *              root (or NaN) means no peaks for the window, as do d = 0, d > d_max and a non-finite Psi_j.
+ *   pairing    Psi_c = Psi_1 + gamma Psi_2, gamma = 0.37 + 0.61 j.  Complex Schur form Psi_c = Z S Z^H by ESPRIT's
+ *              Householder + shifted QR (above) with the whole rows and columns updated and Z accumulated (zlahqr's
+ *              wantt / wantz); a window needing more than 30 QR steps between deflations reports no peaks.  Eigenvector
+ *              k of S: y_k = 1, y_j = 0 for j > k, y_j = -(sum_{l=j+1..k} S_jl y_l) / (S_jj - S_kk) for j = k-1 .. 0,
+ *              a divisor of modulus < smin = max(2^-52 |S_kk|, 2^-1022) replaced by smin (LAPACK ztrevc); x_k = Z y_k.
+ *              phi_jk = x_k^H Psi_j x_k / x_k^H x_k, the two phases of one source, already paired.  They depend only on
+ *              span(E_s).
+ *   direction  omega_j = -arg(phi_j) lambda / (2 pi) = s_j . u_xy; [s1; s2] u_xy = omega solved in fp64, rho = |u_xy|;
+ *              az = atan2(u_y, u_x) in degrees wrapped into [0, 360), el = acos(min(rho, 1)) in degrees (>= 0: a planar
+ *              array cannot tell +el from -el), negated when the handle's el_hi <= 0.  A phi exactly 0 or not finite
+ *              leaves its slot unfilled.
+ *   outputs    azimuth, elevation = float casts (360 -> 0 as in refinement); level = (float)(1 / D(az, el)), D the direct
+ *              fp64 form of the refinement over the M - d noise eigenvectors at the unrounded angles; bin = i n_az + k,
+ *              k = floor(az n_az / 360 + 0.5) mod n_az, i = clamp(floor((el - el_lo)(n_el - 1) / (el_hi - el_lo) + 0.5),
+ *              0, n_el - 1) (i = 0 for n_el = 1).  Slots 0 .. d-1 in descending fp64 level, exact ties to the lower
+ *              azimuth, then the lower elevation, then the lower Schur diagonal index.  Slots d .. n-1, windows without
+ *              peaks and windows with a NaN level report (0, 0, 0, bin -1).  Spectrum and counts are unchanged; the grid
+ *              scan runs only when the spectrum is requested; the bin decode does not run.
+ * Restrictions, checked in either order like 1-D ESPRIT: exclusion_bins = 0, estimator MUSIC, refinement OFF; a current
+ * table from set_geometry_azel() of a lattice (a process_*() call on a set_table() table or on another geometry returns
+ * EINVAL, with no fall-back to grid peaks); n <= d_max (the MDL / AIC count never exceeds n, so it never exceeds d_max
+ * either).  ROOTS, MANIFOLD and DML stay refused on az-el handles.  A call runs covariance (+ calibration), eigensolver
+ * (+ source count), [scan], then one ESPRIT kernel per sub-batch, timed in the top-n slot of the stage timing.
  */
 #define MUSIC_B200_AZEL_MAX_BINS (1u << 20)
 int music_b200_create_azel(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples, uint32_t n_az, uint32_t n_el,
@@ -576,6 +618,13 @@ int music_b200_process_azel_host(music_b200 *h, const float *in_c64, uint32_t nw
                                  float *levels, float *spectrum, int32_t *bins, int32_t *counts);
 int music_b200_process_azel_device(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_azimuth, float *d_elevation,
                                    float *d_levels, float *d_spectrum, int32_t *d_bins, int32_t *d_counts, void *stream);
+
+/*
+ * Test hook of the az-el ESPRIT mode's lattice condition (no device needed): for positions [m][x, y, z] (metres) at
+ * `wavelength`, the lattice shape Mx, My and the steps s = {s1_x, s1_y, s2_x, s2_y}.  Returns EINVAL for a geometry that
+ * is not a lattice, and for invalid arguments.
+ */
+int music_b200_azel_lattice_host(const double *positions_xyz, uint32_t m, double wavelength, int *mx, int *my, double s[4]);
 
 /*
  * Frequency-channelised direction finding (extension, no reference counterpart): an FFT filter bank fused into the

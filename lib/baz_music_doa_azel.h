@@ -47,6 +47,8 @@ public:
     /* retune: element positions [m][x, y, z] (metres) and the wavelength; the table is built on the device */
     void set_array_geometry(const std::vector<std::vector<double> > &positions_xyz, double wavelength);
     /* 0 = the n largest bins (default), 1 = the n largest 2-D local maxima more than exclusion_bins apart */
+    // mode 3 (MUSIC_B200_PEAKS_ESPRIT) on a planar lattice geometry: 2-D ESPRIT, gridless (azimuth, elevation) pairs
+    // (include/music_b200.h); ROOTS, DML and MANIFOLD throw std::invalid_argument on this block
     void set_peak_mode(int mode, unsigned int exclusion_bins);
     /* 0 = n sources in every window (default), 1 = MDL, 2 = AIC estimate of 0..n sources per window */
     void set_source_rule(int rule);

@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Small invocations of the kernels compute-sanitizer should look at (SURVEY.md section 5): run as
   compute-sanitizer --tool racecheck|memcheck|synccheck python tools/sanitize_targets.py <target>
-targets: fused (C1-size windows, 2000 of them + a ragged 1187 + a drain-only 9), fused_jacobi, fused8, covn8, covn16, eig16, multi,
+targets: fused (C1-size windows, 2000 of them + a ragged 1187 + a drain-only 9), fused_jacobi, fused8, covn8, covn16, eig16, esprit2d,
+multi,
 lifecycle (every handle kind created, retuned, grown and destroyed through the host entry points; run it under
   compute-sanitizer --tool memcheck --leak-check full, which reports what a handle leaves allocated)"""
 import os
@@ -46,6 +47,23 @@ elif target == "covn16":
     run(synth.config(5, snapshots=512, resolution=360), (300, 19))
 elif target == "eig16":
     run(synth.config(5, snapshots=128, resolution=180), (64,))
+elif target == "esprit2d":
+    # 2-D ESPRIT on az-el handles (music_esprit2d.cuh): 4 x 4 and 2 x 4 lattices, a ragged window count (the last CTA's
+    # idle warps), d = n on noise windows
+    from gr_baz_b200.music_doa_azel import music_doa_azel
+    lam = 0.5
+    for rows, cols, n in ((4, 4, 3), (2, 4, 2)):
+        m = rows * cols
+        pos = np.array([[c * 0.25, r * 0.25, 0.0] for r in range(rows) for c in range(cols)])
+        rng = np.random.default_rng(m)
+        W = 301
+        x = ((rng.standard_normal((W, 64 * m)) + 1j * rng.standard_normal((W, 64 * m))) * 0.1).astype(np.complex64)
+        az = music_doa_azel(m, n, 64 * m, 72, 19, (0.0, 90.0), pos, lam)
+        az.set_peak_mode("esprit", 0)
+        outs = [np.zeros((W, s), np.float32) for s in (n, n, n, az.resolution)]
+        az.work(W, [x], outs)
+        print("esprit2d ok", m, outs[0][:2])
+        az.close()
 elif target == "multi":
     cfg = synth.config(1)
     resp, table = bench.table_for(cfg)
