@@ -39,6 +39,7 @@
 #include "music_dml.cuh"
 #include "music_beams.cuh"
 #include "music_calib.cuh"
+#include "music_integrate.cuh"
 #include "music_channels.cuh"
 #include "music_focus.cuh"
 
@@ -127,16 +128,17 @@ struct TableSlot {
 };
 
 // A non-owning view of a workspace slot's buffers, or of one channel's run of them (enqueue_channels)
-struct WsView { double *R, *ev, *Vt, *P64; int32_t *cnt, *bins; double *wts; };
+struct WsView { double *R, *ev, *Vt, *P64; int32_t *cnt, *bins; double *wts; unsigned long long *n0; };
 
 struct Workspace {
     DevBuf<double> R, ev, Vt, P64;
     DevBuf<int32_t> cnt;   // per-window source counts (source rule other than FIXED)
     DevBuf<int32_t> bins;  // [windows][n] peak bins for the refinement and the beams when the caller asked for none
     DevBuf<double> wts;    // [windows][n][m] complex beam weights when a beams call asked for none
+    DevBuf<unsigned long long> n0;  // integration: the count since the reset at the sub-batch's first window
     cudaEvent_t scan_done = nullptr;
     bool used = false;
-    WsView view() const { return {R, ev, Vt, P64, cnt, bins, wts}; }
+    WsView view() const { return {R, ev, Vt, P64, cnt, bins, wts, n0}; }
 };
 
 // The modes set by set_peak_mode(), set_refine() and set_estimator(); check_modes() says which combine.
@@ -266,6 +268,15 @@ struct music_b200 {
     DevBuf<unsigned> cal_ctr;
     DevBuf<double> cal_out;
     uint64_t cal_windows = 0;
+    // covariance integration (music_b200_set_integration, music_integrate.cuh), on while integ_alpha > 0: the carry S [m][m]
+    // complex and the window count since the reset on the device, the tile scratch, and the event that orders each
+    // sub-batch's integration after the previous one's, on whichever stream that ran.  integ_fresh: the next integration
+    // starts from S = 0 and count 0.
+    double integ_alpha = 0.0;
+    bool integ_fresh = true, integ_used = false;
+    DevBuf<double> integ_S, integ_tiles;
+    DevBuf<unsigned long long> integ_cnt;
+    cudaEvent_t integ_done = nullptr;
     unsigned steer_guarded = 0;    // entries of the last built table re-evaluated with the host libm
     bool azel = false;             // music_b200_create_azel(): K = n_az * n_el rows, elevation-major (music_azel.cuh)
     AzelGrid grid = {};
@@ -341,6 +352,7 @@ struct music_b200 {
             if (ws[i].scan_done) cudaEventDestroy(ws[i].scan_done);
         }
         if (fused_done) cudaEventDestroy(fused_done);
+        if (integ_done) cudaEventDestroy(integ_done);
         for (cudaEvent_t e : tev) cudaEventDestroy(e);
     }
 };
@@ -701,6 +713,7 @@ struct Plan {
     bool decode = false, refine = false;             // az-el bin decode; peak refinement (the az-el kind after a decode)
     bool beams = false;                              // beam weights (+ beams) after the peaks: the beams entry points
     bool calib = false;                              // correct R after the covariance (and the beam weights) by the calibration
+    bool integ = false;                              // then integrate R across windows (music_b200_set_integration)
     bool ws_p64 = false, ws_counts = false, ws_bins = false, ws_wts = false;  // workspace buffers the kernels write
     bool combine = false;                            // channel handle, INCOHERENT: one spectrum per window from all channels
 };
@@ -722,7 +735,8 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
     // A beams call needs R, which the fused kernels keep in registers: it runs the unfused plan of a call that asks for R.
     const bool beams = o.wts || o.beams;
     const bool fusable = h->fused && !h->chan && !h->azel && music_est && fixed_n && md.refine == MUSIC_B200_REFINE_OFF &&
-                         md.peak == MUSIC_B200_PEAKS_TOP_BINS && h->n == 1 && !o.P64 && !o.R && !o.ev && !beams && !h->calib;
+                         md.peak == MUSIC_B200_PEAKS_TOP_BINS && h->n == 1 && !o.P64 && !o.R && !o.ev && !beams && !h->calib &&
+                         h->integ_alpha == 0.0;
     if (fusable && h->m == 4 && planar_fusable && (!o.spec || h->fused_spec)) p.path = Path::Fused4;
     else if (fusable && h->m == 8 && !planar && !o.spec && h->N >= 128 && h->N % 2 == 0) p.path = Path::Fused8;
 
@@ -754,6 +768,7 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
     p.ws_counts = p.count;
     p.beams = beams;
     p.calib = h->calib;
+    p.integ = h->integ_alpha > 0.0;
     p.ws_bins = p.decode || p.refine || (beams && !o.bins);
     p.ws_wts = beams && !o.wts;
     if (h->chan && h->chan_combine == MUSIC_B200_CHANNELS_INCOHERENT) {
@@ -801,6 +816,7 @@ int ensure_slot(music_b200 *h, Workspace &ws, uint32_t windows, const Plan &p)
     if (const int rc = grow(ws.P64, p.ws_p64 ? w * h->K : 0)) return rc;
     if (const int rc = grow(ws.cnt, p.ws_counts ? w : 0)) return rc;
     if (const int rc = grow(ws.bins, p.ws_bins ? w * h->n : 0)) return rc;
+    if (const int rc = grow(ws.n0, p.integ ? 1 : 0)) return rc;
     return grow(ws.wts, p.ws_wts ? w * h->n * h->m * 2 : 0);
 }
 
@@ -1070,7 +1086,11 @@ const int32_t *launch_eig_stage(music_b200 *h, const Plan &p, const WsView &ws, 
     // per-window model order from the eigenvalues just written (timed with the eigensolver)
     const int32_t *cnt = nullptr;
     if (p.count) {
-        source_count_kernel<<<(W + 127) / 128, 128, 0, st>>>(ws.ev, M, (int)h->n, (int)nsnap, h->source_rule, (int)W, ws.cnt, counts_out);
+        if (p.integ)  // N_eff of each window's integrated covariance in place of the snapshot count
+            source_count_neff_kernel<<<(W + 127) / 128, 128, 0, st>>>(ws.ev, M, (int)h->n, (int)nsnap, h->source_rule, (int)W, h->integ_alpha,
+                                                                    ws.n0, ws.cnt, counts_out);
+        else
+            source_count_kernel<<<(W + 127) / 128, 128, 0, st>>>(ws.ev, M, (int)h->n, (int)nsnap, h->source_rule, (int)W, ws.cnt, counts_out);
         h->launches++;
         cnt = ws.cnt;
     }
@@ -1182,6 +1202,38 @@ void launch_cov_planar(music_b200 *h, const WsView &ws, const PlanarStreams &S, 
     }
 }
 
+// The integration of the W covariances in R (music_integrate.cuh) on `st`, after the previous sub-batch's integration on
+// whichever stream that ran: the handle's carry goes from one sub-batch to the next in enqueue order, which is window
+// order within a call (the host entries' chunks alternate between two streams) and call order across calls.
+int launch_integrate(music_b200 *h, const WsView &ws, uint32_t W, cudaStream_t st)
+{
+    const int E = (int)(2 * h->m * h->m), ntiles = (int)((W + INTEG_T - 1) / INTEG_T);
+    const size_t elems = (size_t)ntiles * E;
+    if (elems > h->integ_tiles.size()) {
+        if (h->integ_used) CU(h, cudaEventSynchronize(h->integ_done));  // the last integration may still read the scratch
+        CU(h, h->integ_tiles.grow(elems));
+    }
+    if (h->integ_used) CU(h, cudaStreamWaitEvent(st, h->integ_done, 0));
+    if (h->integ_fresh) {
+        CU(h, cudaMemsetAsync(h->integ_S, 0, (size_t)E * sizeof(double), st));
+        CU(h, cudaMemsetAsync(h->integ_cnt, 0, sizeof(unsigned long long), st));
+        h->integ_fresh = false;
+    }
+    double *R = ws.R;
+    const double a = h->integ_alpha;
+    const uint32_t last = W - (uint32_t)(ntiles - 1) * INTEG_T;
+    const unsigned blocks = (unsigned)((elems + INTEG_THREADS - 1) / INTEG_THREADS);
+    integ_tiles_kernel<<<blocks, INTEG_THREADS, 0, st>>>(R, h->integ_tiles, E, (int)W, a);
+    integ_carry_kernel<<<E, INTEG_SCAN_THREADS, 0, st>>>(h->integ_tiles, h->integ_S, h->integ_cnt, ws.n0, E, (int)W,
+                                                         std::pow(a, (double)INTEG_T), std::pow(a, (double)last));
+    integ_apply_kernel<<<blocks, INTEG_THREADS, 0, st>>>(R, h->integ_tiles, ws.n0, E, (int)W, a);
+    h->launches += 3;
+    CU(h, cudaGetLastError());
+    CU(h, cudaEventRecord(h->integ_done, st));
+    h->integ_used = true;
+    return MUSIC_B200_OK;
+}
+
 // Enqueue `nwindows` windows on `st`: one persistent fused launch where the shape allows it, otherwise the unfused
 // kernels in sub-batches of at most max_sub_windows(), which bounds the workspace slot `slot` (0 / 1) they run in.
 // out: the outputs of the call; counts (may be NULL) receives the per-window source counts, under the FIXED rule n each.
@@ -1282,6 +1334,11 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, const Ou
             const size_t e = (size_t)W * h->m * h->m;
             calib_apply_kernel<<<(unsigned)((e + CALIB_THREADS - 1) / CALIB_THREADS), CALIB_THREADS, 0, st>>>(v.R, (int)h->m, (int)W, h->cal_c);
             h->launches++;
+        }
+        if (plan.integ) {
+            // the integration across windows, also inside the covariance slot
+            rc = launch_integrate(h, v, W, st);
+            if (rc) return rc;
         }
         if (tev) cudaEventRecord(tev[1], st);
         rc = launch_eig_scan(h, plan, v, W, out.at(w0), table(h), h->N, st, tev,
@@ -1727,6 +1784,7 @@ int retune(music_b200 *h, F fill)
     if (const int rc = alloc_slot(h, h->tables[idle])) return rc;
     if (const int rc = fill(h->tables[idle])) return rc;
     h->cur_table = idle;
+    h->integ_fresh = true;  // the integrated covariances described the old manifold
     return MUSIC_B200_OK;
 }
 
@@ -2311,6 +2369,7 @@ int music_b200_set_calibration(music_b200 *h, const double *gains)
     if (const int rc = for_each_child(h, [&](music_b200 *c) { return music_b200_set_calibration(c, gains); })) return rc;
     h->calib = gains != nullptr;
     h->cal_c = cv;
+    h->integ_fresh = true;  // the carry is kept in corrected coordinates
     for (uint32_t i = 0; i < 2 * h->m; ++i) h->cal_g[i] = gains ? gains[i] : (i % 2 == 0 ? 1.0 : 0.0);
     return MUSIC_B200_OK;
 }
@@ -2321,6 +2380,55 @@ int music_b200_get_calibration(music_b200 *h, double *gains)
     if (!gains) return fail(h, MUSIC_B200_EINVAL, "gains must not be NULL");
     std::lock_guard<std::mutex> g(h->mutex);
     for (uint32_t i = 0; i < 2 * h->m; ++i) gains[i] = h->calib ? h->cal_g[i] : (i % 2 == 0 ? 1.0 : 0.0);
+    return MUSIC_B200_OK;
+}
+
+}  // extern "C"
+
+/* ---- covariance integration across windows (music_integrate.cuh) ---- */
+namespace {
+
+// the handles whose windows form one stream on one device: every other handle refuses integration
+int check_integration(music_b200 *h)
+{
+    if (!h->kids.empty())
+        return fail(h, MUSIC_B200_EINVAL, "integration is not built for multi-device handles (their windows are dealt round-robin "
+                                          "over the devices)");
+    if (h->chan) return fail(h, MUSIC_B200_EINVAL, "per-channel integration is not built: a channel handle takes no integration");
+    if (h->gather_buf)
+        return fail(h, MUSIC_B200_EINVAL, "integration is not built for a handle with a bins all-gather (its windows are one "
+                                          "rank's share of a stream)");
+    return MUSIC_B200_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int music_b200_set_integration(music_b200 *h, double alpha)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (!std::isfinite(alpha) || alpha < 0.0 || alpha >= 1.0)
+        return fail(h, MUSIC_B200_EINVAL, "the forgetting factor must be finite with 0 <= alpha < 1 (got %g)", alpha);
+    std::lock_guard<std::mutex> g(h->mutex);
+    if (const int rc = check_integration(h)) return rc;
+    if (alpha > 0.0 && !h->integ_done) {
+        CU(h, cudaSetDevice(h->device));
+        CU(h, h->integ_S.grow(2 * (size_t)h->m * h->m));
+        CU(h, h->integ_cnt.grow(1));
+        CU(h, cudaEventCreateWithFlags(&h->integ_done, cudaEventDisableTiming));
+    }
+    h->integ_alpha = alpha;
+    h->integ_fresh = true;
+    return MUSIC_B200_OK;
+}
+
+int music_b200_reset_integration(music_b200 *h)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    std::lock_guard<std::mutex> g(h->mutex);
+    if (const int rc = check_integration(h)) return rc;
+    h->integ_fresh = true;
     return MUSIC_B200_OK;
 }
 
@@ -2575,6 +2683,7 @@ int music_b200_gather_create(music_b200 *h, uint32_t total_windows, unsigned cha
     std::lock_guard<std::mutex> g(h->mutex);
     CU(h, cudaSetDevice(h->device));
     if (h->gather_buf) return fail(h, MUSIC_B200_EINVAL, "gather buffer already created");
+    if (h->integ_alpha > 0.0) return fail(h, MUSIC_B200_EINVAL, "the bins all-gather is not built for an integrating handle (set_integration(0) first)");
     static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
     const size_t elems = (size_t)total_windows * h->n;
     // the handle takes the buffers once both exist and are shared: a failure leaves it without a gather buffer

@@ -19,19 +19,15 @@ namespace music {
 
 constexpr int SOURCES_FIXED = 0, SOURCES_MDL = 1, SOURCES_AIC = 2;  // = MUSIC_B200_SOURCES_*
 
-// counts[w] (workspace) and, when given, counts_out[w] (the caller's) for the W windows of ev ([W][M], ascending)
-__global__ void __launch_bounds__(128) source_count_kernel(const double *__restrict__ ev, int M, int nmax, int N, int rule, int W,
-                                                           int32_t *__restrict__ counts, int32_t *__restrict__ counts_out)
+// The count of one window from its ascending eigenvalues lam [M] and Nd looks (the definition above with N = Nd)
+__device__ __forceinline__ int source_count_window(const double *lam, int M, int nmax, double Nd, int rule)
 {
-    const int w = blockIdx.x * blockDim.x + threadIdx.x;
-    if (w >= W) return;
-    const double *lam = ev + (size_t)w * M;
     bool ok = lam[0] > 0.0;
     for (int i = 0; i < M; ++i) ok = ok && isfinite(lam[i]);
     int best = 0;
     if (ok) {
         // explicit roundings: no contraction into FMAs, so that each criterion is the literal expression above
-        const double Nd = (double)N, logN = log(Nd);
+        const double logN = log(Nd);
         double S = 0.0, G = 0.0, bestc = 0.0;
         bool have = false;
         for (int p = 1; p <= M; ++p) {  // p ascending = d descending: "<=" keeps the smallest d among equal minima
@@ -49,6 +45,16 @@ __global__ void __launch_bounds__(128) source_count_kernel(const double *__restr
             }
         }
     }
+    return best;
+}
+
+// counts[w] (workspace) and, when given, counts_out[w] (the caller's) for the W windows of ev ([W][M], ascending)
+__global__ void __launch_bounds__(128) source_count_kernel(const double *__restrict__ ev, int M, int nmax, int N, int rule, int W,
+                                                           int32_t *__restrict__ counts, int32_t *__restrict__ counts_out)
+{
+    const int w = blockIdx.x * blockDim.x + threadIdx.x;
+    if (w >= W) return;
+    const int best = source_count_window(ev + (size_t)w * M, M, nmax, (double)N, rule);
     counts[w] = best;
     if (counts_out) counts_out[w] = best;
 }

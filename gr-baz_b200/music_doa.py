@@ -211,6 +211,18 @@ class music_doa(object):
                                                         d_counts, d_weights, d_beams, stream)
         _capi.check(rc, self._h)
 
+    # -- extension: covariance integration across windows ----------------------------------------------------
+    def set_integration(self, alpha):
+        """Integrate the covariance across windows with forgetting factor ``alpha`` (0 <= alpha < 1; 0, the default, is
+        off): each window's estimators read Rbar_j = S_j / c_j, S_j = alpha S_{j-1} + R_j, c_j = alpha c_{j-1} + 1, over
+        the windows since the last reset, across calls (include/music_b200.h).  MDL / AIC count with N_eff.  Resets the
+        carry; so do ``reset_integration``, ``set_array_response``, ``set_array_geometry`` and ``set_calibration``."""
+        _capi.check(self._lib.music_b200_set_integration(self._h, float(alpha)), self._h)
+
+    def reset_integration(self):
+        """Restart the integration at the next window (the next window's covariance is its own)."""
+        _capi.check(self._lib.music_b200_reset_integration(self._h), self._h)
+
     # -- extension: receiver calibration -----------------------------------------------------------------
     CALIBRATIONS = {"phase": 1, "gain_phase": 2}
 

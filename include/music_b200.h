@@ -459,6 +459,50 @@ int music_b200_calib_solve(music_b200 *h, double az_deg, double el_deg, int kind
                            double *stats /* host [2]: residual, sweeps; may be NULL */);
 
 /*
+ * Covariance integration across windows (extension, no reference counterpart): an exponentially weighted covariance
+ * carried from window to window and from call to call, so that a weak source is detected and located from the recent
+ * past while every window keeps its own output rate and latency.
+ *   setting    music_b200_set_integration(h, alpha): the forgetting factor, finite with 0 <= alpha < 1, otherwise EINVAL
+ *              and the old setting stays.  alpha = 0 (the default) is off: every output, the launch count and the fused /
+ *              unfused path choice are those of a handle that never had integration.  music_b200_reset_integration(h)
+ *              restarts the recurrence at the next window.
+ *   inputs     R_j: the window's fp64 covariance as process_device_ex's d_R returns it with integration off (after the
+ *              calibration when one is set); j = 0, 1, 2, ... the handle's windows in stream order since the last reset,
+ *              through the windows of one call and on into the next call.
+ *   recurrence S_{-1} = 0, c_{-1} = q_{-1} = 0;  S_j = alpha S_{j-1} + R_j,  c_j = alpha c_{j-1} + 1,
+ *              q_j = alpha^2 q_{j-1} + 1;  the integrated covariance is Rbar_j = S_j / c_j (the first window after a reset
+ *              is its own R, bit for bit).
+ *   reads      every stage that reads R reads Rbar_j instead: eigensolver, source count, MVDR preparation, every scan,
+ *              every peak mode (TOP_BINS, LOCAL_MAXIMA, ROOTS, ESPRIT, 2-D ESPRIT, DML, MANIFOLD), refinement, the az-el
+ *              decode and the beam weights; beams are still formed from the window's own raw samples with those
+ *              weights; d_R returns Rbar_j.  Rbar_j keeps R_j's exact Hermitian form (mirrored lower triangle, real
+ *              diagonal): both parts of every entry follow the same operations.
+ *   numerics   the sums are evaluated as a parallel scan over each sub-batch's windows, so their order is not the
+ *              recurrence's: per window max |Rbar_gpu - Rbar_seq| <= 1e-13 max |Rbar_seq|, Rbar_seq the sequential fp64
+ *              recurrence on the same R_j.  The split of the windows into calls changes Rbar within that bound only.
+ *   counts     MDL / AIC use N_eff,j = N c_j^2 / q_j (fp64, per window) in place of N: N at the first window after a
+ *              reset, tending to N (1 + alpha) / (1 - alpha).  The "N <= m" refusals stay on N.
+ *   resets     reset_integration(), every set_integration() (the same alpha included), every table setter (set_table,
+ *              set_geometry, set_geometry_azel: old covariances describe another manifold) and set_calibration() (the
+ *              carry is in corrected coordinates).  Not reset by the peak mode, estimator, source rule, refinement and
+ *              beamformer setters.  calib_accumulate_* keep reading raw, unintegrated covariances.  A call with
+ *              nwindows = 0, or refused with EINVAL before it enqueues anything, leaves the carry untouched.
+ *   ordering   call k + 1 integrates after call k on the same handle, whichever streams they use (an event orders them);
+ *              the host entries' chunks, staged on two streams, and the sub-batches of a call integrate in window order.
+ *   handles    single-device 1-D handles (process_host, _device, _ex, _counts, both planar entries, both beams entries)
+ *              and az-el handles (process_azel_*).  Not built, and refused with EINVAL by set_integration() and
+ *              reset_integration(): multi-device handles (their windows are dealt round-robin over the devices) and with
+ *              them the sharded entry, handles with a bins all-gather (gather_create() is refused while alpha > 0), and
+ *              channel handles (per-channel integration).
+ *   kernels    while alpha > 0 every call runs the unfused kernels (the fused M = 4 / M = 8 kernels keep R in registers)
+ *              plus integ_tiles_kernel, integ_carry_kernel and integ_apply_kernel per sub-batch, timed in the covariance
+ *              slot of the stage timing; MDL / AIC run source_count_neff_kernel.  The carry (S and the window count) lives
+ *              in device buffers of the handle.
+ */
+int music_b200_set_integration(music_b200 *h, double alpha);
+int music_b200_reset_integration(music_b200 *h);
+
+/*
  * Downstream reducers (extension, no reference counterpart): what a GUI-rate consumer such as the DOA
  * compass (/root/reference/python/doa_compass_control.py:102-108) or a plot sink
  * (/root/reference/python/plot_sink.py:38) needs from millions of windows per second.

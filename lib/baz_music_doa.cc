@@ -183,6 +183,21 @@ void baz_music_doa::set_beamformer(int rule, double loading)
 }
 
 /* Extension (not in the reference): receiver calibration, see include/music_b200.h. */
+/* Extension (not in the reference): covariance integration across windows, see include/music_b200.h. */
+void baz_music_doa::set_integration(double alpha)
+{
+    gr::thread::scoped_lock guard(d_mutex);
+    const int rc = music_b200_set_integration(d_handle, alpha);
+    if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa: ") + music_b200_last_error(d_handle));
+}
+
+void baz_music_doa::reset_integration()
+{
+    gr::thread::scoped_lock guard(d_mutex);
+    const int rc = music_b200_reset_integration(d_handle);
+    if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa: ") + music_b200_last_error(d_handle));
+}
+
 void baz_music_doa::set_calibration(const std::vector<std::complex<double> > &gains)
 {
     if (!gains.empty() && gains.size() != d_m) throw std::invalid_argument("music_doa: gains.size() != m");

@@ -80,6 +80,13 @@ public:
     std::vector<std::complex<double> > calibration();
     void calibrate(double angle_deg, int kind, int nitems);
     double last_calibration_residual() const { return d_cal_residual; }
+    /* extension: covariance integration across work() calls (include/music_b200.h).  set_integration(): forgetting
+     * factor 0 <= alpha < 1 (0, the default, is off); each item's estimate reads the exponentially weighted covariance of
+     * the items since the last reset, across calls, and MDL / AIC count with the effective snapshot count.
+     * reset_integration() restarts it at the next item; so do set_integration(), set_array_response(),
+     * set_array_geometry() and set_calibration(). */
+    void set_integration(double alpha);
+    void reset_integration();
 
     /* Integer peak-bin indices of the items produced by the last work() call, [items][n]
      * (not in the reference; -1 marks a slot the reference would leave at (0, 0)). */

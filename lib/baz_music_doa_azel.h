@@ -61,6 +61,9 @@ public:
     std::vector<std::complex<double> > calibration();
     void calibrate(double az_deg, double el_deg, int kind, int nitems);
     double last_calibration_residual() const { return d_cal_residual; }
+    /* covariance integration across work() calls, as for baz_music_doa */
+    void set_integration(double alpha);
+    void reset_integration();
 
     /* flat peak bins b = i * n_az + k of the items produced by the last work() call, [items][n] (-1: unfilled slot) */
     const std::vector<int> &last_bins() const { return d_bins; }
