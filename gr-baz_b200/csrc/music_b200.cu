@@ -1128,8 +1128,7 @@ int launch_eig_scan(music_b200 *h, const Plan &p, const WsView &ws, uint32_t W, 
     const int excl = (int)h->modes.excl;
     switch (p.peaks) {
     case Peaks::Roots:
-        roots_kernel<<<(W + ROOTS_WARPS - 1) / ROOTS_WARPS, ROOTS_WARPS * 32, 0, st>>>(ws.Vt, cnt, M, (int)h->n, (int)h->K, (int)W, tb.geo,
-                                                                                  tb.ula, po);
+        roots_kernel<<<W, ROOTS_THREADS, 0, st>>>(ws.Vt, cnt, M, (int)h->n, (int)h->K, tb.geo, tb.ula, po);
         break;
     case Peaks::Esprit:
         esprit_kernel<<<(W + ESPRIT_WARPS - 1) / ESPRIT_WARPS, ESPRIT_WARPS * 32, 0, st>>>(ws.Vt, cnt, M, (int)h->n, (int)h->K, (int)W,

@@ -8,12 +8,12 @@
 // denominator D(t) = a^H C a, C = G G^H, is to fp64 rounding the trigonometric polynomial sum_{|l| <= L} c_l e^{j l t}
 //     c_0 = tr C + 2 sum_{i<j} beta_ij,0 Re C_ij,   c_l = sum_{i<j} beta_ij,l (2 Re C_ij, l even; 2 j Im C_ij, l odd),
 // and Q(z) = sum_l c_l z^(l + L) has the directions as roots near the unit circle, arg z = t.  The roots come from
-// ROOTS's Aberth-Ehrlich iteration, merge and selection (music_roots.cuh); the full definition is in
+// ROOTS's root finder (roots_solve in music_roots.cuh); the full definition is in
 // include/music_b200.h and is restated by tests/manifold_oracle.py.
 //
 // The order L and the table beta are built on the host with the geometry (manifold_coeffs_host); the kernel reads
 // beta from global memory (<= 120 pairs x 65 orders x 16 B = 125 KB, L2-resident and shared by every window).
-// One CTA per window, thread r <-> root r (P = 2L <= 128: ROOTS's lane <-> root warp does not fit), everything fp64.
+// One CTA of up to four warps per window, thread r <-> root r (P = 2L <= 128), everything fp64.
 #pragma once
 #include <cmath>
 #include <vector>
@@ -141,15 +141,8 @@ __global__ void __launch_bounds__(MF_MAX_THREADS) manifold_kernel(const double *
                                                                   int M, int n, int K, const RefineGeom geo,
                                                                   const double2 *__restrict__ beta, int L, PeakOut out)
 {
-    __shared__ double2 Cs[MAXM * MAXM];        // C = G G^H, upper triangle
-    __shared__ double2 cf[MF_MAX_L + 1];       // c_0 .. c_L
-    __shared__ double lg[MF_MAX_L + 1];        // log2 |c_l| (-inf for 0)
-    __shared__ double ac[MF_MAX_L + 1];        // |c_l|
-    __shared__ int hull[MF_MAX_P + 1], nh_s;
-    __shared__ double2 zs[MF_MAX_P];           // the current approximants
-    __shared__ double keys[MF_MAX_P], tds[MF_MAX_P];
-    __shared__ int nns[MF_MAX_P];
-    __shared__ unsigned char dups[MF_MAX_P], kepts[MF_MAX_P];
+    __shared__ double2 Cs[MAXM * MAXM];  // C = G G^H, upper triangle
+    __shared__ RootsShared<MF_MAX_L> sh;
 
     const int w = blockIdx.x, r = threadIdx.x, NT = blockDim.x;
     const int d = counts ? counts[w] : n;
@@ -186,173 +179,24 @@ __global__ void __launch_bounds__(MF_MAX_THREADS) manifold_kernel(const double *
                     c.y += 2.0 * Cij.x * b.y;
                 }
             }
-        cf[r] = c;
-        ac[r] = hypot(c.x, c.y);
-        lg[r] = (c.x != 0.0 || c.y != 0.0) ? log2(hypot(c.x, c.y)) : -INFINITY;
-    }
-    __syncthreads();
-
-    // t: outermost pairs c_{+-L}, c_{+-(L-1)}, .. that are exactly zero (each a root at 0 and at infinity)
-    bool finite = true;
-    int t = L;
-    for (int l = 0; l <= L; ++l) {
-        const double2 c = cf[l];
-        finite = finite && isfinite(c.x) && isfinite(c.y);
-        if (c.x != 0.0 || c.y != 0.0) t = L - l;
-    }
-    const int H = L - t, P = 2 * H;  // Q reduced to sum_k b_k z^k, k = 0 .. P, b_k = c_{k - H}
-    bool ok = finite && d > 0 && P > 0;  // uniform over the CTA
-    double2 z = make_double2(0.0, 0.0);
-    if (ok) {
-        // starting points on the circles of the Newton polygon (Bini), as in roots_kernel: the upper convex hull of
-        // (k, log2 |b_k|), built by one thread
-        if (r == 0) {
-            int nh = 1;
-            hull[0] = 0;
-            for (int k = 1; k <= P; ++k) {
-                const double lk = lg[k >= H ? k - H : H - k];
-                if (lk == -INFINITY) continue;
-                while (nh >= 2) {
-                    const int i = hull[nh - 2], j = hull[nh - 1];
-                    const double li = lg[i >= H ? i - H : H - i], lj = lg[j >= H ? j - H : H - j];
-                    if ((lj - li) * (k - i) <= (lk - li) * (j - i)) --nh;  // j on or below the chord i -> k
-                    else break;
-                }
-                hull[nh++] = k;
-            }
-            nh_s = nh;
-        }
-        __syncthreads();
-        const int nh = nh_s;
-        int si = 0;
-        while (si + 2 < nh && hull[si + 1] <= r) ++si;
-        const int i0 = hull[si], j0 = hull[si + 1];
-        const double li = lg[i0 >= H ? i0 - H : H - i0], lj = lg[j0 >= H ? j0 - H : H - j0];
-        const double u = exp2((li - lj) / (j0 - i0));
-        double sn, cs;
-        sincospi(2.0 * (r - i0) / (j0 - i0) + 2.0 * i0 / P + 0.5 / P, &sn, &cs);
-        z = make_double2(u * cs, u * sn);
-        if (r < P) zs[r] = z;
-        __syncthreads();
-        bool done = r >= P, conv = false;
-        for (int it = 0; it < ROOTS_MAX_IT; ++it) {
-            double2 wc = make_double2(0.0, 0.0);
-            if (!done) {  // a converged root stays put, so only the others evaluate
-                // Horner for Q and Q'; outside the unit circle for R(w) = w^P Q(1 / w) and R' at w = 1 / z instead, so
-                // that no power of z overflows.  acc = sum_k |b_k| |w|^k
-                const bool outside = z.x * z.x + z.y * z.y > 1.0;
-                const double2 w1 = outside ? cdiv(make_double2(1.0, 0.0), z) : z;
-                const double aw = hypot(w1.x, w1.y);
-                double2 q = cf[H], dq = make_double2(0.0, 0.0);  // b_0 = conj(c_H), b_P = c_H: equal modulus
-                if (outside) q.y = -q.y;
-                double acc = ac[H];
-                for (int k = 1; k <= P; ++k) {
-                    const int l = (outside ? k : P - k) - H;
-                    double2 b = cf[l >= 0 ? l : -l];
-                    if (l < 0) b.y = -b.y;
-                    dq = cmul(dq, w1);
-                    dq.x += q.x; dq.y += q.y;
-                    q = cmul(q, w1);
-                    q.x += b.x; q.y += b.y;
-                    acc = acc * aw + ac[l >= 0 ? l : -l];
-                }
-                if (hypot(q.x, q.y) <= ROOTS_BACK * P * ROOTS_EPS * acc) done = true;
-                // Aberth term sum_{s != r} 1 / (z_r - z_s)
-                double2 S = make_double2(0.0, 0.0);
-                for (int s = 0; s < P; ++s) {
-                    const double2 zz = zs[s];
-                    if (s != r) {
-                        const double dx = z.x - zz.x, dy = z.y - zz.y, rr = 1.0 / (dx * dx + dy * dy);
-                        S.x += dx * rr;
-                        S.y -= dy * rr;
-                    }
-                }
-                if (outside) {
-                    const double2 num = cmul(z, q), nS = cmul(num, S), wd = cmul(w1, dq);
-                    wc = cdiv(num, make_double2(P * q.x - wd.x - nS.x, P * q.y - wd.y - nS.y));
-                } else {
-                    const double2 qS = cmul(q, S);
-                    wc = cdiv(q, make_double2(dq.x - qS.x, dq.y - qS.y));
-                }
-            }
-            __syncthreads();  // every thread has read this step's approximants
-            if (!done) {
-                z.x -= wc.x;
-                z.y -= wc.y;
-                done = wc.x * wc.x + wc.y * wc.y <= ROOTS_STOP * ROOTS_STOP * (z.x * z.x + z.y * z.y);
-                zs[r] = z;
-            }
-            if (__syncthreads_and(done)) {
-                conv = true;
-                break;
-            }
-        }
-        // a window whose iteration has not converged in ROOTS_MAX_IT steps reports no peaks
-        ok = __syncthreads_and(conv && (r >= P || (isfinite(z.x) && isfinite(z.y))));
-    }
-
-    // a double root on the unit circle (the two approximants are each other's nearest root, closer than
-    // ROOTS_MERGE |z|) counts once: both move to the midpoint, the lower index keeps it with modulus 1
-    double key = hypot(z.x, z.y);
-    bool dup = false;
-    if (ok) {
-        int nn = -1;
-        double best = 0.0;
-        if (r < P) {
-            for (int s = 0; s < P; ++s) {
-                const double2 zz = zs[s];
-                const double dd = hypot(z.x - zz.x, z.y - zz.y);
-                if (s != r && (nn < 0 || dd < best)) { nn = s; best = dd; }
-            }
-            nns[r] = nn;
-            keys[r] = key;
-        }
-        __syncthreads();
-        if (r < P && nn >= 0 && nns[nn] == r && best <= ROOTS_MERGE * fmax(key, keys[nn])) {
-            const double2 zn = zs[nn];
-            z = make_double2(0.5 * (z.x + zn.x), 0.5 * (z.y + zn.y));
-            key = 1.0;
-            dup = r > nn;
-        }
-        __syncthreads();  // zs and keys are read above before they are rewritten below
+        roots_set_coeff(sh, r, c);
     }
     // t* = arg z in [0, 360) degrees
-    double tdeg = atan2(z.y, z.x) * REFINE_RAD2DEG;
-    if (tdeg < 0.0) tdeg += 360.0;
-    if (r < P) {
-        keys[r] = key;
-        dups[r] = dup;
-        tds[r] = tdeg;
-    }
-    __syncthreads();
-
-    // keep the H inside roots (ascending modulus, a double root's second copy after every other root of equal modulus,
-    // then index); fill slots in descending modulus, ties to the lower angle
-    int r1 = 0, r2 = 0;
-    for (int s = 0; s < P; ++s) {
-        const double ks = keys[s];
-        const bool ds = dups[s];
-        if (ks < key || (ks == key && (ds < dup || (ds == dup && s < r)))) ++r1;
-    }
-    const bool kept = ok && r < P && r1 < H;
-    if (r < P) kepts[r] = kept;
-    __syncthreads();
-    for (int s = 0; s < P; ++s) {
-        const double ks = keys[s], ts = tds[s];
-        if (kepts[s] && (ks > key || (ks == key && (ts < tdeg || (ts == tdeg && s < r))))) ++r2;
-    }
-    const int f = ok ? min(d, H) : 0;  // filled slots
-    if (kept && r2 < f) {
-        const size_t o = (size_t)w * n + r2;
-        if (z.x == 0.0 && z.y == 0.0) {  // a kept root at 0 has no direction
+    const RootSlot rs = roots_solve(sh, L, d, [](double2 z) {
+        const double t = atan2(z.y, z.x) * REFINE_RAD2DEG;
+        return t < 0.0 ? t + 360.0 : t;
+    });
+    if (rs.slot >= 0) {
+        const size_t o = (size_t)w * n + rs.slot;
+        if (rs.z.x == 0.0 && rs.z.y == 0.0) {  // a kept root at 0 has no direction
             peak_write(out, o, -1, 0.0, K);
         } else {
             double D, D1, D2;
-            refine_eval(geo, G, M, p, tdeg * STEER_DEG2RAD, &D, &D1, &D2);
-            ula_store_slot(out, o, tdeg, D, K);
+            refine_eval(geo, G, M, p, rs.tdeg * STEER_DEG2RAD, &D, &D1, &D2);
+            ula_store_slot(out, o, rs.tdeg, D, K);
         }
     }
-    if (r >= f && r < n) peak_write(out, (size_t)w * n + r, -1, 0.0, K);
+    if (r >= rs.f && r < n) peak_write(out, (size_t)w * n + r, -1, 0.0, K);
 }
 
 }  // namespace music

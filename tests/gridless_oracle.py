@@ -1,6 +1,6 @@
-"""High-precision reference for the gridless ULA peak modes (ROOTS: the Aberth-Ehrlich root finder of roots_kernel;
-ESPRIT: the Hessenberg QR of esprit_eigvals), the bounds a backward-stable root / eigenvalue solver meets, and the
-windows that stress them (not a test module; the same shape as eig_oracle.py).
+"""High-precision reference for the gridless ULA peak modes (ROOTS: the Aberth-Ehrlich root finder roots_solve, which
+roots_kernel shares with manifold_kernel; ESPRIT: the Hessenberg QR of esprit_eigvals), the bounds a backward-stable
+root / eigenvalue solver meets, and the windows that stress them (not a test module; the same shape as eig_oracle.py).
 
 Reference: mpmath at eig_oracle.REF_DPS digits on the fp64 covariance R as given (the GPU's own R wherever R is not
 exact, so that neither the covariance's rounding nor the eigensolver's is charged to the root stage beyond its bound).

@@ -1,8 +1,9 @@
 #!/usr/bin/env python
 """CPU emulation (numpy fp64) of roots_kernel (gr-baz_b200/csrc/music_roots.cuh): the coefficients c_l in the kernel's
-summation order, the outer-pair deflation, the Newton-polygon starting points, the Aberth-Ehrlich lane loop with its
-reversed evaluation outside the unit circle and its stopping rule, the double-root merge and the selection of the slot
-roots.  Lanes are numpy vectors; every lane takes the kernel's decisions.  The keyword switches restore the behaviour
+summation order, then its root finder roots_solve (shared with manifold_kernel): the outer-pair deflation, the
+Newton-polygon starting points, the Aberth-Ehrlich loop over one thread per root with its reversed evaluation outside
+the unit circle and its stopping rule, the double-root merge and the selection of the slot roots.  The threads (called
+lanes here) are numpy vectors; every lane takes the kernel's decisions.  The keyword switches restore the behaviour
 before the fixes (unit-circle starts, plain Horner everywhere, no convergence flag) and plant the defects that
 tests/test_gridless_oracle.py shows the checker failing."""
 import math

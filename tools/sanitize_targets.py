@@ -2,7 +2,7 @@
 """Small invocations of the kernels compute-sanitizer should look at (SURVEY.md section 5): run as
   compute-sanitizer --tool racecheck|memcheck|synccheck python tools/sanitize_targets.py <target>
 targets: fused (C1-size windows, 2000 of them + a ragged 1187 + a drain-only 9), fused_jacobi, fused8, covn8, covn16, eig16, esprit2d,
-multi,
+gridless_roots, multi,
 lifecycle (every handle kind created, retuned, grown and destroyed through the host entry points; run it under
   compute-sanitizer --tool memcheck --leak-check full, which reports what a handle leaves allocated)"""
 import os
@@ -64,6 +64,27 @@ elif target == "esprit2d":
         az.work(W, [x], outs)
         print("esprit2d ok", m, outs[0][:2])
         az.close()
+elif target == "gridless_roots":
+    # the shared root finder of ROOTS and MANIFOLD (music_roots.cuh): ROOTS on x-axis ULAs (one warp per window), MANIFOLD
+    # on UCA 8 (L = 32, one warp), UCA 16 (L = 46, three warps) and a UCA 16 at 0.85 lambda (L = 63, four warps); a
+    # ragged window count with a zero window and a NaN window
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+    import manifold_oracle as mf
+    from helpers import LAM, plan_windows, ula
+
+    for mode, m, n, pos in (("roots", 4, 1, ula(4, "x")), ("roots", 16, 3, ula(16, "x")), ("manifold", 8, 2, mf.uca(8, 0.5, LAM)),
+                            ("manifold", 16, 3, mf.uca(16, 0.5, LAM)), ("manifold", 16, 3, mf.uca(16, 0.85, LAM))):
+        W = 37
+        x, _ = plan_windows(pos, [(1 + w % n, 20.0) for w in range(W)], m, 256)
+        x[3] = 0
+        x[5, 11] = np.nan
+        blk = music_doa(m, n, m * 256, np.ones((360, m), np.complex64), 360)
+        blk.set_array_geometry(pos, LAM)
+        blk.set_peak_mode(mode, 0)
+        ang = np.zeros((W, n), np.float32)
+        blk.work(W, [x], [ang])
+        print(target, "ok", mode, m, ang[:2].tolist())
+        blk.close()
 elif target == "multi":
     cfg = synth.config(1)
     resp, table = bench.table_for(cfg)
