@@ -17,7 +17,8 @@
 //                        the carry out of the last tile becomes S, and the window count since the reset advances by W;
 //   integ_apply_kernel   per tile from its carry-in: S <- alpha S + R_i (the first window after a reset takes S = R_i
 //                        itself), R_i <- S / c_i in place.  c_i takes the closed form (1 - alpha^(n+1)) / (1 - alpha) at
-//                        the tile's first window (n: its count since the reset) and the recurrence after it.
+//                        the tile's first window (n: its count since the reset; integ_one_minus_pow keeps it accurate as
+//                        alpha nears 1) and the recurrence after it.
 // The carry (S and the count) lives in the handle's device buffers, read at the start of each sub-batch and written at its
 // end; the handle orders consecutive sub-batches, on whichever streams they run, with one event.
 // Bytes per window: the tile pass reads R and the apply pass reads and writes it, 16 M^2 bytes each way per pass.
@@ -34,19 +35,29 @@ constexpr int INTEG_T = 32;             // windows per tile
 constexpr int INTEG_THREADS = 256;      // tile and apply kernels
 constexpr int INTEG_SCAN_THREADS = 256; // carry kernel: one CTA per entry
 
+// 1 - a^k for 0 < a < 1 and k >= 1, without the cancellation of 1 - pow(a, k) as a nears 1 (there 1 - pow(a, k) loses
+// all but about -log2(1 - a^k) of its bits): -expm1(k log a), with log a = log1p(a - 1) for a >= 1/2, where a - 1 is
+// exact (Sterbenz), so every step keeps its own few-ulp relative error.
+__device__ __forceinline__ double integ_one_minus_pow(double a, double k)
+{
+    return -expm1(k * (a >= 0.5 ? log1p(a - 1.0) : log(a)));
+}
+
 // c_n = sum_{k <= n} alpha^k, the closed form of c_j = alpha c_{j-1} + 1 at count n since the reset (c_0 = 1 exactly)
 __device__ __forceinline__ double integ_c(double alpha, unsigned long long n)
 {
     if (n == 0) return 1.0;
-    return (1.0 - pow(alpha, (double)n + 1.0)) / (1.0 - alpha);
+    return integ_one_minus_pow(alpha, (double)n + 1.0) / (1.0 - alpha);
 }
 
-// N_eff,n = N c_n^2 / q_n, q_n = sum_{k <= n} alpha^(2k): N at n = 0, tending to N (1 + alpha) / (1 - alpha)
+// N_eff,n = N c_n^2 / q_n, q_n = sum_{k <= n} alpha^(2k): N at n = 0, tending to N (1 + alpha) / (1 - alpha).  q takes
+// 1 - alpha^2 as (1 - alpha)(1 + alpha), and 1 - alpha^(2k) as d (2 - d) with d = 1 - alpha^k: no difference of two
+// rounded numbers near 1.
 __device__ __forceinline__ double integ_neff(double alpha, unsigned long long n, double N)
 {
     if (n == 0) return N;
-    const double c = integ_c(alpha, n), a2 = alpha * alpha;
-    const double q = (1.0 - pow(a2, (double)n + 1.0)) / (1.0 - a2);
+    const double k = (double)n + 1.0, d = integ_one_minus_pow(alpha, k), c = d / (1.0 - alpha);
+    const double q = d * (2.0 - d) / ((1.0 - alpha) * (1.0 + alpha));
     return N * c * c / q;
 }
 

@@ -478,8 +478,14 @@ int music_b200_calib_solve(music_b200 *h, double az_deg, double el_deg, int kind
  *              weights; d_R returns Rbar_j.  Rbar_j keeps R_j's exact Hermitian form (mirrored lower triangle, real
  *              diagonal): both parts of every entry follow the same operations.
  *   numerics   the sums are evaluated as a parallel scan over each sub-batch's windows, so their order is not the
- *              recurrence's: per window max |Rbar_gpu - Rbar_seq| <= 1e-13 max |Rbar_seq|, Rbar_seq the sequential fp64
- *              recurrence on the same R_j.  The split of the windows into calls changes Rbar within that bound only.
+ *              recurrence's.  Against the exact recurrence on the same R_j, per entry and part (eps = 2^-53):
+ *              |Rbar_gpu - Rbar| <= eps |Rbar| + 1.01 eps (L(W_b) Abar_j + carry_j / c_j), where Abar_j =
+ *              sum_k alpha^(j-k) |R_k| / c_j, L(W_b) = 2 ceil(W_b / 32) + 2 ceil(W_b / 8192) + 130 is the rounding depth of
+ *              a sub-batch of W_b windows, and carry_j (in units of eps) the carried error of the sub-batches before:
+ *              E_b = alpha^(W_b) E_(b-1) + L(W_b) c_end Abar_end at the end of sub-batch b, and carry_j = alpha^(windows
+ *              since) E_(b-1) inside sub-batch b (tests/covariance_oracle.py).  c_j and N_eff,j are accurate to a few ulp
+ *              at every alpha, including alpha within 2^-52 of 1.  The split of the windows into calls changes Rbar
+ *              within that bound only.
  *   counts     MDL / AIC use N_eff,j = N c_j^2 / q_j (fp64, per window) in place of N: N at the first window after a
  *              reset, tending to N (1 + alpha) / (1 - alpha).  The "N <= m" refusals stay on N.
  *   resets     reset_integration(), every set_integration() (the same alpha included), every table setter (set_table,
