@@ -184,6 +184,20 @@ __global__ void azel_decode_kernel(const int32_t *__restrict__ bins, int slots, 
 }
 
 // ---- 2-D refinement --------------------------------------------------------------------------------------------------
+// theta_m of element m and its derivatives at (sin, cos) of the azimuth (sp, cp) and the elevation (se, ce), as listed
+// with azel_eval below (theta_epep = -theta); a_m = exp(-j theta_m).  Shared by the refinement and the CRB (music_crb.cuh).
+__device__ __forceinline__ void azel_phase(const AzelGeom &geo, int m, double sp, double cp, double se, double ce, double *th, double *tp,
+                                           double *te, double *tpp, double *tpe)
+{
+    const double x = geo.pos[3 * m], y = geo.pos[3 * m + 1], z = geo.pos[3 * m + 2];
+    const double h = x * cp + y * sp, v = y * cp - x * sp;
+    *th = STEER_TWO_PI * ((ce * h + z * se) / geo.lambda);
+    *tp = STEER_TWO_PI * ((ce * v) / geo.lambda);
+    *te = STEER_TWO_PI * ((z * ce - se * h) / geo.lambda);
+    *tpp = -STEER_TWO_PI * ((ce * h) / geo.lambda);
+    *tpe = -STEER_TWO_PI * ((se * v) / geo.lambda);
+}
+
 // D(ph, ep) = sum_j |g_j^H a|^2 with its gradient and Hessian, e = {D, D_ph, D_ep, D_phph, D_phep, D_epep}.
 // theta_m = 2 pi <p_m, u> / lambda, a_m = exp(-j theta_m); with h = x cos ph + y sin ph, v = y cos ph - x sin ph:
 //   theta_ph = 2 pi cos ep v / lambda,      theta_ep = 2 pi (z cos ep - sin ep h) / lambda,
@@ -198,13 +212,7 @@ __device__ __noinline__ void azel_eval(const AzelGeom &geo, const double2 *__res
     sincos(ep, &se, &ce);
     double ar[MAXM], ai[MAXM], th[MAXM], tp[MAXM], te[MAXM], tpp[MAXM], tpe[MAXM];
     for (int m = 0; m < M; ++m) {
-        const double x = geo.pos[3 * m], y = geo.pos[3 * m + 1], z = geo.pos[3 * m + 2];
-        const double h = x * cp + y * sp, v = y * cp - x * sp;
-        th[m] = STEER_TWO_PI * ((ce * h + z * se) / geo.lambda);
-        tp[m] = STEER_TWO_PI * ((ce * v) / geo.lambda);
-        te[m] = STEER_TWO_PI * ((z * ce - se * h) / geo.lambda);
-        tpp[m] = -STEER_TWO_PI * ((ce * h) / geo.lambda);
-        tpe[m] = -STEER_TWO_PI * ((se * v) / geo.lambda);
+        azel_phase(geo, m, sp, cp, se, ce, &th[m], &tp[m], &te[m], &tpp[m], &tpe[m]);
         double s, c;
         sincos(th[m], &s, &c);
         ar[m] = c;
@@ -251,13 +259,7 @@ __device__ __noinline__ void bartlett_azel_eval(const AzelGeom &geo, const doubl
     sincos(ep, &se, &ce);
     double ar[MAXM], ai[MAXM], th[MAXM], tp[MAXM], te[MAXM], tpp[MAXM], tpe[MAXM];
     for (int m = 0; m < M; ++m) {
-        const double x = geo.pos[3 * m], y = geo.pos[3 * m + 1], z = geo.pos[3 * m + 2];
-        const double h = x * cp + y * sp, v = y * cp - x * sp;
-        th[m] = STEER_TWO_PI * ((ce * h + z * se) / geo.lambda);
-        tp[m] = STEER_TWO_PI * ((ce * v) / geo.lambda);
-        te[m] = STEER_TWO_PI * ((z * ce - se * h) / geo.lambda);
-        tpp[m] = -STEER_TWO_PI * ((ce * h) / geo.lambda);
-        tpe[m] = -STEER_TWO_PI * ((se * v) / geo.lambda);
+        azel_phase(geo, m, sp, cp, se, ce, &th[m], &tp[m], &te[m], &tpp[m], &tpe[m]);
         double s, c;
         sincos(th[m], &s, &c);
         ar[m] = c;

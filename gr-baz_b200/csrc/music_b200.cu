@@ -40,6 +40,7 @@
 #include "music_beams.cuh"
 #include "music_calib.cuh"
 #include "music_integrate.cuh"
+#include "music_crb.cuh"
 #include "music_channels.cuh"
 #include "music_focus.cuh"
 
@@ -171,8 +172,10 @@ struct Outputs {
     double *ev = nullptr;       // [W][m]
     double *wts = nullptr;      // [W][n][m] complex beam weights: beams entry points only
     float *beams = nullptr;     // [W][n][N] complex64 beams: beams entry points only
+    float *std = nullptr;       // [W][sw] the CRB of every slot: crb entry points only
     Gather gather;
     uint32_t n = 0, K = 0, m = 0, N = 0;
+    uint32_t sw = 0;            // floats per window of std: n, 3 n on an az-el handle
 
     // the shape of h's calls and the all-gather h was attached to (music_b200_gather_attach)
     Outputs &shaped(const music_b200 *h);
@@ -193,13 +196,17 @@ struct Outputs {
         skip(o.ev, m);
         skip(o.wts, (size_t)n * m * 2);
         skip(o.beams, (size_t)n * N * 2);
+        skip(o.std, sw);
         for (int p = 0; p < gather.G; ++p) skip(o.gather.peer[p], (size_t)gather.G * n);
         return o;
     }
 
     // the per-window outputs a host call stages through pinned memory (4-byte elements), with their elements per window
     struct Field { void *p; uint32_t per_win; };
-    std::array<Field, 5> window_fields() const { return {{{angles, n}, {elev, n}, {levels, n}, {bins, n}, {counts, 1}}}; }
+    std::array<Field, 6> window_fields() const
+    {
+        return {{{angles, n}, {elev, n}, {levels, n}, {bins, n}, {counts, 1}, {std, sw}}};
+    }
 
     // the rows of a beams call a host call stages through pinned memory, with their bytes per window
     struct Row { void *p; size_t bytes; };
@@ -212,7 +219,7 @@ struct Outputs {
 // the buffers behind a staging slot's outputs, on the device or pinned (the spectrum is staged on the device only)
 template <template <class> class Buf>
 struct StagedOutputs {
-    Buf<float> angles, elev, levels, spec, beams;
+    Buf<float> angles, elev, levels, spec, beams, std;
     Buf<int32_t> bins, counts;
     Buf<double> wts;
 
@@ -220,7 +227,7 @@ struct StagedOutputs {
     {
         Outputs o;
         o.angles = angles; o.elev = elev; o.levels = levels; o.spec = spec;
-        o.beams = beams; o.bins = bins; o.counts = counts; o.wts = wts;
+        o.beams = beams; o.bins = bins; o.counts = counts; o.wts = wts; o.std = std;
         return o.shaped(h);
     }
 };
@@ -324,6 +331,7 @@ struct music_b200 {
     uint32_t host_chunk = 0;
     bool host_spec_alloc = false;
     bool host_beam_alloc = false;      // the staging slots hold beam and weight rows
+    bool host_crb_alloc = false;       // the staging slots hold CRB rows
     cudaStream_t last_fused_stream[2] = {nullptr, nullptr};  // per ticket counter: launches on one stream need no event
 
     // caller memory registered for DMA (cudaHostRegister), newest last: GNU Radio hands work() the same pageable
@@ -365,6 +373,7 @@ Outputs &Outputs::shaped(const music_b200 *h)
     K = h->K;
     m = h->m;
     N = h->N;
+    sw = h->azel ? 3 * h->n : h->n;
     gather = h->gather;
     return *this;
 }
@@ -712,6 +721,7 @@ struct Plan {
     Peaks peaks = Peaks::None;
     bool decode = false, refine = false;             // az-el bin decode; peak refinement (the az-el kind after a decode)
     bool beams = false;                              // beam weights (+ beams) after the peaks: the beams entry points
+    bool crb = false;                                // the CRB of every slot after the peaks (and beams): the crb entries
     bool calib = false;                              // correct R after the covariance (and the beam weights) by the calibration
     bool integ = false;                              // then integrate R across windows (music_b200_set_integration)
     bool ws_p64 = false, ws_counts = false, ws_bins = false, ws_wts = false;  // workspace buffers the kernels write
@@ -735,7 +745,7 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
     // A beams call needs R, which the fused kernels keep in registers: it runs the unfused plan of a call that asks for R.
     const bool beams = o.wts || o.beams;
     const bool fusable = h->fused && !h->chan && !h->azel && music_est && fixed_n && md.refine == MUSIC_B200_REFINE_OFF &&
-                         md.peak == MUSIC_B200_PEAKS_TOP_BINS && h->n == 1 && !o.P64 && !o.R && !o.ev && !beams && !h->calib &&
+                         md.peak == MUSIC_B200_PEAKS_TOP_BINS && h->n == 1 && !o.P64 && !o.R && !o.ev && !beams && !o.std && !h->calib &&
                          h->integ_alpha == 0.0;
     if (fusable && h->m == 4 && planar_fusable && (!o.spec || h->fused_spec)) p.path = Path::Fused4;
     else if (fusable && h->m == 8 && !planar && !o.spec && h->N >= 128 && h->N % 2 == 0) p.path = Path::Fused8;
@@ -767,9 +777,10 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
     p.ws_p64 = p.p64 && !o.P64;
     p.ws_counts = p.count;
     p.beams = beams;
+    p.crb = o.std != nullptr;
     p.calib = h->calib;
     p.integ = h->integ_alpha > 0.0;
-    p.ws_bins = p.decode || p.refine || (beams && !o.bins);
+    p.ws_bins = p.decode || p.refine || ((beams || p.crb) && !o.bins);
     p.ws_wts = beams && !o.wts;
     if (h->chan && h->chan_combine == MUSIC_B200_CHANNELS_INCOHERENT) {
         // every channel's scan writes its fp64 strengths into the workspace; the combine kernel writes the spectrum and
@@ -1063,6 +1074,22 @@ void launch_beams(music_b200 *h, const Plan &p, const WsView &ws, uint32_t W, co
     h->launches++;
 }
 
+// The CRB of every filled slot of W windows from ws.R and the angles (and elevations) and bins po holds, into o.std
+// (music_crb.cuh); under integration N_eff per window from the sub-batch's count ws.n0.
+void launch_crb(music_b200 *h, const Plan &p, const WsView &ws, uint32_t W, const Outputs &o, const PeakOut &po, uint32_t nsnap,
+                cudaStream_t st)
+{
+    const DeviceTable &tb = table(h);
+    const unsigned long long *n0 = p.integ ? ws.n0 : nullptr;
+    if (h->azel)
+        crb_kernel<true><<<W, 32, 0, st>>>(ws.R, po.angles, o.elev, po.bins, n0, (int)h->m, (int)h->n, (int)W, (int)nsnap,
+                                           h->integ_alpha, tb.geo, tb.ageo, o.std);
+    else
+        crb_kernel<false><<<W, 32, 0, st>>>(ws.R, po.angles, nullptr, po.bins, n0, (int)h->m, (int)h->n, (int)W, (int)nsnap,
+                                            h->integ_alpha, tb.geo, tb.ageo, o.std);
+    h->launches++;
+}
+
 // K2 of W windows from ws.R as planned: the eigensolver, the source count from `nsnap` snapshots (into ws.cnt and, when
 // given, counts_out) and the MVDR preparation.  Returns the per-window counts the later stages read (NULL under FIXED).
 const int32_t *launch_eig_stage(music_b200 *h, const Plan &p, const WsView &ws, uint32_t W, int32_t *counts_out, uint32_t nsnap,
@@ -1113,7 +1140,8 @@ void launch_grid_peaks(music_b200 *h, Peaks peaks, const double *p64, uint32_t W
 // (of these W windows), on `st`, as planned.  tev (optional) = timing events [1..4].  An az-el handle's peak bins are decoded into (azimuth, elevation)
 // after the peak rule.  With refinement on, the refine kernel follows (timed with the peak rule) and reads the bins
 // written before it: from the caller's array, or from the workspace when the caller asked for none.  A beams call
-// then forms the weights and beams of the windows at d_in (timed with the peak rule as well).
+// then forms the weights and beams of the windows at d_in, and a CRB call the bound of every slot (both timed with the
+// peak rule as well).
 int launch_eig_scan(music_b200 *h, const Plan &p, const WsView &ws, uint32_t W, const Outputs &o, const DeviceTable &tb, uint32_t nsnap,
                     cudaStream_t st, cudaEvent_t *tev, const float *d_in = nullptr)
 {
@@ -1178,6 +1206,7 @@ int launch_eig_scan(music_b200 *h, const Plan &p, const WsView &ws, uint32_t W, 
         h->launches++;
     }
     if (p.beams) launch_beams(h, p, ws, W, o, po, d_in, st);
+    if (p.crb) launch_crb(h, p, ws, W, o, po, nsnap, st);
     if (tev) cudaEventRecord(tev[4], st);
     if (o.R)
         CU(h, cudaMemcpyAsync(o.R, ws.R, (size_t)W * M * M * 2 * sizeof(double), cudaMemcpyDeviceToDevice, st));
@@ -1244,6 +1273,9 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, const Ou
     if (h->azel && !out.elev) return fail(h, MUSIC_B200_EINVAL, "an az-el handle needs the elevation output");
     if (!planar && (reinterpret_cast<uintptr_t>(d_in) & 15u) != 0) return fail(h, MUSIC_B200_EINVAL, "d_in_c64 must be 16-byte aligned");
     if (const int rc = check_modes(h, h->modes, &table(h))) return rc;
+    if (out.std && !table(h).geometric)
+        return fail(h, MUSIC_B200_EINVAL, "the CRB needs a table built by music_b200_set_geometry%s(); the current one came from "
+                                          "set_table(), which has no geometry", h->azel ? "_azel" : "");
     if (h->source_rule == MUSIC_B200_SOURCES_FIXED && out.counts) {
         fill_counts_kernel<<<(nwindows + 255) / 256, 256, 0, st>>>(out.counts, (int)h->n, (int)nwindows);
         h->launches++;
@@ -1509,16 +1541,18 @@ void host_register(music_b200 *h, const void *ptr, size_t bytes, bool read_only)
     h->hostregs.push_back(music_b200::HostReg{lo, (size_t)(hi - lo)});
 }
 
-int ensure_host_staging(music_b200 *h, uint32_t chunk, bool spec, bool beams)
+int ensure_host_staging(music_b200 *h, uint32_t chunk, bool spec, bool beams, bool crb)
 {
-    if (chunk <= h->host_chunk && (!spec || h->host_spec_alloc) && (!beams || h->host_beam_alloc)) return MUSIC_B200_OK;
+    if (chunk <= h->host_chunk && (!spec || h->host_spec_alloc) && (!beams || h->host_beam_alloc) && (!crb || h->host_crb_alloc))
+        return MUSIC_B200_OK;
     spec = spec || h->host_spec_alloc;
     beams = beams || h->host_beam_alloc;
+    crb = crb || h->host_crb_alloc;
     const uint32_t cap = std::max(chunk, h->host_chunk);
     // every old buffer is freed before the first new one is allocated
     for (HostSlot &sl : h->stage) sl = HostSlot();
     h->host_chunk = 0;
-    h->host_spec_alloc = h->host_beam_alloc = false;
+    h->host_spec_alloc = h->host_beam_alloc = h->host_crb_alloc = false;
     const size_t wn = (size_t)cap * h->n;
     const auto alloc = [&](auto &b) -> int {
         CU(h, b.angles.grow(wn));
@@ -1530,6 +1564,7 @@ int ensure_host_staging(music_b200 *h, uint32_t chunk, bool spec, bool beams)
             CU(h, b.beams.grow(wn * h->N * 2));
         }
         if (h->azel) CU(h, b.elev.grow(wn));
+        if (crb) CU(h, b.std.grow(h->azel ? 3 * wn : wn));
         return MUSIC_B200_OK;
     };
     for (HostSlot &sl : h->stage) {
@@ -1543,6 +1578,7 @@ int ensure_host_staging(music_b200 *h, uint32_t chunk, bool spec, bool beams)
     h->host_chunk = cap;
     h->host_spec_alloc = spec;
     h->host_beam_alloc = beams;
+    h->host_crb_alloc = crb;
     return MUSIC_B200_OK;
 }
 
@@ -1641,7 +1677,7 @@ int stage_host(music_b200 *h, const HostInput &in, uint32_t nwindows, const Outp
         music_b200 *c = lanes[l];
         if (cudaSetDevice(c->device) != cudaSuccess) { rc = fail(h, MUSIC_B200_ECUDA, "cudaSetDevice(%d) failed", c->device); break; }
         c->stage[0].W = c->stage[1].W = 0;  // nothing pending from an earlier (possibly failed) call
-        rc = ensure_host_staging(c, staged, dst.spec != nullptr, beams);
+        rc = ensure_host_staging(c, staged, dst.spec != nullptr, beams, dst.std != nullptr);
         if (rc && c != h) fail(h, rc, "%s", std::string(c->error).c_str());
     }
     const size_t cap = lanes[0]->host_chunk;
@@ -1686,6 +1722,7 @@ int stage_host(music_b200 *h, const HostInput &in, uint32_t nwindows, const Outp
                 if (!dst.counts) o.counts = nullptr;
                 if (!dst.wts) o.wts = nullptr;
                 if (!dst.beams) o.beams = nullptr;
+                if (!dst.std) o.std = nullptr;
                 rc = enqueue_device(c, in.streams ? nullptr : sl.in.get(), W, o, st, s, in.streams ? &S : nullptr, in.hop);
                 if (rc && c != h) fail(h, rc, "%s", std::string(c->error).c_str());
                 if (rc) break;
@@ -2347,6 +2384,49 @@ int music_b200_process_host_beams(music_b200 *h, const float *in_c64, uint32_t n
     return process_host_impl(h, in_c64, nwindows, o);
 }
 
+/* ---- the stochastic CRB of every slot (music_crb.cuh) ---- */
+namespace {
+
+// the checks every crb entry point makes before it runs: the output asked for and aligned, and the beams checks when
+// the call asks for weights or beams
+int check_crb_call(music_b200 *h, const void *out, const void *weights, const void *beams)
+{
+    if (!out) return fail(h, MUSIC_B200_EINVAL, "the CRB output must not be NULL");
+    if ((reinterpret_cast<uintptr_t>(out) & 3u) != 0) return fail(h, MUSIC_B200_EINVAL, "the CRB output must be 4-byte aligned");
+    if (weights || beams) return check_beams_call(h, weights, beams);
+    return MUSIC_B200_OK;
+}
+
+}  // namespace
+
+int music_b200_process_device_crb(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_angles, float *d_levels,
+                                  float *d_spectrum, int32_t *d_bins, int32_t *d_counts, double *d_weights, float *d_beams,
+                                  float *d_std, void *stream)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (const int rc = check_crb_call(h, d_std, d_weights, d_beams)) return rc;
+    Outputs o = caller_outputs(d_angles, d_levels, d_spectrum, d_bins);
+    o.counts = d_counts;
+    o.wts = d_weights;
+    o.beams = d_beams;
+    o.std = d_std;
+    return process_device_impl(h, d_in_c64, nwindows, o, stream);
+}
+
+int music_b200_process_host_crb(music_b200 *h, const float *in_c64, uint32_t nwindows, float *angles, float *levels, float *spectrum,
+                                int32_t *bins, int32_t *counts, double *weights, float *beams, float *std_out)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (h->azel) return fail(h, MUSIC_B200_EINVAL, "an az-el handle takes music_b200_process_azel_host_crb()");
+    if (const int rc = check_crb_call(h, std_out, weights, beams)) return rc;
+    Outputs o = caller_outputs(angles, levels, spectrum, bins);
+    o.counts = counts;
+    o.wts = weights;
+    o.beams = beams;
+    o.std = std_out;
+    return process_host_impl(h, in_c64, nwindows, o);
+}
+
 /* ---- receiver calibration (music_calib.cuh) ---- */
 int music_b200_set_calibration(music_b200 *h, const double *gains)
 {
@@ -2847,31 +2927,73 @@ int music_b200_azel_lattice_host(const double *positions_xyz, uint32_t m, double
     return MUSIC_B200_OK;
 }
 
+namespace {
+
+// The az-el device entry named `entry`, after its own checks: outputs o (the azimuths in o.angles, the elevations in
+// o.elev) in device memory.  process_azel_host_impl: the same for the host entries, outputs in host memory.
+int process_azel_device_impl(music_b200 *h, const char *entry, const float *d_in_c64, uint32_t nwindows, Outputs o, void *stream)
+{
+    if (!h->azel) return fail(h, MUSIC_B200_EINVAL, "%s needs a handle from music_b200_create_azel", entry);
+    if (nwindows && (!o.angles || !o.elev)) return fail(h, MUSIC_B200_EINVAL, "d_azimuth and d_elevation must not be NULL");
+    std::lock_guard<std::mutex> g(h->mutex);
+    NvtxRange range(entry);
+    CU(h, cudaSetDevice(h->device));
+    return enqueue_device(h, d_in_c64, nwindows, o.shaped(h), static_cast<cudaStream_t>(stream), 0);
+}
+
+int process_azel_host_impl(music_b200 *h, const char *entry, const float *in_c64, uint32_t nwindows, Outputs o)
+{
+    if (!h->azel) return fail(h, MUSIC_B200_EINVAL, "%s needs a handle from music_b200_create_azel", entry);
+    if (nwindows && !o.elev) return fail(h, MUSIC_B200_EINVAL, "elevation must not be NULL");
+    return process_host_impl(h, in_c64, nwindows, o);
+}
+
+// the outputs of the az-el entries
+Outputs azel_outputs(float *azimuth, float *elevation, float *levels, float *spectrum, int32_t *bins, int32_t *counts, float *crb)
+{
+    Outputs o = caller_outputs(azimuth, levels, spectrum, bins);
+    o.elev = elevation;
+    o.counts = counts;
+    o.std = crb;
+    return o;
+}
+
+}  // namespace
+
 int music_b200_process_azel_device(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_azimuth, float *d_elevation,
                                    float *d_levels, float *d_spectrum, int32_t *d_bins, int32_t *d_counts, void *stream)
 {
     if (!h) return MUSIC_B200_EINVAL;
-    if (!h->azel) return fail(h, MUSIC_B200_EINVAL, "process_azel_device needs a handle from music_b200_create_azel");
-    if (nwindows && (!d_azimuth || !d_elevation)) return fail(h, MUSIC_B200_EINVAL, "d_azimuth and d_elevation must not be NULL");
-    std::lock_guard<std::mutex> g(h->mutex);
-    NvtxRange range("music_b200_process_azel_device");
-    CU(h, cudaSetDevice(h->device));
-    Outputs o = caller_outputs(d_azimuth, d_levels, d_spectrum, d_bins);
-    o.elev = d_elevation;
-    o.counts = d_counts;
-    return enqueue_device(h, d_in_c64, nwindows, o.shaped(h), static_cast<cudaStream_t>(stream), 0);
+    return process_azel_device_impl(h, "music_b200_process_azel_device", d_in_c64, nwindows,
+                                    azel_outputs(d_azimuth, d_elevation, d_levels, d_spectrum, d_bins, d_counts, nullptr), stream);
 }
 
 int music_b200_process_azel_host(music_b200 *h, const float *in_c64, uint32_t nwindows, float *azimuth, float *elevation,
                                  float *levels, float *spectrum, int32_t *bins, int32_t *counts)
 {
     if (!h) return MUSIC_B200_EINVAL;
-    if (!h->azel) return fail(h, MUSIC_B200_EINVAL, "process_azel_host needs a handle from music_b200_create_azel");
-    if (nwindows && !elevation) return fail(h, MUSIC_B200_EINVAL, "elevation must not be NULL");
-    Outputs o = caller_outputs(azimuth, levels, spectrum, bins);
-    o.elev = elevation;
-    o.counts = counts;
-    return process_host_impl(h, in_c64, nwindows, o);
+    return process_azel_host_impl(h, "music_b200_process_azel_host", in_c64, nwindows,
+                                  azel_outputs(azimuth, elevation, levels, spectrum, bins, counts, nullptr));
+}
+
+int music_b200_process_azel_device_crb(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_azimuth, float *d_elevation,
+                                       float *d_levels, float *d_spectrum, int32_t *d_bins, int32_t *d_counts, float *d_crb, void *stream)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (h->azel)
+        if (const int rc = check_crb_call(h, d_crb, nullptr, nullptr)) return rc;
+    return process_azel_device_impl(h, "music_b200_process_azel_device_crb", d_in_c64, nwindows,
+                                    azel_outputs(d_azimuth, d_elevation, d_levels, d_spectrum, d_bins, d_counts, d_crb), stream);
+}
+
+int music_b200_process_azel_host_crb(music_b200 *h, const float *in_c64, uint32_t nwindows, float *azimuth, float *elevation,
+                                     float *levels, float *spectrum, int32_t *bins, int32_t *counts, float *crb)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (h->azel)
+        if (const int rc = check_crb_call(h, crb, nullptr, nullptr)) return rc;
+    return process_azel_host_impl(h, "music_b200_process_azel_host_crb", in_c64, nwindows,
+                                  azel_outputs(azimuth, elevation, levels, spectrum, bins, counts, crb));
 }
 
 /* ---- frequency-channelised direction finding (music_channels.cuh) ---- */

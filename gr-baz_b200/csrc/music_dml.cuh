@@ -29,16 +29,15 @@ __device__ __forceinline__ const double *dml_row(const double *soa, int k, int M
     return soa + (size_t)(k / TILE) * (2 * M + 1) * TILE + (k % TILE);
 }
 
-// Warp 0: Q[0 .. r-1] (row stride MAXM) = modified Gram-Schmidt, applied twice, of the rows bins[0 .. r-1] in that order;
-// T (row stride MAXM, may be null) receives the upper triangle of A = Q T.  Lane i holds component i.
-__device__ __forceinline__ void dml_mgs2(const double *soa, const int *bins, int r, int M, double2 *Q, double2 *T, int lane)
+// One warp: Q[0 .. r-1] (row stride MAXM) = modified Gram-Schmidt, applied twice, of the vectors a_0 .. a_(r-1) in that
+// order, a_l[i] = row(l, i); T (row stride MAXM, may be null) receives the upper triangle of A = Q T.  Lane i holds
+// component i.  Shared by the DML kernel and the CRB kernel (music_crb.cuh).
+template <class Row>
+__device__ __forceinline__ void mgs2(Row row, int r, int M, double2 *Q, double2 *T, int lane)
 {
     for (int l = 0; l < r; ++l) {
         double2 v = make_double2(0.0, 0.0);
-        if (lane < M) {
-            const double *a = dml_row(soa, bins[l], M);
-            v = make_double2(a[(size_t)(2 * lane) * TILE], a[(size_t)(2 * lane + 1) * TILE]);
-        }
+        if (lane < M) v = row(l, lane);
         for (int j = 0; j < l; ++j) {
             if (T && lane == 0) T[j * MAXM + l] = make_double2(0.0, 0.0);
         }
@@ -57,6 +56,15 @@ __device__ __forceinline__ void dml_mgs2(const double *soa, const int *bins, int
         if (T && lane == 0) T[l * MAXM + l] = make_double2(nrm, 0.0);
         __syncwarp();
     }
+}
+
+// Warp 0 of dml_kernel: mgs2 of the table rows bins[0 .. r-1]
+__device__ __forceinline__ void dml_mgs2(const double *soa, const int *bins, int r, int M, double2 *Q, double2 *T, int lane)
+{
+    mgs2([&](int l, int i) {
+        const double *a = dml_row(soa, bins[l], M);
+        return make_double2(a[(size_t)(2 * i) * TILE], a[(size_t)(2 * i + 1) * TILE]);
+    }, r, M, Q, T, lane);
 }
 
 // R: per window M * M complex doubles (row-major); soa: the table tiles [ceil(K / TILE)][2M + 1][TILE]; counts (may be

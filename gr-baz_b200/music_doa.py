@@ -223,6 +223,33 @@ class music_doa(object):
         """Restart the integration at the next window (the next window's covariance is its own)."""
         _capi.check(self._lib.music_b200_reset_integration(self._h), self._h)
 
+    # -- extension: the stochastic Cramer-Rao bound of every reported direction ------------------------------------
+    def set_crb(self, enable):
+        """True: ``work()`` also returns, through ``last_crb()``, the stochastic Cramer-Rao bound on the standard deviation
+        of every reported angle, in degrees, evaluated on the device at the window's covariance and reported angles
+        (include/music_b200.h).  It is the bound for Gaussian sources in white noise, the same whatever peak mode found
+        the angle, not that estimator's own variance.  Needs a table installed with ``set_array_geometry``.  Under the
+        "top_bins" peak mode with n >= 2 the slots are neighbouring bins of one peak, and their finite values mean
+        nothing: use "local_maxima" or a gridless mode there."""
+        self._crb = bool(enable)
+
+    def crb(self):
+        return getattr(self, "_crb", False)
+
+    def last_crb(self):
+        """float32 (W, n) bound of the last work() call in degrees (0 for unfilled slots, NaN where the window's bound
+        does not exist); None while ``set_crb`` is off.  On a ``music_doa_azel`` block (W, n, 3): std of the azimuth,
+        std of the elevation (degrees) and their correlation."""
+        return getattr(self, "_last_crb", None)
+
+    def process_device_crb(self, d_in, nwindows, d_angles, d_std, d_levels=None, d_spectrum=None, d_bins=None, d_counts=None,
+                           d_weights=None, d_beams=None, stream=None):
+        """Raw device-pointer entry (ints): the outputs of ``process_device_beams`` plus ``d_std`` (float32
+        [nwindows][n], required); ``d_weights`` and ``d_beams`` may both be None, and otherwise need a beamformer."""
+        rc = self._lib.music_b200_process_device_crb(self._h, d_in, int(nwindows), d_angles, d_levels, d_spectrum, d_bins,
+                                                      d_counts, d_weights, d_beams, d_std, stream)
+        _capi.check(rc, self._h)
+
     # -- extension: receiver calibration -----------------------------------------------------------------
     CALIBRATIONS = {"phase": 1, "gain_phase": 2}
 
@@ -331,15 +358,25 @@ class music_doa(object):
         spec = outs[2] if len(outs) > 2 else None
         self._last_bins = np.empty((W, self.n), np.int32)
         lvl_p, spec_p = lvl.ctypes.data if lvl is not None else None, spec.ctypes.data if spec is not None else None
-        self._last_beams = self._last_weights = None
-        if self.beamformer()[0] != "off":
+        self._last_beams = self._last_weights = self._last_crb = None
+        beams = self.beamformer()[0] != "off"
+        if beams:
             N = self.nsamples // self.m
-            self._last_counts = np.empty(W, np.int32)
             self._last_weights = np.empty((W, self.n, self.m), np.complex128)
             self._last_beams = np.empty((W, self.n, N), np.complex64)
+        wts_p = self._last_weights.ctypes.data if beams else None
+        beams_p = self._last_beams.ctypes.data if beams else None
+        if self.crb():
+            # one call for the bound and the beams: two would advance the integration carry twice
+            self._last_counts = np.empty(W, np.int32)
+            self._last_crb = np.empty((W, self.n), np.float32)
+            rc = self._lib.music_b200_process_host_crb(self._h, x.ctypes.data, W, ang.ctypes.data, lvl_p, spec_p,
+                                                       self._last_bins.ctypes.data, self._last_counts.ctypes.data, wts_p, beams_p,
+                                                       self._last_crb.ctypes.data)
+        elif beams:
+            self._last_counts = np.empty(W, np.int32)
             rc = self._lib.music_b200_process_host_beams(self._h, x.ctypes.data, W, ang.ctypes.data, lvl_p, spec_p,
-                                                         self._last_bins.ctypes.data, self._last_counts.ctypes.data,
-                                                         self._last_weights.ctypes.data, self._last_beams.ctypes.data)
+                                                         self._last_bins.ctypes.data, self._last_counts.ctypes.data, wts_p, beams_p)
         elif self.source_rule() == "fixed":
             rc = self._lib.music_b200_process_host(self._h, x.ctypes.data, W, ang.ctypes.data, lvl_p, spec_p, self._last_bins.ctypes.data)
             self._last_counts = np.full(W, self.n, np.int32)

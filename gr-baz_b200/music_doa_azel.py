@@ -93,8 +93,15 @@ class music_doa_azel(music_doa):
         ptr = lambda i: outs[i].ctypes.data if len(outs) > i else None
         self._last_bins = np.empty((W, self.n), np.int32)
         self._last_counts = np.empty(W, np.int32)
-        rc = self._lib.music_b200_process_azel_host(self._h, x.ctypes.data, W, ptr(0), ptr(1), ptr(2), ptr(3),
-                                                    self._last_bins.ctypes.data, self._last_counts.ctypes.data)
+        self._last_crb = None
+        if self.crb():
+            self._last_crb = np.empty((W, self.n, 3), np.float32)
+            rc = self._lib.music_b200_process_azel_host_crb(self._h, x.ctypes.data, W, ptr(0), ptr(1), ptr(2), ptr(3),
+                                                            self._last_bins.ctypes.data, self._last_counts.ctypes.data,
+                                                            self._last_crb.ctypes.data)
+        else:
+            rc = self._lib.music_b200_process_azel_host(self._h, x.ctypes.data, W, ptr(0), ptr(1), ptr(2), ptr(3),
+                                                        self._last_bins.ctypes.data, self._last_counts.ctypes.data)
         _capi.check(rc, self._h)
         return W
 
@@ -103,4 +110,12 @@ class music_doa_azel(music_doa):
         """Raw device-pointer entry (ints); buffers stay resident in HBM."""
         rc = self._lib.music_b200_process_azel_device(self._h, d_in, int(nwindows), d_azimuth, d_elevation, d_levels,
                                                       d_spectrum, d_bins, d_counts, stream)
+        _capi.check(rc, self._h)
+
+    def process_device_crb(self, d_in, nwindows, d_azimuth, d_elevation, d_crb, d_levels=None, d_spectrum=None, d_bins=None,
+                           d_counts=None, stream=None):
+        """Raw device-pointer entry (ints): the outputs of ``process_device`` plus ``d_crb`` (float32
+        [nwindows][n][3], required)."""
+        rc = self._lib.music_b200_process_azel_device_crb(self._h, d_in, int(nwindows), d_azimuth, d_elevation, d_levels,
+                                                          d_spectrum, d_bins, d_counts, d_crb, stream)
         _capi.check(rc, self._h)

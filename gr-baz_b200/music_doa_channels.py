@@ -110,6 +110,12 @@ class music_doa_channels(music_doa):
             _capi.check(self._lib.music_b200_get_table_channel(self._h, c, out[i].ctypes.data), self._h)
         return out if channel is None else out[0]
 
+    def set_crb(self, enable):
+        """The CRB of every slot is not built for channel handles (include/music_b200.h): enabling it raises, as the C
+        entry points refuse a channel handle."""
+        if enable:
+            raise ValueError("the CRB is not built for channel handles")
+
     def process_host(self, x, nwindows, levels=True, spectrum=False, bins=True, counts=False, R=False):
         """The host entry on complex64 windows x, results in the C ABI's channel-major layout: a dict of angles / levels /
         bins (rows, W, n), counts (rows, W), spectrum (rows, W, resolution), R (count, W, m, m) complex128, under

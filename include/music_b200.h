@@ -509,6 +509,69 @@ int music_b200_set_integration(music_b200 *h, double alpha);
 int music_b200_reset_integration(music_b200 *h);
 
 /*
+ * How precise every direction is (extension, no reference counterpart): the stochastic Cramer-Rao bound of each filled
+ * peak slot, evaluated on the device at the window's own covariance and its reported angles (Stoica, Larsson &
+ * Gershman, IEEE SP Letters 8(5), 2001; Stoica & Nehorai, IEEE Trans. ASSP 38(10), 1990).  It is the bound for
+ * Gaussian sources in white noise at the estimated parameters: the measurement variance a tracker, a triangulation or
+ * a display needs, the same whatever peak mode or estimator produced the angles.  It is NOT the variance of the
+ * estimator that produced the angle.  For window w:
+ *   R          the covariance every other stage reads (what process_device_ex's d_R returns: after the calibration and
+ *              the integration).  M = m.
+ *   N          nsamples / m, or while integration is on N_eff,j = N c_j^2 / q_j, the value MDL / AIC use.
+ *   S          the filled slots {i : bins[w][i] >= 0} in slot order (they need not form a prefix), d = |S|.
+ *   steering   for each i in S the reported float angle, widened to fp64, in radians (az-el: the (azimuth, elevation)
+ *              pair): a_i with the refinement's convention (1-D: a_m = exp(-j phi_m); az-el: a_m = exp(-j theta_m)), and
+ *              the derivative columns, 1-D d_i = da/dt = -j psi o a_i; az-el da/daz = -j theta_az o a_i and
+ *              da/del = -j theta_el o a_i (the refinement's psi, theta_az and theta_el).
+ *   algorithm  in fp64:
+ *              1. A = [a_i] = Q T by modified Gram-Schmidt applied twice (as the DML levels).  The window fails if any
+ *                 |T_ii|^2 <= 2^-30 ||a_i||^2.
+ *              2. s2 = (tr R - tr(Q^H R Q)) / (M - d), DML's noise level.  The window fails if s2 <= 0 or not finite.
+ *              3. H = T^-1 (Q^H R Q) T^-H (= A^+ R A^+H), Gamma = T^-1 T^-H (= (A^H A)^-1), P = H - s2 Gamma (the
+ *                 concentrated stochastic-ML source covariance), U = P H^-1 P with H by Cholesky; a pivot that is not
+ *                 > 0 fails the window.  P is never inverted: coherent sources (a rank-deficient P) are fine.
+ *              4. B = D^H (I - Q Q^H) D over the derivative columns (the columns are projected twice, as step 1).  The
+ *                 Fisher matrix over the parameters in slot order: 1-D F_ij = (2 N / s2) Re(B_ij U_ji); az-el with the
+ *                 parameters (az_0, el_0, az_1, el_1, ...) F_(i,u),(j,v) = (2 N / s2) Re((d_iu^H P_perp d_jv) U_ji).
+ *                 With p_m the element positions and pbar their centroid, G = (2 pi / lambda)^2 sum_m |p_m - pbar|^2 bounds
+ *                 B_cc for every direction; the window fails if any B_cc <= 2^-40 G (the parameter is unobservable to
+ *                 first order: its derivative vanishes, or lies in span(A), to rounding).
+ *              5. C = F^-1 by Cholesky: a pivot <= 2^-40 F_kk (before its square root), or NaN, fails the window.
+ *   outputs    1-D std[w][i] = (float)(sqrt(C_ii) 180 / pi), degrees.  Az-el crb[w][i] = {std_az, std_el, rho}: both
+ *              standard deviations in degrees and rho = C_(az,el) / sqrt(C_(az,az) C_(el,el)), the dimensionless
+ *              correlation (from C in radians).  Unfilled slots get 0; in a failed window every filled slot gets NaN.
+ *   caveats    the bound is that of a model with d sources at the reported angles; nothing here tests whether the data
+ *              contain them.  n >= 2 under TOP_BINS puts the slots on neighbouring bins of one peak: such windows get
+ *              finite values, the bound of two sources one bin apart, which mean nothing for one source (use LOCAL_MAXIMA
+ *              or a gridless mode with n >= 2).  The two mirror slots of a line array fail the window (step 1).  A ULA at
+ *              end-fire (0 or 180 degrees, where psi vanishes to rounding), a planar array at el = 0 (da/del = 0) and the
+ *              azimuth at el = +-90 degrees (da/daz = 0) fail it (step 4).
+ * The 1-D entries take the outputs of the beams entries plus d_std [W][n] floats (required); d_weights and d_beams may
+ * both be NULL, and otherwise need a beamformer set (as process_*_beams), so that one call returns angles, beams and
+ * their bounds (two calls would advance the integration twice).  The az-el entries take the outputs of
+ * process_azel_device / _host plus d_crb [W][n][3] floats (required).  Every output is 4-byte aligned (weights and beams
+ * as for the beams entries).  The host entry deals windows over a multi-device handle as process_host does; the device
+ * entry goes to the device the input lives on.  A CRB call runs the unfused kernels: its angles, levels, spectrum, bins,
+ * counts, weights and beams are byte-identical to process_device_ex() with d_R (process_device_beams with weights or
+ * beams) on the same windows.  Per sub-batch it adds crb_kernel after the peak stage (and the refinement and the beam
+ * weights), timed in the top-n slot of the stage timing.
+ * EINVAL, with no fall-back: a current table from set_table() (it has no geometry); channel handles; a 1-D entry on an
+ * az-el handle or the reverse; NULL d_std / d_crb; a misaligned output; weights or beams without a beamformer.
+ * Not built: the CRB of set_table() manifolds (they would need the table's derivative), of channel handles and of the
+ * planar, sharded and gather entries.
+ */
+int music_b200_process_device_crb(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_angles, float *d_levels,
+                                  float *d_spectrum, int32_t *d_bins, int32_t *d_counts, double *d_weights, float *d_beams,
+                                  float *d_std, void *stream);
+int music_b200_process_host_crb(music_b200 *h, const float *in_c64, uint32_t nwindows, float *angles, float *levels,
+                                float *spectrum, int32_t *bins, int32_t *counts, double *weights, float *beams, float *std_out);
+int music_b200_process_azel_device_crb(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_azimuth,
+                                       float *d_elevation, float *d_levels, float *d_spectrum, int32_t *d_bins,
+                                       int32_t *d_counts, float *d_crb, void *stream);
+int music_b200_process_azel_host_crb(music_b200 *h, const float *in_c64, uint32_t nwindows, float *azimuth, float *elevation,
+                                     float *levels, float *spectrum, int32_t *bins, int32_t *counts, float *crb);
+
+/*
  * Downstream reducers (extension, no reference counterpart): what a GUI-rate consumer such as the DOA
  * compass (/root/reference/python/doa_compass_control.py:102-108) or a plot sink
  * (/root/reference/python/plot_sink.py:38) needs from millions of windows per second.

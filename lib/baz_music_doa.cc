@@ -73,7 +73,7 @@ baz_music_doa::baz_music_doa(unsigned int m, unsigned int n, unsigned int nsampl
     : gr::sync_block("music_doa", gr::io_signature::make(1, 1, nsamples * sizeof(gr_complex)),
                      gr::io_signature::make3(1, 3, n * sizeof(float), n * sizeof(float), resolution * sizeof(float))),
       d_m(m), d_n(n), d_nsamples(nsamples), d_resolution(resolution), d_handle(NULL), d_source_rule(MUSIC_B200_SOURCES_FIXED),
-      d_beam_rule(MUSIC_B200_BEAMS_OFF), d_cal_remaining(0), d_cal_angle(0.0), d_cal_kind(MUSIC_B200_CALIB_GAIN_PHASE),
+      d_beam_rule(MUSIC_B200_BEAMS_OFF), d_crb(false), d_cal_remaining(0), d_cal_angle(0.0), d_cal_kind(MUSIC_B200_CALIB_GAIN_PHASE),
       d_cal_residual(std::numeric_limits<double>::quiet_NaN())
 {
     if (array_response.size() != resolution) throw std::invalid_argument("music_doa: array_response.size() != resolution");
@@ -198,6 +198,13 @@ void baz_music_doa::reset_integration()
     if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa: ") + music_b200_last_error(d_handle));
 }
 
+/* Extension (not in the reference): the stochastic CRB of every reported angle, see include/music_b200.h. */
+void baz_music_doa::set_crb(bool enable)
+{
+    gr::thread::scoped_lock guard(d_mutex);
+    d_crb = enable;
+}
+
 void baz_music_doa::set_calibration(const std::vector<std::complex<double> > &gains)
 {
     if (!gains.empty() && gains.size() != d_m) throw std::invalid_argument("music_doa: gains.size() != m");
@@ -245,8 +252,16 @@ int baz_music_doa::work(int noutput_items, gr_vector_const_void_star &input_item
     gr::thread::scoped_lock guard(d_mutex);
     d_bins.resize((size_t)noutput_items * d_n);
     d_beams.clear();
+    d_crb_out.clear();
     int rc;
-    if (d_beam_rule != MUSIC_B200_BEAMS_OFF) {
+    if (d_crb) {
+        /* one call for the bound and the beams: two would advance the integration carry twice */
+        d_counts.resize((size_t)noutput_items);
+        d_crb_out.resize((size_t)noutput_items * d_n);
+        if (d_beam_rule != MUSIC_B200_BEAMS_OFF) d_beams.resize((size_t)noutput_items * d_n * (d_nsamples / d_m));
+        rc = music_b200_process_host_crb(d_handle, in, (uint32_t)noutput_items, out, lvl, out_spectrum, d_bins.data(), d_counts.data(),
+                                         NULL, d_beams.empty() ? NULL : reinterpret_cast<float *>(d_beams.data()), d_crb_out.data());
+    } else if (d_beam_rule != MUSIC_B200_BEAMS_OFF) {
         d_counts.resize((size_t)noutput_items);
         d_beams.resize((size_t)noutput_items * d_n * (d_nsamples / d_m));
         rc = music_b200_process_host_beams(d_handle, in, (uint32_t)noutput_items, out, lvl, out_spectrum, d_bins.data(), d_counts.data(),

@@ -87,6 +87,10 @@ public:
      * set_array_geometry() and set_calibration(). */
     void set_integration(double alpha);
     void reset_integration();
+    /* extension: true = every work() call also returns the stochastic Cramer-Rao bound on the standard deviation of each
+     * reported angle, in degrees (include/music_b200.h), read back with last_crb(); with the beamformer on, the bound and
+     * the beams come from the same single call.  Needs a table from set_array_geometry(). */
+    void set_crb(bool enable);
 
     /* Integer peak-bin indices of the items produced by the last work() call, [items][n]
      * (not in the reference; -1 marks a slot the reference would leave at (0, 0)). */
@@ -97,6 +101,9 @@ public:
     /* Beams of the items produced by the last work() call while set_beamformer() is on, [items][n][nsamples / m]
      * (zeros for unfilled slots); empty while it is off. */
     const std::vector<gr_complex> &last_beams() const { return d_beams; }
+    /* The bound of the items produced by the last work() call while set_crb() is on, [items][n] degrees (0 for unfilled
+     * slots, NaN where the item's bound does not exist); empty while it is off. */
+    const std::vector<float> &last_crb() const { return d_crb_out; }
 
 private:
     std::vector<float> flatten(const array_response_t &array_response) const;
@@ -109,8 +116,10 @@ private:
     std::vector<int> d_bins;
     std::vector<int> d_counts;
     std::vector<gr_complex> d_beams;
+    std::vector<float> d_crb_out;
     int d_source_rule;
     int d_beam_rule;
+    bool d_crb;
     /* calibrate(): items still to accumulate (0: not armed), the source direction and the kind; the last residual */
     int d_cal_remaining;
     double d_cal_angle;

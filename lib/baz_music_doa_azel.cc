@@ -164,6 +164,12 @@ void baz_music_doa_azel::calibrate(double az_deg, double el_deg, int kind, int n
     d_cal_kind = kind;
 }
 
+void baz_music_doa_azel::set_crb(bool enable)
+{
+    gr::thread::scoped_lock guard(d_mutex);
+    d_crb = enable;
+}
+
 int baz_music_doa_azel::work(int noutput_items, gr_vector_const_void_star &input_items, gr_vector_void_star &output_items)
 {
     if (noutput_items <= 0) return 0;
@@ -177,7 +183,10 @@ int baz_music_doa_azel::work(int noutput_items, gr_vector_const_void_star &input
     gr::thread::scoped_lock guard(d_mutex);
     d_bins.resize((size_t)noutput_items * d_n);
     d_counts.resize((size_t)noutput_items);
-    const int rc = music_b200_process_azel_host(d_handle, in, (uint32_t)noutput_items, az, el, lvl, spectrum, d_bins.data(), d_counts.data());
+    d_crb_out.assign(d_crb ? (size_t)noutput_items * d_n * 3 : 0, 0.0f);
+    const int rc = d_crb ? music_b200_process_azel_host_crb(d_handle, in, (uint32_t)noutput_items, az, el, lvl, spectrum, d_bins.data(),
+                                                            d_counts.data(), d_crb_out.data())
+                         : music_b200_process_azel_host(d_handle, in, (uint32_t)noutput_items, az, el, lvl, spectrum, d_bins.data(), d_counts.data());
     if (rc != MUSIC_B200_OK) throw std::runtime_error(std::string("music_doa_azel: ") + music_b200_last_error(d_handle));
     calibration_step(d_handle, in, noutput_items, d_cal_remaining, d_cal_az, d_cal_el, d_cal_kind, d_cal_residual);
     return noutput_items;

@@ -64,6 +64,10 @@ public:
     /* covariance integration across work() calls, as for baz_music_doa */
     void set_integration(double alpha);
     void reset_integration();
+    /* the stochastic Cramer-Rao bound of every reported direction, as for baz_music_doa: last_crb() holds
+     * [items][n][3] = std of the azimuth, std of the elevation (degrees), their correlation */
+    void set_crb(bool enable);
+    const std::vector<float> &last_crb() const { return d_crb_out; }
 
     /* flat peak bins b = i * n_az + k of the items produced by the last work() call, [items][n] (-1: unfilled slot) */
     const std::vector<int> &last_bins() const { return d_bins; }
@@ -78,6 +82,8 @@ private:
     music_b200 *d_handle;
     std::vector<int> d_bins;
     std::vector<int> d_counts;
+    std::vector<float> d_crb_out;
+    bool d_crb = false;
     int d_cal_remaining;
     double d_cal_az, d_cal_el;
     int d_cal_kind;

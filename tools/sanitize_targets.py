@@ -2,7 +2,7 @@
 """Small invocations of the kernels compute-sanitizer should look at (SURVEY.md section 5): run as
   compute-sanitizer --tool racecheck|memcheck|synccheck python tools/sanitize_targets.py <target>
 targets: fused (C1-size windows, 2000 of them + a ragged 1187 + a drain-only 9), fused_jacobi, fused8, covn8, covn16, eig16, esprit2d,
-gridless_roots, multi,
+gridless_roots, crb, multi,
 lifecycle (every handle kind created, retuned, grown and destroyed through the host entry points; run it under
   compute-sanitizer --tool memcheck --leak-check full, which reports what a handle leaves allocated)"""
 import os
@@ -85,6 +85,40 @@ elif target == "gridless_roots":
         blk.work(W, [x], [ang])
         print(target, "ok", mode, m, ang[:2].tolist())
         blk.close()
+elif target == "crb":
+    # the CRB kernel (music_crb.cuh): 1-D at M = 3, 8 and 16 with n up to M - 1 (every slot filled by DML, so d = 15 at
+    # M = 16), and az-el at M = 16 with n = 15 (30 parameters, the largest shared-memory footprint); a zero window and a
+    # NaN window among them
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+    from gr_baz_b200.music_doa_azel import music_doa_azel
+    from helpers import LAM
+
+    W = 37
+    for m, n, mode in ((3, 2, "dml"), (8, 3, "local_maxima"), (16, 15, "dml")):
+        rng = np.random.default_rng(m)
+        x = ((rng.standard_normal((W, 64 * m)) + 1j * rng.standard_normal((W, 64 * m)))).astype(np.complex64)
+        x[3] = 0
+        x[5, 11] = np.nan
+        k = np.arange(m)
+        pos = np.stack([0.5 * LAM * np.cos(2 * np.pi * k / m) * m / 6, 0.5 * LAM * np.sin(2 * np.pi * k / m) * m / 6], 1)
+        blk = music_doa(m, n, 64 * m, np.ones((360, m), np.complex64), 360)
+        blk.set_array_geometry(pos, LAM)
+        blk.set_peak_mode(mode, 0)
+        blk.set_crb(True)
+        blk.work(W, [x], [np.zeros((W, n), np.float32)])
+        print(target, "ok", m, n, mode, blk.last_crb()[:2].tolist())
+        blk.close()
+    m, n = 16, 15
+    rng = np.random.default_rng(16)
+    x = ((rng.standard_normal((W, 64 * m)) + 1j * rng.standard_normal((W, 64 * m)))).astype(np.complex64)
+    x[3] = 0
+    pos = rng.uniform(-0.6, 0.6, (m, 3)) * LAM
+    az = music_doa_azel(m, n, 64 * m, 36, 9, (0.0, 80.0), pos, LAM)
+    az.set_peak_mode("local_maxima", 0)
+    az.set_crb(True)
+    az.work(W, [x], [np.zeros((W, n), np.float32) for _ in range(3)])
+    print(target, "ok az-el", az.last_crb()[:1, :2].tolist())
+    az.close()
 elif target == "multi":
     cfg = synth.config(1)
     resp, table = bench.table_for(cfg)
