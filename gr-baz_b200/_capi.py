@@ -130,6 +130,20 @@ def load():
         L.music_b200_process_azel_device_crb.restype = ctypes.c_int
         L.music_b200_process_azel_host_crb.argtypes = [vp, fp, u32, fp, fp, fp, fp, fp, fp, fp]
         L.music_b200_process_azel_host_crb.restype = ctypes.c_int
+        L.music_b200_set_tracking.argtypes = [vp, ctypes.c_int, dbl, dbl, dbl, dbl, dbl, u32, u32, u32, u32]
+        L.music_b200_set_tracking.restype = ctypes.c_int
+        L.music_b200_reset_tracks.argtypes = [vp]
+        L.music_b200_reset_tracks.restype = ctypes.c_int
+        L.music_b200_get_tracks.argtypes = [vp, fp, fp, ctypes.POINTER(u32)]
+        L.music_b200_get_tracks.restype = ctypes.c_int
+        L.music_b200_process_device_tracks.argtypes = [vp, fp, u32, fp, fp, fp, fp, fp, fp, fp, fp, fp, fp, fp, vp]
+        L.music_b200_process_device_tracks.restype = ctypes.c_int
+        L.music_b200_process_host_tracks.argtypes = [vp, fp, u32, fp, fp, fp, fp, fp, fp, fp, fp, fp, fp, fp]
+        L.music_b200_process_host_tracks.restype = ctypes.c_int
+        L.music_b200_process_azel_device_tracks.argtypes = [vp, fp, u32, fp, fp, fp, fp, fp, fp, fp, fp, fp, fp, vp]
+        L.music_b200_process_azel_device_tracks.restype = ctypes.c_int
+        L.music_b200_process_azel_host_tracks.argtypes = [vp, fp, u32, fp, fp, fp, fp, fp, fp, fp, fp, fp, fp]
+        L.music_b200_process_azel_host_tracks.restype = ctypes.c_int
         L.music_b200_create_azel.argtypes = [ctypes.POINTER(vp), u32, u32, u32, u32, u32, dbl, dbl, fp, dbl, ctypes.c_int]
         L.music_b200_create_azel.restype = ctypes.c_int
         L.music_b200_set_geometry_azel.argtypes = [vp, fp, dbl]
@@ -189,7 +203,9 @@ EXPORTS = [
     "music_b200_set_calibration", "music_b200_get_calibration", "music_b200_calib_reset", "music_b200_calib_accumulate_device",
     "music_b200_calib_accumulate_host", "music_b200_calib_solve", "music_b200_set_integration", "music_b200_reset_integration",
     "music_b200_process_device_crb", "music_b200_process_host_crb", "music_b200_process_azel_device_crb",
-    "music_b200_process_azel_host_crb",
+    "music_b200_process_azel_host_crb", "music_b200_set_tracking", "music_b200_reset_tracks", "music_b200_get_tracks",
+    "music_b200_process_device_tracks", "music_b200_process_host_tracks", "music_b200_process_azel_device_tracks",
+    "music_b200_process_azel_host_tracks",
     "music_b200_create_channels", "music_b200_set_geometry_channels", "music_b200_channel_frequencies",
     "music_b200_get_table_channel", "music_b200_process_channels_device", "music_b200_process_channels_host",
     "music_b200_set_focusing", "music_b200_get_focusing",

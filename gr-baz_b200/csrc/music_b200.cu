@@ -41,6 +41,7 @@
 #include "music_calib.cuh"
 #include "music_integrate.cuh"
 #include "music_crb.cuh"
+#include "music_track.cuh"
 #include "music_channels.cuh"
 #include "music_focus.cuh"
 
@@ -129,7 +130,7 @@ struct TableSlot {
 };
 
 // A non-owning view of a workspace slot's buffers, or of one channel's run of them (enqueue_channels)
-struct WsView { double *R, *ev, *Vt, *P64; int32_t *cnt, *bins; double *wts; unsigned long long *n0; };
+struct WsView { double *R, *ev, *Vt, *P64; int32_t *cnt, *bins; double *wts; unsigned long long *n0; float *std; };
 
 struct Workspace {
     DevBuf<double> R, ev, Vt, P64;
@@ -137,9 +138,10 @@ struct Workspace {
     DevBuf<int32_t> bins;  // [windows][n] peak bins for the refinement and the beams when the caller asked for none
     DevBuf<double> wts;    // [windows][n][m] complex beam weights when a beams call asked for none
     DevBuf<unsigned long long> n0;  // integration: the count since the reset at the sub-batch's first window
+    DevBuf<float> std;     // [windows][sw] the CRB a tracks call under CRB variance reads when the caller asked for none
     cudaEvent_t scan_done = nullptr;
     bool used = false;
-    WsView view() const { return {R, ev, Vt, P64, cnt, bins, wts, n0}; }
+    WsView view() const { return {R, ev, Vt, P64, cnt, bins, wts, n0, std}; }
 };
 
 // The modes set by set_peak_mode(), set_refine() and set_estimator(); check_modes() says which combine.
@@ -172,10 +174,14 @@ struct Outputs {
     double *ev = nullptr;       // [W][m]
     double *wts = nullptr;      // [W][n][m] complex beam weights: beams entry points only
     float *beams = nullptr;     // [W][n][N] complex64 beams: beams entry points only
-    float *std = nullptr;       // [W][sw] the CRB of every slot: crb entry points only
+    float *std = nullptr;       // [W][sw] the CRB of every slot: crb and tracks entry points only
+    int32_t *slot_track = nullptr;   // [W][n] the track each slot's measurement updated or started: tracks entries only
+    int32_t *track_ids = nullptr;    // [W][T] the confirmed track of every carry row
+    float *track_state = nullptr;    // [W][tsw / T] its state
     Gather gather;
     uint32_t n = 0, K = 0, m = 0, N = 0;
     uint32_t sw = 0;            // floats per window of std: n, 3 n on an az-el handle
+    uint32_t T = 0, tsw = 0;    // carry rows of the tracker and floats per window of track_state: 3 T, 6 T on an az-el handle
 
     // the shape of h's calls and the all-gather h was attached to (music_b200_gather_attach)
     Outputs &shaped(const music_b200 *h);
@@ -197,15 +203,19 @@ struct Outputs {
         skip(o.wts, (size_t)n * m * 2);
         skip(o.beams, (size_t)n * N * 2);
         skip(o.std, sw);
+        skip(o.slot_track, n);
+        skip(o.track_ids, T);
+        skip(o.track_state, tsw);
         for (int p = 0; p < gather.G; ++p) skip(o.gather.peer[p], (size_t)gather.G * n);
         return o;
     }
 
     // the per-window outputs a host call stages through pinned memory (4-byte elements), with their elements per window
     struct Field { void *p; uint32_t per_win; };
-    std::array<Field, 6> window_fields() const
+    std::array<Field, 9> window_fields() const
     {
-        return {{{angles, n}, {elev, n}, {levels, n}, {bins, n}, {counts, 1}, {std, sw}}};
+        return {{{angles, n}, {elev, n}, {levels, n}, {bins, n}, {counts, 1}, {std, sw}, {slot_track, n}, {track_ids, T},
+                 {track_state, tsw}}};
     }
 
     // the rows of a beams call a host call stages through pinned memory, with their bytes per window
@@ -219,8 +229,8 @@ struct Outputs {
 // the buffers behind a staging slot's outputs, on the device or pinned (the spectrum is staged on the device only)
 template <template <class> class Buf>
 struct StagedOutputs {
-    Buf<float> angles, elev, levels, spec, beams, std;
-    Buf<int32_t> bins, counts;
+    Buf<float> angles, elev, levels, spec, beams, std, track_state;
+    Buf<int32_t> bins, counts, slot_track, track_ids;
     Buf<double> wts;
 
     Outputs view(const music_b200 *h) const
@@ -228,6 +238,7 @@ struct StagedOutputs {
         Outputs o;
         o.angles = angles; o.elev = elev; o.levels = levels; o.spec = spec;
         o.beams = beams; o.bins = bins; o.counts = counts; o.wts = wts; o.std = std;
+        o.slot_track = slot_track; o.track_ids = track_ids; o.track_state = track_state;
         return o.shaped(h);
     }
 };
@@ -284,6 +295,16 @@ struct music_b200 {
     DevBuf<double> integ_S, integ_tiles;
     DevBuf<unsigned long long> integ_cnt;
     cudaEvent_t integ_done = nullptr;
+    // angle tracking (music_b200_set_tracking, music_track.cuh), on while trk_var is not OFF: the parameters, the carry
+    // (rows, states and next_id) on the device, and the event that orders each sub-batch's tracking after the previous
+    // one's, on whichever stream that ran.  trk_fresh: the next tracking sub-batch starts from empty rows and next_id 0.
+    int trk_var = MUSIC_B200_TRACK_OFF;
+    TrackParams trk = {};
+    bool trk_fresh = true, trk_used = false;
+    DevBuf<int32_t> trk_rows;
+    DevBuf<double> trk_state;
+    DevBuf<unsigned> trk_next;
+    cudaEvent_t trk_done = nullptr;
     unsigned steer_guarded = 0;    // entries of the last built table re-evaluated with the host libm
     bool azel = false;             // music_b200_create_azel(): K = n_az * n_el rows, elevation-major (music_azel.cuh)
     AzelGrid grid = {};
@@ -332,6 +353,7 @@ struct music_b200 {
     bool host_spec_alloc = false;
     bool host_beam_alloc = false;      // the staging slots hold beam and weight rows
     bool host_crb_alloc = false;       // the staging slots hold CRB rows
+    uint32_t host_track_T = 0;         // the staging slots hold tracker rows for this many carry rows
     cudaStream_t last_fused_stream[2] = {nullptr, nullptr};  // per ticket counter: launches on one stream need no event
 
     // caller memory registered for DMA (cudaHostRegister), newest last: GNU Radio hands work() the same pageable
@@ -361,6 +383,7 @@ struct music_b200 {
         }
         if (fused_done) cudaEventDestroy(fused_done);
         if (integ_done) cudaEventDestroy(integ_done);
+        if (trk_done) cudaEventDestroy(trk_done);
         for (cudaEvent_t e : tev) cudaEventDestroy(e);
     }
 };
@@ -374,6 +397,8 @@ Outputs &Outputs::shaped(const music_b200 *h)
     m = h->m;
     N = h->N;
     sw = h->azel ? 3 * h->n : h->n;
+    T = h->trk.T;
+    tsw = (h->azel ? 6 : 3) * T;
     gather = h->gather;
     return *this;
 }
@@ -722,9 +747,10 @@ struct Plan {
     bool decode = false, refine = false;             // az-el bin decode; peak refinement (the az-el kind after a decode)
     bool beams = false;                              // beam weights (+ beams) after the peaks: the beams entry points
     bool crb = false;                                // the CRB of every slot after the peaks (and beams): the crb entries
+    bool track = false;                              // then the tracker (music_track.cuh): the tracks entries
     bool calib = false;                              // correct R after the covariance (and the beam weights) by the calibration
     bool integ = false;                              // then integrate R across windows (music_b200_set_integration)
-    bool ws_p64 = false, ws_counts = false, ws_bins = false, ws_wts = false;  // workspace buffers the kernels write
+    bool ws_p64 = false, ws_counts = false, ws_bins = false, ws_wts = false, ws_std = false;  // workspace buffers the kernels write
     bool combine = false;                            // channel handle, INCOHERENT: one spectrum per window from all channels
 };
 
@@ -744,9 +770,10 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
     for (uint32_t r = 0; planar && r < h->m; ++r) planar_fusable = planar_fusable && (reinterpret_cast<uintptr_t>(planar->p[r]) & 15u) == 0;
     // A beams call needs R, which the fused kernels keep in registers: it runs the unfused plan of a call that asks for R.
     const bool beams = o.wts || o.beams;
+    const bool track = o.slot_track != nullptr;
     const bool fusable = h->fused && !h->chan && !h->azel && music_est && fixed_n && md.refine == MUSIC_B200_REFINE_OFF &&
-                         md.peak == MUSIC_B200_PEAKS_TOP_BINS && h->n == 1 && !o.P64 && !o.R && !o.ev && !beams && !o.std && !h->calib &&
-                         h->integ_alpha == 0.0;
+                         md.peak == MUSIC_B200_PEAKS_TOP_BINS && h->n == 1 && !o.P64 && !o.R && !o.ev && !beams && !o.std && !track &&
+                         !h->calib && h->integ_alpha == 0.0;
     if (fusable && h->m == 4 && planar_fusable && (!o.spec || h->fused_spec)) p.path = Path::Fused4;
     else if (fusable && h->m == 8 && !planar && !o.spec && h->N >= 128 && h->N % 2 == 0) p.path = Path::Fused8;
 
@@ -777,11 +804,13 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
     p.ws_p64 = p.p64 && !o.P64;
     p.ws_counts = p.count;
     p.beams = beams;
-    p.crb = o.std != nullptr;
+    p.track = track;
+    p.crb = o.std != nullptr || (track && h->trk_var == MUSIC_B200_TRACK_CRB);
     p.calib = h->calib;
     p.integ = h->integ_alpha > 0.0;
-    p.ws_bins = p.decode || p.refine || ((beams || p.crb) && !o.bins);
+    p.ws_bins = p.decode || p.refine || ((beams || p.crb || track) && !o.bins);
     p.ws_wts = beams && !o.wts;
+    p.ws_std = p.crb && !o.std;
     if (h->chan && h->chan_combine == MUSIC_B200_CHANNELS_INCOHERENT) {
         // every channel's scan writes its fp64 strengths into the workspace; the combine kernel writes the spectrum and
         // the peak rule (also for n = 1) reads the combined strengths
@@ -800,7 +829,8 @@ uint32_t max_sub_windows(const music_b200 *h, const Plan &p)
 {
     const size_t per_win = (size_t)h->m * h->m * 2 * 8 * 2 + h->m * 8 + (p.ws_p64 ? (size_t)h->K * 8 : 0) +
                            (p.ws_counts ? sizeof(int32_t) : 0) + (p.ws_bins ? h->n * sizeof(int32_t) : 0) +
-                           (p.ws_wts ? (size_t)h->n * h->m * 2 * sizeof(double) : 0);
+                           (p.ws_wts ? (size_t)h->n * h->m * 2 * sizeof(double) : 0) +
+                           (p.ws_std ? (size_t)(h->azel ? 3 : 1) * h->n * sizeof(float) : 0);
     // A SEPARATE / INCOHERENT channel handle's workspace holds C pseudo-windows per window; a COHERENT one holds the
     // windows, and the channel buffer beside it the C covariances of each.
     const size_t C = h->chan ? (size_t)h->cshape.C : 1;
@@ -828,6 +858,7 @@ int ensure_slot(music_b200 *h, Workspace &ws, uint32_t windows, const Plan &p)
     if (const int rc = grow(ws.cnt, p.ws_counts ? w : 0)) return rc;
     if (const int rc = grow(ws.bins, p.ws_bins ? w * h->n : 0)) return rc;
     if (const int rc = grow(ws.n0, p.integ ? 1 : 0)) return rc;
+    if (const int rc = grow(ws.std, p.ws_std ? w * (h->azel ? 3 : 1) * h->n : 0)) return rc;
     return grow(ws.wts, p.ws_wts ? w * h->n * h->m * 2 : 0);
 }
 
@@ -1074,20 +1105,40 @@ void launch_beams(music_b200 *h, const Plan &p, const WsView &ws, uint32_t W, co
     h->launches++;
 }
 
-// The CRB of every filled slot of W windows from ws.R and the angles (and elevations) and bins po holds, into o.std
+// The CRB of every filled slot of W windows from ws.R and the angles (and elevations) and bins po holds, into std
 // (music_crb.cuh); under integration N_eff per window from the sub-batch's count ws.n0.
 void launch_crb(music_b200 *h, const Plan &p, const WsView &ws, uint32_t W, const Outputs &o, const PeakOut &po, uint32_t nsnap,
-                cudaStream_t st)
+                float *std, cudaStream_t st)
 {
     const DeviceTable &tb = table(h);
     const unsigned long long *n0 = p.integ ? ws.n0 : nullptr;
     if (h->azel)
         crb_kernel<true><<<W, 32, 0, st>>>(ws.R, po.angles, o.elev, po.bins, n0, (int)h->m, (int)h->n, (int)W, (int)nsnap,
-                                           h->integ_alpha, tb.geo, tb.ageo, o.std);
+                                           h->integ_alpha, tb.geo, tb.ageo, std);
     else
         crb_kernel<false><<<W, 32, 0, st>>>(ws.R, po.angles, nullptr, po.bins, n0, (int)h->m, (int)h->n, (int)W, (int)nsnap,
-                                            h->integ_alpha, tb.geo, tb.ageo, o.std);
+                                            h->integ_alpha, tb.geo, tb.ageo, std);
     h->launches++;
+}
+
+// The tracker over W windows from the angles (and elevations) and bins po holds and the CRB in std (read under CRB
+// variance), into o's slot_track, track_ids and track_state (music_track.cuh): one CTA, after the previous sub-batch's
+// tracking on whichever stream that ran, so the carry goes from one sub-batch to the next in enqueue order.
+int launch_track(music_b200 *h, uint32_t W, const Outputs &o, const PeakOut &po, const float *std, cudaStream_t st)
+{
+    if (h->trk_used) CU(h, cudaStreamWaitEvent(st, h->trk_done, 0));
+    if (h->azel)
+        track_kernel<2><<<1, 32, 0, st>>>(po.angles, o.elev, po.bins, std, (int)h->n, (int)W, h->trk, h->trk_fresh, h->trk_rows,
+                                          h->trk_state, h->trk_next, o.slot_track, o.track_ids, o.track_state);
+    else
+        track_kernel<1><<<1, 32, 0, st>>>(po.angles, nullptr, po.bins, std, (int)h->n, (int)W, h->trk, h->trk_fresh, h->trk_rows,
+                                          h->trk_state, h->trk_next, o.slot_track, o.track_ids, o.track_state);
+    h->launches++;
+    CU(h, cudaGetLastError());
+    CU(h, cudaEventRecord(h->trk_done, st));
+    h->trk_fresh = false;
+    h->trk_used = true;
+    return MUSIC_B200_OK;
 }
 
 // K2 of W windows from ws.R as planned: the eigensolver, the source count from `nsnap` snapshots (into ws.cnt and, when
@@ -1140,8 +1191,8 @@ void launch_grid_peaks(music_b200 *h, Peaks peaks, const double *p64, uint32_t W
 // (of these W windows), on `st`, as planned.  tev (optional) = timing events [1..4].  An az-el handle's peak bins are decoded into (azimuth, elevation)
 // after the peak rule.  With refinement on, the refine kernel follows (timed with the peak rule) and reads the bins
 // written before it: from the caller's array, or from the workspace when the caller asked for none.  A beams call
-// then forms the weights and beams of the windows at d_in, and a CRB call the bound of every slot (both timed with the
-// peak rule as well).
+// then forms the weights and beams of the windows at d_in, a CRB call the bound of every slot and a tracks call the
+// tracker's outputs (all timed with the peak rule as well).
 int launch_eig_scan(music_b200 *h, const Plan &p, const WsView &ws, uint32_t W, const Outputs &o, const DeviceTable &tb, uint32_t nsnap,
                     cudaStream_t st, cudaEvent_t *tev, const float *d_in = nullptr)
 {
@@ -1206,7 +1257,10 @@ int launch_eig_scan(music_b200 *h, const Plan &p, const WsView &ws, uint32_t W, 
         h->launches++;
     }
     if (p.beams) launch_beams(h, p, ws, W, o, po, d_in, st);
-    if (p.crb) launch_crb(h, p, ws, W, o, po, nsnap, st);
+    float *std = o.std ? o.std : ws.std;
+    if (p.crb) launch_crb(h, p, ws, W, o, po, nsnap, std, st);
+    if (p.track)
+        if (const int rc = launch_track(h, W, o, po, std, st)) return rc;
     if (tev) cudaEventRecord(tev[4], st);
     if (o.R)
         CU(h, cudaMemcpyAsync(o.R, ws.R, (size_t)W * M * M * 2 * sizeof(double), cudaMemcpyDeviceToDevice, st));
@@ -1273,7 +1327,9 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, const Ou
     if (h->azel && !out.elev) return fail(h, MUSIC_B200_EINVAL, "an az-el handle needs the elevation output");
     if (!planar && (reinterpret_cast<uintptr_t>(d_in) & 15u) != 0) return fail(h, MUSIC_B200_EINVAL, "d_in_c64 must be 16-byte aligned");
     if (const int rc = check_modes(h, h->modes, &table(h))) return rc;
-    if (out.std && !table(h).geometric)
+    if (out.slot_track && h->trk_var == MUSIC_B200_TRACK_OFF)
+        return fail(h, MUSIC_B200_EINVAL, "tracking is off (call music_b200_set_tracking() with FIXED or CRB variance)");
+    if ((out.std || (out.slot_track && h->trk_var == MUSIC_B200_TRACK_CRB)) && !table(h).geometric)
         return fail(h, MUSIC_B200_EINVAL, "the CRB needs a table built by music_b200_set_geometry%s(); the current one came from "
                                           "set_table(), which has no geometry", h->azel ? "_azel" : "");
     if (h->source_rule == MUSIC_B200_SOURCES_FIXED && out.counts) {
@@ -1541,18 +1597,21 @@ void host_register(music_b200 *h, const void *ptr, size_t bytes, bool read_only)
     h->hostregs.push_back(music_b200::HostReg{lo, (size_t)(hi - lo)});
 }
 
-int ensure_host_staging(music_b200 *h, uint32_t chunk, bool spec, bool beams, bool crb)
+int ensure_host_staging(music_b200 *h, uint32_t chunk, bool spec, bool beams, bool crb, uint32_t track_T)
 {
-    if (chunk <= h->host_chunk && (!spec || h->host_spec_alloc) && (!beams || h->host_beam_alloc) && (!crb || h->host_crb_alloc))
+    if (chunk <= h->host_chunk && (!spec || h->host_spec_alloc) && (!beams || h->host_beam_alloc) && (!crb || h->host_crb_alloc) &&
+        track_T <= h->host_track_T)
         return MUSIC_B200_OK;
     spec = spec || h->host_spec_alloc;
     beams = beams || h->host_beam_alloc;
     crb = crb || h->host_crb_alloc;
+    track_T = std::max(track_T, h->host_track_T);
     const uint32_t cap = std::max(chunk, h->host_chunk);
     // every old buffer is freed before the first new one is allocated
     for (HostSlot &sl : h->stage) sl = HostSlot();
     h->host_chunk = 0;
     h->host_spec_alloc = h->host_beam_alloc = h->host_crb_alloc = false;
+    h->host_track_T = 0;
     const size_t wn = (size_t)cap * h->n;
     const auto alloc = [&](auto &b) -> int {
         CU(h, b.angles.grow(wn));
@@ -1565,6 +1624,11 @@ int ensure_host_staging(music_b200 *h, uint32_t chunk, bool spec, bool beams, bo
         }
         if (h->azel) CU(h, b.elev.grow(wn));
         if (crb) CU(h, b.std.grow(h->azel ? 3 * wn : wn));
+        if (track_T) {
+            CU(h, b.slot_track.grow(wn));
+            CU(h, b.track_ids.grow((size_t)cap * track_T));
+            CU(h, b.track_state.grow((size_t)cap * track_T * (h->azel ? 6 : 3)));
+        }
         return MUSIC_B200_OK;
     };
     for (HostSlot &sl : h->stage) {
@@ -1579,6 +1643,7 @@ int ensure_host_staging(music_b200 *h, uint32_t chunk, bool spec, bool beams, bo
     h->host_spec_alloc = spec;
     h->host_beam_alloc = beams;
     h->host_crb_alloc = crb;
+    h->host_track_T = track_T;
     return MUSIC_B200_OK;
 }
 
@@ -1677,8 +1742,12 @@ int stage_host(music_b200 *h, const HostInput &in, uint32_t nwindows, const Outp
         music_b200 *c = lanes[l];
         if (cudaSetDevice(c->device) != cudaSuccess) { rc = fail(h, MUSIC_B200_ECUDA, "cudaSetDevice(%d) failed", c->device); break; }
         c->stage[0].W = c->stage[1].W = 0;  // nothing pending from an earlier (possibly failed) call
-        rc = ensure_host_staging(c, staged, dst.spec != nullptr, beams, dst.std != nullptr);
+        rc = ensure_host_staging(c, staged, dst.spec != nullptr, beams, dst.std != nullptr, dst.slot_track ? c->trk.T : 0);
         if (rc && c != h) fail(h, rc, "%s", std::string(c->error).c_str());
+        for (HostSlot &sl : c->stage) {  // the tracker's row count may have changed since the staging was allocated
+            sl.dev.shaped(c);
+            sl.pin.shaped(c);
+        }
     }
     const size_t cap = lanes[0]->host_chunk;
     const uint32_t chunk = in.streams ? std::max<uint32_t>(1, std::min((uint32_t)std::min<size_t>(cap, 1 + (cap * N - N) / in.hop), half)) : staged;
@@ -1723,6 +1792,8 @@ int stage_host(music_b200 *h, const HostInput &in, uint32_t nwindows, const Outp
                 if (!dst.wts) o.wts = nullptr;
                 if (!dst.beams) o.beams = nullptr;
                 if (!dst.std) o.std = nullptr;
+                if (!dst.slot_track) o.slot_track = nullptr;
+                if (!dst.track_ids) { o.track_ids = nullptr; o.track_state = nullptr; }
                 rc = enqueue_device(c, in.streams ? nullptr : sl.in.get(), W, o, st, s, in.streams ? &S : nullptr, in.hop);
                 if (rc && c != h) fail(h, rc, "%s", std::string(c->error).c_str());
                 if (rc) break;
@@ -1821,6 +1892,7 @@ int retune(music_b200 *h, F fill)
     if (const int rc = fill(h->tables[idle])) return rc;
     h->cur_table = idle;
     h->integ_fresh = true;  // the integrated covariances described the old manifold
+    h->trk_fresh = true;    // and the tracks its directions
     return MUSIC_B200_OK;
 }
 
@@ -2427,6 +2499,65 @@ int music_b200_process_host_crb(music_b200 *h, const float *in_c64, uint32_t nwi
     return process_host_impl(h, in_c64, nwindows, o);
 }
 
+/* ---- angle tracking (music_track.cuh) ---- */
+namespace {
+
+// the checks every tracks entry point makes before it runs: tracking on, slot_track asked for, track ids and states both
+// or neither, every tracker output aligned, and the CRB entry's checks on the rest when std is given (the CRB, weights
+// and beams may all be NULL)
+int check_track_call(music_b200 *h, const void *std, const void *weights, const void *beams, const int32_t *slot_track,
+                     const int32_t *track_ids, const float *track_state)
+{
+    if (h->trk_var == MUSIC_B200_TRACK_OFF)
+        return fail(h, MUSIC_B200_EINVAL, "tracking is off (call music_b200_set_tracking() with FIXED or CRB variance)");
+    if (!slot_track) return fail(h, MUSIC_B200_EINVAL, "slot_track must not be NULL");
+    if (!track_ids != !track_state) return fail(h, MUSIC_B200_EINVAL, "track_ids and track_state are given both or neither");
+    for (const void *q : {(const void *)slot_track, (const void *)track_ids, (const void *)track_state, std})
+        if ((reinterpret_cast<uintptr_t>(q) & 3u) != 0) return fail(h, MUSIC_B200_EINVAL, "the tracker outputs and the CRB must be 4-byte aligned");
+    if (weights || beams) return check_beams_call(h, weights, beams);
+    return MUSIC_B200_OK;
+}
+
+Outputs with_tracks(Outputs o, int32_t *slot_track, int32_t *track_ids, float *track_state)
+{
+    o.slot_track = slot_track;
+    o.track_ids = track_ids;
+    o.track_state = track_state;
+    return o;
+}
+
+}  // namespace
+
+int music_b200_process_device_tracks(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_angles, float *d_levels,
+                                     float *d_spectrum, int32_t *d_bins, int32_t *d_counts, double *d_weights, float *d_beams,
+                                     float *d_std, int32_t *d_slot_track, int32_t *d_track_ids, float *d_track_state, void *stream)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (h->azel) return fail(h, MUSIC_B200_EINVAL, "an az-el handle takes music_b200_process_azel_device_tracks()");
+    if (const int rc = check_track_call(h, d_std, d_weights, d_beams, d_slot_track, d_track_ids, d_track_state)) return rc;
+    Outputs o = caller_outputs(d_angles, d_levels, d_spectrum, d_bins);
+    o.counts = d_counts;
+    o.wts = d_weights;
+    o.beams = d_beams;
+    o.std = d_std;
+    return process_device_impl(h, d_in_c64, nwindows, with_tracks(o, d_slot_track, d_track_ids, d_track_state), stream);
+}
+
+int music_b200_process_host_tracks(music_b200 *h, const float *in_c64, uint32_t nwindows, float *angles, float *levels, float *spectrum,
+                                   int32_t *bins, int32_t *counts, double *weights, float *beams, float *std_out, int32_t *slot_track,
+                                   int32_t *track_ids, float *track_state)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (h->azel) return fail(h, MUSIC_B200_EINVAL, "an az-el handle takes music_b200_process_azel_host_tracks()");
+    if (const int rc = check_track_call(h, std_out, weights, beams, slot_track, track_ids, track_state)) return rc;
+    Outputs o = caller_outputs(angles, levels, spectrum, bins);
+    o.counts = counts;
+    o.wts = weights;
+    o.beams = beams;
+    o.std = std_out;
+    return process_host_impl(h, in_c64, nwindows, with_tracks(o, slot_track, track_ids, track_state));
+}
+
 /* ---- receiver calibration (music_calib.cuh) ---- */
 int music_b200_set_calibration(music_b200 *h, const double *gains)
 {
@@ -2508,6 +2639,104 @@ int music_b200_reset_integration(music_b200 *h)
     std::lock_guard<std::mutex> g(h->mutex);
     if (const int rc = check_integration(h)) return rc;
     h->integ_fresh = true;
+    return MUSIC_B200_OK;
+}
+
+}  // extern "C"
+
+/* ---- angle tracking (music_track.cuh) ---- */
+namespace {
+
+// the handles whose windows form one stream on one device, as for the integration: every other handle refuses tracking
+int check_tracking(music_b200 *h)
+{
+    if (!h->kids.empty())
+        return fail(h, MUSIC_B200_EINVAL, "tracking is not built for multi-device handles (their windows are dealt round-robin "
+                                          "over the devices)");
+    if (h->chan) return fail(h, MUSIC_B200_EINVAL, "per-channel tracking is not built: a channel handle takes no tracking");
+    if (h->gather_buf)
+        return fail(h, MUSIC_B200_EINVAL, "tracking is not built for a handle with a bins all-gather (its windows are one "
+                                          "rank's share of a stream)");
+    return MUSIC_B200_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int music_b200_set_tracking(music_b200 *h, int variance, double q, double rate_std0, double floor_deg, double crb_scale,
+                            double gate, uint32_t confirm_hits, uint32_t confirm_window, uint32_t max_misses, uint32_t max_tracks)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (variance != MUSIC_B200_TRACK_OFF && variance != MUSIC_B200_TRACK_FIXED && variance != MUSIC_B200_TRACK_CRB)
+        return fail(h, MUSIC_B200_EINVAL, "unknown measurement variance %d", variance);
+    const auto nonneg = [](double v) { return std::isfinite(v) && v >= 0.0; };
+    if (!nonneg(q) || !nonneg(rate_std0) || !nonneg(floor_deg))
+        return fail(h, MUSIC_B200_EINVAL, "q, rate_std0 and floor_deg must be finite and >= 0 (got %g, %g, %g)", q, rate_std0, floor_deg);
+    if (!std::isfinite(gate) || !(gate > 0.0)) return fail(h, MUSIC_B200_EINVAL, "the gate must be finite and > 0 (got %g)", gate);
+    if (variance == MUSIC_B200_TRACK_FIXED && !(floor_deg > 0.0))
+        return fail(h, MUSIC_B200_EINVAL, "FIXED variance needs floor_deg > 0");
+    if (variance == MUSIC_B200_TRACK_CRB && !(std::isfinite(crb_scale) && crb_scale > 0.0))
+        return fail(h, MUSIC_B200_EINVAL, "CRB variance needs a finite crb_scale > 0 (got %g)", crb_scale);
+    if (confirm_hits < 1 || confirm_hits > confirm_window || confirm_window > 64)
+        return fail(h, MUSIC_B200_EINVAL, "need 1 <= confirm_hits <= confirm_window <= 64 (got %u, %u)", confirm_hits, confirm_window);
+    if (max_misses < 1) return fail(h, MUSIC_B200_EINVAL, "max_misses must be >= 1");
+    if (max_tracks < 1 || max_tracks > MUSIC_B200_TRACK_MAX_ROWS)
+        return fail(h, MUSIC_B200_EINVAL, "max_tracks must be in 1..%d (got %u)", MUSIC_B200_TRACK_MAX_ROWS, max_tracks);
+    std::lock_guard<std::mutex> g(h->mutex);
+    if (const int rc = check_tracking(h)) return rc;
+    if (variance == MUSIC_B200_TRACK_CRB && !table(h).geometric)
+        return fail(h, MUSIC_B200_EINVAL, "CRB variance needs a table built by music_b200_set_geometry%s(); the current one came "
+                                          "from set_table(), which has no geometry", h->azel ? "_azel" : "");
+    if (variance != MUSIC_B200_TRACK_OFF && !h->trk_done) {
+        CU(h, cudaSetDevice(h->device));
+        CU(h, h->trk_rows.grow((size_t)MUSIC_B200_TRACK_MAX_ROWS * TRK_ROW_INTS));
+        CU(h, h->trk_state.grow((size_t)MUSIC_B200_TRACK_MAX_ROWS * track_state_len(2)));
+        CU(h, h->trk_next.grow(1));
+        CU(h, cudaEventCreateWithFlags(&h->trk_done, cudaEventDisableTiming));
+    }
+    TrackParams tp = {};
+    tp.crb = variance == MUSIC_B200_TRACK_CRB;
+    tp.q = q; tp.rate0 = rate_std0; tp.floor = floor_deg; tp.crb_scale = crb_scale; tp.gate = gate;
+    tp.confirm_hits = (int)confirm_hits; tp.confirm_window = (int)confirm_window; tp.max_misses = (int)max_misses;
+    tp.T = (int)max_tracks;
+    h->trk_var = variance;
+    h->trk = tp;
+    h->trk_fresh = true;
+    return MUSIC_B200_OK;
+}
+
+int music_b200_reset_tracks(music_b200 *h)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    std::lock_guard<std::mutex> g(h->mutex);
+    if (const int rc = check_tracking(h)) return rc;
+    h->trk_fresh = true;
+    return MUSIC_B200_OK;
+}
+
+int music_b200_get_tracks(music_b200 *h, int32_t *rows, double *state, uint32_t *next_id)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    std::lock_guard<std::mutex> g(h->mutex);
+    const size_t T = (size_t)h->trk.T, sl = (size_t)track_state_len(h->azel ? 2 : 1);
+    if (h->trk_fresh || !h->trk_used) {
+        // the carry a reset leaves: every row empty
+        for (size_t r = 0; r < T; ++r) {
+            if (rows) {
+                rows[r * TRK_ROW_INTS] = -1;
+                for (int k = 1; k < TRK_ROW_INTS; ++k) rows[r * TRK_ROW_INTS + k] = 0;
+            }
+            if (state) for (size_t k = 0; k < sl; ++k) state[r * sl + k] = 0.0;
+        }
+        if (next_id) *next_id = 0;
+        return MUSIC_B200_OK;
+    }
+    CU(h, cudaSetDevice(h->device));
+    CU(h, cudaEventSynchronize(h->trk_done));
+    if (rows) CU(h, cudaMemcpy(rows, h->trk_rows, T * TRK_ROW_INTS * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    if (state) CU(h, cudaMemcpy(state, h->trk_state, T * sl * sizeof(double), cudaMemcpyDeviceToHost));
+    if (next_id) CU(h, cudaMemcpy(next_id, h->trk_next, sizeof(uint32_t), cudaMemcpyDeviceToHost));
     return MUSIC_B200_OK;
 }
 
@@ -2763,6 +2992,8 @@ int music_b200_gather_create(music_b200 *h, uint32_t total_windows, unsigned cha
     CU(h, cudaSetDevice(h->device));
     if (h->gather_buf) return fail(h, MUSIC_B200_EINVAL, "gather buffer already created");
     if (h->integ_alpha > 0.0) return fail(h, MUSIC_B200_EINVAL, "the bins all-gather is not built for an integrating handle (set_integration(0) first)");
+    if (h->trk_var != MUSIC_B200_TRACK_OFF)
+        return fail(h, MUSIC_B200_EINVAL, "the bins all-gather is not built for a tracking handle (set_tracking(OFF) first)");
     static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
     const size_t elems = (size_t)total_windows * h->n;
     // the handle takes the buffers once both exist and are shared: a failure leaves it without a gather buffer
@@ -2994,6 +3225,31 @@ int music_b200_process_azel_host_crb(music_b200 *h, const float *in_c64, uint32_
         if (const int rc = check_crb_call(h, crb, nullptr, nullptr)) return rc;
     return process_azel_host_impl(h, "music_b200_process_azel_host_crb", in_c64, nwindows,
                                   azel_outputs(azimuth, elevation, levels, spectrum, bins, counts, crb));
+}
+
+int music_b200_process_azel_device_tracks(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_azimuth,
+                                          float *d_elevation, float *d_levels, float *d_spectrum, int32_t *d_bins, int32_t *d_counts,
+                                          float *d_crb, int32_t *d_slot_track, int32_t *d_track_ids, float *d_track_state, void *stream)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (h->azel)
+        if (const int rc = check_track_call(h, d_crb, nullptr, nullptr, d_slot_track, d_track_ids, d_track_state)) return rc;
+    return process_azel_device_impl(h, "music_b200_process_azel_device_tracks", d_in_c64, nwindows,
+                                    with_tracks(azel_outputs(d_azimuth, d_elevation, d_levels, d_spectrum, d_bins, d_counts, d_crb),
+                                                d_slot_track, d_track_ids, d_track_state),
+                                    stream);
+}
+
+int music_b200_process_azel_host_tracks(music_b200 *h, const float *in_c64, uint32_t nwindows, float *azimuth, float *elevation,
+                                        float *levels, float *spectrum, int32_t *bins, int32_t *counts, float *crb, int32_t *slot_track,
+                                        int32_t *track_ids, float *track_state)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (h->azel)
+        if (const int rc = check_track_call(h, crb, nullptr, nullptr, slot_track, track_ids, track_state)) return rc;
+    return process_azel_host_impl(h, "music_b200_process_azel_host_tracks", in_c64, nwindows,
+                                  with_tracks(azel_outputs(azimuth, elevation, levels, spectrum, bins, counts, crb), slot_track,
+                                              track_ids, track_state));
 }
 
 /* ---- frequency-channelised direction finding (music_channels.cuh) ---- */

@@ -250,6 +250,79 @@ class music_doa(object):
                                                       d_counts, d_weights, d_beams, d_std, stream)
         _capi.check(rc, self._h)
 
+    # -- extension: angle tracking across windows ---------------------------------------------------------
+    TRACK_VARIANCES = {"off": 0, "fixed": 1, "crb": 2}
+
+    def set_tracking(self, variance="off", q=0.01, rate_std0=1.0, floor_deg=0.5, crb_scale=1.0, gate=9.0, confirm_hits=3,
+                     confirm_window=5, max_misses=5, max_tracks=8):
+        """Track every source across windows and calls on the device: one constant-velocity Kalman filter per track
+        (angles in degrees, time in windows: ``q`` is the white-acceleration density in deg^2 / window^3), global
+        nearest-neighbour assignment inside the chi-square ``gate``, confirmation after ``confirm_hits`` hits within
+        ``confirm_window`` windows, deletion after ``max_misses`` consecutive misses, at most ``max_tracks`` (<= 32)
+        tracks (include/music_b200.h).  ``variance``: "fixed" (measurement std ``floor_deg``), "crb" (``crb_scale`` times
+        the slot's Cramer-Rao bound plus ``floor_deg``, which needs a table installed with ``set_array_geometry``) or
+        "off" (default).  While it is on, ``work()`` also returns ``last_tracks()``.  Resets the tracks; so do
+        ``reset_tracks``, ``set_array_response`` and ``set_array_geometry``.  Use the "local_maxima" or a gridless peak
+        mode: "top_bins" with n >= 2 puts two slots, and so two tracks, on one source."""
+        if variance not in self.TRACK_VARIANCES:
+            raise ValueError("variance must be one of %s" % sorted(self.TRACK_VARIANCES))
+        _capi.check(self._lib.music_b200_set_tracking(self._h, self.TRACK_VARIANCES[variance], float(q), float(rate_std0),
+                                                      float(floor_deg), float(crb_scale), float(gate), int(confirm_hits),
+                                                      int(confirm_window), int(max_misses), int(max_tracks)), self._h)
+        self._tracking = (variance, int(max_tracks))
+
+    def tracking(self):
+        """the variance in use ("off", "fixed" or "crb")"""
+        return getattr(self, "_tracking", ("off", 0))[0]
+
+    def reset_tracks(self):
+        """Drop every track: the next window starts from no tracks and ids restart at 0."""
+        _capi.check(self._lib.music_b200_reset_tracks(self._h), self._h)
+
+    def tracks(self):
+        """The tracker's carry after the last tracking call: (rows int32 (T, 5) = id, status (0 empty, 1 tentative, 2
+        confirmed), age, hits, consecutive misses; state float64 (T, 2D + (2D)^2) = x then P row-major, D = 1 (2 on a
+        ``music_doa_azel`` block); next_id)."""
+        T = getattr(self, "_tracking", ("off", 0))[1]
+        D = 2 if self._azel() else 1
+        rows = np.zeros((T, 5), np.int32)
+        state = np.zeros((T, 2 * D + 4 * D * D), np.float64)
+        nxt = ctypes.c_uint32(0)
+        ptr = lambda a: a.ctypes.data if T else None  # no rows asked for before set_tracking()
+        _capi.check(self._lib.music_b200_get_tracks(self._h, ptr(rows), ptr(state), ctypes.byref(nxt)), self._h)
+        return rows, state, int(nxt.value)
+
+    def last_tracks(self):
+        """(slot_track int32 (W, n): the track each slot's measurement updated or started, -1 for none; track_ids int32
+        (W, T): the confirmed track of every row, -1 for none; track_state float32 (W, T, 3): angle, rate (degrees per
+        window) and std of the angle of those rows, (W, T, 6) on a ``music_doa_azel`` block: az, rate, el, rate, std az,
+        std el) of the last work() call; None while tracking is off."""
+        return getattr(self, "_last_tracks", None)
+
+    def _azel(self):
+        return False
+
+    def _track_buffers(self, W):
+        """the tracker's outputs of a work() call of W windows (None while tracking is off)"""
+        self._last_tracks = None
+        if self.tracking() == "off":
+            return None
+        T = self._tracking[1]
+        self._last_tracks = (np.empty((W, self.n), np.int32), np.empty((W, T), np.int32),
+                             np.empty((W, T, 6 if self._azel() else 3), np.float32))
+        return [a.ctypes.data for a in self._last_tracks]
+
+    def process_device_tracks(self, d_in, nwindows, d_angles, d_slot_track, d_levels=None, d_spectrum=None, d_bins=None,
+                              d_counts=None, d_weights=None, d_beams=None, d_std=None, d_track_ids=None, d_track_state=None,
+                              stream=None):
+        """Raw device-pointer entry (ints): the outputs of ``process_device_crb`` (``d_std`` may be None) plus
+        ``d_slot_track`` (int32 [nwindows][n], required), ``d_track_ids`` (int32 [nwindows][T]) and ``d_track_state``
+        (float32 [nwindows][T][3]), the last two both or neither."""
+        rc = self._lib.music_b200_process_device_tracks(self._h, d_in, int(nwindows), d_angles, d_levels, d_spectrum, d_bins,
+                                                         d_counts, d_weights, d_beams, d_std, d_slot_track, d_track_ids,
+                                                         d_track_state, stream)
+        _capi.check(rc, self._h)
+
     # -- extension: receiver calibration -----------------------------------------------------------------
     CALIBRATIONS = {"phase": 1, "gain_phase": 2}
 
@@ -366,7 +439,17 @@ class music_doa(object):
             self._last_beams = np.empty((W, self.n, N), np.complex64)
         wts_p = self._last_weights.ctypes.data if beams else None
         beams_p = self._last_beams.ctypes.data if beams else None
-        if self.crb():
+        trk = self._track_buffers(W)
+        if trk is not None:
+            # one call for the tracks, the bound and the beams: two would advance the integration and track carries twice
+            self._last_counts = np.empty(W, np.int32)
+            if self.crb():
+                self._last_crb = np.empty((W, self.n), np.float32)
+            crb_p = self._last_crb.ctypes.data if self.crb() else None
+            rc = self._lib.music_b200_process_host_tracks(self._h, x.ctypes.data, W, ang.ctypes.data, lvl_p, spec_p,
+                                                          self._last_bins.ctypes.data, self._last_counts.ctypes.data, wts_p, beams_p,
+                                                          crb_p, *trk)
+        elif self.crb():
             # one call for the bound and the beams: two would advance the integration carry twice
             self._last_counts = np.empty(W, np.int32)
             self._last_crb = np.empty((W, self.n), np.float32)

@@ -54,6 +54,9 @@ class music_doa_azel(music_doa):
     def name(self):
         return "music_doa_azel"
 
+    def _azel(self):
+        return True
+
     def output_signature(self):
         """(min, max, [item sizes]): azimuth, elevation, level (n floats each), spectrum (n_el * n_az floats)"""
         return (2, 4, [self.n * 4, self.n * 4, self.n * 4, self.resolution * 4])
@@ -94,8 +97,14 @@ class music_doa_azel(music_doa):
         self._last_bins = np.empty((W, self.n), np.int32)
         self._last_counts = np.empty(W, np.int32)
         self._last_crb = None
+        trk = self._track_buffers(W)
         if self.crb():
             self._last_crb = np.empty((W, self.n, 3), np.float32)
+        if trk is not None:
+            rc = self._lib.music_b200_process_azel_host_tracks(self._h, x.ctypes.data, W, ptr(0), ptr(1), ptr(2), ptr(3),
+                                                               self._last_bins.ctypes.data, self._last_counts.ctypes.data,
+                                                               self._last_crb.ctypes.data if self.crb() else None, *trk)
+        elif self.crb():
             rc = self._lib.music_b200_process_azel_host_crb(self._h, x.ctypes.data, W, ptr(0), ptr(1), ptr(2), ptr(3),
                                                             self._last_bins.ctypes.data, self._last_counts.ctypes.data,
                                                             self._last_crb.ctypes.data)
@@ -118,4 +127,14 @@ class music_doa_azel(music_doa):
         [nwindows][n][3], required)."""
         rc = self._lib.music_b200_process_azel_device_crb(self._h, d_in, int(nwindows), d_azimuth, d_elevation, d_levels,
                                                           d_spectrum, d_bins, d_counts, d_crb, stream)
+        _capi.check(rc, self._h)
+
+    def process_device_tracks(self, d_in, nwindows, d_azimuth, d_elevation, d_slot_track, d_levels=None, d_spectrum=None,
+                              d_bins=None, d_counts=None, d_crb=None, d_track_ids=None, d_track_state=None, stream=None):
+        """Raw device-pointer entry (ints): the outputs of ``process_device_crb`` (``d_crb`` may be None) plus
+        ``d_slot_track`` (int32 [nwindows][n], required), ``d_track_ids`` (int32 [nwindows][T]) and ``d_track_state``
+        (float32 [nwindows][T][6]), the last two both or neither."""
+        rc = self._lib.music_b200_process_azel_device_tracks(self._h, d_in, int(nwindows), d_azimuth, d_elevation, d_levels,
+                                                             d_spectrum, d_bins, d_counts, d_crb, d_slot_track, d_track_ids,
+                                                             d_track_state, stream)
         _capi.check(rc, self._h)

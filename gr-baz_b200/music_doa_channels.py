@@ -116,6 +116,12 @@ class music_doa_channels(music_doa):
         if enable:
             raise ValueError("the CRB is not built for channel handles")
 
+    def set_tracking(self, variance="off", **kwargs):
+        """Per-channel tracking is not built (include/music_b200.h): music_b200_set_tracking refuses a channel handle,
+        so this raises whatever the variance."""
+        rc = self._lib.music_b200_set_tracking(self._h, self.TRACK_VARIANCES.get(variance, -1), 0.01, 1.0, 0.5, 1.0, 9.0, 3, 5, 5, 8)
+        _capi.check(rc, self._h)
+
     def process_host(self, x, nwindows, levels=True, spectrum=False, bins=True, counts=False, R=False):
         """The host entry on complex64 windows x, results in the C ABI's channel-major layout: a dict of angles / levels /
         bins (rows, W, n), counts (rows, W), spectrum (rows, W, resolution), R (count, W, m, m) complex128, under

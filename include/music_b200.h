@@ -572,6 +572,112 @@ int music_b200_process_azel_host_crb(music_b200 *h, const float *in_c64, uint32_
                                      float *levels, float *spectrum, int32_t *bins, int32_t *counts, float *crb);
 
 /*
+ * Angle tracking (extension, no reference counterpart): the per-window directions become tracks, each with an identity,
+ * an angle, a rate and an uncertainty, carried across windows and calls on the device.  Slot i of window w and slot i
+ * of window w + 1 need not be the same emitter (slots are filled in order of strength); a track id is.  One
+ * constant-velocity Kalman filter per track (Bar-Shalom, Li & Kirubarajan 2001), global-nearest-neighbour assignment
+ * of each window's measurements to the tracks inside a chi-square gate, M-of-N confirmation and deletion after
+ * consecutive misses (Blackman & Popoli 1999).  Time is counted in windows, so rates are in degrees per window; the
+ * windows are numbered in stream order since the last reset, within a call and on into the next call, as for the
+ * integration.  Everything is fp64 in the order written; float outputs are single casts.
+ *   setting    variance MUSIC_B200_TRACK_OFF (default), _FIXED: the measurement covariance R_i = floor_deg^2 I (needs
+ *              floor_deg > 0), or _CRB: R_i = crb_scale^2 C_crb + floor_deg^2 I (needs crb_scale > 0), where C_crb is the
+ *              slot's CRB (process_*_crb) in degrees^2: sigma^2 in 1-D, [[sa^2, rho sa se], [rho sa se, se^2]] in az-el
+ *              (evaluated as c2 = crb_scale crb_scale, f2 = floor_deg floor_deg, 1-D R = c2 (s s) + f2; az-el R_00 =
+ *              c2 (sa sa) + f2, R_01 = R_10 = c2 ((rho sa) se), R_11 = c2 (se se) + f2; FIXED: R = f2 I).  EINVAL, with the
+ *              old setting kept, unless q >= 0, rate_std0 >= 0, floor_deg >= 0 and gate > 0 are all finite,
+ *              1 <= confirm_hits <= confirm_window <= 64, max_misses >= 1 and 1 <= max_tracks <= 32.
+ *   carry      T = max_tracks rows and a counter next_id (0 after a reset).  A row is empty or a track: id, status
+ *              (TENTATIVE or CONFIRMED), state x, covariance P, age, hits and misses (consecutive).  1-D x = (theta,
+ *              omega); az-el x = (az, omega_az, el, omega_el), two independent axes with the same model.  H picks the
+ *              angle components (theta; az and el).
+ *   window w, in this order:
+ *              1. predict every live row, per axis: F = [[1, 1], [0, 1]], Q = q [[1/3, 1/2], [1/2, 1]] (the white-noise
+ *                 acceleration model with a step of 1; Q = (q / 3, q / 2, q / 2, q)), x <- F x, P <- F P F^T + Q (for each
+ *                 2 x 2 block [[a, b], [c, d]] of P: [[(a + c) + (b + d), b + d], [c + d, d]], then + Q on the diagonal
+ *                 blocks).  theta (az) is wrapped into [0, 360) by v - 360 floor(v / 360).  age += 1 (age, hits and
+ *                 misses saturate at 2^31 - 1).
+ *              2. measurements: the slots i in ascending order with bins[w][i] >= 0 (under CRB also with every CRB entry
+ *                 of the slot finite: a failed CRB window contributes none), z_i = (double)angles[w][i] (az-el: the
+ *                 (azimuth, elevation) pair), R_i as above.
+ *              3. for every live row t and measurement i: nu = z_i - H x_t with the angle (azimuth) component wrapped into
+ *                 [-180, 180) by v - 360 floor((v + 180) / 360); S = H P H^T + R_i; 1-D d2 = (nu nu) / S; az-el with det
+ *                 = S00 S11 - S01 S01, d2 = ((S11 nu0) nu0 - ((2 S01) nu0) nu1 + (S00 nu1) nu1) / det.  The pair is gated
+ *                 in iff d2 <= gate (a NaN d2 never is).
+ *              4. global nearest neighbour: a matching of gated pairs, each row and each measurement used at most once,
+ *                 that minimises sum (d2 - gate) over the matched pairs (the linear assignment on the (rows +
+ *                 measurements)-square matrix of the gated d2 augmented with dummy costs gate / 2).  On exact ties any
+ *                 minimiser may be taken, the same on every run.
+ *              5. update every matched row: 1-D K = P H^T / S; az-el K_j0 = (P_j0 S11 - P_j2 S01) / det, K_j1 = (P_j2 S00 -
+ *                 P_j0 S01) / det; x <- x + K nu, wrapped; P <- (I - K H) P (I - K H)^T + K R K^T (Joseph form), the lower
+ *                 triangle mirrored from the upper; hits += 1, misses = 0.  Every unmatched live row: misses += 1.
+ *              6. status: a TENTATIVE row is confirmed once hits >= confirm_hits, else deleted once it can no longer get
+ *                 there, hits + (confirm_window - age) < confirm_hits; a CONFIRMED row is deleted once misses >=
+ *                 max_misses.
+ *              7. initiation: each unmatched measurement, in ascending slot order, takes the lowest empty row if there is
+ *                 one: id = next_id++ (mod 2^31), TENTATIVE (CONFIRMED at once when confirm_hits = 1), x = (z, 0) per
+ *                 axis, P with R_i in its angle block and rate_std0^2 on each rate diagonal, age = hits = 1, misses = 0.
+ *              8. outputs: slot_track[w][i] = the id of the track slot i's measurement updated or started (tentative or
+ *                 confirmed), -1 otherwise (no measurement, or no free row).  track_ids[w][r] = the id of row r if it holds
+ *                 a CONFIRMED track after step 7, else -1.  track_state[w][r] for those rows, 0 for the others: 1-D
+ *                 {theta, omega, sqrt(P_00)}, az-el {az, omega_az, el, omega_el, sqrt(P_00), sqrt(P_22)}.
+ *   entries    the _tracks entries take the outputs of the CRB entries (d_std / d_crb may be NULL: under CRB variance the
+ *              bound then goes to a workspace) plus d_slot_track [W][n] (required), and d_track_ids [W][T] with
+ *              d_track_state [W][T][3] (az-el [W][T][6]), both or neither; every output 4-byte aligned.  One call
+ *              returns everything a window produces, because two calls would advance the integration and the track
+ *              carry twice.  Every other output is byte-identical to the matching CRB call (process_device_beams with
+ *              weights or beams, process_device_ex with d_R otherwise) on the same windows.  Only the _tracks entries
+ *              read the setting: every other entry ignores it and leaves the carry untouched, so windows sent through
+ *              other entries are a gap in the tracker's time.  Per sub-batch a tracks call adds one track_kernel launch
+ *              (one CTA) after the peak stage, the beams and the CRB, timed in the top-n slot of the stage timing.
+ *              get_tracks() waits for the last tracking call and returns the carry: rows [T][5] = {id, status, age, hits,
+ *              misses} (an empty row is {-1, MUSIC_B200_TRACK_EMPTY, 0, 0, 0}), state [T][2D + (2D)^2] = x then P
+ *              row-major (zeros for an empty row; D = 1, or 2 on an az-el handle), and next_id; any of the three may be
+ *              NULL.
+ *   resets     reset_tracks(), every set_tracking() (the same parameters included) and every table setter (set_table,
+ *              set_geometry, set_geometry_azel).  Not reset by the peak mode, estimator, source rule, refinement,
+ *              beamformer, integration or calibration setters.  A call with nwindows = 0, or refused before it enqueues
+ *              anything, leaves the carry untouched.  Call k + 1 tracks after call k whatever streams they use; the host
+ *              entries' chunks and the sub-batches of a call track in window order.
+ *   EINVAL     with no fall-back: a _tracks call while the variance is OFF; CRB variance with a current table from
+ *              set_table() (FIXED takes any table); set_tracking() / reset_tracks() on multi-device handles, handles with a
+ *              bins all-gather (gather_create() is refused while tracking is on) and channel handles; a 1-D entry on an
+ *              az-el handle or the reverse; NULL d_slot_track; only one of d_track_ids / d_track_state; a misaligned
+ *              output; weights or beams without a beamformer.
+ *   caveats    TOP_BINS with n >= 2 reports neighbouring bins of one peak, which gives two tracks per source: use
+ *              LOCAL_MAXIMA or a gridless mode.  The two mirror slots of a line array under the grid modes become two
+ *              tracks.  Under integration consecutive measurements are correlated, so the filter's sigma is optimistic.
+ *              The CRB is a lower bound: crb_scale and floor_deg absorb the estimator's excess variance and the grid's
+ *              quantisation (without refinement a grid angle carries about (360 / K) / sqrt(12) degrees).
+ */
+#define MUSIC_B200_TRACK_OFF 0
+#define MUSIC_B200_TRACK_FIXED 1
+#define MUSIC_B200_TRACK_CRB 2
+#define MUSIC_B200_TRACK_EMPTY 0      /* get_tracks() row status */
+#define MUSIC_B200_TRACK_TENTATIVE 1
+#define MUSIC_B200_TRACK_CONFIRMED 2
+#define MUSIC_B200_TRACK_MAX_ROWS 32
+int music_b200_set_tracking(music_b200 *h, int variance, double q, double rate_std0, double floor_deg, double crb_scale,
+                            double gate, uint32_t confirm_hits, uint32_t confirm_window, uint32_t max_misses,
+                            uint32_t max_tracks);
+int music_b200_reset_tracks(music_b200 *h);
+int music_b200_get_tracks(music_b200 *h, int32_t *rows, double *state, uint32_t *next_id);
+int music_b200_process_device_tracks(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_angles,
+                                     float *d_levels, float *d_spectrum, int32_t *d_bins, int32_t *d_counts,
+                                     double *d_weights, float *d_beams, float *d_std, int32_t *d_slot_track,
+                                     int32_t *d_track_ids, float *d_track_state, void *stream);
+int music_b200_process_host_tracks(music_b200 *h, const float *in_c64, uint32_t nwindows, float *angles, float *levels,
+                                   float *spectrum, int32_t *bins, int32_t *counts, double *weights, float *beams,
+                                   float *std_out, int32_t *slot_track, int32_t *track_ids, float *track_state);
+int music_b200_process_azel_device_tracks(music_b200 *h, const float *d_in_c64, uint32_t nwindows, float *d_azimuth,
+                                          float *d_elevation, float *d_levels, float *d_spectrum, int32_t *d_bins,
+                                          int32_t *d_counts, float *d_crb, int32_t *d_slot_track, int32_t *d_track_ids,
+                                          float *d_track_state, void *stream);
+int music_b200_process_azel_host_tracks(music_b200 *h, const float *in_c64, uint32_t nwindows, float *azimuth,
+                                        float *elevation, float *levels, float *spectrum, int32_t *bins, int32_t *counts,
+                                        float *crb, int32_t *slot_track, int32_t *track_ids, float *track_state);
+
+/*
  * Downstream reducers (extension, no reference counterpart): what a GUI-rate consumer such as the DOA
  * compass (/root/reference/python/doa_compass_control.py:102-108) or a plot sink
  * (/root/reference/python/plot_sink.py:38) needs from millions of windows per second.

@@ -72,8 +72,8 @@ baz_music_doa::baz_music_doa(unsigned int m, unsigned int n, unsigned int nsampl
                              const array_response_t &array_response, unsigned int resolution)
     : gr::sync_block("music_doa", gr::io_signature::make(1, 1, nsamples * sizeof(gr_complex)),
                      gr::io_signature::make3(1, 3, n * sizeof(float), n * sizeof(float), resolution * sizeof(float))),
-      d_m(m), d_n(n), d_nsamples(nsamples), d_resolution(resolution), d_handle(NULL), d_source_rule(MUSIC_B200_SOURCES_FIXED),
-      d_beam_rule(MUSIC_B200_BEAMS_OFF), d_crb(false), d_cal_remaining(0), d_cal_angle(0.0), d_cal_kind(MUSIC_B200_CALIB_GAIN_PHASE),
+      d_m(m), d_n(n), d_nsamples(nsamples), d_resolution(resolution), d_handle(NULL), d_track_rows(0),
+      d_source_rule(MUSIC_B200_SOURCES_FIXED), d_beam_rule(MUSIC_B200_BEAMS_OFF), d_crb(false), d_cal_remaining(0), d_cal_angle(0.0), d_cal_kind(MUSIC_B200_CALIB_GAIN_PHASE),
       d_cal_residual(std::numeric_limits<double>::quiet_NaN())
 {
     if (array_response.size() != resolution) throw std::invalid_argument("music_doa: array_response.size() != resolution");
@@ -205,6 +205,23 @@ void baz_music_doa::set_crb(bool enable)
     d_crb = enable;
 }
 
+/* Extension (not in the reference): angle tracking across work() calls, see include/music_b200.h. */
+void baz_music_doa::set_tracking(int variance, double q, double rate_std0, double floor_deg, double crb_scale, double gate,
+                                 unsigned int confirm_hits, unsigned int confirm_window, unsigned int max_misses, unsigned int max_tracks)
+{
+    gr::thread::scoped_lock guard(d_mutex);
+    const int rc = music_b200_set_tracking(d_handle, variance, q, rate_std0, floor_deg, crb_scale, gate, confirm_hits, confirm_window,
+                                           max_misses, max_tracks);
+    if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa: ") + music_b200_last_error(d_handle));
+    d_track_rows = variance == MUSIC_B200_TRACK_OFF ? 0 : max_tracks;
+}
+
+void baz_music_doa::reset_tracks()
+{
+    const int rc = music_b200_reset_tracks(d_handle);
+    if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa: ") + music_b200_last_error(d_handle));
+}
+
 void baz_music_doa::set_calibration(const std::vector<std::complex<double> > &gains)
 {
     if (!gains.empty() && gains.size() != d_m) throw std::invalid_argument("music_doa: gains.size() != m");
@@ -253,8 +270,23 @@ int baz_music_doa::work(int noutput_items, gr_vector_const_void_star &input_item
     d_bins.resize((size_t)noutput_items * d_n);
     d_beams.clear();
     d_crb_out.clear();
+    d_slot_track.clear();
+    d_track_ids.clear();
+    d_track_state.clear();
     int rc;
-    if (d_crb) {
+    if (d_track_rows) {
+        /* one call for the tracks, the bound and the beams: two would advance the integration and track carries twice */
+        d_counts.resize((size_t)noutput_items);
+        if (d_crb) d_crb_out.resize((size_t)noutput_items * d_n);
+        if (d_beam_rule != MUSIC_B200_BEAMS_OFF) d_beams.resize((size_t)noutput_items * d_n * (d_nsamples / d_m));
+        d_slot_track.resize((size_t)noutput_items * d_n);
+        d_track_ids.resize((size_t)noutput_items * d_track_rows);
+        d_track_state.resize((size_t)noutput_items * d_track_rows * 3);
+        rc = music_b200_process_host_tracks(d_handle, in, (uint32_t)noutput_items, out, lvl, out_spectrum, d_bins.data(), d_counts.data(),
+                                            NULL, d_beams.empty() ? NULL : reinterpret_cast<float *>(d_beams.data()),
+                                            d_crb_out.empty() ? NULL : d_crb_out.data(), d_slot_track.data(), d_track_ids.data(),
+                                            d_track_state.data());
+    } else if (d_crb) {
         /* one call for the bound and the beams: two would advance the integration carry twice */
         d_counts.resize((size_t)noutput_items);
         d_crb_out.resize((size_t)noutput_items * d_n);

@@ -91,6 +91,16 @@ public:
      * reported angle, in degrees (include/music_b200.h), read back with last_crb(); with the beamformer on, the bound and
      * the beams come from the same single call.  Needs a table from set_array_geometry(). */
     void set_crb(bool enable);
+    /* extension: angle tracking across work() calls (include/music_b200.h).  variance MUSIC_B200_TRACK_OFF (default),
+     * _FIXED or _CRB; the other arguments as music_b200_set_tracking().  While it is on, every work() call also returns
+     * last_slot_track() [items][n] (the track id each slot's measurement updated or started, -1 for none),
+     * last_track_ids() [items][max_tracks] (the confirmed track of every row, -1 for none) and last_track_state()
+     * [items][max_tracks][3] (angle, rate in degrees per item, std of the angle), all from the same single call as the
+     * bound and the beams.  set_tracking() and reset_tracks() drop every track; so do set_array_response() and
+     * set_array_geometry(). */
+    void set_tracking(int variance, double q, double rate_std0, double floor_deg, double crb_scale, double gate,
+                      unsigned int confirm_hits, unsigned int confirm_window, unsigned int max_misses, unsigned int max_tracks);
+    void reset_tracks();
 
     /* Integer peak-bin indices of the items produced by the last work() call, [items][n]
      * (not in the reference; -1 marks a slot the reference would leave at (0, 0)). */
@@ -104,6 +114,9 @@ public:
     /* The bound of the items produced by the last work() call while set_crb() is on, [items][n] degrees (0 for unfilled
      * slots, NaN where the item's bound does not exist); empty while it is off. */
     const std::vector<float> &last_crb() const { return d_crb_out; }
+    const std::vector<int> &last_slot_track() const { return d_slot_track; }
+    const std::vector<int> &last_track_ids() const { return d_track_ids; }
+    const std::vector<float> &last_track_state() const { return d_track_state; }
 
 private:
     std::vector<float> flatten(const array_response_t &array_response) const;
@@ -117,6 +130,9 @@ private:
     std::vector<int> d_counts;
     std::vector<gr_complex> d_beams;
     std::vector<float> d_crb_out;
+    std::vector<int> d_slot_track, d_track_ids;
+    std::vector<float> d_track_state;
+    unsigned int d_track_rows; /* max_tracks while tracking is on, 0 while it is off */
     int d_source_rule;
     int d_beam_rule;
     bool d_crb;

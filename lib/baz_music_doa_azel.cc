@@ -170,6 +170,23 @@ void baz_music_doa_azel::set_crb(bool enable)
     d_crb = enable;
 }
 
+void baz_music_doa_azel::set_tracking(int variance, double q, double rate_std0, double floor_deg, double crb_scale, double gate,
+                                      unsigned int confirm_hits, unsigned int confirm_window, unsigned int max_misses,
+                                      unsigned int max_tracks)
+{
+    gr::thread::scoped_lock guard(d_mutex);
+    const int rc = music_b200_set_tracking(d_handle, variance, q, rate_std0, floor_deg, crb_scale, gate, confirm_hits, confirm_window,
+                                           max_misses, max_tracks);
+    if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa_azel: ") + music_b200_last_error(d_handle));
+    d_track_rows = variance == MUSIC_B200_TRACK_OFF ? 0 : max_tracks;
+}
+
+void baz_music_doa_azel::reset_tracks()
+{
+    const int rc = music_b200_reset_tracks(d_handle);
+    if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa_azel: ") + music_b200_last_error(d_handle));
+}
+
 int baz_music_doa_azel::work(int noutput_items, gr_vector_const_void_star &input_items, gr_vector_void_star &output_items)
 {
     if (noutput_items <= 0) return 0;
@@ -184,9 +201,19 @@ int baz_music_doa_azel::work(int noutput_items, gr_vector_const_void_star &input
     d_bins.resize((size_t)noutput_items * d_n);
     d_counts.resize((size_t)noutput_items);
     d_crb_out.assign(d_crb ? (size_t)noutput_items * d_n * 3 : 0, 0.0f);
-    const int rc = d_crb ? music_b200_process_azel_host_crb(d_handle, in, (uint32_t)noutput_items, az, el, lvl, spectrum, d_bins.data(),
-                                                            d_counts.data(), d_crb_out.data())
-                         : music_b200_process_azel_host(d_handle, in, (uint32_t)noutput_items, az, el, lvl, spectrum, d_bins.data(), d_counts.data());
+    d_slot_track.assign(d_track_rows ? (size_t)noutput_items * d_n : 0, 0);
+    d_track_ids.assign((size_t)noutput_items * d_track_rows, 0);
+    d_track_state.assign((size_t)noutput_items * d_track_rows * 6, 0.0f);
+    int rc;
+    if (d_track_rows)  /* one call for the tracks and the bound: two would advance the carries twice */
+        rc = music_b200_process_azel_host_tracks(d_handle, in, (uint32_t)noutput_items, az, el, lvl, spectrum, d_bins.data(), d_counts.data(),
+                                                 d_crb ? d_crb_out.data() : NULL, d_slot_track.data(), d_track_ids.data(),
+                                                 d_track_state.data());
+    else if (d_crb)
+        rc = music_b200_process_azel_host_crb(d_handle, in, (uint32_t)noutput_items, az, el, lvl, spectrum, d_bins.data(), d_counts.data(),
+                                              d_crb_out.data());
+    else
+        rc = music_b200_process_azel_host(d_handle, in, (uint32_t)noutput_items, az, el, lvl, spectrum, d_bins.data(), d_counts.data());
     if (rc != MUSIC_B200_OK) throw std::runtime_error(std::string("music_doa_azel: ") + music_b200_last_error(d_handle));
     calibration_step(d_handle, in, noutput_items, d_cal_remaining, d_cal_az, d_cal_el, d_cal_kind, d_cal_residual);
     return noutput_items;

@@ -68,6 +68,14 @@ public:
      * [items][n][3] = std of the azimuth, std of the elevation (degrees), their correlation */
     void set_crb(bool enable);
     const std::vector<float> &last_crb() const { return d_crb_out; }
+    /* angle tracking across work() calls, as for baz_music_doa: last_track_state() holds [items][max_tracks][6] = az,
+     * its rate, el, its rate (degrees per item), std of the azimuth, std of the elevation */
+    void set_tracking(int variance, double q, double rate_std0, double floor_deg, double crb_scale, double gate,
+                      unsigned int confirm_hits, unsigned int confirm_window, unsigned int max_misses, unsigned int max_tracks);
+    void reset_tracks();
+    const std::vector<int> &last_slot_track() const { return d_slot_track; }
+    const std::vector<int> &last_track_ids() const { return d_track_ids; }
+    const std::vector<float> &last_track_state() const { return d_track_state; }
 
     /* flat peak bins b = i * n_az + k of the items produced by the last work() call, [items][n] (-1: unfilled slot) */
     const std::vector<int> &last_bins() const { return d_bins; }
@@ -84,6 +92,9 @@ private:
     std::vector<int> d_counts;
     std::vector<float> d_crb_out;
     bool d_crb = false;
+    std::vector<int> d_slot_track, d_track_ids;
+    std::vector<float> d_track_state;
+    unsigned int d_track_rows = 0; /* max_tracks while tracking is on, 0 while it is off */
     int d_cal_remaining;
     double d_cal_az, d_cal_el;
     int d_cal_kind;

@@ -2,7 +2,7 @@
 """Small invocations of the kernels compute-sanitizer should look at (SURVEY.md section 5): run as
   compute-sanitizer --tool racecheck|memcheck|synccheck python tools/sanitize_targets.py <target>
 targets: fused (C1-size windows, 2000 of them + a ragged 1187 + a drain-only 9), fused_jacobi, fused8, covn8, covn16, eig16, esprit2d,
-gridless_roots, crb, multi,
+gridless_roots, crb, tracks, multi,
 lifecycle (every handle kind created, retuned, grown and destroyed through the host entry points; run it under
   compute-sanitizer --tool memcheck --leak-check full, which reports what a handle leaves allocated)"""
 import os
@@ -118,6 +118,34 @@ elif target == "crb":
     az.set_crb(True)
     az.work(W, [x], [np.zeros((W, n), np.float32) for _ in range(3)])
     print(target, "ok az-el", az.last_crb()[:1, :2].tolist())
+    az.close()
+elif target == "tracks":
+    # the tracker (music_track.cuh): 32 rows and 15 slots in 1-D (CRB variance, every slot filled by DML) and az-el, a wide
+    # gate so that ambiguous clusters reach the assignment solve, a zero window and a NaN window (a failed CRB) among
+    # them, and a ragged window count over several input chunks
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+    from gr_baz_b200.music_doa_azel import music_doa_azel
+    from helpers import LAM
+
+    W, m, n = 101, 16, 15
+    rng = np.random.default_rng(32)
+    x = ((rng.standard_normal((W, 64 * m)) + 1j * rng.standard_normal((W, 64 * m)))).astype(np.complex64)
+    x[3] = 0
+    x[5, 11] = np.nan
+    k = np.arange(m)
+    pos = np.stack([0.5 * LAM * np.cos(2 * np.pi * k / m) * m / 6, 0.5 * LAM * np.sin(2 * np.pi * k / m) * m / 6], 1)
+    blk = music_doa(m, n, 64 * m, np.ones((360, m), np.complex64), 360)
+    blk.set_array_geometry(pos, LAM)
+    blk.set_peak_mode("dml", 0)
+    blk.set_tracking("crb", q=1.0, floor_deg=2.0, gate=1e4, confirm_hits=2, confirm_window=3, max_misses=2, max_tracks=32)
+    blk.work(W, [x], [np.zeros((W, n), np.float32)])
+    print(target, "ok 1-D", blk.last_tracks()[0][:2].tolist())
+    blk.close()
+    az = music_doa_azel(m, n, 64 * m, 36, 9, (0.0, 80.0), rng.uniform(-0.6, 0.6, (m, 3)) * LAM, LAM)
+    az.set_peak_mode("local_maxima", 0)
+    az.set_tracking("crb", q=1.0, floor_deg=2.0, gate=1e4, confirm_hits=1, confirm_window=1, max_misses=2, max_tracks=32)
+    az.work(W, [x], [np.zeros((W, n), np.float32) for _ in range(3)])
+    print(target, "ok az-el", az.last_tracks()[1][:1].tolist())
     az.close()
 elif target == "multi":
     cfg = synth.config(1)
