@@ -37,6 +37,7 @@
 #include "music_esprit.cuh"
 #include "music_esprit2d.cuh"
 #include "music_dml.cuh"
+#include "music_wsf.cuh"
 #include "music_beams.cuh"
 #include "music_calib.cuh"
 #include "music_integrate.cuh"
@@ -130,7 +131,7 @@ struct TableSlot {
 };
 
 // A non-owning view of a workspace slot's buffers, or of one channel's run of them (enqueue_channels)
-struct WsView { double *R, *ev, *Vt, *P64; int32_t *cnt, *bins; double *wts; unsigned long long *n0; float *std; };
+struct WsView { double *R, *ev, *Vt, *P64; int32_t *cnt, *bins; double *wts; unsigned long long *n0; float *std; double *X; };
 
 struct Workspace {
     DevBuf<double> R, ev, Vt, P64;
@@ -139,9 +140,10 @@ struct Workspace {
     DevBuf<double> wts;    // [windows][n][m] complex beam weights when a beams call asked for none
     DevBuf<unsigned long long> n0;  // integration: the count since the reset at the sub-batch's first window
     DevBuf<float> std;     // [windows][sw] the CRB a tracks call under CRB variance reads when the caller asked for none
+    DevBuf<double> X;      // [windows][m][m] complex: the WSF matrix the DML search reads (music_wsf.cuh)
     cudaEvent_t scan_done = nullptr;
     bool used = false;
-    WsView view() const { return {R, ev, Vt, P64, cnt, bins, wts, n0, std}; }
+    WsView view() const { return {R, ev, Vt, P64, cnt, bins, wts, n0, std, X}; }
 };
 
 // The modes set by set_peak_mode(), set_refine() and set_estimator(); check_modes() says which combine.
@@ -519,11 +521,12 @@ uint32_t snapshots(const music_b200 *h)
 // hold one (single-device handles, and the children of a multi-device handle).
 int check_modes(music_b200 *h, const Modes &p, const DeviceTable *t)
 {
-    if (p.peak != MUSIC_B200_PEAKS_TOP_BINS && p.peak != MUSIC_B200_PEAKS_LOCAL_MAXIMA && !gridless_mode(p.peak) &&
-        p.peak != MUSIC_B200_PEAKS_DML)
+    const bool subspace_fit = p.peak == MUSIC_B200_PEAKS_DML || p.peak == MUSIC_B200_PEAKS_WSF;
+    if (p.peak != MUSIC_B200_PEAKS_TOP_BINS && p.peak != MUSIC_B200_PEAKS_LOCAL_MAXIMA && !gridless_mode(p.peak) && !subspace_fit)
         return fail(h, MUSIC_B200_EINVAL, "unknown peak mode %d", p.peak);
     if (p.excl >= h->K) return fail(h, MUSIC_B200_EINVAL, "exclusion_bins must be < resolution");
-    if (p.refine != MUSIC_B200_REFINE_OFF && p.refine != MUSIC_B200_REFINE_NEWTON) return fail(h, MUSIC_B200_EINVAL, "unknown refine mode %d", p.refine);
+    if (p.refine != MUSIC_B200_REFINE_OFF && p.refine != MUSIC_B200_REFINE_NEWTON && p.refine != MUSIC_B200_REFINE_JOINT)
+        return fail(h, MUSIC_B200_EINVAL, "unknown refine mode %d", p.refine);
     if (p.est != MUSIC_B200_ESTIMATOR_MUSIC && p.est != MUSIC_B200_ESTIMATOR_MVDR && p.est != MUSIC_B200_ESTIMATOR_BARTLETT)
         return fail(h, MUSIC_B200_EINVAL, "unknown estimator %d", p.est);
     if (!std::isfinite(p.loading) || p.loading < 0.0) return fail(h, MUSIC_B200_EINVAL, "loading must be finite and >= 0 (got %g)", p.loading);
@@ -536,7 +539,7 @@ int check_modes(music_b200 *h, const Modes &p, const DeviceTable *t)
         // per channel only the grid modes are built (include/music_b200.h lists the rest as not built)
         if (p.peak != MUSIC_B200_PEAKS_TOP_BINS && p.peak != MUSIC_B200_PEAKS_LOCAL_MAXIMA)
             return fail(h, MUSIC_B200_EINVAL, "a channel handle takes the TOP_BINS and LOCAL_MAXIMA peak modes only (ROOTS, ESPRIT, "
-                                              "MANIFOLD and DML per channel are not built)");
+                                              "MANIFOLD, DML and WSF per channel are not built)");
         if (p.refine != MUSIC_B200_REFINE_OFF) return fail(h, MUSIC_B200_EINVAL, "peak refinement is not built for channel handles");
         if (h->chan_combine == MUSIC_B200_CHANNELS_INCOHERENT && p.est != MUSIC_B200_ESTIMATOR_MUSIC)
             return fail(h, MUSIC_B200_EINVAL, "the INCOHERENT combine is defined for the MUSIC estimator only");
@@ -567,13 +570,19 @@ int check_modes(music_b200 *h, const Modes &p, const DeviceTable *t)
             return fail(h, MUSIC_B200_EINVAL, "the %s peak mode needs a table built by music_b200_set_geometry() from a uniform linear "
                                               "array with spacing <= lambda / 2 (call set_geometry(), or another peak mode)", name);
     }
-    if (p.peak == MUSIC_B200_PEAKS_DML) {
-        // any 1-D table: DML reads table rows only
-        if (p.excl != 0) return fail(h, MUSIC_B200_EINVAL, "the DML peak mode takes exclusion_bins = 0");
-        if (h->azel) return fail(h, MUSIC_B200_EINVAL, "the DML peak mode is not supported on an az-el handle");
-        if (p.est != MUSIC_B200_ESTIMATOR_MUSIC) return fail(h, MUSIC_B200_EINVAL, "the DML peak mode needs the MUSIC estimator");
-        if (p.refine != MUSIC_B200_REFINE_OFF)
-            return fail(h, MUSIC_B200_EINVAL, "the DML peak mode needs refinement off (NEWTON refines the MUSIC objective)");
+    if (subspace_fit) {
+        // any 1-D table: DML and WSF read table rows only
+        const char *name = p.peak == MUSIC_B200_PEAKS_DML ? "DML" : "WSF";
+        if (p.excl != 0) return fail(h, MUSIC_B200_EINVAL, "the %s peak mode takes exclusion_bins = 0", name);
+        if (h->azel) return fail(h, MUSIC_B200_EINVAL, "the %s peak mode is not supported on an az-el handle", name);
+        if (p.est != MUSIC_B200_ESTIMATOR_MUSIC) return fail(h, MUSIC_B200_EINVAL, "the %s peak mode needs the MUSIC estimator", name);
+        if (p.refine == MUSIC_B200_REFINE_NEWTON)
+            return fail(h, MUSIC_B200_EINVAL, "the %s peak mode takes refinement OFF or JOINT (NEWTON refines the MUSIC objective)", name);
+    }
+    if (p.refine == MUSIC_B200_REFINE_JOINT) {
+        if (!subspace_fit)
+            return fail(h, MUSIC_B200_EINVAL, "JOINT refinement needs the DML or WSF peak mode (NEWTON refines the grid modes)");
+        if (h->chan) return fail(h, MUSIC_B200_EINVAL, "JOINT refinement is not built for channel handles");
     }
     if (t && p.refine != MUSIC_B200_REFINE_OFF && !t->geometric)
         return fail(h, MUSIC_B200_EINVAL, "peak refinement needs a table built by music_b200_set_geometry(); the current one came from "
@@ -745,6 +754,7 @@ struct Plan {
     int est = MUSIC_B200_ESTIMATOR_MUSIC;            // the form of scan_kernel and the refined objective
     Peaks peaks = Peaks::None;
     bool decode = false, refine = false;             // az-el bin decode; peak refinement (the az-el kind after a decode)
+    bool wsf = false, joint = false;                 // the WSF matrix after the eigensolver; JOINT refinement after the peaks
     bool beams = false;                              // beam weights (+ beams) after the peaks: the beams entry points
     bool crb = false;                                // the CRB of every slot after the peaks (and beams): the crb entries
     bool track = false;                              // then the tracker (music_track.cuh): the tracks entries
@@ -761,7 +771,8 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
     const bool music_est = md.est == MUSIC_B200_ESTIMATOR_MUSIC;
     const bool local = md.peak == MUSIC_B200_PEAKS_LOCAL_MAXIMA;
     const bool gridless = gridless_mode(md.peak);
-    const bool dml = md.peak == MUSIC_B200_PEAKS_DML;
+    const bool wsf = md.peak == MUSIC_B200_PEAKS_WSF;
+    const bool dml = md.peak == MUSIC_B200_PEAKS_DML || wsf;  // WSF runs the DML search on its matrix X
     Plan p;
     // The fused kernels find the principal eigenvector only, not every eigenvalue a source count needs nor the noise
     // eigenvectors the peak refinement needs; they compute the MUSIC spectrum only.  Planar streams can take the M = 4
@@ -778,8 +789,8 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
     else if (fusable && h->m == 8 && !planar && !o.spec && h->N >= 128 && h->N % 2 == 0) p.path = Path::Fused8;
 
     // MVDR and Bartlett need the eigensolver only to count sources or when the caller asked for the eigenvalues; DML
-    // (which reads R only) also for the MUSIC spectrum or P64
-    p.eig = (music_est && (!dml || o.spec || o.P64)) || !fixed_n || o.ev;
+    // (which reads R only) also for the MUSIC spectrum or P64; WSF always (X is built from the eigenvectors)
+    p.eig = (music_est && (!dml || o.spec || o.P64)) || !fixed_n || o.ev || wsf;
     p.count = !fixed_n;
     p.mvdr = md.est == MUSIC_B200_ESTIMATOR_MVDR;
     p.est = md.est;
@@ -800,7 +811,9 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
     else if (dml) p.peaks = Peaks::Dml;
     else if (!p.argmax) p.peaks = local && h->azel ? Peaks::Local2D : local ? Peaks::Local : Peaks::TopN;
     p.decode = h->azel && p.peaks != Peaks::Esprit2D;  // the 2-D ESPRIT kernel writes both angles itself
-    p.refine = md.refine != MUSIC_B200_REFINE_OFF;
+    p.refine = md.refine == MUSIC_B200_REFINE_NEWTON;
+    p.joint = md.refine == MUSIC_B200_REFINE_JOINT;
+    p.wsf = wsf;
     p.ws_p64 = p.p64 && !o.P64;
     p.ws_counts = p.count;
     p.beams = beams;
@@ -808,7 +821,7 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
     p.crb = o.std != nullptr || (track && h->trk_var == MUSIC_B200_TRACK_CRB);
     p.calib = h->calib;
     p.integ = h->integ_alpha > 0.0;
-    p.ws_bins = p.decode || p.refine || ((beams || p.crb || track) && !o.bins);
+    p.ws_bins = p.decode || p.refine || p.joint || ((beams || p.crb || track) && !o.bins);
     p.ws_wts = beams && !o.wts;
     p.ws_std = p.crb && !o.std;
     if (h->chan && h->chan_combine == MUSIC_B200_CHANNELS_INCOHERENT) {
@@ -830,7 +843,8 @@ uint32_t max_sub_windows(const music_b200 *h, const Plan &p)
     const size_t per_win = (size_t)h->m * h->m * 2 * 8 * 2 + h->m * 8 + (p.ws_p64 ? (size_t)h->K * 8 : 0) +
                            (p.ws_counts ? sizeof(int32_t) : 0) + (p.ws_bins ? h->n * sizeof(int32_t) : 0) +
                            (p.ws_wts ? (size_t)h->n * h->m * 2 * sizeof(double) : 0) +
-                           (p.ws_std ? (size_t)(h->azel ? 3 : 1) * h->n * sizeof(float) : 0);
+                           (p.ws_std ? (size_t)(h->azel ? 3 : 1) * h->n * sizeof(float) : 0) +
+                           (p.wsf ? (size_t)h->m * h->m * 2 * sizeof(double) : 0);
     // A SEPARATE / INCOHERENT channel handle's workspace holds C pseudo-windows per window; a COHERENT one holds the
     // windows, and the channel buffer beside it the C covariances of each.
     const size_t C = h->chan ? (size_t)h->cshape.C : 1;
@@ -859,6 +873,7 @@ int ensure_slot(music_b200 *h, Workspace &ws, uint32_t windows, const Plan &p)
     if (const int rc = grow(ws.bins, p.ws_bins ? w * h->n : 0)) return rc;
     if (const int rc = grow(ws.n0, p.integ ? 1 : 0)) return rc;
     if (const int rc = grow(ws.std, p.ws_std ? w * (h->azel ? 3 : 1) * h->n : 0)) return rc;
+    if (const int rc = grow(ws.X, p.wsf ? w * mm : 0)) return rc;
     return grow(ws.wts, p.ws_wts ? w * h->n * h->m * 2 : 0);
 }
 
@@ -1172,6 +1187,13 @@ const int32_t *launch_eig_stage(music_b200 *h, const Plan &p, const WsView &ws, 
         h->launches++;
         cnt = ws.cnt;
     }
+    // WSF: the weighted signal-subspace matrix X into ws.X (timed with the eigensolver)
+    if (p.wsf) {
+        const size_t e = (size_t)W * M * M;
+        wsf_x_kernel<<<(unsigned)((e + WSF_X_THREADS - 1) / WSF_X_THREADS), WSF_X_THREADS, 0, st>>>(ws.ev, ws.Vt, cnt, M, (int)h->n,
+                                                                                                  (int)W, ws.X);
+        h->launches++;
+    }
     // MVDR: the rows of L^-1 of R + delta I into ws.Vt (timed with the eigensolver)
     if (p.mvdr) {
         mvdr_prep_kernel<<<(W + PREP_WARPS - 1) / PREP_WARPS, PREP_WARPS * 32, 0, st>>>(ws.R, ws.Vt, M, (int)W, h->modes.loading);
@@ -1225,7 +1247,7 @@ int launch_eig_scan(music_b200 *h, const Plan &p, const WsView &ws, uint32_t W, 
         // M = 16 runs the runtime-M instantiation (its loops have the same 16-entry bound): the fixed-M one spills
         with_scan_m(h->m, [&](auto mt) {
             constexpr int MT = decltype(mt)::value == 16 ? 0 : decltype(mt)::value;
-            dml_kernel<MT><<<W, DML_THREADS, 0, st>>>(ws.R, tb.soa, cnt, M, (int)h->n, (int)h->K, po);
+            dml_kernel<MT><<<W, DML_THREADS, 0, st>>>(p.wsf ? ws.X : ws.R, ws.R, tb.soa, cnt, M, (int)h->n, (int)h->K, po);
         });
         break;
     case Peaks::Local2D: topn_local2d_kernel<<<W, AZEL_LM_THREADS, 0, st>>>(p64, (int)h->n, h->grid.n_az, h->grid.n_el, excl, po, cnt); break;
@@ -1254,6 +1276,12 @@ int launch_eig_scan(music_b200 *h, const Plan &p, const WsView &ws, uint32_t W, 
         else if (p.est == MUSIC_B200_ESTIMATOR_BARTLETT) { REFINE_CASE(EST_BARTLETT) }
         else { REFINE_CASE(EST_MUSIC) }
 #undef REFINE_CASE
+        h->launches++;
+    }
+    if (p.joint) {
+        const int n = (int)h->n;
+        joint_kernel<<<W, 32, (size_t)joint_smem_elems(M, n) * sizeof(double2), st>>>(ws.R, p.wsf ? ws.ev : nullptr, ws.Vt, cnt, po.bins,
+                                                                                      M, n, (int)h->K, tb.geo, po.angles, po.levels);
         h->launches++;
     }
     if (p.beams) launch_beams(h, p, ws, W, o, po, d_in, st);

@@ -67,10 +67,12 @@ __device__ __forceinline__ void dml_mgs2(const double *soa, const int *bins, int
     }, r, M, Q, T, lane);
 }
 
-// R: per window M * M complex doubles (row-major); soa: the table tiles [ceil(K / TILE)][2M + 1][TILE]; counts (may be
-// null): the per-window source count d (else d = n).
+// R: per window M * M complex doubles (row-major), the matrix searched; Rl: the matrix the levels are taken from, in the
+// same layout (under DML both are the window's covariance; under WSF R is the weighted signal-subspace matrix of
+// music_wsf.cuh and Rl the covariance); soa: the table tiles [ceil(K / TILE)][2M + 1][TILE]; counts (may be null): the per-window source
+// count d (else d = n).
 template <int MT>
-__global__ void __launch_bounds__(DML_THREADS) dml_kernel(const double *__restrict__ R, const double *__restrict__ soa,
+__global__ void __launch_bounds__(DML_THREADS) dml_kernel(const double *__restrict__ R, const double *__restrict__ Rl, const double *__restrict__ soa,
                                                           const int32_t *__restrict__ counts, int Mrt, int n, int K, PeakOut out)
 {
     constexpr int MA = MT ? MT : MAXM;
@@ -78,7 +80,7 @@ __global__ void __launch_bounds__(DML_THREADS) dml_kernel(const double *__restri
     __shared__ double2 sR[MAXM * MAXM];   // R (row-major, stride M)
     __shared__ double2 sP[MAXM * MAXM];   // P = I - Q_B Q_B^H (stride M); U = T^-1 for the levels (stride MAXM)
     __shared__ double2 sX[MAXM * MAXM];   // P R (stride M); the levels' C = Q_A^H R Q_A - s2 I (stride MAXM)
-    __shared__ double2 sY[MAXM * MAXM];   // R' = P R P (stride M)
+    __shared__ double2 sY[MAXM * MAXM];   // R' = P R P (stride M); the levels' matrix Rl when it is not R
     __shared__ double2 sQ[MAXM * MAXM];   // Q_B or Q_A, vector l at l * MAXM
     __shared__ double2 sT[MAXM * MAXM];   // T of A = Q_A T (stride MAXM)
     __shared__ int slot[MAXM], sB[MAXM];
@@ -209,8 +211,17 @@ __global__ void __launch_bounds__(DML_THREADS) dml_kernel(const double *__restri
         if (!changed) break;
     }
 
-    // levels: A = Q_A T, s2 = (tr R - tr(Q_A^H R Q_A)) / (M - d), p = diag(T^-1 (Q_A^H R Q_A - s2 I) T^-H)
+    // levels: A = Q_A T, s2 = (tr Rl - tr(Q_A^H Rl Q_A)) / (M - d), p = diag(T^-1 (Q_A^H Rl Q_A - s2 I) T^-H)
     if (ok && wid == 0) {
+        const double2 *sL = sR;
+        if (Rl != R) {
+            const double2 *Lw = reinterpret_cast<const double2 *>(Rl) + w * MM;
+            for (int e = lane; e < MM; e += 32) sY[e] = Lw[e];
+            __syncwarp();
+            sL = sY;
+            trR = 0.0;
+            for (int i = 0; i < M; ++i) trR += sL[i * M + i].x;
+        }
         dml_mgs2(soa, slot, d, M, sQ, sT, lane);
         // C[a][b] = q_a^H R q_b: lane a < d, then the trace terms
         for (int e = lane; e < d * d; e += 32) {
@@ -219,7 +230,7 @@ __global__ void __launch_bounds__(DML_THREADS) dml_kernel(const double *__restri
             for (int i = 0; i < M; ++i) {
                 double2 y = make_double2(0.0, 0.0);  // (R q_b)_i
                 for (int j = 0; j < M; ++j) {
-                    const double2 t = cmul(sR[i * M + j], sQ[b * MAXM + j]);
+                    const double2 t = cmul(sL[i * M + j], sQ[b * MAXM + j]);
                     y.x += t.x;
                     y.y += t.y;
                 }

@@ -113,13 +113,16 @@ class music_doa(object):
         it needs n <= min((Mx - 1) My, Mx (My - 1)) besides the restrictions of ``"roots"``;
         ``"dml"`` = deterministic maximum likelihood by alternating projection: the n table rows whose span captures the
         most power of the covariance, so coherent sources (multipath) are resolved, on any table; levels are
-        least-squares source powers.  It needs ``exclusion_bins`` = 0, the "music" estimator and refinement off; use the
+        least-squares source powers.  It needs ``exclusion_bins`` = 0, the "music" estimator and refinement off or "joint"; use the
         "fixed" source rule for coherent sources;
+        ``"wsf"`` = weighted subspace fitting: DML's search on the eigenvalue-weighted signal subspace, whose
+        large-sample variance is the stochastic CRB; coherent sources need no smoothing.  It has the restrictions of
+        ``"dml"`` and also takes ``set_refine("joint")``;
         ``"manifold"`` = root-MUSIC on any planar array by manifold separation: gridless angles over the whole 360
         degrees from the roots of one polynomial per window, for a geometry installed with ``set_array_geometry``
         spanning about 4.4 wavelengths or less.  It has the restrictions of ``"roots"``; on a line array every source
         also has a mirror root, so use ``"roots"`` or ``"esprit"`` there."""
-        modes = {"top_bins": 0, "local_maxima": 1, "roots": 2, "esprit": 3, "dml": 4, "manifold": 5}
+        modes = {"top_bins": 0, "local_maxima": 1, "roots": 2, "esprit": 3, "dml": 4, "manifold": 5, "wsf": 6}
         if mode not in modes:
             raise ValueError("mode must be one of %s" % sorted(modes))
         _capi.check(self._lib.music_b200_set_peak_mode(self._h, modes[mode], int(exclusion_bins)), self._h)
@@ -145,16 +148,27 @@ class music_doa(object):
         return self._last_counts
 
     # -- extension: off-grid peak refinement -------------------------------------------------------
+    REFINE_MODES = {"off": 0, "newton": 1, "joint": 2}
+
     def set_refine(self, enable):
-        """True: every reported peak is refined off the grid by safeguarded Newton steps on the exact fp64 MUSIC
-        spectrum of the array geometry (include/music_b200.h); angles and levels change, bins and the spectrum stay the
-        grid results.  Needs a table installed with ``set_array_geometry``; False (default) reports grid angles."""
-        _capi.check(self._lib.music_b200_set_refine(self._h, 1 if enable else 0), self._h)
-        self._refine = bool(enable)
+        """True or ``"newton"``: every reported peak is refined off the grid by safeguarded Newton steps on the exact
+        fp64 MUSIC spectrum of the array geometry (include/music_b200.h); angles and levels change, bins and the spectrum
+        stay the grid results.  ``"joint"`` (the "dml" and "wsf" peak modes only): all slots of a window are refined
+        together by Gauss-Newton steps on the peak mode's own criterion.  Both need a table installed with
+        ``set_array_geometry``; False or ``"off"`` (default) reports grid angles."""
+        if isinstance(enable, str):
+            if enable not in self.REFINE_MODES:
+                raise ValueError("refine must be True, False or one of %s" % sorted(self.REFINE_MODES))
+            mode = self.REFINE_MODES[enable]
+        else:
+            mode = 1 if enable else 0
+        _capi.check(self._lib.music_b200_set_refine(self._h, mode), self._h)
+        self._refine = mode
 
     @property
     def refine(self):
-        return getattr(self, "_refine", False)
+        """The refine mode as its C code: 0 = off, 1 = Newton, 2 = joint (false only when off)."""
+        return getattr(self, "_refine", 0)
 
     # -- extension: the spectrum estimator -----------------------------------------------------------
     ESTIMATORS = {"music": 0, "mvdr": 1, "bartlett": 2}

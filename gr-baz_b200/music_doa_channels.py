@@ -12,12 +12,12 @@ window, ``count * n`` angles, ``count * n`` levels and optionally ``count * reso
 channel.  ``combine="incoherent"``: one incoherent wideband MUSIC spectrum per window; items as for :class:`music_doa`.
 ``combine="coherent"``: every channel's covariance is focused onto the centre channel's frequency and summed, and each
 window is one ordinary problem on that sum and the centre channel's table; items as for :class:`music_doa`, and the
-root-MUSIC, ESPRIT, DML and refinement setters work.  ``set_focusing`` chooses the sector of grid bins the focusing
+root-MUSIC, ESPRIT, DML, WSF and NEWTON refinement setters work (JOINT refinement raises).  ``set_focusing`` chooses the sector of grid bins the focusing
 matrices fit, ``focusing`` returns them and their errors.
 ``antenna_array`` holds m [x, y] positions in units of ``spacing`` metres.  Peak mode, estimator and source rule setters,
 the reducers, ``last_bins`` / ``last_counts`` and ``close`` are those of :class:`music_doa`; the modes that are not
-built for channels (beams, calibration, planar input, and under "separate" / "incoherent" root-MUSIC, ESPRIT, DML and
-refinement) raise.
+built for channels (beams, calibration, planar input, and under "separate" / "incoherent" root-MUSIC, ESPRIT, DML, WSF
+and refinement) raise.
 """
 from __future__ import annotations
 

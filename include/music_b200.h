@@ -199,10 +199,28 @@ int music_b200_set_table(music_b200 *h, const float *table_c64);
  *              under TOP_BINS, level = (float)p, bin through the peak-bin all-gather of sharded calls.  Slots d .. n-1
  *              report (0, 0, bin -1).  Spectrum, P64, R, eigenvalues and counts are unchanged.
  * Coherent sources lower the rank MDL / AIC count: use FIXED for them.  DML needs exclusion_bins = 0, estimator MUSIC
- * and refinement OFF (NEWTON refines the MUSIC objective), checked in either order, and no az-el handle; any table from
+ * and refinement OFF or JOINT (NEWTON refines the MUSIC objective), checked in either order, and no az-el handle; any table from
  * set_table() or set_geometry() is accepted.  It runs the unfused kernels: covariance, the eigensolver only for MDL /
  * AIC, the eigenvalues, the spectrum or P64, the MUSIC scan only for the spectrum or P64, then one DML kernel per
  * sub-batch (one CTA per window for all its searches), timed in the top-n slot of the stage timing.
+ *
+ * MUSIC_B200_PEAKS_WSF (extension, weighted subspace fitting, also called MODE; Viberg, Ottersten & Kailath 1991): DML's
+ * search on a weighted signal-subspace matrix X in place of R.  Its large-sample variance is the stochastic CRB of the
+ * _crb entries, on any 1-D geometry, and coherent sources need no smoothing.
+ *   inputs     l_0 <= .. <= l_{M-1} and e_0 .. e_{M-1}: the eigenvalues and eigenvectors of the window's R (the R output,
+ *              after calibration and integration); d = n, or the MDL / AIC count.
+ *   matrix     s2 = (l_0 + .. + l_{M-d-1}) / (M - d); for i = M-d .. M-1, w_i = (l_i - s2)^2 / l_i if l_i > s2, else 0;
+ *              X = sum_i w_i e_i e_i^H (M x M, fp64).  X does not depend on eigenvector phase or on a rotation inside a
+ *              degenerate eigenspace.  d = 0, l_0 <= 0, a non-finite eigenvalue, or every w_i = 0 (tr X = 0) gives a
+ *              window with no peaks.  Under FIXED n with coherent sources the surplus signal eigenvalue is close to s2, so
+ *              its weight is close to 0.
+ *   search     DML's (init, up to 20 Gauss-Seidel sweeps, candidate and tie rules) word for word, with X for R.
+ *   levels     DML's least-squares powers, taken from R (not X) at the chosen rows.
+ *   outputs    as DML: slot order, angles, bins, the peak-bin all-gather and unfilled slots.
+ * WSF has DML's restrictions, checked the same way in either order: exclusion_bins = 0, estimator MUSIC, refinement
+ * OFF or JOINT, no az-el handle and no SEPARATE / INCOHERENT channel handle; any 1-D table from set_table() or
+ * set_geometry().  It runs the unfused kernels: covariance, the eigensolver (always) and the count, one kernel per
+ * sub-batch that forms X (timed in the eigensolver slot of the stage timing), [scan], then the DML kernel on X.
  *
  * MUSIC_B200_PEAKS_MANIFOLD (extension, root-MUSIC by manifold separation): gridless angles over the whole 360 degrees
  * on any planar array, from the roots of one polynomial per window (Belloni, Richter & Koivunen 2007; Rubsamen &
@@ -252,6 +270,7 @@ int music_b200_set_table(music_b200 *h, const float *table_c64);
 #define MUSIC_B200_PEAKS_ESPRIT 3
 #define MUSIC_B200_PEAKS_DML 4
 #define MUSIC_B200_PEAKS_MANIFOLD 5
+#define MUSIC_B200_PEAKS_WSF 6
 int music_b200_set_peak_mode(music_b200 *h, int mode, uint32_t exclusion_bins);
 
 /*
@@ -310,8 +329,38 @@ int music_b200_set_source_rule(music_b200 *h, int rule);
  * set_refine()) fails with EINVAL; there is no silent fall-back to grid angles.
  * Applies to later process_*() calls and to every device of a multi-device handle.
  */
+/*
+ * MUSIC_B200_REFINE_JOINT (extension): a joint Gauss-Newton refinement of all d filled slots of a DML or WSF window on
+ * the analytic steering a(t), a'(t) = -j psi a(t) of NEWTON above.
+ *   factor     X = F F^H: under WSF the columns sqrt(w_i) e_i with w_i > 0 in ascending i; under DML F = L of the
+ *              Cholesky factorisation R = L L^H (X = R).  A DML window whose R is not positive definite (a pivot <= 0)
+ *              keeps what the peak stage wrote, and so does a WSF window without X.
+ *   criterion  t = the slot angles in radians (filled slots in slot order), A(t) = [a(t_i)], D = [a'(t_i)],
+ *              A+ = (A^H A)^-1 A^H, P_perp = I - A A+, V(t) = Re tr(P_perp X) = ||P_perp F||_F^2 (evaluated in this form,
+ *              which stays accurate where V is small).  A^H A counts as positive definite when every pivot l of its
+ *              factorisation exceeds 2^-30 ||a_l||^2.
+ *   step       g_i = -2 Re(A+ X P_perp D)_ii, H = 2 Re((D^H P_perp D) o (A+ X A+^H)^T) (the structure of the CRB's
+ *              Fisher matrix), s = -H^-1 g.  H counts as positive definite when every pivot k of its Cholesky
+ *              factorisation is > 0 and > 2^-40 H_kk.
+ *   iteration  start at t_b,i = (b_i * 360 / K) degrees in radians, box |t_i - t_b,i| <= (360 / K) degrees.  A window
+ *              whose A^H A at the start is not positive definite keeps what the peak stage wrote.  Each step: stop if H
+ *              is not positive definite or max |s_i| <= 1e-12; else try t + s projected onto the box, accepted iff
+ *              A^H A is positive definite there and V strictly decreases, else halve s (up to 30 times); stop when no
+ *              try is accepted, or after 50 steps.
+ *   outputs    angles[w][i] = (float) of t*_i in degrees wrapped into [0, 360), 360 -> 0 as under NEWTON (a slot whose
+ *              t*_i = t_b,i keeps its grid angle); levels = (float) of DML's least-squares powers from R at the analytic
+ *              A(t*).  Bins, spectrum, P64, R, eigenvalues and counts keep their grid values, as under NEWTON, and so
+ *              does the slot order.
+ * JOINT is accepted only with DML or WSF (JOINT under any other peak mode, and any peak mode other than DML and WSF under
+ * JOINT, returns EINVAL; NEWTON under DML and WSF stays EINVAL), on 1-D single- and multi-device handles (channel and
+ * az-el handles return EINVAL), on a table from set_geometry(): a process_*() call on a set_table() table returns EINVAL,
+ * with no fall-back.  One warp per window runs after the peak stage and before beams, CRB and tracking, timed in the
+ * top-n slot of the stage timing; the beams, the CRB and the tracker read the refined angles.
+ * Not built: az-el WSF and JOINT, JOINT for the grid modes (NEWTON serves them), stochastic ML proper, a fused path.
+ */
 #define MUSIC_B200_REFINE_OFF 0
 #define MUSIC_B200_REFINE_NEWTON 1
+#define MUSIC_B200_REFINE_JOINT 2
 int music_b200_set_refine(music_b200 *h, int mode);
 
 /*

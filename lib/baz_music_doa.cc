@@ -157,10 +157,13 @@ void baz_music_doa::set_source_rule(int rule)
 
 /* Extension (not in the reference): off-grid peak refinement on the exact spectrum of the array geometry, see
    include/music_b200.h.  Needs a table installed with set_array_geometry(). */
-void baz_music_doa::set_refine(bool enable)
+void baz_music_doa::set_refine(bool enable) { set_refine_mode(enable ? MUSIC_B200_REFINE_NEWTON : MUSIC_B200_REFINE_OFF); }
+
+/* The refine mode by number: OFF, NEWTON, or JOINT under the DML and WSF peak modes. */
+void baz_music_doa::set_refine_mode(int mode)
 {
     gr::thread::scoped_lock guard(d_mutex);
-    const int rc = music_b200_set_refine(d_handle, enable ? MUSIC_B200_REFINE_NEWTON : MUSIC_B200_REFINE_OFF);
+    const int rc = music_b200_set_refine(d_handle, mode);
     if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa: ") + music_b200_last_error(d_handle));
 }
 

@@ -55,13 +55,17 @@ public:
      * 2 = root-MUSIC, 3 = LS-ESPRIT, each on a uniform linear array set by set_array_geometry() (exclusion_bins must be 0),
      * 4 = deterministic maximum likelihood (coherent sources, any table; exclusion_bins must be 0),
      * 5 = root-MUSIC by manifold separation on any planar array set by set_array_geometry() spanning <= ~4.4 wavelengths
-     * (exclusion_bins must be 0) */
+     * (exclusion_bins must be 0), 6 = weighted subspace fitting (DML's search on the weighted signal subspace, any table;
+     * exclusion_bins must be 0) */
     void set_peak_mode(int mode, unsigned int exclusion_bins);
     /* extension: 0 = n sources in every window (default), 1 = MDL, 2 = AIC estimate of 0..n sources per window */
     void set_source_rule(int rule);
     /* extension: true = refine every peak off the grid on the exact spectrum of the geometry set by
      * set_array_geometry() (bins stay the grid bins); false = grid angles (default) */
     void set_refine(bool enable);
+    /* extension: the refine mode by number: 0 = off, 1 = Newton on the spectrum (as set_refine(true)), 2 = joint
+     * Gauss-Newton refinement of all slots of a window under peak modes 4 and 6 (include/music_b200.h) */
+    void set_refine_mode(int mode);
     /* extension: 0 = MUSIC (default), 1 = MVDR / Capon with diagonal loading loading * tr(R) / m, 2 = Bartlett
      * beamscan (loading must be 0 for 0 and 2) */
     void set_estimator(int estimator, double loading);

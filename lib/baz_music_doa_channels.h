@@ -55,7 +55,7 @@ public:
     void set_array_geometry(const std::vector<std::vector<double> > &positions_xy, double centre_frequency, double sample_rate);
     /* 0 = the n largest bins (default), 1 = the n largest local maxima more than exclusion_bins apart; coherent also
      * 2 = root-MUSIC, 3 = ESPRIT (uniform linear arrays), 4 = DML, 5 = root-MUSIC by manifold separation (any planar
-     * array on the reference channel's geometry) */
+     * array on the reference channel's geometry), 6 = WSF */
     void set_peak_mode(int mode, unsigned int exclusion_bins);
     /* 0 = n sources in every (window, channel) (default), 1 = MDL, 2 = AIC from the segments of each channel */
     void set_source_rule(int rule);

@@ -2,7 +2,7 @@
 """Small invocations of the kernels compute-sanitizer should look at (SURVEY.md section 5): run as
   compute-sanitizer --tool racecheck|memcheck|synccheck python tools/sanitize_targets.py <target>
 targets: fused (C1-size windows, 2000 of them + a ragged 1187 + a drain-only 9), fused_jacobi, fused8, covn8, covn16, eig16, esprit2d,
-gridless_roots, crb, tracks, multi,
+gridless_roots, crb, tracks, wsf, multi,
 lifecycle (every handle kind created, retuned, grown and destroyed through the host entry points; run it under
   compute-sanitizer --tool memcheck --leak-check full, which reports what a handle leaves allocated)"""
 import os
@@ -119,6 +119,28 @@ elif target == "crb":
     az.work(W, [x], [np.zeros((W, n), np.float32) for _ in range(3)])
     print(target, "ok az-el", az.last_crb()[:1, :2].tolist())
     az.close()
+elif target == "wsf":
+    # the WSF matrix and the JOINT refinement (music_wsf.cuh): M = 3, 8 and 16 with n up to M - 1 (d = 15 at M = 16, the
+    # largest shared-memory footprint), under WSF and DML; a zero window and a NaN window among them
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+    from helpers import LAM
+
+    W = 37
+    for m, n, mode in ((3, 2, "wsf"), (8, 3, "dml"), (16, 15, "wsf")):
+        rng = np.random.default_rng(m)
+        x = ((rng.standard_normal((W, 64 * m)) + 1j * rng.standard_normal((W, 64 * m)))).astype(np.complex64)
+        x[3] = 0
+        x[5, 11] = np.nan
+        k = np.arange(m)
+        pos = np.stack([0.5 * LAM * np.cos(2 * np.pi * k / m) * m / 6, 0.5 * LAM * np.sin(2 * np.pi * k / m) * m / 6], 1)
+        blk = music_doa(m, n, 64 * m, np.ones((360, m), np.complex64), 360)
+        blk.set_array_geometry(pos, LAM)
+        blk.set_peak_mode(mode, 0)
+        blk.set_refine("joint")
+        ang = np.zeros((W, n), np.float32)
+        blk.work(W, [x], [ang])
+        print(target, "ok", m, n, mode, ang[:2].tolist())
+        blk.close()
 elif target == "tracks":
     # the tracker (music_track.cuh): 32 rows and 15 slots in 1-D (CRB variance, every slot filled by DML) and az-el, a wide
     # gate so that ambiguous clusters reach the assignment solve, a zero window and a NaN window (a failed CRB) among
