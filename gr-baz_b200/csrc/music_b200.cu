@@ -32,6 +32,7 @@
 #include "music_refine.cuh"
 #include "music_azel.cuh"
 #include "music_estimators.cuh"
+#include "music_iaa.cuh"
 #include "music_roots.cuh"
 #include "music_manifold.cuh"
 #include "music_esprit.cuh"
@@ -152,7 +153,8 @@ struct Modes {
     uint32_t excl = 0;                       // exclusion_bins of the peak mode
     int refine = MUSIC_B200_REFINE_OFF;
     int est = MUSIC_B200_ESTIMATOR_MUSIC;
-    double loading = 0.0;                    // MVDR diagonal loading
+    double loading = 0.0;                    // MVDR and IAA diagonal loading
+    int iaa_iter = IAA_DEFAULT_ITERATIONS;   // IAA iteration count (music_b200_set_iaa_iterations)
 };
 
 // Targets of the fused all-gather of the peak bins (SURVEY.md section 8e): with G > 0 this GPU's windows are the
@@ -527,11 +529,14 @@ int check_modes(music_b200 *h, const Modes &p, const DeviceTable *t)
     if (p.excl >= h->K) return fail(h, MUSIC_B200_EINVAL, "exclusion_bins must be < resolution");
     if (p.refine != MUSIC_B200_REFINE_OFF && p.refine != MUSIC_B200_REFINE_NEWTON && p.refine != MUSIC_B200_REFINE_JOINT)
         return fail(h, MUSIC_B200_EINVAL, "unknown refine mode %d", p.refine);
-    if (p.est != MUSIC_B200_ESTIMATOR_MUSIC && p.est != MUSIC_B200_ESTIMATOR_MVDR && p.est != MUSIC_B200_ESTIMATOR_BARTLETT)
+    const bool iaa = p.est == MUSIC_B200_ESTIMATOR_IAA;
+    if (p.est != MUSIC_B200_ESTIMATOR_MUSIC && p.est != MUSIC_B200_ESTIMATOR_MVDR && p.est != MUSIC_B200_ESTIMATOR_BARTLETT && !iaa)
         return fail(h, MUSIC_B200_EINVAL, "unknown estimator %d", p.est);
     if (!std::isfinite(p.loading) || p.loading < 0.0) return fail(h, MUSIC_B200_EINVAL, "loading must be finite and >= 0 (got %g)", p.loading);
-    if (p.est != MUSIC_B200_ESTIMATOR_MVDR && p.loading != 0.0)
-        return fail(h, MUSIC_B200_EINVAL, "diagonal loading applies to MVDR only (got %g)", p.loading);
+    if (p.est != MUSIC_B200_ESTIMATOR_MVDR && !iaa && p.loading != 0.0)
+        return fail(h, MUSIC_B200_EINVAL, "diagonal loading applies to MVDR and IAA only (got %g)", p.loading);
+    if (iaa && p.refine != MUSIC_B200_REFINE_OFF)
+        return fail(h, MUSIC_B200_EINVAL, "the IAA estimator takes refinement OFF (refinement of IAA peaks is not built)");
     if (p.est == MUSIC_B200_ESTIMATOR_MVDR && p.loading == 0.0 && snapshots(h) <= h->m)
         return fail(h, MUSIC_B200_EINVAL, "MVDR without diagonal loading needs more snapshots than antennas (N = %u, m = %u): R is singular",
                     snapshots(h), h->m);
@@ -794,7 +799,8 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
     p.count = !fixed_n;
     p.mvdr = md.est == MUSIC_B200_ESTIMATOR_MVDR;
     p.est = md.est;
-    p.argmax = h->n == 1 && !local && !gridless && !dml;
+    // IAA writes P64 and leaves the peaks to the grid peak rules
+    p.argmax = h->n == 1 && !local && !gridless && !dml && md.est != MUSIC_B200_ESTIMATOR_IAA;
     p.spec = o.spec != nullptr;
     if (music_est && (gridless || dml)) {
         // the grid spectrum only when the caller asked for it; the angles come from the root, ESPRIT or DML kernel
@@ -925,6 +931,25 @@ void with_scan_form(const Plan &p, const int32_t *cnt, F f)
     else f(ScanForm<EST_MUSIC, false>());
 }
 
+// IAA (music_iaa.cuh) of W windows from ws.R against table tb: P64 [W][K], and the float spectrum when spec != NULL
+void launch_iaa(music_b200 *h, const WsView &ws, uint32_t W, double *p64, float *spec, const DeviceTable &tb, cudaStream_t st)
+{
+    const int M = (int)h->m;
+    with_scan_m(h->m, [&](auto mt) {
+        constexpr int MT = decltype(mt)::value;
+        const auto go = [&](auto tt) {
+            constexpr int T = decltype(tt)::value;
+            const size_t smem = iaa_smem_doubles(M, T) * sizeof(double);
+            iaa_kernel<MT, T><<<(W + T - 1) / T, IAA_THREADS, smem, st>>>(tb.soa, ws.R, M, (int)h->K, (int)W, h->modes.iaa_iter,
+                                                                         h->modes.loading, p64, spec);
+        };
+        if constexpr (MT != 0) go(std::integral_constant<int, iaa_windows(MT)>());
+        else if (M > 8) go(std::integral_constant<int, iaa_windows(16)>());
+        else go(std::integral_constant<int, iaa_windows(2)>());
+    });
+    h->launches++;
+}
+
 // K3, the grid scan of W windows the plan chose against table tb, into the outputs o of these windows.  cnt: the
 // per-window source counts (NULL under the FIXED rule).  scan_kernel stages per window the eigenvectors (MUSIC), the g_j of mvdr_prep_kernel
 // (MVDR) or R (Bartlett).
@@ -932,6 +957,10 @@ void launch_scan(music_b200 *h, const Plan &p, const WsView &ws, uint32_t W, con
                  const int32_t *cnt, const DeviceTable &tb, cudaStream_t st)
 {
     if (p.scan == Scan::None) return;
+    if (p.est == MUSIC_B200_ESTIMATOR_IAA) {
+        launch_iaa(h, ws, W, o.P64 ? o.P64 : ws.P64, o.spec, tb, st);
+        return;
+    }
     const double *soa = tb.soa;
     const double *V = p.est == MUSIC_B200_ESTIMATOR_BARTLETT ? ws.R : ws.Vt;
     float *d_spec = o.spec;
@@ -1999,6 +2028,17 @@ int create_on_device(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples
             CU(h, cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));
         }
         CU(h, cudaFuncSetAttribute(cov4_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)COV_SMEM));
+        // IAA (music_iaa.cuh): each instance opts in to the largest dynamic shared memory of the M it serves
+        CU(h, cudaFuncSetAttribute(iaa_kernel<4, iaa_windows(4)>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (int)(iaa_smem_max(4, 4, iaa_windows(4)) * sizeof(double))));
+        CU(h, cudaFuncSetAttribute(iaa_kernel<8, iaa_windows(8)>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (int)(iaa_smem_max(8, 8, iaa_windows(8)) * sizeof(double))));
+        CU(h, cudaFuncSetAttribute(iaa_kernel<16, iaa_windows(16)>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (int)(iaa_smem_max(16, 16, iaa_windows(16)) * sizeof(double))));
+        CU(h, cudaFuncSetAttribute(iaa_kernel<0, iaa_windows(2)>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (int)(iaa_smem_max(2, 8, iaa_windows(2)) * sizeof(double))));
+        CU(h, cudaFuncSetAttribute(iaa_kernel<0, iaa_windows(16)>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (int)(iaa_smem_max(9, 16, iaa_windows(16)) * sizeof(double))));
         if (chan) return init_channels(h);  // a channel handle takes its first tables at its first retune
         if (const int rc = alloc_slot(h, h->tables[0])) return rc;
         DeviceTable &t = h->tables[0].tabs[0];
@@ -2965,6 +3005,20 @@ int music_b200_set_estimator(music_b200 *h, int estimator, double loading)
     if (const int rc = check_modes(h, p, nullptr)) return rc;
     if (const int rc = for_each_child(h, [&](music_b200 *c) { return music_b200_set_estimator(c, estimator, loading); })) return rc;
     h->modes = p;
+    return MUSIC_B200_OK;
+}
+
+static_assert(IAA_MAX_ITERATIONS == MUSIC_B200_IAA_MAX_ITERATIONS && IAA_DEFAULT_ITERATIONS == MUSIC_B200_IAA_DEFAULT_ITERATIONS,
+              "the IAA iteration bounds of music_iaa.cuh and the header");
+
+int music_b200_set_iaa_iterations(music_b200 *h, int iterations)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (iterations < 1 || iterations > IAA_MAX_ITERATIONS)
+        return fail(h, MUSIC_B200_EINVAL, "the IAA iteration count must be 1 .. %d (got %d)", IAA_MAX_ITERATIONS, iterations);
+    std::lock_guard<std::mutex> g(h->mutex);
+    if (const int rc = for_each_child(h, [&](music_b200 *c) { return music_b200_set_iaa_iterations(c, iterations); })) return rc;
+    h->modes.iaa_iter = iterations;
     return MUSIC_B200_OK;
 }
 

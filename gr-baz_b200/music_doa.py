@@ -171,14 +171,21 @@ class music_doa(object):
         return getattr(self, "_refine", 0)
 
     # -- extension: the spectrum estimator -----------------------------------------------------------
-    ESTIMATORS = {"music": 0, "mvdr": 1, "bartlett": 2}
+    ESTIMATORS = {"music": 0, "mvdr": 1, "bartlett": 2, "iaa": 4}
 
     def set_estimator(self, kind="music", loading=0.0):
         """``"music"`` (default): P = 1 / ||G^H a||^2.  ``"bartlett"``: the delay-and-sum beamscan,
         P = a^H R a / (a^H a)^2.  ``"mvdr"``: the Capon spectrum P = 1 / (a^H (R + delta I)^-1 a) with the diagonal
         loading delta = loading * tr(R) / m; loading 0 needs more snapshots than antennas.  Both new spectra are power
         estimates (include/music_b200.h); the peak rule, ``n`` slots, the source rule and the refinement apply to them
-        unchanged.  ``loading`` must be 0 for "music" and "bartlett"."""
+        unchanged.  ``loading`` must be 0 for "music" and "bartlett".
+        ``"iaa"``: the iterative adaptive approach (Yardibi et al. 2010), a weighted-least-squares power spectrum that
+        starts from Bartlett and re-weights it ``set_iaa_iterations`` times (default 15) with the loading
+        delta = loading * tr(R) / m (any loading >= 0; 0 works for any snapshot count).  It needs no source count,
+        works with fewer snapshots than antennas and resolves coherent sources (multipath) on every block kind and
+        table; its level at a peak is the source's power.  It takes refinement off and the grid peak modes only.  It
+        does not replace "music" for closely spaced uncorrelated sources with plenty of snapshots, which MUSIC resolves
+        and IAA does not."""
         if kind not in self.ESTIMATORS:
             raise ValueError("kind must be one of %s" % sorted(self.ESTIMATORS))
         _capi.check(self._lib.music_b200_set_estimator(self._h, self.ESTIMATORS[kind], float(loading)), self._h)
@@ -188,6 +195,15 @@ class music_doa(object):
     def estimator(self):
         """(kind, loading) in use"""
         return getattr(self, "_estimator", ("music", 0.0))
+
+    def set_iaa_iterations(self, n=15):
+        """The iteration count of the "iaa" estimator: 1 .. 64, default 15 (read only under "iaa")."""
+        _capi.check(self._lib.music_b200_set_iaa_iterations(self._h, int(n)), self._h)
+        self._iaa_iterations = int(n)
+
+    @property
+    def iaa_iterations(self):
+        return getattr(self, "_iaa_iterations", 15)
 
     # -- extension: beamformed source signals ------------------------------------------------------------
     BEAMFORMERS = {"off": 0, "das": 1, "mvdr": 2, "lcmv": 3}

@@ -392,11 +392,52 @@ int music_b200_set_refine(music_b200 *h, int mode);
  * loading == 0 when N <= m (R is singular).  Setting MUSIC (loading 0) again restores the default behaviour exactly.
  * Applies to later process_*() calls (host, device, _ex, _counts, planar, sharded, az-el) and to every device of a
  * multi-device handle.
+ *
+ * MUSIC_B200_ESTIMATOR_IAA, the iterative adaptive approach (Yardibi, Li, Stoica, Xue & Baggeroer 2010): a
+ * nonparametric weighted-least-squares power spectrum on the grid.  It needs no source count and works from R alone, so
+ * it also runs when R is singular (N <= m), and it resolves coherent sources (a path and its reflection).  Its level at
+ * a peak is that source's power in R's units.  Definition, with Rh the window's fp64 covariance every other estimator
+ * reads (the R output, after calibration and integration; per channel R_c on a SEPARATE channel handle, the focused R
+ * on a COHERENT one), a_k table row k widened to fp64, nu_k = ||a_k||^2, I the iteration count
+ * (music_b200_set_iaa_iterations) and delta = loading * tr(Rh) / M:
+ *   p0_k = a_k^H Rh a_k / nu_k^2                  (the Bartlett P, so I = 0 would be Bartlett);
+ *   rows with nu_k = 0 have p_k = 0 at every step and add nothing;
+ *   for i = 1 .. I:  R_i = sum_k p(i-1)_k a_k a_k^H + delta I (fp64),  R_i = L L^H (Cholesky),  S_i = R_i^-1,
+ *                    p(i)_k = (a_k^H S_i Rh S_i a_k) / (a_k^H S_i a_k)^2,  the denominator evaluated as ||L^-1 a_k||^2
+ *                    (a sum of squares that cannot cancel, as MVDR);
+ *   P = p(I).
+ * Every P[k] of a window is NaN - the window reports no peak, (0, 0, bin -1), and its spectrum row is NaN, as under
+ * MVDR - when Rh has a non-finite entry or tr Rh <= 0, when a Cholesky pivot is not > 0 (NaN included), or when any
+ * p(i)_k is not finite.  The spectrum and P64 are P; TOP_BINS, LOCAL_MAXIMA and the az-el 2-D rules pick the peaks from
+ * P unchanged, level = (float)P at the peak; bins, counts (MDL / AIC count from the eigenvalues, as under MVDR) and R
+ * are unchanged.
+ * Accepted on every 1-D entry point (host, device, _ex, _counts, planar, sharded and gather, multi-device, _beams,
+ * _crb, _tracks), on az-el handles (host, device, _crb, _tracks) and on SEPARATE and COHERENT channel handles, with any
+ * finite loading >= 0: loading 0 is accepted for any N, N <= m included.  EINVAL with the ROOTS, ESPRIT, MANIFOLD, DML
+ * or WSF peak modes (they need the MUSIC estimator), with NEWTON or JOINT refinement and with the INCOHERENT combine.
+ * Runs unfused: covariance, [eigensolver + source count under MDL / AIC or when the eigenvalues are asked for], then one
+ * iaa_kernel launch per sub-batch (and per channel), timed in the scan slot, then the grid peak rule.  Its cost is
+ * about 3 K M^2 fp64 FMA per window per iteration (K = table rows; 9x the 1-D cost on a 360 x 91 az-el grid).
+ * Weakness: IAA does not replace MUSIC for closely spaced *uncorrelated* sources with plenty of snapshots.  Two
+ * uncorrelated sources 6 degrees apart on an 8-element lambda / 2 ULA at 10 dB and N = 64 are resolved by MUSIC in every
+ * window and by IAA in none: IAA's resolution there is that of a (sharpened) beam, MUSIC's that of the noise subspace.
+ * Not built: off-grid refinement of IAA peaks, SPICE, a fused path.
  */
 #define MUSIC_B200_ESTIMATOR_MUSIC 0
 #define MUSIC_B200_ESTIMATOR_MVDR 1
 #define MUSIC_B200_ESTIMATOR_BARTLETT 2
+/* IAA is 4, not the next free code 3: releases before IAA answered set_estimator(3) with EINVAL (unknown estimator),
+ * and that answer is kept, so code 3 stays unassigned. */
+#define MUSIC_B200_ESTIMATOR_IAA 4
 int music_b200_set_estimator(music_b200 *h, int estimator, double loading);
+
+/*
+ * The IAA iteration count I (MUSIC_B200_ESTIMATOR_IAA): 1 .. 64, default 15; EINVAL outside.  Applies to later calls
+ * and to every device of a multi-device handle; read only under the IAA estimator.
+ */
+#define MUSIC_B200_IAA_DEFAULT_ITERATIONS 15
+#define MUSIC_B200_IAA_MAX_ITERATIONS 64
+int music_b200_set_iaa_iterations(music_b200 *h, int iterations);
 
 /*
  * Beamformed source signals (extension, no reference counterpart): receive each reported source, a beam steered at

@@ -176,6 +176,14 @@ void baz_music_doa::set_estimator(int estimator, double loading)
     if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa: ") + music_b200_last_error(d_handle));
 }
 
+/* The IAA estimator's iteration count (1 .. 64, default 15), see include/music_b200.h. */
+void baz_music_doa::set_iaa_iterations(int iterations)
+{
+    gr::thread::scoped_lock guard(d_mutex);
+    const int rc = music_b200_set_iaa_iterations(d_handle, iterations);
+    if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa: ") + music_b200_last_error(d_handle));
+}
+
 /* Extension (not in the reference): beamformed source signals, see include/music_b200.h. */
 void baz_music_doa::set_beamformer(int rule, double loading)
 {

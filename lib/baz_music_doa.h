@@ -67,8 +67,10 @@ public:
      * Gauss-Newton refinement of all slots of a window under peak modes 4 and 6 (include/music_b200.h) */
     void set_refine_mode(int mode);
     /* extension: 0 = MUSIC (default), 1 = MVDR / Capon with diagonal loading loading * tr(R) / m, 2 = Bartlett
-     * beamscan (loading must be 0 for 0 and 2) */
+     * beamscan, 4 = IAA with diagonal loading loading * tr(R) / m (loading must be 0 for 0 and 2) */
     void set_estimator(int estimator, double loading);
+    /* the IAA estimator's iteration count: 1 .. 64, default 15 */
+    void set_iaa_iterations(int iterations);
     /* extension: beamformed source signals - 0 = off (default), 1 = delay-and-sum, 2 = MVDR, 3 = LCMV, with diagonal
      * loading loading * tr(R) / m for 2 and 3 (must be 0 for 0 and 1).  While it is on, work() also forms one beam per
      * filled peak slot of every item (include/music_b200.h), read back with last_beams(). */

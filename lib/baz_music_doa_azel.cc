@@ -112,6 +112,14 @@ void baz_music_doa_azel::set_estimator(int estimator, double loading)
     if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa_azel: ") + music_b200_last_error(d_handle));
 }
 
+/* The IAA estimator's iteration count (1 .. 64, default 15), see include/music_b200.h. */
+void baz_music_doa_azel::set_iaa_iterations(int iterations)
+{
+    gr::thread::scoped_lock guard(d_mutex);
+    const int rc = music_b200_set_iaa_iterations(d_handle, iterations);
+    if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa_azel: ") + music_b200_last_error(d_handle));
+}
+
 /* Extension (not in the reference): covariance integration across windows, see include/music_b200.h. */
 void baz_music_doa_azel::set_integration(double alpha)
 {

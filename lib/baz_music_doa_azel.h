@@ -54,8 +54,10 @@ public:
     void set_source_rule(int rule);
     /* true = refine every peak off the grid on the exact spectrum of the geometry (bins stay the grid bins) */
     void set_refine(bool enable);
-    /* 0 = MUSIC (default), 1 = MVDR with diagonal loading loading * tr(R) / m, 2 = Bartlett (loading 0 for 0 and 2) */
+    /* 0 = MUSIC (default), 1 = MVDR with diagonal loading loading * tr(R) / m, 2 = Bartlett, 4 = IAA (loading 0 for 0 and 2) */
     void set_estimator(int estimator, double loading);
+    /* the IAA estimator's iteration count: 1 .. 64, default 15 */
+    void set_iaa_iterations(int iterations);
     /* receiver calibration, as for baz_music_doa; calibrate() takes the source's azimuth and elevation */
     void set_calibration(const std::vector<std::complex<double> > &gains);
     std::vector<std::complex<double> > calibration();

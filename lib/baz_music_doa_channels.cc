@@ -111,6 +111,14 @@ void baz_music_doa_channels::set_estimator(int estimator, double loading)
     if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa_channels: ") + music_b200_last_error(d_handle));
 }
 
+/* The IAA estimator's iteration count (1 .. 64, default 15), see include/music_b200.h. */
+void baz_music_doa_channels::set_iaa_iterations(int iterations)
+{
+    gr::thread::scoped_lock guard(d_mutex);
+    const int rc = music_b200_set_iaa_iterations(d_handle, iterations);
+    if (rc != MUSIC_B200_OK) throw std::invalid_argument(std::string("music_doa_channels: ") + music_b200_last_error(d_handle));
+}
+
 void baz_music_doa_channels::set_focusing(unsigned int first_bin, unsigned int bin_count)
 {
     gr::thread::scoped_lock guard(d_mutex);

@@ -59,8 +59,10 @@ public:
     void set_peak_mode(int mode, unsigned int exclusion_bins);
     /* 0 = n sources in every (window, channel) (default), 1 = MDL, 2 = AIC from the segments of each channel */
     void set_source_rule(int rule);
-    /* 0 = MUSIC (default), 1 = MVDR with diagonal loading loading * tr(R) / m, 2 = Bartlett (loading 0 for 0 and 2) */
+    /* 0 = MUSIC (default), 1 = MVDR with diagonal loading loading * tr(R) / m, 2 = Bartlett, 4 = IAA (loading 0 for 0 and 2) */
     void set_estimator(int estimator, double loading);
+    /* the IAA estimator's iteration count: 1 .. 64, default 15 */
+    void set_iaa_iterations(int iterations);
 
     /* coherent: fit the focusing matrices on grid bins (first_bin + i) mod resolution, i < bin_count */
     void set_focusing(unsigned int first_bin, unsigned int bin_count);

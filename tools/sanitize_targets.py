@@ -2,7 +2,7 @@
 """Small invocations of the kernels compute-sanitizer should look at (SURVEY.md section 5): run as
   compute-sanitizer --tool racecheck|memcheck|synccheck python tools/sanitize_targets.py <target>
 targets: fused (C1-size windows, 2000 of them + a ragged 1187 + a drain-only 9), fused_jacobi, fused8, covn8, covn16, eig16, esprit2d,
-gridless_roots, crb, tracks, wsf, multi,
+gridless_roots, crb, tracks, wsf, iaa, multi,
 lifecycle (every handle kind created, retuned, grown and destroyed through the host entry points; run it under
   compute-sanitizer --tool memcheck --leak-check full, which reports what a handle leaves allocated)"""
 import os
@@ -18,6 +18,15 @@ from gr_baz_b200.music_doa import music_doa
 
 target = sys.argv[1] if len(sys.argv) > 1 else "fused"
 dev = torch.device("cuda:0")
+
+
+def synth_table(m, K):
+    """a UCA table of m elements, lambda / 2 between neighbours"""
+    k = np.arange(m)
+    r = 0.25 / np.sin(np.pi / m) if m > 2 else 0.25
+    pos = np.stack([r * np.cos(2 * np.pi * k / m), r * np.sin(2 * np.pi * k / m)], 1)
+    th = np.arange(K) * 2 * np.pi / K
+    return np.exp(-2j * np.pi * (np.outer(np.cos(th), pos[:, 0]) + np.outer(np.sin(th), pos[:, 1]))).astype(np.complex64)
 
 
 def run(cfg, counts, devices=None):
@@ -140,6 +149,29 @@ elif target == "wsf":
         ang = np.zeros((W, n), np.float32)
         blk.work(W, [x], [ang])
         print(target, "ok", m, n, mode, ang[:2].tolist())
+        blk.close()
+elif target == "iaa":
+    # the IAA kernel (music_iaa.cuh): M = 2, 4 and 16 (T = 8, 8 and 4 windows per CTA; the partial sums alias the tile
+    # region, M = 16 has the largest shared-memory footprint), a ragged window count (37: the last CTA is partly
+    # empty), a zero window and a NaN window (both fail before the first pass), and at M = 4 a noiseless rank-one window
+    # with loading 0, then a run with the spectrum port and a split into host chunks
+    W = 37
+    for m, n, loading in ((2, 1, 0.0), (4, 2, 0.0), (16, 3, 0.01)):
+        rng = np.random.default_rng(m)
+        N = 32
+        x = ((rng.standard_normal((W, N * m)) + 1j * rng.standard_normal((W, N * m)))).astype(np.complex64)
+        x[3] = 0
+        x[5, 11] = np.nan
+        if m == 4:
+            x[7] = np.tile(np.exp(1j * np.arange(m) * 0.7), N).astype(np.complex64)
+        blk = music_doa(m, n, N * m, synth_table(m, 360), 360)
+        blk.set_estimator("iaa", loading)
+        blk.set_iaa_iterations(3)
+        ang = np.zeros((W, n), np.float32)
+        spec = np.zeros((W, 360), np.float32)
+        blk.work(W, [x], [ang, np.zeros((W, n), np.float32), spec])
+        blk.work(9, [x[28:]], [ang[:9]])
+        print(target, "ok", m, n, ang[:2].tolist(), bool(np.isnan(spec[3]).all()), bool(np.isnan(spec[5]).all()))
         blk.close()
 elif target == "tracks":
     # the tracker (music_track.cuh): 32 rows and 15 slots in 1-D (CRB variance, every slot filled by DML) and az-el, a wide
