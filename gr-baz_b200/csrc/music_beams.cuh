@@ -20,8 +20,8 @@
 //   an odd M are also only 8-byte aligned, below the 16 bytes a bulk copy needs.)
 #pragma once
 #include "music_kernels.cuh"
-#include "music_estimators.cuh"
 #include "music_refine.cuh"
+#include "music_warp_la.cuh"
 
 namespace music {
 
@@ -82,12 +82,7 @@ __global__ void __launch_bounds__(BEAM_WARPS * 32) beam_weights_kernel(const dou
         const double2 *Rw = reinterpret_cast<const double2 *>(R) + (size_t)w * M * M;
         for (int e = lane; e < M * M; e += 32) A[e] = Rw[e];
         __syncwarp();
-        double tr = 0.0;  // as in mvdr_prep_kernel
-        for (int i = 0; i < M; ++i) tr += A[i * M + i].x;
-        const double delta = loading * tr / (double)M;
-        __syncwarp();
-        if (lane < M) A[lane * M + lane].x += delta;
-        __syncwarp();
+        warp_load_diagonal(A, M, M, loading, lane);
         ok = warp_cholesky(A, M, lane, [](int, double p) { return p > 0.0; });
     }
     __syncwarp();
@@ -98,26 +93,8 @@ __global__ void __launch_bounds__(BEAM_WARPS * 32) beam_weights_kernel(const dou
             for (int m = 0; m < M; ++m) nrm = fma(y[m].x, y[m].x, fma(y[m].y, y[m].y, nrm));
             for (int m = 0; m < M; ++m) z[m] = make_double2(y[m].x / nrm, y[m].y / nrm);
         } else {
-            for (int k = 0; k < M; ++k) {  // y = L^-1 a, in place
-                double sr = y[k].x, si = y[k].y;
-                for (int q = 0; q < k; ++q) {
-                    const double2 l = A[k * M + q], v = y[q];
-                    sr -= l.x * v.x - l.y * v.y;
-                    si -= l.x * v.y + l.y * v.x;
-                }
-                const double lk = A[k * M + k].x;
-                y[k] = make_double2(sr / lk, si / lk);
-            }
-            for (int k = M - 1; k >= 0; --k) {  // z = L^-H y
-                double sr = y[k].x, si = y[k].y;
-                for (int q = k + 1; q < M; ++q) {
-                    const double2 l = A[q * M + k], v = z[q];  // conj(L[q][k]) z_q
-                    sr -= l.x * v.x + l.y * v.y;
-                    si -= l.x * v.y - l.y * v.x;
-                }
-                const double lk = A[k * M + k].x;
-                z[k] = make_double2(sr / lk, si / lk);
-            }
+            const auto yk = [&](int k) -> double2 & { return y[k]; };  // y = L^-1 a, in place, then z = L^-H y
+            cholesky_solve(A, M, M, yk, yk, [&](int k) -> double2 & { return z[k]; });
             if (rule == BEAM_MVDR) {
                 double nrm = 0.0;
                 for (int m = 0; m < M; ++m) nrm = fma(y[m].x, y[m].x, fma(y[m].y, y[m].y, nrm));
@@ -145,26 +122,8 @@ __global__ void __launch_bounds__(BEAM_WARPS * 32) beam_weights_kernel(const dou
         if (ok && lane < M) {
             // lane m: row m of W = Z G^-1, i.e. u = G^-1 conj(Z[S][m]) and w_{S[r], m} = conj(u_r), in place in column m of Z
             const int m = lane;
-            for (int r = 0; r < d; ++r) {  // C v = conj(z)
-                double sr = Z[S[r] * M + m].x, si = -Z[S[r] * M + m].y;
-                for (int q = 0; q < r; ++q) {
-                    const double2 c = G[r * d + q], v = Z[S[q] * M + m];
-                    sr -= c.x * v.x - c.y * v.y;
-                    si -= c.x * v.y + c.y * v.x;
-                }
-                const double cr = G[r * d + r].x;
-                Z[S[r] * M + m] = make_double2(sr / cr, si / cr);
-            }
-            for (int r = d - 1; r >= 0; --r) {  // C^H u = v
-                double sr = Z[S[r] * M + m].x, si = Z[S[r] * M + m].y;
-                for (int q = r + 1; q < d; ++q) {
-                    const double2 c = G[q * d + r], v = Z[S[q] * M + m];  // conj(C[q][r]) u_q
-                    sr -= c.x * v.x + c.y * v.y;
-                    si -= c.x * v.y - c.y * v.x;
-                }
-                const double cr = G[r * d + r].x;
-                Z[S[r] * M + m] = make_double2(sr / cr, si / cr);
-            }
+            const auto zr = [&](int r) -> double2 & { return Z[S[r] * M + m]; };  // C v = conj(z), then C^H u = v
+            cholesky_solve(G, d, d, [&](int r) { return make_double2(zr(r).x, -zr(r).y); }, zr, zr);
             for (int r = 0; r < d; ++r) Z[S[r] * M + m].y = -Z[S[r] * M + m].y;
         }
     }

@@ -3,7 +3,7 @@
 // After the peak stage, each window's filled slots S = {i : bins[w][i] >= 0} (d = |S|) get the bound on the standard
 // deviation of their angle (1-D) or of their (azimuth, elevation) pair, evaluated at the window's own covariance R and
 // the reported angles (Stoica, Larsson & Gershman 2001; Stoica & Nehorai 1990):
-//   A = [a_i] = Q T (modified Gram-Schmidt applied twice, as dml_mgs2), s2 = (tr R - tr(Q^H R Q)) / (M - d),
+//   A = [a_i] = Q T (modified Gram-Schmidt applied twice, mgs2), s2 = (tr R - tr(Q^H R Q)) / (M - d),
 //   H = T^-1 (Q^H R Q) T^-H,  Gamma = T^-1 T^-H,  P = H - s2 Gamma,  U = P H^-1 P  (H by Cholesky),
 //   B = D^H (I - Q Q^H) D over the derivative columns D,  F = (2 N / s2) Re(B o U^T) per parameter pair,  C = F^-1.
 // The full definition (failure rules, outputs) is in include/music_b200.h and is restated literally by
@@ -15,11 +15,10 @@
 // window.
 #pragma once
 #include "music_kernels.cuh"
-#include "music_estimators.cuh"
 #include "music_refine.cuh"
 #include "music_azel.cuh"
-#include "music_dml.cuh"
 #include "music_integrate.cuh"
+#include "music_warp_la.cuh"
 
 namespace music {
 
@@ -119,29 +118,9 @@ __global__ void __launch_bounds__(32) crb_kernel(const double *__restrict__ R, c
         }
         sC[e] = s;
     }
-    // T^-1 (upper triangular): lane c solves column c by back substitution
-    if (lane < d) {
-        const int c = lane;
-        for (int i = d - 1; i >= 0; --i) {
-            double2 s = make_double2(0.0, 0.0);
-            if (i <= c) {
-                s.x = i == c ? 1.0 : 0.0;
-                for (int q = i + 1; q <= c; ++q) {
-                    const double2 t = cmul(sT[i * MAXM + q], sTi[q * d + c]);
-                    s.x -= t.x;
-                    s.y -= t.y;
-                }
-                const double tii = sT[i * MAXM + i].x;
-                s = make_double2(s.x / tii, s.y / tii);
-            }
-            sTi[i * d + c] = s;
-        }
-    }
+    triu_inverse(sT, MAXM, sTi, d, d, lane);  // T^-1 (upper triangular), column c by lane c
     __syncwarp();
-    double trR = 0.0, trC = 0.0;
-    for (int i = 0; i < M; ++i) trR += sR[i * M + i].x;
-    for (int i = 0; i < d; ++i) trC += sC[i * d + i].x;
-    const double s2 = (trR - trC) / (double)(M - d);
+    const double s2 = (trace_re(sR, M, M) - trace_re(sC, d, d)) / (double)(M - d);
     ok = ok && s2 > 0.0 && isfinite(s2);
 
     // 3. X = T^-1 C; H = X T^-H; P = H - s2 T^-1 T^-H into sC; U = P H^-1 P
@@ -177,26 +156,8 @@ __global__ void __launch_bounds__(32) crb_kernel(const double *__restrict__ R, c
     __syncwarp();
     if (ok && lane < d) {  // column `lane` of Y = H^-1 P: L y = p, then L^H z = y, into sX
         const int c = lane;
-        for (int k = 0; k < d; ++k) {
-            double sr = sC[k * d + c].x, si = sC[k * d + c].y;
-            for (int q = 0; q < k; ++q) {
-                const double2 l = sH[k * d + q], v = sX[q * d + c];
-                sr -= l.x * v.x - l.y * v.y;
-                si -= l.x * v.y + l.y * v.x;
-            }
-            const double lk = sH[k * d + k].x;
-            sX[k * d + c] = make_double2(sr / lk, si / lk);
-        }
-        for (int k = d - 1; k >= 0; --k) {
-            double sr = sX[k * d + c].x, si = sX[k * d + c].y;
-            for (int q = k + 1; q < d; ++q) {
-                const double2 l = sH[q * d + k], v = sX[q * d + c];  // conj(L[q][k]) z_q
-                sr -= l.x * v.x + l.y * v.y;
-                si -= l.x * v.y - l.y * v.x;
-            }
-            const double lk = sH[k * d + k].x;
-            sX[k * d + c] = make_double2(sr / lk, si / lk);
-        }
+        const auto xk = [&](int k) -> double2 & { return sX[k * d + c]; };
+        cholesky_solve(sH, d, d, [&](int k) -> const double2 & { return sC[k * d + c]; }, xk, xk);
     }
     __syncwarp();
     for (int e = lane; ok && e < d * d; e += 32) {  // U = P Y into sTi

@@ -15,6 +15,7 @@
 // Gram-Schmidt twice, the levels) in shared memory, the CTA the M x M products.  Everything is fp64.
 #pragma once
 #include "music_estimators.cuh"
+#include "music_warp_la.cuh"
 
 namespace music {
 
@@ -27,35 +28,6 @@ constexpr double DML_DEN_MIN = 9.313225746154785e-10;  // 2^-30: den(k) must exc
 __device__ __forceinline__ const double *dml_row(const double *soa, int k, int M)
 {
     return soa + (size_t)(k / TILE) * (2 * M + 1) * TILE + (k % TILE);
-}
-
-// One warp: Q[0 .. r-1] (row stride MAXM) = modified Gram-Schmidt, applied twice, of the vectors a_0 .. a_(r-1) in that
-// order, a_l[i] = row(l, i); T (row stride MAXM, may be null) receives the upper triangle of A = Q T.  Lane i holds
-// component i.  Shared by the DML kernel and the CRB kernel (music_crb.cuh).
-template <class Row>
-__device__ __forceinline__ void mgs2(Row row, int r, int M, double2 *Q, double2 *T, int lane)
-{
-    for (int l = 0; l < r; ++l) {
-        double2 v = make_double2(0.0, 0.0);
-        if (lane < M) v = row(l, lane);
-        for (int j = 0; j < l; ++j) {
-            if (T && lane == 0) T[j * MAXM + l] = make_double2(0.0, 0.0);
-        }
-        for (int pass = 0; pass < 2; ++pass) {
-            for (int j = 0; j < l; ++j) {
-                const double2 q = lane < M ? Q[j * MAXM + lane] : make_double2(0.0, 0.0);
-                const double2 p = cjmul(q, v);
-                const double2 c = make_double2(warp_sum(p.x), warp_sum(p.y));
-                v.x -= c.x * q.x - c.y * q.y;
-                v.y -= c.x * q.y + c.y * q.x;
-                if (T && lane == 0) { T[j * MAXM + l].x += c.x; T[j * MAXM + l].y += c.y; }
-            }
-        }
-        const double nrm = sqrt(warp_sum(v.x * v.x + v.y * v.y));
-        if (lane < M) Q[l * MAXM + lane] = make_double2(v.x / nrm, v.y / nrm);
-        if (T && lane == 0) T[l * MAXM + l] = make_double2(nrm, 0.0);
-        __syncwarp();
-    }
 }
 
 // Warp 0 of dml_kernel: mgs2 of the table rows bins[0 .. r-1]
@@ -101,8 +73,7 @@ __global__ void __launch_bounds__(DML_THREADS) dml_kernel(const double *__restri
         fin = fin && isfinite(v.x) && isfinite(v.y);
     }
     bool ok = __syncthreads_and(fin) && d > 0;
-    double trR = 0.0;  // every thread sums the diagonal in the same order
-    for (int i = 0; i < M; ++i) trR += sR[i * M + i].x;
+    double trR = trace_re(sR, M, M);  // every thread sums the diagonal in the same order
     ok = ok && trR > 0.0;
 
     // S(B) over the r bins in sB: the winner into s_win (-1: no candidate)
@@ -219,8 +190,7 @@ __global__ void __launch_bounds__(DML_THREADS) dml_kernel(const double *__restri
             for (int e = lane; e < MM; e += 32) sY[e] = Lw[e];
             __syncwarp();
             sL = sY;
-            trR = 0.0;
-            for (int i = 0; i < M; ++i) trR += sL[i * M + i].x;
+            trR = trace_re(sL, M, M);
         }
         dml_mgs2(soa, slot, d, M, sQ, sT, lane);
         // C[a][b] = q_a^H R q_b: lane a < d, then the trace terms
@@ -241,46 +211,12 @@ __global__ void __launch_bounds__(DML_THREADS) dml_kernel(const double *__restri
             sX[a * MAXM + b] = s;
         }
         __syncwarp();
-        double trQ = 0.0;
-        for (int a = 0; a < d; ++a) trQ += sX[a * MAXM + a].x;
-        const double s2 = (trR - trQ) / (double)(M - d);
+        const double s2 = (trR - trace_re(sX, MAXM, d)) / (double)(M - d);
         __syncwarp();
         if (lane < d) sX[lane * MAXM + lane].x -= s2;
-        // U = T^-1 (upper triangular) into sP: lane c solves column c by back substitution
-        double2 *U = sP;
-        if (lane < d) {
-            const int c = lane;
-            for (int i = d - 1; i >= 0; --i) {
-                double2 s = make_double2(i == c ? 1.0 : 0.0, 0.0);
-                if (i <= c) {
-                    for (int q = i + 1; q <= c; ++q) {
-                        const double2 t = cmul(sT[i * MAXM + q], U[q * MAXM + c]);
-                        s.x -= t.x;
-                        s.y -= t.y;
-                    }
-                    const double tii = sT[i * MAXM + i].x;
-                    s = make_double2(s.x / tii, s.y / tii);
-                } else {
-                    s = make_double2(0.0, 0.0);
-                }
-                U[i * MAXM + c] = s;
-            }
-        }
+        triu_inverse(sT, MAXM, sP, MAXM, d, lane);  // U = T^-1 (upper triangular) into sP, column c by lane c
         __syncwarp();
-        // p_l = sum_{a, b} U[l][a] C[a][b] conj(U[l][b])
-        if (lane < d) {
-            double p = 0.0;
-            for (int a = lane; a < d; ++a) {
-                double2 y = make_double2(0.0, 0.0);
-                for (int b = lane; b < d; ++b) {
-                    const double2 t = cmul(sX[a * MAXM + b], make_double2(U[lane * MAXM + b].x, -U[lane * MAXM + b].y));
-                    y.x += t.x;
-                    y.y += t.y;
-                }
-                p += cmul(U[lane * MAXM + a], y).x;
-            }
-            s_p[lane] = p;
-        }
+        if (lane < d) s_p[lane] = slot_level(sP, MAXM, sX, MAXM, d, lane);
         __syncwarp();
     }
     if (tid == 0) s_none = !ok;

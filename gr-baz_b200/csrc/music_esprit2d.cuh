@@ -16,7 +16,7 @@
 
 #include "music_azel.cuh"
 #include "music_esprit.cuh"
-#include "music_estimators.cuh"
+#include "music_warp_la.cuh"
 
 namespace music {
 

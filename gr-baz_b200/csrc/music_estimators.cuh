@@ -12,6 +12,7 @@
 // include/music_b200.h and is restated literally by tests/estimator_oracle.py.
 #pragma once
 #include "music_kernels.cuh"
+#include "music_warp_la.cuh"
 
 namespace music {
 
@@ -20,39 +21,6 @@ namespace music {
 // shared-memory copies (the factor and its inverse).  About 1.4 k complex flops per window at M = 16, next to the
 // covariance's N * M^2.
 constexpr int PREP_WARPS = 4;
-
-// In-place right-looking Cholesky A = L L^H of the M x M Hermitian matrix A (row-major, lower triangle read) by one
-// warp, A in shared memory; L overwrites the lower triangle with a real diagonal.  pivot_ok(k, d) tests pivot k before
-// its square root; every lane reads the same value, so the warp leaves the loop together.  Returns false on the first
-// pivot that fails (the factor is then incomplete).  mvdr_prep_kernel and beam_weights_kernel (music_beams.cuh).
-template <class PivotOk>
-__device__ __forceinline__ bool warp_cholesky(double2 *A, int M, int lane, PivotOk pivot_ok)
-{
-    bool ok = true;
-    for (int k = 0; k < M; ++k) {
-        const double d = A[k * M + k].x;
-        if (!pivot_ok(k, d)) { ok = false; break; }
-        const double l = sqrt(d);
-        __syncwarp();
-        if (lane == k) A[k * M + k] = make_double2(l, 0.0);
-        if (lane > k && lane < M) {
-            const double2 v = A[lane * M + k];
-            A[lane * M + k] = make_double2(v.x / l, v.y / l);
-        }
-        __syncwarp();
-        const int r = M - 1 - k;  // trailing block: A[i][j] -= L[i][k] conj(L[j][k]) for k < j <= i
-        for (int e = lane; e < r * r; e += 32) {
-            const int i = k + 1 + e / r, j = k + 1 + e % r;
-            if (j > i) continue;
-            const double2 a = A[i * M + k], b = A[j * M + k];
-            double2 &t = A[i * M + j];
-            t.x -= a.x * b.x + a.y * b.y;
-            t.y -= a.y * b.x - a.x * b.y;
-        }
-        __syncwarp();
-    }
-    return ok;
-}
 
 // R [W][M][M] (re, im) -> Vt [W][M][M] (re, im): Vt[w][j][m] = conj((L^-1)[j][m]) for m <= j, 0 for m > j.  A pivot
 // that is not > 0 (NaN included) makes every entry of the window NaN, so its whole spectrum is NaN and the peak rules
@@ -71,34 +39,14 @@ __global__ void __launch_bounds__(PREP_WARPS * 32) mvdr_prep_kernel(const double
     double2 *Gw = reinterpret_cast<double2 *>(Vt) + (size_t)w * MM;
     for (int e = lane; e < MM; e += 32) A[e] = Rw[e];
     __syncwarp();
-    double tr = 0.0;  // every lane sums the diagonal in the same order
-    for (int i = 0; i < M; ++i) tr += A[i * M + i].x;
-    const double delta = loading * tr / (double)M;
-    __syncwarp();
-    if (lane < M) A[lane * M + lane].x += delta;
-    __syncwarp();
+    warp_load_diagonal(A, M, M, loading, lane);
     const bool ok = warp_cholesky(A, M, lane, [](int, double d) { return d > 0.0; });
     if (!ok) {
         const double nan = __longlong_as_double(0x7ff8000000000000LL);
         for (int e = lane; e < MM; e += 32) Gw[e] = make_double2(nan, nan);
         return;
     }
-    // column c of L^-1 by forward substitution (lane c): x_c = 1 / L_cc, x_i = -(sum_{c <= q < i} L_iq x_q) / L_ii
-    if (lane < M) {
-        const int c = lane;
-        for (int i = 0; i < c; ++i) I[i * M + c] = make_double2(0.0, 0.0);
-        I[c * M + c] = make_double2(1.0 / A[c * M + c].x, 0.0);
-        for (int i = c + 1; i < M; ++i) {
-            double sr = 0.0, si = 0.0;
-            for (int q = c; q < i; ++q) {
-                const double2 l = A[i * M + q], x = I[q * M + c];
-                sr += l.x * x.x - l.y * x.y;
-                si += l.x * x.y + l.y * x.x;
-            }
-            const double li = A[i * M + i].x;
-            I[i * M + c] = make_double2(-sr / li, -si / li);
-        }
-    }
+    tril_inverse(A, M, I, M, M, lane);  // L^-1, column c by lane c
     __syncwarp();
     for (int e = lane; e < MM; e += 32) {
         const double2 v = I[e];

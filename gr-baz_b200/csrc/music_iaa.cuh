@@ -22,6 +22,7 @@
 // Cholesky pivot is not > 0 (NaN included), or any p(i)_k is not finite.
 #pragma once
 #include "music_estimators.cuh"
+#include "music_warp_la.cuh"
 
 namespace music {
 
@@ -83,22 +84,7 @@ __device__ bool iaa_prepare(const double *part, int T, int b, int NE, int NP, do
     }
     __syncwarp();
     if (!warp_cholesky(A, M, lane, [](int, double d) { return d > 0.0; })) return false;
-    // column c of L^-1 by forward substitution (lane c), as mvdr_prep_kernel
-    if (lane < M) {
-        const int c = lane;
-        for (int i = 0; i < c; ++i) G[i * M + c] = make_double2(0.0, 0.0);
-        G[c * M + c] = make_double2(1.0 / A[c * M + c].x, 0.0);
-        for (int i = c + 1; i < M; ++i) {
-            double sr = 0.0, si = 0.0;
-            for (int q = c; q < i; ++q) {
-                const double2 l = A[i * M + q], x = G[q * M + c];
-                sr += l.x * x.x - l.y * x.y;
-                si += l.x * x.y + l.y * x.x;
-            }
-            const double li = A[i * M + i].x;
-            G[i * M + c] = make_double2(-sr / li, -si / li);
-        }
-    }
+    tril_inverse(A, M, G, M, M, lane);  // L^-1, column c by lane c
     __syncwarp();
     for (int e = lane; e < M * M; e += 32) {  // Z = L^-1 Rh (the factor in A is no longer read)
         const int r = e / M, c = e % M;

@@ -15,9 +15,8 @@
 // The full definitions are in include/music_b200.h and are restated by tests/wsf_oracle.py.
 #pragma once
 #include "music_kernels.cuh"
-#include "music_estimators.cuh"
 #include "music_refine.cuh"
-#include "music_dml.cuh"
+#include "music_warp_la.cuh"
 
 namespace music {
 
@@ -183,24 +182,7 @@ __global__ void __launch_bounds__(32) joint_kernel(const double *__restrict__ R,
         *V = v2;
         __syncwarp();
         if (!grad) return true;
-        // T^-1 (upper triangular): lane c solves column c by back substitution
-        if (lane < d) {
-            const int c = lane;
-            for (int i = d - 1; i >= 0; --i) {
-                double2 s = make_double2(0.0, 0.0);
-                if (i <= c) {
-                    s.x = i == c ? 1.0 : 0.0;
-                    for (int q = i + 1; q <= c; ++q) {
-                        const double2 t = cmul(sT[i * MAXM + q], sTi[q * d + c]);
-                        s.x -= t.x;
-                        s.y -= t.y;
-                    }
-                    const double tii = sT[i * MAXM + i].x;
-                    s = make_double2(s.x / tii, s.y / tii);
-                }
-                sTi[i * d + c] = s;
-            }
-        }
+        triu_inverse(sT, MAXM, sTi, d, d, lane);  // T^-1 (upper triangular), column c by lane c
         // P_perp D, twice, in place
         for (int c = 0; c < d; ++c) {
             double2 v = lane < M ? sD[c * MAXM + lane] : make_double2(0.0, 0.0);
@@ -324,26 +306,11 @@ __global__ void __launch_bounds__(32) joint_kernel(const double *__restrict__ R,
         sC[e] = s;
     }
     __syncwarp();
-    double trR = 0.0, trC = 0.0;
-    for (int i = 0; i < M; ++i) trR += sR[i * M + i].x;
-    for (int i = 0; i < d; ++i) trC += sC[i * d + i].x;
-    const double s2 = (trR - trC) / (double)(M - d);
+    const double s2 = (trace_re(sR, M, M) - trace_re(sC, d, d)) / (double)(M - d);
     __syncwarp();
     if (lane < d) sC[lane * d + lane].x -= s2;
     __syncwarp();
-    if (lane < d) {  // p_l = sum_{a, b >= l} Ti[l][a] C[a][b] conj(Ti[l][b])
-        double p = 0.0;
-        for (int a = lane; a < d; ++a) {
-            double2 y = make_double2(0.0, 0.0);
-            for (int c = lane; c < d; ++c) {
-                const double2 t = cmul(sC[a * d + c], make_double2(sTi[lane * d + c].x, -sTi[lane * d + c].y));
-                y.x += t.x;
-                y.y += t.y;
-            }
-            p += cmul(sTi[lane * d + a], y).x;
-        }
-        sP[lane] = p;
-    }
+    if (lane < d) sP[lane] = slot_level(sTi, d, sC, d, d, lane);
     __syncwarp();
     if (filled) {
         const size_t o = (size_t)w * n + lane;
