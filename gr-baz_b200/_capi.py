@@ -120,6 +120,14 @@ def load():
         L.music_b200_calib_accumulate_host.restype = ctypes.c_int
         L.music_b200_calib_solve.argtypes = [vp, dbl, dbl, ctypes.c_int, fp, fp]
         L.music_b200_calib_solve.restype = ctypes.c_int
+        L.music_b200_calib_blind_reset.argtypes = [vp]
+        L.music_b200_calib_blind_reset.restype = ctypes.c_int
+        L.music_b200_calib_blind_accumulate_device.argtypes = [vp, fp, u32, u32, vp]
+        L.music_b200_calib_blind_accumulate_device.restype = ctypes.c_int
+        L.music_b200_calib_blind_accumulate_host.argtypes = [vp, fp, u32, u32]
+        L.music_b200_calib_blind_accumulate_host.restype = ctypes.c_int
+        L.music_b200_calib_blind_solve.argtypes = [vp, u32, ctypes.c_int, u32, ctypes.c_uint64, fp, fp, fp]
+        L.music_b200_calib_blind_solve.restype = ctypes.c_int
         L.music_b200_set_integration.argtypes = [vp, dbl]
         L.music_b200_set_integration.restype = ctypes.c_int
         L.music_b200_reset_integration.argtypes = [vp]
@@ -203,7 +211,8 @@ EXPORTS = [
     "music_b200_azel_lattice_host",
     "music_b200_set_beamformer", "music_b200_process_device_beams", "music_b200_process_host_beams",
     "music_b200_set_calibration", "music_b200_get_calibration", "music_b200_calib_reset", "music_b200_calib_accumulate_device",
-    "music_b200_calib_accumulate_host", "music_b200_calib_solve", "music_b200_set_integration", "music_b200_reset_integration",
+    "music_b200_calib_accumulate_host", "music_b200_calib_solve", "music_b200_calib_blind_reset", "music_b200_calib_blind_accumulate_device",
+    "music_b200_calib_blind_accumulate_host", "music_b200_calib_blind_solve", "music_b200_set_integration", "music_b200_reset_integration",
     "music_b200_process_device_crb", "music_b200_process_host_crb", "music_b200_process_azel_device_crb",
     "music_b200_process_azel_host_crb", "music_b200_set_tracking", "music_b200_reset_tracks", "music_b200_get_tracks",
     "music_b200_process_device_tracks", "music_b200_process_host_tracks", "music_b200_process_azel_device_tracks",

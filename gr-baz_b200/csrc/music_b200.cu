@@ -41,6 +41,7 @@
 #include "music_wsf.cuh"
 #include "music_beams.cuh"
 #include "music_calib.cuh"
+#include "music_calib_blind.cuh"
 #include "music_integrate.cuh"
 #include "music_crb.cuh"
 #include "music_track.cuh"
@@ -48,6 +49,8 @@
 #include "music_focus.cuh"
 
 using namespace music;
+
+static_assert(CB_MAX_SEGMENTS == MUSIC_B200_CALIB_MAX_SEGMENTS, "one segment limit");
 
 namespace {
 
@@ -290,6 +293,20 @@ struct music_b200 {
     DevBuf<unsigned> cal_ctr;
     DevBuf<double> cal_out;
     uint64_t cal_windows = 0;
+    // the self-calibration accumulator (music_b200_calib_blind_*, music_calib_blind.cuh; the served device): per segment
+    // the sum of the raw R of its windows (zeroed when allocated and at every reset), calib_accum_kernel's partial sums
+    // and counter, and the window count of every segment accumulated so far
+    DevBuf<double2> cb_acc, cb_part;
+    DevBuf<unsigned> cb_ctr;
+    std::vector<unsigned> cb_count;
+    // the solve's device scratch (music_calib_blind.cuh), grown as the shapes of the solves need
+    struct BlindWork {
+        DevBuf<unsigned> cnt;
+        DevBuf<double> Rw, ev, Vt, mag, Q, qev, qV, jp, J, out, angles;
+        DevBuf<double2> Pi, phi;
+        DevBuf<int> bins;
+        DevBuf<CbState> st;
+    } cb_work;
     // covariance integration (music_b200_set_integration, music_integrate.cuh), on while integ_alpha > 0: the carry S [m][m]
     // complex and the window count since the reset on the device, the tile scratch, and the event that orders each
     // sub-batch's integration after the previous one's, on whichever stream that ran.  integ_fresh: the next integration
@@ -2964,6 +2981,256 @@ int music_b200_calib_solve(music_b200 *h, double az_deg, double el_deg, int kind
     if (stats) {
         stats[0] = out[2 * MAXM];
         stats[1] = out[2 * MAXM + 1];
+    }
+    return MUSIC_B200_OK;
+}
+
+}  // extern "C"
+
+namespace {
+
+// Refusals shared by the self-calibration entry points: az-el and channel handles are out of its scope.
+int check_blind_handle(music_b200 *h)
+{
+    if (h->chan) return fail(h, MUSIC_B200_EINVAL, "self-calibration is not built for channel handles");
+    if (h->azel) return fail(h, MUSIC_B200_EINVAL, "self-calibration is not built for az-el handles");
+    return MUSIC_B200_OK;
+}
+
+// the per-segment sums, partial sums and counter of a served handle (zeroed on first use)
+int ensure_blind_buffers(music_b200 *h)
+{
+    if (h->cb_ctr) return MUSIC_B200_OK;  // (allocated last)
+    const size_t mm = (size_t)h->m * h->m;
+    CU(h, h->cb_acc.grow((size_t)CB_MAX_SEGMENTS * mm));
+    CU(h, h->cb_part.grow((size_t)CALIB_ACC_MAX_CTAS * mm));
+    CU(h, h->cb_ctr.grow(1));
+    CU(h, cudaMemset(h->cb_acc, 0, (size_t)CB_MAX_SEGMENTS * mm * sizeof(double2)));
+    CU(h, cudaMemset(h->cb_ctr, 0, sizeof(unsigned)));
+    CU(h, cudaDeviceSynchronize());  // the memsets ran on the legacy stream; the kernels run on non-blocking ones
+    h->cb_count.clear();
+    return MUSIC_B200_OK;
+}
+
+// nwindows windows in segments of `segment` (validated by the caller): nwindows a multiple of segment, room for the
+// segments in the accumulator
+int check_blind_accumulate(music_b200 *h, uint32_t nwindows, uint32_t segment)
+{
+    if (segment == 0) return fail(h, MUSIC_B200_EINVAL, "segment must be >= 1");
+    if (nwindows % segment != 0) return fail(h, MUSIC_B200_EINVAL, "nwindows (%u) must be a multiple of segment (%u)", nwindows, segment);
+    if (h->cb_count.size() + nwindows / segment > (size_t)CB_MAX_SEGMENTS)
+        return fail(h, MUSIC_B200_EINVAL, "more than %d self-calibration segments", CB_MAX_SEGMENTS);
+    return MUSIC_B200_OK;
+}
+
+// Adds the segments of nwindows windows at d_in (device memory of h, served and locked) to the accumulator, on st: the
+// covariance kernels in sub-batches of whole segments through workspace slot 0, then calib_accum_kernel once per segment
+// into that segment's sum.  A segment's sum depends on its windows alone, however the windows are split across calls.
+int calib_blind_accumulate(music_b200 *h, const float *d_in, uint32_t nwindows, uint32_t segment, cudaStream_t st)
+{
+    if (const int rc = ensure_blind_buffers(h)) return rc;
+    if (const int rc = check_blind_accumulate(h, nwindows, segment)) return rc;
+    Plan plan;  // R only
+    const uint32_t sub = std::max(segment, std::min(nwindows, max_sub_windows(h, plan)) / segment * segment);
+    Workspace &ws = h->ws[0];
+    if (const int rc = ensure_slot(h, ws, (sub + SCAN_B - 1) / SCAN_B * SCAN_B, plan)) return rc;
+    if (ws.used) CU(h, cudaStreamWaitEvent(st, ws.scan_done, 0));
+    const size_t mm = (size_t)h->m * h->m;
+    const int wpc = calib_acc_wpc((int)segment);
+    for (uint32_t w0 = 0; w0 < nwindows; w0 += sub) {
+        const uint32_t W = std::min(sub, nwindows - w0);
+        launch_cov(h, ws.view(), d_in + (size_t)w0 * h->nsamples * 2, W, st, 0);
+        for (uint32_t j = 0; j < W / segment; ++j) {
+            calib_accum_kernel<<<(segment + wpc - 1) / wpc, CALIB_THREADS, 0, st>>>(ws.R + (size_t)j * segment * mm * 2, (int)h->m,
+                                                                                   (int)segment, wpc, h->cb_part, h->cb_ctr,
+                                                                                   h->cb_acc + h->cb_count.size() * mm);
+            h->launches++;
+            h->cb_count.push_back(segment);
+        }
+        CU(h, cudaGetLastError());
+        CU(h, cudaEventRecord(ws.scan_done, st));
+        ws.used = true;
+    }
+    return MUSIC_B200_OK;
+}
+
+// whether the element positions [M][x, y] lie on one line (all coincident included): tests/calib_blind_oracle.py
+bool collinear(const double *pos, uint32_t M)
+{
+    int f = 0;
+    double L2 = 0.0;
+    for (uint32_t m = 0; m < M; ++m) {
+        const double dx = pos[2 * m] - pos[0], dy = pos[2 * m + 1] - pos[1], l = dx * dx + dy * dy;
+        if (l > L2) { L2 = l; f = (int)m; }
+    }
+    if (L2 == 0.0) return true;
+    const double fx = pos[2 * f] - pos[0], fy = pos[2 * f + 1] - pos[1];
+    double c = 0.0;
+    for (uint32_t m = 0; m < M; ++m) c = std::max(c, std::fabs((pos[2 * m] - pos[0]) * fy - (pos[2 * m + 1] - pos[1]) * fx));
+    return c <= 1e-9 * L2;
+}
+
+}  // namespace
+
+extern "C" {
+
+int music_b200_calib_blind_reset(music_b200 *h)
+{
+    h = served(h);
+    if (!h) return MUSIC_B200_EINVAL;
+    if (const int rc = check_blind_handle(h)) return rc;
+    std::lock_guard<std::mutex> g(h->mutex);
+    CU(h, cudaSetDevice(h->device));
+    if (const int rc = ensure_blind_buffers(h)) return rc;
+    CU(h, cudaDeviceSynchronize());  // accumulate calls still in flight on any stream
+    CU(h, cudaMemset(h->cb_acc, 0, h->cb_count.size() * h->m * h->m * sizeof(double2)));
+    CU(h, cudaDeviceSynchronize());
+    h->cb_count.clear();
+    return MUSIC_B200_OK;
+}
+
+int music_b200_calib_blind_accumulate_device(music_b200 *h, const float *d_in_c64, uint32_t nwindows, uint32_t segment, void *stream)
+{
+    h = served(h);
+    if (!h) return MUSIC_B200_EINVAL;
+    if (const int rc = check_blind_handle(h)) return rc;
+    if (segment == 0) return fail(h, MUSIC_B200_EINVAL, "segment must be >= 1");
+    if (nwindows == 0) return MUSIC_B200_OK;
+    if (!d_in_c64) return fail(h, MUSIC_B200_EINVAL, "d_in_c64 must not be NULL");
+    if ((reinterpret_cast<uintptr_t>(d_in_c64) & 15u) != 0) return fail(h, MUSIC_B200_EINVAL, "d_in_c64 must be 16-byte aligned");
+    std::lock_guard<std::mutex> g(h->mutex);
+    CU(h, cudaSetDevice(h->device));
+    return calib_blind_accumulate(h, d_in_c64, nwindows, segment, static_cast<cudaStream_t>(stream));
+}
+
+int music_b200_calib_blind_accumulate_host(music_b200 *h, const float *in_c64, uint32_t nwindows, uint32_t segment)
+{
+    h = served(h);
+    if (!h) return MUSIC_B200_EINVAL;
+    if (const int rc = check_blind_handle(h)) return rc;
+    if (segment == 0) return fail(h, MUSIC_B200_EINVAL, "segment must be >= 1");
+    if (nwindows == 0) return MUSIC_B200_OK;
+    if (!in_c64) return fail(h, MUSIC_B200_EINVAL, "in_c64 must not be NULL");
+    std::lock_guard<std::mutex> g(h->mutex);
+    CU(h, cudaSetDevice(h->device));
+    if (const int rc = ensure_blind_buffers(h)) return rc;
+    if (const int rc = check_blind_accumulate(h, nwindows, segment)) return rc;
+    // chunks of whole segments, ~32 MiB or one segment, through one pinned and one device buffer on the handle's first
+    // stream, as calib_accumulate_host does
+    const size_t win_bytes = (size_t)h->nsamples * 2 * sizeof(float);
+    const uint32_t chunk = std::max<uint32_t>(segment, (uint32_t)std::min<size_t>(nwindows, ((size_t)32 << 20) / win_bytes) / segment * segment);
+    const size_t chunk_floats = (size_t)chunk * h->nsamples * 2;
+    DevBuf<float> d;
+    PinBuf<float> pin;
+    cudaStream_t st = h->streams[0];
+    int rc = MUSIC_B200_OK;
+    if (d.grow(chunk_floats) != cudaSuccess || pin.grow(chunk_floats) != cudaSuccess)
+        rc = fail(h, MUSIC_B200_ENOMEM, "cannot allocate the self-calibration staging buffers");
+    for (uint32_t w0 = 0; w0 < nwindows && rc == MUSIC_B200_OK; w0 += chunk) {
+        const uint32_t W = std::min(chunk, nwindows - w0);
+        CU_BREAK(h, rc, cudaStreamSynchronize(st));  // the previous chunk's upload has left the pinned buffer
+        memcpy(pin, in_c64 + (size_t)w0 * h->nsamples * 2, W * win_bytes);
+        CU_BREAK(h, rc, cudaMemcpyAsync(d, pin, W * win_bytes, cudaMemcpyHostToDevice, st));
+        rc = calib_blind_accumulate(h, d, W, segment, st);
+    }
+    const cudaError_t e = cudaStreamSynchronize(st);
+    if (rc == MUSIC_B200_OK && e != cudaSuccess) rc = fail(h, MUSIC_B200_ECUDA, "stream sync failed: %s", cudaGetErrorString(e));
+    return rc;
+}
+
+int music_b200_calib_blind_solve(music_b200 *h, uint32_t d, int kind, uint32_t starts, uint64_t seed, double *gains, double *angles,
+                                 double *stats)
+{
+    h = served(h);
+    if (!h) return MUSIC_B200_EINVAL;
+    if (const int rc = check_blind_handle(h)) return rc;
+    if (!gains) return fail(h, MUSIC_B200_EINVAL, "gains must not be NULL");
+    if (kind != MUSIC_B200_CALIB_PHASE && kind != MUSIC_B200_CALIB_GAIN_PHASE) return fail(h, MUSIC_B200_EINVAL, "unknown calibration kind %d", kind);
+    if (h->m < 3) return fail(h, MUSIC_B200_EINVAL, "self-calibration needs m >= 3 (got %u)", h->m);
+    if (d < 1 || d > h->m - 2) return fail(h, MUSIC_B200_EINVAL, "self-calibration needs 1 <= d <= m - 2 (got d = %u, m = %u)", d, h->m);
+    if (starts < 1 || starts > (uint32_t)CB_MAX_STARTS) return fail(h, MUSIC_B200_EINVAL, "starts must be in 1 .. %d (got %u)", CB_MAX_STARTS, starts);
+    std::lock_guard<std::mutex> g(h->mutex);
+    const DeviceTable &tb = table(h);
+    if (!tb.geometric)
+        return fail(h, MUSIC_B200_EINVAL, "self-calibration needs a table built from the array geometry (set_geometry); the current one "
+                                          "came from set_table()");
+    if (collinear(tb.geo.pos, h->m))
+        return fail(h, MUSIC_B200_EINVAL, "self-calibration needs elements off one line (on a line a phase ramp along it cannot be told "
+                                          "from a shift of every direction)");
+    if (h->K > (uint32_t)CB_MAX_K) return fail(h, MUSIC_B200_EINVAL, "self-calibration scans tables of at most %d rows (K = %u)", CB_MAX_K, h->K);
+    const uint32_t S = (uint32_t)h->cb_count.size();
+    if (S == 0) return fail(h, MUSIC_B200_EINVAL, "no self-calibration segments accumulated");
+    const int M = (int)h->m, MM = M * M, P = (int)starts, D = (int)d, K = (int)h->K;
+    CU(h, cudaSetDevice(h->device));
+    CU(h, cudaDeviceSynchronize());  // every accumulate call, on whatever stream, has landed
+    auto &b = h->cb_work;
+    CU(h, b.cnt.grow(S));
+    CU(h, b.Rw.grow((size_t)S * MM * 2));
+    CU(h, b.ev.grow((size_t)S * M));
+    CU(h, b.Vt.grow((size_t)S * MM * 2));
+    CU(h, b.mag.grow(M));
+    CU(h, b.Q.grow((size_t)P * MM * 2));
+    CU(h, b.qev.grow((size_t)P * M));
+    CU(h, b.qV.grow((size_t)P * MM * 2));
+    CU(h, b.jp.grow((size_t)P * S));
+    CU(h, b.J.grow(P));
+    CU(h, b.out.grow(CB_OUT));
+    CU(h, b.angles.grow((size_t)S * D));
+    CU(h, b.Pi.grow((size_t)S * MM));
+    CU(h, b.phi.grow((size_t)P * M));
+    CU(h, b.bins.grow((size_t)P * S * D));
+    CU(h, b.st.grow(1));
+    cudaStream_t st = h->streams[0];
+    CU(h, cudaMemcpyAsync(b.cnt, h->cb_count.data(), S * sizeof(unsigned), cudaMemcpyHostToDevice, st));
+    Plan eig;
+    eig.eig = true;
+    const auto solve_eig = [&](double *R, double *ev, double *Vt, uint32_t W) {
+        launch_eig_stage(h, eig, WsView{R, ev, Vt, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr}, W, nullptr, 0, st);
+    };
+    // magnitudes, whitened segments, their noise projectors, the starts
+    cb_prep_kernel<<<1, CB_THREADS, 0, st>>>(h->cb_acc, b.cnt, M, (int)S, b.Rw, b.mag, b.st);
+    solve_eig(b.Rw, b.ev, b.Vt, S);
+    cb_proj_kernel<<<(unsigned)(((size_t)S * MM + CB_THREADS - 1) / CB_THREADS), CB_THREADS, 0, st>>>(b.Vt, M, M - D, (int)S, b.Pi);
+    cb_init_kernel<<<(P * M + 255) / 256, 256, 0, st>>>(b.phi, M, P, seed, b.st);
+    h->launches += 3;
+    CU(h, cudaGetLastError());
+    const size_t smem = (size_t)K * sizeof(double);
+    const auto scan_kernel = M <= 4 ? cb_scan_kernel<4> : M <= 8 ? cb_scan_kernel<8> : cb_scan_kernel<MAXM>;
+    CU(h, cudaFuncSetAttribute(scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const auto iteration = [&](bool polish) -> int {
+        scan_kernel<<<polish ? S : (unsigned)P * S, CB_THREADS, smem, st>>>(tb.soa, K, M, D, (int)S, b.Vt, b.phi, polish, b.st, b.bins, b.jp);
+        cb_q_kernel<<<polish ? 1 : P, CB_THREADS, 0, st>>>(tb.soa, M, D, (int)S, b.Pi, b.bins, b.jp, polish, b.st, b.Q, b.J);
+        solve_eig(b.Q, b.qev, b.qV, polish ? 1 : P);
+        cb_update_kernel<<<polish ? 1 : (P + 127) / 128, polish ? 32 : 128, 0, st>>>(b.qV, M, P, polish, b.st, b.phi);
+        h->launches += 3;
+        CU(h, cudaGetLastError());
+        return MUSIC_B200_OK;
+    };
+    for (int t = 0; t < CB_T1; ++t)
+        if (const int rc = iteration(false)) return rc;
+    cb_select_kernel<<<1, 1, 0, st>>>(b.J, P, b.st);
+    h->launches++;
+    for (int t = 0; t < CB_T2; ++t)
+        if (const int rc = iteration(true)) return rc;
+    cb_out_kernel<<<1, CB_THREADS, 0, st>>>(b.phi, b.mag, b.bins, b.J, M, (int)S, D, K, kind == MUSIC_B200_CALIB_PHASE, b.st, b.out, b.angles);
+    h->launches++;
+    CU(h, cudaGetLastError());
+    double out[CB_OUT];
+    std::vector<double> ang((size_t)S * D);
+    CU(h, cudaMemcpyAsync(out, b.out, sizeof out, cudaMemcpyDeviceToHost, st));
+    CU(h, cudaMemcpyAsync(ang.data(), b.angles, ang.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+    CU(h, cudaStreamSynchronize(st));
+    if (out[2 * MAXM + 3] == CB_NONFINITE_INPUT)
+        return fail(h, MUSIC_B200_EINVAL, "self-calibration failed: a non-finite value in the segment covariances, or an element without power");
+    if (out[2 * MAXM + 3] != CB_OK)
+        return fail(h, MUSIC_B200_EINVAL, "self-calibration failed: the fit is not finite (an eigenvector component of Q vanished)");
+    for (int i = 0; i < 2 * M; ++i) gains[i] = out[i];
+    if (angles) std::copy(ang.begin(), ang.end(), angles);
+    if (stats) {
+        stats[0] = out[2 * MAXM];
+        stats[1] = out[2 * MAXM + 1];
+        stats[2] = out[2 * MAXM + 2];
+        stats[3] = (double)S;
     }
     return MUSIC_B200_OK;
 }

@@ -24,6 +24,8 @@ import numpy as np
 
 from . import _capi
 
+CALIB_MAX_SEGMENTS = 1024  # MUSIC_B200_CALIB_MAX_SEGMENTS
+
 _uid = [0]
 _uid_lock = threading.Lock()
 
@@ -407,6 +409,46 @@ class music_doa(object):
         self.calib_reset()
         self.calib_accumulate(windows)
         return self.calib_solve(angle_deg, el_deg, kind)
+
+    # -- extension: receiver self-calibration without a known source ------------------------------------------------
+    def calib_blind_reset(self):
+        _capi.check(self._lib.music_b200_calib_blind_reset(self._h), self._h)
+
+    def calib_blind_accumulate(self, windows, segment):
+        """adds the segments of ``windows`` (complex64 (W, nsamples), host memory; W a multiple of ``segment``): every
+        ``segment`` consecutive windows form one segment covariance"""
+        x = np.ascontiguousarray(windows, dtype=np.complex64).reshape(-1, self.nsamples)
+        _capi.check(self._lib.music_b200_calib_blind_accumulate_host(self._h, x.ctypes.data, x.shape[0], int(segment)), self._h)
+
+    def calib_blind_accumulate_device(self, d_in, nwindows, segment, stream=None):
+        """raw device-pointer form of ``calib_blind_accumulate`` (enqueued on ``stream``)"""
+        _capi.check(self._lib.music_b200_calib_blind_accumulate_device(self._h, d_in, int(nwindows), int(segment), stream),
+                    self._h)
+
+    def calib_blind_solve(self, nsources, kind="gain_phase", starts=32, seed=0):
+        """the gains fitted to the accumulated segments, each holding ``nsources`` unknown sources: (complex128 (m,)
+        gains, float64 (S, nsources) angles in degrees (NaN where a segment had fewer local minima), stats) with stats a
+        dict of the misfit (small when calibrated), the polish iterations and the winning start.  The segments are
+        kept; nothing is applied."""
+        if kind not in self.CALIBRATIONS:
+            raise ValueError("kind must be one of %s" % sorted(self.CALIBRATIONS))
+        d = int(nsources)
+        g = np.empty(self.m, np.complex128)
+        st = np.empty(4, np.float64)
+        ang = np.empty((CALIB_MAX_SEGMENTS, max(d, 0)), np.float64)  # room for every segment the handle can hold
+        _capi.check(self._lib.music_b200_calib_blind_solve(self._h, d, self.CALIBRATIONS[kind], int(starts), int(seed),
+                                                           g.ctypes.data, ang.ctypes.data, st.ctypes.data), self._h)
+        S = int(st[3])
+        return g, ang[:S].copy(), {"misfit": float(st[0]), "polish": int(st[1]), "start": int(st[2])}
+
+    def calibrate_blind(self, windows, nsources, segment, kind="gain_phase", starts=32, seed=0):
+        """Estimate the receiver gains from ``windows`` (complex64 (W, nsamples)) of unknown emitters, ``nsources`` in
+        every segment of ``segment`` consecutive windows, without a known direction: reset, accumulate and solve on the
+        device.  Returns (gains, angles, stats) as ``calib_blind_solve``; apply the gains with ``set_calibration`` once
+        the misfit looks right.  Needs m >= 3 elements off one line and a table installed with ``set_array_geometry``."""
+        self.calib_blind_reset()
+        self.calib_blind_accumulate(windows, segment)
+        return self.calib_blind_solve(nsources, kind, starts, seed)
 
     # -- extension (SURVEY.md section 8(f) rank 4): GUI-rate reducers -----------------------------
     def reduce_angles(self, angles, levels=None, weighted=False):

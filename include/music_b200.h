@@ -549,6 +549,64 @@ int music_b200_calib_solve(music_b200 *h, double az_deg, double el_deg, int kind
                            double *stats /* host [2]: residual, sweeps; may be NULL */);
 
 /*
+ * Receiver self-calibration without a known source (extension, no reference counterpart): the element gains from windows
+ * of unknown emitters, so that the array can be recalibrated after every retune without a beacon at a surveyed bearing.
+ * Weiss-Friedlander eigenstructure calibration (1990) with the magnitudes read from the diagonal and a multi-start phase
+ * search.  Model as above: x_raw = G (A s + n), G = diag(g).  tests/calib_blind_oracle.py restates it literally.
+ *   segments   music_b200_calib_blind_accumulate_*(h, in, nwindows, segment): nwindows must be a multiple of segment
+ *              (>= 1); every `segment` consecutive windows form one segment, R_s = the mean fp64 covariance of its raw
+ *              windows (before any calibration that is set).  The sources may move between segments but are assumed
+ *              still within one: a single emitter moving past the array, or different emitters in different segments.
+ *              More distinct, well spread directions identify the gains better.  A segment never straddles calls; at
+ *              most MUSIC_B200_CALIB_MAX_SEGMENTS segments are held (EINVAL, nothing added, beyond).  R_s is
+ *              deterministic and does not depend on how the windows are split across calls.
+ *   magnitudes mag_m = sqrt(sum_s Re R_s,mm / S), scaled to sum mag_m^2 = M (exact on a population covariance with a
+ *              geometric table, |a_m| = 1); R_s <- T R_s T with T = diag(1 / mag), which whitens the noise.
+ *   projectors E_s = the M - d smallest-eigenvalue eigenvectors of the whitened R_s from the handle's eigensolver,
+ *              Pi_s = E_s E_s^H, computed once.
+ *   starts     start 0 is phi = 1; start p >= 1 takes phi_m = exp(j theta), theta = pi (2 u - 1), u = (z >> 11) 2^-53,
+ *              z = mix64(seed xor ((p * 256 + m + 1) * 0x9E3779B97F4A7C15 mod 2^64)), mix64 the splitmix64 finaliser
+ *              (z ^= z >> 30, z *= 0xBF58476D1CE4E5B9, z ^= z >> 27, z *= 0x94D049BB133111EB, z ^= z >> 31).
+ *   iteration  for each segment: P_s(k) = ||E_s^H (phi o a_k)||^2 / M over the rows a_k of the handle's table, and the d
+ *              best circular local maxima of q = 1 / P_s by the LOCAL_MAXIMA rule (q > 0, q[k] > q[k-1], q[k] >= q[k+1];
+ *              larger q first, lowest k on ties), bins k_s,1..d in pick order (fewer when fewer exist);
+ *              Q = sum_s sum_i D_k^H Pi_s D_k (D_k = diag(a_k)) in segment then pick order, and J = sum_s J_s in segment
+ *              order with J_s = sum_i P_s(k_s,i) in pick order.
+ *              Then phi <- v / |v| element-wise, v the eigenvector of the smallest eigenvalue of Q (handle's eigensolver)
+ *              rotated so that v_0 is real and positive.  (At a population Q the true phases are its null vector; the
+ *              eigenvector form stays well conditioned there, where W-F's linear constraint Q^-1 e_0 does not.)
+ *   schedule   every start runs 24 iterations; the winner is the start with the smallest J of its 24th iteration (lowest
+ *              index on ties; NaN never wins).  It is polished for up to 30 iterations, stopping after the first one whose
+ *              max_m |phi_new - phi_old| <= 2^-30.  The counts are fixed, so the result is deterministic.
+ *   outputs    gains [m][2]: mag o phi (MUSIC_B200_CALIB_GAIN_PHASE) or phi (MUSIC_B200_CALIB_PHASE); g_0 is real and
+ *              positive.  angles [S][d] (may be NULL): k 360 / K degrees of the last iteration's picks, NaN where a
+ *              segment had fewer than d local maxima.  stats [4] (may be NULL): the misfit J / (S d) of the last
+ *              iteration (in [0, 1], small when calibrated), the polish iterations run, the winning start, S.
+ *   limits     the grid is discrete: a fit can settle where the phase error looks to every segment like a shift of its
+ *              directions by one bin, with a small non-zero misfit and phase errors of the order of the grid step.  24
+ *              iterations per start avoid it in the exact-covariance cases of tests/test_calib_blind_oracle.py (UCA-4 and
+ *              UCA-8, d = 1 and 2, 8 and 16 segments spread over the circle, seeds 0 - 9) but one, UCA-8 with d = 1 and 8
+ *              segments at seed 5, which neither more starts nor more iterations reach.  More segments and spread
+ *              directions avoid it.  On exact covariances the misfit tells it apart (about 1e-4 against 1e-30); on
+ *              measured windows the estimation noise sets the misfit of a good fit too.
+ *   refusals   EINVAL, nothing written, for: an az-el or channel handle (not built); a set_table() table; collinear element
+ *              positions (a phase ramp along the line cannot be told from a shift of every direction); m < 3; d outside
+ *              1 .. m - 2; no segments; starts outside 1 .. 256; a table of more than 24576 rows (the scan holds a
+ *              segment's spectrum in shared memory); non-finite segment covariances or an element without power.
+ *   calls      calib_blind_accumulate_device needs d_in 16-byte aligned, is enqueued on `stream` and does not synchronise;
+ *              _host copies in chunks and returns when done.  solve enqueues a fixed number of kernels on one stream,
+ *              synchronises once, leaves the segments unchanged and does not apply the gains: the caller inspects the
+ *              misfit, then calls set_calibration.  reset empties the segments.  On a multi-device handle devices[0]
+ *              serves them all, and accumulate_device needs its input there.
+ */
+#define MUSIC_B200_CALIB_MAX_SEGMENTS 1024
+int music_b200_calib_blind_reset(music_b200 *h);
+int music_b200_calib_blind_accumulate_device(music_b200 *h, const float *d_in_c64, uint32_t nwindows, uint32_t segment, void *stream);
+int music_b200_calib_blind_accumulate_host(music_b200 *h, const float *in_c64, uint32_t nwindows, uint32_t segment);
+int music_b200_calib_blind_solve(music_b200 *h, uint32_t d, int kind, uint32_t starts, uint64_t seed, double *gains /* host [m][2] */,
+                                 double *angles /* host [S][d] or NULL */, double *stats /* host [4] or NULL */);
+
+/*
  * Covariance integration across windows (extension, no reference counterpart): an exponentially weighted covariance
  * carried from window to window and from call to call, so that a weak source is detected and located from the recent
  * past while every window keeps its own output rate and latency.

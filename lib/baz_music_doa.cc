@@ -74,7 +74,7 @@ baz_music_doa::baz_music_doa(unsigned int m, unsigned int n, unsigned int nsampl
                      gr::io_signature::make3(1, 3, n * sizeof(float), n * sizeof(float), resolution * sizeof(float))),
       d_m(m), d_n(n), d_nsamples(nsamples), d_resolution(resolution), d_handle(NULL), d_track_rows(0),
       d_source_rule(MUSIC_B200_SOURCES_FIXED), d_beam_rule(MUSIC_B200_BEAMS_OFF), d_crb(false), d_cal_remaining(0), d_cal_angle(0.0), d_cal_kind(MUSIC_B200_CALIB_GAIN_PHASE),
-      d_cal_residual(std::numeric_limits<double>::quiet_NaN())
+      d_cal_residual(std::numeric_limits<double>::quiet_NaN()), d_cal_blind(false), d_cal_nsources(1), d_cal_segment(1)
 {
     if (array_response.size() != resolution) throw std::invalid_argument("music_doa: array_response.size() != resolution");
     const std::vector<float> table = flatten(array_response);
@@ -267,6 +267,47 @@ void baz_music_doa::calibrate(double angle_deg, int kind, int nitems)
     d_cal_remaining = nitems;
     d_cal_angle = angle_deg;
     d_cal_kind = kind;
+    d_cal_blind = false;
+}
+
+void baz_music_doa::calibrate_blind(int nsources, int kind, int nitems, int segment)
+{
+    if (segment <= 0 || nitems <= 0 || nitems % segment != 0)
+        throw std::invalid_argument("music_doa: calibrate_blind() needs segment > 0 and nitems a positive multiple of segment");
+    if (kind != MUSIC_B200_CALIB_PHASE && kind != MUSIC_B200_CALIB_GAIN_PHASE) throw std::invalid_argument("music_doa: unknown calibration kind");
+    if (nsources <= 0) throw std::invalid_argument("music_doa: calibrate_blind() needs nsources > 0");
+    gr::thread::scoped_lock guard(d_mutex);
+    const int rc = music_b200_calib_blind_reset(d_handle);
+    if (rc != MUSIC_B200_OK) throw std::runtime_error(std::string("music_doa: ") + music_b200_last_error(d_handle));
+    d_cal_remaining = nitems;
+    d_cal_kind = kind;
+    d_cal_blind = true;
+    d_cal_nsources = nsources;
+    d_cal_segment = segment;
+    d_cal_pending.clear();
+}
+
+/* The armed self-calibration step at the end of work(): accumulate the whole segments of this call's armed items (a
+ * segment split across calls waits in d_cal_pending); once all are in, solve, apply and record the misfit (NaN on
+ * failure, with the old gains kept). */
+void baz_music_doa::calibration_blind_step(const float *in, int noutput_items)
+{
+    if (d_cal_remaining <= 0) return;
+    const int take = noutput_items < d_cal_remaining ? noutput_items : d_cal_remaining;
+    d_cal_remaining -= take;
+    const size_t item = (size_t)d_nsamples * 2;
+    d_cal_pending.insert(d_cal_pending.end(), in, in + (size_t)take * item);
+    const uint32_t whole = (uint32_t)(d_cal_pending.size() / item) / (uint32_t)d_cal_segment * (uint32_t)d_cal_segment;
+    bool ok = whole == 0 || music_b200_calib_blind_accumulate_host(d_handle, d_cal_pending.data(), whole, (uint32_t)d_cal_segment) == MUSIC_B200_OK;
+    d_cal_pending.erase(d_cal_pending.begin(), d_cal_pending.begin() + (ptrdiff_t)(whole * item));
+    if (ok && d_cal_remaining > 0) return;
+    std::vector<double> g(2 * MUSIC_B200_MAX_M);
+    double stats[4];
+    ok = ok && music_b200_calib_blind_solve(d_handle, (uint32_t)d_cal_nsources, d_cal_kind, 32, 0, g.data(), NULL, stats) == MUSIC_B200_OK &&
+         music_b200_set_calibration(d_handle, g.data()) == MUSIC_B200_OK;
+    d_cal_residual = ok ? stats[0] : std::numeric_limits<double>::quiet_NaN();
+    d_cal_remaining = 0;
+    d_cal_pending.clear();
 }
 
 int baz_music_doa::work(int noutput_items, gr_vector_const_void_star &input_items, gr_vector_void_star &output_items)
@@ -317,6 +358,7 @@ int baz_music_doa::work(int noutput_items, gr_vector_const_void_star &input_item
         rc = music_b200_process_host_counts(d_handle, in, (uint32_t)noutput_items, out, lvl, out_spectrum, d_bins.data(), d_counts.data());
     }
     if (rc != MUSIC_B200_OK) throw std::runtime_error(std::string("music_doa: ") + music_b200_last_error(d_handle));
-    calibration_step(d_handle, in, noutput_items, d_cal_remaining, d_cal_angle, 0.0, d_cal_kind, d_cal_residual);
+    if (d_cal_blind) calibration_blind_step(in, noutput_items);
+    else calibration_step(d_handle, in, noutput_items, d_cal_remaining, d_cal_angle, 0.0, d_cal_kind, d_cal_residual);
     return noutput_items;
 }

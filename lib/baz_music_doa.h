@@ -86,6 +86,12 @@ public:
     std::vector<std::complex<double> > calibration();
     void calibrate(double angle_deg, int kind, int nitems);
     double last_calibration_residual() const { return d_cal_residual; }
+    /* extension: self-calibration without a known source (include/music_b200.h).  calibrate_blind(): arms the block like
+     * calibrate() - the next nitems items (a multiple of segment) are also accumulated, every `segment` consecutive items
+     * one segment covariance of nsources unknown emitters; then the block solves for the gains (32 starts, seed 0) and
+     * applies them.  last_calibration_residual() then reads the solve's misfit (small when calibrated), NaN when the
+     * solve failed (the old gains are kept).  Needs m >= 3 elements off one line and a table from set_array_geometry(). */
+    void calibrate_blind(int nsources, int kind, int nitems, int segment);
     /* extension: covariance integration across work() calls (include/music_b200.h).  set_integration(): forgetting
      * factor 0 <= alpha < 1 (0, the default, is off); each item's estimate reads the exponentially weighted covariance of
      * the items since the last reset, across calls, and MDL / AIC count with the effective snapshot count.
@@ -147,7 +153,14 @@ private:
     double d_cal_angle;
     int d_cal_kind;
     double d_cal_residual;
+    /* calibrate_blind(): armed (d_cal_remaining and d_cal_kind serve it too), the source count, the segment length and
+     * the items of a segment a work() call left incomplete */
+    bool d_cal_blind;
+    int d_cal_nsources;
+    int d_cal_segment;
+    std::vector<float> d_cal_pending;
     gr::thread::mutex d_mutex;
+    void calibration_blind_step(const float *in, int noutput_items);
 };
 
 #endif /* INCLUDED_BAZ_MUSIC_DOA_H */
