@@ -8,3 +8,4 @@ package at the repo root.
 
 from .music_doa_azel import music_doa_azel  # noqa: E402,F401  (azimuth + elevation, include/music_b200.h)
 from .music_doa_channels import music_doa_channels  # noqa: E402,F401  (frequency-channelised, include/music_b200.h)
+from .music_doa_coarray import music_doa_coarray  # noqa: E402,F401  (sparse linear arrays, include/music_b200.h)

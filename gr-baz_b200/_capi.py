@@ -178,6 +178,12 @@ def load():
         L.music_b200_process_channels_device.restype = ctypes.c_int
         L.music_b200_process_channels_host.argtypes = [vp, fp, u32, fp, fp, fp, fp, fp, fp]
         L.music_b200_process_channels_host.restype = ctypes.c_int
+        L.music_b200_create_coarray.argtypes = [ctypes.POINTER(vp), u32, u32, u32, u32, fp, fp, dbl, u32, ctypes.c_int]
+        L.music_b200_create_coarray.restype = ctypes.c_int
+        L.music_b200_set_geometry_coarray.argtypes = [vp, fp, dbl]
+        L.music_b200_set_geometry_coarray.restype = ctypes.c_int
+        L.music_b200_coarray_size.argtypes = [vp, ctypes.POINTER(u32)]
+        L.music_b200_coarray_size.restype = ctypes.c_int
         L.music_b200_launch_count.argtypes = [vp]
         L.music_b200_launch_count.restype = ctypes.c_uint64
         L.music_b200_set_stage_timing.argtypes = [vp, ctypes.c_int]
@@ -220,6 +226,7 @@ EXPORTS = [
     "music_b200_create_channels", "music_b200_set_geometry_channels", "music_b200_channel_frequencies",
     "music_b200_get_table_channel", "music_b200_process_channels_device", "music_b200_process_channels_host",
     "music_b200_set_focusing", "music_b200_get_focusing",
+    "music_b200_create_coarray", "music_b200_set_geometry_coarray", "music_b200_coarray_size",
 ]
 
 

@@ -47,6 +47,7 @@
 #include "music_track.cuh"
 #include "music_channels.cuh"
 #include "music_focus.cuh"
+#include "music_coarray.cuh"
 
 using namespace music;
 
@@ -145,6 +146,7 @@ struct Workspace {
     DevBuf<unsigned long long> n0;  // integration: the count since the reset at the sub-batch's first window
     DevBuf<float> std;     // [windows][sw] the CRB a tracks call under CRB variance reads when the caller asked for none
     DevBuf<double> X;      // [windows][m][m] complex: the WSF matrix the DML search reads (music_wsf.cuh)
+    DevBuf<double> Rin;    // co-array handle: [windows][m_in][m_in] complex physical R, mapped into R (music_coarray.cuh)
     cudaEvent_t scan_done = nullptr;
     bool used = false;
     WsView view() const { return {R, ev, Vt, P64, cnt, bins, wts, n0, std, X}; }
@@ -266,6 +268,7 @@ struct HostSlot {
 
 struct music_b200 {
     uint32_t m = 0, n = 0, nsamples = 0, K = 0, N = 0;
+    uint32_t m_in = 0;       // elements per input snapshot: m on every handle but a co-array handle, whose m is Mv
     int device = 0;
     int sm_count = 0;
     std::mutex mutex;        // serialises process_*() and set_table(), like d_mutex (:67, :101)
@@ -346,6 +349,10 @@ struct music_b200 {
     DevBuf<double2> foc_B;       // [C][m][m] B_c
     DevBuf<double> foc_e2;       // [C] squared focusing errors
     DevBuf<double2> foc_Rc;      // the filter bank's [C][W][m][m] covariances of a sub-batch (the workspace holds W windows)
+    // co-array handle (music_b200_create_coarray, music_coarray.cuh): m_in physical elements, m = Mv virtual ones; the
+    // lag table, and the physical R of each sub-batch in its workspace slot's Rin
+    bool coarray = false;
+    CoarrayLags co_lags = {};
 
     // fp64 workspace slots (R, eigenvalues, sorted eigenvectors, optional strengths) of the unfused path: one per
     // staging stream of the host entry points (slot 0 also serves the device entry points)
@@ -527,6 +534,12 @@ bool gridless_mode(int peak)
 
 bool coherent(const music_b200 *h) { return h->chan && h->chan_combine == MUSIC_B200_CHANNELS_COHERENT; }
 
+// EINVAL naming `what` on a co-array handle, which does not serve it (include/music_b200.h lists what it serves)
+int refuse_coarray(music_b200 *h, const char *what)
+{
+    return h->coarray ? fail(h, MUSIC_B200_EINVAL, "%s is not built for co-array handles", what) : MUSIC_B200_OK;
+}
+
 // The independent looks behind each covariance: the N snapshots of a window, on a channel handle its J segments, and
 // behind a focused covariance the J segments of all C channels.
 uint32_t snapshots(const music_b200 *h)
@@ -552,6 +565,16 @@ int check_modes(music_b200 *h, const Modes &p, const DeviceTable *t)
     if (!std::isfinite(p.loading) || p.loading < 0.0) return fail(h, MUSIC_B200_EINVAL, "loading must be finite and >= 0 (got %g)", p.loading);
     if (p.est != MUSIC_B200_ESTIMATOR_MVDR && !iaa && p.loading != 0.0)
         return fail(h, MUSIC_B200_EINVAL, "diagonal loading applies to MVDR and IAA only (got %g)", p.loading);
+    if (h->coarray) {
+        // R_ss is a covariance of the virtual array only under the co-array model, whose noise subspace MUSIC reads
+        if (p.est != MUSIC_B200_ESTIMATOR_MUSIC)
+            return fail(h, MUSIC_B200_EINVAL, "a co-array handle takes the MUSIC estimator only (MVDR, Bartlett and IAA are not built on "
+                                              "the co-array covariance)");
+        if (subspace_fit || p.peak == MUSIC_B200_PEAKS_MANIFOLD)
+            return fail(h, MUSIC_B200_EINVAL, "a co-array handle takes the TOP_BINS, LOCAL_MAXIMA, ROOTS and ESPRIT peak modes only "
+                                              "(DML, WSF and MANIFOLD are not built on the co-array covariance)");
+        if (p.refine == MUSIC_B200_REFINE_JOINT) return fail(h, MUSIC_B200_EINVAL, "a co-array handle takes refinement OFF or NEWTON");
+    }
     if (iaa && p.refine != MUSIC_B200_REFINE_OFF)
         return fail(h, MUSIC_B200_EINVAL, "the IAA estimator takes refinement OFF (refinement of IAA peaks is not built)");
     if (p.est == MUSIC_B200_ESTIMATOR_MVDR && p.loading == 0.0 && snapshots(h) <= h->m)
@@ -800,11 +823,12 @@ Plan plan_call(const music_b200 *h, const Outputs &o, const PlanarStreams *plana
     // eigenvectors the peak refinement needs; they compute the MUSIC spectrum only.  Planar streams can take the M = 4
     // kernel when the 16-byte granularity of its bulk copies allows it.
     bool planar_fusable = !planar || (hop % 2 == 0 && h->N % 2 == 0);
-    for (uint32_t r = 0; planar && r < h->m; ++r) planar_fusable = planar_fusable && (reinterpret_cast<uintptr_t>(planar->p[r]) & 15u) == 0;
+    for (uint32_t r = 0; planar && r < h->m_in; ++r) planar_fusable = planar_fusable && (reinterpret_cast<uintptr_t>(planar->p[r]) & 15u) == 0;
     // A beams call needs R, which the fused kernels keep in registers: it runs the unfused plan of a call that asks for R.
     const bool beams = o.wts || o.beams;
     const bool track = o.slot_track != nullptr;
-    const bool fusable = h->fused && !h->chan && !h->azel && music_est && fixed_n && md.refine == MUSIC_B200_REFINE_OFF &&
+    // a co-array handle never fuses: the fused kernels read the input with M = m, and its input has m_in elements
+    const bool fusable = h->fused && !h->chan && !h->azel && !h->coarray && music_est && fixed_n && md.refine == MUSIC_B200_REFINE_OFF &&
                          md.peak == MUSIC_B200_PEAKS_TOP_BINS && h->n == 1 && !o.P64 && !o.R && !o.ev && !beams && !o.std && !track &&
                          !h->calib && h->integ_alpha == 0.0;
     if (fusable && h->m == 4 && planar_fusable && (!o.spec || h->fused_spec)) p.path = Path::Fused4;
@@ -867,7 +891,8 @@ uint32_t max_sub_windows(const music_b200 *h, const Plan &p)
                            (p.ws_counts ? sizeof(int32_t) : 0) + (p.ws_bins ? h->n * sizeof(int32_t) : 0) +
                            (p.ws_wts ? (size_t)h->n * h->m * 2 * sizeof(double) : 0) +
                            (p.ws_std ? (size_t)(h->azel ? 3 : 1) * h->n * sizeof(float) : 0) +
-                           (p.wsf ? (size_t)h->m * h->m * 2 * sizeof(double) : 0);
+                           (p.wsf ? (size_t)h->m * h->m * 2 * sizeof(double) : 0) +
+                           (h->coarray ? (size_t)h->m_in * h->m_in * 2 * sizeof(double) : 0);
     // A SEPARATE / INCOHERENT channel handle's workspace holds C pseudo-windows per window; a COHERENT one holds the
     // windows, and the channel buffer beside it the C covariances of each.
     const size_t C = h->chan ? (size_t)h->cshape.C : 1;
@@ -897,6 +922,7 @@ int ensure_slot(music_b200 *h, Workspace &ws, uint32_t windows, const Plan &p)
     if (const int rc = grow(ws.n0, p.integ ? 1 : 0)) return rc;
     if (const int rc = grow(ws.std, p.ws_std ? w * (h->azel ? 3 : 1) * h->n : 0)) return rc;
     if (const int rc = grow(ws.X, p.wsf ? w * mm : 0)) return rc;
+    if (const int rc = grow(ws.Rin, h->coarray ? w * h->m_in * h->m_in * 2 : 0)) return rc;
     return grow(ws.wts, p.ws_wts ? w * h->n * h->m * 2 : 0);
 }
 
@@ -1040,10 +1066,10 @@ unsigned *ticket_counter(music_b200 *h, int slot, cudaStream_t st)
     return h->work_ctr + 2 * ((size_t)slot * CTR_RING + e);
 }
 
-// K1: covariance of W windows into ws.R, on `st`.
+// K1: covariance of W windows of m_in elements into ws.R, on `st`.
 void launch_cov(music_b200 *h, const WsView &ws, const float *d_in, uint32_t W, cudaStream_t st, int ctr_slot)
 {
-    const int M = (int)h->m, N = (int)h->N;
+    const int M = (int)h->m_in, N = (int)h->N;
     if (M == 4) {
         // persistent, one CTA per SM, per-warp TMA ring (see cov4_tma_kernel)
         const int grid = std::min<int>(h->sm_count, (int)((W + COV_WARPS - 1) / COV_WARPS));
@@ -1348,7 +1374,7 @@ int launch_eig_scan(music_b200 *h, const Plan &p, const WsView &ws, uint32_t W, 
 void launch_cov_planar(music_b200 *h, const WsView &ws, const PlanarStreams &S, unsigned long long first_snapshot,
                        unsigned hop, uint32_t W, cudaStream_t st)
 {
-    const int M = (int)h->m, N = (int)h->N, T = (M + 3) / 4, wpb = 8;
+    const int M = (int)h->m_in, N = (int)h->N, T = (M + 3) / 4, wpb = 8;
     cov_planar_kernel<false><<<(unsigned)(((long long)W * T + wpb - 1) / wpb), wpb * 32, 0, st>>>(S, first_snapshot, hop, ws.R, (int)W, N, M);
     h->launches++;
     if (T > 1) {
@@ -1363,7 +1389,7 @@ void launch_cov_planar(music_b200 *h, const WsView &ws, const PlanarStreams &S, 
 // order within a call (the host entries' chunks alternate between two streams) and call order across calls.
 int launch_integrate(music_b200 *h, const WsView &ws, uint32_t W, cudaStream_t st)
 {
-    const int E = (int)(2 * h->m * h->m), ntiles = (int)((W + INTEG_T - 1) / INTEG_T);
+    const int E = (int)(2 * h->m_in * h->m_in), ntiles = (int)((W + INTEG_T - 1) / INTEG_T);
     const size_t elems = (size_t)ntiles * E;
     if (elems > h->integ_tiles.size()) {
         if (h->integ_used) CU(h, cudaEventSynchronize(h->integ_done));  // the last integration may still read the scratch
@@ -1484,22 +1510,32 @@ int enqueue_device(music_b200 *h, const float *d_in, uint32_t nwindows, const Ou
     if (rc) return rc;
     if (ws.used) CU(h, cudaStreamWaitEvent(st, ws.scan_done, 0));  // the slot's last user may have run on another stream
     const WsView v = ws.view();
+    // the input side (covariance, calibration, integration) works on the m_in elements of a snapshot: on a co-array
+    // handle in the slot's physical-R buffer, which coarray_kernel then maps into the workspace R
+    WsView vin = v;
+    if (h->coarray) vin.R = ws.Rin;
     for (uint32_t w0 = 0; w0 < nwindows; w0 += sub) {
         const uint32_t W = std::min(sub, nwindows - w0);
         cudaEvent_t *tev = timing_events(h);
         if (tev) cudaEventRecord(tev[0], st);
-        if (planar) launch_cov_planar(h, v, *planar, (unsigned long long)w0 * hop, hop, W, st);
-        else launch_cov(h, v, d_in + (size_t)w0 * h->nsamples * 2, W, st, slot);
+        if (planar) launch_cov_planar(h, vin, *planar, (unsigned long long)w0 * hop, hop, W, st);
+        else launch_cov(h, vin, d_in + (size_t)w0 * h->nsamples * 2, W, st, slot);
         if (plan.calib) {
             // the receiver correction of R, inside the covariance slot of the stage timing
-            const size_t e = (size_t)W * h->m * h->m;
-            calib_apply_kernel<<<(unsigned)((e + CALIB_THREADS - 1) / CALIB_THREADS), CALIB_THREADS, 0, st>>>(v.R, (int)h->m, (int)W, h->cal_c);
+            const size_t e = (size_t)W * h->m_in * h->m_in;
+            calib_apply_kernel<<<(unsigned)((e + CALIB_THREADS - 1) / CALIB_THREADS), CALIB_THREADS, 0, st>>>(vin.R, (int)h->m_in, (int)W, h->cal_c);
             h->launches++;
         }
         if (plan.integ) {
             // the integration across windows, also inside the covariance slot
-            rc = launch_integrate(h, v, W, st);
+            rc = launch_integrate(h, vin, W, st);
             if (rc) return rc;
+        }
+        if (h->coarray) {
+            // R_ss of the virtual array into the workspace R, inside the covariance slot
+            coarray_kernel<<<(W + CO_WARPS - 1) / CO_WARPS, CO_WARPS * 32, 0, st>>>(reinterpret_cast<const double2 *>(vin.R), (int)h->m_in,
+                                                                                (int)W, h->co_lags, reinterpret_cast<double2 *>(v.R));
+            h->launches++;
         }
         if (tev) cudaEventRecord(tev[1], st);
         rc = launch_eig_scan(h, plan, v, W, out.at(w0), table(h), h->N, st, tev,
@@ -1627,6 +1663,24 @@ struct NvtxRange {  // SURVEY.md section 5 tracing hook: ranges show up in nsys 
     explicit NvtxRange(const char *name) { nvtxRangePushA(name); }
     ~NvtxRange() { nvtxRangePop(); }
 };
+
+// Drops every range of ours that overlaps [ptr, ptr + bytes) without holding all of it.  A registration covers whole
+// pages, so it can take in the first or last page of a neighbouring buffer; the driver refuses a copy from or to memory
+// that is registered only in part, so a caller range a copy touches must lie inside one registration or outside all.
+void release_straddling(music_b200 *h, const void *ptr, size_t bytes)
+{
+    if (!ptr || bytes == 0) return;
+    const uintptr_t a = reinterpret_cast<uintptr_t>(ptr), e = a + bytes;
+    for (size_t i = 0; i < h->hostregs.size();) {
+        const music_b200::HostReg &g = h->hostregs[i];
+        if (g.base < e && a < g.base + g.len && !(g.base <= a && e <= g.base + g.len)) {
+            cudaHostUnregister(reinterpret_cast<void *>(g.base));
+            h->hostregs.erase(h->hostregs.begin() + i);
+        } else {
+            ++i;
+        }
+    }
+}
 
 // Makes [ptr, ptr + bytes) DMA-able if it is ordinary pageable memory: page-aligned cudaHostRegister, remembered in
 // the handle (at most 16 ranges, oldest evicted).  Memory that is already pinned (cudaHostAlloc, registered by the
@@ -1845,7 +1899,7 @@ int stage_host(music_b200 *h, const HostInput &in, uint32_t nwindows, const Outp
                 NvtxRange r("music_b200: H2D");
                 if (in.streams) {
                     const size_t seg = (size_t)(W - 1) * in.hop + N;  // snapshots of each stream this chunk touches
-                    for (uint32_t a = 0; a < h->m && rc == MUSIC_B200_OK; ++a) {
+                    for (uint32_t a = 0; a < h->m_in && rc == MUSIC_B200_OK; ++a) {
                         float *d = sl.in + (size_t)a * seg * 2;
                         CU_BREAK(h, rc, cudaMemcpyAsync(d, in.streams[a] + (size_t)i0 * in.hop * 2, seg * 2 * sizeof(float), cudaMemcpyHostToDevice, st));
                         S.p[a] = reinterpret_cast<const float2 *>(d);
@@ -1938,7 +1992,7 @@ int alloc_slot(music_b200 *h, TableSlot &s)
     const size_t C = h->chan ? (size_t)h->cshape.C : 1, c64 = (size_t)h->K * h->m * 2, soa = soa_doubles(h->K, h->m);
     CU(h, s.c64.grow(C * c64));
     CU(h, s.soa.grow(C * soa));
-    if (h->m == 4 && !h->azel && !h->chan) {  // the fused M = 4 kernel's screen layout; no other handle runs that kernel
+    if (h->m == 4 && !h->azel && !h->chan && !h->coarray) {  // the fused M = 4 kernel's screen layout; no other handle runs that kernel
         CU(h, s.fz.grow(fused_table_bytes((int)h->K)));
         CU(h, s.na_max.grow(1));
     }
@@ -1982,8 +2036,16 @@ int check_create(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples)
     return MUSIC_B200_OK;
 }
 
+// The settings music_b200_create_coarray() checked: the physical element count, the lag table and the first virtual table
+struct CoarrayDef {
+    uint32_t m_in;
+    CoarrayLags lags;
+    double pos[2 * MAXM];  // the virtual ULA l s, l < Mv
+    double lambda;
+};
+
 int create_on_device(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples, uint32_t resolution, const float *table_c64,
-                     int device, const AzelGeom *azel, const music_b200 *chan = nullptr)
+                     int device, const AzelGeom *azel, const music_b200 *chan = nullptr, const CoarrayDef *co = nullptr)
 {
     int ndev = 0;
     cudaError_t e = cudaGetDeviceCount(&ndev);
@@ -1998,8 +2060,14 @@ int create_on_device(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples
 
     music_b200 *h = new (std::nothrow) music_b200();
     if (!h) return fail(nullptr, MUSIC_B200_ENOMEM, "out of host memory");
-    h->m = m; h->n = n; h->nsamples = nsamples; h->K = resolution; h->N = nsamples / m;
+    h->m = m; h->n = n; h->nsamples = nsamples; h->K = resolution;
+    h->m_in = co ? co->m_in : m;
+    h->N = nsamples / h->m_in;
     h->device = device; h->sm_count = prop.multiProcessorCount;
+    if (co) {
+        h->coarray = true;
+        h->co_lags = co->lags;
+    }
     if (azel) {
         h->azel = true;
         h->grid = azel->grid;
@@ -2059,6 +2127,7 @@ int create_on_device(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples
         if (chan) return init_channels(h);  // a channel handle takes its first tables at its first retune
         if (const int rc = alloc_slot(h, h->tables[0])) return rc;
         DeviceTable &t = h->tables[0].tabs[0];
+        if (co) return build_table(h, t, co->pos, co->lambda, h->streams[0]);
         return azel ? build_table_azel(h, t, azel->pos, azel->lambda, h->streams[0]) : upload_table(h, t, table_c64, h->streams[0]);
     };
     rc = init();
@@ -2170,6 +2239,7 @@ int music_b200_set_table(music_b200 *h, const float *table_c64)
 {
     if (!h) return MUSIC_B200_EINVAL;
     if (!table_c64) return fail(h, MUSIC_B200_EINVAL, "array response table must not be NULL");
+    if (const int rc = refuse_coarray(h, "set_table (the virtual table is set by music_b200_set_geometry_coarray)")) return rc;
     std::lock_guard<std::mutex> g(h->mutex);
     if (!h->kids.empty())  // multi-device handle: every device holds a full copy of the table (SURVEY.md section 8e)
         return for_each_child(h, [&](music_b200 *c) { return music_b200_set_table(c, table_c64); });
@@ -2194,7 +2264,7 @@ int music_b200_process_planar_device(music_b200 *h, const float *const *d_stream
     if (!d_streams) return fail(h, MUSIC_B200_EINVAL, "d_streams must not be NULL");
     if (hop == 0) return fail(h, MUSIC_B200_EINVAL, "hop must be >= 1 snapshot");
     PlanarStreams S = {};
-    for (uint32_t r = 0; r < h->m; ++r) {
+    for (uint32_t r = 0; r < h->m_in; ++r) {
         if (!d_streams[r] || (reinterpret_cast<uintptr_t>(d_streams[r]) & 7u) != 0)
             return fail(h, MUSIC_B200_EINVAL, "antenna stream %u must be a non-NULL, 8-byte aligned device pointer", r);
         S.p[r] = reinterpret_cast<const float2 *>(d_streams[r]);
@@ -2208,6 +2278,7 @@ int music_b200_process_planar_device(music_b200 *h, const float *const *d_stream
 int music_b200_process_planar_host(music_b200 *h, const float *const *streams, uint32_t hop, uint32_t nwindows,
                                    float *angles, float *levels, float *spectrum, int32_t *bins)
 {
+    music_b200 *const top = h;  // the handle process_host registers caller memory on
     h = served(h);
     if (!h) return MUSIC_B200_EINVAL;
     if (h->azel) return fail(h, MUSIC_B200_EINVAL, "planar input is not supported on an az-el handle");
@@ -2215,9 +2286,20 @@ int music_b200_process_planar_host(music_b200 *h, const float *const *streams, u
     if (nwindows == 0) return MUSIC_B200_OK;
     if (!streams || !angles) return fail(h, MUSIC_B200_EINVAL, "streams and angles must not be NULL");
     if (hop == 0) return fail(h, MUSIC_B200_EINVAL, "hop must be >= 1 snapshot");
-    for (uint32_t r = 0; r < h->m; ++r)
+    for (uint32_t r = 0; r < h->m_in; ++r)
         if (!streams[r]) return fail(h, MUSIC_B200_EINVAL, "antenna stream %u must not be NULL", r);
+    // the chunk copies read the streams (and write the spectrum) straight from and to caller memory
+    const auto release = [&](music_b200 *owner) {
+        const size_t stream_bytes = ((size_t)(nwindows - 1) * hop + h->N) * 2 * sizeof(float);
+        for (uint32_t r = 0; r < h->m_in; ++r) release_straddling(owner, streams[r], stream_bytes);
+        if (spectrum) release_straddling(owner, spectrum, (size_t)nwindows * h->K * sizeof(float));
+    };
+    if (top != h) {
+        std::lock_guard<std::mutex> gt(top->mutex);
+        release(top);
+    }
     std::lock_guard<std::mutex> g(h->mutex);
+    if (top == h) release(h);
     CU(h, cudaSetDevice(h->device));
     HostInput in;
     in.streams = streams;
@@ -2332,6 +2414,7 @@ int music_b200_set_geometry(music_b200 *h, const double *positions_xy, double wa
     if (!h) return MUSIC_B200_EINVAL;
     if (h->azel) return fail(h, MUSIC_B200_EINVAL, "an az-el handle takes music_b200_set_geometry_azel()");
     if (h->chan) return fail(h, MUSIC_B200_EINVAL, "a channel handle takes music_b200_set_geometry_channels()");
+    if (h->coarray) return fail(h, MUSIC_B200_EINVAL, "a co-array handle takes music_b200_set_geometry_coarray()");
     if (!positions_xy) return fail(h, MUSIC_B200_EINVAL, "element positions must not be NULL");
     if (!(wavelength > 0.0) || !std::isfinite(wavelength)) return fail(h, MUSIC_B200_EINVAL, "wavelength must be positive and finite");
     for (uint32_t i = 0; i < 2 * h->m; ++i)
@@ -2431,8 +2514,12 @@ int process_host_impl(music_b200 *h, const float *in_c64, uint32_t nwindows, Out
     NvtxRange range("music_b200_process_host");
     // pageable caller memory (GNU Radio's circular buffers, numpy arrays) is pinned once and found again on later calls
     CU(h, cudaSetDevice(served(h)->device));
-    host_register(h, in_c64, (size_t)nwindows * h->nsamples * 2 * sizeof(float), true);
-    if (dst.spec) host_register(h, dst.spec, (size_t)nwindows * h->K * sizeof(float), false);
+    const size_t in_bytes = (size_t)nwindows * h->nsamples * 2 * sizeof(float), spec_bytes = (size_t)nwindows * h->K * sizeof(float);
+    host_register(h, in_c64, in_bytes, true);
+    if (dst.spec) host_register(h, dst.spec, spec_bytes, false);
+    // the two ranges the chunk copies touch directly, after both registrations (one may have dropped the other)
+    release_straddling(h, in_c64, in_bytes);
+    if (dst.spec) release_straddling(h, dst.spec, spec_bytes);
     HostInput in;
     in.windows = in_c64;
     return stage_host(h, in, nwindows, dst.shaped(h));
@@ -2487,6 +2574,7 @@ namespace {
 // the checks every beams entry point makes before it runs: a beamformer set, an output asked for, the alignment
 int check_beams_call(music_b200 *h, const void *weights, const void *beams)
 {
+    if (const int rc = refuse_coarray(h, "the beams entry")) return rc;
     if (h->beam_rule == MUSIC_B200_BEAMS_OFF)
         return fail(h, MUSIC_B200_EINVAL, "no beamformer set (call music_b200_set_beamformer() with DAS, MVDR or LCMV)");
     if (!weights && !beams) return fail(h, MUSIC_B200_EINVAL, "weights and beams must not both be NULL");
@@ -2502,6 +2590,8 @@ int music_b200_set_beamformer(music_b200 *h, int rule, double loading)
     if (!h) return MUSIC_B200_EINVAL;
     if (h->azel) return fail(h, MUSIC_B200_EINVAL, "the beamformer is not supported on an az-el handle");
     if (h->chan) return fail(h, MUSIC_B200_EINVAL, "wideband beams are not built: a channel handle takes no beamformer");
+    if (rule != MUSIC_B200_BEAMS_OFF)
+        if (const int rc = refuse_coarray(h, "the beamformer")) return rc;
     if (rule != MUSIC_B200_BEAMS_OFF && rule != MUSIC_B200_BEAMS_DAS && rule != MUSIC_B200_BEAMS_MVDR && rule != MUSIC_B200_BEAMS_LCMV)
         return fail(h, MUSIC_B200_EINVAL, "unknown beamformer %d", rule);
     if (!std::isfinite(loading) || loading < 0.0) return fail(h, MUSIC_B200_EINVAL, "loading must be finite and >= 0 (got %g)", loading);
@@ -2548,6 +2638,7 @@ namespace {
 // the call asks for weights or beams
 int check_crb_call(music_b200 *h, const void *out, const void *weights, const void *beams)
 {
+    if (const int rc = refuse_coarray(h, "the CRB")) return rc;
     if (!out) return fail(h, MUSIC_B200_EINVAL, "the CRB output must not be NULL");
     if ((reinterpret_cast<uintptr_t>(out) & 3u) != 0) return fail(h, MUSIC_B200_EINVAL, "the CRB output must be 4-byte aligned");
     if (weights || beams) return check_beams_call(h, weights, beams);
@@ -2597,6 +2688,8 @@ int check_track_call(music_b200 *h, const void *std, const void *weights, const 
         return fail(h, MUSIC_B200_EINVAL, "tracking is off (call music_b200_set_tracking() with FIXED or CRB variance)");
     if (!slot_track) return fail(h, MUSIC_B200_EINVAL, "slot_track must not be NULL");
     if (!track_ids != !track_state) return fail(h, MUSIC_B200_EINVAL, "track_ids and track_state are given both or neither");
+    if (std)
+        if (const int rc = refuse_coarray(h, "the CRB")) return rc;
     for (const void *q : {(const void *)slot_track, (const void *)track_ids, (const void *)track_state, std})
         if ((reinterpret_cast<uintptr_t>(q) & 3u) != 0) return fail(h, MUSIC_B200_EINVAL, "the tracker outputs and the CRB must be 4-byte aligned");
     if (weights || beams) return check_beams_call(h, weights, beams);
@@ -2650,7 +2743,7 @@ int music_b200_set_calibration(music_b200 *h, const double *gains)
     if (h->chan) return fail(h, MUSIC_B200_EINVAL, "per-channel calibration is not built: a channel handle takes no calibration");
     CalibVec cv = {};
     if (gains) {
-        for (uint32_t m = 0; m < h->m; ++m) {
+        for (uint32_t m = 0; m < h->m_in; ++m) {
             const double gr = gains[2 * m], gi = gains[2 * m + 1];
             if (!std::isfinite(gr) || !std::isfinite(gi)) return fail(h, MUSIC_B200_EINVAL, "gain %u is not finite", m);
             // c = 1 / g = conj(g) / |g|^2 in fp64
@@ -2665,7 +2758,7 @@ int music_b200_set_calibration(music_b200 *h, const double *gains)
     h->calib = gains != nullptr;
     h->cal_c = cv;
     h->integ_fresh = true;  // the carry is kept in corrected coordinates
-    for (uint32_t i = 0; i < 2 * h->m; ++i) h->cal_g[i] = gains ? gains[i] : (i % 2 == 0 ? 1.0 : 0.0);
+    for (uint32_t i = 0; i < 2 * h->m_in; ++i) h->cal_g[i] = gains ? gains[i] : (i % 2 == 0 ? 1.0 : 0.0);
     return MUSIC_B200_OK;
 }
 
@@ -2674,7 +2767,7 @@ int music_b200_get_calibration(music_b200 *h, double *gains)
     if (!h) return MUSIC_B200_EINVAL;
     if (!gains) return fail(h, MUSIC_B200_EINVAL, "gains must not be NULL");
     std::lock_guard<std::mutex> g(h->mutex);
-    for (uint32_t i = 0; i < 2 * h->m; ++i) gains[i] = h->calib ? h->cal_g[i] : (i % 2 == 0 ? 1.0 : 0.0);
+    for (uint32_t i = 0; i < 2 * h->m_in; ++i) gains[i] = h->calib ? h->cal_g[i] : (i % 2 == 0 ? 1.0 : 0.0);
     return MUSIC_B200_OK;
 }
 
@@ -2709,7 +2802,7 @@ int music_b200_set_integration(music_b200 *h, double alpha)
     if (const int rc = check_integration(h)) return rc;
     if (alpha > 0.0 && !h->integ_done) {
         CU(h, cudaSetDevice(h->device));
-        CU(h, h->integ_S.grow(2 * (size_t)h->m * h->m));
+        CU(h, h->integ_S.grow(2 * (size_t)h->m_in * h->m_in));
         CU(h, h->integ_cnt.grow(1));
         CU(h, cudaEventCreateWithFlags(&h->integ_done, cudaEventDisableTiming));
     }
@@ -2770,6 +2863,8 @@ int music_b200_set_tracking(music_b200 *h, int variance, double q, double rate_s
         return fail(h, MUSIC_B200_EINVAL, "max_tracks must be in 1..%d (got %u)", MUSIC_B200_TRACK_MAX_ROWS, max_tracks);
     std::lock_guard<std::mutex> g(h->mutex);
     if (const int rc = check_tracking(h)) return rc;
+    if (variance == MUSIC_B200_TRACK_CRB)
+        if (const int rc = refuse_coarray(h, "tracking under CRB variance")) return rc;
     if (variance == MUSIC_B200_TRACK_CRB && !table(h).geometric)
         return fail(h, MUSIC_B200_EINVAL, "CRB variance needs a table built by music_b200_set_geometry%s(); the current one came "
                                           "from set_table(), which has no geometry", h->azel ? "_azel" : "");
@@ -2879,6 +2974,7 @@ int music_b200_calib_reset(music_b200 *h)
     h = served(h);
     if (!h) return MUSIC_B200_EINVAL;
     if (h->chan) return fail(h, MUSIC_B200_EINVAL, "per-channel calibration is not built: a channel handle takes no calibration");
+    if (const int rc = refuse_coarray(h, "calibration estimation (estimate the gains on a plain handle, then set_calibration)")) return rc;
     std::lock_guard<std::mutex> g(h->mutex);
     CU(h, cudaSetDevice(h->device));
     if (const int rc = ensure_calib_buffers(h)) return rc;
@@ -2894,6 +2990,7 @@ int music_b200_calib_accumulate_device(music_b200 *h, const float *d_in_c64, uin
     h = served(h);
     if (!h) return MUSIC_B200_EINVAL;
     if (h->chan) return fail(h, MUSIC_B200_EINVAL, "per-channel calibration is not built: a channel handle takes no calibration");
+    if (const int rc = refuse_coarray(h, "calibration estimation (estimate the gains on a plain handle, then set_calibration)")) return rc;
     if (nwindows == 0) return MUSIC_B200_OK;
     if (!d_in_c64) return fail(h, MUSIC_B200_EINVAL, "d_in_c64 must not be NULL");
     if ((reinterpret_cast<uintptr_t>(d_in_c64) & 15u) != 0) return fail(h, MUSIC_B200_EINVAL, "d_in_c64 must be 16-byte aligned");
@@ -2907,6 +3004,7 @@ int music_b200_calib_accumulate_host(music_b200 *h, const float *in_c64, uint32_
     h = served(h);
     if (!h) return MUSIC_B200_EINVAL;
     if (h->chan) return fail(h, MUSIC_B200_EINVAL, "per-channel calibration is not built: a channel handle takes no calibration");
+    if (const int rc = refuse_coarray(h, "calibration estimation (estimate the gains on a plain handle, then set_calibration)")) return rc;
     if (nwindows == 0) return MUSIC_B200_OK;
     if (!in_c64) return fail(h, MUSIC_B200_EINVAL, "in_c64 must not be NULL");
     std::lock_guard<std::mutex> g(h->mutex);
@@ -2939,6 +3037,7 @@ int music_b200_calib_solve(music_b200 *h, double az_deg, double el_deg, int kind
     h = served(h);
     if (!h) return MUSIC_B200_EINVAL;
     if (h->chan) return fail(h, MUSIC_B200_EINVAL, "per-channel calibration is not built: a channel handle takes no calibration");
+    if (const int rc = refuse_coarray(h, "calibration estimation (estimate the gains on a plain handle, then set_calibration)")) return rc;
     if (!gains) return fail(h, MUSIC_B200_EINVAL, "gains must not be NULL");
     if (kind != MUSIC_B200_CALIB_PHASE && kind != MUSIC_B200_CALIB_GAIN_PHASE) return fail(h, MUSIC_B200_EINVAL, "unknown calibration kind %d", kind);
     if (kind == MUSIC_B200_CALIB_GAIN_PHASE && h->m < 3)
@@ -2993,6 +3092,7 @@ namespace {
 int check_blind_handle(music_b200 *h)
 {
     if (h->chan) return fail(h, MUSIC_B200_EINVAL, "self-calibration is not built for channel handles");
+    if (const int rc = refuse_coarray(h, "self-calibration (estimate the gains on a plain handle, then set_calibration)")) return rc;
     if (h->azel) return fail(h, MUSIC_B200_EINVAL, "self-calibration is not built for az-el handles");
     return MUSIC_B200_OK;
 }
@@ -3240,6 +3340,9 @@ int music_b200_set_source_rule(music_b200 *h, int rule)
     if (!h) return MUSIC_B200_EINVAL;
     if (rule != MUSIC_B200_SOURCES_FIXED && rule != MUSIC_B200_SOURCES_MDL && rule != MUSIC_B200_SOURCES_AIC)
         return fail(h, MUSIC_B200_EINVAL, "unknown source rule %d", rule);
+    if (rule != MUSIC_B200_SOURCES_FIXED && h->coarray)
+        return fail(h, MUSIC_B200_EINVAL, "a co-array handle takes the FIXED source rule only (the eigenvalues of R_ss are squares: "
+                                          "MDL and AIC do not apply)");
     if (rule != MUSIC_B200_SOURCES_FIXED && snapshots(h) <= h->m)
         return fail(h, MUSIC_B200_EINVAL, "MDL / AIC need more snapshots than antennas (N = %u, m = %u)", snapshots(h), h->m);
     if (rule != MUSIC_B200_SOURCES_FIXED && h->chan && h->chan_combine == MUSIC_B200_CHANNELS_INCOHERENT)
@@ -3300,7 +3403,7 @@ int music_b200_create_multi(music_b200 **out, uint32_t m, uint32_t n, uint32_t n
             if (devices[i] == devices[j]) return fail(nullptr, MUSIC_B200_EINVAL, "device %d listed twice", devices[i]);
     music_b200 *h = new (std::nothrow) music_b200();
     if (!h) return fail(nullptr, MUSIC_B200_ENOMEM, "out of host memory");
-    h->m = m; h->n = n; h->nsamples = nsamples; h->K = resolution; h->N = m ? nsamples / m : 0;
+    h->m = m; h->m_in = m; h->n = n; h->nsamples = nsamples; h->K = resolution; h->N = m ? nsamples / m : 0;
     h->device = devices[0];
     if (const char *e = getenv("MUSIC_B200_HOSTREG")) h->hostreg = atoi(e) != 0;
     for (int i = 0; i < ndev; ++i) {
@@ -3337,6 +3440,7 @@ int music_b200_gather_create(music_b200 *h, uint32_t total_windows, unsigned cha
     if (!h->kids.empty()) return fail(h, MUSIC_B200_EINVAL, "gather_create applies to single-device handles (a multi-device handle gathers in process_device_sharded)");
     if (h->azel) return fail(h, MUSIC_B200_EINVAL, "the bins all-gather is not supported on an az-el handle");
     if (h->chan) return fail(h, MUSIC_B200_EINVAL, "the bins all-gather is not built for channel handles");
+    if (const int rc = refuse_coarray(h, "the bins all-gather")) return rc;
     std::lock_guard<std::mutex> g(h->mutex);
     CU(h, cudaSetDevice(h->device));
     if (h->gather_buf) return fail(h, MUSIC_B200_EINVAL, "gather buffer already created");
@@ -3369,6 +3473,7 @@ int music_b200_gather_attach(music_b200 *h, int nranks, int rank, const unsigned
     if (nranks < 1 || nranks > MAX_PEERS || rank < 0 || rank >= nranks) return fail(h, MUSIC_B200_EINVAL, "need 1 <= nranks <= %d and 0 <= rank < nranks", MAX_PEERS);
     if (h->azel) return fail(h, MUSIC_B200_EINVAL, "the bins all-gather is not supported on an az-el handle");
     if (h->chan) return fail(h, MUSIC_B200_EINVAL, "the bins all-gather is not built for channel handles");
+    if (const int rc = refuse_coarray(h, "the bins all-gather")) return rc;
     std::lock_guard<std::mutex> g(h->mutex);
     if (!h->gather_buf) return fail(h, MUSIC_B200_EINVAL, "call gather_create first");
     CU(h, cudaSetDevice(h->device));
@@ -3859,6 +3964,99 @@ int music_b200_process_channels_host(music_b200 *h, const float *in_c64, uint32_
     const cudaError_t e = cudaStreamSynchronize(st);
     if (rc == MUSIC_B200_OK && e != cudaSuccess) rc = fail(h, MUSIC_B200_ECUDA, "stream sync failed: %s", cudaGetErrorString(e));
     return rc;
+}
+
+/* ---- sparse linear arrays through the difference co-array (music_coarray.cuh) ---- */
+namespace {
+
+// the step vector and wavelength of a co-array handle: finite, wavelength > 0, 0 < |s| <= (wavelength / 2)(1 + 1e-12)
+int check_coarray_step(music_b200 *h, const double *step_xy, double wavelength)
+{
+    if (!step_xy) return fail(h, MUSIC_B200_EINVAL, "step_xy must not be NULL");
+    if (!(wavelength > 0.0) || !std::isfinite(wavelength)) return fail(h, MUSIC_B200_EINVAL, "wavelength must be positive and finite");
+    if (!std::isfinite(step_xy[0]) || !std::isfinite(step_xy[1])) return fail(h, MUSIC_B200_EINVAL, "the step must be finite");
+    const double s = std::hypot(step_xy[0], step_xy[1]);
+    if (!(s > 0.0) || s > 0.5 * wavelength * (1.0 + 1e-12))
+        return fail(h, MUSIC_B200_EINVAL, "need 0 < |step| <= wavelength / 2 (got |step| = %g, wavelength = %g)", s, wavelength);
+    return MUSIC_B200_OK;
+}
+
+// the virtual ULA: element l at l s, l < mv
+void coarray_positions(const double *step_xy, uint32_t mv, double *pos)
+{
+    for (uint32_t l = 0; l < mv; ++l) {
+        pos[2 * l] = (double)l * step_xy[0];
+        pos[2 * l + 1] = (double)l * step_xy[1];
+    }
+}
+
+}  // namespace
+
+int music_b200_create_coarray(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples, uint32_t resolution, const int32_t *positions,
+                              const double step_xy[2], double wavelength, uint32_t mv, int device)
+{
+    if (!out) return fail(nullptr, MUSIC_B200_EINVAL, "out must not be NULL");
+    *out = nullptr;
+    if (m < 2 || m > MUSIC_B200_MAX_M) return fail(nullptr, MUSIC_B200_EINVAL, "a co-array handle needs 2 <= m <= %d (got %u)", MUSIC_B200_MAX_M, m);
+    if (!positions) return fail(nullptr, MUSIC_B200_EINVAL, "positions must not be NULL");
+    if (positions[0] != 0) return fail(nullptr, MUSIC_B200_EINVAL, "positions must start at p_0 = 0 (got %d)", positions[0]);
+    for (uint32_t i = 1; i < m; ++i)
+        if (positions[i] <= positions[i - 1]) return fail(nullptr, MUSIC_B200_EINVAL, "positions must be strictly ascending (p_%u = %d)", i, positions[i]);
+    if (nsamples == 0 || nsamples % m != 0) return fail(nullptr, MUSIC_B200_EINVAL, "nsamples must be a positive multiple of m (got %u)", nsamples);
+    if (resolution == 0) return fail(nullptr, MUSIC_B200_EINVAL, "resolution must be > 0");
+    if (const int rc = check_coarray_step(nullptr, step_xy, wavelength)) return rc;
+    // the hole-free extent U, counted up to MAXM + 1: only min(U, MAXM) matters
+    bool has[MAXM + 1] = {};
+    for (uint32_t i = 0; i < m; ++i)
+        for (uint32_t j = 0; j <= i; ++j) {
+            const long long d = (long long)positions[i] - positions[j];
+            if (d <= MAXM) has[d] = true;
+        }
+    uint32_t U = 0;
+    while (U <= (uint32_t)MAXM && has[U]) ++U;
+    const uint32_t cap = std::min<uint32_t>(U, MAXM);
+    if (mv == 0) mv = cap;
+    if (mv < 2 || mv > cap)
+        return fail(nullptr, MUSIC_B200_EINVAL, "need 2 <= mv <= min(U, %d) = %u, U the hole-free extent of the lags (got mv = %u)", MAXM, cap, mv);
+    if (n == 0 || n >= mv) return fail(nullptr, MUSIC_B200_EINVAL, "need 1 <= n < mv (got n=%u, mv=%u)", n, mv);
+    CoarrayDef co = {};
+    co.m_in = m;
+    co.lambda = wavelength;
+    co.lags.mv = (int)mv;
+    int q = 0;
+    for (uint32_t l = 0; l < mv; ++l) {
+        co.lags.start[l] = (unsigned char)q;
+        for (uint32_t i = 0; i < m; ++i)
+            for (uint32_t j = 0; j <= i; ++j)
+                if ((long long)positions[i] - positions[j] == (long long)l) {
+                    co.lags.pi[q] = (unsigned char)i;
+                    co.lags.pj[q] = (unsigned char)j;
+                    ++q;
+                }
+    }
+    co.lags.start[mv] = (unsigned char)q;
+    coarray_positions(step_xy, mv, co.pos);
+    return create_on_device(out, mv, n, nsamples, resolution, nullptr, device, nullptr, nullptr, &co);
+}
+
+int music_b200_set_geometry_coarray(music_b200 *h, const double step_xy[2], double wavelength)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (!h->coarray) return fail(h, MUSIC_B200_EINVAL, "set_geometry_coarray needs a handle from music_b200_create_coarray");
+    if (const int rc = check_coarray_step(h, step_xy, wavelength)) return rc;
+    double pos[2 * MAXM];
+    coarray_positions(step_xy, h->m, pos);
+    std::lock_guard<std::mutex> g(h->mutex);
+    return retune(h, [&](TableSlot &s) { return build_table(h, s.tabs[0], pos, wavelength, h->streams[0]); });
+}
+
+int music_b200_coarray_size(music_b200 *h, uint32_t *mv)
+{
+    if (!h) return MUSIC_B200_EINVAL;
+    if (!h->coarray) return fail(h, MUSIC_B200_EINVAL, "coarray_size needs a handle from music_b200_create_coarray");
+    if (!mv) return fail(h, MUSIC_B200_EINVAL, "mv must not be NULL");
+    *mv = h->m;
+    return MUSIC_B200_OK;
 }
 
 void music_b200_destroy(music_b200 *h)

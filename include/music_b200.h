@@ -1088,6 +1088,55 @@ int music_b200_process_channels_device(music_b200 *h, const float *d_in_c64, uin
 int music_b200_process_channels_host(music_b200 *h, const float *in_c64, uint32_t nwindows, float *angles, float *levels,
                                      float *spectrum, int32_t *bins, int32_t *counts, double *R);
 
+/*
+ * Sparse linear arrays through the difference co-array (music_coarray.cuh; Moffet 1968, Pillai, Bar-Ness & Haber 1985,
+ * Pal & Vaidyanathan 2010, Vaidyanathan & Pal 2011, Liu & Vaidyanathan 2015): up to Mv - 1 uncorrelated sources from
+ * m < Mv antennas.  Restated literally by tests/coarray_oracle.py.
+ *   inputs     m physical elements (2 <= m <= MUSIC_B200_MAX_M) at integer positions p_0 = 0 < p_1 < ... < p_{m-1} in
+ *              units of the step s = (s_x, s_y) metres (finite, 0 < |s| <= (lambda / 2)(1 + 1e-12)), the wavelength lambda
+ *              (finite, > 0) and the virtual size Mv.  Each input snapshot holds the m physical channels, nsamples a
+ *              positive multiple of m, N = nsamples / m snapshots per window.
+ *   extent     U = the largest value with every lag 0 .. U - 1 some p_i - p_j.  2 <= Mv <= min(U, 16); mv = 0 chooses
+ *              min(U, 16) (music_b200_coarray_size() reads it back).  E.g. the nested array {0, 1, 2, 3, 4, 9, 14, 19} has
+ *              U = 20 and runs with Mv = 16.  1 <= n < Mv: n may exceed m.
+ *   lag table  for l = 0 .. Mv - 1 the pairs (i, j) with p_i - p_j = l in ascending i, c_l of them (built at create).
+ *   per window R = the window's fp64 covariance of the m physical channels, after calibration and integration exactly as
+ *              on a 1-D handle (both act on the physical R, before the mapping: the mapping is not linear, so an
+ *              integrated co-array covariance is the map of the integrated R, not an average of maps);
+ *              z_l = (1 / c_l) sum R_ij over the lag-l pairs in table order;
+ *              T_ab = z_{a-b} for a >= b, conj(z_{b-a}) for a < b (Hermitian Toeplitz, Mv x Mv);
+ *              R_ss = (1 / Mv) T T^H, each entry a sum over k ascending, computed for a >= b, the upper triangle its
+ *              conjugate mirror, the diagonal real.  R_ss (= T^2 / Mv) has T's eigenvectors and is positive semi-definite,
+ *              so the ascending eigensolver puts the noise subspace first even where a finite-sample T is indefinite.
+ *   problem    R_ss is the window's R for every later stage and for the R and eigenvalue outputs of
+ *              music_b200_process_device_ex ([W][Mv][Mv] and [W][Mv]).  The table is the steering table of the Mv-element
+ *              ULA at l s, l < Mv, built by the set_geometry() table builder with M = Mv (bit-identical to a plain
+ *              handle's set_geometry() on those positions; ROOTS and ESPRIT see a ULA).  get_table() returns [K][Mv].
+ *              Angles follow the plain x-axis ULA conventions: ROOTS and ESPRIT give mirror-free angles; the grid modes
+ *              on a line array carry the mirror peaks.
+ *   caveat     the co-array model needs mutually uncorrelated sources.  Correlated or coherent sources break the Toeplitz
+ *              structure: DML, WSF or IAA on a plain handle serve them.
+ * Accepted: estimator MUSIC; peak modes TOP_BINS, LOCAL_MAXIMA, ROOTS, ESPRIT; refinement OFF or NEWTON (on the virtual
+ * ULA's analytic steering); source rule FIXED; set_calibration() with m physical gains; set_integration(); the process
+ * host / device / device_ex / counts / planar entries and the tracks entries under FIXED variance; the spectrum port, the
+ * reducers, stage timing and get_table().  Refused with EINVAL, in either setting order: MVDR, Bartlett and IAA; DML, WSF
+ * and MANIFOLD; MDL and AIC (the eigenvalues of R_ss are squares, so the Wishart-based criteria do not apply); JOINT
+ * refinement; the CRB entries and tracking under CRB variance; the beamformer and the beams entries; calib_accumulate /
+ * calib_solve and every calib_blind_* call (estimate the gains on a plain handle of the same receivers, then call
+ * set_calibration() here); set_table() and set_geometry(); the sharded and gather entries.  create_multi() makes no
+ * co-array handle.
+ * A call never takes the fused kernels: per sub-batch the covariance of the m channels, the calibration and the
+ * integration write a physical-R buffer beside the workspace, coarray_kernel maps it into the workspace R (timed in the
+ * covariance slot of the stage timing), then the plain unfused stages run on Mv.
+ * music_b200_create_coarray: argument checks (EINVAL) before device checks (ENODEVICE).
+ * music_b200_set_geometry_coarray: the retune after an LO change - the virtual table rebuilt from a new step and
+ * wavelength through the table double buffer, resetting integration and tracks like every retune.
+ */
+int music_b200_create_coarray(music_b200 **out, uint32_t m, uint32_t n, uint32_t nsamples, uint32_t resolution, const int32_t *positions,
+                              const double step_xy[2], double wavelength, uint32_t mv, int device);
+int music_b200_set_geometry_coarray(music_b200 *h, const double step_xy[2], double wavelength);
+int music_b200_coarray_size(music_b200 *h, uint32_t *mv);
+
 /* Copies the table currently in use (float[resolution][m][2]) back to host memory. */
 int music_b200_get_table(music_b200 *h, float *table_c64);
 

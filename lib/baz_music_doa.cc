@@ -88,6 +88,34 @@ baz_music_doa::baz_music_doa(unsigned int m, unsigned int n, unsigned int nsampl
             unique_id(), m, n, nsamples, resolution);
 }
 
+/* Extension (not in the reference): a sparse linear array through its difference co-array, see include/music_b200.h. */
+baz_music_doa_sptr baz_make_music_doa_coarray(unsigned int m, unsigned int n, unsigned int nsamples, unsigned int resolution,
+                                              const std::vector<int> &positions, const std::vector<double> &step_xy,
+                                              double wavelength, unsigned int mv)
+{
+    if (positions.size() != m) throw std::invalid_argument("music_doa: positions.size() != m");
+    if (step_xy.size() != 2) throw std::invalid_argument("music_doa: step_xy must be [s_x, s_y]");
+    music_b200 *h = NULL;
+    const int rc = music_b200_create_coarray(&h, m, n, nsamples, resolution, positions.data(), step_xy.data(), wavelength, mv,
+                                             device_from_env());
+    if (rc == MUSIC_B200_EINVAL) throw std::invalid_argument(std::string("music_doa: ") + music_b200_last_error(NULL));
+    if (rc != MUSIC_B200_OK) throw std::runtime_error(std::string("music_doa: ") + music_b200_last_error(NULL));
+    return baz_music_doa_sptr(new baz_music_doa(h, m, n, nsamples, resolution));
+}
+
+baz_music_doa::baz_music_doa(music_b200 *handle, unsigned int m, unsigned int n, unsigned int nsamples, unsigned int resolution)
+    : gr::sync_block("music_doa", gr::io_signature::make(1, 1, nsamples * sizeof(gr_complex)),
+                     gr::io_signature::make3(1, 3, n * sizeof(float), n * sizeof(float), resolution * sizeof(float))),
+      d_m(m), d_n(n), d_nsamples(nsamples), d_resolution(resolution), d_handle(handle), d_track_rows(0),
+      d_source_rule(MUSIC_B200_SOURCES_FIXED), d_beam_rule(MUSIC_B200_BEAMS_OFF), d_crb(false), d_cal_remaining(0), d_cal_angle(0.0), d_cal_kind(MUSIC_B200_CALIB_GAIN_PHASE),
+      d_cal_residual(std::numeric_limits<double>::quiet_NaN()), d_cal_blind(false), d_cal_nsources(1), d_cal_segment(1)
+{
+    uint32_t mv = 0;
+    music_b200_coarray_size(d_handle, &mv);
+    fprintf(stderr, "[%s<%li>] MUSIC DOA co-array: M: %d, virtual M: %u, N: %d, # samples: %d, angular resolution: %d\n", name().c_str(),
+            unique_id(), m, mv, n, nsamples, resolution);
+}
+
 baz_music_doa::~baz_music_doa() { music_b200_destroy(d_handle); }
 
 std::vector<float> baz_music_doa::flatten(const array_response_t &array_response) const
@@ -134,6 +162,16 @@ void baz_music_doa::set_array_geometry(const std::vector<std::vector<double> > &
     fprintf(stderr, "[%s<%li>] Updating array response\n", name().c_str(), unique_id());
     gr::thread::scoped_lock guard(d_mutex);
     const int rc = music_b200_set_geometry(d_handle, flat.data(), wavelength, NULL);
+    if (rc == MUSIC_B200_EINVAL) throw std::invalid_argument(std::string("music_doa: ") + music_b200_last_error(d_handle));
+    if (rc != MUSIC_B200_OK) throw std::runtime_error(std::string("music_doa: ") + music_b200_last_error(d_handle));
+}
+
+void baz_music_doa::set_coarray_geometry(const std::vector<double> &step_xy, double wavelength)
+{
+    if (step_xy.size() != 2) throw std::invalid_argument("music_doa: step_xy must be [s_x, s_y]");
+    fprintf(stderr, "[%s<%li>] Updating array response\n", name().c_str(), unique_id());
+    gr::thread::scoped_lock guard(d_mutex);
+    const int rc = music_b200_set_geometry_coarray(d_handle, step_xy.data(), wavelength);
     if (rc == MUSIC_B200_EINVAL) throw std::invalid_argument(std::string("music_doa: ") + music_b200_last_error(d_handle));
     if (rc != MUSIC_B200_OK) throw std::runtime_error(std::string("music_doa: ") + music_b200_last_error(d_handle));
 }

@@ -33,6 +33,14 @@ typedef std::pair<double, double> doa_t;                   /* (angle in degrees,
 
 baz_music_doa_sptr baz_make_music_doa(unsigned int m, unsigned int n, unsigned int nsamples,
                                       const array_response_t &array_response, unsigned int resolution);
+/* extension: a sparse linear array read through its difference co-array (include/music_b200.h,
+ * music_b200_create_coarray): m physical elements at the integer positions p_0 = 0 < p_1 < ... times the step
+ * step_xy = [s_x, s_y] metres, the wavelength, and the virtual size mv (0: the largest the array's lags fill, up to 16),
+ * with up to mv - 1 sources (n may exceed m).  The block has the ports of baz_music_doa; set_coarray_geometry() is its
+ * retune, and the setters the co-array handle refuses throw. */
+baz_music_doa_sptr baz_make_music_doa_coarray(unsigned int m, unsigned int n, unsigned int nsamples, unsigned int resolution,
+                                              const std::vector<int> &positions, const std::vector<double> &step_xy,
+                                              double wavelength, unsigned int mv);
 
 class baz_music_doa : public gr::sync_block
 {
@@ -42,6 +50,11 @@ private:
 
     baz_music_doa(unsigned int m, unsigned int n, unsigned int nsamples, const array_response_t &array_response,
                   unsigned int resolution);
+    friend baz_music_doa_sptr baz_make_music_doa_coarray(unsigned int m, unsigned int n, unsigned int nsamples,
+                                                         unsigned int resolution, const std::vector<int> &positions,
+                                                         const std::vector<double> &step_xy, double wavelength, unsigned int mv);
+    /* around a handle already created (the co-array factory) */
+    baz_music_doa(music_b200 *handle, unsigned int m, unsigned int n, unsigned int nsamples, unsigned int resolution);
 
 public:
     ~baz_music_doa();
@@ -51,6 +64,9 @@ public:
     void set_array_response(const array_response_t &array_response);
     /* extension: device-side table build from element positions [m][x, y] (metres) and the wavelength */
     void set_array_geometry(const std::vector<std::vector<double> > &positions_xy, double wavelength);
+    /* extension: the retune of a co-array block (baz_make_music_doa_coarray) after an LO change: the step [s_x, s_y]
+     * metres and the wavelength; resets integration and tracks */
+    void set_coarray_geometry(const std::vector<double> &step_xy, double wavelength);
     /* extension: 0 = the reference's n largest bins (default), 1 = n largest local maxima > exclusion_bins apart,
      * 2 = root-MUSIC, 3 = LS-ESPRIT, each on a uniform linear array set by set_array_geometry() (exclusion_bins must be 0),
      * 4 = deterministic maximum likelihood (coherent sources, any table; exclusion_bins must be 0),
